@@ -45,8 +45,20 @@ enum {
   MP_FLAG_DEBUG_NO_FENCE = 1u << 7,     /* skip the generic->async proxy fence */
   MP_FLAG_DEBUG_TOP_SPRITE_ONLY = 1u << 8, /* every cell drawn as its top sprite */
   MP_FLAG_DEBUG_PLAIN_LANE_MAP = 1u << 9,  /* mp_create only: deal cells to lanes in plain order (A/B) */
-  MP_FLAG_DEBUG_SCATTER_LANE_MAP = 1u << 10 /* mp_create only: fully conflict-free dealing that scatters a cell's rows over turns (A/B) */
+  MP_FLAG_DEBUG_SCATTER_LANE_MAP = 1u << 10, /* mp_create only: fully conflict-free dealing that scatters a cell's rows over turns (A/B) */
+  MP_FLAG_DEBUG_NO_PREMERGE = 1u << 11,    /* mp_create only: no pre-merged sprites, every stacked cell is composited per pixel */
+  /* mp_create only: forced render layout (teams per CTA 2-4, warps per team 4-16, log2 of the WORLD.RGB strip rows 1-2)
+   * instead of the one the engine scores best; all three fields zero = the engine's choice. A layout whose shared memory
+   * or thread count does not fit makes mp_create fail with MP_E_UNSUPPORTED. Pack with MP_RENDER_LAYOUT(). */
+  MP_FLAG_LAYOUT_TEAMS_SHIFT = 16, /* 3 bits */
+  MP_FLAG_LAYOUT_WARPS_SHIFT = 19, /* 5 bits */
+  MP_FLAG_LAYOUT_WLOG_SHIFT = 24,  /* 2 bits */
+  MP_FLAG_LAYOUT_MASK = 0x3ffu << 16
 };
+#define MP_RENDER_LAYOUT(teams, warps, wlog) \
+  (((uint32_t)(teams) << MP_FLAG_LAYOUT_TEAMS_SHIFT) | ((uint32_t)(warps) << MP_FLAG_LAYOUT_WARPS_SHIFT) | ((uint32_t)(wlog) << MP_FLAG_LAYOUT_WLOG_SHIFT))
+/* Flags that only mp_create reads; mp_set_flags keeps the values given at creation. */
+#define MP_FLAGS_CREATE_ONLY (MP_FLAG_DEBUG_PLAIN_LANE_MAP | MP_FLAG_DEBUG_SCATTER_LANE_MAP | MP_FLAG_DEBUG_NO_PREMERGE | MP_FLAG_LAYOUT_MASK)
 
 /* Device buffers owned by the engine; valid until mp_destroy. Contents are overwritten by the
  * next mp_step/mp_reset on the same handle. B = num_envs, P = players. */
@@ -106,6 +118,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
 /* Replaces Lab2dWrapper.close (wrappers/base.py:82-84). */
 int mp_destroy(mp_handle h);
 
+/* Changes the per-launch flags (render outputs, diagnostics); the MP_FLAGS_CREATE_ONLY bits keep their creation values. */
 int mp_set_flags(mp_handle h, uint32_t flags);
 
 /* Replaces dmlab2d.Environment.reset (wrappers/base.py:30-32; api_factory.lua:85-102): every
@@ -214,8 +227,12 @@ int mp_state_save(mp_handle h, void* host_dst, void* stream);
 int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stream);
 
 /* Diagnostic: how the renderer was laid out for this substrate: teams per CTA, threads per team, log2 of the pixel
- * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes. */
-int mp_debug_render_plan(mp_handle h, int32_t out[8]);
+ * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes,
+ * then the lane -> cell dealing built for player strips and for WORLD.RGB strips (0 plain, 2 scattered colouring,
+ * 1 + 16 * spare wavefronts for the default whole-cell dealing) and the cells per lane of the k_render instantiation
+ * (NCP for player strips, NCW for WORLD.RGB strips). */
+#define MP_RENDER_PLAN_FIELDS 12
+int mp_debug_render_plan(mp_handle h, int32_t out[MP_RENDER_PLAN_FIELDS]);
 
 /* Diagnostic: the renderer's sprite tables. *n_total = atlas sprites including the pre-merged ones;
  * pair[n_total * n_total] = pre-merged sprite for (bottom, top) or 0; flags[n_total] bit 0 opaque,

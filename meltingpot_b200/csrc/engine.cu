@@ -233,6 +233,7 @@ struct mp_engine {
   std::vector<std::pair<void*, size_t>> state_spans;  // what mp_state_save / mp_state_load copy
   uint64_t state_bytes = 0;
   int lane_map_players = 0, lane_map_world = 0;  // 0 plain, 2 scattered colouring, 1 + 16 * (extra wavefronts left) whole-cell dealing
+  int inst_ncp = 0, inst_ncw = 0;                // the k_render<NCP, NCW> instantiation this engine launches
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob: a snapshot only loads into an engine built from the same blob
 
   template <typename T>
@@ -541,6 +542,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     if ((int)pair_of[base].size() <= top) pair_of[base].resize(top + 1, 0);
     if (pair_of[base][top]) return pair_of[base][top];
     if (n_now() >= kMaxAtlasSprites) return 0;  // budget: the atlas has to fit in shared memory next to the staging buffers
+    if (E->flags & MP_FLAG_DEBUG_NO_PREMERGE) return 0;  // budget zero: every stack takes the general compositing path
     int id = n_now();
     img.resize((size_t)(id + 1) * 1024);
     for (int f = 0; f < 4; ++f)
@@ -694,15 +696,30 @@ int build_plan(mp_engine* E) {
   // Teams per CTA x warps per team x WORLD.RGB strip height: among the layouts that fit in shared memory, the one
   // with the most useful warps in flight. A team draws one env at a time, so its warps share that env's strips; with
   // few strips per warp the end-of-env barrier and the last straggling strip weigh more (score below).
+  // A layout forced through the flags (MP_RENDER_LAYOUT) replaces the search; it must fit like any candidate.
+  const int f_teams = (E->flags >> MP_FLAG_LAYOUT_TEAMS_SHIFT) & 7, f_warps = (E->flags >> MP_FLAG_LAYOUT_WARPS_SHIFT) & 31,
+            f_wlog = (E->flags >> MP_FLAG_LAYOUT_WLOG_SHIFT) & 3;
+  const bool forced = (E->flags & MP_FLAG_LAYOUT_MASK) != 0;
+  if (forced) {
+    if (f_teams < 2 || f_teams > RENDER_MAX_TEAMS || f_warps < 4 || f_warps > TEAM_THREADS / 32 || f_wlog < 1 || f_wlog > 2)
+      return fail(MP_E_INVALID, "render layout (%d teams, %d warps, wstrip_log2 %d) outside 2-%d / 4-%d / 1-2", f_teams, f_warps, f_wlog,
+                  RENDER_MAX_TEAMS, TEAM_THREADS / 32);
+    if (f_teams * f_warps > RENDER_MAX_THREADS / 32)
+      return fail(MP_E_UNSUPPORTED, "render layout of %d teams x %d warps exceeds %d threads per CTA", f_teams, f_warps, RENDER_MAX_THREADS);
+  }
   R.smem_bytes = 1 << 30;
+  int need_forced = 0;
   double best = -1.0;
   for (int teams = 2; teams <= RENDER_MAX_TEAMS; ++teams)
     for (int warps = TEAM_THREADS / 32; warps >= 4; --warps) {
       if (teams * warps > RENDER_MAX_THREADS / 32) continue;
+      if (forced && (teams != f_teams || warps != f_warps)) continue;
       for (int wlog = 2; wlog >= 1; --wlog) {
+        if (forced && wlog != f_wlog) continue;
         const int stage = RENDER_SLOTS * round_up(std::max(R.view_w * 192, T.W * 24 * (1 << wlog)), 128);
         const int team_bytes = round_up(R.grid_bytes, 128) + round_up(T.cells * R.rec_stride * 2, 128) + warps * stage;
         const int total = R.off_team0 + teams * team_bytes;
+        if (forced) need_forced = total;
         if (total > kRenderSmemLimit) continue;
         const double items = T.P * R.view_h + (8 >> wlog) * T.H, per_warp = items / warps;
         // (constants fitted to measurements on the eight substrates: about three strips' worth of idle time per env and
@@ -717,6 +734,9 @@ int build_plan(mp_engine* E) {
         }
       }
     }
+  if (forced && R.smem_bytes > kRenderSmemLimit)
+    return fail(MP_E_UNSUPPORTED, "render layout (%d teams, %d warps, wstrip_log2 %d) needs %d B of shared memory (> %d)", f_teams, f_warps,
+                f_wlog, need_forced, kRenderSmemLimit);
   if (R.smem_bytes > kRenderSmemLimit) return fail(MP_E_UNSUPPORTED, "render kernel needs %d B of shared memory (> 227 KB)", R.smem_bytes);
   return MP_OK;
 }
@@ -929,10 +949,10 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   E->step_smem = E->family == MPB_FAMILY_TERRITORY ? territory_scratch_bytes(T) : warp_scratch_bytes(T);
   {  // cells per lane per strip: ceil(view_w / 4) for player rows, ceil(W / 8) for world half-rows
     const int ncp = (E->R.view_w + 3) / 4, ncw = (T.W + (32 >> E->R.wstrip_log2) - 1) / (32 >> E->R.wstrip_log2);
-    if (ncp <= 3 && ncw <= 3) { E->render_fn = k_render<3, 3, false>; E->render_gather_fn = k_render<3, 3, true>; }
-    else if (ncp <= 3 && ncw <= 4) { E->render_fn = k_render<3, 4, false>; E->render_gather_fn = k_render<3, 4, true>; }
-    else if (ncp <= 3 && ncw <= 5) { E->render_fn = k_render<3, 5, false>; E->render_gather_fn = k_render<3, 5, true>; }
-    else if (ncp <= 4 && ncw <= 5) { E->render_fn = k_render<4, 5, false>; E->render_gather_fn = k_render<4, 5, true>; }
+    if (ncp <= 3 && ncw <= 3) { E->render_fn = k_render<3, 3, false>; E->render_gather_fn = k_render<3, 3, true>; E->inst_ncp = 3; E->inst_ncw = 3; }
+    else if (ncp <= 3 && ncw <= 4) { E->render_fn = k_render<3, 4, false>; E->render_gather_fn = k_render<3, 4, true>; E->inst_ncp = 3; E->inst_ncw = 4; }
+    else if (ncp <= 3 && ncw <= 5) { E->render_fn = k_render<3, 5, false>; E->render_gather_fn = k_render<3, 5, true>; E->inst_ncp = 3; E->inst_ncw = 5; }
+    else if (ncp <= 4 && ncw <= 5) { E->render_fn = k_render<4, 5, false>; E->render_gather_fn = k_render<4, 5, true>; E->inst_ncp = 4; E->inst_ncw = 5; }
     else { mp_destroy(E); return fail(MP_E_UNSUPPORTED, "view of %d cells / map of %d cells wide (max 16 / 40)", E->R.view_w, T.W); }
     // lane -> cell dealing (see make_lane_map_cells / make_lane_map): whole cells per lane group with the cell order chosen
     // to minimise store bank conflicts by default; the fully conflict-free scattered colouring or the plain order for A/B.
@@ -995,7 +1015,7 @@ int mp_destroy(mp_handle h) {
 
 int mp_set_flags(mp_handle h, uint32_t flags) {
   if (!h) return fail(MP_E_INVALID, "null handle");
-  h->flags = flags;
+  h->flags = (flags & ~(uint32_t)MP_FLAGS_CREATE_ONLY) | (h->flags & (uint32_t)MP_FLAGS_CREATE_ONLY);
   return MP_OK;
 }
 
@@ -1335,10 +1355,11 @@ int mp_launch_count(mp_handle h, uint64_t* out) {
   return MP_OK;
 }
 
-int mp_debug_render_plan(mp_handle h, int32_t out[8]) {
+int mp_debug_render_plan(mp_handle h, int32_t out[MP_RENDER_PLAN_FIELDS]) {
   if (!h || !out) return fail(MP_E_INVALID, "mp_debug_render_plan: null argument");
   const RenderPlan& R = h->R;
-  const int32_t v[8] = {R.n_teams, R.team_threads, R.wstrip_log2, R.smem_bytes, R.n_total, R.rec_stride, R.stage_bytes, R.grid_bytes};
+  const int32_t v[MP_RENDER_PLAN_FIELDS] = {R.n_teams, R.team_threads, R.wstrip_log2, R.smem_bytes, R.n_total, R.rec_stride, R.stage_bytes,
+                                            R.grid_bytes, h->lane_map_players, h->lane_map_world, h->inst_ncp, h->inst_ncw};
   memcpy(out, v, sizeof v);
   return MP_OK;
 }

@@ -19,6 +19,38 @@ LIB_PATH = os.environ.get('MP_ENGINE_LIB') or os.path.join(_HERE, 'libmpengine.s
 MP_FLAG_RENDER_WORLD = 1
 MP_FLAG_RENDER_PLAYERS = 2
 MP_FLAG_DEFAULT = 3
+MP_FLAG_DEBUG_PLAIN_LANE_MAP = 1 << 9
+MP_FLAG_DEBUG_SCATTER_LANE_MAP = 1 << 10
+MP_FLAG_DEBUG_NO_PREMERGE = 1 << 11
+MP_FLAG_LAYOUT_MASK = 0x3ff << 16
+# mp_debug_render_plan's lane-map kinds (the default whole-cell dealing is 1 + 16 * spare wavefronts)
+LANE_MAP_PLAIN, LANE_MAP_SCATTER = 0, 2
+
+# Ranges of a forced render layout (include/mp_engine.h, MP_RENDER_LAYOUT): teams per CTA, warps per team, log2 of
+# the pixel rows per WORLD.RGB strip.
+RENDER_LAYOUT_RANGES = ((2, 4), (4, 16), (1, 2))
+
+
+def pack_render_layout(teams: int, warps: int, wstrip_log2: int) -> int:
+  """Flag bits that make mp_create use this render layout instead of the one it scores best."""
+  vals = (teams, warps, wstrip_log2)
+  for name, v, (lo, hi) in zip(('teams', 'warps', 'wstrip_log2'), vals, RENDER_LAYOUT_RANGES):
+    if int(v) != v or not lo <= v <= hi:
+      raise ValueError(f'render layout {name}={v!r} outside {lo}..{hi}')
+  return (int(teams) << 16) | (int(warps) << 19) | (int(wstrip_log2) << 24)
+
+
+def unpack_render_layout(flags: int):
+  """(teams, warps, wstrip_log2) forced by `flags`, or None when the engine chooses."""
+  if not flags & MP_FLAG_LAYOUT_MASK:
+    return None
+  return (flags >> 16) & 7, (flags >> 19) & 31, (flags >> 24) & 3
+
+
+def render_layout_candidates():
+  """Every (teams, warps, wstrip_log2) the engine's layout search considers (teams * warps <= 32 warps per CTA)."""
+  (t0, t1), (w0, w1), (l0, l1) = RENDER_LAYOUT_RANGES
+  return [(t, w, l) for t in range(t0, t1 + 1) for w in range(w0, w1 + 1) for l in range(l0, l1 + 1) if t * w <= 32]
 
 EXPORTED_SYMBOLS = (
     'mp_create', 'mp_destroy', 'mp_set_flags', 'mp_reset', 'mp_step',
@@ -170,7 +202,10 @@ class Engine:
   """One engine handle = `num_envs` env instances on one GPU."""
 
   def __init__(self, blob: bytes, num_envs: int, device: int = 0, seed: int = 1,
-               env_index_base: int = 0, flags: int = MP_FLAG_DEFAULT):
+               env_index_base: int = 0, flags: int = MP_FLAG_DEFAULT, render_layout=None):
+    """render_layout: (teams, warps per team, wstrip_log2) to force instead of the engine's choice (diagnostic)."""
+    if render_layout is not None:
+      flags = (flags & ~MP_FLAG_LAYOUT_MASK) | pack_render_layout(*render_layout)
     import torch  # pylint: disable=g-import-not-at-top
     if not torch.cuda.is_available():
       raise EngineError('CUDA is not available: the CUDA engine has no CPU path')
@@ -436,10 +471,11 @@ class Engine:
     _check(self._lib.mp_state_load(self._h, buf, ctypes.c_uint64(len(snapshot)), self._stream(stream)))
 
   def render_plan(self):
-    """Layout the renderer chose for this substrate (diagnostic)."""
-    out = (ctypes.c_int32 * 8)()
+    """Layout the renderer chose for this substrate, the lane maps it built and its k_render<ncp, ncw> (diagnostic)."""
+    keys = ('teams', 'team_threads', 'wstrip_log2', 'smem_bytes', 'atlas_sprites', 'rec_stride', 'stage_bytes', 'grid_bytes',
+            'lane_map_players', 'lane_map_world', 'ncp', 'ncw')
+    out = (ctypes.c_int32 * len(keys))()
     _check(self._lib.mp_debug_render_plan(self._h, out))
-    keys = ('teams', 'team_threads', 'wstrip_log2', 'smem_bytes', 'atlas_sprites', 'rec_stride', 'stage_bytes', 'grid_bytes')
     return dict(zip(keys, (int(v) for v in out)))
 
   def render_tables(self):

@@ -228,9 +228,9 @@ class OracleBatch:
     assert a.ndim == 2 and a.shape[0] == self.n_envs
     lib().oracle_batch_step_actions(self._h, _ptr(a, ctypes.c_int32), n_threads)
 
-  def dump(self, n_threads: int, shapes, pixels: bool = False, max_events: int = 256):
+  def dump(self, n_threads: int, shapes, pixels: bool = False, max_events: int = 256, kinds=('rgb', 'world')):
     """Every output of every env, laid out like the engine's buffers. `shapes` = dict(P, L, cells, n_scalar,
-    rgb=(h, w), world=(h, w)). Event rows are sorted per env."""
+    rgb=(h, w), world=(h, w)). Event rows are sorted per env. With `pixels`, the images named in `kinds` too."""
     B, P = self.n_envs, shapes['P']
     out = {
         'reward': np.zeros((B, P), np.float64), 'discount': np.zeros((B,), np.float64),
@@ -238,8 +238,9 @@ class OracleBatch:
         'avatars': np.zeros((B, P, 4), np.int32), 'grid': np.zeros((B, shapes['L'], shapes['cells']), np.uint16),
         'events': np.zeros((B, max_events, 3), np.int32), 'n_events': np.zeros((B,), np.int32),
     }
-    if pixels:
+    if pixels and 'rgb' in kinds:
       out['rgb'] = np.zeros((B, P) + tuple(shapes['rgb']) + (3,), np.uint8)
+    if pixels and 'world' in kinds:
       out['world'] = np.zeros((B,) + tuple(shapes['world']) + (3,), np.uint8)
     vp = lambda k: out[k].ctypes.data if k in out else None
     lib().oracle_batch_dump(self._h, n_threads, vp('reward'), vp('discount'), vp('step_type'), vp('scalar_obs'),

@@ -84,28 +84,38 @@ def _event_keys(events, counts):
 
 
 def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_every=10, actions_fn=None,
-                  env_index_base=0, threads=None):
+                  env_index_base=0, threads=None, flags=None, render_layout=None, pixels_at=None, on_step=None):
   """EVERY env of the batch against the oracle: rewards, discount, step type, scalar observations, avatar state, the
-  whole sprite grid and the events on every step, every RGB byte of every env every `pixels_every` steps."""
+  whole sprite grid and the events on every step, every RGB byte of every env every `pixels_every` steps (or on the
+  steps t where `pixels_at(t)` holds; t = 0 is the reset). `flags` / `render_layout` go to the Engine; only the images
+  the flags produce are compared, and an image buffer the flags leave out is filled with a sentinel before the reset
+  and must still hold it on every pixel check. `on_step(t, eng)` runs after each check."""
   import os
   import torch
   from meltingpot_b200 import engine
   threads = threads or os.cpu_count() or 1
-  eng = engine.Engine(blob, num_envs, device=0, seed=seed, env_index_base=env_index_base)
+  flags = engine.MP_FLAG_DEFAULT if flags is None else flags
+  eng = engine.Engine(blob, num_envs, device=0, seed=seed, env_index_base=env_index_base, flags=flags,
+                      render_layout=render_layout)
   P, A = eng.num_players, eng.num_actions
   bf = eng.buffers
   shapes = dict(P=P, L=int(bf.grid_layers), cells=int(bf.grid_cells), n_scalar=eng.num_scalar_obs,
                 rgb=(int(bf.rgb_h), int(bf.rgb_w)), world=(int(bf.world_h), int(bf.world_w)))
   max_ev = int(bf.max_events)
+  kinds = [k for k, bit in (('rgb', engine.MP_FLAG_RENDER_PLAYERS), ('world', engine.MP_FLAG_RENDER_WORLD)) if flags & bit]
+  absent = [t for k, t in (('rgb', eng.rgb), ('world', eng.world_rgb)) if k not in kinds]
+  for t in absent:
+    t.fill_(_SENTINEL)
   batch = oracle.OracleBatch(blob, num_envs, seed=seed + env_index_base)  # oracle_batch_create starts episode 0
   rng = np.random.default_rng(action_seed)
   eng.reset()
-  stats = dict(rewards=0.0, lasts=0, events=0, pixel_checks=0, envs=num_envs)
+  stats = dict(rewards=0.0, lasts=0, events=0, pixel_checks=0, envs=num_envs, last_steps=[], mids_after_restart=0)
+  restarted = np.zeros(num_envs, bool)
 
   def check(t):
     torch.cuda.synchronize()
-    px = (t % pixels_every) == 0
-    want = batch.dump(threads, shapes, pixels=px, max_events=max_ev)
+    px = pixels_at(t) if pixels_at is not None else (t % pixels_every) == 0
+    want = batch.dump(threads, shapes, pixels=px, max_events=max_ev, kinds=kinds)
     where = f'step {t}'
 
     def same(name, got, exp):
@@ -113,7 +123,8 @@ def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_eve
         bad = np.argwhere(got != exp)
         raise AssertionError(f'{name} {where}: {len(bad)} mismatches, first at {bad[0].tolist()} (env first): gpu {got[tuple(bad[0])]} oracle {exp[tuple(bad[0])]}')
 
-    same('step_type', eng.step_type.cpu().numpy(), want['step_type'])
+    st = eng.step_type.cpu().numpy()
+    same('step_type', st, want['step_type'])
     same('discount', eng.discount.cpu().numpy(), want['discount'])
     same('reward', eng.reward.cpu().numpy(), want['reward'])
     if shapes['n_scalar']:
@@ -125,12 +136,23 @@ def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_eve
     assert int(nev.max(initial=0)) <= max_ev, f'{where}: {int(nev.max())} events exceed max_events {max_ev}'
     same('events', _event_keys(eng.events.cpu().numpy(), nev), _event_keys(want['events'], want['n_events']))
     if px:
-      same('RGB', eng.rgb.cpu().numpy(), want['rgb'])
-      same('WORLD.RGB', eng.world_rgb.cpu().numpy(), want['world'])
+      if 'rgb' in kinds:
+        same('RGB', eng.rgb.cpu().numpy(), want['rgb'])
+      if 'world' in kinds:
+        same('WORLD.RGB', eng.world_rgb.cpu().numpy(), want['world'])
+      for img in absent:
+        assert bool((img == _SENTINEL).all()), f'{where}: an image the flags leave out was written'
       stats['pixel_checks'] += 1
     stats['rewards'] += float(want['reward'].sum())
-    stats['lasts'] += int((want['step_type'] == 2).sum())
+    stats['lasts'] += int((st == 2).sum())
+    if (st == 2).any():
+      stats['last_steps'].append(t)
+    stats['mids_after_restart'] += int(((st == 1) & restarted).sum())
+    if t > 0:
+      restarted[st == 0] = True
     stats['events'] += int(want['n_events'].sum())
+    if on_step is not None:
+      on_step(t, eng)
 
   check(0)
   for t in range(1, steps + 1):
@@ -142,3 +164,51 @@ def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_eve
   eng.close()
   batch.close()
   return stats
+
+
+_SENTINEL = 0xA5
+# the engine's per-env state and timestep buffers (everything a later step depends on or a caller reads)
+# (event rows are compared as sorted keys: the rows of one step are in no particular order)
+_STATE_VIEWS = ('reward', 'discount', 'step_type', 'scalar_obs', 'avatar_state', 'grid', 'event_count', 'timestep_packed')
+
+
+def lockstep(blob, num_envs, steps, seed, variants, action_seed=0, actions_fn=None, env_index_base=0):
+  """Steps an engine with the default options and one engine per entry of `variants` (Engine keyword arguments such as
+  `flags` / `render_layout`), all built from the same blob, seed and B, with the same actions. After the reset and
+  after every step each variant's images (those its flags produce) and state buffers must equal the default engine's,
+  compared on the device. The default engine follows the same action stream as compare_batch with the same
+  `action_seed` / `actions_fn`, so a compare_batch run anchors the chain to the oracle. Returns each variant's
+  render_plan()."""
+  import torch
+  from meltingpot_b200 import engine
+  ref = engine.Engine(blob, num_envs, device=0, seed=seed, env_index_base=env_index_base)
+  twins = [engine.Engine(blob, num_envs, device=0, seed=seed, env_index_base=env_index_base, **v) for v in variants]
+  P, A = ref.num_players, ref.num_actions
+  rng = np.random.default_rng(action_seed)
+
+  def check(t):
+    ref_events = _event_keys(ref.events.cpu().numpy(), ref.event_count.cpu().numpy())
+    for v, tw in zip(variants, twins):
+      f = v.get('flags', engine.MP_FLAG_DEFAULT)
+      names = list(_STATE_VIEWS) + (['rgb'] if f & engine.MP_FLAG_RENDER_PLAYERS else []) + (['world_rgb'] if f & engine.MP_FLAG_RENDER_WORLD else [])
+      for name in names:
+        if not torch.equal(getattr(tw, name), getattr(ref, name)):
+          raise AssertionError(f'{name} differs from the default engine at step {t} (B={num_envs}, {v}, plan {tw.render_plan()})')
+      if not np.array_equal(_event_keys(tw.events.cpu().numpy(), tw.event_count.cpu().numpy()), ref_events):
+        raise AssertionError(f'events differ from the default engine at step {t} (B={num_envs}, {v})')
+
+  ref.reset()
+  for tw in twins:
+    tw.reset()
+  check(0)
+  for t in range(1, steps + 1):
+    acts = actions_fn(t, num_envs, P, A, rng) if actions_fn is not None else rng.integers(0, A, size=(num_envs, P))
+    acts = torch.from_numpy(np.ascontiguousarray(acts, np.int32)).cuda()
+    ref.step(acts)
+    for tw in twins:
+      tw.step(acts)
+    check(t)
+  plans = [tw.render_plan() for tw in twins]
+  for e in [ref] + twins:
+    e.close()
+  return plans

@@ -20,31 +20,57 @@ def _cmp(eng, envs, where):
 
 def test_masked_reset_restarts_only_the_selected_envs(clean_up_blob, oracle):
   # mp_reset(env_mask): the reference has one env per object, so a "masked reset" is env[i].reset() for some i.
+  _masked_reset(clean_up_blob, 'clean_up', oracle)
+
+
+@pytest.mark.parametrize('name,players', [('commons_harvest__open', 7), ('territory__rooms', 9),
+                                          ('territory__inside_out', 5), ('coins', 2), ('coop_mining', 6)])
+def test_masked_reset_of_every_kernel_family(name, players, oracle):
+  # The other kernel families (territory computes its reset condition apart from the others), plus inside_out, whose
+  # reset also redraws the env's 'choice' resource layout.
+  from meltingpot_b200 import substrates
+  _masked_reset(substrates.load_blob(name, ('default',) * players), name, oracle)
+
+
+def _masked_reset(blob, name, oracle):
   import torch
   from meltingpot_b200 import engine
-  B, P, seed = 12, 7, 40
-  eng = engine.Engine(clean_up_blob, B, device=0, seed=seed)
-  envs = [oracle.OracleEnv(clean_up_blob, seed + b) for b in range(B)]
+  B, seed = 12, 40
+  eng = engine.Engine(blob, B, device=0, seed=seed)
+  P, A = eng.num_players, eng.num_actions
+  envs = [oracle.OracleEnv(blob, seed + b) for b in range(B)]
   eng.reset()
   for e in envs:
     e.reset()
   rng = np.random.default_rng(2)
   def play(k, tag):
     for t in range(k):
-      a = np.ascontiguousarray(rng.integers(0, 9, (B, P)), np.int32)
+      a = np.ascontiguousarray(rng.integers(0, A, (B, P)), np.int32)
       eng.step(torch.from_numpy(a).cuda())
       for b, e in enumerate(envs):
         e.step(a[b])
       if t % 5 == 4:
         _cmp(eng, envs, f'{tag} step {t}')
   play(25, 'before')
+  grid_before = eng.grid.cpu().numpy()
   mask = np.zeros(B, np.uint8); mask[[1, 4, 5, 10]] = 1
   eng.reset(torch.from_numpy(mask).cuda())
   for b in np.nonzero(mask)[0]:
     envs[b].reset()  # next episode of that env only
   _cmp(eng, envs, 'after masked reset')
+  for b, e in enumerate(envs):
+    np.testing.assert_array_equal(e.grid(), eng.grid.cpu().numpy().view(np.uint16)[b][:, :e.grid().shape[1]],
+                                  err_msg=f'grid after masked reset env {b}')
   st = eng.step_type.cpu().numpy()
   assert (st[mask == 1] == 0).all() and (st[mask == 0] == 1).all()  # FIRST only where reset
+  if name == 'territory__inside_out':
+    from meltingpot_b200 import blob as blob_lib
+    sec = blob_lib.unpack(blob)
+    cells, res_layer = sec['tr_res'][:, 1].astype(np.int64), int(sec['tr_ip'][1])
+    layout = lambda g: g[:, res_layer][:, cells] != 0
+    before, after = layout(grid_before), layout(eng.grid.cpu().numpy())
+    for b in range(B):  # masked envs redraw their resource layout, the others keep theirs
+      assert np.array_equal(before[b], after[b]) == (mask[b] == 0), f'resource layout env {b}'
   play(25, 'after')
 
 
