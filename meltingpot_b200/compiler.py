@@ -964,6 +964,10 @@ def _commons_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
           continue
         j = cell_to_apple.get(y * W + x)
         if j is not None:
+          if k == nbr.shape[1]:
+            raise NotImplementedError(f'DensityRegrow radius {radius}: the disc around the apple at ({cx}, {cy}) holds '
+                                      f'more than {nbr.shape[1]} other apples (the kernel keeps at most '
+                                      f'{nbr.shape[1]} neighbours per apple)')
           nbr[i, k] = j
           k += 1
   def avatar_comp(comp):

@@ -216,7 +216,8 @@ __device__ __forceinline__ uint16_t cell_value(int sprite, int orient) { return 
 
 // Maps (x, y) into the map; returns false if it falls outside a BOUNDED map.
 // On a TORUS every caller stays within one map width / height of the map (moves, beam footprints and
-// view windows are all smaller than the map; mp_create checks it), so a conditional add wraps.
+// view windows are all smaller than the map: mp_create refuses views and beams that are not, see beam_fits_torus),
+// so a conditional add wraps.
 __device__ __forceinline__ bool wrap_or_reject(const Tables& T, int& x, int& y) {
   if (T.topology == 1) {
     x += x < 0 ? T.W : (x >= T.W ? -T.W : 0);

@@ -87,6 +87,14 @@ bool make_beam_geom(int length, int radius, BeamGeom* g) {
   return true;
 }
 
+// A beam of `length` cells forward and `radius` to each side covers forward offsets 0..length and lateral offsets
+// -radius..radius around the shooter. On a TORUS map that is smaller than the map in both directions, each footprint
+// cell wraps with one conditional add (wrap_or_reject) and no two cells of a footprint land on the same map cell.
+bool beam_fits_torus(const Tables& T, int length, int radius) {
+  const int m = std::min(T.W, T.H);
+  return T.topology != 1 || (length < m && 2 * radius + 1 <= m);
+}
+
 // Deals the cells of one strip to lanes so that the 64-bit staging stores of every half-warp are bank-conflict free.
 // A strip is `n_rows` pixel rows (8 for a player cell-row, 4 or 2 for WORLD.RGB) by `n_cells` cells of 24 bytes at a
 // row pitch of `pitch_slots` 8-byte slots; lane l draws pixel row l % n_rows in each of its `iters` turns. A 64-bit
@@ -344,6 +352,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     for (int h = 0; h < (int)hits.count / 2; ++h) if (hits.data[h * 2] == T.zap_layer) T.zap_hit = h;
     if (T.zap_cooldown <= 0) return fail(MP_E_UNSUPPORTED, "non-positive zap cooldown");
     if (!make_beam_geom(ip[13], ip[14], &T.zap_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (!beam_fits_torus(T, ip[13], ip[14])) return fail(MP_E_UNSUPPORTED, "zap beam (length %d, radius %d) does not fit the %dx%d TORUS map", ip[13], ip[14], T.W, T.H);
     T.end_min_frames = ip[26]; T.end_interval = ip[27];
     if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
     return MP_OK;
@@ -364,6 +373,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     for (int h = 0; h < (int)hits.count / 2; ++h) if (hits.data[h * 2] == T.clean_layer) T.clean_hit = h;
     if (T.clean_cooldown < 0) return fail(MP_E_UNSUPPORTED, "negative clean cooldown");
     if (!make_beam_geom(ip[19], ip[20], &T.clean_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (!beam_fits_torus(T, ip[19], ip[20])) return fail(MP_E_UNSUPPORTED, "clean beam (length %d, radius %d) does not fit the %dx%d TORUS map", ip[19], ip[20], T.W, T.H);
     T.dirt_delay = ip[25]; T.taste_role = ip[28];
     if (T.taste_role != 0) return fail(MP_E_UNSUPPORTED, "Taste roles other than 'free'");
     T.grow_rate = dp[0]; T.grow_depletion = dp[1]; T.grow_restoration = dp[2]; T.eat_reward = dp[3];
@@ -420,6 +430,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     if (T.zap_cooldown < 1 || T.mine_window < 1 || T.mine_window > 255 || T.mine_length < 1) return fail(MP_E_UNSUPPORTED, "MineBeam / Ore parameters out of range");
     if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
     if (T.zap_hit < 0 || T.zap_hit > 7) return fail(MP_E_UNSUPPORTED, "mine hit id %d", T.zap_hit);
+    if (!beam_fits_torus(T, T.mine_length, 0)) return fail(MP_E_UNSUPPORTED, "mine beam (length %d) does not fit the %dx%d TORUS map", T.mine_length, T.W, T.H);
     T.mine_rate[0] = dp[0]; T.mine_rate[1] = dp[1]; T.end_prob = dp[2];
     T.mine_reward[0] = dp[4]; T.mine_reward[1] = dp[5]; T.extract_reward[0] = dp[6]; T.extract_reward[1] = dp[7];
     v_apple.resize((size_t)T.nA * 4);
@@ -440,11 +451,15 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     if ((rc = zapper(ip))) return rc;
     if (T.zap_respawn <= T.max_frames) return fail(MP_E_UNSUPPORTED, "territory kernel assumes avatars never respawn (framesTillRespawn %d)", T.zap_respawn);
     if (!make_beam_geom(ip[18], ip[19], &T.claim_geom) || !make_beam_geom(1, 0, &T.brush_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (!beam_fits_torus(T, ip[18], ip[19])) return fail(MP_E_UNSUPPORTED, "claim beam (length %d, radius %d) does not fit the %dx%d TORUS map", ip[18], ip[19], T.W, T.H);
     T.claim_wait = ip[20]; T.brush_layer = ip[23]; T.claim_layer = ip[24];
     if (T.claim_layer != T.dmg_layer) return fail(MP_E_UNSUPPORTED, "territory: claim beam layer must be the damage indicator layer");
     T.res_health0 = ip[28]; T.res_reward_delay = ip[29]; T.res_repair_delay = ip[30]; T.tr_taste_role = ip[31];
     if (T.tr_taste_role != 0) return fail(MP_E_UNSUPPORTED, "territory Taste roles other than 'none'");
     if (T.res_health0 < 1 || T.res_health0 > 200) return fail(MP_E_UNSUPPORTED, "resource health %d", T.res_health0);
+    // the resource age and frames-since-zapped counters saturate at 65535 (step_territory.cuh)
+    if (T.res_reward_delay > 65535 || T.res_repair_delay > 65535)
+      return fail(MP_E_UNSUPPORTED, "rewardDelay %d / delayTillSelfRepair %d (max 65535)", T.res_reward_delay, T.res_repair_delay);
     for (int l = 0; l < T.mark_n_levels; ++l) {
       T.mark_inc[l] = ip[32 + 4 * l]; T.mark_remove[l] = ip[33 + 4 * l]; T.mark_freeze[l] = ip[34 + 4 * l]; T.mark_sprite[l] = ip[35 + 4 * l];
       T.mark_src_reward[l] = dp[8 + 2 * l]; T.mark_tgt_reward[l] = dp[9 + 2 * l];
@@ -1310,7 +1325,7 @@ int mp_state_save(mp_handle h, void* host_dst, void* stream) {
   if (!h || !host_dst) return fail(MP_E_INVALID, "mp_state_save: null argument");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
-  SnapshotHeader hd{{'M', 'P', 'S', '2'}, 2u, (uint64_t)h->B, h->state_bytes, (uint64_t)h->state_spans.size(), h->S.seed, h->blob_hash};
+  SnapshotHeader hd{{'M', 'P', 'S', '3'}, 3u, (uint64_t)h->B, h->state_bytes, (uint64_t)h->state_spans.size(), h->S.seed, h->blob_hash};
   memcpy(host_dst, &hd, sizeof(hd));
   uint8_t* dst = static_cast<uint8_t*>(host_dst) + sizeof(hd);
   for (const auto& sp : h->state_spans) {
@@ -1326,7 +1341,7 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
   if (nbytes < sizeof(SnapshotHeader)) return fail(MP_E_INVALID, "mp_state_load: %llu bytes is shorter than a snapshot header", (unsigned long long)nbytes);
   SnapshotHeader hd;
   memcpy(&hd, host_src, sizeof(hd));
-  if (memcmp(hd.magic, "MPS2", 4) != 0 || hd.version != 2u) return fail(MP_E_INVALID, "mp_state_load: not a snapshot (or one of an older engine)");
+  if (memcmp(hd.magic, "MPS3", 4) != 0 || hd.version != 3u) return fail(MP_E_INVALID, "mp_state_load: not a snapshot (or one of an older engine)");
   if (hd.num_envs != (uint64_t)h->B || hd.payload_bytes != h->state_bytes || hd.n_spans != h->state_spans.size())
     return fail(MP_E_INVALID, "mp_state_load: snapshot of %llu envs / %llu bytes does not fit this engine (%d envs / %llu bytes)",
                 (unsigned long long)hd.num_envs, (unsigned long long)hd.payload_bytes, h->B, (unsigned long long)h->state_bytes);

@@ -214,7 +214,7 @@ __device__ void clean_up_step(const Tables& T, const State& S, int b, int lane, 
     const double dirt = (double)dirt_count, clean = (double)(T.nD - dirt_count);
     const double fraction = dirt / (dirt + clean);
     double interpolation = (fraction - T.grow_depletion) / (T.grow_restoration - T.grow_depletion);
-    interpolation = fmin(interpolation, 1.0);
+    interpolation = 1.0 < interpolation ? 1.0 : interpolation;  // Lua 5.1 math.min: a NaN (0/0) stays NaN, no growth (policy A.22)
     const double probability = T.grow_rate * interpolation;
     if (probability > 0.0) {  // u >= 0 can never be below a non-positive (or NaN) probability
       for (int k = lane; k < T.nA; k += 32) {

@@ -23,7 +23,10 @@
 enum { RF_ACTIVE = 1, RF_NEVER_CLAIMED = 2, RF_DESTROYED = 4, RF_ABSENT = 8 /* not drawn into this episode's map ('choice' prefab) */ };
 // fam_u8 sub-arrays (each nR_pad long), fam_u16 sub-arrays.
 enum { RU_STATE = 0, RU_HEALTH = 1, RU_FLAGS = 2, RU_CLAIMER = 3, RU_IND = 4, RU_DMG = 5, RU_TEX = 6, RU_COUNT = 7 };
-enum { RS_FSZ = 0, RS_FRAME = 1, RS_COUNT = 2 };
+// RS_AGE is the resource's age in the frame about to run: frames since its last state change, which the updaters'
+// startFrame (components.lua:101,115) is compared with and the oracle computes as frame - state_frame; saturated at 65535. mp_create refuses delays above that, so the
+// comparisons with rewardDelay / delayTillSelfRepair / 5 stay exact in episodes of any length.
+enum { RS_FSZ = 0, RS_AGE = 1, RS_COUNT = 2 };
 // av_extra columns
 enum { AX_FREEZE = 0, AX_REMOVAL = 1, AX_FLAGS = 2 /* bit0 movement allowed, bit1 zapping disallowed, bit2 marking on grid */,
        AX_NOZAP = 3, AX_LEVEL = 4, AX_MARK_T = 5, AX_SHOWN = 6 /* level whose sprite the marking shows */, AX_CLAIM_COOL = 7 };
@@ -35,7 +38,7 @@ struct TerritoryScratch {
   uint8_t* r2_changed;
   uint8_t* was[4];         // state / reward indicator / damage indicator / texture as the frame started (round 2 writes the grid on change)
   uint16_t* fsz;
-  uint16_t* frame;
+  uint16_t* age;
   uint32_t* bm_zap; uint32_t* bm_brush; uint32_t* bm_claim;  // cells already carrying a hit sprite
   int* cnt;                // [MP_MAX_PLAYERS] rewards provided this frame per avatar
   // per-CTA copies of static tables that sit on the frame's serial chain (an L2 round trip each otherwise)
@@ -52,7 +55,7 @@ __host__ __device__ inline size_t territory_table_bytes(const Tables& T) {
 
 __host__ __device__ inline size_t tr_round16(size_t n) { return (n + 15) & ~(size_t)15; }
 
-// Layout: [fsz | frame] (as in fam_u16) then [r[0..RU_COUNT)] (as in fam_u8), both 16-byte aligned and contiguous so that
+// Layout: [fsz | age] (as in fam_u16) then [r[0..RU_COUNT)] (as in fam_u8), both 16-byte aligned and contiguous so that
 // a frame moves them between HBM and shared memory with 128-bit accesses; then r2_state, r2_changed, the four
 // frame-start copies round 2 compares against, occ, the hit-sprite bitmaps and the reward counters.
 __host__ __device__ inline size_t territory_scratch_bytes(const Tables& T) {
@@ -64,7 +67,7 @@ __device__ __forceinline__ TerritoryScratch carve_territory(const Tables& T, uin
   TerritoryScratch s;
   size_t words = (size_t)(T.cells + 31) / 32 + 1;
   s.fsz = (uint16_t*)base; base += 2 * T.nR_pad;
-  s.frame = (uint16_t*)base; base += 2 * T.nR_pad;
+  s.age = (uint16_t*)base; base += 2 * T.nR_pad;
   for (int i = 0; i < RU_COUNT; ++i) { s.r[i] = base; base += T.nR_pad; }
   s.r2_state = base; base += T.nR_pad;
   s.r2_changed = base; base += T.nR_pad;
@@ -100,7 +103,7 @@ __device__ void territory_init(const Tables& T, const State& S, int b, int lane,
     u8[RU_FLAGS * T.nR_pad + k] = RF_NEVER_CLAIMED;
     u8[RU_CLAIMER * T.nR_pad + k] = 0xFF;
     u8[RU_IND * T.nR_pad + k] = 0; u8[RU_DMG * T.nR_pad + k] = 0; u8[RU_TEX * T.nR_pad + k] = 0;
-    u16[RS_FSZ * T.nR_pad + k] = 0; u16[RS_FRAME * T.nR_pad + k] = 0;
+    u16[RS_FSZ * T.nR_pad + k] = 0; u16[RS_AGE * T.nR_pad + k] = 0;
     if (T.tr_res_cond && !choice_present(T, T.tr_res_cond[k * 2], (uint32_t)T.tr_res_cond[k * 2 + 1], episode, k0, k1)) {
       // This episode's map has plain floor here: the resource, its texture and its two indicators were not created.
       // Kept as a destroyed resource that never had a texture: nothing stands on the cell, nothing is drawn, nothing updates.
@@ -267,7 +270,7 @@ __device__ void territory_frame(const Tables& T, const State& S, int b, int lane
   for (int k = lane; k < T.nR; k += 32) {
     const int st = sc.r[RU_STATE][k];
     if (st < 2) continue;
-    const int age = n - (int)sc.frame[k];
+    const int age = sc.age[k];
     const int claimer = sc.r[RU_CLAIMER][k];
     if (age >= T.res_reward_delay) {
       uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)sc.res_obj[k], RS_OBJECT, k0, k1);
@@ -469,7 +472,7 @@ __device__ void territory_frame(const Tables& T, const State& S, int b, int lane
   for (int k = lane; k < T.nR; k += 32) {
     const int cell = sc.res_cell[k];
     const int st_new = sc.r2_state[k];
-    if (sc.r2_changed[k]) sc.frame[k] = (uint16_t)n;
+    sc.age[k] = sc.r2_changed[k] ? (uint16_t)1 : (uint16_t)min((int)sc.age[k] + 1, 65535);  // age in frame n + 1
     const uint8_t was_state = sc.was[0][k], was_ind = sc.was[1][k], was_dmg = sc.was[2][k], was_tex = sc.was[3][k];
     sc.r[RU_STATE][k] = (uint8_t)st_new;
     if (st_new != was_state) grid[(size_t)T.res_layer * T.cells_pad + cell] = resource_sprite_value(T, st_new);

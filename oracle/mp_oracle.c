@@ -873,7 +873,7 @@ static void simulation_update(OrEnv* e) {
           double dirt = (double)e->dirt_count, clean = (double)e->clean_count;
           double fraction = dirt / (dirt + clean);
           double interpolation = (fraction - c->dp[1]) / (c->dp[2] - c->dp[1]);
-          interpolation = fmin(interpolation, 1.0);
+          interpolation = 1.0 < interpolation ? 1.0 : interpolation; /* math.min keeps a NaN (policy A.22) */
           double probability = c->dp[0] * interpolation;
           uint32_t w[4]; rng(e, RS_OBJECT, oi, w);
           if (u01(w[0], w[1]) < probability) enqueue(e, ACT_SET_STATE, oi, c->ip[0], 0, 0);
