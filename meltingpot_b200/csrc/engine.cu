@@ -225,7 +225,8 @@ struct mp_engine {
   int32_t* d_avatar_dbg = nullptr;
   uint64_t launches = 0;
   int sm_count = 0;
-  size_t step_smem = 0;
+  void (*step_fn)(Tables, State, const int32_t*, const uint8_t*, int) = nullptr;
+  size_t step_smem = 0;  // dynamic shared memory of one state-transition launch
   void (*render_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
   void (*render_gather_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
   // mp_gather_obs_*: this rank's stacked-observation block [flags 256 B][2 slots][rgb of all ranks | world_rgb of all ranks]
@@ -788,6 +789,19 @@ __global__ void k_debug_obs(Tables T, State S, int32_t* position, int32_t* orien
   }
 }
 
+// The state-transition kernel of each substrate family and the dynamic shared memory one launch of it takes.
+using StepFn = void (*)(Tables, State, const int32_t*, const uint8_t*, int);
+const StepFn kStepKernels[] = {k_step<CleanUp>, k_step<Commons>, k_step<Territory>, k_step<Coins>, k_step<Mining>};
+StepFn step_kernel(int family, const Tables& T, size_t* smem) {
+  switch (family) {
+    case MPB_FAMILY_CLEAN_UP: *smem = step_smem_bytes<CleanUp>(T); return k_step<CleanUp>;
+    case MPB_FAMILY_COMMONS_HARVEST: *smem = step_smem_bytes<Commons>(T); return k_step<Commons>;
+    case MPB_FAMILY_COINS: *smem = step_smem_bytes<Coins>(T); return k_step<Coins>;
+    case MPB_FAMILY_COOP_MINING: *smem = step_smem_bytes<Mining>(T); return k_step<Mining>;
+    default: *smem = step_smem_bytes<Territory>(T); return k_step<Territory>;
+  }
+}
+
 int raise_flags(mp_engine* E, cudaStream_t st) {
   E->x_pending_raise = false;
   k_exchange_push<<<std::min(E->sm_count, (E->B + 7) / 8), 256, 0, st>>>(E->T, E->S);
@@ -800,16 +814,13 @@ int raise_flags(mp_engine* E, cudaStream_t st) {
 int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int mode, cudaStream_t st, bool render_follows = true) {
   const int blocks = (E->B + 3) / 4;
   if (E->S.x_world) E->S.x_step = ++E->x_seq;
-  void (*fn)(Tables, State, const int32_t*, const uint8_t*, int) =
-      E->family == MPB_FAMILY_CLEAN_UP ? k_step_clean_up : E->family == MPB_FAMILY_COMMONS_HARVEST ? k_step_commons :
-      E->family == MPB_FAMILY_COINS ? k_step_coins : E->family == MPB_FAMILY_COOP_MINING ? k_step_mining : k_step_territory;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(128); cfg.dynamicSmemBytes = E->step_smem * 4 + (E->family == MPB_FAMILY_CLEAN_UP ? clean_up_table_bytes(E->T) : E->family == MPB_FAMILY_TERRITORY ? territory_table_bytes(E->T) : 0); cfg.stream = st;
+  cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(128); cfg.dynamicSmemBytes = E->step_smem; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, fn, E->T, E->S, actions, mask, mode));
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->step_fn, E->T, E->S, actions, mask, mode));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st); }
@@ -961,7 +972,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     cudaError_t ce = cudaMemcpy(S.env, env0.data(), env0.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
     if (ce != cudaSuccess) { mp_destroy(E); return fail(MP_E_CUDA, "cudaMemcpy(env) failed: %s", cudaGetErrorString(ce)); }
   }
-  E->step_smem = E->family == MPB_FAMILY_TERRITORY ? territory_scratch_bytes(T) : warp_scratch_bytes(T);
+  E->step_fn = step_kernel(E->family, T, &E->step_smem);
   {  // cells per lane per strip: ceil(view_w / 4) for player rows, ceil(W / 8) for world half-rows
     const int ncp = (E->R.view_w + 3) / 4, ncw = (T.W + (32 >> E->R.wstrip_log2) - 1) / (32 >> E->R.wstrip_log2);
     if (ncp <= 3 && ncw <= 3) { E->render_fn = k_render<3, 3, false>; E->render_gather_fn = k_render<3, 3, true>; E->inst_ncp = 3; E->inst_ncw = 3; }
@@ -989,13 +1000,10 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   if (ce == cudaSuccess) ce = cudaFuncSetAttribute(E->render_gather_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
   {
     static int step_smem_max[MP_MAX_DEVICES] = {};
-    const int need = (int)(E->step_smem * 4 + (E->family == MPB_FAMILY_CLEAN_UP ? clean_up_table_bytes(T) : E->family == MPB_FAMILY_TERRITORY ? territory_table_bytes(T) : 0));
+    const int need = (int)E->step_smem;
     if (ce == cudaSuccess && need > 48 * 1024 && need > step_smem_max[device]) {
-      ce = cudaFuncSetAttribute(k_step_clean_up, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-      if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k_step_commons, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-      if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k_step_territory, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-      if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k_step_coins, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-      if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k_step_mining, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+      for (StepFn fn : kStepKernels)
+        if (ce == cudaSuccess) ce = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
       if (ce == cudaSuccess) step_smem_max[device] = need;
     }
   }

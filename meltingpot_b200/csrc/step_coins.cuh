@@ -10,234 +10,134 @@
 // (liveStateA / liveStateB, superOverlay). There are no beams and avatars never leave the map.
 #pragma once
 
-#include "common.cuh"
-#include "step_clean_up.cuh"  // WarpScratch
+#include "step_common.cuh"
 
-// Episode start for coins: every coin waits, the two avatars draw their spawn points.
-__device__ void coins_reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
-  int32_t* env = S.env + (size_t)b * ENV_COLS;
-  const int episode = env[ENV_EPISODE] + 1;
-  const uint64_t key = S.seed + (uint64_t)b;
-  const uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-  uint16_t* grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  __syncwarp();
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(T.init_grid);
-    uint4* dst = reinterpret_cast<uint4*>(grid);
-    const int n16 = T.L * T.cells_pad / 8;
-    for (int i = lane; i < n16; i += 32) dst[i] = src[i];
-  }
-  for (int k = lane; k < T.nA; k += 32) S.apple[(size_t)b * T.nA_pad + k] = 0;
-  __syncwarp();
-  // _avatarStart: partial Fisher-Yates over the spawn group (base_simulation.lua:396-445), policy A.10.
-  const int n = T.n_spawn_init[0];
-  for (int i = lane; i < n && i < 64; i += 32) sc.tmp[i] = (int16_t)T.spawn_init_cell[0][i];
-  __syncwarp();
-  if (lane == 0) {
-    for (int p = 0; p < T.P; ++p) {
-      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)p, RS_AVATAR_RESET, k0, k1);
-      int r = p + (int)pick(w.x, (uint32_t)(n - p));
-      int16_t t = sc.tmp[p]; sc.tmp[p] = sc.tmp[r]; sc.tmp[r] = t;
+struct Coins {
+  using Scratch = WarpScratch;
+  static constexpr bool kStagesTables = false;
+  __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
+  __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
+  __device__ static void stage(const Tables&, uint8_t*) {}
+  __device__ static WarpScratch carve(const Tables& T, uint8_t* base, const uint8_t*) { return carve_scratch(T, base); }
+
+  // Episode start for coins: every coin waits, the two avatars draw their spawn points (policy A.10).
+  __device__ static void reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
+    const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
+    __syncwarp();
+    copy_init_grid(T, grid, lane);
+    for (int k = lane; k < T.nA; k += 32) S.apple[(size_t)b * T.nA_pad + k] = 0;
+    __syncwarp();
+    const auto all = [](int) { return true; };
+    spawn_group(T, S, b, lane, grid, sc.tmp, T.spawn_init_cell[0], T.n_spawn_init[0], all, all, episode, k0, k1, [&](int) {
+      S.av_extra[((size_t)b * T.P + lane) * 8] = 0;  // cumulativeCoinsCollected (GlobalCoinCollectionTracker:reset :203-207)
+      for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = 0.0;
+    });
+    // api:start ends with one grid:update (api_factory.lua:101): the ChoiceCoinRegrow updaters already fire at frame 0.
+    // (Spawn points are not coin cells, so no avatar can be standing on a coin that appears now.)
+    for (int k = lane; k < T.nA; k += 32) {
+      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
+      if (u01(w.x, w.y) < T.coin_rate) {
+        const int type = (int)pick(w.z, 2u);
+        S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)(1 + type);
+        grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = cell_value(T.coin_sprite[type], 0);
+      }
     }
+    reset_env_row(T, S, b, lane, episode, 0);
   }
-  __syncwarp();
-  if (lane < T.P) {
-    uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)lane, RS_AVATAR_RESET, k0, k1);
-    const int cell = sc.tmp[lane], orient = (int)(w.y & 3u);
-    int32_t* av = S.avatar + ((size_t)b * T.P + lane) * 4;
-    av[AV_X] = cell % T.W; av[AV_Y] = cell / T.W; av[AV_ORIENT] = orient; av[AV_ALIVE] = 1;
-    int32_t* tm = S.av_timer + ((size_t)b * T.P + lane) * 4;
-    tm[0] = 0; tm[1] = 0; tm[2] = 0; tm[3] = 0;
-    S.av_extra[((size_t)b * T.P + lane) * 8] = 0;  // cumulativeCoinsCollected (GlobalCoinCollectionTracker:reset :203-207)
-    grid[(size_t)T.avatar_layer * T.cells_pad + cell] = cell_value(T.avatar_sprite[lane], orient);
-    S.reward[(size_t)b * T.P + lane] = 0.0;
-    S.packed[(size_t)b * (T.P + 2) + lane] = 0.0;
-    for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = 0.0;
-  }
-  // api:start ends with one grid:update (api_factory.lua:101): the ChoiceCoinRegrow updaters already fire at frame 0.
-  // (Spawn points are not coin cells, so no avatar can be standing on a coin that appears now.)
-  for (int k = lane; k < T.nA; k += 32) {
-    uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-    if (u01(w.x, w.y) < T.coin_rate) {
-      const int type = (int)pick(w.z, 2u);
-      S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)(1 + type);
-      grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = cell_value(T.coin_sprite[type], 0);
-    }
-  }
-  if (lane == 0) {
-    env[ENV_STEP] = 0; env[ENV_EPISODE] = episode; env[ENV_DONE] = 0; env[ENV_DIRT] = 0;
-    env[ENV_CLEANED] = 0; env[ENV_ATE] = 0; env[ENV_BEAM] = 0;
-    S.discount[b] = 0.0; S.step_type[b] = 0;
-    S.packed[(size_t)b * (T.P + 2) + T.P] = 0.0; S.packed[(size_t)b * (T.P + 2) + T.P + 1] = 0.0;
-  }
-  __syncwarp();
-}
 
-__device__ void coins_step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
-  int32_t* env = S.env + (size_t)b * ENV_COLS;
-  const int n = env[ENV_STEP] + 1;
-  const int episode = env[ENV_EPISODE];
-  const uint64_t key = S.seed + (uint64_t)b;
-  const uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-  uint16_t* grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  const bool is_av = lane < T.P;
-  uint8_t* s_state = sc.apple;  // [nA_pad] bits 0-1 state code, bits 4-5 state queued by ChoiceCoinRegrow, bit 6 collected
+  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+    const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
+    const bool is_av = lane < T.P;
+    uint8_t* s_state = sc.apple;  // [nA_pad] bits 0-1 state code, bits 4-5 state queued by ChoiceCoinRegrow, bit 6 collected
 
-  int x = 0, y = 0, orient = 0, cumulative = 0;
-  int act_move = 0, act_turn = 0;
-  if (is_av) {
-    const int4 a = *reinterpret_cast<const int4*>(S.avatar + ((size_t)b * T.P + lane) * 4);
-    x = a.x; y = a.y; orient = a.z;
-    cumulative = S.av_extra[((size_t)b * T.P + lane) * 8];
-    int id = actions[(size_t)b * T.P + lane];
-    if (id < 0 || id >= T.n_actions) id = 0;
-    const int4 at = *reinterpret_cast<const int4*>(T.action_table + id * 4);
-    act_move = at.x; act_turn = at.y;
-  }
-  const int x0 = x, y0 = y, orient0 = orient;
-  double reward = 0.0;     // Avatar:preUpdate (avatar_library.lua:330-332)
-  int partner_mismatch = 0;  // PartnerTracker:preUpdate (coins/components.lua:303-306)
-  bool cont = true;
+    int4 a, t, act;
+    load_avatar(T, S, b, lane, actions, T.action_table, a, t, act);
+    int x = a.x, y = a.y, orient = a.z, cumulative = is_av ? S.av_extra[((size_t)b * T.P + lane) * 8] : 0;
+    const int act_move = act.x, act_turn = act.y;
+    const int x0 = x, y0 = y, orient0 = orient;
+    double reward = 0.0;     // Avatar:preUpdate (avatar_library.lua:330-332)
+    int partner_mismatch = 0;  // PartnerTracker:preUpdate (coins/components.lua:303-306)
+    bool cont = true;
 
-  for (int i = lane; i < T.cells_pad / 4; i += 32)
-    reinterpret_cast<uint32_t*>(sc.occ)[i] = reinterpret_cast<const uint32_t*>(T.solid)[i];
-  for (int k = lane; k < T.nA; k += 32) s_state[k] = S.apple[(size_t)b * T.nA_pad + k];
-  __syncwarp();
-  if (is_av) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
-  __syncwarp();
+    init_occupancy(T, sc.occ, T.solid, lane);
+    for (int k = lane; k < T.nA; k += 32) s_state[k] = S.apple[(size_t)b * T.nA_pad + k];
+    __syncwarp();
+    if (is_av) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
+    __syncwarp();
 
-  // ---- updaters -------------------------------------------------------------------------------------
-  // 150 Avatar movement: the frame's random visiting order (policy A.7).
-  int rank = 99;
-  {
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)lane, RS_AVATAR, k0, k1);
-    const uint32_t mykey = w.x;
-    int r = 0;
-    for (int q = 0; q < T.P; ++q) {
-      const uint32_t kq = __shfl_sync(MP_FULL, mykey, q);
-      if (kq < mykey || (kq == mykey && q < lane)) ++r;
-    }
-    if (is_av) rank = r;
-  }
-  // 100 StochasticIntervalEpisodeEnding (the scene registers first), then ChoiceCoinRegrow on every waiting coin:
-  // probability regrowRate, then random:choice of the two live states (coins/components.lua:183-194).
-  if (n >= T.end_min_frames && ((n + 1) % T.end_interval) == 0) {
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, SCENE_DRAW_EPISODE_END, RS_SCENE, k0, k1);
-    if (u01(w.x, w.y) < T.end_prob) cont = false;
-  }
-  for (int k = lane; k < T.nA; k += 32) {
-    if ((s_state[k] & 3) != 0) continue;
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-    if (u01(w.x, w.y) < T.coin_rate) s_state[k] |= (uint8_t)((1 + pick(w.z, 2u)) << 4);
-  }
-  __syncwarp();
-
-  // Coin:onEnter for collector `who` on coin `k` (every lane calls this with the same arguments).
-  auto collect = [&](int who, int k) {
-    const int type = (s_state[k] & 3) - 1;
-    const bool match = type == T.coin_type[who];
-    const double* R = T.coin_reward[who];  // self match, self mismatch, other match, other mismatch (Role multipliers folded in)
-    if (lane == who) {
-      reward += match ? R[0] : R[1];
-      ++cumulative;
-      if (T.coin_terminate && cumulative >= T.coin_terminate_n) cont = false;
-      emit_event(S, b, EV_COIN_CONSUMED, who + 1, match ? 1 : 0);
-    } else if (is_av) {  // Coin:rewardOthers (:74-85) and PartnerTracker:reportMatch / reportMismatch (:324-330)
-      reward += match ? R[2] : R[3];
-      if (!match) partner_mismatch = 1;
+    // ---- updaters -------------------------------------------------------------------------------------
+    // 150 Avatar movement: the frame's random visiting order (policy A.7).
+    const int rank = visit_rank(T, lane, n, episode, k0, k1);
+    // 100 StochasticIntervalEpisodeEnding (the scene registers first), then ChoiceCoinRegrow on every waiting coin:
+    // probability regrowRate, then random:choice of the two live states (coins/components.lua:183-194).
+    cont = episode_continues(T, n, episode, k0, k1);
+    for (int k = lane; k < T.nA; k += 32) {
+      if ((s_state[k] & 3) != 0) continue;
+      uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
+      if (u01(w.x, w.y) < T.coin_rate) s_state[k] |= (uint8_t)((1 + pick(w.z, 2u)) << 4);
     }
     __syncwarp();
-    if (lane == 0) s_state[k] |= 64;  // setState(waitState) is queued: the coin stays where it is until round 2
-    __syncwarp();
-  };
 
-  // ---- round 1: moves in the frame's order, then the queued coin states in object order -----------------
-  for (int r = 0; r < T.P; ++r) {
-    const unsigned m = __ballot_sync(MP_FULL, is_av && rank == r);
-    const int src = __ffs(m) - 1;
-    const int s_turn = __shfl_sync(MP_FULL, act_turn, src), s_move = __shfl_sync(MP_FULL, act_move, src);
-    int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
-    if (s_turn != 0) so = (so + s_turn) & 3;
-    if (s_move != 0) {
-      const int d = (so + s_move - 1) & 3;
-      int nx = sx + dir_dx(d), ny = sy + dir_dy(d);
-      const bool inb = wrap_or_reject(T, nx, ny);
-      if (inb && sc.occ[ny * T.W + nx] == 0) {
-        __syncwarp();
-        if (lane == 0) { sc.occ[sy * T.W + sx] = 0; sc.occ[ny * T.W + nx] = (uint8_t)(src + 1); }
-        sx = nx; sy = ny;
+    // Coin:onEnter for collector `who` on coin `k` (every lane calls this with the same arguments).
+    auto collect = [&](int who, int k) {
+      const int type = (s_state[k] & 3) - 1;
+      const bool match = type == T.coin_type[who];
+      const double* R = T.coin_reward[who];  // self match, self mismatch, other match, other mismatch (Role multipliers folded in)
+      if (lane == who) {
+        reward += match ? R[0] : R[1];
+        ++cumulative;
+        if (T.coin_terminate && cumulative >= T.coin_terminate_n) cont = false;
+        emit_event(S, b, EV_COIN_CONSUMED, who + 1, match ? 1 : 0);
+      } else if (is_av) {  // Coin:rewardOthers (:74-85) and PartnerTracker:reportMatch / reportMismatch (:324-330)
+        reward += match ? R[2] : R[3];
+        if (!match) partner_mismatch = 1;
       }
       __syncwarp();
-      const int ci = T.apple_of_cell[sy * T.W + sx];  // policy A.5: `enter` fires on the final cell, moved or blocked
+      if (lane == 0) s_state[k] |= 64;  // setState(waitState) is queued: the coin stays where it is until round 2
+      __syncwarp();
+    };
+
+    // ---- round 1: moves in the frame's order, then the queued coin states in object order -----------------
+    // policy A.5: `enter` fires on the final cell, moved or blocked
+    move_avatars(T, lane, rank, true, act_turn, act_move, x, y, orient, sc.occ, [&](int src, int cell) {
+      const int ci = T.apple_of_cell[cell];
       if (ci >= 0 && (s_state[ci] & 3) != 0 && !(s_state[ci] & 64)) collect(src, ci);
+    });
+    const int partner_cont = __all_sync(MP_FULL, cont);  // (cont is per lane so far: either collector may end the episode)
+    cont = partner_cont;
+    for (int base = 0; base < T.nA; base += 32) {
+      const int k = base + lane;
+      const int queued = k < T.nA ? (s_state[k] >> 4) & 3 : 0;
+      if (queued) s_state[k] = (uint8_t)queued;  // now live (placed on superOverlay)
+      __syncwarp();
+      // a coin that appears under a standing avatar is entered at once (contact is symmetric on placement, policy A.5)
+      const int o = queued ? sc.occ[T.ch_apple[k * 4 + 1]] : 0;
+      unsigned gm = __ballot_sync(MP_FULL, o >= 1 && o <= T.P);
+      while (gm) {
+        const int c = __ffs(gm) - 1; gm &= gm - 1;
+        collect(__shfl_sync(MP_FULL, o, c) - 1, base + c);
+      }
     }
-    if (lane == src) { x = sx; y = sy; orient = so; }
-    __syncwarp();
-  }
-  const int partner_cont = __all_sync(MP_FULL, cont);  // (cont is per lane so far: either collector may end the episode)
-  cont = partner_cont;
-  for (int base = 0; base < T.nA; base += 32) {
-    const int k = base + lane;
-    const int queued = k < T.nA ? (s_state[k] >> 4) & 3 : 0;
-    if (queued) s_state[k] = (uint8_t)queued;  // now live (placed on superOverlay)
-    __syncwarp();
-    // a coin that appears under a standing avatar is entered at once (contact is symmetric on placement, policy A.5)
-    const int o = queued ? sc.occ[T.ch_apple[k * 4 + 1]] : 0;
-    unsigned gm = __ballot_sync(MP_FULL, o >= 1 && o <= T.P);
-    while (gm) {
-      const int c = __ffs(gm) - 1; gm &= gm - 1;
-      collect(__shfl_sync(MP_FULL, o, c) - 1, base + c);
+    cont = __all_sync(MP_FULL, cont);
+
+    // ---- round 2 + write back ------------------------------------------------------------------------------
+    for (int k = lane; k < T.nA; k += 32) {
+      const uint8_t now = (s_state[k] & 64) ? 0 : (s_state[k] & 3);
+      const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
+      if (now != was) {
+        S.apple[(size_t)b * T.nA_pad + k] = now;
+        grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = now ? cell_value(T.coin_sprite[now - 1], 0) : (uint16_t)0;
+      }
     }
-  }
-  cont = __all_sync(MP_FULL, cont);
+    draw_avatars(T, grid, lane, x0, y0, orient0, 1, x, y, orient, 1);
 
-  // ---- round 2 + write back ------------------------------------------------------------------------------
-  for (int k = lane; k < T.nA; k += 32) {
-    const uint8_t now = (s_state[k] & 64) ? 0 : (s_state[k] & 3);
-    const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
-    if (now != was) {
-      S.apple[(size_t)b * T.nA_pad + k] = now;
-      grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = now ? cell_value(T.coin_sprite[now - 1], 0) : (uint16_t)0;
+    const bool done = !cont || n >= T.max_frames;
+    if (is_av) {
+      *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, 1);
+      S.av_extra[((size_t)b * T.P + lane) * 8] = cumulative;
+      for (int k = 0; k < T.n_scalar; ++k)  // MISMATCHED_COIN_COLLECTED_BY_PARTNER (coins.py AvatarMetricReporter)
+        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 2 ? (double)partner_mismatch : 0.0;
     }
+    store_timestep(T, S, b, lane, n, reward, done ? 2 : 1, 0);
   }
-  const bool changed = is_av && (x != x0 || y != y0 || orient != orient0);
-  if (changed) grid[(size_t)T.avatar_layer * T.cells_pad + y0 * T.W + x0] = 0;
-  __syncwarp();
-  if (changed) grid[(size_t)T.avatar_layer * T.cells_pad + y * T.W + x] = cell_value(T.avatar_sprite[lane], orient);
-
-  const bool done = !cont || n >= T.max_frames;
-  if (is_av) {
-    *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, 1);
-    S.av_extra[((size_t)b * T.P + lane) * 8] = cumulative;
-    S.reward[(size_t)b * T.P + lane] = reward;
-    S.packed[(size_t)b * (T.P + 2) + lane] = reward;
-    for (int k = 0; k < T.n_scalar; ++k)  // MISMATCHED_COIN_COLLECTED_BY_PARTNER (coins.py AvatarMetricReporter)
-      S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 2 ? (double)partner_mismatch : 0.0;
-  }
-  if (lane == 0) {
-    env[ENV_STEP] = n; env[ENV_DONE] = done ? 1 : 0; env[ENV_BEAM] = 0;
-    S.discount[b] = done ? 0.0 : 1.0;
-    S.step_type[b] = done ? 2 : 1;
-    S.packed[(size_t)b * (T.P + 2) + T.P] = done ? 0.0 : 1.0;
-    S.packed[(size_t)b * (T.P + 2) + T.P + 1] = done ? 2.0 : 1.0;
-  }
-}
-
-__global__ void __launch_bounds__(128, 8) k_step_coins(Tables T, State S, const int32_t* __restrict__ actions,
-                                                   const uint8_t* __restrict__ mask, int mode) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // Programmatic dependent launch, both ways: let the renderer that follows in the stream stage its tables while this
-  // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  const int b = blockIdx.x * 4 + warp;
-  if (b >= S.B) return;
-  WarpScratch sc = carve_scratch(T, smem + warp * warp_scratch_bytes(T));
-  if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
-    event_begin(lane);
-    if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) coins_reset(T, S, b, lane, sc);
-    else coins_step(T, S, b, lane, actions, sc);
-    event_end(S, b, lane);
-  }
-}
+};

@@ -4,7 +4,7 @@
 //   meltingpot/lua/levels/commons_harvest/components.lua (Neighborhoods, DensityRegrow)
 //   meltingpot/lua/modules/component_library.lua:953-1002 (Edible)
 //   meltingpot/lua/modules/avatar_library.lua (Avatar, Zapper)
-// in the same closed form as step_clean_up.cuh: lanes are avatars, beam footprint cells, apples or
+// in the closed form of step_common.cuh: lanes are avatars, beam footprint cells, apples or
 // the disc neighbours of one apple, depending on the phase.
 //
 // Apple state codes (State.apple): 0 live ('apple', lowerPhysical), 1 'appleWait', 2 + k 'appleWait_k'.
@@ -12,345 +12,206 @@
 // incremental (and order dependent) bookkeeping -- see _beginLive / _endLive below.
 #pragma once
 
-#include "common.cuh"
-#include "step_clean_up.cuh"  // WarpScratch, beam_scan
+#include "step_common.cuh"
 
 __device__ __forceinline__ bool ch_is_wait(uint8_t s) { return s != 0; }
 
-// Episode start for commons_harvest.
-__device__ void commons_reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
-  int32_t* env = S.env + (size_t)b * ENV_COLS;
-  const int episode = env[ENV_EPISODE] + 1;
-  const uint64_t key = S.seed + (uint64_t)b;
-  const uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-  uint16_t* grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  __syncwarp();
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(T.init_grid);
-    uint4* dst = reinterpret_cast<uint4*>(grid);
-    const int n16 = T.L * T.cells_pad / 8;
-    for (int i = lane; i < n16; i += 32) dst[i] = src[i];
-  }
-  for (int k = lane; k < T.nA; k += 32) {  // DensityRegrow:start -> count 0; all apples start live
-    S.apple[(size_t)b * T.nA_pad + k] = T.ch_apple[k * 4 + 2] ? 0 : 1;
-    S.apple_count[(size_t)b * T.nA_pad + k] = 0;
-  }
-  __syncwarp();
-  // _avatarStart: one partial Fisher-Yates per spawn group (base_simulation.lua:396-445).
-  for (int g = 0; g < 2; ++g) {
-    const int n = T.n_spawn_init[g];
-    if (n == 0) continue;
-    for (int i = lane; i < n && i < 64; i += 32) sc.tmp[i] = (int16_t)T.spawn_init_cell[g][i];
+struct Commons {
+  using Scratch = WarpScratch;
+  static constexpr bool kStagesTables = false;
+  __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
+  __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
+  __device__ static void stage(const Tables&, uint8_t*) {}
+  __device__ static WarpScratch carve(const Tables& T, uint8_t* base, const uint8_t*) { return carve_scratch(T, base); }
+
+  // Episode start for commons_harvest: one spawn group per initial group of avatars.
+  __device__ static void reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
+    const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
     __syncwarp();
-    if (lane == 0) {
-      int j = 0;
-      for (int p = 0; p < T.P; ++p) {
-        if (T.avatar_init_group[p] != g) continue;
-        uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)p, RS_AVATAR_RESET, k0, k1);
-        int r = j + (int)pick(w.x, (uint32_t)(n - j));
-        int16_t t = sc.tmp[j]; sc.tmp[j] = sc.tmp[r]; sc.tmp[r] = t;
-        sc.occ[p] = (uint8_t)j;  // slot of avatar p inside this group's shuffle
-        ++j;
-      }
+    copy_init_grid(T, grid, lane);
+    for (int k = lane; k < T.nA; k += 32) {  // DensityRegrow:start -> count 0; all apples start live
+      S.apple[(size_t)b * T.nA_pad + k] = T.ch_apple[k * 4 + 2] ? 0 : 1;
+      S.apple_count[(size_t)b * T.nA_pad + k] = 0;
     }
     __syncwarp();
-    if (lane < T.P && T.avatar_init_group[lane] == g) {
-      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)lane, RS_AVATAR_RESET, k0, k1);
-      int cell = sc.tmp[sc.occ[lane]], orient = (int)(w.y & 3u);
-      int32_t* av = S.avatar + ((size_t)b * T.P + lane) * 4;
-      av[AV_X] = cell % T.W; av[AV_Y] = cell / T.W; av[AV_ORIENT] = orient; av[AV_ALIVE] = 1;
-      int32_t* tm = S.av_timer + ((size_t)b * T.P + lane) * 4;
-      tm[TM_ZAP] = 0; tm[TM_BEAM2] = 0; tm[TM_FRAME] = 0; tm[3] = 0;
-      grid[(size_t)T.avatar_layer * T.cells_pad + cell] = cell_value(T.avatar_sprite[lane], orient);
-      S.reward[(size_t)b * T.P + lane] = 0.0;
-      S.packed[(size_t)b * (T.P + 2) + lane] = 0.0;
-      for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 : 0.0;
+    for (int g = 0; g < 2; ++g) {
+      if (T.n_spawn_init[g] == 0) continue;
+      spawn_group(T, S, b, lane, grid, sc.tmp, T.spawn_init_cell[g], T.n_spawn_init[g], [&](int p) { return T.avatar_init_group[p] == g; },
+                  [](int) { return true; }, episode, k0, k1, [&](int) {
+        for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 : 0.0;
+      });
+    }
+    reset_env_row(T, S, b, lane, episode, 0);
+  }
+
+  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+    const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
+    const bool is_av = lane < T.P;
+    uint8_t* s_state = sc.apple;  // [nA_pad] bits 0-4 state code, bit 5 sprouts, bit 6 eaten
+    uint8_t* s_count = sc.dirt;   // [nA_pad]
+    int16_t* s_events = sc.tmp;   // eaten-apple queue (round 2), in event order
+
+    int4 a, t, act;
+    load_avatar(T, S, b, lane, actions, T.action_table, a, t, act);
+    int x = a.x, y = a.y, orient = a.z, alive = a.w, zap_cool = t.x, state_frame = t.z;
+    const int act_move = act.x, act_turn = act.y, act_zap = act.z;
+    const int x0 = x, y0 = y, orient0 = orient, alive0 = alive;
+    double reward = 0.0;
+
+    init_occupancy(T, sc.occ, T.solid, lane);
+    for (int k = lane; k < T.nA; k += 32) { s_state[k] = S.apple[(size_t)b * T.nA_pad + k]; s_count[k] = S.apple_count[(size_t)b * T.nA_pad + k]; }
+    const int words = (T.cells + 31) / 32 + 1;
+    for (int i = lane; i < words; i += 32) sc.beam_zap[i] = 0;
+    __syncwarp();
+    if (is_av && alive) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
+    if (env[ENV_BEAM]) clear_layer(T, grid, T.zap_layer, lane);
+    __syncwarp();
+    int beam_dirty = 0;
+
+    // ---- simulation:update: DensityRegrow:update -> _updateWaitState (components.lua:147-193) ------
+    // and the priority-10 sprout updaters (:92-123), evaluated on the state the apple has NOW.
+    for (int k = lane; k < T.nA; k += 32) {
+      const uint8_t st = s_state[k];
+      if (!ch_is_wait(st)) continue;
+      if (st >= 2) {  // in some appleWait_j: its updater fires with probability probs[min(j, n-1)]
+        const int j = st - 2;
+        const double p = T.ch_probs[j < T.ch_n_probs ? j : T.ch_n_probs - 1];
+        if (p > 0.0) {
+          uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
+          if (u01(w.x, w.y) < p) s_state[k] |= 32;
+        }
+      }
+      // relabel to appleWait_count and toggle the grass below (processed first in the queue)
+      int c = s_count[k]; if (c >= T.ch_n_wait) c = T.ch_n_wait - 1;
+      s_state[k] = (s_state[k] & 32) | (uint8_t)(2 + c);
+      const int cell = T.ch_apple[k * 4 + 1];
+      if (T.ch_apple[k * 4 + 3] >= 0)
+        grid[(size_t)T.grass_layer * T.cells_pad + cell] = cell_value(c == 0 ? T.dess_sprite : T.grass_sprite, 0);
     }
     __syncwarp();
-  }
-  if (lane == 0) {
-    env[ENV_STEP] = 0; env[ENV_EPISODE] = episode; env[ENV_DONE] = 0; env[ENV_DIRT] = 0;
-    env[ENV_CLEANED] = 0; env[ENV_ATE] = 0; env[ENV_BEAM] = 0;
-    S.discount[b] = 0.0; S.step_type[b] = 0;
-    S.packed[(size_t)b * (T.P + 2) + T.P] = 0.0; S.packed[(size_t)b * (T.P + 2) + T.P + 1] = 0.0;
-  }
-  __syncwarp();
-}
 
-__device__ void commons_step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
-  int32_t* env = S.env + (size_t)b * ENV_COLS;
-  const int n = env[ENV_STEP] + 1;
-  const int episode = env[ENV_EPISODE];
-  const uint64_t key = S.seed + (uint64_t)b;
-  const uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-  uint16_t* grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  const bool is_av = lane < T.P;
-  uint8_t* s_state = sc.apple;  // [nA_pad] bits 0-4 state code, bit 5 sprouts, bit 6 eaten
-  uint8_t* s_count = sc.dirt;   // [nA_pad]
-  int16_t* s_events = sc.tmp;   // eaten-apple queue (round 2), in event order
+    // ---- updaters ------------------------------------------------------------------------------------
+    const int rank = visit_rank(T, lane, n, episode, k0, k1);
+    bool fire_zap = false;
+    if (is_av && alive) { if (zap_cool > 0) --zap_cool; else if (act_zap == 1) { zap_cool = T.zap_cooldown; fire_zap = true; } }
+    const bool want_respawn = is_av && !alive && (n - state_frame) >= T.zap_respawn;
+    const bool cont = episode_continues(T, n, episode, k0, k1);
 
-  int x = 0, y = 0, orient = 0, alive = 0, zap_cool = 0, state_frame = 0;
-  int act_move = 0, act_turn = 0, act_zap = 0;
-  if (is_av) {
-    const int4 a = *reinterpret_cast<const int4*>(S.avatar + ((size_t)b * T.P + lane) * 4);
-    const int4 t = *reinterpret_cast<const int4*>(S.av_timer + ((size_t)b * T.P + lane) * 4);
-    x = a.x; y = a.y; orient = a.z; alive = a.w; zap_cool = t.x; state_frame = t.z;
-    int id = actions[(size_t)b * T.P + lane];
-    if (id < 0 || id >= T.n_actions) id = 0;
-    const int4 at = *reinterpret_cast<const int4*>(T.action_table + id * 4);
-    act_move = at.x; act_turn = at.y; act_zap = at.z;
-  }
-  const int x0 = x, y0 = y, orient0 = orient, alive0 = alive;
-  double reward = 0.0;
-
-  for (int i = lane; i < T.cells_pad / 4; i += 32)
-    reinterpret_cast<uint32_t*>(sc.occ)[i] = reinterpret_cast<const uint32_t*>(T.solid)[i];
-  for (int k = lane; k < T.nA; k += 32) { s_state[k] = S.apple[(size_t)b * T.nA_pad + k]; s_count[k] = S.apple_count[(size_t)b * T.nA_pad + k]; }
-  const int words = (T.cells + 31) / 32 + 1;
-  for (int i = lane; i < words; i += 32) sc.beam_zap[i] = 0;
-  __syncwarp();
-  if (is_av && alive) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
-  if (env[ENV_BEAM]) {
-    uint4 z = make_uint4(0, 0, 0, 0);
-    uint4* lz = reinterpret_cast<uint4*>(grid + (size_t)T.zap_layer * T.cells_pad);
-    for (int i = lane; i < T.cells_pad / 8; i += 32) lz[i] = z;
-  }
-  __syncwarp();
-  int beam_dirty = 0;
-
-  // ---- simulation:update: DensityRegrow:update -> _updateWaitState (components.lua:147-193) ------
-  // and the priority-10 sprout updaters (:92-123), evaluated on the state the apple has NOW.
-  for (int k = lane; k < T.nA; k += 32) {
-    const uint8_t st = s_state[k];
-    if (!ch_is_wait(st)) continue;
-    if (st >= 2) {  // in some appleWait_j: its updater fires with probability probs[min(j, n-1)]
-      const int j = st - 2;
-      const double p = T.ch_probs[j < T.ch_n_probs ? j : T.ch_n_probs - 1];
-      if (p > 0.0) {
-        uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-        if (u01(w.x, w.y) < p) s_state[k] |= 32;
-      }
-    }
-    // relabel to appleWait_count and toggle the grass below (processed first in the queue)
-    int c = s_count[k]; if (c >= T.ch_n_wait) c = T.ch_n_wait - 1;
-    s_state[k] = (s_state[k] & 32) | (uint8_t)(2 + c);
-    const int cell = T.ch_apple[k * 4 + 1];
-    if (T.ch_apple[k * 4 + 3] >= 0)
-      grid[(size_t)T.grass_layer * T.cells_pad + cell] = cell_value(c == 0 ? T.dess_sprite : T.grass_sprite, 0);
-  }
-  __syncwarp();
-
-  // ---- updaters ------------------------------------------------------------------------------------
-  int rank = 0;
-  {
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)lane, RS_AVATAR, k0, k1);
-    uint32_t mykey = w.x;
-    for (int q = 0; q < T.P; ++q) {
-      uint32_t kq = __shfl_sync(MP_FULL, mykey, q);
-      if (is_av && (kq < mykey || (kq == mykey && q < lane))) ++rank;
-    }
-    if (!is_av) rank = 99;
-  }
-  bool fire_zap = false;
-  if (is_av && alive) { if (zap_cool > 0) --zap_cool; else if (act_zap == 1) { zap_cool = T.zap_cooldown; fire_zap = true; } }
-  const bool want_respawn = is_av && !alive && (n - state_frame) >= T.zap_respawn;
-  bool cont = true;
-  if (n >= T.end_min_frames && ((n + 1) % T.end_interval) == 0) {
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, SCENE_DRAW_EPISODE_END, RS_SCENE, k0, k1);
-    if (u01(w.x, w.y) < T.end_prob) cont = false;
-  }
-
-  // ---- round 1 ---------------------------------------------------------------------------------------
-  int n_events = 0;  // uniform across the warp
-  // moves
-  for (int r = 0; r < T.P; ++r) {
-    unsigned m = __ballot_sync(MP_FULL, is_av && rank == r);
-    int src = __ffs(m) - 1;
-    int s_alive = __shfl_sync(MP_FULL, alive, src);
-    if (!s_alive) continue;
-    int s_turn = __shfl_sync(MP_FULL, act_turn, src), s_move = __shfl_sync(MP_FULL, act_move, src);
-    int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
-    if (s_turn != 0) so = (so + s_turn) & 3;
-    bool ate = false;
-    if (s_move != 0) {
-      int d = (so + s_move - 1) & 3;
-      int nx = sx + dir_dx(d), ny = sy + dir_dy(d);
-      bool inb = wrap_or_reject(T, nx, ny);
-      if (inb && sc.occ[ny * T.W + nx] == 0) {
-        __syncwarp();
-        if (lane == 0) { sc.occ[sy * T.W + sx] = 0; sc.occ[ny * T.W + nx] = (uint8_t)(src + 1); }
-        sx = nx; sy = ny;
-      }
-      const int ai = T.apple_of_cell[sy * T.W + sx];
-      ate = ai >= 0 && (s_state[ai] & 31) == 0;  // Edible:onEnter on a live apple (component_library.lua:990-1002)
-      const bool fresh = ate && !(s_state[ai] & 64);  // a second setState(appleWait) would be a no-op
+    // ---- round 1 ---------------------------------------------------------------------------------------
+    int n_events = 0;  // uniform across the warp
+    // Edible:onEnter of an avatar arriving on `cell` with a live apple (component_library.lua:990-1002); a second
+    // setState(appleWait) of the same apple would be a no-op, so the queue holds each apple once.
+    const auto eat = [&](int src, int cell) {
+      const int ai = T.apple_of_cell[cell];
+      const bool ate = ai >= 0 && (s_state[ai] & 31) == 0;
+      const bool fresh = ate && !(s_state[ai] & 64);
       __syncwarp();
       if (fresh) {
         if (lane == 0) { s_state[ai] |= 64; s_events[n_events] = (int16_t)ai; }
         ++n_events;
       }
-    }
-    if (lane == src) { x = sx; y = sy; orient = so; if (ate) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, src + 1, 0); } }
-    __syncwarp();
-  }
-  // zap beams
-  unsigned zapped = 0;
-  for (int r = 0; r < T.P; ++r) {
-    unsigned m = __ballot_sync(MP_FULL, is_av && rank == r && fire_zap);
-    if (!m) continue;
-    int src = __ffs(m) - 1;
-    int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
-    const BeamGeom& G = T.zap_geom;
-    int cell = -1; bool blocked = false; int hit_avatar = -1;
-    if (lane < G.n) {
-      int f = so, rgt = (so + 1) & 3;
-      int cx = sx + dir_dx(f) * G.fwd[lane] + dir_dx(rgt) * G.lat[lane];
-      int cy = sy + dir_dy(f) * G.fwd[lane] + dir_dy(rgt) * G.lat[lane];
-      if (!wrap_or_reject(T, cx, cy)) blocked = true;
-      else {
-        cell = cy * T.W + cx;
+      if (ate && lane == src) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, src + 1, 0); }
+    };
+    move_avatars(T, lane, rank, is_av && alive, act_turn, act_move, x, y, orient, sc.occ, eat);
+    // zap beams
+    unsigned zapped = 0;
+    for (int r = 0; r < T.P; ++r) {
+      unsigned m = __ballot_sync(MP_FULL, is_av && rank == r && fire_zap);
+      if (!m) continue;
+      int src = __ffs(m) - 1;
+      int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
+      const BeamGeom& G = T.zap_geom;
+      const int cell = beam_cell(T, G, lane, sx, sy, so);
+      int hit_avatar = -1;
+    bool blocked = cell < 0 && lane < G.n;  // off the map
+      if (cell >= 0) {
         if (T.cell_flags[cell] & (1 << T.zap_hit)) blocked = true;
         int o = sc.occ[cell];
         if (o >= 1 && o <= T.P && o - 1 != src) { hit_avatar = o - 1; blocked = true; }
       }
-    }
-    bool vis;
-    beam_scan(G, lane, blocked, vis);
-    unsigned hm = __ballot_sync(MP_FULL, vis && hit_avatar >= 0);
-    while (hm) {
-      int c = __ffs(hm) - 1; hm &= hm - 1;
-      int t = __shfl_sync(MP_FULL, hit_avatar, c);
-      if (lane == t) reward += T.zap_penalty;
-      if (lane == src) { reward += T.zap_reward; emit_event(S, b, EV_ZAP, src + 1, t + 1); }
-      if (T.zap_remove) zapped |= 1u << t;
-    }
-    if (vis && !blocked && cell >= 0) {
-      uint32_t bit = 1u << (cell & 31);
-      uint32_t old = atomicOr(&sc.beam_zap[cell >> 5], bit);
-      if (!(old & bit)) grid[(size_t)T.zap_layer * T.cells_pad + cell] = cell_value(T.zap_sprite, so);
-      beam_dirty = 1;
-    }
-    __syncwarp();
-  }
-  beam_dirty = __any_sync(MP_FULL, beam_dirty);
-  // respawns (teleportToGroup to the post-initial spawn group)
-  for (int r = 0; r < T.P; ++r) {
-    unsigned m = __ballot_sync(MP_FULL, is_av && rank == r && want_respawn);
-    if (!m) continue;
-    int src = __ffs(m) - 1;
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)src, RS_AVATAR, k0, k1);
-    int target = T.spawn_cell[pick(w.y, (uint32_t)T.n_spawn)];
-    if (sc.occ[target] != 0) continue;
-    __syncwarp();
-    if (lane == 0) sc.occ[target] = (uint8_t)(src + 1);
-    int ai = T.apple_of_cell[target];
-    bool ate = ai >= 0 && (s_state[ai] & 31) == 0;
-    bool fresh = ate && !(s_state[ai] & 64);
-    __syncwarp();
-    if (fresh && lane == 0) { s_state[ai] |= 64; s_events[n_events] = (int16_t)ai; }
-    if (fresh) ++n_events;
-    if (lane == src) {
-      x = target % T.W; y = target / T.W; orient = (int)(w.z & 3u); alive = 1; state_frame = n;
-      if (ate) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, src + 1, 0); }
-    }
-    __syncwarp();
-  }
-  // sprouts, in object order: setState(live) -> _beginLive (components.lua:206-219) -> contact.
-  for (int base = 0; base < T.nA; base += 32) {
-    int k = base + lane;
-    unsigned sm = __ballot_sync(MP_FULL, k < T.nA && (s_state[k] & 32));
-    while (sm) {
-      const int i = base + __ffs(sm) - 1; sm &= sm - 1;
-      __syncwarp();
-      if (lane == 0) s_state[i] = 0;  // live
-      __syncwarp();
-      if (lane < 16) {  // every wait neighbour inside the disc gains one
-        const int j = T.ch_nbr[i * 16 + lane];
-        if (j >= 0 && ch_is_wait(s_state[j] & 31)) s_count[j] += 1;
+      bool vis;
+      beam_scan(G, lane, blocked, vis);
+      unsigned hm = __ballot_sync(MP_FULL, vis && hit_avatar >= 0);
+      while (hm) {
+        int c = __ffs(hm) - 1; hm &= hm - 1;
+        int t = __shfl_sync(MP_FULL, hit_avatar, c);
+        if (lane == t) reward += T.zap_penalty;
+        if (lane == src) { reward += T.zap_reward; emit_event(S, b, EV_ZAP, src + 1, t + 1); }
+        if (T.zap_remove) zapped |= 1u << t;
       }
-      const int cell = T.ch_apple[i * 4 + 1];
-      const int o = sc.occ[cell];
-      if (o >= 1 && o <= T.P) {  // an avatar stands here: eaten at once
-        if (lane == o - 1) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, o, 0); }
+      if (vis && !blocked) { draw_hit_sprite(T, grid, sc.beam_zap, T.zap_layer, cell, cell_value(T.zap_sprite, so)); beam_dirty = 1; }
+      __syncwarp();
+    }
+    beam_dirty = __any_sync(MP_FULL, beam_dirty);
+    // respawns (teleportToGroup to the post-initial spawn group)
+    respawn_avatars(T, lane, rank, want_respawn, n, episode, k0, k1, sc.occ, x, y, orient, alive, state_frame, eat);
+    // sprouts, in object order: setState(live) -> _beginLive (components.lua:206-219) -> contact.
+    for (int base = 0; base < T.nA; base += 32) {
+      int k = base + lane;
+      unsigned sm = __ballot_sync(MP_FULL, k < T.nA && (s_state[k] & 32));
+      while (sm) {
+        const int i = base + __ffs(sm) - 1; sm &= sm - 1;
         __syncwarp();
-        if (lane == 0) { s_state[i] |= 64; s_events[n_events] = (int16_t)i; }
-        ++n_events;
+        if (lane == 0) s_state[i] = 0;  // live
+        __syncwarp();
+        if (lane < 16) {  // every wait neighbour inside the disc gains one
+          const int j = T.ch_nbr[i * 16 + lane];
+          if (j >= 0 && ch_is_wait(s_state[j] & 31)) s_count[j] += 1;
+        }
+        const int cell = T.ch_apple[i * 4 + 1];
+        const int o = sc.occ[cell];
+        if (o >= 1 && o <= T.P) {  // an avatar stands here: eaten at once
+          if (lane == o - 1) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, o, 0); }
+          __syncwarp();
+          if (lane == 0) { s_state[i] |= 64; s_events[n_events] = (int16_t)i; }
+          ++n_events;
+        }
+        __syncwarp();
       }
+    }
+
+    // ---- round 2: setState(appleWait) of eaten apples -> _endLive (components.lua:221-240) ----------
+    for (int e = 0; e < n_events; ++e) {
+      const int i = s_events[e];
+      __syncwarp();
+      if (lane == 0) s_state[i] = 1;  // plain 'appleWait' (layer logic)
+      __syncwarp();
+      int live = 0;
+      if (lane < 16) {
+        const int j = T.ch_nbr[i * 16 + lane];
+        if (j >= 0) {
+          if (ch_is_wait(s_state[j] & 31)) s_count[j] -= 1; else live = 1;
+        }
+      }
+      const unsigned lm = __ballot_sync(MP_FULL, live);
+      if (lane == 0) s_count[i] = (uint8_t)__popc(lm);  // liveNeighbors inside the disc (self is no longer live)
       __syncwarp();
     }
-  }
+    if (is_av && (zapped >> lane & 1u)) { alive = 0; state_frame = n; }
 
-  // ---- round 2: setState(appleWait) of eaten apples -> _endLive (components.lua:221-240) ----------
-  for (int e = 0; e < n_events; ++e) {
-    const int i = s_events[e];
-    __syncwarp();
-    if (lane == 0) s_state[i] = 1;  // plain 'appleWait' (layer logic)
-    __syncwarp();
-    int live = 0;
-    if (lane < 16) {
-      const int j = T.ch_nbr[i * 16 + lane];
-      if (j >= 0) {
-        if (ch_is_wait(s_state[j] & 31)) s_count[j] -= 1; else live = 1;
+    // ---- write back -----------------------------------------------------------------------------------
+    for (int k = lane; k < T.nA; k += 32) {
+      const uint8_t now = s_state[k] & 31;
+      const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
+      if (now != was) {
+        S.apple[(size_t)b * T.nA_pad + k] = now;
+        const int cell = T.ch_apple[k * 4 + 1];
+        if ((now == 0) != (was == 0)) {  // moved between lowerPhysical and logic
+          grid[(size_t)T.apple_layer * T.cells_pad + cell] = now == 0 ? cell_value(T.apple_sprite, 0) : (uint16_t)0;
+          grid[(size_t)T.wait_layer * T.cells_pad + cell] = now == 0 ? (uint16_t)0 : cell_value(T.wait_sprite, 0);
+        }
       }
+      S.apple_count[(size_t)b * T.nA_pad + k] = s_count[k];
     }
-    const unsigned lm = __ballot_sync(MP_FULL, live);
-    if (lane == 0) s_count[i] = (uint8_t)__popc(lm);  // liveNeighbors inside the disc (self is no longer live)
-    __syncwarp();
-  }
-  if (is_av && (zapped >> lane & 1u)) { alive = 0; state_frame = n; }
+    draw_avatars(T, grid, lane, x0, y0, orient0, alive0, x, y, orient, alive);
 
-  // ---- write back -----------------------------------------------------------------------------------
-  for (int k = lane; k < T.nA; k += 32) {
-    const uint8_t now = s_state[k] & 31;
-    const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
-    if (now != was) {
-      S.apple[(size_t)b * T.nA_pad + k] = now;
-      const int cell = T.ch_apple[k * 4 + 1];
-      if ((now == 0) != (was == 0)) {  // moved between lowerPhysical and logic
-        grid[(size_t)T.apple_layer * T.cells_pad + cell] = now == 0 ? cell_value(T.apple_sprite, 0) : (uint16_t)0;
-        grid[(size_t)T.wait_layer * T.cells_pad + cell] = now == 0 ? (uint16_t)0 : cell_value(T.wait_sprite, 0);
-      }
+    const bool done = !cont || n >= T.max_frames;
+    if (is_av) {
+      *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, alive);
+      *reinterpret_cast<int4*>(S.av_timer + ((size_t)b * T.P + lane) * 4) = make_int4(zap_cool, 0, state_frame, 0);
+      for (int k = 0; k < T.n_scalar; ++k)
+        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = alive ? fmax(1.0 - (double)zap_cool / (double)T.zap_cooldown, 0.0) : 0.0;
     }
-    S.apple_count[(size_t)b * T.nA_pad + k] = s_count[k];
+    store_timestep(T, S, b, lane, n, reward, done ? 2 : 1, beam_dirty);
   }
-  const bool changed = is_av && (x != x0 || y != y0 || orient != orient0 || alive != alive0);
-  if (changed && alive0) grid[(size_t)T.avatar_layer * T.cells_pad + y0 * T.W + x0] = 0;
-  __syncwarp();
-  if (changed && alive) grid[(size_t)T.avatar_layer * T.cells_pad + y * T.W + x] = cell_value(T.avatar_sprite[lane], orient);
-
-  const bool done = !cont || n >= T.max_frames;
-  if (is_av) {
-    *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, alive);
-    *reinterpret_cast<int4*>(S.av_timer + ((size_t)b * T.P + lane) * 4) = make_int4(zap_cool, 0, state_frame, 0);
-    S.reward[(size_t)b * T.P + lane] = reward;
-    S.packed[(size_t)b * (T.P + 2) + lane] = reward;
-    for (int k = 0; k < T.n_scalar; ++k)
-      S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = alive ? fmax(1.0 - (double)zap_cool / (double)T.zap_cooldown, 0.0) : 0.0;
-  }
-  if (lane == 0) {
-    env[ENV_STEP] = n; env[ENV_DONE] = done ? 1 : 0; env[ENV_BEAM] = beam_dirty;
-    S.discount[b] = done ? 0.0 : 1.0;
-    S.step_type[b] = done ? 2 : 1;
-    S.packed[(size_t)b * (T.P + 2) + T.P] = done ? 0.0 : 1.0;
-    S.packed[(size_t)b * (T.P + 2) + T.P + 1] = done ? 2.0 : 1.0;
-  }
-}
-
-__global__ void __launch_bounds__(128, 8) k_step_commons(Tables T, State S, const int32_t* __restrict__ actions,
-                                                     const uint8_t* __restrict__ mask, int mode) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // Programmatic dependent launch, both ways: let the renderer that follows in the stream stage its tables while this
-  // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  const int b = blockIdx.x * 4 + warp;
-  if (b >= S.B) return;
-  WarpScratch sc = carve_scratch(T, smem + warp * warp_scratch_bytes(T));
-  if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
-    event_begin(lane);
-    if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) commons_reset(T, S, b, lane, sc);
-    else commons_step(T, S, b, lane, actions, sc);
-    event_end(S, b, lane);
-  }
-}
+};

@@ -19,282 +19,176 @@
 // land in the next round.
 #pragma once
 
-#include "common.cuh"
-#include "step_clean_up.cuh"  // WarpScratch
+#include "step_common.cuh"
 
-__device__ void mining_reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
-  int32_t* env = S.env + (size_t)b * ENV_COLS;
-  const int episode = env[ENV_EPISODE] + 1;
-  const uint64_t key = S.seed + (uint64_t)b;
-  const uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-  uint16_t* grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  __syncwarp();
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(T.init_grid);
-    uint4* dst = reinterpret_cast<uint4*>(grid);
-    const int n16 = T.L * T.cells_pad / 8;
-    for (int i = lane; i < n16; i += 32) dst[i] = src[i];
-  }
-  for (int k = lane; k < T.nA; k += 32) {  // Ore:reset (:96-103): every ore waits, nobody is mining
-    S.apple[(size_t)b * T.nA_pad + k] = 0;
-    S.dirt[(size_t)b * T.nD_pad + k] = 0;
-    S.apple_count[(size_t)b * T.nA_pad + k] = 0;
-  }
-  __syncwarp();
-  // _avatarStart: partial Fisher-Yates over the spawn group (base_simulation.lua:396-445), policy A.10.
-  const int n = T.n_spawn_init[0];
-  for (int i = lane; i < n && i < 64; i += 32) sc.tmp[i] = (int16_t)T.spawn_init_cell[0][i];
-  __syncwarp();
-  if (lane == 0) {
-    for (int p = 0; p < T.P; ++p) {
-      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)p, RS_AVATAR_RESET, k0, k1);
-      int r = p + (int)pick(w.x, (uint32_t)(n - p));
-      int16_t t = sc.tmp[p]; sc.tmp[p] = sc.tmp[r]; sc.tmp[r] = t;
-    }
-  }
-  __syncwarp();
-  if (lane < T.P) {
-    uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)lane, RS_AVATAR_RESET, k0, k1);
-    const int cell = sc.tmp[lane], orient = (int)(w.y & 3u);
-    int32_t* av = S.avatar + ((size_t)b * T.P + lane) * 4;
-    av[AV_X] = cell % T.W; av[AV_Y] = cell / T.W; av[AV_ORIENT] = orient; av[AV_ALIVE] = 1;
-    int32_t* tm = S.av_timer + ((size_t)b * T.P + lane) * 4;
-    tm[0] = 0; tm[1] = 0; tm[2] = 0; tm[3] = 0;  // MineBeam:start (:254-261): ready to shoot
-    grid[(size_t)T.avatar_layer * T.cells_pad + cell] = cell_value(T.avatar_sprite[lane], orient);
-    S.reward[(size_t)b * T.P + lane] = 0.0;
-    S.packed[(size_t)b * (T.P + 2) + lane] = 0.0;
-    for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 : 0.0;
-  }
-  __syncwarp();
-  // api:start ends with one grid:update (api_factory.lua:101): the FixedRateRegrow updaters already fire at frame 0
-  // (the component updates do not run then). Spawn points are not ore cells; the avatar check is kept for symmetry.
-  for (int k = lane; k < T.nA; k += 32) {
-    uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-    const bool first = u01(w.x, w.y) < T.mine_rate[0], second = u01(w.z, w.w) < T.mine_rate[1];
-    const int cell = T.ch_apple[k * 4 + 1];
-    if ((first || second) && grid[(size_t)T.avatar_layer * T.cells_pad + cell] == 0) {
-      const int now = second ? 2 : 1;
-      S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)now;
-      grid[(size_t)T.apple_layer * T.cells_pad + cell] = cell_value(T.ore_sprite[now], 0);
-    }
-  }
-  if (lane == 0) {
-    env[ENV_STEP] = 0; env[ENV_EPISODE] = episode; env[ENV_DONE] = 0; env[ENV_DIRT] = 0;
-    env[ENV_CLEANED] = 0; env[ENV_ATE] = 0; env[ENV_BEAM] = 0;
-    S.discount[b] = 0.0; S.step_type[b] = 0;
-    S.packed[(size_t)b * (T.P + 2) + T.P] = 0.0; S.packed[(size_t)b * (T.P + 2) + T.P + 1] = 0.0;
-  }
-  __syncwarp();
-}
+struct Mining {
+  using Scratch = WarpScratch;
+  static constexpr bool kStagesTables = false;
+  __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
+  __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
+  __device__ static void stage(const Tables&, uint8_t*) {}
+  __device__ static WarpScratch carve(const Tables& T, uint8_t* base, const uint8_t*) { return carve_scratch(T, base); }
 
-__device__ void mining_step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
-  int32_t* env = S.env + (size_t)b * ENV_COLS;
-  const int n = env[ENV_STEP] + 1;
-  const int episode = env[ENV_EPISODE];
-  const uint64_t key = S.seed + (uint64_t)b;
-  const uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-  uint16_t* grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  const bool is_av = lane < T.P;
-  // bits 0-1 state code; bits 2-3 state set in round 1 (1 single-miner ore, 2 two-miner ore; by a reset or by
-  // regrowth, never both); bits 4-5 what the frame's last hit asked for (1 partial state, 2 wait state)
-  uint8_t* s_state = sc.apple;
-  uint8_t* s_miners = sc.dirt;
-  uint8_t* cd = S.apple_count + (size_t)b * T.nA_pad;  // count-down, touched by its own lane or by lane 0 between barriers
-
-  int x = 0, y = 0, orient = 0, cool = 0;
-  int act_move = 0, act_turn = 0, act_mine = 0;
-  if (is_av) {
-    const int4 a = *reinterpret_cast<const int4*>(S.avatar + ((size_t)b * T.P + lane) * 4);
-    x = a.x; y = a.y; orient = a.z;
-    cool = S.av_timer[((size_t)b * T.P + lane) * 4];
-    int id = actions[(size_t)b * T.P + lane];
-    if (id < 0 || id >= T.n_actions) id = 0;
-    const int4 at = *reinterpret_cast<const int4*>(T.action_table + id * 4);
-    act_move = at.x; act_turn = at.y; act_mine = at.z;
-  }
-  const int x0 = x, y0 = y, orient0 = orient;
-  double reward = 0.0;  // Avatar:preUpdate (avatar_library.lua:330-332)
-
-  for (int i = lane; i < T.cells_pad / 4; i += 32)
-    reinterpret_cast<uint32_t*>(sc.occ)[i] = reinterpret_cast<const uint32_t*>(T.solid)[i];
-  for (int k = lane; k < T.nA; k += 32) { s_state[k] = S.apple[(size_t)b * T.nA_pad + k]; s_miners[k] = S.dirt[(size_t)b * T.nD_pad + k]; }
-  const int words = (T.cells + 31) / 32 + 1;
-  for (int i = lane; i < words; i += 32) sc.beam_zap[i] = 0;
-  __syncwarp();
-  if (is_av) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
-  if (env[ENV_BEAM]) {  // hit sprites last one frame (policy A.8)
-    uint4 z = make_uint4(0, 0, 0, 0);
-    uint4* lz = reinterpret_cast<uint4*>(grid + (size_t)T.zap_layer * T.cells_pad);
-    for (int i = lane; i < T.cells_pad / 8; i += 32) lz[i] = z;
-  }
-  __syncwarp();
-
-  // ---- component updates -----------------------------------------------------------------------------
-  // MineBeam:update (:236-252): cool down, then fire if asked to and ready.
-  bool fire = false;
-  if (is_av) { if (cool > 0) --cool; if (act_mine == 1 && cool == 0) { cool = T.zap_cooldown; fire = true; } }
-  // Ore:update (:104-109): the window of a partly mined ore runs out -> reset: forget the miners, back to raw.
-  for (int k = lane; k < T.nA; k += 32) {
-    if (cd[k] > 0 && --cd[k] == 0) {
-      s_miners[k] = 0;
-      if ((s_state[k] & 3) != 0) s_state[k] |= 2 << 2;
-    }
-  }
-  // ---- updaters --------------------------------------------------------------------------------------
-  // 200 FixedRateRegrow (:41-57): one updater per live state, each with its own draw, only where no avatar stands
-  // (positions as the frame started); if both fire the second setState wins.
-  for (int k = lane; k < T.nA; k += 32) {
-    if ((s_state[k] & 3) != 0) continue;
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-    const bool first = u01(w.x, w.y) < T.mine_rate[0], second = u01(w.z, w.w) < T.mine_rate[1];
-    if ((first || second) && sc.occ[T.ch_apple[k * 4 + 1]] == 0) s_state[k] |= (second ? 2 : 1) << 2;
-  }
-  // 150 Avatar movement: the frame's random visiting order (policy A.7).
-  int rank = 99;
-  {
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)lane, RS_AVATAR, k0, k1);
-    const uint32_t mykey = w.x;
-    int r = 0;
-    for (int q = 0; q < T.P; ++q) {
-      const uint32_t kq = __shfl_sync(MP_FULL, mykey, q);
-      if (kq < mykey || (kq == mykey && q < lane)) ++r;
-    }
-    if (is_av) rank = r;
-  }
-  // 100 StochasticIntervalEpisodeEnding
-  bool cont = true;
-  if (n >= T.end_min_frames && ((n + 1) % T.end_interval) == 0) {
-    uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, SCENE_DRAW_EPISODE_END, RS_SCENE, k0, k1);
-    if (u01(w.x, w.y) < T.end_prob) cont = false;
-  }
-  __syncwarp();
-
-  // ---- round 1a: the beams, shooter by shooter in avatar order (they entered the queue during the updates) ----
-  int beam_dirty = 0;
-  for (int src = 0; src < T.P; ++src) {
-    if (!__shfl_sync(MP_FULL, (int)fire, src)) continue;
-    const int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
-    for (int i = 1; i <= T.mine_length; ++i) {  // radius 0: one ray (every lane walks it)
-      int cx = sx + dir_dx(so) * i, cy = sy + dir_dy(so) * i;
-      if (!wrap_or_reject(T, cx, cy)) break;
-      const int cell = cy * T.W + cx;
-      bool blocked = (T.cell_flags[cell] >> T.zap_hit) & 1;  // BeamBlocker 'mine' (walls)
-      const int k = T.apple_of_cell[cell];
-      const int st = k >= 0 ? (s_state[k] & 3) : 0;
-      if (st != 0) {  // Ore:onHit (:118-150): a raw or partial ore takes the hit and stops the beam
-        blocked = true;
-        if (st == 1) {
-          // single-miner ore: mined and extracted by the same hit; partial, raw (reset), wait are queued -> wait
-          if (lane == src) {
-            reward += T.mine_reward[0] + T.extract_reward[0];
-            emit_event(S, b, EV_MINING, src + 1, 1);
-            emit_event(S, b, EV_EXTRACTION, src + 1, 1);
-          }
-          __syncwarp();  // every lane has read the ore's state byte before lane 0 rewrites it
-          if (lane == 0) s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (2 << 4));
-        } else {
-          const unsigned miners = s_miners[k] | (1u << src);  // Ore:addMiner (:110-114)
-          if (lane == src) { reward += T.mine_reward[1]; emit_event(S, b, EV_MINING, src + 1, 2); }
-          if (__popc(miners) == 2) {  // enough miners: both extract, then Ore:reset and the wait state
-            if (is_av && ((miners >> lane) & 1u)) {
-              reward += T.extract_reward[1];
-              emit_event(S, b, EV_EXTRACTION, lane + 1, 2);
-              emit_event(S, b, EV_EXTRACTION_PAIR, lane + 1, (__ffs(miners & ~(1u << lane))) | (2 << 8));
-            }
-            __syncwarp();
-            if (lane == 0) { s_miners[k] = 0; cd[k] = 0; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (2 << 4)); }
-          } else {
-            __syncwarp();
-            if (lane == 0) { s_miners[k] = (uint8_t)miners; cd[k] = (uint8_t)T.mine_window; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (1 << 4)); }
-          }
-        }
-        __syncwarp();
-      }
-      if (blocked) break;
-      if (lane == 0 && grid[(size_t)T.zap_layer * T.cells_pad + cell] == 0 && !((sc.beam_zap[cell >> 5] >> (cell & 31)) & 1u)) {
-        sc.beam_zap[cell >> 5] |= 1u << (cell & 31);
-        grid[(size_t)T.zap_layer * T.cells_pad + cell] = cell_value(T.zap_sprite, so);
-      }
-      beam_dirty = 1;
-      __syncwarp();
-    }
-  }
-  // ---- round 1b: resets and regrowth take effect (no contact callbacks on these pieces) ---------------------
-  for (int k = lane; k < T.nA; k += 32) {
-    const int r1 = (s_state[k] >> 2) & 3;
-    if (r1) s_state[k] = (uint8_t)((s_state[k] & ~0x0f) | r1);
-  }
-  __syncwarp();
-  // ---- round 1c: moves in the frame's order ------------------------------------------------------------------
-  for (int r = 0; r < T.P; ++r) {
-    const unsigned m = __ballot_sync(MP_FULL, is_av && rank == r);
-    const int src = __ffs(m) - 1;
-    const int s_turn = __shfl_sync(MP_FULL, act_turn, src), s_move = __shfl_sync(MP_FULL, act_move, src);
-    int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
-    if (s_turn != 0) so = (so + s_turn) & 3;
-    if (s_move != 0) {
-      const int d = (so + s_move - 1) & 3;
-      int nx = sx + dir_dx(d), ny = sy + dir_dy(d);
-      const bool inb = wrap_or_reject(T, nx, ny);
-      if (inb && sc.occ[ny * T.W + nx] == 0) {
-        __syncwarp();
-        if (lane == 0) { sc.occ[sy * T.W + sx] = 0; sc.occ[ny * T.W + nx] = (uint8_t)(src + 1); }
-        sx = nx; sy = ny;
-      }
-    }
-    if (lane == src) { x = sx; y = sy; orient = so; }
+  // Episode start: the avatars draw their spawn points (policy A.10); MineBeam:start (:254-261) leaves them ready to shoot.
+  __device__ static void reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
+    const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
     __syncwarp();
-  }
-
-  // ---- round 2 + write back ------------------------------------------------------------------------------
-  for (int k = lane; k < T.nA; k += 32) {
-    const int q2 = (s_state[k] >> 4) & 3;
-    const uint8_t now = q2 == 2 ? 0 : (q2 == 1 ? 3 : (s_state[k] & 3));
-    const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
-    if (now != was) {
-      S.apple[(size_t)b * T.nA_pad + k] = now;
-      grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = cell_value(T.ore_sprite[now], 0);
+    copy_init_grid(T, grid, lane);
+    for (int k = lane; k < T.nA; k += 32) {  // Ore:reset (:96-103): every ore waits, nobody is mining
+      S.apple[(size_t)b * T.nA_pad + k] = 0;
+      S.dirt[(size_t)b * T.nD_pad + k] = 0;
+      S.apple_count[(size_t)b * T.nA_pad + k] = 0;
     }
-    S.dirt[(size_t)b * T.nD_pad + k] = s_miners[k];
+    __syncwarp();
+    const auto all = [](int) { return true; };
+    spawn_group(T, S, b, lane, grid, sc.tmp, T.spawn_init_cell[0], T.n_spawn_init[0], all, all, episode, k0, k1, [&](int) {
+      for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 : 0.0;
+    });
+    // api:start ends with one grid:update (api_factory.lua:101): the FixedRateRegrow updaters already fire at frame 0
+    // (the component updates do not run then). Spawn points are not ore cells; the avatar check is kept for symmetry.
+    for (int k = lane; k < T.nA; k += 32) {
+      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
+      const bool first = u01(w.x, w.y) < T.mine_rate[0], second = u01(w.z, w.w) < T.mine_rate[1];
+      const int cell = T.ch_apple[k * 4 + 1];
+      if ((first || second) && grid[(size_t)T.avatar_layer * T.cells_pad + cell] == 0) {
+        const int now = second ? 2 : 1;
+        S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)now;
+        grid[(size_t)T.apple_layer * T.cells_pad + cell] = cell_value(T.ore_sprite[now], 0);
+      }
+    }
+    reset_env_row(T, S, b, lane, episode, 0);
   }
-  const bool changed = is_av && (x != x0 || y != y0 || orient != orient0);
-  if (changed) grid[(size_t)T.avatar_layer * T.cells_pad + y0 * T.W + x0] = 0;
-  __syncwarp();
-  if (changed) grid[(size_t)T.avatar_layer * T.cells_pad + y * T.W + x] = cell_value(T.avatar_sprite[lane], orient);
 
-  const bool done = !cont || n >= T.max_frames;
-  if (is_av) {
-    *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, 1);
-    S.av_timer[((size_t)b * T.P + lane) * 4] = cool;
-    S.reward[(size_t)b * T.P + lane] = reward;
-    S.packed[(size_t)b * (T.P + 2) + lane] = reward;
-    for (int k = 0; k < T.n_scalar; ++k)  // READY_TO_SHOOT = MineBeam:readyToShoot (:186-189)
-      S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 - (double)cool / (double)T.zap_cooldown : 0.0;
-  }
-  if (lane == 0) {
-    env[ENV_STEP] = n; env[ENV_DONE] = done ? 1 : 0; env[ENV_BEAM] = beam_dirty;
-    S.discount[b] = done ? 0.0 : 1.0;
-    S.step_type[b] = done ? 2 : 1;
-    S.packed[(size_t)b * (T.P + 2) + T.P] = done ? 0.0 : 1.0;
-    S.packed[(size_t)b * (T.P + 2) + T.P + 1] = done ? 2.0 : 1.0;
-  }
-}
+  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+    const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
+    const bool is_av = lane < T.P;
+    // bits 0-1 state code; bits 2-3 state set in round 1 (1 single-miner ore, 2 two-miner ore; by a reset or by
+    // regrowth, never both); bits 4-5 what the frame's last hit asked for (1 partial state, 2 wait state)
+    uint8_t* s_state = sc.apple;
+    uint8_t* s_miners = sc.dirt;
+    uint8_t* cd = S.apple_count + (size_t)b * T.nA_pad;  // count-down, touched by its own lane or by lane 0 between barriers
 
-__global__ void __launch_bounds__(128, 8) k_step_mining(Tables T, State S, const int32_t* __restrict__ actions,
-                                                    const uint8_t* __restrict__ mask, int mode) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // Programmatic dependent launch, both ways: let the renderer that follows in the stream stage its tables while this
-  // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  const int b = blockIdx.x * 4 + warp;
-  if (b >= S.B) return;
-  WarpScratch sc = carve_scratch(T, smem + warp * warp_scratch_bytes(T));
-  if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
-    event_begin(lane);
-    if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) mining_reset(T, S, b, lane, sc);
-    else mining_step(T, S, b, lane, actions, sc);
-    event_end(S, b, lane);
+    int4 a, t, act;
+    load_avatar(T, S, b, lane, actions, T.action_table, a, t, act);
+    int x = a.x, y = a.y, orient = a.z, cool = t.x;
+    const int act_move = act.x, act_turn = act.y, act_mine = act.z;
+    const int x0 = x, y0 = y, orient0 = orient;
+    double reward = 0.0;  // Avatar:preUpdate (avatar_library.lua:330-332)
+
+    init_occupancy(T, sc.occ, T.solid, lane);
+    for (int k = lane; k < T.nA; k += 32) { s_state[k] = S.apple[(size_t)b * T.nA_pad + k]; s_miners[k] = S.dirt[(size_t)b * T.nD_pad + k]; }
+    const int words = (T.cells + 31) / 32 + 1;
+    for (int i = lane; i < words; i += 32) sc.beam_zap[i] = 0;
+    __syncwarp();
+    if (is_av) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
+    if (env[ENV_BEAM]) clear_layer(T, grid, T.zap_layer, lane);
+    __syncwarp();
+
+    // ---- component updates -----------------------------------------------------------------------------
+    // MineBeam:update (:236-252): cool down, then fire if asked to and ready.
+    bool fire = false;
+    if (is_av) { if (cool > 0) --cool; if (act_mine == 1 && cool == 0) { cool = T.zap_cooldown; fire = true; } }
+    // Ore:update (:104-109): the window of a partly mined ore runs out -> reset: forget the miners, back to raw.
+    for (int k = lane; k < T.nA; k += 32) {
+      if (cd[k] > 0 && --cd[k] == 0) {
+        s_miners[k] = 0;
+        if ((s_state[k] & 3) != 0) s_state[k] |= 2 << 2;
+      }
+    }
+    // ---- updaters --------------------------------------------------------------------------------------
+    // 200 FixedRateRegrow (:41-57): one updater per live state, each with its own draw, only where no avatar stands
+    // (positions as the frame started); if both fire the second setState wins.
+    for (int k = lane; k < T.nA; k += 32) {
+      if ((s_state[k] & 3) != 0) continue;
+      uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
+      const bool first = u01(w.x, w.y) < T.mine_rate[0], second = u01(w.z, w.w) < T.mine_rate[1];
+      if ((first || second) && sc.occ[T.ch_apple[k * 4 + 1]] == 0) s_state[k] |= (second ? 2 : 1) << 2;
+    }
+    // 150 Avatar movement: the frame's random visiting order (policy A.7).
+    const int rank = visit_rank(T, lane, n, episode, k0, k1);
+    // 100 StochasticIntervalEpisodeEnding
+    const bool cont = episode_continues(T, n, episode, k0, k1);
+    __syncwarp();
+
+    // ---- round 1a: the beams, shooter by shooter in avatar order (they entered the queue during the updates) ----
+    int beam_dirty = 0;
+    for (int src = 0; src < T.P; ++src) {
+      if (!__shfl_sync(MP_FULL, (int)fire, src)) continue;
+      const int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
+      for (int i = 1; i <= T.mine_length; ++i) {  // radius 0: one ray (every lane walks it)
+        int cx = sx + dir_dx(so) * i, cy = sy + dir_dy(so) * i;
+        if (!wrap_or_reject(T, cx, cy)) break;
+        const int cell = cy * T.W + cx;
+        bool blocked = (T.cell_flags[cell] >> T.zap_hit) & 1;  // BeamBlocker 'mine' (walls)
+        const int k = T.apple_of_cell[cell];
+        const int st = k >= 0 ? (s_state[k] & 3) : 0;
+        if (st != 0) {  // Ore:onHit (:118-150): a raw or partial ore takes the hit and stops the beam
+          blocked = true;
+          if (st == 1) {
+            // single-miner ore: mined and extracted by the same hit; partial, raw (reset), wait are queued -> wait
+            if (lane == src) {
+              reward += T.mine_reward[0] + T.extract_reward[0];
+              emit_event(S, b, EV_MINING, src + 1, 1);
+              emit_event(S, b, EV_EXTRACTION, src + 1, 1);
+            }
+            __syncwarp();  // every lane has read the ore's state byte before lane 0 rewrites it
+            if (lane == 0) s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (2 << 4));
+          } else {
+            const unsigned miners = s_miners[k] | (1u << src);  // Ore:addMiner (:110-114)
+            if (lane == src) { reward += T.mine_reward[1]; emit_event(S, b, EV_MINING, src + 1, 2); }
+            if (__popc(miners) == 2) {  // enough miners: both extract, then Ore:reset and the wait state
+              if (is_av && ((miners >> lane) & 1u)) {
+                reward += T.extract_reward[1];
+                emit_event(S, b, EV_EXTRACTION, lane + 1, 2);
+                emit_event(S, b, EV_EXTRACTION_PAIR, lane + 1, (__ffs(miners & ~(1u << lane))) | (2 << 8));
+              }
+              __syncwarp();
+              if (lane == 0) { s_miners[k] = 0; cd[k] = 0; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (2 << 4)); }
+            } else {
+              __syncwarp();
+              if (lane == 0) { s_miners[k] = (uint8_t)miners; cd[k] = (uint8_t)T.mine_window; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (1 << 4)); }
+            }
+          }
+          __syncwarp();
+        }
+        if (blocked) break;
+        if (lane == 0 && grid[(size_t)T.zap_layer * T.cells_pad + cell] == 0 && !((sc.beam_zap[cell >> 5] >> (cell & 31)) & 1u)) {
+          sc.beam_zap[cell >> 5] |= 1u << (cell & 31);
+          grid[(size_t)T.zap_layer * T.cells_pad + cell] = cell_value(T.zap_sprite, so);
+        }
+        beam_dirty = 1;
+        __syncwarp();
+      }
+    }
+    // ---- round 1b: resets and regrowth take effect (no contact callbacks on these pieces) ---------------------
+    for (int k = lane; k < T.nA; k += 32) {
+      const int r1 = (s_state[k] >> 2) & 3;
+      if (r1) s_state[k] = (uint8_t)((s_state[k] & ~0x0f) | r1);
+    }
+    __syncwarp();
+    // ---- round 1c: moves in the frame's order ------------------------------------------------------------------
+    move_avatars(T, lane, rank, true, act_turn, act_move, x, y, orient, sc.occ, [](int, int) {});
+
+    // ---- round 2 + write back ------------------------------------------------------------------------------
+    for (int k = lane; k < T.nA; k += 32) {
+      const int q2 = (s_state[k] >> 4) & 3;
+      const uint8_t now = q2 == 2 ? 0 : (q2 == 1 ? 3 : (s_state[k] & 3));
+      const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
+      if (now != was) {
+        S.apple[(size_t)b * T.nA_pad + k] = now;
+        grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = cell_value(T.ore_sprite[now], 0);
+      }
+      S.dirt[(size_t)b * T.nD_pad + k] = s_miners[k];
+    }
+    draw_avatars(T, grid, lane, x0, y0, orient0, 1, x, y, orient, 1);
+
+    const bool done = !cont || n >= T.max_frames;
+    if (is_av) {
+      *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, 1);
+      S.av_timer[((size_t)b * T.P + lane) * 4] = cool;
+      for (int k = 0; k < T.n_scalar; ++k)  // READY_TO_SHOOT = MineBeam:readyToShoot (:186-189)
+        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 - (double)cool / (double)T.zap_cooldown : 0.0;
+    }
+    store_timestep(T, S, b, lane, n, reward, done ? 2 : 1, beam_dirty);
   }
-}
+};
