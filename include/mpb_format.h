@@ -10,6 +10,12 @@
  * File = MpbHeader, n_sections x MpbSection, then 16-byte aligned payloads.
  * Plain C99; shared by the CUDA engine (meltingpot_b200/csrc) and by the CPU
  * oracle (oracle/), which otherwise share no code.
+ *
+ * The meta fields, ids, table columns and every slot of the family parameter
+ * blocks "<fam>_ip" / "<fam>_dp" are named here. The compiler mirrors these
+ * enums by name (META, FAMILY, FP, CU_I, ... in compiler.py) and
+ * tests/test_blob_layout_cpu.py checks the mirrors against this file; the
+ * engine decodes a family's blocks in that family's step_<family>.cuh.
  */
 #ifndef MPB_FORMAT_H_
 #define MPB_FORMAT_H_
@@ -73,6 +79,95 @@ enum MpbMeta {
 };
 
 enum MpbFamily { MPB_FAMILY_CLEAN_UP = 1, MPB_FAMILY_COMMONS_HARVEST = 2, MPB_FAMILY_TERRITORY = 3, MPB_FAMILY_COINS = 4, MPB_FAMILY_COOP_MINING = 5 };
+
+/* Family parameter blocks. The blob of family <fam> carries its scalar parameters in two sections, "<fam>_ip"
+ * (int32[MPB_<FAM>_I_COUNT]) and "<fam>_dp" (f64[MPB_<FAM>_D_COUNT]), with <fam> one of cu (clean_up), ch
+ * (commons_harvest), tr (territory), co (coins) and cm (coop_mining). Every slot the compiler writes has a name below;
+ * the others are 0. A run of slots ending in _0, _1, ... is an array and is read as first slot + index. */
+
+/* Zapper and StochasticIntervalEpisodeEnding slots the int32 blocks of clean_up, commons_harvest and territory share. */
+enum MpbFamilyShared {
+  MPB_FP_ZAP_COOLDOWN = 12, MPB_FP_ZAP_LENGTH = 13, MPB_FP_ZAP_RADIUS = 14, MPB_FP_ZAP_RESPAWN = 15 /* framesTillRespawn */,
+  MPB_FP_ZAP_REMOVE = 16 /* removeHitPlayer */, MPB_FP_ZAP_LAYER = 21, MPB_FP_ZAP_SPRITE = 22,
+  MPB_FP_END_MIN_FRAMES = 26, MPB_FP_END_INTERVAL = 27
+};
+
+enum MpbCleanUpI {
+  MPB_CU_I_N_APPLES = 0, MPB_CU_I_N_DIRT = 1, MPB_CU_I_N_WATER = 2, MPB_CU_I_APPLE_LAYER = 3, MPB_CU_I_APPLE_SPRITE = 4,
+  MPB_CU_I_DIRT_LAYER = 5, MPB_CU_I_DIRT_SPRITE = 6, MPB_CU_I_DIRT_WAIT_LAYER = 7, MPB_CU_I_WATER_LAYER = 8,
+  MPB_CU_I_N_ANIM = 9, MPB_CU_I_ANIM_FRAMES = 10 /* gameFramesPerAnimationFrame */, MPB_CU_I_ANIM_RANDOM = 11,
+  MPB_CU_I_CLEAN_COOLDOWN = 18, MPB_CU_I_CLEAN_LENGTH = 19, MPB_CU_I_CLEAN_RADIUS = 20, MPB_CU_I_CLEAN_LAYER = 23,
+  MPB_CU_I_CLEAN_SPRITE = 24, MPB_CU_I_DIRT_DELAY = 25, MPB_CU_I_TASTE_ROLE = 28,
+  MPB_CU_I_COUNT = 48
+};
+enum MpbCleanUpD {
+  MPB_CU_D_GROW_RATE = 0, MPB_CU_D_GROW_DEPLETION = 1, MPB_CU_D_GROW_RESTORATION = 2, MPB_CU_D_EAT_REWARD = 3,
+  MPB_CU_D_ZAP_PENALTY = 4, MPB_CU_D_ZAP_REWARD = 5, MPB_CU_D_DIRT_PROB = 6, MPB_CU_D_END_PROB = 7,
+  MPB_CU_D_TASTE_AMOUNT = 8,
+  MPB_CU_D_COUNT = 16
+};
+
+enum MpbCommonsI {
+  MPB_CH_I_N_APPLES = 0, MPB_CH_I_APPLE_LAYER = 1, MPB_CH_I_APPLE_SPRITE = 2, MPB_CH_I_WAIT_LAYER = 3,
+  MPB_CH_I_WAIT_SPRITE = 4, MPB_CH_I_N_WAIT = 5 /* appleWait_<k> states */, MPB_CH_I_N_PROBS = 6,
+  MPB_CH_I_GRASS_LAYER = 7, MPB_CH_I_GRASS_SPRITE = 8, MPB_CH_I_DESS_SPRITE = 9,
+  MPB_CH_I_COUNT = 48
+};
+enum MpbCommonsD {
+  MPB_CH_D_PROB_0 = 0, MPB_CH_D_PROB_1 = 1, MPB_CH_D_PROB_2 = 2, MPB_CH_D_PROB_3 = 3 /* regrowthProbabilities */,
+  MPB_CH_D_EAT_REWARD = 4, MPB_CH_D_ZAP_PENALTY = 5, MPB_CH_D_ZAP_REWARD = 6, MPB_CH_D_END_PROB = 7,
+  MPB_CH_D_COUNT = 16
+};
+
+/* Marking level l (0-based) of territory: int32 slots MPB_TR_I_MARK_*_0 + 4 l, f64 slots MPB_TR_D_MARK_*_0 + 2 l. */
+enum MpbTerritoryI {
+  MPB_TR_I_N_RES = 0, MPB_TR_I_RES_LAYER = 1, MPB_TR_I_UNCLAIMED_SPRITE = 2, MPB_TR_I_TEX_LAYER = 3,
+  MPB_TR_I_TEX_SPRITE = 4, MPB_TR_I_IND_LAYER = 5, MPB_TR_I_DMG_LAYER = 6, MPB_TR_I_DMG_SPRITE = 7,
+  MPB_TR_I_MARK_LAYER = 8, MPB_TR_I_MARK_INITIAL_LEVEL = 9, MPB_TR_I_MARK_RECOVERY = 10, MPB_TR_I_MARK_N_LEVELS = 11,
+  MPB_TR_I_CLAIM_LENGTH = 18, MPB_TR_I_CLAIM_RADIUS = 19, MPB_TR_I_CLAIM_WAIT = 20, MPB_TR_I_BRUSH_LAYER = 23,
+  MPB_TR_I_CLAIM_LAYER = 24, MPB_TR_I_RES_HEALTH = 28, MPB_TR_I_RES_REWARD_DELAY = 29, MPB_TR_I_RES_REPAIR_DELAY = 30,
+  MPB_TR_I_TASTE_ROLE = 31,
+  MPB_TR_I_MARK_INC_0 = 32, MPB_TR_I_MARK_REMOVE_0 = 33, MPB_TR_I_MARK_FREEZE_0 = 34, MPB_TR_I_MARK_SPRITE_0 = 35,
+  MPB_TR_I_MARK_INC_1 = 36, MPB_TR_I_MARK_REMOVE_1 = 37, MPB_TR_I_MARK_FREEZE_1 = 38, MPB_TR_I_MARK_SPRITE_1 = 39,
+  MPB_TR_I_MARK_INC_2 = 40, MPB_TR_I_MARK_REMOVE_2 = 41, MPB_TR_I_MARK_FREEZE_2 = 42, MPB_TR_I_MARK_SPRITE_2 = 43,
+  MPB_TR_I_COUNT = 64
+};
+enum MpbTerritoryD {
+  MPB_TR_D_RES_REWARD = 0, MPB_TR_D_RES_RATE = 1, MPB_TR_D_RES_REPAIR_PROB = 2, MPB_TR_D_ZAP_PENALTY = 3,
+  MPB_TR_D_ZAP_REWARD = 4, MPB_TR_D_END_PROB = 5, MPB_TR_D_TASTE_AMOUNT = 6, MPB_TR_D_TASTE_MULT = 7,
+  MPB_TR_D_MARK_SRC_REWARD_0 = 8, MPB_TR_D_MARK_TGT_REWARD_0 = 9, MPB_TR_D_MARK_SRC_REWARD_1 = 10,
+  MPB_TR_D_MARK_TGT_REWARD_1 = 11, MPB_TR_D_MARK_SRC_REWARD_2 = 12, MPB_TR_D_MARK_TGT_REWARD_2 = 13,
+  MPB_TR_D_COUNT = 16
+};
+
+enum MpbCoinsI {
+  MPB_CO_I_N_COINS = 0, MPB_CO_I_COIN_LAYER = 1, MPB_CO_I_COIN_SPRITE_0 = 2, MPB_CO_I_COIN_SPRITE_1 = 3 /* liveStateA, B */,
+  MPB_CO_I_TERMINATE = 4, MPB_CO_I_TERMINATE_N = 5, MPB_CO_I_END_MIN_FRAMES = 6, MPB_CO_I_END_INTERVAL = 7,
+  MPB_CO_I_COIN_TYPE_0 = 8, MPB_CO_I_COIN_TYPE_1 = 9 /* PlayerCoinType of each player */,
+  MPB_CO_I_COUNT = 48
+};
+/* Coin rewards as collecting player p pays them (base reward x p's Role multiplier): slots MPB_CO_D_REWARD_0_* + 4 p. */
+enum MpbCoinsD {
+  MPB_CO_D_REGROW_RATE = 0, MPB_CO_D_END_PROB = 1,
+  MPB_CO_D_REWARD_0_SELF_MATCH = 4, MPB_CO_D_REWARD_0_SELF_MISMATCH = 5, MPB_CO_D_REWARD_0_OTHER_MATCH = 6,
+  MPB_CO_D_REWARD_0_OTHER_MISMATCH = 7, MPB_CO_D_REWARD_1_SELF_MATCH = 8, MPB_CO_D_REWARD_1_SELF_MISMATCH = 9,
+  MPB_CO_D_REWARD_1_OTHER_MATCH = 10, MPB_CO_D_REWARD_1_OTHER_MISMATCH = 11,
+  MPB_CO_D_COUNT = 16
+};
+
+/* Ore sprites 0..3: wait, single-miner raw, two-miner raw, two-miner partial. Ore types 0 / 1: one miner / two miners. */
+enum MpbMiningI {
+  MPB_CM_I_N_ORES = 0, MPB_CM_I_ORE_LAYER = 1, MPB_CM_I_ORE_SPRITE_0 = 2, MPB_CM_I_ORE_SPRITE_1 = 3,
+  MPB_CM_I_ORE_SPRITE_2 = 4, MPB_CM_I_ORE_SPRITE_3 = 5, MPB_CM_I_MINE_WINDOW = 6, MPB_CM_I_MINE_COOLDOWN = 7,
+  MPB_CM_I_MINE_LENGTH = 8, MPB_CM_I_MINE_LAYER = 9, MPB_CM_I_MINE_SPRITE = 10, MPB_CM_I_END_MIN_FRAMES = 11,
+  MPB_CM_I_END_INTERVAL = 12, MPB_CM_I_MINE_HIT = 13,
+  MPB_CM_I_COUNT = 48
+};
+enum MpbMiningD {
+  MPB_CM_D_RATE_0 = 0, MPB_CM_D_RATE_1 = 1 /* FixedRateRegrow liveRates */, MPB_CM_D_END_PROB = 2,
+  MPB_CM_D_MINE_REWARD_0 = 4, MPB_CM_D_MINE_REWARD_1 = 5, MPB_CM_D_EXTRACT_REWARD_0 = 6, MPB_CM_D_EXTRACT_REWARD_1 = 7,
+  MPB_CM_D_COUNT = 16
+};
 
 /* Primitive action fields (columns of section "action_table"). */
 enum MpbActionField { MPB_ACT_MOVE = 0, MPB_ACT_TURN = 1, MPB_ACT_FIRE_ZAP = 2 /* fireZap | mine */, MPB_ACT_FIRE_2 = 3 /* fireClean | fireClaim */ };

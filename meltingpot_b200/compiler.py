@@ -20,6 +20,7 @@ checkout.
 
 from __future__ import annotations
 
+import collections
 import copy
 import json
 import os
@@ -61,6 +62,41 @@ ACTION_FIELDS = {'move': 0, 'turn': 1, 'fireZap': 2, 'mine': 2, 'fireClean': 3,
                  'fireClaim': 3}
 SCALAR_OBS = {'READY_TO_SHOOT': 0, 'NUM_OTHERS_WHO_CLEANED_THIS_STEP': 1,
               'MISMATCHED_COIN_COLLECTED_BY_PARTNER': 2}
+# Family parameter blocks: MPB_FP_* (shared by the int32 blocks of clean_up, commons_harvest and territory) and
+# MPB_<CU|CH|TR|CO|CM>_<I|D>_*; COUNT is the block's size.
+FP = dict(ZAP_COOLDOWN=12, ZAP_LENGTH=13, ZAP_RADIUS=14, ZAP_RESPAWN=15, ZAP_REMOVE=16, ZAP_LAYER=21, ZAP_SPRITE=22,
+          END_MIN_FRAMES=26, END_INTERVAL=27)
+CU_I = dict(N_APPLES=0, N_DIRT=1, N_WATER=2, APPLE_LAYER=3, APPLE_SPRITE=4, DIRT_LAYER=5, DIRT_SPRITE=6,
+            DIRT_WAIT_LAYER=7, WATER_LAYER=8, N_ANIM=9, ANIM_FRAMES=10, ANIM_RANDOM=11, CLEAN_COOLDOWN=18,
+            CLEAN_LENGTH=19, CLEAN_RADIUS=20, CLEAN_LAYER=23, CLEAN_SPRITE=24, DIRT_DELAY=25, TASTE_ROLE=28, COUNT=48)
+CU_D = dict(GROW_RATE=0, GROW_DEPLETION=1, GROW_RESTORATION=2, EAT_REWARD=3, ZAP_PENALTY=4, ZAP_REWARD=5,
+            DIRT_PROB=6, END_PROB=7, TASTE_AMOUNT=8, COUNT=16)
+CH_I = dict(N_APPLES=0, APPLE_LAYER=1, APPLE_SPRITE=2, WAIT_LAYER=3, WAIT_SPRITE=4, N_WAIT=5, N_PROBS=6,
+            GRASS_LAYER=7, GRASS_SPRITE=8, DESS_SPRITE=9, COUNT=48)
+CH_D = dict(PROB_0=0, PROB_1=1, PROB_2=2, PROB_3=3, EAT_REWARD=4, ZAP_PENALTY=5, ZAP_REWARD=6, END_PROB=7, COUNT=16)
+TR_I = dict(N_RES=0, RES_LAYER=1, UNCLAIMED_SPRITE=2, TEX_LAYER=3, TEX_SPRITE=4, IND_LAYER=5, DMG_LAYER=6,
+            DMG_SPRITE=7, MARK_LAYER=8, MARK_INITIAL_LEVEL=9, MARK_RECOVERY=10, MARK_N_LEVELS=11, CLAIM_LENGTH=18,
+            CLAIM_RADIUS=19, CLAIM_WAIT=20, BRUSH_LAYER=23, CLAIM_LAYER=24, RES_HEALTH=28, RES_REWARD_DELAY=29,
+            RES_REPAIR_DELAY=30, TASTE_ROLE=31, COUNT=64,
+            **{f'MARK_{f}_{l}': 32 + 4 * l + k for l in range(3)
+               for k, f in enumerate(('INC', 'REMOVE', 'FREEZE', 'SPRITE'))})
+TR_D = dict(RES_REWARD=0, RES_RATE=1, RES_REPAIR_PROB=2, ZAP_PENALTY=3, ZAP_REWARD=4, END_PROB=5, TASTE_AMOUNT=6,
+            TASTE_MULT=7, COUNT=16,
+            **{f'MARK_{f}_REWARD_{l}': 8 + 2 * l + k for l in range(3) for k, f in enumerate(('SRC', 'TGT'))})
+CO_I = dict(N_COINS=0, COIN_LAYER=1, COIN_SPRITE_0=2, COIN_SPRITE_1=3, TERMINATE=4, TERMINATE_N=5,
+            END_MIN_FRAMES=6, END_INTERVAL=7, COIN_TYPE_0=8, COIN_TYPE_1=9, COUNT=48)
+_COIN_REWARDS = ('SELF_MATCH', 'SELF_MISMATCH', 'OTHER_MATCH', 'OTHER_MISMATCH')
+CO_D = dict(REGROW_RATE=0, END_PROB=1, COUNT=16,
+            **{f'REWARD_{p}_{r}': 4 + 4 * p + k for p in range(2) for k, r in enumerate(_COIN_REWARDS)})
+CM_I = dict(N_ORES=0, ORE_LAYER=1, ORE_SPRITE_0=2, ORE_SPRITE_1=3, ORE_SPRITE_2=4, ORE_SPRITE_3=5, MINE_WINDOW=6,
+            MINE_COOLDOWN=7, MINE_LENGTH=8, MINE_LAYER=9, MINE_SPRITE=10, END_MIN_FRAMES=11, END_INTERVAL=12,
+            MINE_HIT=13, COUNT=48)
+CM_D = dict(RATE_0=0, RATE_1=1, END_PROB=2, MINE_REWARD_0=4, MINE_REWARD_1=5, EXTRACT_REWARD_0=6,
+            EXTRACT_REWARD_1=7, COUNT=16)
+# family -> (section prefix, int32 block layout, f64 block layout)
+FAMILY_PARAMS = {'clean_up': ('cu', {**FP, **CU_I}, CU_D), 'commons_harvest': ('ch', {**FP, **CH_I}, CH_D),
+                 'territory': ('tr', {**FP, **TR_I}, TR_D), 'coins': ('co', CO_I, CO_D),
+                 'coop_mining': ('cm', CM_I, CM_D)}
 COMPASS = {'N': 0, 'E': 1, 'S': 2, 'W': 3}
 BASE_LAYERS = ['logic', 'alternateLogic', 'background', 'lowerPhysical',
                'upperPhysical', 'overlay', 'superOverlay']
@@ -568,8 +604,8 @@ class WorldModel:
         post = kw.get('postInitialSpawnGroup', '_DEFAULT')
         ip[4] = -1 if post == '_DEFAULT' else self.groups.index(post)
         view = kw['view']
-        ip[5:9] = [int(view['left']), int(view['right']), int(view['forward']),
-                   int(view['backward'])]
+        for i, side in enumerate(('left', 'right', 'forward', 'backward')):
+          ip[5 + i] = int(view[side])
         if view.get('centered', False):
           raise NotImplementedError('centered views')
         if self.view is None:
@@ -785,17 +821,100 @@ def _objects_with(model: WorldModel, comp: str):
   return out
 
 
+_Entity = collections.namedtuple('_Entity', 'oid cell state kind comp')
+
+
+def _entities(model: WorldModel, comp: str) -> List[_Entity]:
+  """The objects with component `comp`, in object order: id, cell, initial state, kind and the component's row."""
+  rows = []
+  for oid, ci in _objects_with(model, comp):
+    kid, x, y, _, st = model.objects[oid]
+    rows.append(_Entity(oid, y * model.W + x, st, kid, ci))
+  return rows
+
+
+def _one_kind(rows: List[_Entity], what: str) -> int:
+  """The kind all of `rows` share."""
+  kid = rows[0].kind
+  if any(r.kind != kid for r in rows):
+    raise NotImplementedError(f'heterogeneous {what} prefabs')
+  return kid
+
+
+def _kind_comps(model: WorldModel, kid: int, comp: str) -> List[int]:
+  """Rows of the components `comp` of kind `kid`."""
+  k = model.kinds[kid]
+  return [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP[comp]]
+
+
+def _comp_params(model: WorldModel, ci: int):
+  """(int params, f64 params) of component row `ci`."""
+  return model.comps_i[ci][1:], model.comps_d[ci]
+
+
+def _avatar_comps(model: WorldModel, comp: str):
+  """The parameters of component `comp` of every avatar, in avatar object order."""
+  return [_comp_params(model, _kind_comps(model, model.objects[oid][0], comp)[0]) for oid in model.avatar_objs]
+
+
+def _avatar_comp(model: WorldModel, comp: str):
+  """The parameters of component `comp`, which must be identical across avatars."""
+  rows = _avatar_comps(model, comp)
+  if any(r != rows[0] for r in rows[1:]):
+    raise NotImplementedError(f'per-avatar {comp} parameters')
+  return rows[0]
+
+
+def _scene_comp(model: WorldModel, comp: str):
+  """The parameters of the scene's component `comp` (the scene is object 0)."""
+  rows = _kind_comps(model, model.objects[0][0], comp)
+  if not rows:
+    raise KeyError(comp)
+  return _comp_params(model, rows[0])
+
+
+def _hits(model: WorldModel) -> Dict[str, tuple]:
+  """Hit name -> (layer, sprite) of its beam."""
+  return {h[0]: (model.layers.index(h[1]), model.sprites.index(h[2])) for h in model.hits}
+
+
+def _zapper_params(zap, hits, ending) -> Dict[str, int]:
+  """The MPB_FP_* slots from the Zapper and StochasticIntervalEpisodeEnding int params."""
+  return dict(ZAP_COOLDOWN=zap[0], ZAP_LENGTH=zap[1], ZAP_RADIUS=zap[2], ZAP_RESPAWN=zap[3], ZAP_REMOVE=zap[4],
+              ZAP_LAYER=hits['zapHit'][0], ZAP_SPRITE=hits['zapHit'][1], END_MIN_FRAMES=ending[0],
+              END_INTERVAL=ending[1])
+
+
+def _store_params(sections: Dict[str, np.ndarray], family: str, ints: Mapping[str, Any], floats: Mapping[str, Any]):
+  """Writes the family's "<prefix>_ip" and "<prefix>_dp" blocks: each value in the slot of its name, 0 elsewhere."""
+  prefix, int_layout, float_layout = FAMILY_PARAMS[family]
+  for suffix, layout, values, dtype in (('_ip', int_layout, ints, np.int32), ('_dp', float_layout, floats, np.float64)):
+    block = np.zeros(layout['COUNT'], dtype)
+    for name, value in values.items():
+      if name == 'COUNT' or name not in layout:
+        raise KeyError(f'{prefix}{suffix} has no slot {name!r}')
+      block[layout[name]] = value
+    sections[prefix + suffix] = block
+
+
+def family_params(sections: Mapping[str, np.ndarray]) -> Dict[str, Any]:
+  """Slot name -> value of both parameter blocks of a blob's family; `sections` is the unpacked blob."""
+  family = {v: k for k, v in FAMILY.items()}[int(sections['meta'][META['FAMILY']])]
+  prefix, int_layout, float_layout = FAMILY_PARAMS[family]
+  out = {k: int(sections[prefix + '_ip'][i]) for k, i in int_layout.items() if k != 'COUNT'}
+  out.update({k: float(sections[prefix + '_dp'][i]) for k, i in float_layout.items() if k != 'COUNT'})
+  return out
+
+
 def _avatar_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   """Tables shared by all families: avatars, spawn points, blockers."""
   P = model.num_players
   av = np.zeros((P, 8), np.int32)  # obj id, live sprite, layer, spawn group, post group
   for oid in model.avatar_objs:
     kid = model.objects[oid][0]
-    k = model.kinds[kid]
-    ci = [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP['Avatar']][0]
-    ip = model.comps_i[ci][1:]
+    ip = model.comps_i[_kind_comps(model, kid, 'Avatar')[0]][1:]
     idx0 = ip[0]
-    alive = model.states[k[0] + ip[1]]
+    alive = model.states[model.kinds[kid][0] + ip[1]]
     av[idx0] = [oid, alive[1], alive[0], ip[3], ip[4], 0, 0, 0]
   sections['av_table'] = av
   # Spawn cells per group, in object (piece) order.
@@ -818,113 +937,65 @@ def _avatar_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   flags = np.zeros(model.H * model.W, np.uint8)
   for oid, ci in _objects_with(model, 'BeamBlocker'):
     kid, x, y, _, _ = model.objects[oid]
-    k = model.kinds[kid]
-    for c in range(k[2], k[2] + k[3]):
-      if model.comps_i[c][0] == COMP['BeamBlocker'] and model.comps_i[c][1] >= 0:
+    for c in _kind_comps(model, kid, 'BeamBlocker'):
+      if model.comps_i[c][1] >= 0:
         flags[y * model.W + x] |= 1 << model.comps_i[c][1]
   sections['cell_flags'] = flags
 
 
 def _clean_up_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   """SoA tables for the clean_up step kernel (SURVEY.md Appendix B.1)."""
-  W = model.W
-  ip = np.zeros(48, np.int32)
-  dp = np.zeros(16, np.float64)
-  def entity(comp):
-    rows = []
-    for oid, ci in _objects_with(model, comp):
-      kid, x, y, orient, st = model.objects[oid]
-      rows.append((oid, y * W + x, st, kid, ci))
-    return rows
-  apples = entity('AppleGrow')
-  dirts = entity('DirtTracker')
-  waters = entity('Animation')
-  kid_a, ci_a = apples[0][3], apples[0][4]
-  for row in apples:
-    if row[3] != kid_a:
-      raise NotImplementedError('heterogeneous apple prefabs')
+  apples = _entities(model, 'AppleGrow')
+  dirts = _entities(model, 'DirtTracker')
+  waters = _entities(model, 'Animation')
+  kid_a = _one_kind(apples, 'apple')
   ka = model.kinds[kid_a]
-  apple_state = model.states[ka[0] + model.comps_i[ci_a][1]]
-  edible = [c for c in range(ka[2], ka[2] + ka[3]) if model.comps_i[c][0] == COMP['Edible']][0]
-  sections['cu_apple'] = np.array([[r[0], r[1], int(r[2] == model.comps_i[ci_a][1])] for r in apples], np.int32)
+  grow_i, grow_d = _comp_params(model, apples[0].comp)
+  apple_state = model.states[ka[0] + grow_i[0]]
+  edible = _kind_comps(model, kid_a, 'Edible')[0]
+  sections['cu_apple'] = np.array([[r.oid, r.cell, int(r.state == grow_i[0])] for r in apples], np.int32)
   # Dirt: both prefabs share states; column 2 = initially dirty.
   dirt_rows = []
   dirt_layer = dirt_sprite = wait_layer = None
   for r in dirts:
-    k = model.kinds[r[3]]
-    cip = model.comps_i[r[4]][1:]
-    active, inactive = cip[0], cip[1]
+    k = model.kinds[r.kind]
+    active, inactive = model.comps_i[r.comp][1:3]
     sa, sw = model.states[k[0] + active], model.states[k[0] + inactive]
     if dirt_layer is None:
       dirt_layer, dirt_sprite, wait_layer = sa[0], sa[1], sw[0]
     elif (dirt_layer, dirt_sprite, wait_layer) != (sa[0], sa[1], sw[0]):
       raise NotImplementedError('heterogeneous dirt prefabs')
-    dirt_rows.append([r[0], r[1], int(r[2] == active)])
+    dirt_rows.append([r.oid, r.cell, int(r.state == active)])
   sections['cu_dirt'] = np.array(dirt_rows, np.int32)
-  kw_ = model.kinds[waters[0][3]]
-  anim = model.comps_i[waters[0][4]][1:]
+  kw_ = model.kinds[waters[0].kind]
+  anim = model.comps_i[waters[0].comp][1:]
   n_anim = anim[0]
   water_sprites = [model.states[kw_[0] + anim[1 + i]][1] for i in range(n_anim)]
-  water_layer = model.states[kw_[0] + anim[1]][0]
-  sections['cu_water'] = np.array([[r[0], r[1]] for r in waters], np.int32)
+  sections['cu_water'] = np.array([[r.oid, r.cell] for r in waters], np.int32)
   sections['cu_water_sprites'] = np.array(water_sprites, np.int32)
-  # Avatar components (identical kwargs across avatars are required).
-  def avatar_comp(comp):
-    rows = []
-    for oid in model.avatar_objs:
-      k = model.kinds[model.objects[oid][0]]
-      ci = [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP[comp]][0]
-      rows.append((model.comps_i[ci][1:], model.comps_d[ci]))
-    for r in rows[1:]:
-      if comp != 'Avatar' and r != rows[0]:
-        raise NotImplementedError(f'per-avatar {comp} parameters')
-    return rows[0]
-  zi, zd = avatar_comp('Zapper')
-  ci_, _ = avatar_comp('Cleaner')
-  ti, td = avatar_comp('Taste')
-  scene_k = model.kinds[model.objects[0][0]]
-  def scene_comp(comp):
-    for c in range(scene_k[2], scene_k[2] + scene_k[3]):
-      if model.comps_i[c][0] == COMP[comp]:
-        return model.comps_i[c][1:], model.comps_d[c]
-    raise KeyError(comp)
-  si_, sd_ = scene_comp('DirtSpawner')
-  ei_, ed_ = scene_comp('StochasticIntervalEpisodeEnding')
-  hits = {h[0]: (model.layers.index(h[1]), model.sprites.index(h[2])) for h in model.hits}
-  ip[0:8] = [len(apples), len(dirts), len(waters), apple_state[0], apple_state[1],
-             dirt_layer, dirt_sprite, wait_layer]
-  ip[8:12] = [water_layer, n_anim, anim[9], anim[11]]
-  ip[12:18] = [zi[0], zi[1], zi[2], zi[3], zi[4], 0]          # zapper
-  ip[18:21] = [ci_[0], ci_[1], ci_[2]]                       # cleaner
-  ip[21:25] = [hits['zapHit'][0], hits['zapHit'][1], hits['cleanHit'][0], hits['cleanHit'][1]]
-  ip[25] = si_[0]
-  ip[26:28] = [ei_[0], ei_[1]]
-  ip[28] = ti[0]
-  ip[29] = 0  # scene object id
-  ag = model.comps_d[ci_a]
-  dp[0:3] = ag[0:3]
-  dp[3] = model.comps_d[edible][0]
-  dp[4], dp[5] = zd[0], zd[1]
-  dp[6] = sd_[0]
-  dp[7] = ed_[0]
-  dp[8] = td[0]
-  sections['cu_ip'] = ip
-  sections['cu_dp'] = dp
+  zi, zd = _avatar_comp(model, 'Zapper')
+  cl, _ = _avatar_comp(model, 'Cleaner')
+  ti, td = _avatar_comp(model, 'Taste')
+  di, dd = _scene_comp(model, 'DirtSpawner')
+  ei, ed = _scene_comp(model, 'StochasticIntervalEpisodeEnding')
+  hits = _hits(model)
+  _store_params(sections, 'clean_up', dict(
+      N_APPLES=len(apples), N_DIRT=len(dirts), N_WATER=len(waters), APPLE_LAYER=apple_state[0],
+      APPLE_SPRITE=apple_state[1], DIRT_LAYER=dirt_layer, DIRT_SPRITE=dirt_sprite, DIRT_WAIT_LAYER=wait_layer,
+      WATER_LAYER=model.states[kw_[0] + anim[1]][0], N_ANIM=n_anim, ANIM_FRAMES=anim[9], ANIM_RANDOM=anim[11],
+      **_zapper_params(zi, hits, ei), CLEAN_COOLDOWN=cl[0], CLEAN_LENGTH=cl[1], CLEAN_RADIUS=cl[2],
+      CLEAN_LAYER=hits['cleanHit'][0], CLEAN_SPRITE=hits['cleanHit'][1], DIRT_DELAY=di[0], TASTE_ROLE=ti[0]), dict(
+      GROW_RATE=grow_d[0], GROW_DEPLETION=grow_d[1], GROW_RESTORATION=grow_d[2], EAT_REWARD=model.comps_d[edible][0],
+      ZAP_PENALTY=zd[0], ZAP_REWARD=zd[1], DIRT_PROB=dd[0], END_PROB=ed[0], TASTE_AMOUNT=td[0]))
 
 
 def _commons_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   """SoA tables for the commons_harvest step kernel (SURVEY.md Appendix B.2)."""
   W = model.W
-  apples = []
-  for oid, ci in _objects_with(model, 'DensityRegrow'):
-    kid, x, y, orient, st = model.objects[oid]
-    apples.append((oid, y * W + x, st, kid, ci))
-  kid_a, ci_a = apples[0][3], apples[0][4]
-  if any(r[3] != kid_a for r in apples):
-    raise NotImplementedError('heterogeneous apple prefabs')
+  apples = _entities(model, 'DensityRegrow')
+  kid_a = _one_kind(apples, 'apple')
   ka = model.kinds[kid_a]
-  dr = model.comps_i[ci_a][1:]
-  drd = model.comps_d[ci_a]
+  dr, drd = _comp_params(model, apples[0].comp)
   live_state, wait0, n_wait, plain_wait, n_probs = dr[0], dr[1], dr[2], dr[3], dr[4]
   if not dr[5]:
     raise NotImplementedError('canRegrowIfOccupied=False')
@@ -933,7 +1004,7 @@ def _commons_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   plain = model.states[ka[0] + plain_wait]
   if plain[0] != waitk[0] or plain[1] != waitk[1]:
     raise NotImplementedError('wait states with different layers/sprites')
-  edible = [c for c in range(ka[2], ka[2] + ka[3]) if model.comps_i[c][0] == COMP['Edible']][0]
+  edible = _kind_comps(model, kid_a, 'Edible')[0]
   if model.comps_i[edible][1] != live_state or model.comps_i[edible][2] != plain_wait:
     raise NotImplementedError('Edible states differ from DensityRegrow states')
   # grass under each apple (background layer)
@@ -947,11 +1018,11 @@ def _commons_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
     if kid == grass_kind:
       grass_at[y * W + x] = oid
   radius = drd[0]
-  cell_to_apple = {r[1]: i for i, r in enumerate(apples)}
+  cell_to_apple = {r.cell: i for i, r in enumerate(apples)}
   nbr = np.full((len(apples), 16), -1, np.int32)
   r_int = int(radius)
   for i, row in enumerate(apples):
-    cx, cy = row[1] % W, row[1] // W
+    cx, cy = row.cell % W, row.cell // W
     k = 0
     for dy in range(-r_int, r_int + 1):   # same scan order as the oracle (irrelevant to results)
       for dx in range(-r_int, r_int + 1):
@@ -970,107 +1041,59 @@ def _commons_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
                                       f'{nbr.shape[1]} neighbours per apple)')
           nbr[i, k] = j
           k += 1
-  def avatar_comp(comp):
-    rows = []
-    for oid in model.avatar_objs:
-      k = model.kinds[model.objects[oid][0]]
-      ci = [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP[comp]][0]
-      rows.append((model.comps_i[ci][1:], model.comps_d[ci]))
-    for r in rows[1:]:
-      if r != rows[0]:
-        raise NotImplementedError(f'per-avatar {comp} parameters')
-    return rows[0]
-  zi, zd = avatar_comp('Zapper')
-  scene_k = model.kinds[model.objects[0][0]]
-  end = [c for c in range(scene_k[2], scene_k[2] + scene_k[3])
-         if model.comps_i[c][0] == COMP['StochasticIntervalEpisodeEnding']][0]
-  ei, ed = model.comps_i[end][1:], model.comps_d[end]
-  hits = {h[0]: (model.layers.index(h[1]), model.sprites.index(h[2])) for h in model.hits}
-  ip = np.zeros(48, np.int32)
-  dp = np.zeros(16, np.float64)
-  ip[0:8] = [len(apples), live[0], live[1], waitk[0], waitk[1], n_wait, n_probs, grass_state[0]]
-  ip[8:10] = [grass_state[1], dess_state[1]]
-  ip[12:18] = [zi[0], zi[1], zi[2], zi[3], zi[4], 0]
-  ip[21:23] = [hits['zapHit'][0], hits['zapHit'][1]]
-  ip[26:28] = [ei[0], ei[1]]
-  dp[0:n_probs] = drd[1:1 + n_probs]
-  dp[4] = model.comps_d[edible][0]
-  dp[5], dp[6] = zd[0], zd[1]
-  dp[7] = ed[0]
-  sections['ch_ip'] = ip
-  sections['ch_dp'] = dp
-  sections['ch_apple'] = np.array([[r[0], r[1], int(r[2] == live_state), grass_at.get(r[1], -1)] for r in apples], np.int32)
+  zi, zd = _avatar_comp(model, 'Zapper')
+  ei, ed = _scene_comp(model, 'StochasticIntervalEpisodeEnding')
+  probs = drd[1:1 + min(n_probs, 4)]  # mp_create refuses more than four
+  _store_params(sections, 'commons_harvest', dict(
+      N_APPLES=len(apples), APPLE_LAYER=live[0], APPLE_SPRITE=live[1], WAIT_LAYER=waitk[0], WAIT_SPRITE=waitk[1],
+      N_WAIT=n_wait, N_PROBS=n_probs, GRASS_LAYER=grass_state[0], GRASS_SPRITE=grass_state[1],
+      DESS_SPRITE=dess_state[1], **_zapper_params(zi, _hits(model), ei)), dict(
+      {f'PROB_{i}': p for i, p in enumerate(probs)}, EAT_REWARD=model.comps_d[edible][0], ZAP_PENALTY=zd[0],
+      ZAP_REWARD=zd[1], END_PROB=ed[0]))
+  sections['ch_apple'] = np.array([[r.oid, r.cell, int(r.state == live_state), grass_at.get(r.cell, -1)] for r in apples],
+                                  np.int32)
   sections['ch_nbr'] = nbr
 
 
 def _coins_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   """SoA tables for the coins step kernel (lua/levels/coins/components.lua)."""
-  W, P = model.W, model.num_players
-  if P != 2:
+  if model.num_players != 2:
     raise NotImplementedError('coins supports exactly two players (coins/components.lua:93-96)')
-  coins = []
-  for oid, ci in _objects_with(model, 'Coin'):
-    kid, x, y, orient, st = model.objects[oid]
-    coins.append((oid, y * W + x, kid, ci, st))
-  kid_c, ci_c = coins[0][2], coins[0][3]
-  if any(c[2] != kid_c for c in coins):
-    raise NotImplementedError('heterogeneous coin prefabs')
+  coins = _entities(model, 'Coin')
+  kid_c = _one_kind(coins, 'coin')
   kc = model.kinds[kid_c]
-  coin_i, coin_d = model.comps_i[ci_c][1:], model.comps_d[ci_c]
-  regrow = [c for c in range(kc[2], kc[2] + kc[3]) if model.comps_i[c][0] == COMP['ChoiceCoinRegrow']][0]
-  ri, rd = model.comps_i[regrow][1:], model.comps_d[regrow]
+  coin_i, coin_d = _comp_params(model, coins[0].comp)
+  ri, rd = _comp_params(model, _kind_comps(model, kid_c, 'ChoiceCoinRegrow')[0])
   if ri[2] != coin_i[0]:
     raise NotImplementedError('Coin and ChoiceCoinRegrow wait states differ')
-  if any(c[4] != coin_i[0] for c in coins):
+  if any(c.state != coin_i[0] for c in coins):
     raise NotImplementedError('coins that do not start in the wait state')
   live_a, live_b = model.states[kc[0] + ri[0]], model.states[kc[0] + ri[1]]
   if live_a[0] != live_b[0]:
     raise NotImplementedError('coin types on different layers')
-  def avatar_row(comp):
-    rows = []
-    for oid in model.avatar_objs:
-      k = model.kinds[model.objects[oid][0]]
-      ci = [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP[comp]][0]
-      rows.append((model.comps_i[ci][1:], model.comps_d[ci]))
-    return rows
-  types = [r[0][0] for r in avatar_row('PlayerCoinType')]
-  roles = [r[1] for r in avatar_row('CoinsRole')]
-  scene_k = model.kinds[model.objects[0][0]]
-  end = [c for c in range(scene_k[2], scene_k[2] + scene_k[3])
-         if model.comps_i[c][0] == COMP['StochasticIntervalEpisodeEnding']][0]
-  ei, ed = model.comps_i[end][1:], model.comps_d[end]
-  ip = np.zeros(48, np.int32)
-  dp = np.zeros(16, np.float64)
-  ip[0:8] = [len(coins), live_a[0], live_a[1], live_b[1], coin_i[1], coin_i[2], ei[0], ei[1]]
-  ip[8:10] = types
-  dp[0] = rd[0]
-  dp[1] = ed[0]
-  # the four rewards as each collecting player pays them: base reward x that player's Role multiplier
-  for p in range(2):
-    for k in range(4):
-      dp[4 + p * 4 + k] = coin_d[k] * roles[p][k]
-  sections['co_ip'] = ip
-  sections['co_dp'] = dp
-  sections['co_coin'] = np.array([[c[0], c[1]] for c in coins], np.int32)
+  types = [i[0] for i, _ in _avatar_comps(model, 'PlayerCoinType')]
+  roles = [d for _, d in _avatar_comps(model, 'CoinsRole')]
+  ei, ed = _scene_comp(model, 'StochasticIntervalEpisodeEnding')
+  _store_params(sections, 'coins', dict(
+      N_COINS=len(coins), COIN_LAYER=live_a[0], COIN_SPRITE_0=live_a[1], COIN_SPRITE_1=live_b[1], TERMINATE=coin_i[1],
+      TERMINATE_N=coin_i[2], END_MIN_FRAMES=ei[0], END_INTERVAL=ei[1], COIN_TYPE_0=types[0], COIN_TYPE_1=types[1]), dict(
+      REGROW_RATE=rd[0], END_PROB=ed[0],
+      # the four rewards as each collecting player pays them: base reward x that player's Role multiplier
+      **{f'REWARD_{p}_{name}': coin_d[k] * roles[p][k] for p in range(2) for k, name in enumerate(_COIN_REWARDS)}))
+  sections['co_coin'] = np.array([[c.oid, c.cell] for c in coins], np.int32)
 
 
 def _mining_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   """SoA tables for the coop_mining step kernel (lua/levels/coop_mining/components.lua)."""
-  W = model.W
-  ores = []
-  for oid, ci in _objects_with(model, 'FixedRateRegrow'):
-    kid, x, y, orient, st = model.objects[oid]
-    ores.append((oid, y * W + x, kid, ci, st))
-  kid_o, ci_r = ores[0][2], ores[0][3]
-  if any(o[2] != kid_o for o in ores):
-    raise NotImplementedError('heterogeneous ore prefabs')
+  ores = _entities(model, 'FixedRateRegrow')
+  kid_o = _one_kind(ores, 'ore')
   ko = model.kinds[kid_o]
-  ri, rd = model.comps_i[ci_r][1:], model.comps_d[ci_r]
-  ore_comps = [c for c in range(ko[2], ko[2] + ko[3]) if model.comps_i[c][0] == COMP['Ore']]
+  ri, rd = _comp_params(model, ores[0].comp)
+  ore_comps = _kind_comps(model, kid_o, 'Ore')
   if ri[0] != 2 or len(ore_comps) != 2:
     raise NotImplementedError('coop_mining needs two ore types (two Ore components, two live states)')
   wait = ri[5]
-  if any(o[4] != wait for o in ores):
+  if any(o.state != wait for o in ores):
     raise NotImplementedError('ores that do not start in the wait state')
   # which Ore component owns which live state; "single" ore: one miner extracts, "joint" ore: two miners within the window
   by_raw = {model.comps_i[c][2]: model.comps_i[c][1:] for c in ore_comps}
@@ -1081,47 +1104,30 @@ def _mining_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   layers = {st(i)[0] for i in (wait, single[1], joint[1], joint[2])}
   if len(layers) != 1:
     raise NotImplementedError('ore states on different layers')
-  beams = []
-  for oid in model.avatar_objs:
-    k = model.kinds[model.objects[oid][0]]
-    ci = [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP['MineBeam']][0]
-    beams.append((model.comps_i[ci][1:], model.comps_d[ci]))
-  if any(b != beams[0] for b in beams[1:]):
-    raise NotImplementedError('per-avatar MineBeam parameters')
-  bi, bd = beams[0]
+  bi, bd = _avatar_comp(model, 'MineBeam')
   if bi[2] != 0:
     raise NotImplementedError('mine beams with a radius')
-  scene_k = model.kinds[model.objects[0][0]]
-  end = [c for c in range(scene_k[2], scene_k[2] + scene_k[3])
-         if model.comps_i[c][0] == COMP['StochasticIntervalEpisodeEnding']][0]
-  ei, ed = model.comps_i[end][1:], model.comps_d[end]
-  hits = {h[0]: (model.layers.index(h[1]), model.sprites.index(h[2])) for h in model.hits}
-  ip = np.zeros(48, np.int32)
-  dp = np.zeros(16, np.float64)
-  ip[0:8] = [len(ores), st(wait)[0], st(wait)[1], st(single[1])[1], st(joint[1])[1], st(joint[2])[1], joint[4], bi[0]]
-  ip[8:14] = [bi[1], hits['mine'][0], hits['mine'][1], ei[0], ei[1], bi[3]]
-  dp[0:3] = [rd[0], rd[1], ed[0]]
-  dp[4:8] = bd[0:4]
-  sections['cm_ip'] = ip
-  sections['cm_dp'] = dp
-  sections['cm_ore'] = np.array([[o[0], o[1]] for o in ores], np.int32)
+  ei, ed = _scene_comp(model, 'StochasticIntervalEpisodeEnding')
+  hits = _hits(model)
+  _store_params(sections, 'coop_mining', dict(
+      N_ORES=len(ores), ORE_LAYER=st(wait)[0], ORE_SPRITE_0=st(wait)[1], ORE_SPRITE_1=st(single[1])[1],
+      ORE_SPRITE_2=st(joint[1])[1], ORE_SPRITE_3=st(joint[2])[1], MINE_WINDOW=joint[4], MINE_COOLDOWN=bi[0],
+      MINE_LENGTH=bi[1], MINE_LAYER=hits['mine'][0], MINE_SPRITE=hits['mine'][1], END_MIN_FRAMES=ei[0],
+      END_INTERVAL=ei[1], MINE_HIT=bi[3]), dict(
+      RATE_0=rd[0], RATE_1=rd[1], END_PROB=ed[0], MINE_REWARD_0=bd[0], MINE_REWARD_1=bd[1], EXTRACT_REWARD_0=bd[2],
+      EXTRACT_REWARD_1=bd[3]))
+  sections['cm_ore'] = np.array([[o.oid, o.cell] for o in ores], np.int32)
 
 
 def _territory_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   """SoA tables for the territory step kernel (SURVEY.md Appendix B.3)."""
   W, P = model.W, model.num_players
   L = model.layers.index
-  SP = model.sprites.index
-  res = []
-  for oid, ci in _objects_with(model, 'Resource'):
-    kid, x, y, orient, st = model.objects[oid]
-    res.append((oid, y * W + x, kid, ci, st))
-  kid_r, ci_r = res[0][2], res[0][3]
-  if any(r[2] != kid_r for r in res):
-    raise NotImplementedError('heterogeneous resource prefabs')
+  res = _entities(model, 'Resource')
+  kid_r = _one_kind(res, 'resource')
   kr = model.kinds[kid_r]
   rnames = model.state_names[kid_r]
-  rc, rd = model.comps_i[ci_r][1:], model.comps_d[ci_r]
+  rc, rd = _comp_params(model, res[0].comp)
   if rnames.index('unclaimed') != 0 or rnames.index('destroyed') != 1 or rc[4] != 2:
     raise NotImplementedError('resource states must be unclaimed, destroyed, claimed_by_1..P')
   def st_of(kind_name, state):
@@ -1130,16 +1136,9 @@ def _territory_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   unclaimed = st_of('resource', 'unclaimed')
   tex = st_of('resource_texture', 'unclaimed')
   dmg = st_of('damage_indicator', 'damaged')
-  def avatar_comp(comp):
-    rows = []
-    for oid in model.avatar_objs:
-      k = model.kinds[model.objects[oid][0]]
-      ci = [c for c in range(k[2], k[2] + k[3]) if model.comps_i[c][0] == COMP[comp]][0]
-      rows.append((model.comps_i[ci][1:], model.comps_d[ci]))
-    return rows
-  zap = avatar_comp('Zapper')
-  claim = avatar_comp('ResourceClaimer')
-  taste = avatar_comp('TerritoryTaste')
+  zap = _avatar_comps(model, 'Zapper')
+  claim = _avatar_comps(model, 'ResourceClaimer')
+  taste = _avatar_comps(model, 'TerritoryTaste')
   for rows, skip in ((zap, ()), (claim, (0, 4)), (taste, ())):
     for r in rows[1:]:
       a = [v for i, v in enumerate(r[0]) if i not in skip]; b = [v for i, v in enumerate(rows[0][0]) if i not in skip]
@@ -1152,49 +1151,37 @@ def _territory_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
   marks = _objects_with(model, 'GraduatedSanctionsMarking')
   if len(marks) != P:
     raise NotImplementedError('territory needs one GraduatedSanctionsMarking object per avatar')
-  mk = model.comps_i[marks[0][1]][1:]
-  mkd = model.comps_d[marks[0][1]]
+  mk, mkd = _comp_params(model, marks[0][1])
   for i, (oid, ci) in enumerate(marks):
     if model.comps_i[ci][1] != i or model.comps_i[ci][2:] != list(model.comps_i[marks[0][1]][2:]):
       raise NotImplementedError('per-avatar marking parameters')
   mkind = model.objects[marks[0][0]][0]
   mnames = model.state_names[mkind]
   level_states = [model.states[model.kinds[mkind][0] + mnames.index(f'level_{l + 1}')] for l in range(mk[5])]
-  scene_k = model.kinds[model.objects[0][0]]
-  end = [c for c in range(scene_k[2], scene_k[2] + scene_k[3])
-         if model.comps_i[c][0] == COMP['StochasticIntervalEpisodeEnding']][0]
-  ei, ed = model.comps_i[end][1:], model.comps_d[end]
-  hits = {h[0]: (L(h[1]), SP(h[2])) for h in model.hits}
-  ip = np.zeros(64, np.int32)
-  dp = np.zeros(16, np.float64)
-  ip[0:8] = [len(res), unclaimed[0], unclaimed[1], tex[0], tex[1], L('overlay'), dmg[0], dmg[1]]
-  ip[8:12] = [level_states[0][0], mk[2], mk[3], mk[5]]
-  ip[12:18] = [zi[0], zi[1], zi[2], zi[3], zi[4], 0]
-  ip[18:21] = [cli[1], cli[2], cli[3]]
-  ip[21:23] = [hits['zapHit'][0], hits['zapHit'][1]]
-  ip[23] = L('directionIndicatorLayer')
-  ip[24] = L('superDirectionIndicatorLayer')
-  ip[26:28] = [ei[0], ei[1]]
-  ip[28:32] = [rc[0], rc[2], rc[3], ti[0]]
+  ei, ed = _scene_comp(model, 'StochasticIntervalEpisodeEnding')
+  hits = _hits(model)
+  ints = dict(N_RES=len(res), RES_LAYER=unclaimed[0], UNCLAIMED_SPRITE=unclaimed[1], TEX_LAYER=tex[0],
+              TEX_SPRITE=tex[1], IND_LAYER=L('overlay'), DMG_LAYER=dmg[0], DMG_SPRITE=dmg[1],
+              MARK_LAYER=level_states[0][0], MARK_INITIAL_LEVEL=mk[2], MARK_RECOVERY=mk[3], MARK_N_LEVELS=mk[5],
+              **_zapper_params(zi, hits, ei), CLAIM_LENGTH=cli[1], CLAIM_RADIUS=cli[2], CLAIM_WAIT=cli[3],
+              BRUSH_LAYER=L('directionIndicatorLayer'), CLAIM_LAYER=L('superDirectionIndicatorLayer'),
+              RES_HEALTH=rc[0], RES_REWARD_DELAY=rc[2], RES_REPAIR_DELAY=rc[3], TASTE_ROLE=ti[0])
+  floats = dict(RES_REWARD=rd[0], RES_RATE=rd[1], RES_REPAIR_PROB=rd[2], ZAP_PENALTY=zd[0], ZAP_REWARD=zd[1],
+                END_PROB=ed[0], TASTE_AMOUNT=td[0], TASTE_MULT=td[1])
   for l in range(mk[5]):
-    ip[32 + 4 * l: 36 + 4 * l] = [mk[7 + 3 * l], mk[8 + 3 * l], mk[9 + 3 * l], level_states[l][1]]
-  dp[0:3] = [rd[0], rd[1], rd[2]]
-  dp[3], dp[4] = zd[0], zd[1]
-  dp[5] = ed[0]
-  dp[6], dp[7] = td[0], td[1]
-  for l in range(mk[5]):
-    dp[8 + 2 * l], dp[9 + 2 * l] = mkd[2 * l], mkd[2 * l + 1]
-  sections['tr_ip'] = ip
-  sections['tr_dp'] = dp
-  sections['tr_res'] = np.array([[r[0], r[1], r[4]] for r in res], np.int32)
+    ints.update({f'MARK_INC_{l}': mk[7 + 3 * l], f'MARK_REMOVE_{l}': mk[8 + 3 * l], f'MARK_FREEZE_{l}': mk[9 + 3 * l],
+                 f'MARK_SPRITE_{l}': level_states[l][1]})
+    floats.update({f'MARK_SRC_REWARD_{l}': mkd[2 * l], f'MARK_TGT_REWARD_{l}': mkd[2 * l + 1]})
+  _store_params(sections, 'territory', ints, floats)
+  sections['tr_res'] = np.array([[r.oid, r.cell, r.state] for r in res], np.int32)
   if model.choice_options:  # resources that exist only on some tickets of their 'choice' group (territory__inside_out's A / B cells)
-    cond = np.array([model.obj_choice[r[0]] for r in res], np.int32).reshape(-1, 2)
+    cond = np.array([model.obj_choice[r.oid] for r in res], np.int32).reshape(-1, 2)
     by_cell = {}
     for oid, (kid, x, y, orient, st) in enumerate(model.objects):
       if model.obj_choice[oid][0] >= 0 and model.kind_names[kid] in ('resource', 'resource_texture', 'reward_indicator', 'damage_indicator'):
         by_cell.setdefault(y * model.W + x, set()).add(tuple(model.obj_choice[oid]))
     for r in res:  # the four pieces of a resource cell come and go together
-      if len(by_cell.get(r[1], {tuple(model.obj_choice[r[0]])})) != 1 or (model.obj_choice[r[0]][0] >= 0) != (r[1] in by_cell):
+      if len(by_cell.get(r.cell, {tuple(model.obj_choice[r.oid])})) != 1 or (model.obj_choice[r.oid][0] >= 0) != (r.cell in by_cell):
         raise NotImplementedError('a resource and its texture / indicators must share one choice condition')
     sections['tr_res_cond'] = cond
   per_player = np.zeros((P, 4), np.int32)

@@ -4,7 +4,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -13,6 +12,7 @@
 #include "../../include/mp_engine.h"
 #include "../../include/mpb_format.h"
 #include "common.cuh"
+#include "family_load.h"
 #include "render.cuh"
 #include "step_clean_up.cuh"
 #include "step_commons.cuh"
@@ -22,78 +22,10 @@
 
 namespace {
 
-thread_local std::string g_error;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof buf, fmt, ap);
-  va_end(ap);
-  g_error = buf;
-  return code;
-}
-
-#define CUDA_TRY(expr)                                                                          \
-  do {                                                                                          \
-    cudaError_t e_ = (expr);                                                                    \
-    if (e_ != cudaSuccess) return fail(MP_E_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e_)); \
-  } while (0)
-
-template <typename T>
-struct Section {
-  const T* data = nullptr;
-  std::vector<uint32_t> shape;
-  size_t count = 0;
-};
-
-template <typename T>
-bool get_section(const void* blob, size_t n, const char* name, int dtype, Section<T>* out) {
-  const MpbSection* s = mpb_find(blob, n, name);
-  if (!s || (int)s->dtype != dtype) return false;
-  out->data = static_cast<const T*>(mpb_data(blob, s));
-  out->shape.assign(s->shape, s->shape + s->ndim);
-  out->count = s->nbytes / sizeof(T);
-  return true;
-}
-
-int round_up(int v, int m) { return (v + m - 1) / m * m; }
-
 constexpr int kRenderSmemLimit = 227 * 1024 - 2560;  // dynamic shared memory: the 227 KB opt-in maximum less k_render's static arrays
 constexpr int kMaxAtlasSprites = 96;
 #define MP_MAX_DEVICES 64
 #define MP_EXCHANGE_HEADER 256  // bytes reserved for the per-rank flags in front of the gathered rows  // sprites incl. pre-merged ones kept in shared memory by k_render
-
-// Beam footprint in visiting order (policy A.8): centre ray, then for each side the lateral cells
-// outwards, each followed by its forward ray of length `length - k`.
-bool make_beam_geom(int length, int radius, BeamGeom* g) {
-  std::vector<int> lat, fwd, parent;
-  int prev = -1;
-  for (int i = 1; i <= length; ++i) { lat.push_back(0); fwd.push_back(i); parent.push_back(prev); prev = (int)lat.size() - 1; }
-  for (int side = 0; side < 2; ++side) {
-    int sign = side == 0 ? -1 : 1;
-    int prev_lat = -1;
-    for (int k = 1; k <= radius; ++k) {
-      lat.push_back(sign * k); fwd.push_back(0); parent.push_back(prev_lat);
-      prev_lat = (int)lat.size() - 1;
-      int pf = prev_lat;
-      for (int i = 1; i <= length - k; ++i) { lat.push_back(sign * k); fwd.push_back(i); parent.push_back(pf); pf = (int)lat.size() - 1; }
-    }
-  }
-  if (lat.size() > MP_MAX_BEAM_CELLS) return false;
-  g->n = (int)lat.size();
-  g->depth = length + radius;
-  for (int i = 0; i < g->n; ++i) { g->lat[i] = (int8_t)lat[i]; g->fwd[i] = (int8_t)fwd[i]; g->parent[i] = (int8_t)parent[i]; }
-  return true;
-}
-
-// A beam of `length` cells forward and `radius` to each side covers forward offsets 0..length and lateral offsets
-// -radius..radius around the shooter. On a TORUS map that is smaller than the map in both directions, each footprint
-// cell wraps with one conditional add (wrap_or_reject) and no two cells of a footprint land on the same map cell.
-bool beam_fits_torus(const Tables& T, int length, int radius) {
-  const int m = std::min(T.W, T.H);
-  return T.topology != 1 || (length < m && 2 * radius + 1 <= m);
-}
 
 // Deals the cells of one strip to lanes so that the 64-bit staging stores of every half-warp are bank-conflict free.
 // A strip is `n_rows` pixel rows (8 for a player cell-row, 4 or 2 for WORLD.RGB) by `n_cells` cells of 24 bytes at a
@@ -194,13 +126,30 @@ int make_lane_map_cells(int n_rows, int n_cells, int pitch_slots, int iters, uin
   return best;
 }
 
+// One row per substrate family: the blob decode (host, step_<family>.cuh) and the state-transition kernel with the
+// dynamic shared memory one launch of it takes.
+using StepFn = void (*)(Tables, State, const int32_t*, const uint8_t*, int);
+struct FamilyEntry {
+  int id;  // MpbFamily
+  int (*load)(FamilyLoad&, Tables&);
+  StepFn step;
+  size_t (*step_smem)(const Tables&);
+};
+const FamilyEntry kFamilies[] = {
+    {MPB_FAMILY_CLEAN_UP, CleanUp::load, k_step<CleanUp>, step_smem_bytes<CleanUp>},
+    {MPB_FAMILY_COMMONS_HARVEST, Commons::load, k_step<Commons>, step_smem_bytes<Commons>},
+    {MPB_FAMILY_TERRITORY, Territory::load, k_step<Territory>, step_smem_bytes<Territory>},
+    {MPB_FAMILY_COINS, Coins::load, k_step<Coins>, step_smem_bytes<Coins>},
+    {MPB_FAMILY_COOP_MINING, Mining::load, k_step<Mining>, step_smem_bytes<Mining>},
+};
+
 }  // namespace
 
 struct mp_engine {
   int device = 0;
   int B = 0;
   uint32_t flags = MP_FLAG_DEFAULT;
-  int family = 0;
+  const FamilyEntry* family = nullptr;
   int n_total = 0;  // atlas sprites incl. pre-merged
   Tables T{};
   State S{};
@@ -225,7 +174,6 @@ struct mp_engine {
   int32_t* d_avatar_dbg = nullptr;
   uint64_t launches = 0;
   int sm_count = 0;
-  void (*step_fn)(Tables, State, const int32_t*, const uint8_t*, int) = nullptr;
   size_t step_smem = 0;  // dynamic shared memory of one state-transition launch
   void (*render_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
   void (*render_gather_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
@@ -245,17 +193,6 @@ struct mp_engine {
   int inst_ncp = 0, inst_ncw = 0;                // the k_render<NCP, NCW> instantiation this engine launches
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob: a snapshot only loads into an engine built from the same blob
 
-  template <typename T>
-  int upload(const std::vector<T>& host, const T** out) {
-    void* p = nullptr;
-    size_t bytes = std::max<size_t>(host.size() * sizeof(T), 16);
-    CUDA_TRY(cudaMalloc(&p, bytes));
-    allocs.push_back(p);
-    CUDA_TRY(cudaMemset(p, 0, bytes));
-    if (!host.empty()) CUDA_TRY(cudaMemcpy(p, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice));
-    *out = static_cast<const T*>(p);
-    return MP_OK;
-  }
   template <typename T>
   int alloc(size_t count, T** out) {
     void* p = nullptr;
@@ -282,7 +219,6 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   NEED(atlas, MPB_U8) NEED(sprite_opaque, MPB_U8) NEED(cell_flags, MPB_U8) NEED(init_grid, MPB_U16)
   const int32_t* m = meta.data;
   Tables& T = E->T;
-  E->family = m[MPB_META_FAMILY];
   T.W = m[MPB_META_W]; T.H = m[MPB_META_H]; T.cells = T.W * T.H; T.cells_pad = round_up(T.cells, 8);
   T.L = m[MPB_META_L]; T.P = m[MPB_META_P]; T.topology = m[MPB_META_TOPOLOGY]; T.max_frames = m[MPB_META_MAX_FRAMES];
   T.view_l = m[MPB_META_VIEW_LEFT]; T.view_r = m[MPB_META_VIEW_RIGHT]; T.view_f = m[MPB_META_VIEW_FORWARD]; T.view_b = m[MPB_META_VIEW_BACKWARD];
@@ -298,7 +234,8 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   if (T.topology == 1 && (T.view_l + T.view_r + 1 > T.W || T.view_f + T.view_b + 1 > T.H || T.view_l + T.view_r + 1 > T.H || T.view_f + T.view_b + 1 > T.W))
     return fail(MP_E_UNSUPPORTED, "TORUS map smaller than the view window");
   for (int k = 0; k < T.n_scalar; ++k) T.scalar_obs[k] = scalar_obs.data[k];
-  if (E->family != MPB_FAMILY_CLEAN_UP && E->family != MPB_FAMILY_COMMONS_HARVEST && E->family != MPB_FAMILY_TERRITORY && E->family != MPB_FAMILY_COINS && E->family != MPB_FAMILY_COOP_MINING) return fail(MP_E_UNSUPPORTED, "substrate family %d has no CUDA state-transition kernel yet", E->family);
+  for (const FamilyEntry& f : kFamilies) if (f.id == m[MPB_META_FAMILY]) E->family = &f;
+  if (!E->family) return fail(MP_E_UNSUPPORTED, "substrate family %d has no CUDA state-transition kernel yet", m[MPB_META_FAMILY]);
 
   // ---- avatars ---------------------------------------------------------------------------------
   T.avatar_layer = av_table.data[2];
@@ -341,167 +278,25 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   if (T.n_spawn < 1) return fail(MP_E_INVALID, "empty respawn group");
 
   // ---- family tables -----------------------------------------------------------------------------
-  int rc;
-  std::vector<int32_t> v_apple, v_dirt, v_water;
-  std::vector<std::vector<int>> hint_stacks;  // sprite stacks (bottom up) worth a pre-merged sprite before the generic enumeration
   T.nA = T.nD = T.nW = 0; T.nR = 0; T.nR_pad = 16;
   T.n_anim = 1; T.anim_frames = 1; T.clean_layer = 0;
-  auto zapper = [&](const int32_t* ip) -> int {  // shared Zapper block of cu_ip / ch_ip
-    T.zap_cooldown = ip[12]; T.zap_respawn = ip[15]; T.zap_remove = ip[16];
-    T.zap_layer = ip[21]; T.zap_sprite = ip[22];
-    T.zap_hit = 0;
-    for (int h = 0; h < (int)hits.count / 2; ++h) if (hits.data[h * 2] == T.zap_layer) T.zap_hit = h;
-    if (T.zap_cooldown <= 0) return fail(MP_E_UNSUPPORTED, "non-positive zap cooldown");
-    if (!make_beam_geom(ip[13], ip[14], &T.zap_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
-    if (!beam_fits_torus(T, ip[13], ip[14])) return fail(MP_E_UNSUPPORTED, "zap beam (length %d, radius %d) does not fit the %dx%d TORUS map", ip[13], ip[14], T.W, T.H);
-    T.end_min_frames = ip[26]; T.end_interval = ip[27];
-    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
-    return MP_OK;
-  };
-  if (E->family == MPB_FAMILY_CLEAN_UP) {
-    Section<int32_t> cu_ip, cu_apple, cu_dirt, cu_water, cu_water_sprites;
-    Section<double> cu_dp;
-    NEED(cu_ip, MPB_I32) NEED(cu_dp, MPB_F64) NEED(cu_apple, MPB_I32) NEED(cu_dirt, MPB_I32) NEED(cu_water, MPB_I32) NEED(cu_water_sprites, MPB_I32)
-    const int32_t* ip = cu_ip.data; const double* dp = cu_dp.data;
-    T.nA = ip[0]; T.nD = ip[1]; T.nW = ip[2];
-    T.apple_layer = ip[3]; T.apple_sprite = ip[4]; T.dirt_layer = ip[5]; T.dirt_sprite = ip[6];
-    T.water_layer = ip[8]; T.n_anim = ip[9]; T.anim_frames = ip[10]; T.anim_random = ip[11];
-    if (T.n_anim < 1 || T.n_anim > 8 || T.anim_frames < 1) return fail(MP_E_UNSUPPORTED, "animation with %d states / %d frames", T.n_anim, T.anim_frames);
-    for (int i = 0; i < T.n_anim; ++i) T.water_sprite[i] = cu_water_sprites.data[i];
-    if ((rc = zapper(ip))) return rc;
-    T.clean_cooldown = ip[18]; T.clean_layer = ip[23]; T.clean_sprite = ip[24];
-    T.clean_hit = 1;
-    for (int h = 0; h < (int)hits.count / 2; ++h) if (hits.data[h * 2] == T.clean_layer) T.clean_hit = h;
-    if (T.clean_cooldown < 0) return fail(MP_E_UNSUPPORTED, "negative clean cooldown");
-    if (!make_beam_geom(ip[19], ip[20], &T.clean_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
-    if (!beam_fits_torus(T, ip[19], ip[20])) return fail(MP_E_UNSUPPORTED, "clean beam (length %d, radius %d) does not fit the %dx%d TORUS map", ip[19], ip[20], T.W, T.H);
-    T.dirt_delay = ip[25]; T.taste_role = ip[28];
-    if (T.taste_role != 0) return fail(MP_E_UNSUPPORTED, "Taste roles other than 'free'");
-    T.grow_rate = dp[0]; T.grow_depletion = dp[1]; T.grow_restoration = dp[2]; T.eat_reward = dp[3];
-    T.zap_penalty = dp[4]; T.zap_reward = dp[5]; T.dirt_prob = dp[6]; T.end_prob = dp[7]; T.taste_amount = dp[8];
-    v_apple.assign(cu_apple.data, cu_apple.data + cu_apple.count);
-    v_dirt.assign(cu_dirt.data, cu_dirt.data + cu_dirt.count);
-    v_water.assign(cu_water.data, cu_water.data + cu_water.count);
-    if ((rc = E->upload(v_apple, &T.apple)) || (rc = E->upload(v_dirt, &T.dirt)) || (rc = E->upload(v_water, &T.water))) return rc;
-  } else if (E->family == MPB_FAMILY_COMMONS_HARVEST) {
-    Section<int32_t> ch_ip, ch_apple, ch_nbr;
-    Section<double> ch_dp;
-    NEED(ch_ip, MPB_I32) NEED(ch_dp, MPB_F64) NEED(ch_apple, MPB_I32) NEED(ch_nbr, MPB_I32)
-    const int32_t* ip = ch_ip.data; const double* dp = ch_dp.data;
-    T.nA = ip[0]; T.apple_layer = ip[1]; T.apple_sprite = ip[2]; T.wait_layer = ip[3]; T.wait_sprite = ip[4];
-    T.ch_n_wait = ip[5]; T.ch_n_probs = ip[6]; T.grass_layer = ip[7]; T.grass_sprite = ip[8]; T.dess_sprite = ip[9];
-    if (T.ch_n_wait < 1 || T.ch_n_wait > 29 || T.ch_n_probs < 1 || T.ch_n_probs > 4) return fail(MP_E_UNSUPPORTED, "DensityRegrow with %d wait states / %d probabilities", T.ch_n_wait, T.ch_n_probs);
-    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d apples (max 2048)", T.nA);
-    if ((rc = zapper(ip))) return rc;
-    for (int i = 0; i < 4; ++i) T.ch_probs[i] = dp[i];
-    T.eat_reward = dp[4]; T.zap_penalty = dp[5]; T.zap_reward = dp[6]; T.end_prob = dp[7];
-    v_apple.assign(ch_apple.data, ch_apple.data + ch_apple.count);
-    std::vector<int32_t> v_nbr(ch_nbr.data, ch_nbr.data + ch_nbr.count);
-    if ((rc = E->upload(v_apple, &T.ch_apple)) || (rc = E->upload(v_nbr, &T.ch_nbr))) return rc;
-  }
-  else if (E->family == MPB_FAMILY_COINS) {
-    Section<int32_t> co_ip, co_coin;
-    Section<double> co_dp;
-    NEED(co_ip, MPB_I32) NEED(co_dp, MPB_F64) NEED(co_coin, MPB_I32)
-    const int32_t* ip = co_ip.data; const double* dp = co_dp.data;
-    if (T.P != 2) return fail(MP_E_UNSUPPORTED, "coins needs exactly two players (got %d)", T.P);
-    T.nA = ip[0]; T.apple_layer = ip[1]; T.coin_sprite[0] = ip[2]; T.coin_sprite[1] = ip[3];
-    T.coin_terminate = ip[4]; T.coin_terminate_n = ip[5]; T.end_min_frames = ip[6]; T.end_interval = ip[7];
-    T.coin_type[0] = ip[8]; T.coin_type[1] = ip[9];
-    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d coins (max 2048)", T.nA);
-    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
-    T.coin_rate = dp[0]; T.end_prob = dp[1];
-    for (int p = 0; p < 2; ++p) for (int k = 0; k < 4; ++k) T.coin_reward[p][k] = dp[4 + p * 4 + k];
-    T.zap_layer = 0; T.zap_cooldown = 1;
-    v_apple.resize((size_t)T.nA * 4);
-    for (int k = 0; k < T.nA; ++k) { v_apple[k * 4] = co_coin.data[k * 2]; v_apple[k * 4 + 1] = co_coin.data[k * 2 + 1]; v_apple[k * 4 + 2] = 0; v_apple[k * 4 + 3] = -1; }
-    if ((rc = E->upload(v_apple, &T.ch_apple))) return rc;
-  }
-  else if (E->family == MPB_FAMILY_COOP_MINING) {
-    Section<int32_t> cm_ip, cm_ore;
-    Section<double> cm_dp;
-    NEED(cm_ip, MPB_I32) NEED(cm_dp, MPB_F64) NEED(cm_ore, MPB_I32)
-    const int32_t* ip = cm_ip.data; const double* dp = cm_dp.data;
-    T.nA = ip[0]; T.apple_layer = ip[1];
-    for (int i = 0; i < 4; ++i) T.ore_sprite[i] = ip[2 + i];
-    T.mine_window = ip[6]; T.zap_cooldown = ip[7]; T.mine_length = ip[8]; T.zap_layer = ip[9]; T.zap_sprite = ip[10];
-    T.end_min_frames = ip[11]; T.end_interval = ip[12]; T.zap_hit = ip[13];
-    if (T.P > 8) return fail(MP_E_UNSUPPORTED, "coop_mining with %d players (max 8: miners are kept as a bit mask)", T.P);
-    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d ores (max 2048)", T.nA);
-    if (T.zap_cooldown < 1 || T.mine_window < 1 || T.mine_window > 255 || T.mine_length < 1) return fail(MP_E_UNSUPPORTED, "MineBeam / Ore parameters out of range");
-    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
-    if (T.zap_hit < 0 || T.zap_hit > 7) return fail(MP_E_UNSUPPORTED, "mine hit id %d", T.zap_hit);
-    if (!beam_fits_torus(T, T.mine_length, 0)) return fail(MP_E_UNSUPPORTED, "mine beam (length %d) does not fit the %dx%d TORUS map", T.mine_length, T.W, T.H);
-    T.mine_rate[0] = dp[0]; T.mine_rate[1] = dp[1]; T.end_prob = dp[2];
-    T.mine_reward[0] = dp[4]; T.mine_reward[1] = dp[5]; T.extract_reward[0] = dp[6]; T.extract_reward[1] = dp[7];
-    v_apple.resize((size_t)T.nA * 4);
-    for (int k = 0; k < T.nA; ++k) { v_apple[k * 4] = cm_ore.data[k * 2]; v_apple[k * 4 + 1] = cm_ore.data[k * 2 + 1]; v_apple[k * 4 + 2] = 0; v_apple[k * 4 + 3] = -1; }
-    if ((rc = E->upload(v_apple, &T.ch_apple))) return rc;
-  }
-  else {  // MPB_FAMILY_TERRITORY
-    Section<int32_t> tr_ip, tr_res, tr_player_sprites;
-    Section<double> tr_dp;
-    Section<uint8_t> tr_wall;
-    NEED(tr_ip, MPB_I32) NEED(tr_dp, MPB_F64) NEED(tr_res, MPB_I32) NEED(tr_player_sprites, MPB_I32) NEED(tr_wall, MPB_U8)
-    const int32_t* ip = tr_ip.data; const double* dp = tr_dp.data;
-    T.nR = ip[0]; T.nR_pad = round_up(std::max(T.nR, 64), 16);
-    T.res_layer = ip[1]; T.unclaimed_sprite = ip[2]; T.tex_layer = ip[3]; T.tex_sprite = ip[4]; T.ind_layer = ip[5];
-    T.dmg_layer = ip[6]; T.dmg_sprite = ip[7]; T.mark_layer = ip[8]; T.mark_initial_level = ip[9]; T.mark_recovery = ip[10]; T.mark_n_levels = ip[11];
-    if (T.res_layer != T.avatar_layer) return fail(MP_E_UNSUPPORTED, "territory: resources and avatars must share a layer");
-    if (T.mark_n_levels < 1 || T.mark_n_levels > 3) return fail(MP_E_UNSUPPORTED, "%d marking levels (1..3)", T.mark_n_levels);
-    if ((rc = zapper(ip))) return rc;
-    if (T.zap_respawn <= T.max_frames) return fail(MP_E_UNSUPPORTED, "territory kernel assumes avatars never respawn (framesTillRespawn %d)", T.zap_respawn);
-    if (!make_beam_geom(ip[18], ip[19], &T.claim_geom) || !make_beam_geom(1, 0, &T.brush_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
-    if (!beam_fits_torus(T, ip[18], ip[19])) return fail(MP_E_UNSUPPORTED, "claim beam (length %d, radius %d) does not fit the %dx%d TORUS map", ip[18], ip[19], T.W, T.H);
-    T.claim_wait = ip[20]; T.brush_layer = ip[23]; T.claim_layer = ip[24];
-    if (T.claim_layer != T.dmg_layer) return fail(MP_E_UNSUPPORTED, "territory: claim beam layer must be the damage indicator layer");
-    T.res_health0 = ip[28]; T.res_reward_delay = ip[29]; T.res_repair_delay = ip[30]; T.tr_taste_role = ip[31];
-    if (T.tr_taste_role != 0) return fail(MP_E_UNSUPPORTED, "territory Taste roles other than 'none'");
-    if (T.res_health0 < 1 || T.res_health0 > 200) return fail(MP_E_UNSUPPORTED, "resource health %d", T.res_health0);
-    // the resource age and frames-since-zapped counters saturate at 65535 (step_territory.cuh)
-    if (T.res_reward_delay > 65535 || T.res_repair_delay > 65535)
-      return fail(MP_E_UNSUPPORTED, "rewardDelay %d / delayTillSelfRepair %d (max 65535)", T.res_reward_delay, T.res_repair_delay);
-    for (int l = 0; l < T.mark_n_levels; ++l) {
-      T.mark_inc[l] = ip[32 + 4 * l]; T.mark_remove[l] = ip[33 + 4 * l]; T.mark_freeze[l] = ip[34 + 4 * l]; T.mark_sprite[l] = ip[35 + 4 * l];
-      T.mark_src_reward[l] = dp[8 + 2 * l]; T.mark_tgt_reward[l] = dp[9 + 2 * l];
-    }
-    T.res_reward = dp[0]; T.res_rate = dp[1]; T.res_repair_prob = dp[2]; T.zap_penalty = dp[3]; T.zap_reward = dp[4]; T.end_prob = dp[5];
-    T.tr_taste_amount = dp[6]; T.tr_taste_mult = dp[7];
-    for (int p = 0; p < T.P; ++p) {
-      const int32_t* ps = tr_player_sprites.data + p * 4;
-      T.claimed_sprite[p] = ps[0]; T.dry_sprite[p] = ps[1]; T.brush_sprite[p] = ps[2]; T.claimbeam_sprite[p] = ps[3];
-    }
-    for (int p = 0; p < T.P; ++p) {  // wet paint on the resource texture, then dry paint on top: what most resource cells show
-      hint_stacks.push_back({T.tex_sprite, T.claimed_sprite[p]});
-      hint_stacks.push_back({T.tex_sprite, T.claimed_sprite[p], T.dry_sprite[p]});
-    }
-    std::vector<int32_t> v_res(tr_res.data, tr_res.data + tr_res.count);
-    std::vector<int16_t> res_of(T.cells_pad, -1);
-    for (int k = 0; k < T.nR; ++k) res_of[v_res[k * 3 + 1]] = (int16_t)k;
-    std::vector<uint8_t> wall(T.cells_pad, 0);
-    memcpy(wall.data(), tr_wall.data, std::min<size_t>(tr_wall.count, T.cells));
-    if ((rc = E->upload(v_res, &T.tr_res)) || (rc = E->upload(res_of, &T.res_of_cell)) || (rc = E->upload(wall, &T.wall))) return rc;
-    Section<int32_t> tr_res_cond;
-    if (get_section(blob, n, "tr_res_cond", MPB_I32, &tr_res_cond)) {
-      if ((int)tr_res_cond.count != T.nR * 2) return fail(MP_E_INVALID, "blob: tr_res_cond has %zu values for %d resources", tr_res_cond.count, T.nR);
-      std::vector<int32_t> v(tr_res_cond.data, tr_res_cond.data + tr_res_cond.count);
-      if ((rc = E->upload(v, &T.tr_res_cond))) return rc;
-    }
-  }
+  FamilyLoad ld{blob, n, hits, E->allocs};
+  int rc;
+  if ((rc = E->family->load(ld, T))) return rc;
 #undef NEED
   {  // 'choice' prefabs left to the engine (drawn per env and episode)
     Section<int32_t> choice_groups, obj_choice, spawn_cond;
     if (get_section(blob, n, "choice_groups", MPB_I32, &choice_groups)) {
-      if (E->family != MPB_FAMILY_TERRITORY) return fail(MP_E_UNSUPPORTED, "per-env 'choice' prefabs are implemented for the territory family only (compile with a build_seed)");
+      if (E->family->id != MPB_FAMILY_TERRITORY) return fail(MP_E_UNSUPPORTED, "per-env 'choice' prefabs are implemented for the territory family only (compile with a build_seed)");
       T.n_choice = (int)choice_groups.count;
       for (size_t g = 0; g < choice_groups.count; ++g) if (choice_groups.data[g] < 1 || choice_groups.data[g] > 31) return fail(MP_E_INVALID, "blob: choice group with %d options", choice_groups.data[g]);
       std::vector<int32_t> v(choice_groups.data, choice_groups.data + choice_groups.count);
-      if ((rc = E->upload(v, &T.choice_n))) return rc;
+      if ((rc = upload(E->allocs, v, &T.choice_n))) return rc;
       snprintf(name, sizeof name, "spawn_cond_%d", respawn_group);
       if (get_section(blob, n, name, MPB_I32, &spawn_cond)) {
         if ((int)spawn_cond.count != T.n_spawn * 2 || T.n_spawn > 64) return fail(MP_E_UNSUPPORTED, "%d conditional spawn candidates (max 64)", T.n_spawn);
         std::vector<int32_t> c(spawn_cond.data, spawn_cond.data + spawn_cond.count);
-        if ((rc = E->upload(c, &T.spawn_cond))) return rc;
+        if ((rc = upload(E->allocs, c, &T.spawn_cond))) return rc;
       }
     }
   }
@@ -510,13 +305,13 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   // ---- device copies -----------------------------------------------------------------------------
   std::vector<uint16_t> grid0((size_t)T.L * T.cells_pad, 0);
   for (int l = 0; l < T.L; ++l) memcpy(&grid0[(size_t)l * T.cells_pad], init_grid.data + (size_t)l * T.cells, T.cells * sizeof(uint16_t));
-  if ((rc = E->upload(grid0, &T.init_grid))) return rc;
+  if ((rc = upload(E->allocs, grid0, &T.init_grid))) return rc;
   std::vector<int32_t> act(action_table.data, action_table.data + action_table.count);
-  if ((rc = E->upload(act, &T.action_table))) return rc;
-  if ((rc = E->upload(v_spawn, &T.spawn_cell))) return rc;
+  if ((rc = upload(E->allocs, act, &T.action_table))) return rc;
+  if ((rc = upload(E->allocs, v_spawn, &T.spawn_cell))) return rc;
   for (int k = 0; k < 2; ++k) {
     if (v_init[k].empty()) { T.spawn_init_cell[k] = T.spawn_cell; continue; }
-    if ((rc = E->upload(v_init[k], &T.spawn_init_cell[k]))) return rc;
+    if ((rc = upload(E->allocs, v_init[k], &T.spawn_init_cell[k]))) return rc;
   }
   std::vector<uint8_t> solid(T.cells_pad, 0), flags(T.cells_pad, 0);
   for (int o = 0; o < m[MPB_META_N_OBJECTS]; ++o) {  // non-avatar pieces that start on the avatar layer
@@ -527,13 +322,11 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     if (st[MPB_STATE_LAYER] == T.avatar_layer) solid[od[MPB_OBJ_Y] * T.W + od[MPB_OBJ_X]] = 255;
   }
   memcpy(flags.data(), cell_flags.data, std::min<size_t>(cell_flags.count, T.cells));
-  if ((rc = E->upload(solid, &T.solid)) || (rc = E->upload(flags, &T.cell_flags))) return rc;
+  if ((rc = upload(E->allocs, solid, &T.solid)) || (rc = upload(E->allocs, flags, &T.cell_flags))) return rc;
   std::vector<int16_t> apple_of(T.cells_pad, -1), dirt_of(T.cells_pad, -1);
-  T.dirt_count0 = 0;
-  const int apple_cols = E->family == MPB_FAMILY_CLEAN_UP ? 3 : 4;
-  for (int k = 0; k < T.nA; ++k) apple_of[v_apple[k * apple_cols + 1]] = (int16_t)k;
-  for (int j = 0; j < T.nD; ++j) { dirt_of[v_dirt[j * 3 + 1]] = (int16_t)j; T.dirt_count0 += v_dirt[j * 3 + 2]; }
-  if ((rc = E->upload(apple_of, &T.apple_of_cell)) || (rc = E->upload(dirt_of, &T.dirt_of_cell))) return rc;
+  for (size_t k = 0; k < ld.apple_cells.size(); ++k) apple_of[ld.apple_cells[k]] = (int16_t)k;
+  for (size_t j = 0; j < ld.dirt_cells.size(); ++j) dirt_of[ld.dirt_cells[j]] = (int16_t)j;
+  if ((rc = upload(E->allocs, apple_of, &T.apple_of_cell)) || (rc = upload(E->allocs, dirt_of, &T.dirt_of_cell))) return rc;
 
   // ---- render tables ------------------------------------------------------------------------------
   if (atlas.count != (size_t)T.n_sprites * 1024) return fail(MP_E_INVALID, "atlas has %zu bytes, expected %d", atlas.count, T.n_sprites * 1024);
@@ -598,7 +391,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
         }
       }
     }
-    for (const auto& hs : hint_stacks) {
+    for (const auto& hs : ld.hint_stacks) {
       if (hs.empty() || !opq[hs[0]]) continue;
       int cur = hs[0];
       for (size_t q = 1; q < hs.size() && cur; ++q) { if (remapped[hs[q]] || remapped[cur]) break; cur = merged_id(cur, hs[q]); }
@@ -659,7 +452,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     for (int row = 0; row < 8; ++row)
       for (int half = 0; half < 2; ++half)
         memcpy(&at[(size_t)s * 256 + half * 128 + row * 16], &img[(size_t)s * 256 + row * 32 + half * 16], 16);
-  if ((rc = E->upload(at, &T.atlas))) return rc;
+  if ((rc = upload(E->allocs, at, &T.atlas))) return rc;
   std::vector<int16_t> smap((size_t)(T.P + 1) * n_total);
   for (int v = 0; v <= T.P; ++v)
     for (int s = 0; s < n_total; ++s)
@@ -689,7 +482,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     for (int px = 0; px < 256 && black; ++px) { const uint8_t* q = &img[(size_t)i * 1024 + px * 4]; black = q[0] == 0 && q[1] == 0 && q[2] == 0; }
     if (black) E->black_sprite = i;
   }
-  if ((rc = E->upload(smap, &T.sprite_map)) || (rc = E->upload(sflags, &T.sprite_opaque)) || (rc = E->upload(pair, &T.sprite_pair))) return rc;
+  if ((rc = upload(E->allocs, smap, &T.sprite_map)) || (rc = upload(E->allocs, sflags, &T.sprite_opaque)) || (rc = upload(E->allocs, pair, &T.sprite_pair))) return rc;
   return MP_OK;
 }
 
@@ -789,19 +582,6 @@ __global__ void k_debug_obs(Tables T, State S, int32_t* position, int32_t* orien
   }
 }
 
-// The state-transition kernel of each substrate family and the dynamic shared memory one launch of it takes.
-using StepFn = void (*)(Tables, State, const int32_t*, const uint8_t*, int);
-const StepFn kStepKernels[] = {k_step<CleanUp>, k_step<Commons>, k_step<Territory>, k_step<Coins>, k_step<Mining>};
-StepFn step_kernel(int family, const Tables& T, size_t* smem) {
-  switch (family) {
-    case MPB_FAMILY_CLEAN_UP: *smem = step_smem_bytes<CleanUp>(T); return k_step<CleanUp>;
-    case MPB_FAMILY_COMMONS_HARVEST: *smem = step_smem_bytes<Commons>(T); return k_step<Commons>;
-    case MPB_FAMILY_COINS: *smem = step_smem_bytes<Coins>(T); return k_step<Coins>;
-    case MPB_FAMILY_COOP_MINING: *smem = step_smem_bytes<Mining>(T); return k_step<Mining>;
-    default: *smem = step_smem_bytes<Territory>(T); return k_step<Territory>;
-  }
-}
-
 int raise_flags(mp_engine* E, cudaStream_t st) {
   E->x_pending_raise = false;
   k_exchange_push<<<std::min(E->sm_count, (E->B + 7) / 8), 256, 0, st>>>(E->T, E->S);
@@ -820,7 +600,7 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->step_fn, E->T, E->S, actions, mask, mode));
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->family->step, E->T, E->S, actions, mask, mode));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st); }
@@ -972,7 +752,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     cudaError_t ce = cudaMemcpy(S.env, env0.data(), env0.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
     if (ce != cudaSuccess) { mp_destroy(E); return fail(MP_E_CUDA, "cudaMemcpy(env) failed: %s", cudaGetErrorString(ce)); }
   }
-  E->step_fn = step_kernel(E->family, T, &E->step_smem);
+  E->step_smem = E->family->step_smem(T);
   {  // cells per lane per strip: ceil(view_w / 4) for player rows, ceil(W / 8) for world half-rows
     const int ncp = (E->R.view_w + 3) / 4, ncw = (T.W + (32 >> E->R.wstrip_log2) - 1) / (32 >> E->R.wstrip_log2);
     if (ncp <= 3 && ncw <= 3) { E->render_fn = k_render<3, 3, false>; E->render_gather_fn = k_render<3, 3, true>; E->inst_ncp = 3; E->inst_ncw = 3; }
@@ -1002,8 +782,8 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     static int step_smem_max[MP_MAX_DEVICES] = {};
     const int need = (int)E->step_smem;
     if (ce == cudaSuccess && need > 48 * 1024 && need > step_smem_max[device]) {
-      for (StepFn fn : kStepKernels)
-        if (ce == cudaSuccess) ce = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+      for (const FamilyEntry& f : kFamilies)
+        if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
       if (ce == cudaSuccess) step_smem_max[device] = need;
     }
   }

@@ -1,0 +1,149 @@
+// family_load.h -- host side: the blob access, error reporting and device uploads that build_tables (engine.cu) and the
+// family loaders (`load` in each step_<family>.cuh) share. engine.cu is the only translation unit; it includes this
+// header through the family headers.
+#pragma once
+
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdarg>
+#include <cstdio>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/mp_engine.h"
+#include "../../include/mpb_format.h"
+#include "common.cuh"
+
+namespace {
+
+thread_local std::string g_error;
+
+int fail(int code, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof buf, fmt, ap);
+  va_end(ap);
+  g_error = buf;
+  return code;
+}
+
+#define CUDA_TRY(expr)                                                                          \
+  do {                                                                                          \
+    cudaError_t e_ = (expr);                                                                    \
+    if (e_ != cudaSuccess) return fail(MP_E_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e_)); \
+  } while (0)
+
+template <typename T>
+struct Section {
+  const T* data = nullptr;
+  std::vector<uint32_t> shape;
+  size_t count = 0;
+};
+
+template <typename T>
+bool get_section(const void* blob, size_t n, const char* name, int dtype, Section<T>* out) {
+  const MpbSection* s = mpb_find(blob, n, name);
+  if (!s || (int)s->dtype != dtype) return false;
+  out->data = static_cast<const T*>(mpb_data(blob, s));
+  out->shape.assign(s->shape, s->shape + s->ndim);
+  out->count = s->nbytes / sizeof(T);
+  return true;
+}
+
+int round_up(int v, int m) { return (v + m - 1) / m * m; }
+
+// Copies `host` into a new zero-padded device allocation (at least 16 bytes), recorded in `allocs`.
+template <typename T>
+int upload(std::vector<void*>& allocs, const std::vector<T>& host, const T** out) {
+  void* p = nullptr;
+  size_t bytes = std::max<size_t>(host.size() * sizeof(T), 16);
+  CUDA_TRY(cudaMalloc(&p, bytes));
+  allocs.push_back(p);
+  CUDA_TRY(cudaMemset(p, 0, bytes));
+  if (!host.empty()) CUDA_TRY(cudaMemcpy(p, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice));
+  *out = static_cast<const T*>(p);
+  return MP_OK;
+}
+
+// Beam footprint in visiting order (policy A.8): centre ray, then for each side the lateral cells
+// outwards, each followed by its forward ray of length `length - k`.
+bool make_beam_geom(int length, int radius, BeamGeom* g) {
+  std::vector<int> lat, fwd, parent;
+  int prev = -1;
+  for (int i = 1; i <= length; ++i) { lat.push_back(0); fwd.push_back(i); parent.push_back(prev); prev = (int)lat.size() - 1; }
+  for (int side = 0; side < 2; ++side) {
+    int sign = side == 0 ? -1 : 1;
+    int prev_lat = -1;
+    for (int k = 1; k <= radius; ++k) {
+      lat.push_back(sign * k); fwd.push_back(0); parent.push_back(prev_lat);
+      prev_lat = (int)lat.size() - 1;
+      int pf = prev_lat;
+      for (int i = 1; i <= length - k; ++i) { lat.push_back(sign * k); fwd.push_back(i); parent.push_back(pf); pf = (int)lat.size() - 1; }
+    }
+  }
+  if (lat.size() > MP_MAX_BEAM_CELLS) return false;
+  g->n = (int)lat.size();
+  g->depth = length + radius;
+  for (int i = 0; i < g->n; ++i) { g->lat[i] = (int8_t)lat[i]; g->fwd[i] = (int8_t)fwd[i]; g->parent[i] = (int8_t)parent[i]; }
+  return true;
+}
+
+// A beam of `length` cells forward and `radius` to each side covers forward offsets 0..length and lateral offsets
+// -radius..radius around the shooter. On a TORUS map that is smaller than the map in both directions, each footprint
+// cell wraps with one conditional add (wrap_or_reject) and no two cells of a footprint land on the same map cell.
+bool beam_fits_torus(const Tables& T, int length, int radius) {
+  const int m = std::min(T.W, T.H);
+  return T.topology != 1 || (length < m && 2 * radius + 1 <= m);
+}
+
+// What build_tables hands a family's loader, and what the loader hands back besides the Tables fields it sets. On entry
+// the Tables hold the geometry, the avatar tables and zero entity counts.
+struct FamilyLoad {
+  const void* blob;
+  size_t n;
+  Section<int32_t> hits;               // [n_hits][2] layer, sprite
+  std::vector<void*>& allocs;          // the engine's device allocations
+  std::vector<int32_t> apple_cells;    // cell of each apple / coin / ore: apple_of_cell
+  std::vector<int32_t> dirt_cells;     // cell of each dirt: dirt_of_cell
+  std::vector<std::vector<int>> hint_stacks;  // sprite stacks (bottom up) worth a pre-merged sprite before the generic enumeration
+
+  template <typename T>
+  int need(const char* name, int dtype, Section<T>* out) const {
+    return get_section(blob, n, name, dtype, out) ? MP_OK : fail(MP_E_INVALID, "blob: missing section '%s'", name);
+  }
+  // The family's parameter blocks "<prefix>_ip" (int32[n_int]) and "<prefix>_dp" (f64[n_f64]), see mpb_format.h.
+  int params(const char* prefix, size_t n_int, size_t n_f64, const int32_t** ip, const double** dp) const {
+    char name[16];
+    Section<int32_t> si;
+    Section<double> sd;
+    int rc;
+    snprintf(name, sizeof name, "%s_ip", prefix);
+    if ((rc = need(name, MPB_I32, &si))) return rc;
+    if (si.count < n_int) return fail(MP_E_INVALID, "blob: section '%s' has %zu values (expected %zu)", name, si.count, n_int);
+    snprintf(name, sizeof name, "%s_dp", prefix);
+    if ((rc = need(name, MPB_F64, &sd))) return rc;
+    if (sd.count < n_f64) return fail(MP_E_INVALID, "blob: section '%s' has %zu values (expected %zu)", name, sd.count, n_f64);
+    *ip = si.data; *dp = sd.data;
+    return MP_OK;
+  }
+};
+
+// The Zapper and episode-ending slots (MPB_FP_*) of clean_up, commons_harvest and territory.
+int load_zapper(const FamilyLoad& ld, Tables& T, const int32_t* ip) {
+  T.zap_cooldown = ip[MPB_FP_ZAP_COOLDOWN]; T.zap_respawn = ip[MPB_FP_ZAP_RESPAWN]; T.zap_remove = ip[MPB_FP_ZAP_REMOVE];
+  T.zap_layer = ip[MPB_FP_ZAP_LAYER]; T.zap_sprite = ip[MPB_FP_ZAP_SPRITE];
+  T.zap_hit = 0;
+  for (int h = 0; h < (int)ld.hits.count / 2; ++h) if (ld.hits.data[h * 2] == T.zap_layer) T.zap_hit = h;
+  const int length = ip[MPB_FP_ZAP_LENGTH], radius = ip[MPB_FP_ZAP_RADIUS];
+  if (T.zap_cooldown <= 0) return fail(MP_E_UNSUPPORTED, "non-positive zap cooldown");
+  if (!make_beam_geom(length, radius, &T.zap_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+  if (!beam_fits_torus(T, length, radius)) return fail(MP_E_UNSUPPORTED, "zap beam (length %d, radius %d) does not fit the %dx%d TORUS map", length, radius, T.W, T.H);
+  T.end_min_frames = ip[MPB_FP_END_MIN_FRAMES]; T.end_interval = ip[MPB_FP_END_INTERVAL];
+  if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
+  return MP_OK;
+}
+
+}  // namespace

@@ -10,9 +10,50 @@
 // water) depending on the phase; envs never interact, so nothing leaves the warp.
 #pragma once
 
+#include "family_load.h"
 #include "step_common.cuh"
 
 struct CleanUp {
+  // Host: the clean_up tables of the blob (compiler.py _clean_up_tables): cu_ip / cu_dp, apples, dirt and water.
+  static int load(FamilyLoad& ld, Tables& T) {
+    const int32_t* ip;
+    const double* dp;
+    Section<int32_t> apple, dirt, water, water_sprites;
+    int rc;
+    if ((rc = ld.params("cu", MPB_CU_I_COUNT, MPB_CU_D_COUNT, &ip, &dp)) || (rc = ld.need("cu_apple", MPB_I32, &apple)) ||
+        (rc = ld.need("cu_dirt", MPB_I32, &dirt)) || (rc = ld.need("cu_water", MPB_I32, &water)) ||
+        (rc = ld.need("cu_water_sprites", MPB_I32, &water_sprites)))
+      return rc;
+    T.nA = ip[MPB_CU_I_N_APPLES]; T.nD = ip[MPB_CU_I_N_DIRT]; T.nW = ip[MPB_CU_I_N_WATER];
+    T.apple_layer = ip[MPB_CU_I_APPLE_LAYER]; T.apple_sprite = ip[MPB_CU_I_APPLE_SPRITE];
+    T.dirt_layer = ip[MPB_CU_I_DIRT_LAYER]; T.dirt_sprite = ip[MPB_CU_I_DIRT_SPRITE];
+    T.water_layer = ip[MPB_CU_I_WATER_LAYER]; T.n_anim = ip[MPB_CU_I_N_ANIM];
+    T.anim_frames = ip[MPB_CU_I_ANIM_FRAMES]; T.anim_random = ip[MPB_CU_I_ANIM_RANDOM];
+    if (T.n_anim < 1 || T.n_anim > 8 || T.anim_frames < 1) return fail(MP_E_UNSUPPORTED, "animation with %d states / %d frames", T.n_anim, T.anim_frames);
+    for (int i = 0; i < T.n_anim; ++i) T.water_sprite[i] = water_sprites.data[i];
+    if ((rc = load_zapper(ld, T, ip))) return rc;
+    T.clean_cooldown = ip[MPB_CU_I_CLEAN_COOLDOWN]; T.clean_layer = ip[MPB_CU_I_CLEAN_LAYER]; T.clean_sprite = ip[MPB_CU_I_CLEAN_SPRITE];
+    T.clean_hit = 1;
+    for (int h = 0; h < (int)ld.hits.count / 2; ++h) if (ld.hits.data[h * 2] == T.clean_layer) T.clean_hit = h;
+    const int length = ip[MPB_CU_I_CLEAN_LENGTH], radius = ip[MPB_CU_I_CLEAN_RADIUS];
+    if (T.clean_cooldown < 0) return fail(MP_E_UNSUPPORTED, "negative clean cooldown");
+    if (!make_beam_geom(length, radius, &T.clean_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (!beam_fits_torus(T, length, radius)) return fail(MP_E_UNSUPPORTED, "clean beam (length %d, radius %d) does not fit the %dx%d TORUS map", length, radius, T.W, T.H);
+    T.dirt_delay = ip[MPB_CU_I_DIRT_DELAY]; T.taste_role = ip[MPB_CU_I_TASTE_ROLE];
+    if (T.taste_role != 0) return fail(MP_E_UNSUPPORTED, "Taste roles other than 'free'");
+    T.grow_rate = dp[MPB_CU_D_GROW_RATE]; T.grow_depletion = dp[MPB_CU_D_GROW_DEPLETION];
+    T.grow_restoration = dp[MPB_CU_D_GROW_RESTORATION]; T.eat_reward = dp[MPB_CU_D_EAT_REWARD];
+    T.zap_penalty = dp[MPB_CU_D_ZAP_PENALTY]; T.zap_reward = dp[MPB_CU_D_ZAP_REWARD]; T.dirt_prob = dp[MPB_CU_D_DIRT_PROB];
+    T.end_prob = dp[MPB_CU_D_END_PROB]; T.taste_amount = dp[MPB_CU_D_TASTE_AMOUNT];
+    std::vector<int32_t> v_apple(apple.data, apple.data + apple.count), v_dirt(dirt.data, dirt.data + dirt.count);
+    std::vector<int32_t> v_water(water.data, water.data + water.count);
+    if ((rc = upload(ld.allocs, v_apple, &T.apple)) || (rc = upload(ld.allocs, v_dirt, &T.dirt)) || (rc = upload(ld.allocs, v_water, &T.water))) return rc;
+    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 3 + 1]);
+    T.dirt_count0 = 0;
+    for (int j = 0; j < T.nD; ++j) { ld.dirt_cells.push_back(v_dirt[j * 3 + 1]); T.dirt_count0 += v_dirt[j * 3 + 2]; }
+    return MP_OK;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

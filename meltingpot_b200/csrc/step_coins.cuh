@@ -10,9 +10,36 @@
 // (liveStateA / liveStateB, superOverlay). There are no beams and avatars never leave the map.
 #pragma once
 
+#include "family_load.h"
 #include "step_common.cuh"
 
 struct Coins {
+  // Host: the coins tables of the blob (compiler.py _coins_tables): co_ip / co_dp and the coins, which take the place
+  // of the apples (ch_apple, apple_of_cell, apple_layer).
+  static int load(FamilyLoad& ld, Tables& T) {
+    const int32_t* ip;
+    const double* dp;
+    Section<int32_t> coin;
+    int rc;
+    if ((rc = ld.params("co", MPB_CO_I_COUNT, MPB_CO_D_COUNT, &ip, &dp)) || (rc = ld.need("co_coin", MPB_I32, &coin))) return rc;
+    if (T.P != 2) return fail(MP_E_UNSUPPORTED, "coins needs exactly two players (got %d)", T.P);
+    T.nA = ip[MPB_CO_I_N_COINS]; T.apple_layer = ip[MPB_CO_I_COIN_LAYER];
+    T.coin_sprite[0] = ip[MPB_CO_I_COIN_SPRITE_0]; T.coin_sprite[1] = ip[MPB_CO_I_COIN_SPRITE_1];
+    T.coin_terminate = ip[MPB_CO_I_TERMINATE]; T.coin_terminate_n = ip[MPB_CO_I_TERMINATE_N];
+    T.end_min_frames = ip[MPB_CO_I_END_MIN_FRAMES]; T.end_interval = ip[MPB_CO_I_END_INTERVAL];
+    T.coin_type[0] = ip[MPB_CO_I_COIN_TYPE_0]; T.coin_type[1] = ip[MPB_CO_I_COIN_TYPE_1];
+    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d coins (max 2048)", T.nA);
+    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
+    T.coin_rate = dp[MPB_CO_D_REGROW_RATE]; T.end_prob = dp[MPB_CO_D_END_PROB];
+    for (int p = 0; p < 2; ++p) for (int k = 0; k < 4; ++k) T.coin_reward[p][k] = dp[MPB_CO_D_REWARD_0_SELF_MATCH + 4 * p + k];
+    T.zap_layer = 0; T.zap_cooldown = 1;
+    std::vector<int32_t> v_apple((size_t)T.nA * 4);  // ch_apple rows: obj id, cell, 0, -1
+    for (int k = 0; k < T.nA; ++k) { v_apple[k * 4] = coin.data[k * 2]; v_apple[k * 4 + 1] = coin.data[k * 2 + 1]; v_apple[k * 4 + 2] = 0; v_apple[k * 4 + 3] = -1; }
+    if ((rc = upload(ld.allocs, v_apple, &T.ch_apple))) return rc;
+    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 4 + 1]);
+    return MP_OK;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

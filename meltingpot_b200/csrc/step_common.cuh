@@ -53,9 +53,9 @@ __host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * 
 // mode 0: step (envs whose last step was LAST start a new episode instead, policy A.17)
 // mode 1: reset envs selected by `mask` (all if null)
 //
-// A Family provides: Scratch, kStagesTables, scratch_bytes(T) per warp, table_bytes(T) per CTA, stage(T, tables) (copies
-// static tables into shared memory), carve(T, warp_base, tables), reset(T, S, b, lane, sc) and
-// step(T, S, b, lane, actions, sc).
+// A Family provides: the host-side load(FamilyLoad&, T) that decodes its blob sections (family_load.h), Scratch,
+// kStagesTables, scratch_bytes(T) per warp, table_bytes(T) per CTA, stage(T, tables) (copies static tables into shared
+// memory), carve(T, warp_base, tables), reset(T, S, b, lane, sc) and step(T, S, b, lane, actions, sc).
 template <class Family>
 __global__ void __launch_bounds__(128, 8) k_step(Tables T, State S, const int32_t* __restrict__ actions,
                                                  const uint8_t* __restrict__ mask, int mode) {

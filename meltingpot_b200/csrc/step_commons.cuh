@@ -12,11 +12,38 @@
 // incremental (and order dependent) bookkeeping -- see _beginLive / _endLive below.
 #pragma once
 
+#include "family_load.h"
 #include "step_common.cuh"
 
 __device__ __forceinline__ bool ch_is_wait(uint8_t s) { return s != 0; }
 
 struct Commons {
+  // Host: the commons_harvest tables of the blob (compiler.py _commons_tables): ch_ip / ch_dp, apples and their
+  // regrowth-disc neighbours.
+  static int load(FamilyLoad& ld, Tables& T) {
+    const int32_t* ip;
+    const double* dp;
+    Section<int32_t> apple, nbr;
+    int rc;
+    if ((rc = ld.params("ch", MPB_CH_I_COUNT, MPB_CH_D_COUNT, &ip, &dp)) || (rc = ld.need("ch_apple", MPB_I32, &apple)) ||
+        (rc = ld.need("ch_nbr", MPB_I32, &nbr)))
+      return rc;
+    T.nA = ip[MPB_CH_I_N_APPLES]; T.apple_layer = ip[MPB_CH_I_APPLE_LAYER]; T.apple_sprite = ip[MPB_CH_I_APPLE_SPRITE];
+    T.wait_layer = ip[MPB_CH_I_WAIT_LAYER]; T.wait_sprite = ip[MPB_CH_I_WAIT_SPRITE];
+    T.ch_n_wait = ip[MPB_CH_I_N_WAIT]; T.ch_n_probs = ip[MPB_CH_I_N_PROBS]; T.grass_layer = ip[MPB_CH_I_GRASS_LAYER];
+    T.grass_sprite = ip[MPB_CH_I_GRASS_SPRITE]; T.dess_sprite = ip[MPB_CH_I_DESS_SPRITE];
+    if (T.ch_n_wait < 1 || T.ch_n_wait > 29 || T.ch_n_probs < 1 || T.ch_n_probs > 4) return fail(MP_E_UNSUPPORTED, "DensityRegrow with %d wait states / %d probabilities", T.ch_n_wait, T.ch_n_probs);
+    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d apples (max 2048)", T.nA);
+    if ((rc = load_zapper(ld, T, ip))) return rc;
+    for (int i = 0; i < 4; ++i) T.ch_probs[i] = dp[MPB_CH_D_PROB_0 + i];
+    T.eat_reward = dp[MPB_CH_D_EAT_REWARD]; T.zap_penalty = dp[MPB_CH_D_ZAP_PENALTY]; T.zap_reward = dp[MPB_CH_D_ZAP_REWARD];
+    T.end_prob = dp[MPB_CH_D_END_PROB];
+    std::vector<int32_t> v_apple(apple.data, apple.data + apple.count), v_nbr(nbr.data, nbr.data + nbr.count);
+    if ((rc = upload(ld.allocs, v_apple, &T.ch_apple)) || (rc = upload(ld.allocs, v_nbr, &T.ch_nbr))) return rc;
+    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 4 + 1]);
+    return MP_OK;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

@@ -19,9 +19,39 @@
 // land in the next round.
 #pragma once
 
+#include "family_load.h"
 #include "step_common.cuh"
 
 struct Mining {
+  // Host: the coop_mining tables of the blob (compiler.py _mining_tables): cm_ip / cm_dp and the ores, which take the
+  // place of the apples (ch_apple, apple_of_cell, apple_layer); the mine beam takes the place of the zapper (zap_*).
+  static int load(FamilyLoad& ld, Tables& T) {
+    const int32_t* ip;
+    const double* dp;
+    Section<int32_t> ore;
+    int rc;
+    if ((rc = ld.params("cm", MPB_CM_I_COUNT, MPB_CM_D_COUNT, &ip, &dp)) || (rc = ld.need("cm_ore", MPB_I32, &ore))) return rc;
+    T.nA = ip[MPB_CM_I_N_ORES]; T.apple_layer = ip[MPB_CM_I_ORE_LAYER];
+    for (int i = 0; i < 4; ++i) T.ore_sprite[i] = ip[MPB_CM_I_ORE_SPRITE_0 + i];
+    T.mine_window = ip[MPB_CM_I_MINE_WINDOW]; T.zap_cooldown = ip[MPB_CM_I_MINE_COOLDOWN]; T.mine_length = ip[MPB_CM_I_MINE_LENGTH];
+    T.zap_layer = ip[MPB_CM_I_MINE_LAYER]; T.zap_sprite = ip[MPB_CM_I_MINE_SPRITE];
+    T.end_min_frames = ip[MPB_CM_I_END_MIN_FRAMES]; T.end_interval = ip[MPB_CM_I_END_INTERVAL]; T.zap_hit = ip[MPB_CM_I_MINE_HIT];
+    if (T.P > 8) return fail(MP_E_UNSUPPORTED, "coop_mining with %d players (max 8: miners are kept as a bit mask)", T.P);
+    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d ores (max 2048)", T.nA);
+    if (T.zap_cooldown < 1 || T.mine_window < 1 || T.mine_window > 255 || T.mine_length < 1) return fail(MP_E_UNSUPPORTED, "MineBeam / Ore parameters out of range");
+    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
+    if (T.zap_hit < 0 || T.zap_hit > 7) return fail(MP_E_UNSUPPORTED, "mine hit id %d", T.zap_hit);
+    if (!beam_fits_torus(T, T.mine_length, 0)) return fail(MP_E_UNSUPPORTED, "mine beam (length %d) does not fit the %dx%d TORUS map", T.mine_length, T.W, T.H);
+    T.mine_rate[0] = dp[MPB_CM_D_RATE_0]; T.mine_rate[1] = dp[MPB_CM_D_RATE_1]; T.end_prob = dp[MPB_CM_D_END_PROB];
+    T.mine_reward[0] = dp[MPB_CM_D_MINE_REWARD_0]; T.mine_reward[1] = dp[MPB_CM_D_MINE_REWARD_1];
+    T.extract_reward[0] = dp[MPB_CM_D_EXTRACT_REWARD_0]; T.extract_reward[1] = dp[MPB_CM_D_EXTRACT_REWARD_1];
+    std::vector<int32_t> v_apple((size_t)T.nA * 4);  // ch_apple rows: obj id, cell, 0, -1
+    for (int k = 0; k < T.nA; ++k) { v_apple[k * 4] = ore.data[k * 2]; v_apple[k * 4 + 1] = ore.data[k * 2 + 1]; v_apple[k * 4 + 2] = 0; v_apple[k * 4 + 3] = -1; }
+    if ((rc = upload(ld.allocs, v_apple, &T.ch_apple))) return rc;
+    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 4 + 1]);
+    return MP_OK;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

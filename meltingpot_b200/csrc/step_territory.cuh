@@ -16,6 +16,7 @@
 // already fires during api:start's grid:update).
 #pragma once
 
+#include "family_load.h"
 #include "step_common.cuh"
 
 // Resource state codes: 0 unclaimed, 1 destroyed, 2 + i claimed_by_(i+1).
@@ -83,6 +84,73 @@ __device__ __forceinline__ uint16_t resource_sprite_value(const Tables& T, int s
 }
 
 struct Territory {
+  // Host: the territory tables of the blob (compiler.py _territory_tables): tr_ip / tr_dp, resources, per-player
+  // sprites, walls and the 'choice' conditions of the resources.
+  static int load(FamilyLoad& ld, Tables& T) {
+    const int32_t* ip;
+    const double* dp;
+    Section<int32_t> res, player_sprites;
+    Section<uint8_t> wall_sec;
+    int rc;
+    if ((rc = ld.params("tr", MPB_TR_I_COUNT, MPB_TR_D_COUNT, &ip, &dp)) || (rc = ld.need("tr_res", MPB_I32, &res)) ||
+        (rc = ld.need("tr_player_sprites", MPB_I32, &player_sprites)) || (rc = ld.need("tr_wall", MPB_U8, &wall_sec)))
+      return rc;
+    T.nR = ip[MPB_TR_I_N_RES]; T.nR_pad = round_up(std::max(T.nR, 64), 16);
+    T.res_layer = ip[MPB_TR_I_RES_LAYER]; T.unclaimed_sprite = ip[MPB_TR_I_UNCLAIMED_SPRITE];
+    T.tex_layer = ip[MPB_TR_I_TEX_LAYER]; T.tex_sprite = ip[MPB_TR_I_TEX_SPRITE]; T.ind_layer = ip[MPB_TR_I_IND_LAYER];
+    T.dmg_layer = ip[MPB_TR_I_DMG_LAYER]; T.dmg_sprite = ip[MPB_TR_I_DMG_SPRITE]; T.mark_layer = ip[MPB_TR_I_MARK_LAYER];
+    T.mark_initial_level = ip[MPB_TR_I_MARK_INITIAL_LEVEL]; T.mark_recovery = ip[MPB_TR_I_MARK_RECOVERY];
+    T.mark_n_levels = ip[MPB_TR_I_MARK_N_LEVELS];
+    if (T.res_layer != T.avatar_layer) return fail(MP_E_UNSUPPORTED, "territory: resources and avatars must share a layer");
+    if (T.mark_n_levels < 1 || T.mark_n_levels > 3) return fail(MP_E_UNSUPPORTED, "%d marking levels (1..3)", T.mark_n_levels);
+    if ((rc = load_zapper(ld, T, ip))) return rc;
+    if (T.zap_respawn <= T.max_frames) return fail(MP_E_UNSUPPORTED, "territory kernel assumes avatars never respawn (framesTillRespawn %d)", T.zap_respawn);
+    const int length = ip[MPB_TR_I_CLAIM_LENGTH], radius = ip[MPB_TR_I_CLAIM_RADIUS];
+    if (!make_beam_geom(length, radius, &T.claim_geom) || !make_beam_geom(1, 0, &T.brush_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (!beam_fits_torus(T, length, radius)) return fail(MP_E_UNSUPPORTED, "claim beam (length %d, radius %d) does not fit the %dx%d TORUS map", length, radius, T.W, T.H);
+    T.claim_wait = ip[MPB_TR_I_CLAIM_WAIT]; T.brush_layer = ip[MPB_TR_I_BRUSH_LAYER]; T.claim_layer = ip[MPB_TR_I_CLAIM_LAYER];
+    if (T.claim_layer != T.dmg_layer) return fail(MP_E_UNSUPPORTED, "territory: claim beam layer must be the damage indicator layer");
+    T.res_health0 = ip[MPB_TR_I_RES_HEALTH]; T.res_reward_delay = ip[MPB_TR_I_RES_REWARD_DELAY];
+    T.res_repair_delay = ip[MPB_TR_I_RES_REPAIR_DELAY]; T.tr_taste_role = ip[MPB_TR_I_TASTE_ROLE];
+    if (T.tr_taste_role != 0) return fail(MP_E_UNSUPPORTED, "territory Taste roles other than 'none'");
+    if (T.res_health0 < 1 || T.res_health0 > 200) return fail(MP_E_UNSUPPORTED, "resource health %d", T.res_health0);
+    // the resource age and frames-since-zapped counters saturate at 65535 (see RS_AGE)
+    if (T.res_reward_delay > 65535 || T.res_repair_delay > 65535)
+      return fail(MP_E_UNSUPPORTED, "rewardDelay %d / delayTillSelfRepair %d (max 65535)", T.res_reward_delay, T.res_repair_delay);
+    const int istride = MPB_TR_I_MARK_INC_1 - MPB_TR_I_MARK_INC_0, dstride = MPB_TR_D_MARK_SRC_REWARD_1 - MPB_TR_D_MARK_SRC_REWARD_0;
+    for (int l = 0; l < T.mark_n_levels; ++l) {
+      const int32_t* li = ip + istride * l;
+      const double* dl = dp + dstride * l;
+      T.mark_inc[l] = li[MPB_TR_I_MARK_INC_0]; T.mark_remove[l] = li[MPB_TR_I_MARK_REMOVE_0];
+      T.mark_freeze[l] = li[MPB_TR_I_MARK_FREEZE_0]; T.mark_sprite[l] = li[MPB_TR_I_MARK_SPRITE_0];
+      T.mark_src_reward[l] = dl[MPB_TR_D_MARK_SRC_REWARD_0]; T.mark_tgt_reward[l] = dl[MPB_TR_D_MARK_TGT_REWARD_0];
+    }
+    T.res_reward = dp[MPB_TR_D_RES_REWARD]; T.res_rate = dp[MPB_TR_D_RES_RATE]; T.res_repair_prob = dp[MPB_TR_D_RES_REPAIR_PROB];
+    T.zap_penalty = dp[MPB_TR_D_ZAP_PENALTY]; T.zap_reward = dp[MPB_TR_D_ZAP_REWARD]; T.end_prob = dp[MPB_TR_D_END_PROB];
+    T.tr_taste_amount = dp[MPB_TR_D_TASTE_AMOUNT]; T.tr_taste_mult = dp[MPB_TR_D_TASTE_MULT];
+    for (int p = 0; p < T.P; ++p) {
+      const int32_t* ps = player_sprites.data + p * 4;
+      T.claimed_sprite[p] = ps[0]; T.dry_sprite[p] = ps[1]; T.brush_sprite[p] = ps[2]; T.claimbeam_sprite[p] = ps[3];
+    }
+    for (int p = 0; p < T.P; ++p) {  // wet paint on the resource texture, then dry paint on top: what most resource cells show
+      ld.hint_stacks.push_back({T.tex_sprite, T.claimed_sprite[p]});
+      ld.hint_stacks.push_back({T.tex_sprite, T.claimed_sprite[p], T.dry_sprite[p]});
+    }
+    std::vector<int32_t> v_res(res.data, res.data + res.count);
+    std::vector<int16_t> res_of(T.cells_pad, -1);
+    for (int k = 0; k < T.nR; ++k) res_of[v_res[k * 3 + 1]] = (int16_t)k;
+    std::vector<uint8_t> wall(T.cells_pad, 0);
+    memcpy(wall.data(), wall_sec.data, std::min<size_t>(wall_sec.count, T.cells));
+    if ((rc = upload(ld.allocs, v_res, &T.tr_res)) || (rc = upload(ld.allocs, res_of, &T.res_of_cell)) || (rc = upload(ld.allocs, wall, &T.wall))) return rc;
+    Section<int32_t> res_cond;
+    if (get_section(ld.blob, ld.n, "tr_res_cond", MPB_I32, &res_cond)) {
+      if ((int)res_cond.count != T.nR * 2) return fail(MP_E_INVALID, "blob: tr_res_cond has %zu values for %d resources", res_cond.count, T.nR);
+      std::vector<int32_t> v(res_cond.data, res_cond.data + res_cond.count);
+      if ((rc = upload(ld.allocs, v, &T.tr_res_cond))) return rc;
+    }
+    return MP_OK;
+  }
+
   using Scratch = TerritoryScratch;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return territory_scratch_bytes(T); }

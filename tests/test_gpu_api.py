@@ -64,9 +64,9 @@ def _masked_reset(blob, name, oracle):
   st = eng.step_type.cpu().numpy()
   assert (st[mask == 1] == 0).all() and (st[mask == 0] == 1).all()  # FIRST only where reset
   if name == 'territory__inside_out':
-    from meltingpot_b200 import blob as blob_lib
+    from meltingpot_b200 import blob as blob_lib, compiler
     sec = blob_lib.unpack(blob)
-    cells, res_layer = sec['tr_res'][:, 1].astype(np.int64), int(sec['tr_ip'][1])
+    cells, res_layer = sec['tr_res'][:, 1].astype(np.int64), compiler.family_params(sec)['RES_LAYER']
     layout = lambda g: g[:, res_layer][:, cells] != 0
     before, after = layout(grid_before), layout(eng.grid.cpu().numpy())
     for b in range(B):  # masked envs redraw their resource layout, the others keep theirs

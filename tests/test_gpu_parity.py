@@ -230,10 +230,10 @@ def test_config5_sweep_at_2048_envs(name, players, oracle):
 def test_inside_out_envs_of_one_batch_have_their_own_layouts(territory_inside_out_blob):
   # Deviation A.20 is gone for 'choice' prefabs: every env (and episode) draws its own resources / spawn points.
   import torch
-  from meltingpot_b200 import blob as blob_lib, engine
+  from meltingpot_b200 import blob as blob_lib, compiler, engine
   sec = blob_lib.unpack(territory_inside_out_blob)
   cells = torch.as_tensor(sec['tr_res'][:, 1].astype(np.int64), device='cuda')
-  res_layer = int(sec['tr_ip'][1])
+  res_layer = compiler.family_params(sec)['RES_LAYER']
   eng = engine.Engine(territory_inside_out_blob, 256, seed=3)
   eng.reset()
   torch.cuda.synchronize()

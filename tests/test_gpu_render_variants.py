@@ -223,10 +223,10 @@ def _episode_ends(blob):
 
 def _resource_layout(blob):
   import torch
-  from meltingpot_b200 import blob as blob_lib
+  from meltingpot_b200 import blob as blob_lib, compiler
   sec = blob_lib.unpack(blob)
   cells = torch.as_tensor(sec['tr_res'][:, 1].astype(np.int64), device='cuda')
-  res_layer = int(sec['tr_ip'][1])
+  res_layer = compiler.family_params(sec)['RES_LAYER']
   return lambda eng: (eng.grid[:, res_layer][:, cells] != 0).cpu().numpy()
 
 

@@ -5,6 +5,7 @@ import json
 import numpy as np
 
 from meltingpot_b200 import blob as mpb
+from meltingpot_b200 import compiler
 from meltingpot_b200 import substrates
 from tests import settings_golden
 
@@ -21,22 +22,23 @@ def test_layout_and_specs(coins_blob):
   assert info['world_rgb_shape'] == [136, 136, 3]           # padded to the maximum map (coins.py:45-84, timestep_spec)
   assert info['individual_observation_names'] == ['RGB', 'MISMATCHED_COIN_COLLECTED_BY_PARTNER']
   assert len(info['action_set']) == 7                       # no zapping in coins
-  ip, dp = sec['co_ip'], sec['co_dp']
-  assert sorted(int(t) for t in ip[8:10]) == [0, 1]         # the two players own different coin types
-  assert list(dp[4:8]) == [1.0, 1.0, 0.0, -2.0]             # self match, self mismatch, other match, other mismatch
+  params = compiler.family_params(sec)
+  assert sorted((params['COIN_TYPE_0'], params['COIN_TYPE_1'])) == [0, 1]  # the two players own different coin types
+  # player 1's self match, self mismatch, other match, other mismatch
+  assert [params[f'REWARD_0_{r}'] for r in ('SELF_MATCH', 'SELF_MISMATCH', 'OTHER_MATCH', 'OTHER_MISMATCH')] == [1.0, 1.0, 0.0, -2.0]
 
 
 def test_build_seed_fixes_the_python_side_randomness():
   a = settings_golden.compile('coins', 2, 3)
   assert a == settings_golden.compile('coins', 2, 3)
-  shapes = {tuple(int(v) for v in mpb.unpack(settings_golden.compile('coins', 2, s))['co_ip'][:1]) for s in range(6)}
+  shapes = {compiler.family_params(mpb.unpack(settings_golden.compile('coins', 2, s)))['N_COINS'] for s in range(6)}
   assert len(shapes) > 1  # different seeds draw different map sizes (coin counts)
   assert settings_golden.compile('coins', 2, substrates.BUILD_SEEDS['coins']) == substrates.load_blob('coins', ('default',) * 2)
 
 
 def test_coins_appear_are_collected_and_pay_by_type(oracle, coins_blob):
   sec, info = _tables(coins_blob)
-  types = [int(t) for t in sec['co_ip'][8:10]]
+  types = [compiler.family_params(sec)[f'COIN_TYPE_{p}'] for p in range(2)]
   coin_kind = info['kinds'].index('coin')
   names = info['kind_states'][coin_kind]
   env = oracle.OracleEnv(coins_blob, 7)

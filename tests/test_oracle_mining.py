@@ -5,6 +5,7 @@ import json
 import numpy as np
 
 from meltingpot_b200 import blob as mpb
+from meltingpot_b200 import compiler
 
 
 def _tables(blob):
@@ -33,7 +34,8 @@ def test_layout(coop_mining_blob):
   assert int(meta[0]) == 5 and int(meta[4]) == 6 and (int(meta[1]), int(meta[2])) == (27, 27)
   assert info['hits'] == ['mine'] and info['layers'][-1] == 'beamMine'   # MineBeam:addHits (:191-197)
   assert info['individual_observation_names'] == ['RGB', 'READY_TO_SHOOT']
-  assert list(sec['cm_dp'][4:8]) == [0.0, 0.0, 1.0, 8.0]                  # role 'none': mining pays 0, extracting 1 / 8
+  params = compiler.family_params(sec)
+  assert [params[k] for k in ('MINE_REWARD_0', 'MINE_REWARD_1', 'EXTRACT_REWARD_0', 'EXTRACT_REWARD_1')] == [0.0, 0.0, 1.0, 8.0]  # role 'none': mining pays 0, extracting 1 / 8
 
 
 def test_iron_is_extracted_by_one_miner_and_the_beam_cools_down(oracle, coop_mining_blob):

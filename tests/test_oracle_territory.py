@@ -7,6 +7,7 @@ import json
 import numpy as np
 
 from meltingpot_b200 import blob as blob_lib
+from meltingpot_b200 import compiler
 
 NOOP, FORWARD, BACKWARD, STEP_LEFT, STEP_RIGHT, TURN_LEFT, TURN_RIGHT, ZAP, CLAIM = range(9)
 N, E, S, W = range(4)
@@ -197,7 +198,7 @@ def test_inside_out_choice_prefabs_are_drawn_per_env_and_per_episode(territory_i
     e = oracle.OracleEnv(territory_inside_out_blob, 100 + seed)
     e.reset()
     g = e.grid()
-    res_layer = int(sec['tr_ip'][1])
+    res_layer = compiler.family_params(sec)['RES_LAYER']
     layouts.append(g[res_layer].copy())
     unclaimed = g[res_layer][0 * 0 + sec['tr_res'][:, 1]] == g[res_layer][int(sec['tr_res'][np.argmax(cond[:, 0] < 0), 1])]
     counts.append(int(unclaimed.sum()))  # resource cells that show the 'unclaimed' resource sprite

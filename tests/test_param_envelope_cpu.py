@@ -9,6 +9,7 @@ reference's Lua states are pinned with citations, as in test_oracle_semantics.py
 import numpy as np
 import pytest
 
+from meltingpot_b200 import compiler
 from tests import variants as V
 
 ENV_SEED = 7
@@ -24,60 +25,66 @@ def _differs_from_stock(variant, sec):
   return any(k not in stock or stock[k].shape != v.shape or not np.array_equal(stock[k], v) for k, v in mine.items())
 
 
-# Decoded family fields for the variants whose knob has a slot of its own (compiler.py _*_tables).
+def _has(**want):
+  """The blob's family parameters (compiler.family_params) include `want`."""
+  return lambda s: all(compiler.family_params(s)[k] == v for k, v in want.items())
+
+
+# Decoded family fields for the variants whose knob has a slot of its own (include/mpb_format.h).
 CARRIES = {
-    'clean_up/zap_cooldown_1': lambda s: s['cu_ip'][12] == 1,
-    'clean_up/zap_lateral_28': lambda s: tuple(s['cu_ip'][13:15]) == (6, 2),
-    'clean_up/zap_line_32': lambda s: tuple(s['cu_ip'][13:15]) == (32, 0),
-    'clean_up/respawn_1': lambda s: s['cu_ip'][15] == 1,
-    'clean_up/keep_hit_player': lambda s: s['cu_ip'][16] == 0,
-    'clean_up/non_dyadic_rewards': lambda s: (s['cu_dp'][3], s['cu_dp'][4], s['cu_dp'][5]) == (0.1, 0.3, 0.7),
-    'clean_up/clean_cooldown_0': lambda s: s['cu_ip'][18] == 0,
-    'clean_up/clean_line_32': lambda s: tuple(s['cu_ip'][19:21]) == (32, 0),
-    'clean_up/dirt_fills_river': lambda s: s['cu_ip'][25] == 0 and s['cu_dp'][6] == 1.0,
-    'clean_up/apple_growth_rate_1': lambda s: s['cu_dp'][0] == 1.0,
-    'clean_up/apple_thresholds_equal': lambda s: s['cu_dp'][1] == s['cu_dp'][2] == 0.0,
-    'clean_up/animation_every_frame_random_start_True': lambda s: tuple(s['cu_ip'][10:12]) == (1, 1),
-    'clean_up/animation_every_frame_random_start_False': lambda s: tuple(s['cu_ip'][10:12]) == (1, 0),
-    'commons_harvest/zap_line_32': lambda s: tuple(s['ch_ip'][13:15]) == (32, 0),
-    'commons_harvest/zap_lateral_28': lambda s: tuple(s['ch_ip'][13:15]) == (6, 2),
-    'commons_harvest/respawn_1': lambda s: s['ch_ip'][15] == 1,
-    'commons_harvest/keep_hit_player': lambda s: s['ch_ip'][16] == 0,
-    'commons_harvest/non_dyadic_rewards': lambda s: (s['ch_dp'][4], s['ch_dp'][5], s['ch_dp'][6]) == (0.1, 0.3, 0.7),
-    'commons/regrow_always': lambda s: list(s['ch_dp'][:4]) == [1.0] * 4,
-    'commons/regrow_never': lambda s: list(s['ch_dp'][:4]) == [0.0] * 4,
-    'commons/radius_1': lambda s: s['ch_ip'][5] == 5,
-    'commons/radius_2_98': lambda s: s['ch_ip'][5] == 29 and (s['ch_nbr'] >= 0).sum(axis=1).max() >= 12,
-    'territory/zap_lateral_28': lambda s: tuple(s['tr_ip'][13:15]) == (6, 2),
-    'territory/health_1': lambda s: s['tr_ip'][28] == 1,
-    'territory/health_200': lambda s: s['tr_ip'][28] == 200,
-    'territory/fast_rewards': lambda s: tuple(s['tr_ip'][29:31]) == (0, 0) and tuple(s['tr_dp'][:3]) == (0.3, 1.0, 1.0),
-    'territory/reward_delay_65535': lambda s: s['tr_ip'][29] == 65535,
-    'territory/claim_wait_5': lambda s: s['tr_ip'][20] == 5,
-    'territory/open_beams_32': lambda s: tuple(s['tr_ip'][13:15]) == (32, 0) and tuple(s['tr_ip'][18:20]) == (32, 0),
-    'territory/rooms_zap_20': lambda s: tuple(s['tr_ip'][13:15]) == (20, 0),
-    'territory/rooms_zap_radius_10': lambda s: tuple(s['tr_ip'][13:15]) == (1, 10),
-    'territory/sanctions_1_level': lambda s: s['tr_ip'][11] == 1 and s['tr_ip'][10] == 1 and s['tr_ip'][34] == 2,
-    'territory/sanctions_3_levels': lambda s: s['tr_ip'][11] == 3 and s['tr_ip'][41] == 1 and s['tr_ip'][42] == 0,
-    'territory/sanctions_recovery_1': lambda s: s['tr_ip'][10] == 1,
-    'coins/regrow_rate_1': lambda s: s['co_dp'][0] == 1.0,
-    'coins/terminate_at_3': lambda s: tuple(s['co_ip'][4:6]) == (1, 3),
-    'coins/non_dyadic_rewards': lambda s: abs(s['co_dp'][4] - 0.3 * 1.1) < 1e-15 and abs(s['co_dp'][6] + 0.1 * 3.0) < 1e-15,
-    'coop_mining/live_rates_1': lambda s: tuple(s['cm_dp'][:2]) == (1.0, 1.0),
-    'coop_mining/mining_window_1': lambda s: s['cm_ip'][6] == 1,
-    'coop_mining/mining_window_255': lambda s: s['cm_ip'][6] == 255,
-    'coop_mining/mine_cooldown_1': lambda s: s['cm_ip'][7] == 1,
-    'coop_mining/mine_line_32': lambda s: s['cm_ip'][8] == 32,
+    'clean_up/zap_cooldown_1': _has(ZAP_COOLDOWN=1),
+    'clean_up/zap_lateral_28': _has(ZAP_LENGTH=6, ZAP_RADIUS=2),
+    'clean_up/zap_line_32': _has(ZAP_LENGTH=32, ZAP_RADIUS=0),
+    'clean_up/respawn_1': _has(ZAP_RESPAWN=1),
+    'clean_up/keep_hit_player': _has(ZAP_REMOVE=0),
+    'clean_up/non_dyadic_rewards': _has(EAT_REWARD=0.1, ZAP_PENALTY=0.3, ZAP_REWARD=0.7),
+    'clean_up/clean_cooldown_0': _has(CLEAN_COOLDOWN=0),
+    'clean_up/clean_line_32': _has(CLEAN_LENGTH=32, CLEAN_RADIUS=0),
+    'clean_up/dirt_fills_river': _has(DIRT_DELAY=0, DIRT_PROB=1.0),
+    'clean_up/apple_growth_rate_1': _has(GROW_RATE=1.0),
+    'clean_up/apple_thresholds_equal': _has(GROW_DEPLETION=0.0, GROW_RESTORATION=0.0),
+    'clean_up/animation_every_frame_random_start_True': _has(ANIM_FRAMES=1, ANIM_RANDOM=1),
+    'clean_up/animation_every_frame_random_start_False': _has(ANIM_FRAMES=1, ANIM_RANDOM=0),
+    'commons_harvest/zap_line_32': _has(ZAP_LENGTH=32, ZAP_RADIUS=0),
+    'commons_harvest/zap_lateral_28': _has(ZAP_LENGTH=6, ZAP_RADIUS=2),
+    'commons_harvest/respawn_1': _has(ZAP_RESPAWN=1),
+    'commons_harvest/keep_hit_player': _has(ZAP_REMOVE=0),
+    'commons_harvest/non_dyadic_rewards': _has(EAT_REWARD=0.1, ZAP_PENALTY=0.3, ZAP_REWARD=0.7),
+    'commons/regrow_always': _has(PROB_0=1.0, PROB_1=1.0, PROB_2=1.0, PROB_3=1.0),
+    'commons/regrow_never': _has(PROB_0=0.0, PROB_1=0.0, PROB_2=0.0, PROB_3=0.0),
+    'commons/radius_1': _has(N_WAIT=5),
+    'commons/radius_2_98': lambda s: _has(N_WAIT=29)(s) and (s['ch_nbr'] >= 0).sum(axis=1).max() >= 12,
+    'territory/zap_lateral_28': _has(ZAP_LENGTH=6, ZAP_RADIUS=2),
+    'territory/health_1': _has(RES_HEALTH=1),
+    'territory/health_200': _has(RES_HEALTH=200),
+    'territory/fast_rewards': _has(RES_REWARD_DELAY=0, RES_REPAIR_DELAY=0, RES_REWARD=0.3, RES_RATE=1.0, RES_REPAIR_PROB=1.0),
+    'territory/reward_delay_65535': _has(RES_REWARD_DELAY=65535),
+    'territory/claim_wait_5': _has(CLAIM_WAIT=5),
+    'territory/open_beams_32': _has(ZAP_LENGTH=32, ZAP_RADIUS=0, CLAIM_LENGTH=32, CLAIM_RADIUS=0),
+    'territory/rooms_zap_20': _has(ZAP_LENGTH=20, ZAP_RADIUS=0),
+    'territory/rooms_zap_radius_10': _has(ZAP_LENGTH=1, ZAP_RADIUS=10),
+    'territory/sanctions_1_level': _has(MARK_N_LEVELS=1, MARK_RECOVERY=1, MARK_FREEZE_0=2),
+    'territory/sanctions_3_levels': _has(MARK_N_LEVELS=3, MARK_REMOVE_2=1, MARK_FREEZE_2=0),
+    'territory/sanctions_recovery_1': _has(MARK_RECOVERY=1),
+    'coins/regrow_rate_1': _has(REGROW_RATE=1.0),
+    'coins/terminate_at_3': _has(TERMINATE=1, TERMINATE_N=3),
+    'coins/non_dyadic_rewards': lambda s: (abs(compiler.family_params(s)['REWARD_0_SELF_MATCH'] - 0.3 * 1.1) < 1e-15 and
+                                           abs(compiler.family_params(s)['REWARD_0_OTHER_MATCH'] + 0.1 * 3.0) < 1e-15),
+    'coop_mining/live_rates_1': _has(RATE_0=1.0, RATE_1=1.0),
+    'coop_mining/mining_window_1': _has(MINE_WINDOW=1),
+    'coop_mining/mining_window_255': _has(MINE_WINDOW=255),
+    'coop_mining/mine_cooldown_1': _has(MINE_COOLDOWN=1),
+    'coop_mining/mine_line_32': _has(MINE_LENGTH=32),
 }
-for _fam, _ip in (('clean_up', 'cu_ip'), ('commons_harvest', 'ch_ip'), ('territory', 'tr_ip')):
-  CARRIES.setdefault(f'{_fam}/zap_cooldown_1', lambda s, _ip=_ip: s[_ip][12] == 1)
+for _fam in ('clean_up', 'commons_harvest', 'territory'):
+  CARRIES.setdefault(f'{_fam}/zap_cooldown_1', _has(ZAP_COOLDOWN=1))
 for _v in V.PARITY:
   if '/end_every_frame' in _v.name:
     CARRIES[_v.name] = lambda s: True  # StochasticIntervalEpisodeEnding lives in the comps tables (checked below)
   if '/hard_cap_' in _v.name:
-    CARRIES[_v.name] = lambda s, cap=int(_v.name.rsplit('_', 1)[1]): s['meta'][7] == cap
+    CARRIES[_v.name] = lambda s, cap=int(_v.name.rsplit('_', 1)[1]): s['meta'][compiler.META['MAX_FRAMES']] == cap
   if '/view_' in _v.name:
-    CARRIES[_v.name] = lambda s: True  # the view window is checked by the reach predicate (meta 15..18)
+    CARRIES[_v.name] = lambda s: True  # the view window is checked by the reach predicate (meta VIEW_*)
 
 
 def test_every_parity_variant_has_a_decoded_check():
@@ -144,7 +151,8 @@ def test_hard_cap_ends_the_episode_on_its_last_frame(oracle):
 
 
 def _coin_sprites(sec):
-  return int(sec['co_ip'][2]), int(sec['co_ip'][3])
+  params = compiler.family_params(sec)
+  return params['COIN_SPRITE_0'], params['COIN_SPRITE_1']
 
 
 def test_coin_regrow_rate_1_regrows_every_waiting_coin_on_the_next_frame(oracle):
@@ -152,7 +160,7 @@ def test_coin_regrow_rate_1_regrows_every_waiting_coin_on_the_next_frame(oracle)
   # at 1.0 it fires on the first frame a coin spends waiting, so a coin collected on one step is back on the next.
   blob = V.compile('coins/regrow_rate_1')
   sec = V.sections(blob)
-  n_coins = int(sec['co_ip'][0])
+  n_coins = compiler.family_params(sec)['N_COINS']
   env = oracle.OracleEnv(blob, ENV_SEED)
   env.reset()
   rng = np.random.default_rng(3)
@@ -198,7 +206,7 @@ def test_apple_growth_with_equal_thresholds_is_nan_and_grows_nothing(oracle):
   # argument wins unless another is smaller), and random:uniform() < NaN is false: no apple grows (policy A.22). With a
   # clean river and no dirt spawning the fraction is 0 on every frame.
   stats, sec = _rollout(V.compile('clean_up/apple_thresholds_equal'), oracle, 8, 200)
-  assert stats['sprite_max'][int(sec['cu_ip'][4])] == 0
+  assert stats['sprite_max'][compiler.family_params(sec)['APPLE_SPRITE']] == 0
   # with the shipped thresholds (depletion 0.4, restoration 0) the same clean river grows apples at the full rate
   stats, sec = _rollout(V.compile('clean_up/apple_growth_rate_1'), oracle, 8, 200)
-  assert stats['sprite_grew'][int(sec['cu_ip'][4])] > 0
+  assert stats['sprite_grew'][compiler.family_params(sec)['APPLE_SPRITE']] > 0

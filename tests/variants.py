@@ -27,6 +27,7 @@ import types
 
 import numpy as np
 
+from meltingpot_b200 import compiler
 from tests import settings_golden
 
 # ---- settings overrides -----------------------------------------------------------------------------------------------
@@ -214,12 +215,17 @@ def _cap_pattern(cap):
   return reach
 
 
-def _grew(ip_name, ip_index):
-  return lambda s, sec: s['sprite_grew'][int(sec[ip_name][ip_index])] > 0
+def _param(sec, name):
+  """Family parameter `name` (a slot of include/mpb_format.h) of a blob's decoded sections."""
+  return compiler.family_params(sec)[name]
 
 
-def _never_grew(ip_name, ip_index):
-  return lambda s, sec: s['sprite_grew'][int(sec[ip_name][ip_index])] == 0 and s['sprite_fell'][int(sec[ip_name][ip_index])] > 0
+def _grew(sprite_param):
+  return lambda s, sec: s['sprite_grew'][_param(sec, sprite_param)] > 0
+
+
+def _never_grew(sprite_param):
+  return lambda s, sec: s['sprite_grew'][_param(sec, sprite_param)] == 0 and s['sprite_fell'][_param(sec, sprite_param)] > 0
 
 
 def _variants():
@@ -263,18 +269,18 @@ def _variants():
   add('clean_up/clean_line_32', 'clean_up', 7, None, [kw('Cleaner', beamLength=32, beamRadius=0)], 'parity',
       reach=lambda s, sec: EV(s, 'player_cleaned') > 0)
   add('clean_up/dirt_fills_river', 'clean_up', 7, None, [kw('DirtSpawner', dirtSpawnProbability=1.0, delayStartOfDirtSpawning=0)],
-      'parity', reach=lambda s, sec: s['sprite_max'][int(sec['cu_ip'][6])] == int(sec['cu_ip'][1]))
+      'parity', reach=lambda s, sec: s['sprite_max'][_param(sec, 'DIRT_SPRITE')] == _param(sec, 'N_DIRT'))
   add('clean_up/apple_growth_rate_1', 'clean_up', 7, None, [river, kw('AppleGrow', maxAppleGrowthRate=1.0)], 'parity',
-      reach=lambda s, sec: EV(s, 'edible_consumed') > 0 and _grew('cu_ip', 4)(s, sec))
+      reach=lambda s, sec: EV(s, 'edible_consumed') > 0 and _grew('APPLE_SPRITE')(s, sec))
   add('clean_up/apple_thresholds_equal', 'clean_up', 7, None,
       [river, kw('AppleGrow', thresholdDepletion=0.0, thresholdRestoration=0.0, maxAppleGrowthRate=1.0),
        kw('DirtSpawner', dirtSpawnProbability=0.0)], 'parity',
       # the river stays clean, so the dirt fraction equals both thresholds on every frame: 0/0, and no apple ever grows
-      reach=lambda s, sec: s['sprite_max'][int(sec['cu_ip'][6])] == 0 and s['sprite_max'][int(sec['cu_ip'][4])] == 0)
+      reach=lambda s, sec: s['sprite_max'][_param(sec, 'DIRT_SPRITE')] == 0 and s['sprite_max'][_param(sec, 'APPLE_SPRITE')] == 0)
   for rnd in (True, False):
     add(f'clean_up/animation_every_frame_random_start_{rnd}', 'clean_up', 7, None,
         [kw('Animation', gameFramesPerAnimationFrame=1, randomStartFrame=rnd)], 'parity', steps=60,
-        probe=lambda sec: [int(x) for x in sec['cu_water_sprites'][:int(sec['cu_ip'][9])]],
+        probe=lambda sec: [int(x) for x in sec['cu_water_sprites'][:_param(sec, 'N_ANIM')]],
         reach=(lambda s, sec: len(s['sprites_seen']) > 2 and all(a != b for a, b in zip(s['sprites_seen'], s['sprites_seen'][1:]))
                and sum(1 for n in s['sprites_seen'][0] if n) > 1) if rnd else
               (lambda s, sec: len(s['sprites_seen']) > 2 and all(sum(1 for n in c if n) == 1 for c in s['sprites_seen'])
@@ -282,14 +288,14 @@ def _variants():
   # ---- commons_harvest
   ch = 'commons_harvest__open'
   add('commons/regrow_always', ch, 7, None, [kw('DensityRegrow', regrowthProbabilities=[1.0, 1.0, 1.0, 1.0])], 'parity',
-      reach=lambda s, sec: EV(s, 'edible_consumed') > 0 and _grew('ch_ip', 2)(s, sec))
+      reach=lambda s, sec: EV(s, 'edible_consumed') > 0 and _grew('APPLE_SPRITE')(s, sec))
   add('commons/regrow_never', ch, 7, None, [kw('DensityRegrow', regrowthProbabilities=[0.0, 0.0, 0.0, 0.0])], 'parity',
-      reach=lambda s, sec: EV(s, 'edible_consumed') > 0 and _never_grew('ch_ip', 2)(s, sec))
+      reach=lambda s, sec: EV(s, 'edible_consumed') > 0 and _never_grew('APPLE_SPRITE')(s, sec))
   grow = kw('DensityRegrow', regrowthProbabilities=[0.0, 0.2, 0.4, 0.8])
   add('commons/radius_1', ch, 7, None, [density_radius(1.0), grow], 'parity',
-      reach=lambda s, sec: int(sec['ch_ip'][5]) == 5 and EV(s, 'edible_consumed') > 0 and _grew('ch_ip', 2)(s, sec))
+      reach=lambda s, sec: _param(sec, 'N_WAIT') == 5 and EV(s, 'edible_consumed') > 0 and _grew('APPLE_SPRITE')(s, sec))
   add('commons/radius_2_98', ch, 7, None, [density_radius(2.98), grow], 'parity',
-      reach=lambda s, sec: int(sec['ch_ip'][5]) == 29 and EV(s, 'edible_consumed') > 0 and _grew('ch_ip', 2)(s, sec))
+      reach=lambda s, sec: _param(sec, 'N_WAIT') == 29 and EV(s, 'edible_consumed') > 0 and _grew('APPLE_SPRITE')(s, sec))
   add('commons/radius_3', ch, 7, None, [density_radius(3.0)], 'refused', 'engine')
   # a 5x5 block of apples: the radius-2.98 disc around its centre holds 24 other apples
   add('commons/dense_disc', ch, 7, None, [density_radius(2.98), map_rows(lambda rows: [
@@ -299,7 +305,7 @@ def _variants():
   add('territory/health_1', tr, 9, None, [kw('Resource', initialHealth=1)], 'parity',
       reach=lambda s, sec: EV(s, 'destroyed_resource') > 0)
   add('territory/health_200', tr, 9, None, [kw('Resource', initialHealth=200)], 'parity',
-      reach=lambda s, sec: EV(s, 'destroyed_resource') == 0 and s['sprite_max'][int(sec['tr_ip'][7])] > 0)
+      reach=lambda s, sec: EV(s, 'destroyed_resource') == 0 and s['sprite_max'][_param(sec, 'DMG_SPRITE')] > 0)
   add('territory/health_201', tr, 9, None, [kw('Resource', initialHealth=201)], 'refused', 'engine')
   add('territory/fast_rewards', tr, 9, None,
       [kw('Resource', rewardDelay=0, delayTillSelfRepair=0, selfRepairProbability=1.0, rewardRate=1.0, reward=0.3)], 'parity',
@@ -323,11 +329,11 @@ def _variants():
   add('territory/rooms_zap_25', tr, 9, None, [kw('Zapper', beamLength=25, beamRadius=0)], 'refused', 'engine')
   add('territory/sanctions_1_level', tr, 9, None,
       [marking_levels([dict(levelIncrement=0, sourceReward=0.25, targetReward=-0.5, freeze=2)], 1), kw('Zapper', cooldownTime=1)],
-      'parity', reach=lambda s, sec: int(sec['tr_ip'][11]) == 1 and EV(s, 'sanctioning') > 0 and _nondyadic(s))
+      'parity', reach=lambda s, sec: _param(sec, 'MARK_N_LEVELS') == 1 and EV(s, 'sanctioning') > 0 and _nondyadic(s))
   add('territory/sanctions_3_levels', tr, 9, None,
       [marking_levels([dict(levelIncrement=1, freeze=2), dict(levelIncrement=1, freeze=3, sourceReward=0.7),
                        dict(levelIncrement=-2, remove=True, targetReward=-0.3)], 50), kw('Zapper', cooldownTime=1)],
-      'parity', reach=lambda s, sec: int(sec['tr_ip'][11]) == 3 and EV(s, 'removal_due_to_sanctioning') > 0 and _nondyadic(s))
+      'parity', reach=lambda s, sec: _param(sec, 'MARK_N_LEVELS') == 3 and EV(s, 'removal_due_to_sanctioning') > 0 and _nondyadic(s))
   # the shipped two levels, back to level 1 one frame after a hit: a removal needs two hits on consecutive frames
   add('territory/sanctions_recovery_1', tr, 9, None, [kw('GraduatedSanctionsMarking', recoveryTime=1), kw('Zapper', cooldownTime=1)],
       'parity', reach=lambda s, sec: EV(s, 'sanctioning') > 0 and 20 * EV(s, 'removal_due_to_sanctioning') <= EV(s, 'sanctioning'))
@@ -349,7 +355,7 @@ def _variants():
   add('coop_mining/live_rates_1', cm, 6, None, [ores], 'parity', reach=lambda s, sec: EV(s, 'mining') > 0 and EV(s, 'extraction') > 0)
   for w in (1, 255):
     add(f'coop_mining/mining_window_{w}', cm, 6, None, [ores, kw('Ore', miningWindow=w)], 'parity',
-        reach=lambda s, sec, w=w: int(sec['cm_ip'][6]) == w and EV(s, 'mining') > 0)
+        reach=lambda s, sec, w=w: _param(sec, 'MINE_WINDOW') == w and EV(s, 'mining') > 0)
   add('coop_mining/mining_window_256', cm, 6, None, [ores, kw('Ore', miningWindow=256)], 'refused', 'engine')
   add('coop_mining/mine_cooldown_1', cm, 6, None, [ores, kw('MineBeam', cooldownTime=1)], 'parity',
       reach=lambda s, sec: EV(s, 'mining') > 0)
@@ -362,7 +368,7 @@ def _variants():
     for name, geom in (('1x1', (0, 0, 0, 0)), ('5', (2, 2, 2, 2)), ('asymmetric', (0, 7, 2, 6)), ('12', (5, 6, 9, 1)),
                        ('13', (6, 6, 9, 1)), ('16', (7, 8, 9, 1)), ('tall', (5, 5, 14, 1))):
       add(f'{fam}/view_{name}', sub, p, None, [view(*geom)], 'parity', steps=40,
-          reach=lambda s, sec, geom=geom: tuple(int(x) for x in sec['meta'][15:19]) == geom)
+          reach=lambda s, sec, geom=geom: _view(sec) == geom)
     add(f'{fam}/view_17', sub, p, None, [view(8, 8, 9, 1)], 'refused', 'engine')
   return v
 
@@ -405,10 +411,15 @@ def sections(blob):
   return _sec(blob)
 
 
+def _view(sec):
+  """(left, right, forward, backward) of the view window of a blob's decoded sections."""
+  return tuple(int(sec['meta'][compiler.META[k]]) for k in ('VIEW_LEFT', 'VIEW_RIGHT', 'VIEW_FORWARD', 'VIEW_BACKWARD'))
+
+
 def view_geometry(blob):
-  m = _sec(blob)['meta']
-  return types.SimpleNamespace(left=int(m[15]), right=int(m[16]), forward=int(m[17]), backward=int(m[18]),
-                               width=int(m[15]) + int(m[16]) + 1, height=int(m[17]) + int(m[18]) + 1)
+  left, right, forward, backward = _view(_sec(blob))
+  return types.SimpleNamespace(left=left, right=right, forward=forward, backward=backward, width=left + right + 1,
+                               height=forward + backward + 1)
 
 
 def probe_sprites(variant, blob):
