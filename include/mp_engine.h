@@ -37,7 +37,7 @@ enum {
   MP_FLAG_RENDER_WORLD = 1u << 0, /* produce WORLD.RGB (base_simulation.lua:347-362) */
   MP_FLAG_RENDER_PLAYERS = 1u << 1, /* produce {i}.RGB (avatar_library.lua:264-276) */
   MP_FLAG_DEFAULT = 3u,
-  /* Diagnostics for tools/render_ceiling.py (the images are wrong or absent while any is set):
+  /* Diagnostics for tools/render_bound.py (the images are wrong or absent while any is set):
    * time the renderer's store path and its compositing separately. */
   MP_FLAG_DEBUG_NO_COMPOSE = 1u << 4,   /* issue the stores without drawing */
   MP_FLAG_DEBUG_NO_STORE = 1u << 5,     /* draw without storing */

@@ -531,9 +531,12 @@ int build_plan(mp_engine* E) {
         if (forced) need_forced = total;
         if (total > kRenderSmemLimit) continue;
         const double items = T.P * R.view_h + (8 >> wlog) * T.H, per_warp = items / warps;
-        // (constants fitted to measurements on the eight substrates: about three strips' worth of idle time per env and
-        //  warp, 2-row WORLD.RGB strips ~15 % slower than 4-row ones, a small cost per extra team)
-        const double score = teams * warps * per_warp / (per_warp + 3.0) * (wlog == 2 ? 1.0 : 0.85) * (1.0 - 0.01 * teams);
+        // (constants fitted to a sweep of every feasible layout of the nine substrates on an H100 SXM,
+        //  profiles/render_layouts_h100.jsonl: about 18 warps per SM keep the write stream full and more only add idle
+        //  time, about four strips' worth of idle time per env and warp at the team barriers, 2-row WORLD.RGB strips
+        //  ~15 % slower than 4-row ones, and each extra team ~10 % better: teams out of phase fill each other's per-env
+        //  gaps in the write stream)
+        const double score = std::min(teams * warps, 18) * per_warp / (per_warp + 4.0) * (wlog == 2 ? 1.0 : 0.85) * (1.0 + 0.1 * teams);
         if (score > best + 1e-9) {
           best = score;
           R.n_teams = teams; R.team_threads = warps * 32; R.wstrip_log2 = wlog; R.stage_bytes = stage;

@@ -22,8 +22,14 @@
 //      cell shows to this viewer (a rotated single sprite, or a multi-sprite record) and the eight
 //      lanes that draw its pixel rows fetch that by shuffle; multi-sprite cells are composited by
 //      the lanes that hold them, by selection where every alpha is 0 or 255, arithmetic otherwise.
-// The kernel is bound by instruction latency on the SM (no pipe is saturated), not by HBM: measured
-// with the stores disabled it takes about as long as with them (tools/render_ceiling.py).
+// What bounds it on H100 (tools/render_bound.py; H100 80GB HBM3 SXM at 700 W, clean_up x 4096, 3 x 10-warp layout):
+// the full kernel took 0.430 ms, with the stores alone (no compositing) 0.427 ms, with the compositing alone 0.200 ms,
+// and a torch fill_ of the same 1.16 GB took 0.355 ms. Compositing therefore hides under the stores, but the store
+// stream itself runs ~20 % below the write ceiling. More staging slots do not close the gap: built with two or three
+// slots per warp, at the layouts that then fit, the kernel was no faster, stores alone included, and a bare loop of
+// one-slot 2 KB bulk stores on 8-32 warps per SM reaches the fill_ rate. What is left is the per-env skeleton (grid
+// wait, per-cell pass, team barriers: 0.066 ms alone), during which a team has no stores in flight. More teams with
+// fewer warps each cover those gaps better (the layout score in build_plan).
 #pragma once
 
 #include <cstdio>
@@ -36,7 +42,7 @@
 #define TEAM_THREADS 512
 #endif
 #ifndef RENDER_SLOTS
-#define RENDER_SLOTS 1  // staging slots per warp (32 warps per SM hide the TMA read of a single slot)
+#define RENDER_SLOTS 1  // staging slots per warp (measured on H100: 2 or 3 bought nothing, see the header)
 #endif
 
 struct RenderPlan {  // host-computed constants of the tiling

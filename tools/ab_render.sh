@@ -1,7 +1,5 @@
 #!/bin/bash
 # A/B the render kernel across prebuilt library variants (diagnostic).
 for lib in build_variants/lib_*.so; do
-  for a in "territory__rooms 9" "clean_up 7" "commons_harvest__open 16"; do
-    echo -n "$lib $a: "; MP_ENGINE_LIB=$PWD/$lib python tools/render_ceiling.py $a 4096 300 | tail -1 | cut -c1-400
-  done
+  echo "$lib"; MP_ENGINE_LIB=$PWD/$lib python tools/render_bound.py | cut -c1-400
 done
