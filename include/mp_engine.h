@@ -164,7 +164,12 @@ int mp_reset_host(mp_handle h, const mp_host_outputs* out, void* stream);
  * device-side image / scalar staging set used; consecutive calls alternate slots, so step t+1's kernels run while
  * step t's observations are still crossing PCIe. mp_wait(h, slot) blocks until the outputs of the last call on
  * that slot are complete in the host buffers. `actions_host` and `out`'s buffers must stay untouched from the call
- * until mp_wait on the same slot returns. Steps are still applied in call order (one state per env). */
+ * until mp_wait on the same slot returns. Steps are still applied in call order (one state per env). A call refused
+ * with an error (e.g. `out` names events, which are not staged per slot) enqueues nothing and steps no env.
+ * Slot 0 renders into the engine's own images (mp_buffers.rgb / world_rgb); every other call that renders there
+ * (mp_step, mp_render, mp_step_host, mp_reset, mp_reset_host, mp_state_load) first waits, on its stream, for slot 0's
+ * copy-out, so it may be issued before mp_wait(h, 0). Slot 1 renders into a set of its own: after a slot-1 call,
+ * mp_buffers holds that step's scalars and state, and the images of the last render into the engine's own set. */
 int mp_step_host_async(mp_handle h, const int32_t* actions_host, const mp_host_outputs* out, int slot, void* stream);
 int mp_wait(mp_handle h, int slot);
 

@@ -615,6 +615,9 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
 
 int launch_render(mp_engine* E, cudaStream_t st) {
   if (!(E->flags & (MP_FLAG_RENDER_WORLD | MP_FLAG_RENDER_PLAYERS))) return E->x_pending_raise ? raise_flags(E, st) : MP_OK;
+  // The engine's own images are also slot 0's of mp_step_host_async: a render into them must not start before that
+  // slot's device->host copy has read them, whichever call issues it. (The slot-1 render has its own set.)
+  if (E->async_ready && E->S.rgb != E->slot[1].rgb) CUDA_TRY(cudaStreamWaitEvent(st, E->slot[0].copied, 0));
   E->S.x_raise = E->x_pending_raise ? 1 : 0;
   E->x_pending_raise = false;
   const int blocks = std::min(E->B, E->sm_count);  // every CTA has at least one env (balanced rounds + cooperative tail)
@@ -903,6 +906,8 @@ int async_setup(mp_engine* E) {
 
 int mp_step_host_async(mp_handle h, const int32_t* actions_host, const mp_host_outputs* out, int slot, void* stream) {
   if (!h || !actions_host || slot < 0 || slot > 1) return fail(MP_E_INVALID, "mp_step_host_async: null handle / actions or slot outside 0..1");
+  // (every argument is checked before anything is enqueued: a refused call leaves the envs where they were)
+  if (out && (out->events || out->event_count)) return fail(MP_E_INVALID, "mp_step_host_async: events are not staged per slot; read them with mp_step_host");
   DeviceGuard guard(h->device);
   int rc = async_setup(h);
   if (rc) return rc;
@@ -919,7 +924,6 @@ int mp_step_host_async(mp_handle h, const int32_t* actions_host, const mp_host_o
   CUDA_TRY(cudaMemcpyAsync(sl.scalars, h->scalar_block, h->scalar_block_bytes, cudaMemcpyDeviceToDevice, st));
   CUDA_TRY(cudaEventRecord(sl.computed, st));
   CUDA_TRY(cudaStreamWaitEvent(h->copy_stream, sl.computed, 0));
-  if (out && (out->events || out->event_count)) return fail(MP_E_INVALID, "mp_step_host_async: events are not staged per slot; read them with mp_step_host");
   if (out) {
     const size_t B = h->B, P = h->T.P;
     cudaStream_t cs = h->copy_stream;

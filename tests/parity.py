@@ -83,6 +83,91 @@ def _event_keys(events, counts):
   return key
 
 
+def shapes_of(eng):
+  """The output shapes OracleBatch.dump / env_dump lay their arrays out with, for this engine."""
+  bf = eng.buffers
+  return dict(P=eng.num_players, L=int(bf.grid_layers), cells=int(bf.grid_cells), n_scalar=eng.num_scalar_obs,
+              rgb=(int(bf.rgb_h), int(bf.rgb_w)), world=(int(bf.world_h), int(bf.world_w)))
+
+
+def device_outputs(eng, kinds=('rgb', 'world')):
+  """Every output in the engine's own buffers (mp_buffers) as host arrays keyed like OracleBatch.dump; of the images,
+  those named in `kinds`. Synchronises the device first."""
+  import torch
+  torch.cuda.synchronize()
+  got = dict(step_type=eng.step_type.cpu().numpy(), discount=eng.discount.cpu().numpy(), reward=eng.reward.cpu().numpy(),
+             scalar_obs=eng.scalar_obs.cpu().numpy()[:eng.num_scalar_obs], avatars=eng.avatar_state.cpu().numpy(),
+             grid=eng.grid.cpu().numpy().view(np.uint16)[:, :, :int(eng.buffers.grid_cells)],
+             n_events=eng.event_count.cpu().numpy(), events=eng.events.cpu().numpy())
+  if 'rgb' in kinds:
+    got['rgb'] = eng.rgb.cpu().numpy()
+  if 'world' in kinds:
+    got['world'] = eng.world_rgb.cpu().numpy()
+  return got
+
+
+_HOST_KEYS = dict(rgb='rgb', world_rgb='world', reward='reward', discount='discount', step_type='step_type',
+                  scalar_obs='scalar_obs', events='events', event_count='n_events')
+
+
+def host_outputs(out, n_scalar):
+  """The arrays of a host output set (Engine.make_host_outputs names) keyed like OracleBatch.dump."""
+  got = {_HOST_KEYS[k]: v.numpy() for k, v in out.items() if k in _HOST_KEYS and v is not None}
+  if 'scalar_obs' in got:
+    got['scalar_obs'] = got['scalar_obs'][:n_scalar]
+  return got
+
+
+def env_dump(envs, shapes, pixels=False, max_events=256, kinds=('rgb', 'world')):
+  """OracleBatch.dump for a list of OracleEnv (env b of the batch = envs[b]), for runs an OracleBatch cannot follow."""
+  from oracle import binding
+  code_of = {v: k for k, v in binding.EVENT_NAMES.items()}
+  B, P = len(envs), shapes['P']
+  out = {'reward': np.stack([e.rewards() for e in envs]), 'discount': np.array([e.discount() for e in envs]),
+         'step_type': np.array([e.step_type() for e in envs], np.int64),
+         'scalar_obs': np.zeros((max(shapes['n_scalar'], 1), B, P), np.float64),
+         'avatars': np.stack([e.avatars() for e in envs]), 'grid': np.stack([e.grid() for e in envs]),
+         'events': np.zeros((B, max_events, 3), np.int32), 'n_events': np.zeros((B,), np.int32)}
+  for b, e in enumerate(envs):
+    out['scalar_obs'][:shapes['n_scalar'], b] = e.scalar_obs().T
+    rows = [(code_of[name], x, y) for name, x, y in e.events()]
+    out['n_events'][b] = len(rows)
+    out['events'][b, :len(rows)] = np.array(rows, np.int32).reshape(-1, 3)
+  if pixels and 'rgb' in kinds:
+    out['rgb'] = np.stack([e.rgb() for e in envs])
+  if pixels and 'world' in kinds:
+    out['world'] = np.stack([e.world_rgb() for e in envs])
+  return out
+
+
+def check_outputs(got, want, where):
+  """Each array of `got` (device_outputs / host_outputs) must equal the same entry of `want` (OracleBatch.dump /
+  env_dump) bit for bit; event rows are compared as sorted keys, since the rows of one step are in no particular order."""
+
+  def same(name, g, exp):
+    assert g.shape == exp.shape, f'{name} {where}: shape {g.shape}, oracle {exp.shape}'
+    if not np.array_equal(g, exp):
+      bad = np.argwhere(g != exp)
+      raise AssertionError(f'{name} {where}: {len(bad)} mismatches, first at {bad[0].tolist()} (env first): gpu {g[tuple(bad[0])]} oracle {exp[tuple(bad[0])]}')
+
+  for key, name in (('step_type', 'step_type'), ('discount', 'discount'), ('reward', 'reward'), ('avatars', 'avatars'),
+                    ('grid', 'grid')):
+    if key in got:
+      same(name, got[key], want[key])
+  if 'scalar_obs' in got:
+    same('scalar_obs', got['scalar_obs'], want['scalar_obs'][:len(got['scalar_obs'])])
+  if 'n_events' in got:
+    nev = got['n_events']
+    same('event count', nev, want['n_events'])
+    if 'events' in got:
+      max_ev = got['events'].shape[1]
+      assert int(nev.max(initial=0)) <= max_ev, f'{where}: {int(nev.max())} events exceed max_events {max_ev}'
+      same('events', _event_keys(got['events'], nev), _event_keys(want['events'], want['n_events']))
+  for key, name in (('rgb', 'RGB'), ('world', 'WORLD.RGB')):
+    if key in got:
+      same(name, got[key], want[key])
+
+
 def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_every=10, actions_fn=None,
                   env_index_base=0, threads=None, flags=None, render_layout=None, pixels_at=None, on_step=None):
   """EVERY env of the batch against the oracle: rewards, discount, step type, scalar observations, avatar state, the
@@ -98,10 +183,8 @@ def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_eve
   eng = engine.Engine(blob, num_envs, device=0, seed=seed, env_index_base=env_index_base, flags=flags,
                       render_layout=render_layout)
   P, A = eng.num_players, eng.num_actions
-  bf = eng.buffers
-  shapes = dict(P=P, L=int(bf.grid_layers), cells=int(bf.grid_cells), n_scalar=eng.num_scalar_obs,
-                rgb=(int(bf.rgb_h), int(bf.rgb_w)), world=(int(bf.world_h), int(bf.world_w)))
-  max_ev = int(bf.max_events)
+  shapes = shapes_of(eng)
+  max_ev = int(eng.buffers.max_events)
   kinds = [k for k, bit in (('rgb', engine.MP_FLAG_RENDER_PLAYERS), ('world', engine.MP_FLAG_RENDER_WORLD)) if flags & bit]
   absent = [t for k, t in (('rgb', eng.rgb), ('world', eng.world_rgb)) if k not in kinds]
   for t in absent:
@@ -113,35 +196,14 @@ def compare_batch(blob, oracle, num_envs, steps, seed, action_seed=0, pixels_eve
   restarted = np.zeros(num_envs, bool)
 
   def check(t):
-    torch.cuda.synchronize()
     px = pixels_at(t) if pixels_at is not None else (t % pixels_every) == 0
+    got = device_outputs(eng, kinds if px else ())
     want = batch.dump(threads, shapes, pixels=px, max_events=max_ev, kinds=kinds)
-    where = f'step {t}'
-
-    def same(name, got, exp):
-      if not np.array_equal(got, exp):
-        bad = np.argwhere(got != exp)
-        raise AssertionError(f'{name} {where}: {len(bad)} mismatches, first at {bad[0].tolist()} (env first): gpu {got[tuple(bad[0])]} oracle {exp[tuple(bad[0])]}')
-
-    st = eng.step_type.cpu().numpy()
-    same('step_type', st, want['step_type'])
-    same('discount', eng.discount.cpu().numpy(), want['discount'])
-    same('reward', eng.reward.cpu().numpy(), want['reward'])
-    if shapes['n_scalar']:
-      same('scalar_obs', eng.scalar_obs.cpu().numpy()[:shapes['n_scalar']], want['scalar_obs'][:shapes['n_scalar']])
-    same('avatars', eng.avatar_state.cpu().numpy(), want['avatars'])
-    same('grid', eng.grid.cpu().numpy().view(np.uint16)[:, :, :shapes['cells']], want['grid'])
-    nev = eng.event_count.cpu().numpy()
-    same('event count', nev, want['n_events'])
-    assert int(nev.max(initial=0)) <= max_ev, f'{where}: {int(nev.max())} events exceed max_events {max_ev}'
-    same('events', _event_keys(eng.events.cpu().numpy(), nev), _event_keys(want['events'], want['n_events']))
+    check_outputs(got, want, f'step {t}')
+    st = got['step_type']
     if px:
-      if 'rgb' in kinds:
-        same('RGB', eng.rgb.cpu().numpy(), want['rgb'])
-      if 'world' in kinds:
-        same('WORLD.RGB', eng.world_rgb.cpu().numpy(), want['world'])
       for img in absent:
-        assert bool((img == _SENTINEL).all()), f'{where}: an image the flags leave out was written'
+        assert bool((img == _SENTINEL).all()), f'step {t}: an image the flags leave out was written'
       stats['pixel_checks'] += 1
     stats['rewards'] += float(want['reward'].sum())
     stats['lasts'] += int((st == 2).sum())

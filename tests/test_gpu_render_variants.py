@@ -176,8 +176,8 @@ def test_partial_render_flags_match_the_oracle(name, players, oracle):
   from meltingpot_b200 import engine
   blob = _blob(name, players)
   B = _sm_count() + 7  # cooperative tail only: CTAs 0-6 render two envs, the others one
-  for flags in (engine.MP_FLAG_RENDER_PLAYERS, engine.MP_FLAG_RENDER_WORLD):
-    # (compare_batch fills the image the flags leave out with a sentinel and checks it is never written)
+  for flags in (engine.MP_FLAG_RENDER_PLAYERS, engine.MP_FLAG_RENDER_WORLD, 0):
+    # (compare_batch fills the images the flags leave out with a sentinel and checks they are never written)
     stats = parity.compare_batch(blob, oracle, num_envs=B, steps=6, seed=29, flags=flags, pixels_every=1)
     assert stats['pixel_checks'] == 7
 

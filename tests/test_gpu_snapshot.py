@@ -16,7 +16,8 @@ def _play(eng, acts):
   return out, eng.rgb.cpu().numpy().copy(), eng.world_rgb.cpu().numpy().copy(), eng.grid.cpu().numpy().copy()
 
 
-@pytest.mark.parametrize('fixture', ['clean_up_blob', 'commons_blob', 'territory_blob'])
+@pytest.mark.parametrize('fixture', ['clean_up_blob', 'commons_blob', 'territory_blob', 'coins_blob', 'coop_mining_blob',
+                                     'territory_inside_out_blob'])
 def test_restore_replays_identically(fixture, request):
   import torch
   from meltingpot_b200 import engine
