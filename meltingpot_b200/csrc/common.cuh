@@ -1,4 +1,5 @@
-// common.cuh -- device-side tables, per-env state layout and RNG shared by the kernels.
+// common.cuh -- what the kernels share: the tables every kernel reads (Tables), the per-env state layout (State), the
+// step's events and the RNG. Each substrate family's own parameters are in its step_<family>.cuh.
 //
 // Data layout in HBM (struct-of-arrays, env instance on the leading axis):
 //   grid        u16 [B][L][cells_pad]   sprite grid: 0 empty, else 1 + sprite*4 + orientation.
@@ -38,77 +39,41 @@ struct BeamGeom {  // one beam footprint, cells in visiting order (policy A.8)
   int8_t parent[MP_MAX_BEAM_CELLS];  // cell that must be visited and unblocked first, or -1
 };
 
+// What every kernel reads: the map, the view, the avatars and their spawn points, the episode ending, the sizes of the
+// per-env entity arrays and the render tables. What only one family's state transition reads is in that family's
+// Params (step_<family>.cuh).
 struct Tables {
   // geometry
   int W, H, cells, cells_pad, L, P, topology, max_frames;
   int view_l, view_r, view_f, view_b, n_sprites, oob_sprite, oov_sprite, n_actions, n_scalar;
   int scalar_obs[4];
-  // shared avatar machinery
+  // avatars and spawn points
   int avatar_layer, n_spawn;
   int avatar_sprite[MP_MAX_PLAYERS];
-  int zap_cooldown, zap_respawn, zap_remove, zap_layer, zap_sprite, zap_hit;
-  double zap_penalty, zap_reward;
-  BeamGeom zap_geom;
-  // clean_up family
-  int nA, nD, nW, nA_pad, nD_pad, nW_pad;
-  int apple_layer, apple_sprite, dirt_layer, dirt_sprite, water_layer, n_anim, anim_frames, anim_random;
-  int water_sprite[8];
-  int clean_cooldown, clean_layer, clean_sprite, clean_hit;
-  BeamGeom clean_geom;
-  int dirt_delay, end_min_frames, end_interval, taste_role, dirt_count0;
-  double grow_rate, grow_depletion, grow_restoration, eat_reward, dirt_prob, end_prob, taste_amount;
-  // commons_harvest family
-  int wait_layer, wait_sprite, grass_layer, grass_sprite, dess_sprite, ch_n_wait, ch_n_probs;
-  double ch_probs[4];
+  const int32_t* spawn_cell;   // [n_spawn]
   // initial spawn groups (Avatar spawnGroup vs postInitialSpawnGroup, avatar_library.lua:121-125,322-328)
   int n_spawn_init[2];
   int avatar_init_group[MP_MAX_PLAYERS];
   const int32_t* spawn_init_cell[2];
-  const int32_t* ch_apple;     // [nA][4] obj id, cell, initially live, grass obj id
-  // territory family
-  int nR, nR_pad, res_layer, unclaimed_sprite, tex_layer, tex_sprite, ind_layer, dmg_layer, dmg_sprite, mark_layer;
-  int mark_initial_level, mark_recovery, mark_n_levels, mark_inc[3], mark_remove[3], mark_freeze[3], mark_sprite[3];
-  double mark_src_reward[3], mark_tgt_reward[3];
-  int claim_wait, brush_layer, claim_layer, res_health0, res_reward_delay, res_repair_delay, tr_taste_role;
-  double res_reward, res_rate, res_repair_prob, tr_taste_amount, tr_taste_mult;
-  int claimed_sprite[MP_MAX_PLAYERS], dry_sprite[MP_MAX_PLAYERS], brush_sprite[MP_MAX_PLAYERS], claimbeam_sprite[MP_MAX_PLAYERS];
-  BeamGeom claim_geom, brush_geom;
-  const int32_t* tr_res;       // [nR][3] obj id, cell, initial state
-  const int16_t* res_of_cell;  // [cells_pad] resource index or -1
-  const uint8_t* wall;         // [cells_pad] 1 where an AllBeamBlocker piece stands
   // 'choice' prefabs drawn per env and episode (prefab_utils.lua:63-65): ticket of group g = pick(philox(0, episode, g, RS_CHOICE).x, choice_n[g])
   int n_choice;
   const int32_t* choice_n;     // [n_choice] options per group
   const int32_t* spawn_cond;   // [n_spawn][2] (group or -1, ticket mask) of each spawn candidate, or null
-  const int32_t* tr_res_cond;  // [nR][2] same for each resource, or null
-  const int32_t* ch_nbr;       // [nA][16] apples inside the regrowth disc (excluding self), -1 padded
+  // StochasticIntervalEpisodeEnding (every family)
+  int end_min_frames, end_interval;
+  double end_prob;
+  // per-env entity arrays of State: apple / apple_count [nA_pad], dirt [nD_pad], water [nW_pad], fam_u8 / fam_u16 rows of nR_pad
+  int nA, nD, nW, nR, nA_pad, nD_pad, nW_pad, nR_pad;
   // device tables
   const uint16_t* init_grid;   // [L][cells_pad]
   const int32_t* action_table; // [n_actions][4]
-  const int32_t* apple;        // [nA][3] obj id, cell, initially live
-  const int32_t* dirt;         // [nD][3] obj id, cell, initially dirty
-  const int32_t* water;        // [nW][2] obj id, cell
-  const int32_t* spawn_cell;   // [n_spawn]
   const uint8_t* solid;        // [cells_pad] 255 where the avatar layer is statically occupied
   const uint8_t* cell_flags;   // [cells_pad] bit h: a BeamBlocker for hit h sits here
-  const int16_t* apple_of_cell;  // [cells_pad] apple index or -1
-  const int16_t* dirt_of_cell;   // [cells_pad] dirt index or -1
   // render tables
   const uint8_t* atlas;        // [n_total][4][2][8][16]: facing, half (px 0-3 | 4-7), row, 16 B (n_total includes pre-merged sprites)
   const int16_t* sprite_map;   // [P+1][n_total]
   const uint8_t* sprite_opaque;  // [n_total] bit 0: every pixel alpha 255 and never remapped; bit 1: remapped for some viewer
   const uint8_t* sprite_pair;    // [n_total][n_total] pre-merged sprite for (opaque base, sprite on top) or 0
-  // coins family (step_coins.cuh); the coins reuse ch_apple / apple_of_cell / apple_layer
-  int coin_sprite[2];          // sprite of coin type 0 / 1 (liveStateA / liveStateB)
-  int coin_type[2];            // PlayerCoinType of each player
-  double coin_reward[2][4];    // per collecting player: self match, self mismatch, other match, other mismatch
-  double coin_rate;            // ChoiceCoinRegrow regrowRate
-  int coin_terminate, coin_terminate_n;
-  // coop_mining family (step_mining.cuh); ores reuse ch_apple / apple_of_cell / apple_layer, the beam reuses zap_*
-  int ore_sprite[4];           // wait, single-miner raw, two-miner raw, two-miner partial
-  int mine_window, mine_length;
-  double mine_rate[2];         // FixedRateRegrow liveRates
-  double mine_reward[2], extract_reward[2];  // per ore type (1 miner, 2 miners)
 };
 
 struct State {

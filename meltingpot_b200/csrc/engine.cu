@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <variant>
 #include <vector>
 
 #include "../../include/mp_engine.h"
@@ -126,21 +127,37 @@ int make_lane_map_cells(int n_rows, int n_cells, int pitch_slots, int iters, uin
   return best;
 }
 
-// One row per substrate family: the blob decode (host, step_<family>.cuh) and the state-transition kernel with the
-// dynamic shared memory one launch of it takes.
-using StepFn = void (*)(Tables, State, const int32_t*, const uint8_t*, int);
+// One row per substrate family: the blob decode into the family's Params (host, step_<family>.cuh) and the
+// state-transition kernel with the dynamic shared memory one launch of it takes. An engine keeps the Params of its
+// family in a FamilyParams; only the row's own functions look inside it.
+using FamilyParams = std::variant<CleanUp::Params, Commons::Params, Territory::Params, Coins::Params, Mining::Params>;
 struct FamilyEntry {
   int id;  // MpbFamily
-  int (*load)(FamilyLoad&, Tables&);
-  StepFn step;
+  int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
+  cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int);
   size_t (*step_smem)(const Tables&);
+  const void* step;  // k_step<Family>
 };
+
+template <class Family>
+int load_family(FamilyLoad& ld, const Tables& T, FamilyParams& params) {
+  return Family::load(ld, T, params.emplace<typename Family::Params>());
+}
+template <class Family>
+cudaError_t launch_family(const cudaLaunchConfig_t& cfg, const Tables& T, const FamilyParams& params, const State& S,
+                          const int32_t* actions, const uint8_t* mask, int mode) {
+  return cudaLaunchKernelEx(&cfg, k_step<Family>, T, std::get<typename Family::Params>(params), S, actions, mask, mode);
+}
+template <class Family>
+FamilyEntry family_entry(int id) {
+  return {id, load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>)};
+}
 const FamilyEntry kFamilies[] = {
-    {MPB_FAMILY_CLEAN_UP, CleanUp::load, k_step<CleanUp>, step_smem_bytes<CleanUp>},
-    {MPB_FAMILY_COMMONS_HARVEST, Commons::load, k_step<Commons>, step_smem_bytes<Commons>},
-    {MPB_FAMILY_TERRITORY, Territory::load, k_step<Territory>, step_smem_bytes<Territory>},
-    {MPB_FAMILY_COINS, Coins::load, k_step<Coins>, step_smem_bytes<Coins>},
-    {MPB_FAMILY_COOP_MINING, Mining::load, k_step<Mining>, step_smem_bytes<Mining>},
+    family_entry<CleanUp>(MPB_FAMILY_CLEAN_UP),
+    family_entry<Commons>(MPB_FAMILY_COMMONS_HARVEST),
+    family_entry<Territory>(MPB_FAMILY_TERRITORY),
+    family_entry<Coins>(MPB_FAMILY_COINS),
+    family_entry<Mining>(MPB_FAMILY_COOP_MINING),
 };
 
 }  // namespace
@@ -152,6 +169,8 @@ struct mp_engine {
   const FamilyEntry* family = nullptr;
   int n_total = 0;  // atlas sprites incl. pre-merged
   Tables T{};
+  FamilyParams params;
+  int beam_cells = 0;  // FamilyLoad::beam_cells: sizes State::max_events
   State S{};
   RenderPlan R{};
   mp_buffers buffers{};
@@ -278,12 +297,13 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   if (T.n_spawn < 1) return fail(MP_E_INVALID, "empty respawn group");
 
   // ---- family tables -----------------------------------------------------------------------------
-  T.nA = T.nD = T.nW = 0; T.nR = 0; T.nR_pad = 16;
-  T.n_anim = 1; T.anim_frames = 1; T.clean_layer = 0;
   FamilyLoad ld{blob, n, hits, E->allocs};
   int rc;
-  if ((rc = E->family->load(ld, T))) return rc;
+  if ((rc = E->family->load(ld, T, E->params))) return rc;
 #undef NEED
+  T.nA = ld.nA; T.nD = ld.nD; T.nW = ld.nW; T.nR = ld.nR; T.nR_pad = ld.nR_pad;
+  T.end_min_frames = ld.end_min_frames; T.end_interval = ld.end_interval; T.end_prob = ld.end_prob;
+  E->beam_cells = ld.beam_cells;
   {  // 'choice' prefabs left to the engine (drawn per env and episode)
     Section<int32_t> choice_groups, obj_choice, spawn_cond;
     if (get_section(blob, n, "choice_groups", MPB_I32, &choice_groups)) {
@@ -323,10 +343,6 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   }
   memcpy(flags.data(), cell_flags.data, std::min<size_t>(cell_flags.count, T.cells));
   if ((rc = upload(E->allocs, solid, &T.solid)) || (rc = upload(E->allocs, flags, &T.cell_flags))) return rc;
-  std::vector<int16_t> apple_of(T.cells_pad, -1), dirt_of(T.cells_pad, -1);
-  for (size_t k = 0; k < ld.apple_cells.size(); ++k) apple_of[ld.apple_cells[k]] = (int16_t)k;
-  for (size_t j = 0; j < ld.dirt_cells.size(); ++j) dirt_of[ld.dirt_cells[j]] = (int16_t)j;
-  if ((rc = upload(E->allocs, apple_of, &T.apple_of_cell)) || (rc = upload(E->allocs, dirt_of, &T.dirt_of_cell))) return rc;
 
   // ---- render tables ------------------------------------------------------------------------------
   if (atlas.count != (size_t)T.n_sprites * 1024) return fail(MP_E_INVALID, "atlas has %zu bytes, expected %d", atlas.count, T.n_sprites * 1024);
@@ -603,7 +619,7 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->family->step, E->T, E->S, actions, mask, mode));
+  CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st); }
@@ -717,8 +733,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   {  // Worst case of events one step can emit per env: per avatar, every cell of every beam footprint can carry a hit
      // with up to three events (zap + sanctioning + removal), plus the contact / regrowth events (<= 4) and the pair
      // events of coop_mining (<= P). Sized so that emit_event never drops a row.
-    const int beam_cells = T.zap_geom.n + T.clean_geom.n + T.claim_geom.n + T.brush_geom.n;
-    S.max_events = round_up(std::max(MP_MIN_EVENTS, T.P * (3 * beam_cells + 4 + T.P)), 16);
+    S.max_events = round_up(std::max(MP_MIN_EVENTS, T.P * (3 * E->beam_cells + 4 + T.P)), 16);
   }
   S.fam_u8_stride = std::max(16, RU_COUNT * T.nR_pad); S.fam_u16_stride = std::max(16, RS_COUNT * T.nR_pad);
   if ((rc = E->alloc(B * T.L * T.cells_pad, &S.grid)) || (rc = E->alloc(B * P * 4, &S.avatar)) || (rc = E->alloc(B * P * 4, &S.av_timer)) ||

@@ -16,6 +16,13 @@
 #include "../../include/mpb_format.h"
 #include "common.cuh"
 
+// The Zapper component (avatar_library.lua:570-850) of the clean_up, commons_harvest and territory avatars.
+struct Zapper {
+  int cooldown, respawn, remove, layer, sprite, hit;  // respawn: framesTillRespawn; remove: removeHitPlayer; hit: its hit id
+  double penalty, reward;
+  BeamGeom geom;
+};
+
 namespace {
 
 thread_local std::string g_error;
@@ -99,15 +106,18 @@ bool beam_fits_torus(const Tables& T, int length, int radius) {
   return T.topology != 1 || (length < m && 2 * radius + 1 <= m);
 }
 
-// What build_tables hands a family's loader, and what the loader hands back besides the Tables fields it sets. On entry
-// the Tables hold the geometry, the avatar tables and zero entity counts.
+// What build_tables hands a family's loader (`load(FamilyLoad&, const Tables&, Params&)`), and what the loader hands
+// back besides its Params. On entry the Tables hold the geometry and the avatar tables.
 struct FamilyLoad {
   const void* blob;
   size_t n;
   Section<int32_t> hits;               // [n_hits][2] layer, sprite
   std::vector<void*>& allocs;          // the engine's device allocations
-  std::vector<int32_t> apple_cells;    // cell of each apple / coin / ore: apple_of_cell
-  std::vector<int32_t> dirt_cells;     // cell of each dirt: dirt_of_cell
+  // handed back: the Tables fields the family decides
+  int nA = 0, nD = 0, nW = 0, nR = 0, nR_pad = 16;  // per-env entity counts (State's array sizes, Tables::nA...)
+  int end_min_frames = 0, end_interval = 0;          // StochasticIntervalEpisodeEnding
+  double end_prob = 0.0;
+  int beam_cells = 0;                  // footprint cells of the beams State::max_events provides for
   std::vector<std::vector<int>> hint_stacks;  // sprite stacks (bottom up) worth a pre-merged sprite before the generic enumeration
 
   template <typename T>
@@ -131,18 +141,36 @@ struct FamilyLoad {
   }
 };
 
-// The Zapper and episode-ending slots (MPB_FP_*) of clean_up, commons_harvest and territory.
-int load_zapper(const FamilyLoad& ld, Tables& T, const int32_t* ip) {
-  T.zap_cooldown = ip[MPB_FP_ZAP_COOLDOWN]; T.zap_respawn = ip[MPB_FP_ZAP_RESPAWN]; T.zap_remove = ip[MPB_FP_ZAP_REMOVE];
-  T.zap_layer = ip[MPB_FP_ZAP_LAYER]; T.zap_sprite = ip[MPB_FP_ZAP_SPRITE];
-  T.zap_hit = 0;
-  for (int h = 0; h < (int)ld.hits.count / 2; ++h) if (ld.hits.data[h * 2] == T.zap_layer) T.zap_hit = h;
+// The cell -> entity index of the n entities of section `name`, entity k standing on cell rows.data[k * row_len + 1]:
+// [cells_pad] index or -1. Refuses a section shorter than n rows or an entity off the map, so that neither this index nor
+// the kernels, which read the section's first n rows, reach past what the blob holds.
+int upload_cell_index(FamilyLoad& ld, const Tables& T, const char* name, const Section<int32_t>& rows, int n, int row_len,
+                      const int16_t** out) {
+  if (n < 0 || rows.count < (size_t)n * row_len)
+    return fail(MP_E_INVALID, "blob: section '%s' has %zu values for %d entities of %d", name, rows.count, n, row_len);
+  std::vector<int16_t> of(T.cells_pad, -1);
+  for (int k = 0; k < n; ++k) {
+    const int cell = rows.data[k * row_len + 1];
+    if (cell < 0 || cell >= T.cells) return fail(MP_E_INVALID, "blob: section '%s' puts entity %d on cell %d of a %d-cell map", name, k, cell, T.cells);
+    of[cell] = (int16_t)k;
+  }
+  return upload(ld.allocs, of, out);
+}
+
+// The Zapper and episode-ending slots (MPB_FP_*) of clean_up, commons_harvest and territory. The penalty and reward sit
+// in each family's own f64 slots.
+int load_zapper(FamilyLoad& ld, const Tables& T, const int32_t* ip, double penalty, double reward, Zapper& z) {
+  z.cooldown = ip[MPB_FP_ZAP_COOLDOWN]; z.respawn = ip[MPB_FP_ZAP_RESPAWN]; z.remove = ip[MPB_FP_ZAP_REMOVE];
+  z.layer = ip[MPB_FP_ZAP_LAYER]; z.sprite = ip[MPB_FP_ZAP_SPRITE];
+  z.hit = 0;
+  for (int h = 0; h < (int)ld.hits.count / 2; ++h) if (ld.hits.data[h * 2] == z.layer) z.hit = h;
+  z.penalty = penalty; z.reward = reward;
   const int length = ip[MPB_FP_ZAP_LENGTH], radius = ip[MPB_FP_ZAP_RADIUS];
-  if (T.zap_cooldown <= 0) return fail(MP_E_UNSUPPORTED, "non-positive zap cooldown");
-  if (!make_beam_geom(length, radius, &T.zap_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+  if (z.cooldown <= 0) return fail(MP_E_UNSUPPORTED, "non-positive zap cooldown");
+  if (!make_beam_geom(length, radius, &z.geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
   if (!beam_fits_torus(T, length, radius)) return fail(MP_E_UNSUPPORTED, "zap beam (length %d, radius %d) does not fit the %dx%d TORUS map", length, radius, T.W, T.H);
-  T.end_min_frames = ip[MPB_FP_END_MIN_FRAMES]; T.end_interval = ip[MPB_FP_END_INTERVAL];
-  if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
+  ld.end_min_frames = ip[MPB_FP_END_MIN_FRAMES]; ld.end_interval = ip[MPB_FP_END_INTERVAL];
+  if (ld.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
   return MP_OK;
 }
 

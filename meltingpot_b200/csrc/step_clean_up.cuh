@@ -14,8 +14,23 @@
 #include "step_common.cuh"
 
 struct CleanUp {
+  struct Params {
+    Zapper zap;
+    int apple_layer, apple_sprite, dirt_layer, dirt_sprite, water_layer, n_anim, anim_frames, anim_random;
+    int water_sprite[8];
+    int clean_cooldown, clean_layer, clean_sprite, clean_hit;
+    BeamGeom clean_geom;
+    int dirt_delay, dirt_count0;
+    double grow_rate, grow_depletion, grow_restoration, eat_reward, dirt_prob;
+    const int32_t* apple;          // [nA][3] obj id, cell, initially live
+    const int32_t* dirt;           // [nD][3] obj id, cell, initially dirty
+    const int32_t* water;          // [nW][2] obj id, cell
+    const int16_t* apple_of_cell;  // [cells_pad] apple index or -1
+    const int16_t* dirt_of_cell;   // [cells_pad] dirt index or -1
+  };
+
   // Host: the clean_up tables of the blob (compiler.py _clean_up_tables): cu_ip / cu_dp, apples, dirt and water.
-  static int load(FamilyLoad& ld, Tables& T) {
+  static int load(FamilyLoad& ld, const Tables& T, Params& F) {
     const int32_t* ip;
     const double* dp;
     Section<int32_t> apple, dirt, water, water_sprites;
@@ -24,51 +39,55 @@ struct CleanUp {
         (rc = ld.need("cu_dirt", MPB_I32, &dirt)) || (rc = ld.need("cu_water", MPB_I32, &water)) ||
         (rc = ld.need("cu_water_sprites", MPB_I32, &water_sprites)))
       return rc;
-    T.nA = ip[MPB_CU_I_N_APPLES]; T.nD = ip[MPB_CU_I_N_DIRT]; T.nW = ip[MPB_CU_I_N_WATER];
-    T.apple_layer = ip[MPB_CU_I_APPLE_LAYER]; T.apple_sprite = ip[MPB_CU_I_APPLE_SPRITE];
-    T.dirt_layer = ip[MPB_CU_I_DIRT_LAYER]; T.dirt_sprite = ip[MPB_CU_I_DIRT_SPRITE];
-    T.water_layer = ip[MPB_CU_I_WATER_LAYER]; T.n_anim = ip[MPB_CU_I_N_ANIM];
-    T.anim_frames = ip[MPB_CU_I_ANIM_FRAMES]; T.anim_random = ip[MPB_CU_I_ANIM_RANDOM];
-    if (T.n_anim < 1 || T.n_anim > 8 || T.anim_frames < 1) return fail(MP_E_UNSUPPORTED, "animation with %d states / %d frames", T.n_anim, T.anim_frames);
-    for (int i = 0; i < T.n_anim; ++i) T.water_sprite[i] = water_sprites.data[i];
-    if ((rc = load_zapper(ld, T, ip))) return rc;
-    T.clean_cooldown = ip[MPB_CU_I_CLEAN_COOLDOWN]; T.clean_layer = ip[MPB_CU_I_CLEAN_LAYER]; T.clean_sprite = ip[MPB_CU_I_CLEAN_SPRITE];
-    T.clean_hit = 1;
-    for (int h = 0; h < (int)ld.hits.count / 2; ++h) if (ld.hits.data[h * 2] == T.clean_layer) T.clean_hit = h;
+    ld.nA = ip[MPB_CU_I_N_APPLES]; ld.nD = ip[MPB_CU_I_N_DIRT]; ld.nW = ip[MPB_CU_I_N_WATER];
+    F.apple_layer = ip[MPB_CU_I_APPLE_LAYER]; F.apple_sprite = ip[MPB_CU_I_APPLE_SPRITE];
+    F.dirt_layer = ip[MPB_CU_I_DIRT_LAYER]; F.dirt_sprite = ip[MPB_CU_I_DIRT_SPRITE];
+    F.water_layer = ip[MPB_CU_I_WATER_LAYER]; F.n_anim = ip[MPB_CU_I_N_ANIM];
+    F.anim_frames = ip[MPB_CU_I_ANIM_FRAMES]; F.anim_random = ip[MPB_CU_I_ANIM_RANDOM];
+    if (F.n_anim < 1 || F.n_anim > 8 || F.anim_frames < 1) return fail(MP_E_UNSUPPORTED, "animation with %d states / %d frames", F.n_anim, F.anim_frames);
+    for (int i = 0; i < F.n_anim; ++i) F.water_sprite[i] = water_sprites.data[i];
+    if ((rc = load_zapper(ld, T, ip, dp[MPB_CU_D_ZAP_PENALTY], dp[MPB_CU_D_ZAP_REWARD], F.zap))) return rc;
+    F.clean_cooldown = ip[MPB_CU_I_CLEAN_COOLDOWN]; F.clean_layer = ip[MPB_CU_I_CLEAN_LAYER]; F.clean_sprite = ip[MPB_CU_I_CLEAN_SPRITE];
+    F.clean_hit = 1;
+    for (int h = 0; h < (int)ld.hits.count / 2; ++h) if (ld.hits.data[h * 2] == F.clean_layer) F.clean_hit = h;
     const int length = ip[MPB_CU_I_CLEAN_LENGTH], radius = ip[MPB_CU_I_CLEAN_RADIUS];
-    if (T.clean_cooldown < 0) return fail(MP_E_UNSUPPORTED, "negative clean cooldown");
-    if (!make_beam_geom(length, radius, &T.clean_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (F.clean_cooldown < 0) return fail(MP_E_UNSUPPORTED, "negative clean cooldown");
+    if (!make_beam_geom(length, radius, &F.clean_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
     if (!beam_fits_torus(T, length, radius)) return fail(MP_E_UNSUPPORTED, "clean beam (length %d, radius %d) does not fit the %dx%d TORUS map", length, radius, T.W, T.H);
-    T.dirt_delay = ip[MPB_CU_I_DIRT_DELAY]; T.taste_role = ip[MPB_CU_I_TASTE_ROLE];
-    if (T.taste_role != 0) return fail(MP_E_UNSUPPORTED, "Taste roles other than 'free'");
-    T.grow_rate = dp[MPB_CU_D_GROW_RATE]; T.grow_depletion = dp[MPB_CU_D_GROW_DEPLETION];
-    T.grow_restoration = dp[MPB_CU_D_GROW_RESTORATION]; T.eat_reward = dp[MPB_CU_D_EAT_REWARD];
-    T.zap_penalty = dp[MPB_CU_D_ZAP_PENALTY]; T.zap_reward = dp[MPB_CU_D_ZAP_REWARD]; T.dirt_prob = dp[MPB_CU_D_DIRT_PROB];
-    T.end_prob = dp[MPB_CU_D_END_PROB]; T.taste_amount = dp[MPB_CU_D_TASTE_AMOUNT];
+    ld.beam_cells = F.zap.geom.n + F.clean_geom.n;
+    F.dirt_delay = ip[MPB_CU_I_DIRT_DELAY];
+    if (ip[MPB_CU_I_TASTE_ROLE] != 0) return fail(MP_E_UNSUPPORTED, "Taste roles other than 'free'");
+    F.grow_rate = dp[MPB_CU_D_GROW_RATE]; F.grow_depletion = dp[MPB_CU_D_GROW_DEPLETION];
+    F.grow_restoration = dp[MPB_CU_D_GROW_RESTORATION]; F.eat_reward = dp[MPB_CU_D_EAT_REWARD];
+    F.dirt_prob = dp[MPB_CU_D_DIRT_PROB]; ld.end_prob = dp[MPB_CU_D_END_PROB];
     std::vector<int32_t> v_apple(apple.data, apple.data + apple.count), v_dirt(dirt.data, dirt.data + dirt.count);
     std::vector<int32_t> v_water(water.data, water.data + water.count);
-    if ((rc = upload(ld.allocs, v_apple, &T.apple)) || (rc = upload(ld.allocs, v_dirt, &T.dirt)) || (rc = upload(ld.allocs, v_water, &T.water))) return rc;
-    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 3 + 1]);
-    T.dirt_count0 = 0;
-    for (int j = 0; j < T.nD; ++j) { ld.dirt_cells.push_back(v_dirt[j * 3 + 1]); T.dirt_count0 += v_dirt[j * 3 + 2]; }
+    if ((rc = upload(ld.allocs, v_apple, &F.apple)) || (rc = upload(ld.allocs, v_dirt, &F.dirt)) || (rc = upload(ld.allocs, v_water, &F.water)) ||
+        (rc = upload_cell_index(ld, T, "cu_apple", apple, ld.nA, 3, &F.apple_of_cell)) || (rc = upload_cell_index(ld, T, "cu_dirt", dirt, ld.nD, 3, &F.dirt_of_cell)))
+      return rc;
+    F.dirt_count0 = 0;
+    for (int j = 0; j < ld.nD; ++j) F.dirt_count0 += v_dirt[j * 3 + 2];
     return MP_OK;
   }
 
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
-  __host__ __device__ static size_t table_bytes(const Tables& T) { return scratch_round16((size_t)T.cells_pad * 6) + scratch_round16((size_t)T.n_actions * 16); }
+  __host__ __device__ static size_t table_bytes(const Tables& T) { return scratch_round16((size_t)T.cells_pad * 6) + (size_t)T.n_actions * 16 + 2 * sizeof(BeamGeom); }
 
-  // Per-CTA tables: apple_of and dirt_of (int16), solid and flags (8-byte aligned: cells_pad is a multiple of 8), then the
-  // action table.
-  __device__ static void stage(const Tables& T, uint8_t* tb) {
+  // Per-CTA tables: apple_of and dirt_of (int16), solid and flags (8-byte aligned: cells_pad is a multiple of 8), the
+  // action table, then the zap and clean beam footprints. Each lane reads its own footprint cell; read from the kernel
+  // parameters instead, the two footprints cost this kernel 24 B more stack and 32 / 48 B more spill stores / loads.
+  __device__ static void stage(const Tables& T, const Params& F, uint8_t* tb) {
     int16_t* s_apple_of = reinterpret_cast<int16_t*>(tb);
     int16_t* s_dirt_of = s_apple_of + T.cells_pad;
     uint8_t* s_solid = reinterpret_cast<uint8_t*>(s_dirt_of + T.cells_pad);
     uint8_t* s_flags = s_solid + T.cells_pad;
     int32_t* s_act = reinterpret_cast<int32_t*>(tb + scratch_round16((size_t)T.cells_pad * 6));
-    for (int i = threadIdx.x; i < T.cells_pad; i += (int)blockDim.x) { s_apple_of[i] = T.apple_of_cell[i]; s_dirt_of[i] = T.dirt_of_cell[i]; s_flags[i] = T.cell_flags[i]; s_solid[i] = T.solid[i]; }
+    for (int i = threadIdx.x; i < T.cells_pad; i += (int)blockDim.x) { s_apple_of[i] = F.apple_of_cell[i]; s_dirt_of[i] = F.dirt_of_cell[i]; s_flags[i] = T.cell_flags[i]; s_solid[i] = T.solid[i]; }
     for (int i = threadIdx.x; i < T.n_actions * 4; i += (int)blockDim.x) s_act[i] = T.action_table[i];
+    BeamGeom* s_beams = reinterpret_cast<BeamGeom*>(s_act + T.n_actions * 4);
+    if (threadIdx.x == 0) { s_beams[0] = F.zap.geom; s_beams[1] = F.clean_geom; }
   }
 
   __device__ static WarpScratch carve(const Tables& T, uint8_t* base, const uint8_t* tb) {
@@ -80,32 +99,35 @@ struct CleanUp {
     sc.act_table = reinterpret_cast<const int32_t*>(tb + scratch_round16((size_t)T.cells_pad * 6));
     return sc;
   }
+  // The zap and clean beam footprints, right after the action table (found from act_table: one more pointer in the
+  // scratch struct spills as well).
+  __device__ static const BeamGeom* beams(const Tables& T, const WarpScratch& sc) { return reinterpret_cast<const BeamGeom*>(sc.act_table + T.n_actions * 4); }
 
-  __device__ static void reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
+  __device__ static void reset(const Tables& T, const Params& F, const State& S, int b, int lane, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
     __syncwarp();
     copy_init_grid(T, grid, lane);
-    for (int k = lane; k < T.nA; k += 32) S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)T.apple[k * 3 + 2];
-    for (int j = lane; j < T.nD; j += 32) S.dirt[(size_t)b * T.nD_pad + j] = (uint8_t)T.dirt[j * 3 + 2];
+    for (int k = lane; k < T.nA; k += 32) S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)F.apple[k * 3 + 2];
+    for (int j = lane; j < T.nD; j += 32) S.dirt[(size_t)b * T.nD_pad + j] = (uint8_t)F.dirt[j * 3 + 2];
     __syncwarp();
     // Animation:postStart random start frame (component_library.lua:1064-1068).
     for (int k = lane; k < T.nW; k += 32) {
       int phase = 0;
-      if (T.anim_random) {
-        uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.water[k * 2], RS_OBJECT_RESET, k0, k1);
-        phase = (int)pick(w.x, (uint32_t)T.n_anim);
+      if (F.anim_random) {
+        uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)F.water[k * 2], RS_OBJECT_RESET, k0, k1);
+        phase = (int)pick(w.x, (uint32_t)F.n_anim);
       }
       S.water[(size_t)b * T.nW_pad + k] = (uint8_t)phase;
-      grid[(size_t)T.water_layer * T.cells_pad + T.water[k * 2 + 1]] = cell_value(T.water_sprite[phase], 0);
+      grid[(size_t)F.water_layer * T.cells_pad + F.water[k * 2 + 1]] = cell_value(F.water_sprite[phase], 0);
     }
     const auto all = [](int) { return true; };
     spawn_group(T, S, b, lane, grid, sc.tmp, T.spawn_cell, T.n_spawn, all, all, episode, k0, k1, [&](int) {
       for (int k = 0; k < T.n_scalar; ++k) S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 : 0.0;
     });
-    reset_env_row(T, S, b, lane, episode, T.dirt_count0);
+    reset_env_row(T, S, b, lane, episode, F.dirt_count0);
   }
 
-  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
     int dirt_count = env[ENV_DIRT];
     const unsigned cleaned_prev = (unsigned)env[ENV_CLEANED];
@@ -138,17 +160,17 @@ struct CleanUp {
     __syncwarp();
     if (is_av && alive) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
     // Hit sprites live for one frame (policy A.8): clear both beam layers if the last frame drew any.
-    if (env[ENV_BEAM]) { clear_layer(T, grid, T.zap_layer, lane); clear_layer(T, grid, T.clean_layer, lane); }
+    if (env[ENV_BEAM]) { clear_layer(T, grid, F.zap.layer, lane); clear_layer(T, grid, F.clean_layer, lane); }
     __syncwarp();
     int beam_dirty = 0;
 
     // ---- simulation:update --------------------------------------------------------------------
     // DirtSpawner:update (clean_up/components.lua:329-340); its _timeStep equals n here.
     int spawn_dirt = -1;
-    if (n > T.dirt_delay) {
+    if (n > F.dirt_delay) {
       uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, SCENE_DRAW_DIRT, RS_SCENE, k0, k1);
       int n_inactive = T.nD - dirt_count;
-      if (u01(w.x, w.y) < T.dirt_prob && n_inactive > 0) {
+      if (u01(w.x, w.y) < F.dirt_prob && n_inactive > 0) {
         int kth = (int)pick(w.z, (uint32_t)n_inactive);  // k-th inactive dirt in piece order
         for (int base = 0; base < T.nD; base += 32) {
           int j = base + lane;
@@ -170,12 +192,12 @@ struct CleanUp {
     {
       const double dirt = (double)dirt_count, clean = (double)(T.nD - dirt_count);
       const double fraction = dirt / (dirt + clean);
-      double interpolation = (fraction - T.grow_depletion) / (T.grow_restoration - T.grow_depletion);
+      double interpolation = (fraction - F.grow_depletion) / (F.grow_restoration - F.grow_depletion);
       interpolation = 1.0 < interpolation ? 1.0 : interpolation;  // Lua 5.1 math.min: a NaN (0/0) stays NaN, no growth (policy A.22)
-      const double probability = T.grow_rate * interpolation;
+      const double probability = F.grow_rate * interpolation;
       if (probability > 0.0) {  // u >= 0 can never be below a non-positive (or NaN) probability
         for (int k = lane; k < T.nA; k += 32) {
-          uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.apple[k * 3], RS_OBJECT, k0, k1);
+          uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)F.apple[k * 3], RS_OBJECT, k0, k1);
           if (u01(w.x, w.y) < probability && !(sc.apple[k] & 1)) sc.apple[k] |= 4;  // grows this frame
         }
       }
@@ -189,11 +211,11 @@ struct CleanUp {
     // 140 Zapper zap (:613-631) and Cleaner clean (clean_up/components.lua:201-219).
     bool fire_zap = false, fire_clean = false;
     if (is_av && alive) {
-      if (zap_cool > 0) --zap_cool; else if (act_zap == 1) { zap_cool = T.zap_cooldown; fire_zap = true; }
-      if (clean_cool > 0) --clean_cool; else if (act_clean == 1) { clean_cool = T.clean_cooldown; fire_clean = true; }
+      if (zap_cool > 0) --zap_cool; else if (act_zap == 1) { zap_cool = F.zap.cooldown; fire_zap = true; }
+      if (clean_cool > 0) --clean_cool; else if (act_clean == 1) { clean_cool = F.clean_cooldown; fire_clean = true; }
     }
     // 135 Zapper respawn (:638-649): state = waitState, startFrame = framesTillRespawn.
-    const bool want_respawn = is_av && !alive && (n - state_frame) >= T.zap_respawn;
+    const bool want_respawn = is_av && !alive && (n - state_frame) >= F.zap.respawn;
     // 100 StochasticIntervalEpisodeEnding
     const bool cont = episode_continues(T, n, episode, k0, k1);
     // 4 AllNonselfCumulants:getCumulants (clean_up/components.lua:535-545); 2 GlobalData reset.
@@ -210,14 +232,14 @@ struct CleanUp {
       int eater = -1;
       if (grows) {
         sc.apple[k] = (sc.apple[k] & ~4) | 1;
-        int o = sc.occ[T.apple[k * 3 + 1]];
+        int o = sc.occ[F.apple[k * 3 + 1]];
         if (o >= 1 && o <= T.P) { eater = o - 1; sc.apple[k] |= 2; }
       }
       unsigned m = __ballot_sync(MP_FULL, eater >= 0);
       while (m) {  // in apple (object) order
         int src = __ffs(m) - 1; m &= m - 1;
         int e = __shfl_sync(MP_FULL, eater, src);
-        if (lane == e) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, e + 1, 0); }
+        if (lane == e) { reward += F.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, e + 1, 0); }
         ate_now |= 1u << e;
       }
     }
@@ -228,7 +250,7 @@ struct CleanUp {
       const bool ate = ai >= 0 && (sc.apple[ai] & 1);
       __syncwarp();
       if (ate && lane == 0) sc.apple[ai] |= 2;
-      if (ate && lane == src) { reward += T.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, src + 1, 0); }
+      if (ate && lane == src) { reward += F.eat_reward; emit_event(S, b, EV_EDIBLE_CONSUMED, src + 1, 0); }
       if (ate) ate_now |= 1u << src;
     };
     // (c) turns and moves, avatar by avatar in this frame's order.
@@ -236,7 +258,7 @@ struct CleanUp {
     // (d) zap beams, then (e) clean beams, shooter by shooter.
     unsigned zapped = 0;
     for (int pass = 0; pass < 2; ++pass) {
-      const BeamGeom& G = pass == 0 ? T.zap_geom : T.clean_geom;
+      const BeamGeom& G = beams(T, sc)[pass];
       for (int r = 0; r < T.P; ++r) {
         unsigned m = __ballot_sync(MP_FULL, is_av && rank == r && (pass == 0 ? fire_zap : fire_clean));
         if (!m) continue;
@@ -246,7 +268,7 @@ struct CleanUp {
         int hit_avatar = -1, hit_dirt = -1;
       bool blocked = cell < 0 && lane < G.n;  // off the map
         if (cell >= 0) {
-          int hit = pass == 0 ? T.zap_hit : T.clean_hit;
+          int hit = pass == 0 ? F.zap.hit : F.clean_hit;
           if (sc.flags[cell] & (1 << hit)) blocked = true;  // BeamBlocker:onHit
           if (pass == 0) {
             int o = sc.occ[cell];
@@ -264,9 +286,9 @@ struct CleanUp {
           while (hm) {
             int c = __ffs(hm) - 1; hm &= hm - 1;
             int t = __shfl_sync(MP_FULL, hit_avatar, c);
-            if (lane == t) reward += T.zap_penalty;   // zapped avatar is still alive in this round
-            if (lane == src) { reward += T.zap_reward; emit_event(S, b, EV_ZAP, src + 1, t + 1); }
-            if (T.zap_remove) zapped |= 1u << t;
+            if (lane == t) reward += F.zap.penalty;   // zapped avatar is still alive in this round
+            if (lane == src) { reward += F.zap.reward; emit_event(S, b, EV_ZAP, src + 1, t + 1); }
+            if (F.zap.remove) zapped |= 1u << t;
           }
         } else {
           bool cleaned = vis && hit_dirt >= 0;
@@ -274,8 +296,8 @@ struct CleanUp {
           if (__any_sync(MP_FULL, cleaned)) cleaned_now |= 1u << src;  // Cleaner:setCumulant
         }
         if (vis && !blocked) {
-          draw_hit_sprite(T, grid, pass == 0 ? sc.beam_zap : sc.beam_2, pass == 0 ? T.zap_layer : T.clean_layer, cell,
-                          cell_value(pass == 0 ? T.zap_sprite : T.clean_sprite, so));
+          draw_hit_sprite(T, grid, pass == 0 ? sc.beam_zap : sc.beam_2, pass == 0 ? F.zap.layer : F.clean_layer, cell,
+                          cell_value(pass == 0 ? F.zap.sprite : F.clean_sprite, so));
           beam_dirty = 1;
         }
         __syncwarp();
@@ -293,7 +315,7 @@ struct CleanUp {
       uint8_t now = (v & 1) && !(v & 2);
       if (now != was) {
         S.apple[(size_t)b * T.nA_pad + k] = now;
-        grid[(size_t)T.apple_layer * T.cells_pad + T.apple[k * 3 + 1]] = now ? cell_value(T.apple_sprite, 0) : (uint16_t)0;
+        grid[(size_t)F.apple_layer * T.cells_pad + F.apple[k * 3 + 1]] = now ? cell_value(F.apple_sprite, 0) : (uint16_t)0;
       }
     }
     int d_delta = 0;
@@ -304,18 +326,18 @@ struct CleanUp {
       if ((v & 1) && (v & 2)) --d_delta;  // DirtTracker:onStateChange (clean_up/components.lua:118-129)
       if (now != was) {
         S.dirt[(size_t)b * T.nD_pad + j] = now;
-        grid[(size_t)T.dirt_layer * T.cells_pad + T.dirt[j * 3 + 1]] = now ? cell_value(T.dirt_sprite, 0) : (uint16_t)0;
+        grid[(size_t)F.dirt_layer * T.cells_pad + F.dirt[j * 3 + 1]] = now ? cell_value(F.dirt_sprite, 0) : (uint16_t)0;
       }
     }
     for (int o = 16; o > 0; o >>= 1) d_delta += __shfl_xor_sync(MP_FULL, d_delta, o);
     dirt_count += d_delta;
     // water Animation (component_library.lua:1070-1094): every piece flips every anim_frames frames.
-    if (n % T.anim_frames == 0) {
-      const int turn = (n / T.anim_frames) % T.n_anim;  // (uniform: the divisions are done once, not per piece)
+    if (n % F.anim_frames == 0) {
+      const int turn = (n / F.anim_frames) % F.n_anim;  // (uniform: the divisions are done once, not per piece)
       for (int k = lane; k < T.nW; k += 32) {
         int phase = (int)S.water[(size_t)b * T.nW_pad + k] + turn;
-        if (phase >= T.n_anim) phase -= T.n_anim;
-        grid[(size_t)T.water_layer * T.cells_pad + T.water[k * 2 + 1]] = cell_value(T.water_sprite[phase], 0);
+        if (phase >= F.n_anim) phase -= F.n_anim;
+        grid[(size_t)F.water_layer * T.cells_pad + F.water[k * 2 + 1]] = cell_value(F.water_sprite[phase], 0);
       }
     }
     draw_avatars(T, grid, lane, x0, y0, orient0, alive0, x, y, orient, alive);
@@ -328,7 +350,7 @@ struct CleanUp {
       for (int k = 0; k < T.n_scalar; ++k) {
         double v;
         if (T.scalar_obs[k] == 0)  // Zapper:readyToShoot (avatar_library.lua:737-744)
-          v = alive ? fmax(1.0 - (double)zap_cool / (double)T.zap_cooldown, 0.0) : 0.0;
+          v = alive ? fmax(1.0 - (double)zap_cool / (double)F.zap.cooldown, 0.0) : 0.0;
         else
           v = (double)num_others_cleaned;
         S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = v;

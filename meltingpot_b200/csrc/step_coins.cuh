@@ -14,29 +14,36 @@
 #include "step_common.cuh"
 
 struct Coins {
-  // Host: the coins tables of the blob (compiler.py _coins_tables): co_ip / co_dp and the coins, which take the place
-  // of the apples (ch_apple, apple_of_cell, apple_layer).
-  static int load(FamilyLoad& ld, Tables& T) {
+  struct Params {
+    int coin_layer;
+    int coin_sprite[2];           // sprite of coin type 0 / 1 (liveStateA / liveStateB)
+    int coin_type[2];             // PlayerCoinType of each player
+    double coin_reward[2][4];     // per collecting player: self match, self mismatch, other match, other mismatch
+    double coin_rate;             // ChoiceCoinRegrow regrowRate
+    int terminate, terminate_n;   // the episode ends once a player has collected terminate_n coins (if terminate)
+    const int32_t* coin;          // [nA][2] obj id, cell
+    const int16_t* coin_of_cell;  // [cells_pad] coin index or -1
+  };
+
+  // Host: the coins tables of the blob (compiler.py _coins_tables): co_ip / co_dp and the coins.
+  static int load(FamilyLoad& ld, const Tables& T, Params& F) {
     const int32_t* ip;
     const double* dp;
     Section<int32_t> coin;
     int rc;
     if ((rc = ld.params("co", MPB_CO_I_COUNT, MPB_CO_D_COUNT, &ip, &dp)) || (rc = ld.need("co_coin", MPB_I32, &coin))) return rc;
     if (T.P != 2) return fail(MP_E_UNSUPPORTED, "coins needs exactly two players (got %d)", T.P);
-    T.nA = ip[MPB_CO_I_N_COINS]; T.apple_layer = ip[MPB_CO_I_COIN_LAYER];
-    T.coin_sprite[0] = ip[MPB_CO_I_COIN_SPRITE_0]; T.coin_sprite[1] = ip[MPB_CO_I_COIN_SPRITE_1];
-    T.coin_terminate = ip[MPB_CO_I_TERMINATE]; T.coin_terminate_n = ip[MPB_CO_I_TERMINATE_N];
-    T.end_min_frames = ip[MPB_CO_I_END_MIN_FRAMES]; T.end_interval = ip[MPB_CO_I_END_INTERVAL];
-    T.coin_type[0] = ip[MPB_CO_I_COIN_TYPE_0]; T.coin_type[1] = ip[MPB_CO_I_COIN_TYPE_1];
-    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d coins (max 2048)", T.nA);
-    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
-    T.coin_rate = dp[MPB_CO_D_REGROW_RATE]; T.end_prob = dp[MPB_CO_D_END_PROB];
-    for (int p = 0; p < 2; ++p) for (int k = 0; k < 4; ++k) T.coin_reward[p][k] = dp[MPB_CO_D_REWARD_0_SELF_MATCH + 4 * p + k];
-    T.zap_layer = 0; T.zap_cooldown = 1;
-    std::vector<int32_t> v_apple((size_t)T.nA * 4);  // ch_apple rows: obj id, cell, 0, -1
-    for (int k = 0; k < T.nA; ++k) { v_apple[k * 4] = coin.data[k * 2]; v_apple[k * 4 + 1] = coin.data[k * 2 + 1]; v_apple[k * 4 + 2] = 0; v_apple[k * 4 + 3] = -1; }
-    if ((rc = upload(ld.allocs, v_apple, &T.ch_apple))) return rc;
-    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 4 + 1]);
+    ld.nA = ip[MPB_CO_I_N_COINS]; F.coin_layer = ip[MPB_CO_I_COIN_LAYER];
+    F.coin_sprite[0] = ip[MPB_CO_I_COIN_SPRITE_0]; F.coin_sprite[1] = ip[MPB_CO_I_COIN_SPRITE_1];
+    F.terminate = ip[MPB_CO_I_TERMINATE]; F.terminate_n = ip[MPB_CO_I_TERMINATE_N];
+    ld.end_min_frames = ip[MPB_CO_I_END_MIN_FRAMES]; ld.end_interval = ip[MPB_CO_I_END_INTERVAL];
+    F.coin_type[0] = ip[MPB_CO_I_COIN_TYPE_0]; F.coin_type[1] = ip[MPB_CO_I_COIN_TYPE_1];
+    if (ld.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d coins (max 2048)", ld.nA);
+    if (ld.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
+    F.coin_rate = dp[MPB_CO_D_REGROW_RATE]; ld.end_prob = dp[MPB_CO_D_END_PROB];
+    for (int p = 0; p < 2; ++p) for (int k = 0; k < 4; ++k) F.coin_reward[p][k] = dp[MPB_CO_D_REWARD_0_SELF_MATCH + 4 * p + k];
+    std::vector<int32_t> v_coin(coin.data, coin.data + coin.count);
+    if ((rc = upload(ld.allocs, v_coin, &F.coin)) || (rc = upload_cell_index(ld, T, "co_coin", coin, ld.nA, 2, &F.coin_of_cell))) return rc;
     return MP_OK;
   }
 
@@ -44,11 +51,11 @@ struct Coins {
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
-  __device__ static void stage(const Tables&, uint8_t*) {}
+  __device__ static void stage(const Tables&, const Params&, uint8_t*) {}
   __device__ static WarpScratch carve(const Tables& T, uint8_t* base, const uint8_t*) { return carve_scratch(T, base); }
 
   // Episode start for coins: every coin waits, the two avatars draw their spawn points (policy A.10).
-  __device__ static void reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
+  __device__ static void reset(const Tables& T, const Params& F, const State& S, int b, int lane, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
     __syncwarp();
     copy_init_grid(T, grid, lane);
@@ -62,17 +69,17 @@ struct Coins {
     // api:start ends with one grid:update (api_factory.lua:101): the ChoiceCoinRegrow updaters already fire at frame 0.
     // (Spawn points are not coin cells, so no avatar can be standing on a coin that appears now.)
     for (int k = lane; k < T.nA; k += 32) {
-      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-      if (u01(w.x, w.y) < T.coin_rate) {
+      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)F.coin[k * 2], RS_OBJECT, k0, k1);
+      if (u01(w.x, w.y) < F.coin_rate) {
         const int type = (int)pick(w.z, 2u);
         S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)(1 + type);
-        grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = cell_value(T.coin_sprite[type], 0);
+        grid[(size_t)F.coin_layer * T.cells_pad + F.coin[k * 2 + 1]] = cell_value(F.coin_sprite[type], 0);
       }
     }
     reset_env_row(T, S, b, lane, episode, 0);
   }
 
-  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
     const bool is_av = lane < T.P;
     uint8_t* s_state = sc.apple;  // [nA_pad] bits 0-1 state code, bits 4-5 state queued by ChoiceCoinRegrow, bit 6 collected
@@ -100,20 +107,20 @@ struct Coins {
     cont = episode_continues(T, n, episode, k0, k1);
     for (int k = lane; k < T.nA; k += 32) {
       if ((s_state[k] & 3) != 0) continue;
-      uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-      if (u01(w.x, w.y) < T.coin_rate) s_state[k] |= (uint8_t)((1 + pick(w.z, 2u)) << 4);
+      uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)F.coin[k * 2], RS_OBJECT, k0, k1);
+      if (u01(w.x, w.y) < F.coin_rate) s_state[k] |= (uint8_t)((1 + pick(w.z, 2u)) << 4);
     }
     __syncwarp();
 
     // Coin:onEnter for collector `who` on coin `k` (every lane calls this with the same arguments).
     auto collect = [&](int who, int k) {
       const int type = (s_state[k] & 3) - 1;
-      const bool match = type == T.coin_type[who];
-      const double* R = T.coin_reward[who];  // self match, self mismatch, other match, other mismatch (Role multipliers folded in)
+      const bool match = type == F.coin_type[who];
+      const double* R = F.coin_reward[who];  // self match, self mismatch, other match, other mismatch (Role multipliers folded in)
       if (lane == who) {
         reward += match ? R[0] : R[1];
         ++cumulative;
-        if (T.coin_terminate && cumulative >= T.coin_terminate_n) cont = false;
+        if (F.terminate && cumulative >= F.terminate_n) cont = false;
         emit_event(S, b, EV_COIN_CONSUMED, who + 1, match ? 1 : 0);
       } else if (is_av) {  // Coin:rewardOthers (:74-85) and PartnerTracker:reportMatch / reportMismatch (:324-330)
         reward += match ? R[2] : R[3];
@@ -127,7 +134,7 @@ struct Coins {
     // ---- round 1: moves in the frame's order, then the queued coin states in object order -----------------
     // policy A.5: `enter` fires on the final cell, moved or blocked
     move_avatars(T, lane, rank, true, act_turn, act_move, x, y, orient, sc.occ, [&](int src, int cell) {
-      const int ci = T.apple_of_cell[cell];
+      const int ci = F.coin_of_cell[cell];
       if (ci >= 0 && (s_state[ci] & 3) != 0 && !(s_state[ci] & 64)) collect(src, ci);
     });
     const int partner_cont = __all_sync(MP_FULL, cont);  // (cont is per lane so far: either collector may end the episode)
@@ -138,7 +145,7 @@ struct Coins {
       if (queued) s_state[k] = (uint8_t)queued;  // now live (placed on superOverlay)
       __syncwarp();
       // a coin that appears under a standing avatar is entered at once (contact is symmetric on placement, policy A.5)
-      const int o = queued ? sc.occ[T.ch_apple[k * 4 + 1]] : 0;
+      const int o = queued ? sc.occ[F.coin[k * 2 + 1]] : 0;
       unsigned gm = __ballot_sync(MP_FULL, o >= 1 && o <= T.P);
       while (gm) {
         const int c = __ffs(gm) - 1; gm &= gm - 1;
@@ -153,7 +160,7 @@ struct Coins {
       const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
       if (now != was) {
         S.apple[(size_t)b * T.nA_pad + k] = now;
-        grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = now ? cell_value(T.coin_sprite[now - 1], 0) : (uint16_t)0;
+        grid[(size_t)F.coin_layer * T.cells_pad + F.coin[k * 2 + 1]] = now ? cell_value(F.coin_sprite[now - 1], 0) : (uint16_t)0;
       }
     }
     draw_avatars(T, grid, lane, x0, y0, orient0, 1, x, y, orient, 1);

@@ -53,11 +53,13 @@ __host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * 
 // mode 0: step (envs whose last step was LAST start a new episode instead, policy A.17)
 // mode 1: reset envs selected by `mask` (all if null)
 //
-// A Family provides: the host-side load(FamilyLoad&, T) that decodes its blob sections (family_load.h), Scratch,
-// kStagesTables, scratch_bytes(T) per warp, table_bytes(T) per CTA, stage(T, tables) (copies static tables into shared
-// memory), carve(T, warp_base, tables), reset(T, S, b, lane, sc) and step(T, S, b, lane, actions, sc).
+// A Family provides: Params (what only its kernel reads), the host-side load(FamilyLoad&, T, Params&) that decodes its
+// blob sections (family_load.h), Scratch, kStagesTables, scratch_bytes(T) per warp, table_bytes(T) per CTA,
+// stage(T, F, tables) (copies static tables into shared memory), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
+// and step(T, F, S, b, lane, actions, sc). F is a grid constant: without it, the compiler copies a small Params that is
+// indexed with a run-time value (coins' coin_reward[who], coop_mining's ore_sprite[state]) to the stack.
 template <class Family>
-__global__ void __launch_bounds__(128, 8) k_step(Tables T, State S, const int32_t* __restrict__ actions,
+__global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant__ typename Family::Params F, State S, const int32_t* __restrict__ actions,
                                                  const uint8_t* __restrict__ mask, int mode) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -65,7 +67,7 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, State S, const int32_
   // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   uint8_t* tables = smem + 4 * Family::scratch_bytes(T);
-  if constexpr (Family::kStagesTables) Family::stage(T, tables);  // before the dependency wait: the tables never change
+  if constexpr (Family::kStagesTables) Family::stage(T, F, tables);  // before the dependency wait: the tables never change
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if constexpr (Family::kStagesTables) __syncthreads();
   const int b = blockIdx.x * 4 + warp;
@@ -73,8 +75,8 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, State S, const int32_
   typename Family::Scratch sc = Family::carve(T, smem + warp * Family::scratch_bytes(T), tables);
   if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
     event_begin(lane);
-    if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, S, b, lane, sc);
-    else Family::step(T, S, b, lane, actions, sc);
+    if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, F, S, b, lane, sc);
+    else Family::step(T, F, S, b, lane, actions, sc);
     event_end(S, b, lane);
   }
 }

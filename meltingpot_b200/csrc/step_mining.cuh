@@ -23,32 +23,40 @@
 #include "step_common.cuh"
 
 struct Mining {
-  // Host: the coop_mining tables of the blob (compiler.py _mining_tables): cm_ip / cm_dp and the ores, which take the
-  // place of the apples (ch_apple, apple_of_cell, apple_layer); the mine beam takes the place of the zapper (zap_*).
-  static int load(FamilyLoad& ld, Tables& T) {
+  struct Params {
+    int ore_layer;
+    int ore_sprite[4];            // wait, single-miner raw, two-miner raw, two-miner partial
+    int mine_window;              // frames a partly mined two-miner ore waits for its second miner
+    int mine_cooldown, mine_length, mine_layer, mine_sprite, mine_hit;  // MineBeam
+    double mine_rate[2];          // FixedRateRegrow liveRates
+    double mine_reward[2], extract_reward[2];  // per ore type (1 miner, 2 miners)
+    const int32_t* ore;           // [nA][2] obj id, cell
+    const int16_t* ore_of_cell;   // [cells_pad] ore index or -1
+  };
+
+  // Host: the coop_mining tables of the blob (compiler.py _mining_tables): cm_ip / cm_dp and the ores.
+  static int load(FamilyLoad& ld, const Tables& T, Params& F) {
     const int32_t* ip;
     const double* dp;
     Section<int32_t> ore;
     int rc;
     if ((rc = ld.params("cm", MPB_CM_I_COUNT, MPB_CM_D_COUNT, &ip, &dp)) || (rc = ld.need("cm_ore", MPB_I32, &ore))) return rc;
-    T.nA = ip[MPB_CM_I_N_ORES]; T.apple_layer = ip[MPB_CM_I_ORE_LAYER];
-    for (int i = 0; i < 4; ++i) T.ore_sprite[i] = ip[MPB_CM_I_ORE_SPRITE_0 + i];
-    T.mine_window = ip[MPB_CM_I_MINE_WINDOW]; T.zap_cooldown = ip[MPB_CM_I_MINE_COOLDOWN]; T.mine_length = ip[MPB_CM_I_MINE_LENGTH];
-    T.zap_layer = ip[MPB_CM_I_MINE_LAYER]; T.zap_sprite = ip[MPB_CM_I_MINE_SPRITE];
-    T.end_min_frames = ip[MPB_CM_I_END_MIN_FRAMES]; T.end_interval = ip[MPB_CM_I_END_INTERVAL]; T.zap_hit = ip[MPB_CM_I_MINE_HIT];
+    ld.nA = ip[MPB_CM_I_N_ORES]; F.ore_layer = ip[MPB_CM_I_ORE_LAYER];
+    for (int i = 0; i < 4; ++i) F.ore_sprite[i] = ip[MPB_CM_I_ORE_SPRITE_0 + i];
+    F.mine_window = ip[MPB_CM_I_MINE_WINDOW]; F.mine_cooldown = ip[MPB_CM_I_MINE_COOLDOWN]; F.mine_length = ip[MPB_CM_I_MINE_LENGTH];
+    F.mine_layer = ip[MPB_CM_I_MINE_LAYER]; F.mine_sprite = ip[MPB_CM_I_MINE_SPRITE];
+    ld.end_min_frames = ip[MPB_CM_I_END_MIN_FRAMES]; ld.end_interval = ip[MPB_CM_I_END_INTERVAL]; F.mine_hit = ip[MPB_CM_I_MINE_HIT];
     if (T.P > 8) return fail(MP_E_UNSUPPORTED, "coop_mining with %d players (max 8: miners are kept as a bit mask)", T.P);
-    if (T.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d ores (max 2048)", T.nA);
-    if (T.zap_cooldown < 1 || T.mine_window < 1 || T.mine_window > 255 || T.mine_length < 1) return fail(MP_E_UNSUPPORTED, "MineBeam / Ore parameters out of range");
-    if (T.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
-    if (T.zap_hit < 0 || T.zap_hit > 7) return fail(MP_E_UNSUPPORTED, "mine hit id %d", T.zap_hit);
-    if (!beam_fits_torus(T, T.mine_length, 0)) return fail(MP_E_UNSUPPORTED, "mine beam (length %d) does not fit the %dx%d TORUS map", T.mine_length, T.W, T.H);
-    T.mine_rate[0] = dp[MPB_CM_D_RATE_0]; T.mine_rate[1] = dp[MPB_CM_D_RATE_1]; T.end_prob = dp[MPB_CM_D_END_PROB];
-    T.mine_reward[0] = dp[MPB_CM_D_MINE_REWARD_0]; T.mine_reward[1] = dp[MPB_CM_D_MINE_REWARD_1];
-    T.extract_reward[0] = dp[MPB_CM_D_EXTRACT_REWARD_0]; T.extract_reward[1] = dp[MPB_CM_D_EXTRACT_REWARD_1];
-    std::vector<int32_t> v_apple((size_t)T.nA * 4);  // ch_apple rows: obj id, cell, 0, -1
-    for (int k = 0; k < T.nA; ++k) { v_apple[k * 4] = ore.data[k * 2]; v_apple[k * 4 + 1] = ore.data[k * 2 + 1]; v_apple[k * 4 + 2] = 0; v_apple[k * 4 + 3] = -1; }
-    if ((rc = upload(ld.allocs, v_apple, &T.ch_apple))) return rc;
-    for (int k = 0; k < T.nA; ++k) ld.apple_cells.push_back(v_apple[k * 4 + 1]);
+    if (ld.nA > 2048) return fail(MP_E_UNSUPPORTED, "%d ores (max 2048)", ld.nA);
+    if (F.mine_cooldown < 1 || F.mine_window < 1 || F.mine_window > 255 || F.mine_length < 1) return fail(MP_E_UNSUPPORTED, "MineBeam / Ore parameters out of range");
+    if (ld.end_interval < 1) return fail(MP_E_INVALID, "episode interval < 1");
+    if (F.mine_hit < 0 || F.mine_hit > 7) return fail(MP_E_UNSUPPORTED, "mine hit id %d", F.mine_hit);
+    if (!beam_fits_torus(T, F.mine_length, 0)) return fail(MP_E_UNSUPPORTED, "mine beam (length %d) does not fit the %dx%d TORUS map", F.mine_length, T.W, T.H);
+    F.mine_rate[0] = dp[MPB_CM_D_RATE_0]; F.mine_rate[1] = dp[MPB_CM_D_RATE_1]; ld.end_prob = dp[MPB_CM_D_END_PROB];
+    F.mine_reward[0] = dp[MPB_CM_D_MINE_REWARD_0]; F.mine_reward[1] = dp[MPB_CM_D_MINE_REWARD_1];
+    F.extract_reward[0] = dp[MPB_CM_D_EXTRACT_REWARD_0]; F.extract_reward[1] = dp[MPB_CM_D_EXTRACT_REWARD_1];
+    std::vector<int32_t> v_ore(ore.data, ore.data + ore.count);
+    if ((rc = upload(ld.allocs, v_ore, &F.ore)) || (rc = upload_cell_index(ld, T, "cm_ore", ore, ld.nA, 2, &F.ore_of_cell))) return rc;
     return MP_OK;
   }
 
@@ -56,11 +64,11 @@ struct Mining {
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
-  __device__ static void stage(const Tables&, uint8_t*) {}
+  __device__ static void stage(const Tables&, const Params&, uint8_t*) {}
   __device__ static WarpScratch carve(const Tables& T, uint8_t* base, const uint8_t*) { return carve_scratch(T, base); }
 
   // Episode start: the avatars draw their spawn points (policy A.10); MineBeam:start (:254-261) leaves them ready to shoot.
-  __device__ static void reset(const Tables& T, const State& S, int b, int lane, WarpScratch& sc) {
+  __device__ static void reset(const Tables& T, const Params& F, const State& S, int b, int lane, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
     __syncwarp();
     copy_init_grid(T, grid, lane);
@@ -77,19 +85,19 @@ struct Mining {
     // api:start ends with one grid:update (api_factory.lua:101): the FixedRateRegrow updaters already fire at frame 0
     // (the component updates do not run then). Spawn points are not ore cells; the avatar check is kept for symmetry.
     for (int k = lane; k < T.nA; k += 32) {
-      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-      const bool first = u01(w.x, w.y) < T.mine_rate[0], second = u01(w.z, w.w) < T.mine_rate[1];
-      const int cell = T.ch_apple[k * 4 + 1];
+      uint4 w = philox4x32_10(0u, (uint32_t)episode, (uint32_t)F.ore[k * 2], RS_OBJECT, k0, k1);
+      const bool first = u01(w.x, w.y) < F.mine_rate[0], second = u01(w.z, w.w) < F.mine_rate[1];
+      const int cell = F.ore[k * 2 + 1];
       if ((first || second) && grid[(size_t)T.avatar_layer * T.cells_pad + cell] == 0) {
         const int now = second ? 2 : 1;
         S.apple[(size_t)b * T.nA_pad + k] = (uint8_t)now;
-        grid[(size_t)T.apple_layer * T.cells_pad + cell] = cell_value(T.ore_sprite[now], 0);
+        grid[(size_t)F.ore_layer * T.cells_pad + cell] = cell_value(F.ore_sprite[now], 0);
       }
     }
     reset_env_row(T, S, b, lane, episode, 0);
   }
 
-  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
     const bool is_av = lane < T.P;
     // bits 0-1 state code; bits 2-3 state set in round 1 (1 single-miner ore, 2 two-miner ore; by a reset or by
@@ -111,13 +119,13 @@ struct Mining {
     for (int i = lane; i < words; i += 32) sc.beam_zap[i] = 0;
     __syncwarp();
     if (is_av) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
-    if (env[ENV_BEAM]) clear_layer(T, grid, T.zap_layer, lane);
+    if (env[ENV_BEAM]) clear_layer(T, grid, F.mine_layer, lane);
     __syncwarp();
 
     // ---- component updates -----------------------------------------------------------------------------
     // MineBeam:update (:236-252): cool down, then fire if asked to and ready.
     bool fire = false;
-    if (is_av) { if (cool > 0) --cool; if (act_mine == 1 && cool == 0) { cool = T.zap_cooldown; fire = true; } }
+    if (is_av) { if (cool > 0) --cool; if (act_mine == 1 && cool == 0) { cool = F.mine_cooldown; fire = true; } }
     // Ore:update (:104-109): the window of a partly mined ore runs out -> reset: forget the miners, back to raw.
     for (int k = lane; k < T.nA; k += 32) {
       if (cd[k] > 0 && --cd[k] == 0) {
@@ -130,9 +138,9 @@ struct Mining {
     // (positions as the frame started); if both fire the second setState wins.
     for (int k = lane; k < T.nA; k += 32) {
       if ((s_state[k] & 3) != 0) continue;
-      uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)T.ch_apple[k * 4], RS_OBJECT, k0, k1);
-      const bool first = u01(w.x, w.y) < T.mine_rate[0], second = u01(w.z, w.w) < T.mine_rate[1];
-      if ((first || second) && sc.occ[T.ch_apple[k * 4 + 1]] == 0) s_state[k] |= (second ? 2 : 1) << 2;
+      uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)F.ore[k * 2], RS_OBJECT, k0, k1);
+      const bool first = u01(w.x, w.y) < F.mine_rate[0], second = u01(w.z, w.w) < F.mine_rate[1];
+      if ((first || second) && sc.occ[F.ore[k * 2 + 1]] == 0) s_state[k] |= (second ? 2 : 1) << 2;
     }
     // 150 Avatar movement: the frame's random visiting order (policy A.7).
     const int rank = visit_rank(T, lane, n, episode, k0, k1);
@@ -145,19 +153,19 @@ struct Mining {
     for (int src = 0; src < T.P; ++src) {
       if (!__shfl_sync(MP_FULL, (int)fire, src)) continue;
       const int sx = __shfl_sync(MP_FULL, x, src), sy = __shfl_sync(MP_FULL, y, src), so = __shfl_sync(MP_FULL, orient, src);
-      for (int i = 1; i <= T.mine_length; ++i) {  // radius 0: one ray (every lane walks it)
+      for (int i = 1; i <= F.mine_length; ++i) {  // radius 0: one ray (every lane walks it)
         int cx = sx + dir_dx(so) * i, cy = sy + dir_dy(so) * i;
         if (!wrap_or_reject(T, cx, cy)) break;
         const int cell = cy * T.W + cx;
-        bool blocked = (T.cell_flags[cell] >> T.zap_hit) & 1;  // BeamBlocker 'mine' (walls)
-        const int k = T.apple_of_cell[cell];
+        bool blocked = (T.cell_flags[cell] >> F.mine_hit) & 1;  // BeamBlocker 'mine' (walls)
+        const int k = F.ore_of_cell[cell];
         const int st = k >= 0 ? (s_state[k] & 3) : 0;
         if (st != 0) {  // Ore:onHit (:118-150): a raw or partial ore takes the hit and stops the beam
           blocked = true;
           if (st == 1) {
             // single-miner ore: mined and extracted by the same hit; partial, raw (reset), wait are queued -> wait
             if (lane == src) {
-              reward += T.mine_reward[0] + T.extract_reward[0];
+              reward += F.mine_reward[0] + F.extract_reward[0];
               emit_event(S, b, EV_MINING, src + 1, 1);
               emit_event(S, b, EV_EXTRACTION, src + 1, 1);
             }
@@ -165,10 +173,10 @@ struct Mining {
             if (lane == 0) s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (2 << 4));
           } else {
             const unsigned miners = s_miners[k] | (1u << src);  // Ore:addMiner (:110-114)
-            if (lane == src) { reward += T.mine_reward[1]; emit_event(S, b, EV_MINING, src + 1, 2); }
+            if (lane == src) { reward += F.mine_reward[1]; emit_event(S, b, EV_MINING, src + 1, 2); }
             if (__popc(miners) == 2) {  // enough miners: both extract, then Ore:reset and the wait state
               if (is_av && ((miners >> lane) & 1u)) {
-                reward += T.extract_reward[1];
+                reward += F.extract_reward[1];
                 emit_event(S, b, EV_EXTRACTION, lane + 1, 2);
                 emit_event(S, b, EV_EXTRACTION_PAIR, lane + 1, (__ffs(miners & ~(1u << lane))) | (2 << 8));
               }
@@ -176,15 +184,15 @@ struct Mining {
               if (lane == 0) { s_miners[k] = 0; cd[k] = 0; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (2 << 4)); }
             } else {
               __syncwarp();
-              if (lane == 0) { s_miners[k] = (uint8_t)miners; cd[k] = (uint8_t)T.mine_window; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (1 << 4)); }
+              if (lane == 0) { s_miners[k] = (uint8_t)miners; cd[k] = (uint8_t)F.mine_window; s_state[k] = (uint8_t)((s_state[k] & ~(3 << 4)) | (1 << 4)); }
             }
           }
           __syncwarp();
         }
         if (blocked) break;
-        if (lane == 0 && grid[(size_t)T.zap_layer * T.cells_pad + cell] == 0 && !((sc.beam_zap[cell >> 5] >> (cell & 31)) & 1u)) {
+        if (lane == 0 && grid[(size_t)F.mine_layer * T.cells_pad + cell] == 0 && !((sc.beam_zap[cell >> 5] >> (cell & 31)) & 1u)) {
           sc.beam_zap[cell >> 5] |= 1u << (cell & 31);
-          grid[(size_t)T.zap_layer * T.cells_pad + cell] = cell_value(T.zap_sprite, so);
+          grid[(size_t)F.mine_layer * T.cells_pad + cell] = cell_value(F.mine_sprite, so);
         }
         beam_dirty = 1;
         __syncwarp();
@@ -206,7 +214,7 @@ struct Mining {
       const uint8_t was = S.apple[(size_t)b * T.nA_pad + k];
       if (now != was) {
         S.apple[(size_t)b * T.nA_pad + k] = now;
-        grid[(size_t)T.apple_layer * T.cells_pad + T.ch_apple[k * 4 + 1]] = cell_value(T.ore_sprite[now], 0);
+        grid[(size_t)F.ore_layer * T.cells_pad + F.ore[k * 2 + 1]] = cell_value(F.ore_sprite[now], 0);
       }
       S.dirt[(size_t)b * T.nD_pad + k] = s_miners[k];
     }
@@ -217,7 +225,7 @@ struct Mining {
       *reinterpret_cast<int4*>(S.avatar + ((size_t)b * T.P + lane) * 4) = make_int4(x, y, orient, 1);
       S.av_timer[((size_t)b * T.P + lane) * 4] = cool;
       for (int k = 0; k < T.n_scalar; ++k)  // READY_TO_SHOOT = MineBeam:readyToShoot (:186-189)
-        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 - (double)cool / (double)T.zap_cooldown : 0.0;
+        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = T.scalar_obs[k] == 0 ? 1.0 - (double)cool / (double)F.mine_cooldown : 0.0;
     }
     store_timestep(T, S, b, lane, n, reward, done ? 2 : 1, beam_dirty);
   }

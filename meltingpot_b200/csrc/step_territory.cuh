@@ -77,16 +77,31 @@ __device__ __forceinline__ TerritoryScratch carve_territory(const Tables& T, uin
   return s;
 }
 
-__device__ __forceinline__ uint16_t resource_sprite_value(const Tables& T, int state) {
-  if (state == 0) return cell_value(T.unclaimed_sprite, 0);
-  if (state == 1) return 0;
-  return cell_value(T.claimed_sprite[state - 2], 0);
-}
-
 struct Territory {
+  struct Params {
+    Zapper zap;
+    int res_layer, unclaimed_sprite, tex_layer, tex_sprite, ind_layer, dmg_layer, dmg_sprite, mark_layer;
+    int mark_initial_level, mark_recovery, mark_n_levels, mark_inc[3], mark_remove[3], mark_freeze[3], mark_sprite[3];
+    double mark_src_reward[3], mark_tgt_reward[3];
+    int claim_wait, brush_layer, claim_layer, res_health0, res_reward_delay, res_repair_delay, tr_taste_role;
+    double res_reward, res_rate, res_repair_prob;
+    int claimed_sprite[MP_MAX_PLAYERS], dry_sprite[MP_MAX_PLAYERS], brush_sprite[MP_MAX_PLAYERS], claimbeam_sprite[MP_MAX_PLAYERS];
+    BeamGeom claim_geom, brush_geom;
+    const int32_t* tr_res;       // [nR][3] obj id, cell, initial state
+    const int16_t* res_of_cell;  // [cells_pad] resource index or -1
+    const uint8_t* wall;         // [cells_pad] 1 where an AllBeamBlocker piece stands
+    const int32_t* tr_res_cond;  // [nR][2] (group or -1, ticket mask) of each resource ('choice' prefabs, Tables::choice_n), or null
+  };
+
+  __device__ __forceinline__ static uint16_t resource_sprite_value(const Params& F, int state) {
+    if (state == 0) return cell_value(F.unclaimed_sprite, 0);
+    if (state == 1) return 0;
+    return cell_value(F.claimed_sprite[state - 2], 0);
+  }
+
   // Host: the territory tables of the blob (compiler.py _territory_tables): tr_ip / tr_dp, resources, per-player
   // sprites, walls and the 'choice' conditions of the resources.
-  static int load(FamilyLoad& ld, Tables& T) {
+  static int load(FamilyLoad& ld, const Tables& T, Params& F) {
     const int32_t* ip;
     const double* dp;
     Section<int32_t> res, player_sprites;
@@ -95,58 +110,58 @@ struct Territory {
     if ((rc = ld.params("tr", MPB_TR_I_COUNT, MPB_TR_D_COUNT, &ip, &dp)) || (rc = ld.need("tr_res", MPB_I32, &res)) ||
         (rc = ld.need("tr_player_sprites", MPB_I32, &player_sprites)) || (rc = ld.need("tr_wall", MPB_U8, &wall_sec)))
       return rc;
-    T.nR = ip[MPB_TR_I_N_RES]; T.nR_pad = round_up(std::max(T.nR, 64), 16);
-    T.res_layer = ip[MPB_TR_I_RES_LAYER]; T.unclaimed_sprite = ip[MPB_TR_I_UNCLAIMED_SPRITE];
-    T.tex_layer = ip[MPB_TR_I_TEX_LAYER]; T.tex_sprite = ip[MPB_TR_I_TEX_SPRITE]; T.ind_layer = ip[MPB_TR_I_IND_LAYER];
-    T.dmg_layer = ip[MPB_TR_I_DMG_LAYER]; T.dmg_sprite = ip[MPB_TR_I_DMG_SPRITE]; T.mark_layer = ip[MPB_TR_I_MARK_LAYER];
-    T.mark_initial_level = ip[MPB_TR_I_MARK_INITIAL_LEVEL]; T.mark_recovery = ip[MPB_TR_I_MARK_RECOVERY];
-    T.mark_n_levels = ip[MPB_TR_I_MARK_N_LEVELS];
-    if (T.res_layer != T.avatar_layer) return fail(MP_E_UNSUPPORTED, "territory: resources and avatars must share a layer");
-    if (T.mark_n_levels < 1 || T.mark_n_levels > 3) return fail(MP_E_UNSUPPORTED, "%d marking levels (1..3)", T.mark_n_levels);
-    if ((rc = load_zapper(ld, T, ip))) return rc;
-    if (T.zap_respawn <= T.max_frames) return fail(MP_E_UNSUPPORTED, "territory kernel assumes avatars never respawn (framesTillRespawn %d)", T.zap_respawn);
+    ld.nR = ip[MPB_TR_I_N_RES]; ld.nR_pad = round_up(std::max(ld.nR, 64), 16);
+    F.res_layer = ip[MPB_TR_I_RES_LAYER]; F.unclaimed_sprite = ip[MPB_TR_I_UNCLAIMED_SPRITE];
+    F.tex_layer = ip[MPB_TR_I_TEX_LAYER]; F.tex_sprite = ip[MPB_TR_I_TEX_SPRITE]; F.ind_layer = ip[MPB_TR_I_IND_LAYER];
+    F.dmg_layer = ip[MPB_TR_I_DMG_LAYER]; F.dmg_sprite = ip[MPB_TR_I_DMG_SPRITE]; F.mark_layer = ip[MPB_TR_I_MARK_LAYER];
+    F.mark_initial_level = ip[MPB_TR_I_MARK_INITIAL_LEVEL]; F.mark_recovery = ip[MPB_TR_I_MARK_RECOVERY];
+    F.mark_n_levels = ip[MPB_TR_I_MARK_N_LEVELS];
+    if (F.res_layer != T.avatar_layer) return fail(MP_E_UNSUPPORTED, "territory: resources and avatars must share a layer");
+    if (F.mark_n_levels < 1 || F.mark_n_levels > 3) return fail(MP_E_UNSUPPORTED, "%d marking levels (1..3)", F.mark_n_levels);
+    if ((rc = load_zapper(ld, T, ip, dp[MPB_TR_D_ZAP_PENALTY], dp[MPB_TR_D_ZAP_REWARD], F.zap))) return rc;
+    if (F.zap.respawn <= T.max_frames) return fail(MP_E_UNSUPPORTED, "territory kernel assumes avatars never respawn (framesTillRespawn %d)", F.zap.respawn);
     const int length = ip[MPB_TR_I_CLAIM_LENGTH], radius = ip[MPB_TR_I_CLAIM_RADIUS];
-    if (!make_beam_geom(length, radius, &T.claim_geom) || !make_beam_geom(1, 0, &T.brush_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
+    if (!make_beam_geom(length, radius, &F.claim_geom) || !make_beam_geom(1, 0, &F.brush_geom)) return fail(MP_E_UNSUPPORTED, "beam footprint larger than %d cells", MP_MAX_BEAM_CELLS);
     if (!beam_fits_torus(T, length, radius)) return fail(MP_E_UNSUPPORTED, "claim beam (length %d, radius %d) does not fit the %dx%d TORUS map", length, radius, T.W, T.H);
-    T.claim_wait = ip[MPB_TR_I_CLAIM_WAIT]; T.brush_layer = ip[MPB_TR_I_BRUSH_LAYER]; T.claim_layer = ip[MPB_TR_I_CLAIM_LAYER];
-    if (T.claim_layer != T.dmg_layer) return fail(MP_E_UNSUPPORTED, "territory: claim beam layer must be the damage indicator layer");
-    T.res_health0 = ip[MPB_TR_I_RES_HEALTH]; T.res_reward_delay = ip[MPB_TR_I_RES_REWARD_DELAY];
-    T.res_repair_delay = ip[MPB_TR_I_RES_REPAIR_DELAY]; T.tr_taste_role = ip[MPB_TR_I_TASTE_ROLE];
-    if (T.tr_taste_role != 0) return fail(MP_E_UNSUPPORTED, "territory Taste roles other than 'none'");
-    if (T.res_health0 < 1 || T.res_health0 > 200) return fail(MP_E_UNSUPPORTED, "resource health %d", T.res_health0);
+    ld.beam_cells = F.zap.geom.n + F.claim_geom.n + F.brush_geom.n;
+    F.claim_wait = ip[MPB_TR_I_CLAIM_WAIT]; F.brush_layer = ip[MPB_TR_I_BRUSH_LAYER]; F.claim_layer = ip[MPB_TR_I_CLAIM_LAYER];
+    if (F.claim_layer != F.dmg_layer) return fail(MP_E_UNSUPPORTED, "territory: claim beam layer must be the damage indicator layer");
+    F.res_health0 = ip[MPB_TR_I_RES_HEALTH]; F.res_reward_delay = ip[MPB_TR_I_RES_REWARD_DELAY];
+    F.res_repair_delay = ip[MPB_TR_I_RES_REPAIR_DELAY]; F.tr_taste_role = ip[MPB_TR_I_TASTE_ROLE];
+    if (F.tr_taste_role != 0) return fail(MP_E_UNSUPPORTED, "territory Taste roles other than 'none'");
+    if (F.res_health0 < 1 || F.res_health0 > 200) return fail(MP_E_UNSUPPORTED, "resource health %d", F.res_health0);
     // the resource age and frames-since-zapped counters saturate at 65535 (see RS_AGE)
-    if (T.res_reward_delay > 65535 || T.res_repair_delay > 65535)
-      return fail(MP_E_UNSUPPORTED, "rewardDelay %d / delayTillSelfRepair %d (max 65535)", T.res_reward_delay, T.res_repair_delay);
+    if (F.res_reward_delay > 65535 || F.res_repair_delay > 65535)
+      return fail(MP_E_UNSUPPORTED, "rewardDelay %d / delayTillSelfRepair %d (max 65535)", F.res_reward_delay, F.res_repair_delay);
     const int istride = MPB_TR_I_MARK_INC_1 - MPB_TR_I_MARK_INC_0, dstride = MPB_TR_D_MARK_SRC_REWARD_1 - MPB_TR_D_MARK_SRC_REWARD_0;
-    for (int l = 0; l < T.mark_n_levels; ++l) {
+    for (int l = 0; l < F.mark_n_levels; ++l) {
       const int32_t* li = ip + istride * l;
       const double* dl = dp + dstride * l;
-      T.mark_inc[l] = li[MPB_TR_I_MARK_INC_0]; T.mark_remove[l] = li[MPB_TR_I_MARK_REMOVE_0];
-      T.mark_freeze[l] = li[MPB_TR_I_MARK_FREEZE_0]; T.mark_sprite[l] = li[MPB_TR_I_MARK_SPRITE_0];
-      T.mark_src_reward[l] = dl[MPB_TR_D_MARK_SRC_REWARD_0]; T.mark_tgt_reward[l] = dl[MPB_TR_D_MARK_TGT_REWARD_0];
+      F.mark_inc[l] = li[MPB_TR_I_MARK_INC_0]; F.mark_remove[l] = li[MPB_TR_I_MARK_REMOVE_0];
+      F.mark_freeze[l] = li[MPB_TR_I_MARK_FREEZE_0]; F.mark_sprite[l] = li[MPB_TR_I_MARK_SPRITE_0];
+      F.mark_src_reward[l] = dl[MPB_TR_D_MARK_SRC_REWARD_0]; F.mark_tgt_reward[l] = dl[MPB_TR_D_MARK_TGT_REWARD_0];
     }
-    T.res_reward = dp[MPB_TR_D_RES_REWARD]; T.res_rate = dp[MPB_TR_D_RES_RATE]; T.res_repair_prob = dp[MPB_TR_D_RES_REPAIR_PROB];
-    T.zap_penalty = dp[MPB_TR_D_ZAP_PENALTY]; T.zap_reward = dp[MPB_TR_D_ZAP_REWARD]; T.end_prob = dp[MPB_TR_D_END_PROB];
-    T.tr_taste_amount = dp[MPB_TR_D_TASTE_AMOUNT]; T.tr_taste_mult = dp[MPB_TR_D_TASTE_MULT];
+    F.res_reward = dp[MPB_TR_D_RES_REWARD]; F.res_rate = dp[MPB_TR_D_RES_RATE]; F.res_repair_prob = dp[MPB_TR_D_RES_REPAIR_PROB];
+    ld.end_prob = dp[MPB_TR_D_END_PROB];
     for (int p = 0; p < T.P; ++p) {
       const int32_t* ps = player_sprites.data + p * 4;
-      T.claimed_sprite[p] = ps[0]; T.dry_sprite[p] = ps[1]; T.brush_sprite[p] = ps[2]; T.claimbeam_sprite[p] = ps[3];
+      F.claimed_sprite[p] = ps[0]; F.dry_sprite[p] = ps[1]; F.brush_sprite[p] = ps[2]; F.claimbeam_sprite[p] = ps[3];
     }
     for (int p = 0; p < T.P; ++p) {  // wet paint on the resource texture, then dry paint on top: what most resource cells show
-      ld.hint_stacks.push_back({T.tex_sprite, T.claimed_sprite[p]});
-      ld.hint_stacks.push_back({T.tex_sprite, T.claimed_sprite[p], T.dry_sprite[p]});
+      ld.hint_stacks.push_back({F.tex_sprite, F.claimed_sprite[p]});
+      ld.hint_stacks.push_back({F.tex_sprite, F.claimed_sprite[p], F.dry_sprite[p]});
     }
     std::vector<int32_t> v_res(res.data, res.data + res.count);
-    std::vector<int16_t> res_of(T.cells_pad, -1);
-    for (int k = 0; k < T.nR; ++k) res_of[v_res[k * 3 + 1]] = (int16_t)k;
     std::vector<uint8_t> wall(T.cells_pad, 0);
     memcpy(wall.data(), wall_sec.data, std::min<size_t>(wall_sec.count, T.cells));
-    if ((rc = upload(ld.allocs, v_res, &T.tr_res)) || (rc = upload(ld.allocs, res_of, &T.res_of_cell)) || (rc = upload(ld.allocs, wall, &T.wall))) return rc;
+    if ((rc = upload(ld.allocs, v_res, &F.tr_res)) || (rc = upload_cell_index(ld, T, "tr_res", res, ld.nR, 3, &F.res_of_cell)) ||
+        (rc = upload(ld.allocs, wall, &F.wall)))
+      return rc;
     Section<int32_t> res_cond;
     if (get_section(ld.blob, ld.n, "tr_res_cond", MPB_I32, &res_cond)) {
-      if ((int)res_cond.count != T.nR * 2) return fail(MP_E_INVALID, "blob: tr_res_cond has %zu values for %d resources", res_cond.count, T.nR);
+      if ((int)res_cond.count != ld.nR * 2) return fail(MP_E_INVALID, "blob: tr_res_cond has %zu values for %d resources", res_cond.count, ld.nR);
       std::vector<int32_t> v(res_cond.data, res_cond.data + res_cond.count);
-      if ((rc = upload(ld.allocs, v, &T.tr_res_cond))) return rc;
+      if ((rc = upload(ld.allocs, v, &F.tr_res_cond))) return rc;
     }
     return MP_OK;
   }
@@ -157,13 +172,13 @@ struct Territory {
   __host__ __device__ static size_t table_bytes(const Tables& T) { return territory_table_bytes(T); }
 
   // Per-CTA tables: wall255, res_of (int16 per cell), res_cell (int16) and res_obj (int32 per resource).
-  __device__ static void stage(const Tables& T, uint8_t* tb) {
+  __device__ static void stage(const Tables& T, const Params& F, uint8_t* tb) {
     uint8_t* s_wall = tb; tb += scratch_round16(T.cells_pad);
     int16_t* s_res_of = reinterpret_cast<int16_t*>(tb); tb += scratch_round16((size_t)T.cells_pad * 2);
     int16_t* s_res_cell = reinterpret_cast<int16_t*>(tb); tb += (size_t)T.nR_pad * 2;
     int32_t* s_res_obj = reinterpret_cast<int32_t*>(tb);
-    for (int i = threadIdx.x; i < T.cells_pad; i += (int)blockDim.x) { s_wall[i] = T.wall[i] ? 255 : 0; s_res_of[i] = T.res_of_cell[i]; }
-    for (int i = threadIdx.x; i < T.nR_pad; i += (int)blockDim.x) { s_res_cell[i] = i < T.nR ? (int16_t)T.tr_res[i * 3 + 1] : (int16_t)0; s_res_obj[i] = i < T.nR ? T.tr_res[i * 3] : 0; }
+    for (int i = threadIdx.x; i < T.cells_pad; i += (int)blockDim.x) { s_wall[i] = F.wall[i] ? 255 : 0; s_res_of[i] = F.res_of_cell[i]; }
+    for (int i = threadIdx.x; i < T.nR_pad; i += (int)blockDim.x) { s_res_cell[i] = i < T.nR ? (int16_t)F.tr_res[i * 3 + 1] : (int16_t)0; s_res_obj[i] = i < T.nR ? F.tr_res[i * 3] : 0; }
   }
 
   __device__ static TerritoryScratch carve(const Tables& T, uint8_t* base, const uint8_t* tb) {
@@ -176,24 +191,24 @@ struct Territory {
   }
 
   // Raw state of a new episode (before frame 0 runs).
-  __device__ static void init(const Tables& T, const State& S, int b, int lane, TerritoryScratch& sc, uint16_t* grid, int episode, uint32_t k0, uint32_t k1) {
+  __device__ static void init(const Tables& T, const Params& F, const State& S, int b, int lane, TerritoryScratch& sc, uint16_t* grid, int episode, uint32_t k0, uint32_t k1) {
     uint8_t* u8 = S.fam_u8 + (size_t)b * S.fam_u8_stride;
     uint16_t* u16 = S.fam_u16 + (size_t)b * S.fam_u16_stride;
     copy_init_grid(T, grid, lane);
     for (int k = lane; k < T.nR; k += 32) {  // Resource:reset (components.lua:73-80)
-      u8[RU_STATE * T.nR_pad + k] = (uint8_t)T.tr_res[k * 3 + 2];
-      u8[RU_HEALTH * T.nR_pad + k] = (uint8_t)T.res_health0;
+      u8[RU_STATE * T.nR_pad + k] = (uint8_t)F.tr_res[k * 3 + 2];
+      u8[RU_HEALTH * T.nR_pad + k] = (uint8_t)F.res_health0;
       u8[RU_FLAGS * T.nR_pad + k] = RF_NEVER_CLAIMED;
       u8[RU_CLAIMER * T.nR_pad + k] = 0xFF;
       u8[RU_IND * T.nR_pad + k] = 0; u8[RU_DMG * T.nR_pad + k] = 0; u8[RU_TEX * T.nR_pad + k] = 0;
       u16[RS_FSZ * T.nR_pad + k] = 0; u16[RS_AGE * T.nR_pad + k] = 0;
-      if (T.tr_res_cond && !choice_present(T, T.tr_res_cond[k * 2], (uint32_t)T.tr_res_cond[k * 2 + 1], episode, k0, k1)) {
+      if (F.tr_res_cond && !choice_present(T, F.tr_res_cond[k * 2], (uint32_t)F.tr_res_cond[k * 2 + 1], episode, k0, k1)) {
         // This episode's map has plain floor here: the resource, its texture and its two indicators were not created.
         // Kept as a destroyed resource that never had a texture: nothing stands on the cell, nothing is drawn, nothing updates.
-        const int cell = T.tr_res[k * 3 + 1];
+        const int cell = F.tr_res[k * 3 + 1];
         u8[RU_STATE * T.nR_pad + k] = 1; u8[RU_FLAGS * T.nR_pad + k] = RF_DESTROYED | RF_ABSENT; u8[RU_TEX * T.nR_pad + k] = 1;
-        grid[(size_t)T.res_layer * T.cells_pad + cell] = 0; grid[(size_t)T.tex_layer * T.cells_pad + cell] = 0;
-        grid[(size_t)T.ind_layer * T.cells_pad + cell] = 0; grid[(size_t)T.dmg_layer * T.cells_pad + cell] = 0;
+        grid[(size_t)F.res_layer * T.cells_pad + cell] = 0; grid[(size_t)F.tex_layer * T.cells_pad + cell] = 0;
+        grid[(size_t)F.ind_layer * T.cells_pad + cell] = 0; grid[(size_t)F.dmg_layer * T.cells_pad + cell] = 0;
       }
     }
     // spawn: with 'choice' spawn points the group's members are this episode's draw
@@ -203,12 +218,12 @@ struct Territory {
                 episode, k0, k1, [&](int) {
       int32_t* ax = S.av_extra + ((size_t)b * T.P + lane) * 8;
       ax[AX_FREEZE] = 0; ax[AX_REMOVAL] = 0; ax[AX_FLAGS] = 1; ax[AX_NOZAP] = 0;
-      ax[AX_LEVEL] = T.mark_initial_level; ax[AX_MARK_T] = 0; ax[AX_SHOWN] = T.mark_initial_level; ax[AX_CLAIM_COOL] = 0;
+      ax[AX_LEVEL] = F.mark_initial_level; ax[AX_MARK_T] = 0; ax[AX_SHOWN] = F.mark_initial_level; ax[AX_CLAIM_COOL] = 0;
     });
   }
 
   // One frame. `actions` is null on frame 0 of an episode: every avatar does nothing.
-  __device__ static void frame(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, TerritoryScratch& sc,
+  __device__ static void frame(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, TerritoryScratch& sc,
                                const Frame& f) {
     const auto [env, grid, k0, k1, n, episode] = f;
     uint8_t* u8 = S.fam_u8 + (size_t)b * S.fam_u8_stride;
@@ -253,9 +268,9 @@ struct Territory {
     for (int k = lane; k < T.nR; k += 32) if (sc.r[RU_STATE][k] != 1) sc.occ[sc.res_cell[k]] = 254;  // resources stand on the avatar layer
     if (is_av && alive) sc.occ[y * T.W + x] = (uint8_t)(lane + 1);
     // hit sprites live one frame (policy A.8)
-    if (env[ENV_BEAM] & 1) clear_layer(T, grid, T.zap_layer, lane);
-    if (env[ENV_BEAM] & 2) clear_layer(T, grid, T.brush_layer, lane);
-    if (env[ENV_BEAM] & 4) for (int c = lane; c < T.cells; c += 32) { const int rr = sc.res_of[c]; if (rr < 0 || (sc.r[RU_FLAGS][rr] & RF_ABSENT)) grid[(size_t)T.claim_layer * T.cells_pad + c] = 0; }
+    if (env[ENV_BEAM] & 1) clear_layer(T, grid, F.zap.layer, lane);
+    if (env[ENV_BEAM] & 2) clear_layer(T, grid, F.brush_layer, lane);
+    if (env[ENV_BEAM] & 4) for (int c = lane; c < T.cells; c += 32) { const int rr = sc.res_of[c]; if (rr < 0 || (sc.r[RU_FLAGS][rr] & RF_ABSENT)) grid[(size_t)F.claim_layer * T.cells_pad + c] = 0; }
     __syncwarp();
     int beam_dirty = 0;
 
@@ -268,7 +283,7 @@ struct Territory {
       if (removal == 1) removed_now = alive != 0;  // setState(waitState): first item of this frame's queue
       removal = removal > 0 ? removal - 1 : 0;
       // Zapper:update (:713-724)
-      if (nozap) zap_cool = T.zap_cooldown + 1;
+      if (nozap) zap_cool = F.zap.cooldown + 1;
       const int old = nozap_cnt;
       nozap_cnt = nozap_cnt > 0 ? nozap_cnt - 1 : 0;
       if (old == 1) nozap = 0;
@@ -276,12 +291,12 @@ struct Territory {
     for (int k = lane; k < T.nR; k += 32) {
       // Resource:update (components.lua:184-197) -> damage indicator setStates (applied in round 1)
       int health = sc.r[RU_HEALTH][k];
-      if (health < T.res_health0) {
+      if (health < F.res_health0) {
         int dmg = 1;
         int fsz = sc.fsz[k];
-        if (fsz >= T.res_repair_delay) {
+        if (fsz >= F.res_repair_delay) {
           uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)sc.res_obj[k], RS_OBJECT, k0, k1);
-          if (u01(w.x, w.y) < T.res_repair_prob) { ++health; if (health == T.res_health0) dmg = 0; }
+          if (u01(w.x, w.y) < F.res_repair_prob) { ++health; if (health == F.res_health0) dmg = 0; }
         }
         sc.r[RU_HEALTH][k] = (uint8_t)health;
         sc.r[RU_DMG][k] = (uint8_t)dmg;
@@ -296,8 +311,8 @@ struct Territory {
     // ---- updaters --------------------------------------------------------------------------------
     const int rank = visit_rank(T, lane, n, episode, k0, k1);
     bool fire_zap = false, fire_claim = false;
-    if (is_av && alive) { if (zap_cool > 0) --zap_cool; else if (act_zap == 1) { zap_cool = T.zap_cooldown; fire_zap = true; } }  // 140
-    if (is_av && T.claim_wait >= 0) { if (claim_cool > 0) --claim_cool; else if (act_claim == 1) { claim_cool = T.claim_wait; fire_claim = true; } }  // 100 (no alive check)
+    if (is_av && alive) { if (zap_cool > 0) --zap_cool; else if (act_zap == 1) { zap_cool = F.zap.cooldown; fire_zap = true; } }  // 140
+    if (is_av && F.claim_wait >= 0) { if (claim_cool > 0) --claim_cool; else if (act_claim == 1) { claim_cool = F.claim_wait; fire_claim = true; } }  // 100 (no alive check)
     const bool cont = episode_continues(T, n, episode, k0, k1);
     const unsigned alive_mask0 = __ballot_sync(MP_FULL, is_av && alive);
     // 100 Resource provideRewards (:82-99) and 2 releaseClaimOfDeadAgent (:100-112), on frame-start state
@@ -306,9 +321,9 @@ struct Territory {
       if (st < 2) continue;
       const int age = sc.age[k];
       const int claimer = sc.r[RU_CLAIMER][k];
-      if (age >= T.res_reward_delay) {
+      if (age >= F.res_reward_delay) {
         uint4 w = philox4x32_10((uint32_t)n, (uint32_t)episode, (uint32_t)sc.res_obj[k], RS_OBJECT, k0, k1);
-        if (u01(w.z, w.w) < T.res_rate && claimer != 0xFF) {
+        if (u01(w.z, w.w) < F.res_rate && claimer != 0xFF) {
           if (alive_mask0 >> claimer & 1u) atomicAdd(&sc.cnt[claimer], 1);  // Avatar:addReward skips avatars in their wait state
           sc.r[RU_FLAGS][k] |= RF_ACTIVE;
         }
@@ -320,13 +335,13 @@ struct Territory {
     }
     __syncwarp();
     if (is_av) {
-      const double amount = T.tr_taste_role == 2 ? 0.0 : T.res_reward;  // Taste:addDefaultReward (:348-356)
+      const double amount = F.tr_taste_role == 2 ? 0.0 : F.res_reward;  // Taste:addDefaultReward (:348-356)
       for (int i = 0; i < sc.cnt[lane]; ++i) reward += amount;
     }
     // 3 GraduatedSanctionsMarking resetToInitialLevel (avatar_library.lua:1009-1026)
-    if (is_av && alive && level != T.mark_initial_level) {
+    if (is_av && alive && level != F.mark_initial_level) {
       ++mark_t;
-      if (mark_t == T.mark_recovery) { level = T.mark_initial_level; shown = level; mark_t = 0; }
+      if (mark_t == F.mark_recovery) { level = F.mark_initial_level; shown = level; mark_t = 0; }
     }
 
     // ---- round 1 ---------------------------------------------------------------------------------
@@ -341,7 +356,7 @@ struct Territory {
     move_avatars(T, lane, rank, is_av && alive && move_ok, act_turn, act_move, x, y, orient, sc.occ, [](int, int) {});
     // beams: pass 0 zap (140), pass 1 paintbrush (130), pass 2 claim (100)
     for (int pass = 0; pass < 3; ++pass) {
-      const BeamGeom& G = pass == 0 ? T.zap_geom : (pass == 1 ? T.brush_geom : T.claim_geom);
+      const BeamGeom& G = pass == 0 ? F.zap.geom : (pass == 1 ? F.brush_geom : F.claim_geom);
       if (pass == 1 && G.n == 1 && G.fwd[0] == 1 && G.lat[0] == 0) {
         // Paintbrush (territory/components.lua:362-412): every living avatar fires a one-cell beam every frame. The nine
         // beams are resolved together, one lane per avatar, with exactly the outcome of visiting them in this frame's
@@ -381,7 +396,7 @@ struct Territory {
         }
         if (cell >= 0 && first_cell == rank) {
           atomicOr(&sc.bm_brush[cell >> 5], 1u << (cell & 31));
-          grid[(size_t)T.brush_layer * T.cells_pad + cell] = cell_value(T.brush_sprite[lane], orient);
+          grid[(size_t)F.brush_layer * T.cells_pad + cell] = cell_value(F.brush_sprite[lane], orient);
           beam_dirty |= 2;
         }
         __syncwarp();
@@ -417,7 +432,7 @@ struct Territory {
                 int h = (int)sc.r[RU_HEALTH][rr] - 1;
                 sc.fsz[rr] = 0;
                 if (h == 0) {
-                  h = T.res_health0;
+                  h = F.res_health0;
                   sc.r2_state[rr] = 1; sc.r2_changed[rr] = 1;
                   sc.r[RU_FLAGS][rr] = (sc.r[RU_FLAGS][rr] & ~RF_ACTIVE) | RF_DESTROYED;
                   sc.r[RU_TEX][rr] = 1; sc.r[RU_DMG][rr] = 0;  // texture 'destroyed', damage indicator 'inactive' (round 2)
@@ -427,19 +442,19 @@ struct Territory {
               }
             } else {
               // Zapper:onHit (avatar_library.lua:652-681), then the marking on the same cell (:1049-1093)
-              if (lane == t) reward += T.zap_penalty;
-              if (lane == src) { reward += T.zap_reward; emit_event(S, b, EV_ZAP, src + 1, t + 1); }
+              if (lane == t) reward += F.zap.penalty;
+              if (lane == src) { reward += F.zap.reward; emit_event(S, b, EV_ZAP, src + 1, t + 1); }
               const int t_mk = __shfl_sync(MP_FULL, mk_on, t), t_level = __shfl_sync(MP_FULL, level, t);
-              if (t_mk && t_level >= 1 && t_level <= T.mark_n_levels) {
+              if (t_mk && t_level >= 1 && t_level <= F.mark_n_levels) {
                 const int l = t_level - 1;
-                if (lane == src) reward += T.mark_src_reward[l];
+                if (lane == src) reward += F.mark_src_reward[l];
                 if (lane == t) {
-                  reward += T.mark_tgt_reward[l];
-                  level += T.mark_inc[l];
-                  if (T.mark_remove[l]) { removal = 1; move_ok = 0; freeze = 1; nozap = 1; nozap_cnt = 1; emit_event(S, b, EV_REMOVAL, src + 1, t + 1); }
+                  reward += F.mark_tgt_reward[l];
+                  level += F.mark_inc[l];
+                  if (F.mark_remove[l]) { removal = 1; move_ok = 0; freeze = 1; nozap = 1; nozap_cnt = 1; emit_event(S, b, EV_REMOVAL, src + 1, t + 1); }
                   else {
                     shown = level;  // _setLevel (round 2)
-                    if (T.mark_freeze[l] > 0) { move_ok = 0; freeze = T.mark_freeze[l]; nozap = 1; nozap_cnt = T.mark_freeze[l]; }
+                    if (F.mark_freeze[l] > 0) { move_ok = 0; freeze = F.mark_freeze[l]; nozap = 1; nozap_cnt = F.mark_freeze[l]; }
                   }
                   mark_t = 0;
                   emit_event(S, b, EV_SANCTIONING, src + 1, t + 1);
@@ -460,8 +475,8 @@ struct Territory {
         }
         if (vis && !blocked) {
           uint32_t* bm = pass == 0 ? sc.bm_zap : (pass == 1 ? sc.bm_brush : sc.bm_claim);
-          const int layer = pass == 0 ? T.zap_layer : (pass == 1 ? T.brush_layer : T.claim_layer);
-          const int sprite = pass == 0 ? T.zap_sprite : (pass == 1 ? T.brush_sprite[src] : T.claimbeam_sprite[src]);
+          const int layer = pass == 0 ? F.zap.layer : (pass == 1 ? F.brush_layer : F.claim_layer);
+          const int sprite = pass == 0 ? F.zap.sprite : (pass == 1 ? F.brush_sprite[src] : F.claimbeam_sprite[src]);
           const int rr_here = pass == 2 ? sc.res_of[cell] : -1;
           const bool layer_free = rr_here < 0 || (sc.r[RU_FLAGS][rr_here] & RF_ABSENT);  // a resource's damage indicator occupies the claim layer
           if (layer_free) { draw_hit_sprite(T, grid, bm, layer, cell, cell_value(sprite, so)); beam_dirty |= 1 << pass; }
@@ -479,10 +494,10 @@ struct Territory {
       sc.age[k] = sc.r2_changed[k] ? (uint16_t)1 : (uint16_t)min((int)sc.age[k] + 1, 65535);  // age in frame n + 1
       const uint8_t was_state = sc.was[0][k], was_ind = sc.was[1][k], was_dmg = sc.was[2][k], was_tex = sc.was[3][k];
       sc.r[RU_STATE][k] = (uint8_t)st_new;
-      if (st_new != was_state) grid[(size_t)T.res_layer * T.cells_pad + cell] = resource_sprite_value(T, st_new);
-      if (sc.r[RU_IND][k] != was_ind) grid[(size_t)T.ind_layer * T.cells_pad + cell] = sc.r[RU_IND][k] ? cell_value(T.dry_sprite[sc.r[RU_IND][k] - 1], 0) : (uint16_t)0;
-      if (sc.r[RU_DMG][k] != was_dmg) grid[(size_t)T.dmg_layer * T.cells_pad + cell] = sc.r[RU_DMG][k] ? cell_value(T.dmg_sprite, 0) : (uint16_t)0;
-      if (sc.r[RU_TEX][k] != was_tex) grid[(size_t)T.tex_layer * T.cells_pad + cell] = sc.r[RU_TEX][k] ? (uint16_t)0 : cell_value(T.tex_sprite, 0);
+      if (st_new != was_state) grid[(size_t)F.res_layer * T.cells_pad + cell] = resource_sprite_value(F, st_new);
+      if (sc.r[RU_IND][k] != was_ind) grid[(size_t)F.ind_layer * T.cells_pad + cell] = sc.r[RU_IND][k] ? cell_value(F.dry_sprite[sc.r[RU_IND][k] - 1], 0) : (uint16_t)0;
+      if (sc.r[RU_DMG][k] != was_dmg) grid[(size_t)F.dmg_layer * T.cells_pad + cell] = sc.r[RU_DMG][k] ? cell_value(F.dmg_sprite, 0) : (uint16_t)0;
+      if (sc.r[RU_TEX][k] != was_tex) grid[(size_t)F.tex_layer * T.cells_pad + cell] = sc.r[RU_TEX][k] ? (uint16_t)0 : cell_value(F.tex_sprite, 0);
     }
     __syncwarp();
     {
@@ -496,9 +511,9 @@ struct Territory {
     // avatars and their markings
     const bool av_changed = draw_avatars(T, grid, lane, x0, y0, orient0, alive0, x, y, orient, alive);
     const bool mk_changed = is_av && (av_changed || mk_on != mk_on0 || shown != shown0);
-    if (mk_changed && mk_on0) grid[(size_t)T.mark_layer * T.cells_pad + y0 * T.W + x0] = 0;
+    if (mk_changed && mk_on0) grid[(size_t)F.mark_layer * T.cells_pad + y0 * T.W + x0] = 0;
     __syncwarp();
-    if (mk_changed && mk_on) grid[(size_t)T.mark_layer * T.cells_pad + y * T.W + x] = cell_value(T.mark_sprite[shown - 1], orient);
+    if (mk_changed && mk_on) grid[(size_t)F.mark_layer * T.cells_pad + y * T.W + x] = cell_value(F.mark_sprite[shown - 1], orient);
 
     const bool done = n > 0 && (!cont || n >= T.max_frames);
     if (is_av) {
@@ -508,21 +523,21 @@ struct Territory {
       ax[AX_FREEZE] = freeze; ax[AX_REMOVAL] = removal; ax[AX_FLAGS] = move_ok | (nozap << 1) | (mk_on << 2); ax[AX_NOZAP] = nozap_cnt;
       ax[AX_LEVEL] = level; ax[AX_MARK_T] = mark_t; ax[AX_SHOWN] = shown; ax[AX_CLAIM_COOL] = claim_cool;
       for (int k = 0; k < T.n_scalar; ++k)
-        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = alive ? fmax(1.0 - (double)zap_cool / (double)T.zap_cooldown, 0.0) : 0.0;
+        S.scalar_obs[((size_t)k * S.B + b) * T.P + lane] = alive ? fmax(1.0 - (double)zap_cool / (double)F.zap.cooldown, 0.0) : 0.0;
     }
     store_timestep(T, S, b, lane, n, n == 0 ? 0.0 : reward, n == 0 ? 0 : (done ? 2 : 1), beam_dirty);
   }
 
   // Every episode starts with the raw state of init, then runs frame 0.
-  __device__ static void reset(const Tables& T, const State& S, int b, int lane, TerritoryScratch& sc) {
+  __device__ static void reset(const Tables& T, const Params& F, const State& S, int b, int lane, TerritoryScratch& sc) {
     const Frame f = begin_frame(T, S, b, true);
     __syncwarp();
-    init(T, S, b, lane, sc, f.grid, f.episode, f.k0, f.k1);
+    init(T, F, S, b, lane, sc, f.grid, f.episode, f.k0, f.k1);
     reset_env_row(T, S, b, lane, f.episode, 0);
-    frame(T, S, b, lane, nullptr, sc, f);
+    frame(T, F, S, b, lane, nullptr, sc, f);
   }
 
-  __device__ static void step(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions, TerritoryScratch& sc) {
-    frame(T, S, b, lane, actions, sc, begin_frame(T, S, b, false));
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, TerritoryScratch& sc) {
+    frame(T, F, S, b, lane, actions, sc, begin_frame(T, S, b, false));
   }
 };

@@ -119,6 +119,23 @@ def test_variant_is_refused_at_create(name):
     engine.Engine(blob, 4, seed=1)
 
 
+@pytest.mark.parametrize('substrate,section', [('clean_up', 'cu_dirt'), ('commons_harvest__open', 'ch_apple'),
+                                               ('territory__rooms', 'tr_res'), ('coins', 'co_coin'), ('coop_mining', 'cm_ore')])
+def test_entity_table_short_or_off_the_map_is_refused_at_create(substrate, section):
+  # The kernels read the first n rows of each entity table, and every table's cell column feeds a cell -> entity index.
+  from meltingpot_b200 import blob as mpb, engine, substrates
+  sec = mpb.unpack(substrates.load_blob(substrate))
+  short = dict(sec)
+  short[section] = sec[section][:-1]
+  off_map = dict(sec)
+  off_map[section] = sec[section].copy()
+  off_map[section][-1, 1] = int(sec['meta'][1]) * int(sec['meta'][2])  # W * H: one past the last cell
+  for bad, what in ((short, r'has \d+ values for'), (off_map, 'puts entity')):
+    with pytest.raises(ValueError, match=f"mp_engine error -1: blob: section '{section}' {what}"):  # MP_E_INVALID
+      engine.Engine(mpb.pack(bad), 4, seed=1)
+  engine.Engine(mpb.pack(sec), 4, seed=1).close()
+
+
 def test_territory_past_frame_65535_matches_the_oracle(oracle):
   # One episode of 70,000 frames. A resource's age (frames since its last state change) decides when its claim starts
   # paying (rewardDelay) and when the claim of a removed avatar is released (5 frames); past frame 65,535 a 16-bit
