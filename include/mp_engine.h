@@ -115,6 +115,36 @@ typedef struct mp_buffers {
 int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uint64_t seed,
               uint64_t env_index_base, uint32_t flags, mp_handle* out);
 
+/* Heterogeneous batch: one engine whose envs each run under one of `n_variants` (1..MP_MAX_VARIANTS) compiled blobs of
+ * the same substrate, as separate reference builds with different `prefab_overrides` (builder.py:70-87) would. Env b
+ * starts under variant env_variant_host[b] (host array of num_envs bytes; NULL = every env variant 0) and gives, byte
+ * for byte, what env b of an mp_create engine built from its variant's blob with the same seed and env_index_base
+ * gives. The variants must be compatible, which is checked once here; otherwise this fails with MP_E_UNSUPPORTED and
+ * mp_last_error names the first section or parameter that differs:
+ *   - every blob section other than the family's parameter blocks ("<fam>_ip", "<fam>_dp"), "comps", "comps_f" and
+ *     "info_json" is byte-identical: the map, sprites, atlas, view, action table and 'choice' groups agree;
+ *   - each variant passes every check mp_create makes;
+ *   - the entity counts, the episode ending and the beam footprints agree;
+ *   - the family's parameters differ only in its scalar knobs (cooldowns, rewards, probabilities, rates, delays, ...):
+ *     layers, sprites, hit ids, beam shapes and whatever sizes per-env state agree.
+ * Envs of an engine with more than one variant run a separate instantiation of the state-transition kernel that reads
+ * each env's parameters from a device array; with one variant this is mp_create. */
+#define MP_MAX_VARIANTS 256
+int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n_variants, const uint8_t* env_variant_host,
+                       int num_envs, int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out);
+
+/* Reassigns envs to variants: copies `env_variant` (DEVICE pointer to num_envs bytes) into the pending assignments on
+ * `stream`. An env takes its pending variant when its next episode starts (the auto-reset after LAST, or mp_reset), never
+ * mid-episode, as the reference's ResetWrapper rebuilds its env on every reset; reset envs with a mask to switch them
+ * at once. A value >= n_variants runs as variant 0. Only for engines with more than one variant. */
+int mp_set_env_variants(mp_handle h, const uint8_t* env_variant, void* stream);
+
+/* The variant set: its size and the DEVICE arrays (u8 [B]) of the variant each env's current episode runs (`active`)
+ * and its next episode will run (`pending`, writable like mp_set_env_variants). Both NULL with one variant. Snapshots
+ * (mp_state_save) of a multi-variant engine include both arrays and load only into an engine built from the same
+ * blobs in the same order. */
+int mp_env_variants(mp_handle h, int* n_variants, uint8_t** active, uint8_t** pending);
+
 /* Replaces Lab2dWrapper.close (wrappers/base.py:82-84). */
 int mp_destroy(mp_handle h);
 

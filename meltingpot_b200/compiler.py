@@ -1203,13 +1203,36 @@ def _territory_tables(model: WorldModel, sections: Dict[str, np.ndarray]):
 # ---------------------------------------------------------------------------
 # Entry points
 # ---------------------------------------------------------------------------
+def apply_prefab_overrides(settings: Mapping[str, Any],
+                           overrides: Optional[Mapping[str, Mapping[str, Mapping[str, Any]]]]) -> Dict[str, Any]:
+  """`builder.apply_prefab_overrides` (builder.py:70-87) on a plain settings dict: {prefab: {component: {kwarg: value}}}
+  sets each kwarg on the FIRST component of that name in `simulation.prefabs[prefab]`. Returns a new settings dict;
+  neither argument is modified. Only prefabs are reached, so avatars (built into `gameObjects`) keep their kwargs."""
+  settings = copy.deepcopy(dict(settings))
+  prefabs = settings['simulation'].get('prefabs', {})
+  for prefab, override in (overrides or {}).items():
+    for component, arg_overrides in override.items():
+      for arg_name, arg_override in arg_overrides.items():
+        if prefab not in prefabs:
+          raise ValueError(f"Prefab override for '{prefab}' given, but not available in `prefabs`.")
+        named = [c for c in prefabs[prefab].get('components', []) if c.get('component') == component]
+        if not named:  # game_object_utils.get_first_named_component
+          raise ValueError(f"No component with name '{component}' found.")
+        named[0]['kwargs'][arg_name] = copy.deepcopy(arg_override)
+  return settings
+
+
 def compile_settings(settings: Mapping[str, Any],
                      config: Optional[Any] = None,
-                     build_seed: Optional[int] = None) -> bytes:
+                     build_seed: Optional[int] = None,
+                     prefab_overrides: Optional[Mapping[str, Any]] = None) -> bytes:
   """lab2d settings (+ optional substrate config for API metadata) -> blob.
 
-  `build_seed` resolves 'choice' prefabs (see _expand_prefab); configs without them ignore it.
+  `build_seed` resolves 'choice' prefabs (see _expand_prefab); configs without them ignore it. `prefab_overrides` are
+  applied first, as the reference builder applies them (apply_prefab_overrides).
   """
+  if prefab_overrides:
+    settings = apply_prefab_overrides(settings, prefab_overrides)
   model = WorldModel(settings, build_seed)
   rewarded = model.avatar_roles & model.rewarded_roles
   if rewarded:
@@ -1301,8 +1324,9 @@ def compile_settings(settings: Mapping[str, Any],
 
 def compile_substrate(name: str, roles: Optional[Sequence[str]] = None,
                       root: Optional[str] = None,
-                      build_seed: Optional[int] = None) -> bytes:
-  """Compiles a named reference substrate (needs a reference checkout)."""
+                      build_seed: Optional[int] = None,
+                      prefab_overrides: Optional[Mapping[str, Any]] = None) -> bytes:
+  """Compiles a named reference substrate (needs a reference checkout), with the reference's `prefab_overrides`."""
   config = load_reference_config(name, root)
   roles = tuple(roles) if roles is not None else tuple(config.default_player_roles)
   # Some builders draw from Python's global `random` (coins.py:45-84,488: map size and the two coin types):
@@ -1314,4 +1338,4 @@ def compile_substrate(name: str, roles: Optional[Sequence[str]] = None,
     settings = config.lab2d_settings_builder(roles=roles, config=config)
   finally:
     random.setstate(state)
-  return compile_settings(settings, config, build_seed)
+  return compile_settings(settings, config, build_seed, prefab_overrides)

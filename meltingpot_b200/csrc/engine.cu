@@ -131,12 +131,25 @@ int make_lane_map_cells(int n_rows, int n_cells, int pitch_slots, int iters, uin
 // state-transition kernel with the dynamic shared memory one launch of it takes. An engine keeps the Params of its
 // family in a FamilyParams; only the row's own functions look inside it.
 using FamilyParams = std::variant<CleanUp::Params, Commons::Params, Territory::Params, Coins::Params, Mining::Params>;
+// The per-env variant set of an engine (mp_create_variants): the device array of Params and the per-env assignments.
+struct VariantSet {
+  const void* params = nullptr;  // Family::Params [n]
+  uint8_t* active = nullptr;     // [B] the variant each env's current episode runs
+  uint8_t* pending = nullptr;    // [B] the variant each env's next episode runs
+  int n = 1;
+};
 struct FamilyEntry {
   int id;  // MpbFamily
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
   cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int);
   size_t (*step_smem)(const Tables&);
-  const void* step;  // k_step<Family>
+  const void* step;           // k_step<Family>
+  // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field), the upload of base's Params with
+  // each variant's knobs (base holds the engine's device tables), and the k_step<Family, ParamVariants> launch
+  int (*same_shape)(const FamilyParams&, const FamilyParams&);
+  int (*upload_variants)(std::vector<void*>&, const FamilyParams& base, const std::vector<FamilyParams>&, const void**);
+  cudaError_t (*launch_variants)(const cudaLaunchConfig_t&, const Tables&, const VariantSet&, const State&, const int32_t*, const uint8_t*, int);
+  const void* step_variants;  // k_step<Family, ParamVariants<Family::Params>>
 };
 
 template <class Family>
@@ -149,8 +162,31 @@ cudaError_t launch_family(const cudaLaunchConfig_t& cfg, const Tables& T, const 
   return cudaLaunchKernelEx(&cfg, k_step<Family>, T, std::get<typename Family::Params>(params), S, actions, mask, mode);
 }
 template <class Family>
+int same_shape_family(const FamilyParams& a, const FamilyParams& b) {
+  return Family::same_shape(std::get<typename Family::Params>(a), std::get<typename Family::Params>(b));
+}
+template <class Family>
+int upload_variants_family(std::vector<void*>& allocs, const FamilyParams& base, const std::vector<FamilyParams>& variants, const void** out) {
+  using P = typename Family::Params;
+  std::vector<P> host(variants.size(), std::get<P>(base));
+  for (size_t v = 0; v < variants.size(); ++v) Family::copy_knobs(host[v], std::get<P>(variants[v]));
+  const P* d = nullptr;
+  int rc = upload(allocs, host, &d);
+  *out = d;
+  return rc;
+}
+template <class Family>
+cudaError_t launch_variants_family(const cudaLaunchConfig_t& cfg, const Tables& T, const VariantSet& V, const State& S,
+                                   const int32_t* actions, const uint8_t* mask, int mode) {
+  using P = typename Family::Params;
+  const ParamVariants<P> src{static_cast<const P*>(V.params), V.active, V.pending, V.n};
+  return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode);
+}
+template <class Family>
 FamilyEntry family_entry(int id) {
-  return {id, load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>)};
+  return {id, load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
+          same_shape_family<Family>, upload_variants_family<Family>, launch_variants_family<Family>,
+          reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>)};
 }
 const FamilyEntry kFamilies[] = {
     family_entry<CleanUp>(MPB_FAMILY_CLEAN_UP),
@@ -210,7 +246,8 @@ struct mp_engine {
   uint64_t state_bytes = 0;
   int lane_map_players = 0, lane_map_world = 0;  // 0 plain, 2 scattered colouring, 1 + 16 * (extra wavefronts left) whole-cell dealing
   int inst_ncp = 0, inst_ncw = 0;                // the k_render<NCP, NCW> instantiation this engine launches
-  uint64_t blob_hash = 0;  // FNV-1a of the compiled blob: a snapshot only loads into an engine built from the same blob
+  uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
+  VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
 
   template <typename T>
   int alloc(size_t count, T** out) {
@@ -619,7 +656,8 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode));
+  if (E->variants.n > 1) CUDA_TRY(E->family->launch_variants(cfg, E->T, E->variants, E->S, actions, mask, mode));
+  else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st); }
@@ -803,8 +841,10 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     static int step_smem_max[MP_MAX_DEVICES] = {};
     const int need = (int)E->step_smem;
     if (ce == cudaSuccess && need > 48 * 1024 && need > step_smem_max[device]) {
-      for (const FamilyEntry& f : kFamilies)
+      for (const FamilyEntry& f : kFamilies) {
         if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+        if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step_variants, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+      }
       if (ce == cudaSuccess) step_smem_max[device] = need;
     }
   }
@@ -821,6 +861,135 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   E->render_bytes = (uint64_t)P * E->R.player_bytes + (uint64_t)E->R.world_bytes + (uint64_t)T.L * T.cells * 2;
   E->algo_bytes = (uint64_t)P * E->R.player_bytes + (uint64_t)E->R.world_bytes + 8ull * ((1 + T.n_scalar) * P + 2) + 8ull * P + 2ull * T.L * T.cells * 2;
   *out = E;
+  return MP_OK;
+}
+
+namespace {
+// Rule (a) of mp_create_variants: variant `v` has the same sections as variant 0, byte for byte, except the family's
+// parameter blocks, the component tables and the metadata string.
+int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
+  const MpbHeader* h0 = static_cast<const MpbHeader*>(b0);
+  const MpbHeader* hv = static_cast<const MpbHeader*>(bv);
+  if (n0 < sizeof(MpbHeader) || nv < sizeof(MpbHeader) || memcmp(hv->magic, MPB_MAGIC, 4) != 0 || hv->version != MPB_VERSION ||
+      nv < sizeof(MpbHeader) + (size_t)hv->n_sections * sizeof(MpbSection))
+    return fail(MP_E_INVALID, "blob: not an MPB%u blob", MPB_VERSION);
+  auto free_to_differ = [](const char* name) {
+    const size_t len = strnlen(name, MPB_NAME_LEN);
+    return (len == 5 && name[2] == '_' && (name[3] == 'i' || name[3] == 'd') && name[4] == 'p') || !strcmp(name, "comps") ||
+           !strcmp(name, "comps_f") || !strcmp(name, "info_json");
+  };
+  const MpbSection* s0 = reinterpret_cast<const MpbSection*>(h0 + 1);
+  const MpbSection* sv = reinterpret_cast<const MpbSection*>(hv + 1);
+  auto check = [&](const MpbSection* s, uint32_t count, const void* other, size_t n_other, const void* own) -> int {
+    for (uint32_t i = 0; i < count; ++i) {
+      char name[MPB_NAME_LEN + 1] = {};
+      memcpy(name, s[i].name, MPB_NAME_LEN);
+      if (free_to_differ(name)) continue;
+      const MpbSection* t = mpb_find(other, n_other, name);
+      if (!t || t->dtype != s[i].dtype || t->ndim != s[i].ndim || memcmp(t->shape, s[i].shape, sizeof t->shape) != 0 ||
+          t->nbytes != s[i].nbytes || memcmp(mpb_data(other, t), mpb_data(own, &s[i]), s[i].nbytes) != 0)
+        return fail(MP_E_UNSUPPORTED, "section '%s' differs (variants may differ only in the family's parameters)", name);
+    }
+    return MP_OK;
+  };
+  int rc = check(s0, h0->n_sections, bv, nv, b0);
+  return rc ? rc : check(sv, hv->n_sections, b0, n0, bv);
+}
+
+uint64_t fnv1a(const void* p, size_t n, uint64_t h = 1469598103934665603ull) {
+  const uint8_t* bp = static_cast<const uint8_t*>(p);
+  for (size_t i = 0; i < n; ++i) { h ^= bp[i]; h *= 1099511628211ull; }
+  return h;
+}
+
+// Rules (b)-(d) of mp_create_variants for an engine built from variant 0, then the variant set's device arrays.
+int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host) {
+  struct Decided { int nA, nD, nW, nR, nR_pad, end_min_frames, end_interval, beam_cells; double end_prob; std::vector<std::vector<int>> hints; };
+  std::vector<FamilyParams> params(n);
+  std::vector<Decided> decided;
+  std::vector<void*> scratch;  // the loaders' device uploads: every variant uses the engine's own (same sections)
+  int rc = MP_OK;
+  for (int v = 0; v < n && rc == MP_OK; ++v) {
+    Section<int32_t> hits;
+    if (!get_section(blobs[v], blob_bytes[v], "hits", MPB_I32, &hits)) { rc = fail(MP_E_INVALID, "blob: missing section 'hits'"); break; }
+    FamilyLoad ld{blobs[v], blob_bytes[v], hits, scratch};
+    if ((rc = E->family->load(ld, E->T, params[v]))) break;
+    decided.push_back({ld.nA, ld.nD, ld.nW, ld.nR, ld.nR_pad, ld.end_min_frames, ld.end_interval, ld.beam_cells, ld.end_prob, ld.hint_stacks});
+    const Decided& a = decided[0];
+    const Decided& b = decided[v];
+    if (a.nA != b.nA || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
+    else if (a.end_min_frames != b.end_min_frames || a.end_interval != b.end_interval || memcmp(&a.end_prob, &b.end_prob, sizeof a.end_prob) != 0)
+      rc = fail(MP_E_UNSUPPORTED, "episode ending differs");
+    else if (a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
+    else if (a.hints != b.hints) rc = fail(MP_E_UNSUPPORTED, "pre-merged sprite hints differ");
+    else rc = E->family->same_shape(params[0], params[v]);
+    if (rc) g_error = "variant " + std::to_string(v) + ": " + g_error;
+  }
+  for (void* p : scratch) cudaFree(p);
+  if (rc) return rc;
+  if ((rc = E->family->upload_variants(E->allocs, E->params, params, &E->variants.params))) return rc;
+  const size_t B = E->B;
+  std::vector<uint8_t> assign(B, 0);
+  if (env_variant_host) assign.assign(env_variant_host, env_variant_host + B);
+  const uint8_t* d = nullptr;
+  if ((rc = upload(E->allocs, assign, &d))) return rc;
+  E->variants.active = const_cast<uint8_t*>(d);
+  if ((rc = upload(E->allocs, assign, &d))) return rc;
+  E->variants.pending = const_cast<uint8_t*>(d);
+  E->variants.n = n;
+  // snapshots carry the assignments, and only load into an engine with the same variants in the same order
+  E->state_spans.push_back({E->variants.active, B}); E->state_spans.push_back({E->variants.pending, B});
+  E->state_bytes += 2 * B;
+  uint64_t h = fnv1a(&n, sizeof n);
+  for (int v = 0; v < n; ++v) { const uint64_t hv = fnv1a(blobs[v], blob_bytes[v]); h = fnv1a(&hv, sizeof hv, h); }
+  E->blob_hash = h;
+  return MP_OK;
+}
+}  // namespace
+
+int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n_variants, const uint8_t* env_variant_host, int num_envs,
+                       int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
+  if (!blobs || !blob_bytes || !out || num_envs < 1 || n_variants < 1 || n_variants > MP_MAX_VARIANTS)
+    return fail(MP_E_INVALID, "mp_create_variants: bad arguments (1..%d variants)", MP_MAX_VARIANTS);
+  *out = nullptr;
+  for (int v = 0; v < n_variants; ++v) if (!blobs[v]) return fail(MP_E_INVALID, "mp_create_variants: null blob %d", v);
+  if (env_variant_host)
+    for (int b = 0; b < num_envs; ++b)
+      if (env_variant_host[b] >= n_variants) return fail(MP_E_INVALID, "mp_create_variants: env %d assigned variant %d of %d", b, env_variant_host[b], n_variants);
+  for (int v = 1; v < n_variants; ++v)
+    if (int rc = same_sections(blobs[0], blob_bytes[0], blobs[v], blob_bytes[v])) {
+      g_error = "variant " + std::to_string(v) + ": " + g_error;
+      return rc;
+    }
+  mp_handle E = nullptr;
+  int rc = mp_create(blobs[0], blob_bytes[0], num_envs, device, seed, env_index_base, flags, &E);
+  if (rc) return rc;
+  if (n_variants > 1) {
+    DeviceGuard guard(device);
+    if ((rc = setup_variants(E, blobs, blob_bytes, n_variants, env_variant_host))) {
+      const std::string msg = g_error;
+      mp_destroy(E);
+      g_error = msg;
+      return rc;
+    }
+  }
+  *out = E;
+  return MP_OK;
+}
+
+int mp_set_env_variants(mp_handle h, const uint8_t* env_variant, void* stream) {
+  if (!h || !env_variant) return fail(MP_E_INVALID, "mp_set_env_variants: null argument");
+  if (h->variants.n < 2) return fail(MP_E_INVALID, "mp_set_env_variants: the engine has one parameter set (create it with mp_create_variants)");
+  DeviceGuard guard(h->device);
+  CUDA_TRY(cudaMemcpyAsync(h->variants.pending, env_variant, (size_t)h->B, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return MP_OK;
+}
+
+int mp_env_variants(mp_handle h, int* n_variants, uint8_t** active, uint8_t** pending) {
+  if (!h) return fail(MP_E_INVALID, "null handle");
+  if (n_variants) *n_variants = h->variants.n;
+  if (active) *active = h->variants.active;
+  if (pending) *pending = h->variants.pending;
   return MP_OK;
 }
 

@@ -157,6 +157,19 @@ int upload_cell_index(FamilyLoad& ld, const Tables& T, const char* name, const S
   return upload(ld.allocs, of, out);
 }
 
+// Per-env variants (mp_create_variants): a family's same_shape(a, b) checks, field by field, that two Params agree on
+// everything outside the family's scalar knobs (what is staged per CTA or shapes per-env state); copy_knobs(dst, src)
+// copies those knobs. The Zapper's knobs are its cooldown, respawn, removal, penalty and reward. MP_SAME compares one field's bytes (Params are value-initialised, so padding and unused array
+// entries are zero) and names it when they differ.
+#define MP_SAME(field)                                                                                                  \
+  if (memcmp(&a.field, &b.field, sizeof(a.field)) != 0)                                                               \
+    return fail(MP_E_UNSUPPORTED, "Params field '%s' differs (variants may differ only in the family's scalar knobs)", #field);
+
+#define MP_SAME_ZAPPER MP_SAME(zap.layer) MP_SAME(zap.sprite) MP_SAME(zap.hit) MP_SAME(zap.geom)
+void copy_zapper_knobs(Zapper& dst, const Zapper& src) {
+  dst.cooldown = src.cooldown; dst.respawn = src.respawn; dst.remove = src.remove; dst.penalty = src.penalty; dst.reward = src.reward;
+}
+
 // The Zapper and episode-ending slots (MPB_FP_*) of clean_up, commons_harvest and territory. The penalty and reward sit
 // in each family's own f64 slots.
 int load_zapper(FamilyLoad& ld, const Tables& T, const int32_t* ip, double penalty, double reward, Zapper& z) {

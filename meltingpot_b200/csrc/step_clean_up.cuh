@@ -70,6 +70,20 @@ struct CleanUp {
     return MP_OK;
   }
 
+  // Host: per-env variants may differ in the Zapper and Cleaner cooldowns and rewards, DirtSpawner, AppleGrow, Edible
+  // and the water Animation's timing; layers, sprites, hits, beam footprints and the number of animation states agree.
+  static int same_shape(const Params& a, const Params& b) {
+    MP_SAME_ZAPPER MP_SAME(apple_layer) MP_SAME(apple_sprite) MP_SAME(dirt_layer) MP_SAME(dirt_sprite) MP_SAME(water_layer) MP_SAME(n_anim)
+    MP_SAME(water_sprite) MP_SAME(clean_layer) MP_SAME(clean_sprite) MP_SAME(clean_hit) MP_SAME(clean_geom) MP_SAME(dirt_count0)
+    return MP_OK;
+  }
+  static void copy_knobs(Params& dst, const Params& src) {
+    copy_zapper_knobs(dst.zap, src.zap);
+    dst.clean_cooldown = src.clean_cooldown; dst.dirt_delay = src.dirt_delay; dst.dirt_prob = src.dirt_prob;
+    dst.grow_rate = src.grow_rate; dst.grow_depletion = src.grow_depletion; dst.grow_restoration = src.grow_restoration;
+    dst.eat_reward = src.eat_reward; dst.anim_frames = src.anim_frames; dst.anim_random = src.anim_random;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

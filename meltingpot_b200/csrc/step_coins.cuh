@@ -47,6 +47,16 @@ struct Coins {
     return MP_OK;
   }
 
+  // Host: per-env variants may differ in the coin rewards, the regrowth rate and the termination rule.
+  static int same_shape(const Params& a, const Params& b) {
+    MP_SAME(coin_layer) MP_SAME(coin_sprite) MP_SAME(coin_type)
+    return MP_OK;
+  }
+  static void copy_knobs(Params& dst, const Params& src) {
+    memcpy(dst.coin_reward, src.coin_reward, sizeof dst.coin_reward);
+    dst.coin_rate = src.coin_rate; dst.terminate = src.terminate; dst.terminate_n = src.terminate_n;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

@@ -8,6 +8,8 @@
 // behaviour into the helpers below as lambdas.
 #pragma once
 
+#include <type_traits>
+
 #include "common.cuh"
 
 __host__ __device__ inline size_t scratch_round16(size_t n) { return (n + 15) & ~(size_t)15; }
@@ -53,21 +55,49 @@ __host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * 
 // mode 0: step (envs whose last step was LAST start a new episode instead, policy A.17)
 // mode 1: reset envs selected by `mask` (all if null)
 //
+// Per-env parameter variants (mp_create_variants): env b runs under params[active[b]]. An episode start first takes the
+// env's pending assignment (active[b] = pending[b]), so a reassignment never changes an episode that is under way.
+// Every variant stages the same per-CTA tables (the compatibility check of mp_create_variants), so stage() reads params[0].
+template <class Params>
+struct ParamVariants {
+  const Params* __restrict__ params;  // [n]
+  uint8_t* active;                    // [B]
+  const uint8_t* pending;             // [B]
+  int n;
+};
+
+// The variant env b advances under: on an episode start its pending assignment, which lane 0 makes the active one; an
+// index outside the set reads as variant 0.
+template <class Params>
+__device__ __forceinline__ const Params& env_params(const ParamVariants<Params>& V, int b, int lane, bool reset) {
+  int k = reset ? V.pending[b] : V.active[b];
+  if (k >= V.n) k = 0;
+  if (reset && lane == 0) V.active[b] = (uint8_t)k;
+  return V.params[k];
+}
+
 // A Family provides: Params (what only its kernel reads), the host-side load(FamilyLoad&, T, Params&) that decodes its
 // blob sections (family_load.h), Scratch, kStagesTables, scratch_bytes(T) per warp, table_bytes(T) per CTA,
 // stage(T, F, tables) (copies static tables into shared memory), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
-// and step(T, F, S, b, lane, actions, sc). F is a grid constant: without it, the compiler copies a small Params that is
-// indexed with a run-time value (coins' coin_reward[who], coop_mining's ore_sprite[state]) to the stack.
-template <class Family>
-__global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant__ typename Family::Params F, State S, const int32_t* __restrict__ actions,
+// and step(T, F, S, b, lane, actions, sc), and on the host same_shape(a, b) and copy_knobs(dst, src) for per-env
+// variants. `Source` is the family's Params (one blob) or ParamVariants<Params>. A single Params is a grid constant:
+// without it, the compiler copies a small Params that is indexed with a run-time value (coins' coin_reward[who],
+// coop_mining's ore_sprite[state]) to the stack, and passed on as it is, it keeps its constant-bank reads. Variants are
+// read through the L1 from the device array.
+template <class Family, class Source = typename Family::Params>
+__global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant__ Source src, State S, const int32_t* __restrict__ actions,
                                                  const uint8_t* __restrict__ mask, int mode) {
+  constexpr bool kVariants = !std::is_same<Source, typename Family::Params>::value;
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // Programmatic dependent launch, both ways: let the renderer that follows in the stream stage its tables while this
   // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   uint8_t* tables = smem + 4 * Family::scratch_bytes(T);
-  if constexpr (Family::kStagesTables) Family::stage(T, F, tables);  // before the dependency wait: the tables never change
+  if constexpr (Family::kStagesTables) {  // before the dependency wait: the tables never change
+    if constexpr (kVariants) Family::stage(T, src.params[0], tables);
+    else Family::stage(T, src, tables);
+  }
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if constexpr (Family::kStagesTables) __syncthreads();
   const int b = blockIdx.x * 4 + warp;
@@ -75,8 +105,15 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
   typename Family::Scratch sc = Family::carve(T, smem + warp * Family::scratch_bytes(T), tables);
   if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
     event_begin(lane);
-    if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, F, S, b, lane, sc);
-    else Family::step(T, F, S, b, lane, actions, sc);
+    if constexpr (kVariants) {
+      const bool reset = mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE];
+      const typename Family::Params& F = env_params(src, b, lane, reset);
+      if (reset) Family::reset(T, F, S, b, lane, sc);
+      else Family::step(T, F, S, b, lane, actions, sc);
+    } else {
+      if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, src, S, b, lane, sc);
+      else Family::step(T, src, S, b, lane, actions, sc);
+    }
     event_end(S, b, lane);
   }
 }

@@ -54,6 +54,18 @@ struct Commons {
     return MP_OK;
   }
 
+  // Host: per-env variants may differ in the Zapper knobs, the DensityRegrow probabilities and the Edible reward.
+  static int same_shape(const Params& a, const Params& b) {
+    MP_SAME_ZAPPER MP_SAME(apple_layer) MP_SAME(apple_sprite) MP_SAME(wait_layer) MP_SAME(wait_sprite) MP_SAME(grass_layer) MP_SAME(grass_sprite)
+    MP_SAME(dess_sprite) MP_SAME(ch_n_wait) MP_SAME(ch_n_probs)
+    return MP_OK;
+  }
+  static void copy_knobs(Params& dst, const Params& src) {
+    copy_zapper_knobs(dst.zap, src.zap);
+    for (int i = 0; i < 4; ++i) dst.ch_probs[i] = src.ch_probs[i];
+    dst.eat_reward = src.eat_reward;
+  }
+
   using Scratch = WarpScratch;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }

@@ -166,6 +166,28 @@ struct Territory {
     return MP_OK;
   }
 
+  // Host: per-env variants may differ in the Zapper knobs, the marking's initial level, recovery, per-level increments,
+  // removals, freezes and rewards, the claim wait and the Resource knobs; layers, sprites, beams, the number of marking
+  // levels and the Taste role agree.
+  static int same_shape(const Params& a, const Params& b) {
+    MP_SAME_ZAPPER MP_SAME(res_layer) MP_SAME(unclaimed_sprite) MP_SAME(tex_layer) MP_SAME(tex_sprite) MP_SAME(ind_layer) MP_SAME(dmg_layer)
+    MP_SAME(dmg_sprite) MP_SAME(mark_layer) MP_SAME(mark_n_levels) MP_SAME(mark_sprite) MP_SAME(brush_layer) MP_SAME(claim_layer)
+    MP_SAME(tr_taste_role) MP_SAME(claimed_sprite) MP_SAME(dry_sprite) MP_SAME(brush_sprite) MP_SAME(claimbeam_sprite)
+    MP_SAME(claim_geom) MP_SAME(brush_geom)
+    return MP_OK;
+  }
+  static void copy_knobs(Params& dst, const Params& src) {
+    copy_zapper_knobs(dst.zap, src.zap);
+    dst.mark_initial_level = src.mark_initial_level; dst.mark_recovery = src.mark_recovery;
+    for (int l = 0; l < 3; ++l) {
+      dst.mark_inc[l] = src.mark_inc[l]; dst.mark_remove[l] = src.mark_remove[l]; dst.mark_freeze[l] = src.mark_freeze[l];
+      dst.mark_src_reward[l] = src.mark_src_reward[l]; dst.mark_tgt_reward[l] = src.mark_tgt_reward[l];
+    }
+    dst.claim_wait = src.claim_wait; dst.res_health0 = src.res_health0; dst.res_reward_delay = src.res_reward_delay;
+    dst.res_repair_delay = src.res_repair_delay; dst.res_reward = src.res_reward; dst.res_rate = src.res_rate;
+    dst.res_repair_prob = src.res_repair_prob;
+  }
+
   using Scratch = TerritoryScratch;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return territory_scratch_bytes(T); }

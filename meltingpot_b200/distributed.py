@@ -94,7 +94,9 @@ class ShardedSubstrate:
   """One rank's shard of a globally indexed batch of env instances."""
 
   def __init__(self, name: str, roles, global_num_envs: int, seed: int, device: Optional[int] = None,
-               world_rgb: bool = True, group=None):
+               world_rgb: bool = True, group=None, prefab_overrides=None, env_variant=None):
+    """prefab_overrides / env_variant: as substrate.build_batched, with env_variant indexed by GLOBAL env; each rank
+    takes the slice of its own envs."""
     import torch.distributed as dist  # pylint: disable=g-import-not-at-top
     from meltingpot_b200 import substrate  # pylint: disable=g-import-not-at-top
     self._group = group
@@ -104,8 +106,14 @@ class ShardedSubstrate:
     if device is None:
       import torch  # pylint: disable=g-import-not-at-top
       device = torch.cuda.current_device()
+    local_variant = None
+    if env_variant is not None:
+      if len(env_variant) != global_num_envs:
+        raise ValueError(f'env_variant has {len(env_variant)} entries for {global_num_envs} envs')
+      local_variant = list(env_variant[self.env_index_base:self.env_index_base + self.local_num_envs])
     self.local = substrate.build_batched(name, roles=roles, num_envs=self.local_num_envs, device=device, seed=seed,
-                                         env_index_base=self.env_index_base, world_rgb=world_rgb)
+                                         env_index_base=self.env_index_base, world_rgb=world_rgb,
+                                         prefab_overrides=prefab_overrides, env_variant=local_variant)
 
   def reset(self):
     return self.local.reset()

@@ -59,7 +59,7 @@ EXPORTED_SYMBOLS = (
     'mp_step_host_async', 'mp_wait', 'mp_exchange_create', 'mp_ipc_export', 'mp_ipc_open', 'mp_enable_peer_access',
     'mp_exchange_connect', 'mp_exchange_wait', 'mp_exchange_slot', 'mp_debug_lane_map', 'mp_debug_observations',
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
-    'mp_last_error', 'mp_version',
+    'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_last_error', 'mp_version',
 )
 
 
@@ -109,6 +109,11 @@ def load_library() -> ctypes.CDLL:
   lib.mp_create.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int,
                             ctypes.c_int, ctypes.c_uint64, ctypes.c_uint64,
                             ctypes.c_uint32, ctypes.POINTER(vp)]
+  lib.mp_create_variants.argtypes = [ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_size_t), ctypes.c_int, vp,
+                                     ctypes.c_int, ctypes.c_int, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint32,
+                                     ctypes.POINTER(vp)]
+  lib.mp_set_env_variants.argtypes = [vp, vp, vp]
+  lib.mp_env_variants.argtypes = [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(vp), ctypes.POINTER(vp)]
   lib.mp_destroy.argtypes = [vp]
   lib.mp_set_flags.argtypes = [vp, ctypes.c_uint32]
   lib.mp_reset.argtypes = [vp, vp, vp]
@@ -201,9 +206,11 @@ class _CudaView:
 class Engine:
   """One engine handle = `num_envs` env instances on one GPU."""
 
-  def __init__(self, blob: bytes, num_envs: int, device: int = 0, seed: int = 1,
-               env_index_base: int = 0, flags: int = MP_FLAG_DEFAULT, render_layout=None):
-    """render_layout: (teams, warps per team, wstrip_log2) to force instead of the engine's choice (diagnostic)."""
+  def __init__(self, blob, num_envs: int, device: int = 0, seed: int = 1,
+               env_index_base: int = 0, flags: int = MP_FLAG_DEFAULT, render_layout=None, env_variant=None):
+    """blob: one compiled substrate, or a list of compatible variants of one (mp_create_variants), e.g. compiled with
+    different `prefab_overrides`; env b then starts under variant env_variant[b] (default 0 for every env).
+    render_layout: (teams, warps per team, wstrip_log2) to force instead of the engine's choice (diagnostic)."""
     if render_layout is not None:
       flags = (flags & ~MP_FLAG_LAYOUT_MASK) | pack_render_layout(*render_layout)
     import torch  # pylint: disable=g-import-not-at-top
@@ -211,17 +218,34 @@ class Engine:
       raise EngineError('CUDA is not available: the CUDA engine has no CPU path')
     self._torch = torch
     self._lib = load_library()
-    self._blob = bytes(blob)
+    blobs = [bytes(b) for b in blob] if isinstance(blob, (list, tuple)) else None
+    self._blob = blobs[0] if blobs else bytes(blob)
     self.device = int(device)
     self.num_envs = int(num_envs)
     torch.cuda.init()
     with torch.cuda.device(self.device):
       torch.cuda.current_stream()  # make sure the primary context exists
     handle = ctypes.c_void_p()
-    _check(self._lib.mp_create(self._blob, len(self._blob), self.num_envs,
-                               self.device, ctypes.c_uint64(seed),
-                               ctypes.c_uint64(env_index_base),
-                               ctypes.c_uint32(flags), ctypes.byref(handle)))
+    if blobs is None:
+      if env_variant is not None:
+        raise ValueError('env_variant needs a list of blobs')
+      _check(self._lib.mp_create(self._blob, len(self._blob), self.num_envs,
+                                 self.device, ctypes.c_uint64(seed),
+                                 ctypes.c_uint64(env_index_base),
+                                 ctypes.c_uint32(flags), ctypes.byref(handle)))
+    else:
+      assign = None
+      if env_variant is not None:
+        ids = np.asarray(env_variant, np.int64).reshape(-1)
+        if ids.shape != (self.num_envs,) or ids.min(initial=0) < 0 or ids.max(initial=0) >= len(blobs):
+          raise ValueError(f'env_variant must hold {self.num_envs} variant indices in 0..{len(blobs) - 1}')
+        assign = np.ascontiguousarray(ids, np.uint8)
+      arr = (ctypes.c_char_p * len(blobs))(*blobs)
+      sizes = (ctypes.c_size_t * len(blobs))(*[len(b) for b in blobs])
+      _check(self._lib.mp_create_variants(arr, sizes, len(blobs), assign.ctypes.data if assign is not None else None,
+                                          self.num_envs, self.device, ctypes.c_uint64(seed),
+                                          ctypes.c_uint64(env_index_base), ctypes.c_uint32(flags),
+                                          ctypes.byref(handle)))
     self._owner = _Handle(self._lib, handle)
     self._h = handle
     bufs = MpBuffers()
@@ -247,10 +271,31 @@ class Engine:
     self.timestep_packed = view(bufs.timestep_packed, (B, P + 2), '<f8', torch.float64)
     self.events = view(bufs.events, (B, bufs.max_events, 3), '<i4', torch.int32)
     self.event_count = view(bufs.event_count, (B,), '<i4', torch.int32)
+    n, active, pending = ctypes.c_int(1), ctypes.c_void_p(), ctypes.c_void_p()
+    _check(self._lib.mp_env_variants(self._h, ctypes.byref(n), ctypes.byref(active), ctypes.byref(pending)))
+    self.num_variants = int(n.value)
+    # uint8 [B]: the variant each env's current episode runs / its next episode will run (None with one variant)
+    self.active_variant = view(active.value, (B,), '|u1', torch.uint8) if active.value else None
+    self.pending_variant = view(pending.value, (B,), '|u1', torch.uint8) if pending.value else None
 
   # -- lifecycle -----------------------------------------------------------------
   _VIEWS = ('rgb', 'world_rgb', 'reward', 'discount', 'step_type', 'scalar_obs', 'avatar_state', 'grid',
-            'timestep_packed', 'events', 'event_count', 'gathered', 'gathered_rgb', 'gathered_world_rgb')
+            'timestep_packed', 'events', 'event_count', 'gathered', 'gathered_rgb', 'gathered_world_rgb',
+            'active_variant', 'pending_variant')
+
+  def set_env_variant(self, ids, stream=None) -> None:
+    """Assigns env b to variant ids[b] from its next episode start on (the auto-reset after LAST or a reset); an
+    episode under way keeps its parameters. Reset envs with a mask to switch them at once."""
+    torch = self._torch
+    ids = torch.as_tensor(ids)
+    if self.num_variants < 2:
+      raise ValueError('set_env_variant needs an engine built from a list of blobs')
+    if ids.shape != (self.num_envs,) or bool((ids < 0).any()) or bool((ids >= self.num_variants).any()):
+      raise ValueError(f'ids must hold {self.num_envs} variant indices in 0..{self.num_variants - 1}')
+    ids = ids.to(device=torch.device('cuda', self.device), dtype=torch.uint8).contiguous()
+    stream = torch.cuda.current_stream(self.device) if stream is None else stream
+    _check(self._lib.mp_set_env_variants(self._h, ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(stream.cuda_stream)))
+    ids.record_stream(stream)  # the copy reads `ids` on `stream`
 
   def close(self) -> None:
     """Drops this object's references. mp_destroy runs when the last tensor view handed out has been released too

@@ -165,20 +165,23 @@ class BatchedSubstrate:
   next `step`/`reset`; clone what must be kept.
   """
 
-  def __init__(self, blob: bytes, num_envs: int, device: int = 0, seed: Optional[int] = None,
-               env_index_base: int = 0, world_rgb: bool = True):
+  def __init__(self, blob, num_envs: int, device: int = 0, seed: Optional[int] = None,
+               env_index_base: int = 0, world_rgb: bool = True, env_variant=None):
+    """blob: a compiled substrate, or a list of variants of one (e.g. compiled with different `prefab_overrides`),
+    env b starting under variant env_variant[b] (see Engine)."""
     from meltingpot_b200 import engine as engine_lib  # pylint: disable=g-import-not-at-top
     if seed is None:
       seed = int(np.random.randint(1, _MAX_SEED))
-    self._info = _info(blob)
+    first = blob[0] if isinstance(blob, (list, tuple)) else blob
+    self._info = _info(first)
     flags = engine_lib.MP_FLAG_RENDER_PLAYERS | (engine_lib.MP_FLAG_RENDER_WORLD if world_rgb else 0)
     self._engine = engine_lib.Engine(blob, num_envs, device=device, seed=seed,
-                                     env_index_base=env_index_base, flags=flags)
+                                     env_index_base=env_index_base, flags=flags, env_variant=env_variant)
     self.num_envs = num_envs
     self.num_players = self._engine.num_players
     self.num_actions = self._engine.num_actions
     self.seed = seed
-    sections = blob_lib.unpack(blob)
+    sections = blob_lib.unpack(first)
     self._scalar_names = [_SCALAR_NAMES[int(k)] for k in sections['scalar_obs']]
     self._world_rgb = world_rgb
 
@@ -207,6 +210,10 @@ class BatchedSubstrate:
       actions = actions.to(torch.int32)
     self._engine.step(actions.contiguous())
     return self._timestep()
+
+  def set_env_variant(self, ids) -> None:
+    """Moves env b to variant ids[b] from its next episode start on (reset(mask) to switch at once)."""
+    self._engine.set_env_variant(ids)
 
   def debug_observations(self, layer: bool = True, zap_matrix: bool = True):
     """The reference's debug observations of the current timestep as int32 tensors: 'POSITION' [B, P, 2],
@@ -434,11 +441,21 @@ class SubstrateFactory:
     return Substrate(blob, self._config, device=self._device, env_seed=env_seed)
 
   def build_batched(self, roles: Sequence[str], num_envs: int, seed: Optional[int] = None,
-                    env_index_base: int = 0, world_rgb: bool = True) -> BatchedSubstrate:
+                    env_index_base: int = 0, world_rgb: bool = True, prefab_overrides=None,
+                    env_variant=None) -> BatchedSubstrate:
     _validate_roles(self._config, roles)
-    blob = substrate_blobs.load_blob(self._name, tuple(roles))
+    if prefab_overrides is None:
+      if env_variant is not None:
+        raise ValueError('env_variant needs a sequence of prefab_overrides')
+      blob = substrate_blobs.load_blob(self._name, tuple(roles))
+    elif isinstance(prefab_overrides, Mapping):  # one parameter set for every env
+      if env_variant is not None:
+        raise ValueError('env_variant needs a sequence of prefab_overrides')
+      blob = substrate_blobs.compile_with_overrides(self._name, tuple(roles), prefab_overrides)
+    else:  # one variant per entry
+      blob = [substrate_blobs.compile_with_overrides(self._name, tuple(roles), o) for o in prefab_overrides]
     return BatchedSubstrate(blob, num_envs, device=self._device, seed=seed,
-                            env_index_base=env_index_base, world_rgb=world_rgb)
+                            env_index_base=env_index_base, world_rgb=world_rgb, env_variant=env_variant)
 
 
 def get_factory(name: str, device: int = 0) -> SubstrateFactory:
@@ -461,7 +478,12 @@ def build_from_config(config: config_dict.ConfigDict, *, roles: Sequence[str],
 
 def build_batched(name: str, *, roles: Sequence[str], num_envs: int, device: int = 0,
                   seed: Optional[int] = None, env_index_base: int = 0,
-                  world_rgb: bool = True) -> BatchedSubstrate:
-  """Builds `num_envs` instances on one GPU; see `BatchedSubstrate`."""
-  return get_factory(name, device).build_batched(roles, num_envs, seed=seed,
-                                                 env_index_base=env_index_base, world_rgb=world_rgb)
+                  world_rgb: bool = True, prefab_overrides=None, env_variant=None) -> BatchedSubstrate:
+  """Builds `num_envs` instances on one GPU; see `BatchedSubstrate`.
+
+  `prefab_overrides` (the reference builder's, builder.py:70-87) is one mapping for every env, or a sequence of
+  mappings: a heterogeneous batch whose env b runs variant env_variant[b] (default 0). Compiling overrides needs a
+  reference checkout."""
+  return get_factory(name, device).build_batched(roles, num_envs, seed=seed, env_index_base=env_index_base,
+                                                 world_rgb=world_rgb, prefab_overrides=prefab_overrides,
+                                                 env_variant=env_variant)

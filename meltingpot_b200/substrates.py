@@ -53,6 +53,16 @@ def load_blob(name: str, roles: Optional[Sequence[str]] = None) -> bytes:
   return compiler.compile_substrate(name, roles, build_seed=BUILD_SEEDS.get(name))
 
 
+def compile_with_overrides(name: str, roles: Sequence[str], prefab_overrides) -> bytes:
+  """The blob of `name` with `roles` and the reference's `prefab_overrides` (compiled from a reference checkout)."""
+  from meltingpot_b200 import compiler  # pylint: disable=g-import-not-at-top
+  if compiler.reference_root() is None:
+    raise FileNotFoundError(
+        f'prefab_overrides for {name!r} need a Melting Pot reference checkout to compile from '
+        '(set MELTINGPOT_REFERENCE_ROOT)')
+  return compiler.compile_substrate(name, roles, build_seed=BUILD_SEEDS.get(name), prefab_overrides=prefab_overrides)
+
+
 def _is_default_role(name: str, role: str) -> bool:
   del name
   return role == 'default'
