@@ -61,7 +61,7 @@ enum {
 #define MP_FLAGS_CREATE_ONLY (MP_FLAG_DEBUG_PLAIN_LANE_MAP | MP_FLAG_DEBUG_SCATTER_LANE_MAP | MP_FLAG_DEBUG_NO_PREMERGE | MP_FLAG_LAYOUT_MASK)
 
 /* Device buffers owned by the engine; valid until mp_destroy. Contents are overwritten by the
- * next mp_step/mp_reset on the same handle. B = num_envs, P = players. */
+ * next mp_step/mp_reset on the same handle (mp_step_into / mp_reset_into: see there for the images). B = num_envs, P = players. */
 typedef struct mp_buffers {
   int32_t num_envs, num_players;
   int32_t rgb_h, rgb_w;     /* per-player view in pixels (88 x 88 for clean_up) */
@@ -163,6 +163,36 @@ int mp_reset(mp_handle h, const uint8_t* env_mask, void* stream);
  * all observations. Asynchronous on `stream`. */
 int mp_step(mp_handle h, const int32_t* actions, void* stream);
 
+/* Caller-owned DEVICE outputs of one step, e.g. slot t of a learner's [T, B, ...] or [B, T, ...] trajectory buffer.
+ * Every pointer is optional (NULL: that output is not delivered by this call). Each output is B per-env records at a
+ * byte stride between env b and b + 1; inside a record the layout is that of mp_buffers. */
+typedef struct mp_device_outputs {
+  uint8_t* rgb;       uint64_t rgb_env_stride;        /* [B] x (u8 [P][rgb_h][rgb_w][3], dense) */
+  uint8_t* world_rgb; uint64_t world_rgb_env_stride;  /* [B] x (u8 [world_h][world_w][3], dense) */
+  double*  reward;    uint64_t reward_env_stride;     /* [B] x f64 [P] */
+  double*  discount;  uint64_t discount_env_stride;   /* [B] x f64 */
+  int64_t* step_type; uint64_t step_type_env_stride;  /* [B] x i64 */
+  double*  scalar_obs; uint64_t scalar_obs_env_stride, scalar_obs_stride; /* [n_scalar] x [B] x f64 [P] */
+} mp_device_outputs;
+
+/* mp_step / mp_reset whose outputs go into `out` (any subset):
+ *   - the images named in `out` are stored by the renderer straight into `out` (no second pass over HBM) and the
+ *     engine's own images are not written; an image `out` leaves NULL is rendered into the engine's own set as usual;
+ *   - reward, discount, step type and scalar observations are written to the engine's scalar block as always (the
+ *     exchange, the host paths and mp_buffers read them there) and also delivered into `out` by the kernel that follows
+ *     the state transition, so the call launches exactly as many kernels as mp_step / mp_reset (with rendering off and
+ *     no exchange connected, the rows travel by device-to-device copies on `stream`);
+ *   - afterwards mp_buffers holds that step's state and scalars, plus the images of the last render into the engine's
+ *     own set (as after a slot-1 mp_step_host_async call).
+ * Every check runs before anything is enqueued; a refused call (MP_E_INVALID) steps no env. Refused: image pointers or
+ * image env strides that are not multiples of 16 (the TMA bulk store's alignment); scalar pointers or strides that are
+ * not multiples of 8, or of 2 GiB or more; an env stride smaller than one env's bytes; scalar_obs rows (n_scalar x B
+ * rows of P doubles) that overlap, or scalar_obs on a substrate without scalar observations; an image the current render
+ * flags switch off; an output whose extent does not lie in one device allocation on the engine's device; outputs whose
+ * extents overlap each other or the engine's own buffers. */
+int mp_step_into(mp_handle h, const int32_t* actions, const mp_device_outputs* out, void* stream);
+int mp_reset_into(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, void* stream);
+
 /* State transition only / rendering only (mp_step == mp_step_state + mp_render). */
 int mp_step_state(mp_handle h, const int32_t* actions, void* stream);
 int mp_render(mp_handle h, void* stream);
@@ -197,8 +227,9 @@ int mp_reset_host(mp_handle h, const mp_host_outputs* out, void* stream);
  * until mp_wait on the same slot returns. Steps are still applied in call order (one state per env). A call refused
  * with an error (e.g. `out` names events, which are not staged per slot) enqueues nothing and steps no env.
  * Slot 0 renders into the engine's own images (mp_buffers.rgb / world_rgb); every other call that renders there
- * (mp_step, mp_render, mp_step_host, mp_reset, mp_reset_host, mp_state_load) first waits, on its stream, for slot 0's
- * copy-out, so it may be issued before mp_wait(h, 0). Slot 1 renders into a set of its own: after a slot-1 call,
+ * (mp_step, mp_render, mp_step_host, mp_reset, mp_reset_host, mp_state_load, and mp_step_into / mp_reset_into when
+ * `out` leaves a rendered image NULL) first waits, on its stream, for slot 0's copy-out, so it may be issued before
+ * mp_wait(h, 0). Slot 1 renders into a set of its own, as mp_step_into does into a dense target: after a slot-1 call,
  * mp_buffers holds that step's scalars and state, and the images of the last render into the engine's own set. */
 int mp_step_host_async(mp_handle h, const int32_t* actions_host, const mp_host_outputs* out, int slot, void* stream);
 int mp_wait(mp_handle h, int slot);

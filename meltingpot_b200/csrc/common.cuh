@@ -76,6 +76,17 @@ struct Tables {
   const uint8_t* sprite_pair;    // [n_total][n_total] pre-merged sprite for (opaque base, sprite on top) or 0
 };
 
+// Caller-owned destinations of a step's scalar outputs (mp_device_outputs): any pointer may be null. Strides in bytes;
+// scalar_obs row (k, b) starts at scalar_obs + k * scalar_obs_stride + b * scalar_obs_env_stride.
+struct ScalarTargets {
+  double* reward;
+  double* discount;
+  int64_t* step_type;
+  double* scalar_obs;
+  uint64_t reward_stride, discount_stride, step_type_stride, scalar_obs_env_stride, scalar_obs_stride;
+  int on;  // any of the four is set
+};
+
 struct State {
   int B;
   uint64_t seed;  // key of env b = seed + b (env_index_base already folded in)
@@ -118,6 +129,11 @@ struct State {
   uint8_t* g_rgb[MP_MAX_PEERS];
   uint8_t* g_wrgb[MP_MAX_PEERS];
   const unsigned long long* g_flags;       // local flags[r] = last render rank r has fully delivered here
+  // Where k_render stores env b's images: rgb + b * rgb_env_stride (player p at + p * player_bytes) and
+  // world_rgb + b * world_env_stride, in bytes. The engine's own images are the dense case; mp_step_into points them at
+  // a caller's tensors. (Kept behind every field the state-transition kernels read.)
+  uint64_t rgb_env_stride, world_env_stride;
+  ScalarTargets out;                       // the step's scalar rows into caller-owned memory (mp_step_into), or none
 };
 
 // Events of the current step (the reference's events:add calls on the hot path). Types follow
@@ -224,10 +240,36 @@ __device__ __forceinline__ void exchange_push(const Tables& T, const State& S) {
   }
 }
 
+// Delivery of the step's reward, discount, step type and scalar observations from the engine's scalar block into the
+// caller's rows (State::out), by the kernel that follows the state transition, like exchange_push: one warp per env,
+// called by every thread of every CTA of the delivering grid.
+__device__ __forceinline__ void deliver_scalars(const Tables& T, const State& S) {
+  const ScalarTargets& o = S.out;
+  if (!o.on) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = (int)blockDim.x >> 5;
+  const int P = T.P, n = P + 2 + (o.scalar_obs ? T.n_scalar * P : 0);
+  for (int b = (int)blockIdx.x + warp * (int)gridDim.x; b < S.B; b += n_warps * (int)gridDim.x) {
+    for (int i = lane; i < n; i += 32) {
+      if (i < P) {
+        if (o.reward) reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.reward) + b * o.reward_stride)[i] = S.reward[(size_t)b * P + i];
+      } else if (i == P) {
+        if (o.discount) *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.discount) + b * o.discount_stride) = S.discount[b];
+      } else if (i == P + 1) {
+        if (o.step_type) *reinterpret_cast<int64_t*>(reinterpret_cast<uint8_t*>(o.step_type) + b * o.step_type_stride) = S.step_type[b];
+      } else {
+        const int k = (i - P - 2) / P, p = i - P - 2 - k * P;
+        reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.scalar_obs) + k * o.scalar_obs_stride + b * o.scalar_obs_env_stride)[p] =
+            S.scalar_obs[((size_t)k * S.B + b) * P + p];
+      }
+    }
+  }
+}
+
 // Delivery when no render follows the state transition (mp_step_state on its own, or rendering switched off).
 __global__ void __launch_bounds__(256) k_exchange_push(Tables T, State S) {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   exchange_push(T, S);
+  deliver_scalars(T, S);
 }
 
 // The consumer side, enqueued by EVERY rank after its step (mp_exchange_wait; stream-ordered after the kernel that

@@ -638,9 +638,10 @@ __global__ void k_debug_obs(Tables T, State S, int32_t* position, int32_t* orien
   }
 }
 
-int raise_flags(mp_engine* E, cudaStream_t st) {
+// `S`: the engine's state with the step's targets applied (apply_outputs), for the scalar rows k_exchange_push delivers.
+int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
   E->x_pending_raise = false;
-  k_exchange_push<<<std::min(E->sm_count, (E->B + 7) / 8), 256, 0, st>>>(E->T, E->S);
+  k_exchange_push<<<std::min(E->sm_count, (E->B + 7) / 8), 256, 0, st>>>(E->T, S);
   ++E->launches;
   CUDA_TRY(cudaGetLastError());
   return MP_OK;
@@ -660,18 +661,50 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode));
   if (E->S.x_world) {
     E->x_pending_raise = true;
-    if (!render_follows) { ++E->launches; return raise_flags(E, st); }
+    if (!render_follows) { ++E->launches; return raise_flags(E, st, E->S); }
   }
   ++E->launches;
   CUDA_TRY(cudaGetLastError());
   return MP_OK;
 }
 
-int launch_render(mp_engine* E, cudaStream_t st) {
-  if (!(E->flags & (MP_FLAG_RENDER_WORLD | MP_FLAG_RENDER_PLAYERS))) return E->x_pending_raise ? raise_flags(E, st) : MP_OK;
+// Points a launch's copy of the state at the targets of `o` (checked by check_device_outputs, or the engine's own
+// second image set of mp_step_host_async slot 1): the images it names replace the engine's own, its scalar rows are added.
+void apply_outputs(const mp_device_outputs& o, State& S) {
+  if (o.rgb) { S.rgb = o.rgb; S.rgb_env_stride = o.rgb_env_stride; }
+  if (o.world_rgb) { S.world_rgb = o.world_rgb; S.world_env_stride = o.world_rgb_env_stride; }
+  S.out = ScalarTargets{o.reward, o.discount, o.step_type, o.scalar_obs, o.reward_env_stride, o.discount_env_stride,
+                        o.step_type_env_stride, o.scalar_obs_env_stride, o.scalar_obs_stride, 0};
+  S.out.on = o.reward || o.discount || o.step_type || o.scalar_obs;
+}
+
+// The scalar rows of a step that no kernel follows (rendering off, no exchange): strided device-to-device copies, so
+// that a step into a target launches no more kernels than a plain one.
+int copy_scalars(mp_engine* E, const ScalarTargets& o, cudaStream_t st) {
+  const size_t B = E->B, P = E->T.P;
+  const State& S = E->S;
+  if (o.reward) CUDA_TRY(cudaMemcpy2DAsync(o.reward, o.reward_stride, S.reward, P * 8, P * 8, B, cudaMemcpyDeviceToDevice, st));
+  if (o.discount) CUDA_TRY(cudaMemcpy2DAsync(o.discount, o.discount_stride, S.discount, 8, 8, B, cudaMemcpyDeviceToDevice, st));
+  if (o.step_type) CUDA_TRY(cudaMemcpy2DAsync(o.step_type, o.step_type_stride, S.step_type, 8, 8, B, cudaMemcpyDeviceToDevice, st));
+  for (int k = 0; o.scalar_obs && k < E->T.n_scalar; ++k)
+    CUDA_TRY(cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(o.scalar_obs) + k * o.scalar_obs_stride, o.scalar_obs_env_stride,
+                               S.scalar_obs + k * B * P, P * 8, P * 8, B, cudaMemcpyDeviceToDevice, st));
+  return MP_OK;
+}
+
+// `out`: where this render's outputs go besides / instead of the engine's own buffers (see apply_outputs), or null.
+int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = nullptr) {
+  const bool players = E->flags & MP_FLAG_RENDER_PLAYERS, world = E->flags & MP_FLAG_RENDER_WORLD;
+  if (!players && !world) {
+    State S = E->S;
+    if (out) apply_outputs(*out, S);
+    if (E->x_pending_raise) return raise_flags(E, st, S);
+    return S.out.on ? copy_scalars(E, S.out, st) : MP_OK;
+  }
   // The engine's own images are also slot 0's of mp_step_host_async: a render into them must not start before that
-  // slot's device->host copy has read them, whichever call issues it. (The slot-1 render has its own set.)
-  if (E->async_ready && E->S.rgb != E->slot[1].rgb) CUDA_TRY(cudaStreamWaitEvent(st, E->slot[0].copied, 0));
+  // slot's device->host copy has read them, whichever call issues it. (A render into a target does not touch them.)
+  const bool own_images = (players && !(out && out->rgb)) || (world && !(out && out->world_rgb));
+  if (E->async_ready && own_images) CUDA_TRY(cudaStreamWaitEvent(st, E->slot[0].copied, 0));
   E->S.x_raise = E->x_pending_raise ? 1 : 0;
   E->x_pending_raise = false;
   const int blocks = std::min(E->B, E->sm_count);  // every CTA has at least one env (balanced rounds + cooperative tail)
@@ -701,7 +734,9 @@ int launch_render(mp_engine* E, cudaStream_t st) {
       E->S.g_wrgb[r] = base + E->g_world_off + (size_t)E->g_rank * E->B * R.world_bytes;
     }
   }
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, gather ? E->render_gather_fn : E->render_fn, E->T, E->S, R, E->flags));
+  State S = E->S;
+  if (out) apply_outputs(*out, S);
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, gather ? E->render_gather_fn : E->render_fn, E->T, S, R, E->flags));
   if (gather) {
     k_gather_raise<<<1, 32, 0, st>>>(E->d_g_flag_ptrs, E->g_world, E->g_rank, E->g_seq);
     ++E->launches;
@@ -791,6 +826,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     S.step_type = reinterpret_cast<int64_t*>(S.discount + B);
     S.scalar_obs = reinterpret_cast<double*>(S.step_type + B);
   }
+  S.rgb_env_stride = P * E->R.player_bytes; S.world_env_stride = E->R.world_bytes;  // the own images: dense
   {  // everything a later step depends on, plus the current timestep scalars; the images are re-rendered on load
     const size_t ns = std::max<size_t>(1, T.n_scalar);
     auto span = [&](void* p, size_t bytes) { E->state_spans.push_back({p, bytes}); E->state_bytes += bytes; };
@@ -1036,6 +1072,115 @@ int mp_step(mp_handle h, const int32_t* actions, void* stream) {
   return rc ? rc : mp_render(h, stream);
 }
 
+}  // extern "C"
+
+namespace {
+// Every check of mp_step_into / mp_reset_into (include/mp_engine.h), before anything is enqueued: a pointer that fails
+// one never reaches a kernel. Extents are computed in 128 bits, so no stride can wrap them around.
+int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn) {
+  if (!o) return fail(MP_E_INVALID, "%s: null outputs (use mp_step / mp_reset)", fn);
+  typedef unsigned __int128 u128;
+  const uint64_t B = E->B, P = E->T.P, n = E->T.n_scalar;
+  struct Out { const char* name; uintptr_t p; u128 extent; };
+  std::vector<Out> outs;
+  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_env, uint64_t align, u128 extra) -> int {
+    if (!p) return MP_OK;
+    if ((uintptr_t)p % align || stride % align)
+      return fail(MP_E_INVALID, "%s: %s pointer or env stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
+    if (stride < per_env)
+      return fail(MP_E_INVALID, "%s: %s env stride of %llu bytes is smaller than one env's %llu bytes", fn, name,
+                  (unsigned long long)stride, (unsigned long long)per_env);
+    if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s env stride of 2 GiB or more", fn, name);
+    outs.push_back({name, (uintptr_t)p, (u128)(B - 1) * stride + per_env + extra});
+    return MP_OK;
+  };
+  if (o->rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
+  if (o->world_rgb && !(E->flags & MP_FLAG_RENDER_WORLD)) return fail(MP_E_INVALID, "%s: world_rgb asked for, but the render flags switch WORLD.RGB off", fn);
+  if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
+  if (o->scalar_obs && o->scalar_obs_stride % 8) return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes", fn);
+  int rc;
+  if ((rc = add("rgb", o->rgb, o->rgb_env_stride, P * E->R.player_bytes, 16, 0)) ||
+      (rc = add("world_rgb", o->world_rgb, o->world_rgb_env_stride, (uint64_t)E->R.world_bytes, 16, 0)) ||
+      (rc = add("reward", o->reward, o->reward_env_stride, P * 8, 8, 0)) ||
+      (rc = add("discount", o->discount, o->discount_env_stride, 8, 8, 0)) ||
+      (rc = add("step_type", o->step_type, o->step_type_env_stride, 8, 8, 0)) ||
+      (rc = add("scalar_obs", o->scalar_obs, o->scalar_obs_env_stride, P * 8, 8, (u128)(n - 1) * o->scalar_obs_stride)))
+    return rc;
+  for (const Out& x : outs)
+    if (x.extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, x.name);
+  if (o->scalar_obs) {
+    // The n x B rows of P doubles start at k * s + b * e. Rows of one k are e >= P * 8 apart; rows j = k' - k apart
+    // are |j * s + m * e| apart, m = b' - b in [-(B - 1), B - 1], closest at m = -floor(j * s / e) or one below.
+    const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_env_stride;
+    for (uint64_t j = 1; j < n; ++j) {
+      const u128 d = (u128)j * s, q = d / e, r = d % e;
+      const u128 gap = q > B - 1 ? d - (u128)(B - 1) * e : (q + 1 <= B - 1 ? std::min<u128>(r, e - r) : r);
+      if (gap < P * 8) return fail(MP_E_INVALID, "%s: scalar_obs rows overlap (env stride %llu, stride %llu bytes)", fn,
+                                   (unsigned long long)e, (unsigned long long)s);
+    }
+  }
+  // each extent inside one device allocation on the engine's device (cuMemGetAddressRange through the runtime's driver
+  // entry point, as mp_ipc_export does, so the library does not link libcuda)
+  typedef int (*GetRange)(unsigned long long*, size_t*, unsigned long long);
+  void* range_fn = nullptr;
+  cudaDriverEntryPointQueryResult qr;
+  CUDA_TRY(cudaGetDriverEntryPoint("cuMemGetAddressRange", &range_fn, cudaEnableDefault, &qr));
+  if (!range_fn || qr != cudaDriverEntryPointSuccess) return fail(MP_E_CUDA, "cuMemGetAddressRange is not available");
+  for (const Out& x : outs) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, (const void*)x.p) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(MP_E_INVALID, "%s: %s is not a device pointer", fn, x.name);
+    }
+    if (a.type != cudaMemoryTypeDevice) return fail(MP_E_INVALID, "%s: %s is not device memory", fn, x.name);
+    if (a.device != E->device) return fail(MP_E_INVALID, "%s: %s lies on device %d, the engine runs on device %d", fn, x.name, a.device, E->device);
+    unsigned long long base = 0;
+    size_t size = 0;
+    if (reinterpret_cast<GetRange>(range_fn)(&base, &size, (unsigned long long)x.p) != 0)
+      return fail(MP_E_INVALID, "%s: %s is not in a device allocation", fn, x.name);
+    if ((u128)x.p + x.extent > (u128)base + size)
+      return fail(MP_E_INVALID, "%s: %s runs %llu bytes past the end of its allocation", fn, x.name,
+                  (unsigned long long)((u128)x.p + x.extent - ((u128)base + size)));
+  }
+  // no extent overlaps another output or the engine's own buffers
+  std::vector<std::pair<uintptr_t, uint64_t>> own;
+  for (const auto& sp : E->state_spans) own.push_back({(uintptr_t)sp.first, sp.second});
+  own.push_back({(uintptr_t)E->S.rgb, B * P * E->R.player_bytes});
+  own.push_back({(uintptr_t)E->S.world_rgb, B * E->R.world_bytes});
+  if (E->async_ready) {
+    own.push_back({(uintptr_t)E->slot[1].rgb, B * P * E->R.player_bytes});
+    own.push_back({(uintptr_t)E->slot[1].world_rgb, B * E->R.world_bytes});
+  }
+  for (size_t i = 0; i < outs.size(); ++i) {
+    const u128 lo = outs[i].p, hi = lo + outs[i].extent;
+    for (size_t j = i + 1; j < outs.size(); ++j)
+      if (lo < (u128)outs[j].p + outs[j].extent && (u128)outs[j].p < hi)
+        return fail(MP_E_INVALID, "%s: %s and %s overlap", fn, outs[i].name, outs[j].name);
+    for (const auto& sp : own)
+      if (lo < (u128)sp.first + sp.second && (u128)sp.first < hi) return fail(MP_E_INVALID, "%s: %s overlaps the engine's own buffers", fn, outs[i].name);
+  }
+  return MP_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int mp_step_into(mp_handle h, const int32_t* actions, const mp_device_outputs* out, void* stream) {
+  if (!h || !actions) return fail(MP_E_INVALID, "mp_step_into: null handle or actions");
+  DeviceGuard guard(h->device);
+  int rc = check_device_outputs(h, out, "mp_step_into");
+  if (!rc) rc = launch_state(h, actions, nullptr, 0, (cudaStream_t)stream);
+  return rc ? rc : launch_render(h, (cudaStream_t)stream, out);
+}
+
+int mp_reset_into(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, void* stream) {
+  if (!h) return fail(MP_E_INVALID, "null handle");
+  DeviceGuard guard(h->device);
+  int rc = check_device_outputs(h, out, "mp_reset_into");
+  if (!rc) rc = launch_state(h, nullptr, env_mask, 1, (cudaStream_t)stream);
+  return rc ? rc : launch_render(h, (cudaStream_t)stream, out);
+}
+
 int mp_get_buffers(mp_handle h, mp_buffers* out) {
   if (!h || !out) return fail(MP_E_INVALID, "null argument");
   *out = h->buffers;
@@ -1100,11 +1245,12 @@ int mp_step_host_async(mp_handle h, const int32_t* actions_host, const mp_host_o
   CUDA_TRY(cudaStreamWaitEvent(st, sl.copied, 0));  // the copy-out that last used this slot's device buffers has drained
   CUDA_TRY(cudaMemcpyAsync(sl.actions, actions_host, (size_t)h->B * h->T.P * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   if ((rc = launch_state(h, sl.actions, nullptr, 0, st))) return rc;
-  uint8_t* rgb0 = h->S.rgb; uint8_t* world0 = h->S.world_rgb;
-  h->S.rgb = sl.rgb; h->S.world_rgb = sl.world_rgb;
-  rc = launch_render(h, st);
-  h->S.rgb = rgb0; h->S.world_rgb = world0;
-  if (rc) return rc;
+  mp_device_outputs second{};  // slot 1: a dense target in the engine's second image set
+  if (slot == 1) {
+    if (h->flags & MP_FLAG_RENDER_PLAYERS) { second.rgb = sl.rgb; second.rgb_env_stride = (uint64_t)h->T.P * h->R.player_bytes; }
+    if (h->flags & MP_FLAG_RENDER_WORLD) { second.world_rgb = sl.world_rgb; second.world_rgb_env_stride = (uint64_t)h->R.world_bytes; }
+  }
+  if ((rc = launch_render(h, st, slot == 1 ? &second : nullptr))) return rc;
   CUDA_TRY(cudaMemcpyAsync(sl.scalars, h->scalar_block, h->scalar_block_bytes, cudaMemcpyDeviceToDevice, st));
   CUDA_TRY(cudaEventRecord(sl.computed, st));
   CUDA_TRY(cudaStreamWaitEvent(h->copy_stream, sl.computed, 0));

@@ -406,9 +406,12 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
         if (!(flags & 128u)) fence_async_smem();  // make this lane's writes visible to the async (TMA) proxy
         __syncwarp();
         if (lane == 0 && !(flags & 32u)) {
-          const size_t off = ((size_t)b * T.P + p) * R.player_bytes + (size_t)cy * R.pitem_bytes;
-          bulk_store(S.rgb + off, buf, (uint32_t)R.pitem_bytes, store_policy);
-          if (GATHER) for (int r = 0; r < S.g_world; ++r) bulk_store(S.g_rgb[r] + off, buf, (uint32_t)R.pitem_bytes, store_policy);
+          const size_t in_env = (size_t)p * R.player_bytes + (size_t)cy * R.pitem_bytes;
+          bulk_store(S.rgb + b * S.rgb_env_stride + in_env, buf, (uint32_t)R.pitem_bytes, store_policy);
+          if (GATHER) {  // the stacked slots stay dense, whatever the local target's stride
+            const size_t off = (size_t)b * T.P * R.player_bytes + in_env;
+            for (int r = 0; r < S.g_world; ++r) bulk_store(S.g_rgb[r] + off, buf, (uint32_t)R.pitem_bytes, store_policy);
+          }
         }
       } else {
         const int wi = item - R.n_player_items, wy = wi >> (3 - wlog);
@@ -434,15 +437,20 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
         if (!(flags & 128u)) fence_async_smem();
         __syncwarp();
         if (lane == 0 && !(flags & 32u)) {
-          const size_t off = (size_t)b * R.world_bytes + (size_t)wi * R.witem_bytes;
-          bulk_store(S.world_rgb + off, buf, (uint32_t)R.witem_bytes, store_policy);
-          if (GATHER) for (int r = 0; r < S.g_world; ++r) bulk_store(S.g_wrgb[r] + off, buf, (uint32_t)R.witem_bytes, store_policy);
+          const size_t in_env = (size_t)wi * R.witem_bytes;
+          bulk_store(S.world_rgb + b * S.world_env_stride + in_env, buf, (uint32_t)R.witem_bytes, store_policy);
+          if (GATHER) {
+            const size_t off = (size_t)b * R.world_bytes + in_env;
+            for (int r = 0; r < S.g_world; ++r) bulk_store(S.g_wrgb[r] + off, buf, (uint32_t)R.witem_bytes, store_policy);
+          }
         }
       }
     }
-    // this rank's timestep rows -> every rank's gathered buffer: by each warp once it has run out of strips of its first
-    // env, so the loads and the remote stores overlap the other warps' drawing instead of delaying the kernel's start
+    // this rank's timestep rows -> every rank's gathered buffer (and the step's scalar rows -> the caller's target): by
+    // each warp once it has run out of strips of its first env, so the loads and the stores overlap the other warps'
+    // drawing instead of delaying the kernel's start
     if (S.x_raise && it == 0) exchange_push(T, S);
+    if (S.out.on && it == 0) deliver_scalars(T, S);  // (tested here, not only inside: measured, k_render<3, 3, true> spills otherwise)
     group_sync(bar_id, gthreads);  // every warp is done with s_rec / s_view
     if (gtid == 0) *next_ctr = 0;
     // (the reset is ordered before the next env's item loop by the group barrier after its cell pass)

@@ -115,11 +115,12 @@ class ShardedSubstrate:
                                          env_index_base=self.env_index_base, world_rgb=world_rgb,
                                          prefab_overrides=prefab_overrides, env_variant=local_variant)
 
-  def reset(self):
-    return self.local.reset()
+  def reset(self, out=None):
+    """out: a BatchedTimeStep of this rank's envs to fill (BatchedSubstrate.step)."""
+    return self.local.reset(out=out)
 
-  def step(self, local_actions):
-    return self.local.step(local_actions)
+  def step(self, local_actions, out=None):
+    return self.local.step(local_actions, out=out)
 
   # -- engine-level exchanges (peer-memory stores from the kernels; no collective per step) ---------------------------
   def connect(self, observations: bool = False) -> None:

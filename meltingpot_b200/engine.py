@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Dict, Optional
+from typing import Any, Dict, Mapping, NamedTuple, Optional, Tuple
 
 import numpy as np
 
@@ -59,7 +59,8 @@ EXPORTED_SYMBOLS = (
     'mp_step_host_async', 'mp_wait', 'mp_exchange_create', 'mp_ipc_export', 'mp_ipc_open', 'mp_enable_peer_access',
     'mp_exchange_connect', 'mp_exchange_wait', 'mp_exchange_slot', 'mp_debug_lane_map', 'mp_debug_observations',
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
-    'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_last_error', 'mp_version',
+    'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
+    'mp_version',
 )
 
 
@@ -92,6 +93,71 @@ class MpHostOutputs(ctypes.Structure):
   ]
 
 
+class MpDeviceOutputs(ctypes.Structure):
+  _fields_ = [
+      ('rgb', ctypes.c_void_p), ('rgb_env_stride', ctypes.c_uint64),
+      ('world_rgb', ctypes.c_void_p), ('world_rgb_env_stride', ctypes.c_uint64),
+      ('reward', ctypes.c_void_p), ('reward_env_stride', ctypes.c_uint64),
+      ('discount', ctypes.c_void_p), ('discount_env_stride', ctypes.c_uint64),
+      ('step_type', ctypes.c_void_p), ('step_type_env_stride', ctypes.c_uint64),
+      ('scalar_obs', ctypes.c_void_p), ('scalar_obs_env_stride', ctypes.c_uint64), ('scalar_obs_stride', ctypes.c_uint64),
+  ]
+
+
+# The outputs a step can deliver into caller-owned tensors (mp_step_into), each with the axis that indexes envs.
+DEVICE_OUTPUTS = ('rgb', 'world_rgb', 'reward', 'discount', 'step_type', 'scalar_obs')
+
+
+class TensorLayout(NamedTuple):
+  """What describe_outputs needs of a tensor: shape and strides in elements, dtype, device and address."""
+  shape: Tuple[int, ...]
+  stride: Tuple[int, ...]
+  dtype: Any
+  device: Any
+  data_ptr: int
+
+
+def layout_of(t) -> TensorLayout:
+  return TensorLayout(tuple(t.shape), tuple(t.stride()), t.dtype, t.device, int(t.data_ptr()))
+
+
+def describe_outputs(out: Mapping[str, TensorLayout], views: Mapping[str, Tuple[Tuple[int, ...], Any]], device: int) -> MpDeviceOutputs:
+  """The mp_device_outputs of `out` (name -> TensorLayout of a CUDA tensor). `views` maps each output name to the shape
+  and dtype of the engine's own view of it; each tensor must have that shape and dtype, live on cuda:`device`, and be
+  dense in every axis but the env axis (axis 0; axes 0 and 1 for scalar_obs, whose axis 1 indexes envs). Alignment,
+  allocation bounds and overlaps are checked by the C call."""
+  import torch  # pylint: disable=g-import-not-at-top
+  s = MpDeviceOutputs()
+  for name, t in out.items():
+    if t is None:
+      continue
+    if name not in DEVICE_OUTPUTS:
+      raise ValueError(f'out: unknown output {name!r} (one of {", ".join(DEVICE_OUTPUTS)})')
+    shape, dtype = views[name]
+    if tuple(t.shape) != tuple(shape):
+      raise ValueError(f'out[{name!r}]: shape {tuple(t.shape)}, the engine\'s is {tuple(shape)}')
+    if t.dtype != dtype:
+      raise ValueError(f'out[{name!r}]: dtype {t.dtype}, the engine\'s is {dtype}')
+    dev = torch.device(t.device)
+    if dev.type != 'cuda' or dev.index != device:
+      raise ValueError(f'out[{name!r}]: on {dev}, the engine runs on cuda:{device}')
+    env_axis = 1 if name == 'scalar_obs' else 0
+    dense = 1
+    for axis in range(len(shape) - 1, env_axis, -1):
+      if shape[axis] != 1 and t.stride[axis] != dense:
+        raise ValueError(f'out[{name!r}]: axis {axis} has stride {t.stride[axis]}, must be {dense} '
+                         f'(only the env axis{" and the observation axis" if env_axis else ""} may be strided)')
+      dense *= shape[axis]
+    item = torch.empty((), dtype=dtype).element_size()
+    # with one env (one observation) the stride is never used: pass the dense one
+    env_stride = (t.stride[env_axis] if shape[env_axis] > 1 else dense) * item
+    setattr(s, name, ctypes.c_void_p(int(t.data_ptr)))
+    setattr(s, f'{name}_env_stride', env_stride)
+    if name == 'scalar_obs':
+      s.scalar_obs_stride = (t.stride[0] if shape[0] > 1 else shape[1] * dense) * item
+  return s
+
+
 _lib = None
 
 
@@ -118,6 +184,8 @@ def load_library() -> ctypes.CDLL:
   lib.mp_set_flags.argtypes = [vp, ctypes.c_uint32]
   lib.mp_reset.argtypes = [vp, vp, vp]
   lib.mp_step.argtypes = [vp, vp, vp]
+  lib.mp_step_into.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), vp]
+  lib.mp_reset_into.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), vp]
   lib.mp_step_state.argtypes = [vp, vp, vp]
   lib.mp_render.argtypes = [vp, vp]
   lib.mp_get_buffers.argtypes = [vp, ctypes.POINTER(MpBuffers)]
@@ -321,17 +389,38 @@ class Engine:
   def set_flags(self, flags: int) -> None:
     _check(self._lib.mp_set_flags(self._h, ctypes.c_uint32(flags)))
 
-  def reset(self, mask=None, stream=None) -> None:
+  def reset(self, mask=None, stream=None, out=None) -> None:
+    """out: as for step."""
     ptr = None
     if mask is not None:
       assert mask.dtype == self._torch.uint8 and mask.is_cuda and mask.numel() == self.num_envs
       ptr = ctypes.c_void_p(mask.data_ptr())
-    _check(self._lib.mp_reset(self._h, ptr, self._stream(stream)))
+    if out is None:
+      _check(self._lib.mp_reset(self._h, ptr, self._stream(stream)))
+    else:
+      s = self._device_outputs(out)
+      _check(self._lib.mp_reset_into(self._h, ptr, ctypes.byref(s), self._stream(stream)))
 
-  def step(self, actions, stream=None) -> None:
-    """actions: int32 CUDA tensor [B, P] of discrete action ids."""
+  def step(self, actions, stream=None, out=None) -> None:
+    """actions: int32 CUDA tensor [B, P] of discrete action ids.
+
+    out: {name: CUDA tensor} for any of DEVICE_OUTPUTS (mp_step_into): the step's images are rendered straight into
+    out['rgb'] / out['world_rgb'] instead of this engine's own image buffers, and its scalars are written into the
+    others as well as into this engine's buffers. Shapes and dtypes are those of the engine's views (rgb, reward, ...);
+    the env axis may have any stride (and the observation axis of scalar_obs), every other axis is dense."""
     self._check_actions(actions)
-    _check(self._lib.mp_step(self._h, ctypes.c_void_p(actions.data_ptr()), self._stream(stream)))
+    if out is None:
+      _check(self._lib.mp_step(self._h, ctypes.c_void_p(actions.data_ptr()), self._stream(stream)))
+    else:
+      s = self._device_outputs(out)
+      _check(self._lib.mp_step_into(self._h, ctypes.c_void_p(actions.data_ptr()), ctypes.byref(s), self._stream(stream)))
+
+  def output_views(self):
+    """name -> (shape, dtype) of the engine's own view of each output a step can deliver into caller tensors."""
+    return {name: (tuple(getattr(self, name).shape), getattr(self, name).dtype) for name in DEVICE_OUTPUTS}
+
+  def _device_outputs(self, out) -> MpDeviceOutputs:
+    return describe_outputs({k: (None if v is None else layout_of(v)) for k, v in out.items()}, self.output_views(), self.device)
 
   def step_state(self, actions, stream=None) -> None:
     self._check_actions(actions)

@@ -162,7 +162,8 @@ class BatchedSubstrate:
   """`num_envs` independent instances of a substrate on one GPU.
 
   Observations are zero-copy views of the engine's output buffers and are overwritten by the
-  next `step`/`reset`; clone what must be kept.
+  next `step`/`reset`; clone what must be kept, or step into tensors of your own with
+  `step(actions, out=traj.at(t))` (see `trajectory`), which costs no copy.
   """
 
   def __init__(self, blob, num_envs: int, device: int = 0, seed: Optional[int] = None,
@@ -199,17 +200,63 @@ class BatchedSubstrate:
     obs[_COLLECTIVE_REWARD_OBS] = e.reward.sum(dim=1)
     return BatchedTimeStep(step_type=e.step_type, reward=e.reward, discount=e.discount, observation=obs)
 
-  def reset(self, mask=None) -> BatchedTimeStep:
-    self._engine.reset(mask)
-    return self._timestep()
+  def reset(self, mask=None, out: Optional[BatchedTimeStep] = None) -> BatchedTimeStep:
+    """out: as for step."""
+    if out is None:
+      self._engine.reset(mask)
+      return self._timestep()
+    self._engine.reset(mask, out=self._engine_outputs(out))
+    return self._fill_collective(out)
 
-  def step(self, actions) -> BatchedTimeStep:
-    """actions: integer tensor [B, P] on the engine's device (int32 preferred)."""
+  def step(self, actions, out: Optional[BatchedTimeStep] = None) -> BatchedTimeStep:
+    """actions: integer tensor [B, P] on the engine's device (int32 preferred).
+
+    out: a BatchedTimeStep of caller-owned tensors to fill and return instead of views of the engine's buffers, e.g.
+    `trajectory(T).at(t)`: the engine renders the images straight into it and delivers the scalars there too, so a
+    learner keeps T steps without copying them."""
     import torch  # pylint: disable=g-import-not-at-top
     if actions.dtype != torch.int32:
       actions = actions.to(torch.int32)
-    self._engine.step(actions.contiguous())
-    return self._timestep()
+    if out is None:
+      self._engine.step(actions.contiguous())
+      return self._timestep()
+    self._engine.step(actions.contiguous(), out=self._engine_outputs(out))
+    return self._fill_collective(out)
+
+  def trajectory(self, T: int, time_major: bool = True) -> 'Trajectory':
+    """Tensors for T timesteps of every output, COLLECTIVE_REWARD included, laid out [T, B, ...] (time_major) or
+    [B, T, ...]; `at(t)` is slot t as a BatchedTimeStep for step(..., out=) / reset(..., out=)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    e = self._engine
+    return Trajectory(int(T), self.num_envs, self.num_players, e.rgb.shape[1:], e.world_rgb.shape[1:] if self._world_rgb else None,
+                      self._scalar_names, bool(time_major), torch.device('cuda', e.device))
+
+  def _engine_outputs(self, ts: BatchedTimeStep):
+    """The engine's output tensors of a BatchedTimeStep (the scalar observations as one [n, B, P] view)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    obs = ts.observation
+    out = {'rgb': obs.get('RGB'), 'world_rgb': obs.get('WORLD.RGB') if self._world_rgb else None,
+           'reward': ts.reward, 'discount': ts.discount, 'step_type': ts.step_type}
+    scalars = [obs[name] for name in self._scalar_names if name in obs]
+    if scalars:
+      if len(scalars) != len(self._scalar_names):
+        raise ValueError(f'out: give all of {self._scalar_names} or none')
+      first = scalars[0]
+      step = (scalars[1].data_ptr() - first.data_ptr()) // first.element_size() if len(scalars) > 1 else first.numel()
+      for k, s in enumerate(scalars):  # views of one tensor, evenly spaced, as trajectory() makes them
+        if (s.shape != first.shape or s.stride() != first.stride() or s.dtype != first.dtype or s.device != first.device
+            or s.untyped_storage().data_ptr() != first.untyped_storage().data_ptr()
+            or s.data_ptr() != first.data_ptr() + k * step * first.element_size()):
+          raise ValueError('out: the scalar observations must be evenly spaced views of one tensor (see trajectory())')
+      out['scalar_obs'] = torch.as_strided(first, (len(scalars),) + tuple(first.shape), (step,) + tuple(first.stride()))
+    return out
+
+  def _fill_collective(self, ts: BatchedTimeStep) -> BatchedTimeStep:
+    import torch  # pylint: disable=g-import-not-at-top
+    collective = ts.observation.get(_COLLECTIVE_REWARD_OBS)
+    if collective is not None:
+      torch.sum(ts.reward, dim=1, out=collective)
+    return ts
 
   def set_env_variant(self, ids) -> None:
     """Moves env b to variant ids[b] from its next episode start on (reset(mask) to switch at once)."""
@@ -244,6 +291,45 @@ class BatchedSubstrate:
 
   def __exit__(self, *unused):
     self.close()
+
+
+class Trajectory:
+  """T timesteps of a BatchedSubstrate's outputs in caller-owned CUDA tensors (BatchedSubstrate.trajectory).
+
+  Fields mirror BatchedTimeStep with a time axis: step_type int64, reward float64 [.., P], discount float64 and
+  observation {name: tensor}, each [T, B, ...] when time_major else [B, T, ...]."""
+
+  def __init__(self, T: int, num_envs: int, num_players: int, rgb_shape, world_rgb_shape, scalar_names: Sequence[str],
+               time_major: bool, device):
+    """rgb_shape: one env's [P, h, w, 3]; world_rgb_shape: one env's [H, W, 3], or None without WORLD.RGB."""
+    import torch  # pylint: disable=g-import-not-at-top
+    if T < 1:
+      raise ValueError(f'a trajectory needs T >= 1 slots, got {T}')
+    self.T, self.time_major = T, time_major
+    B, P = num_envs, num_players
+
+    def new(shape, dtype):
+      return torch.zeros(((T, B) if time_major else (B, T)) + tuple(shape), dtype=dtype, device=device)
+
+    self.step_type = new((), torch.int64)
+    self.reward = new((P,), torch.float64)
+    self.discount = new((), torch.float64)
+    self.observation = {'RGB': new(tuple(rgb_shape), torch.uint8)}
+    if scalar_names:  # one tensor, so that slot t of every scalar observation is one [n, B, P] view for the engine
+      scalars = torch.zeros((len(scalar_names),) + tuple(self.reward.shape), dtype=torch.float64, device=device)
+      for k, name in enumerate(scalar_names):
+        self.observation[name] = scalars[k]
+    if world_rgb_shape is not None:
+      self.observation['WORLD.RGB'] = new(tuple(world_rgb_shape), torch.uint8)
+    self.observation[_COLLECTIVE_REWARD_OBS] = new((), torch.float64)
+
+  def at(self, t: int) -> BatchedTimeStep:
+    """Slot t as a BatchedTimeStep of views ([B, ...] each)."""
+    if not -self.T <= t < self.T:
+      raise IndexError(f'slot {t} of a trajectory of {self.T}')
+    pick = (lambda x: x[t]) if self.time_major else (lambda x: x[:, t])
+    return BatchedTimeStep(step_type=pick(self.step_type), reward=pick(self.reward), discount=pick(self.discount),
+                           observation={k: pick(v) for k, v in self.observation.items()})
 
 
 # ---------------------------------------------------------------------------------------------
