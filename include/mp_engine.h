@@ -283,7 +283,8 @@ int mp_algorithmic_bytes(mp_handle h, uint64_t* per_env_step, uint64_t* render_p
 
 /* Snapshot / restore of every env instance (SURVEY.md section 8f, row N4). The reference has no counterpart
  * (a dmlab2d env cannot be cloned); here the state is a handful of SoA arrays and the random numbers are
- * addressed by (seed, env, frame), so a byte copy is a complete checkpoint. A snapshot is an opaque string of
+ * addressed by (key, frame), where each env's Philox key is per-env state (seed + env_index_base + b at creation),
+ * so a byte copy is a complete checkpoint. A snapshot is an opaque string of
  * mp_state_size() bytes in host memory, valid for an engine created from the same blob with the same num_envs,
  * seed and env_index_base: the header records the env count, payload size, RNG key and a hash of the blob, and
  * mp_state_load rejects (MP_E_INVALID) a buffer whose `nbytes` or header does not match this engine.
@@ -291,6 +292,32 @@ int mp_algorithmic_bytes(mp_handle h, uint64_t* per_env_step, uint64_t* render_p
 int mp_state_size(mp_handle h, uint64_t* bytes);
 int mp_state_save(mp_handle h, void* host_dst, void* stream);
 int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stream);
+
+/* Per-env state bank on the device: single envs are stored into rows of a caller-owned bank and restored from them,
+ * without a round trip through host memory. A record holds one env's state rows, its timestep and its RNG key, so an
+ * env restored from another env's record is that env's twin (a clone: store, then restore into other envs). Every size
+ * in a record follows from the blob, so a record restores into any engine built from the same blob (or the same ordered
+ * variant set), whatever its num_envs, seed, env_index_base or device. Images are not stored; a restore re-renders.
+ *
+ * mp_state_record_bytes: bytes of one record (a multiple of 16) and the 16-byte tag every record of this engine starts
+ * with (either pointer may be NULL). */
+int mp_state_record_bytes(mp_handle h, uint64_t* bytes, uint8_t tag[16]);
+
+/* Bank row k (k < n_slots) receives env env_of_slot[k] when 0 <= env_of_slot[k] < B; otherwise row k is left untouched.
+ * env_of_slot: DEVICE i32 [n_slots]. bank: DEVICE, n_slots * record_bytes, 16-byte aligned, inside one allocation on the
+ * engine's device and outside the engine's own buffers. Asynchronous on `stream`; one kernel. */
+int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* bank, void* stream);
+
+/* Env b receives bank row slot_of_env[b] when 0 <= slot_of_env[b] < n_slots and that row's tag is this engine's;
+ * otherwise env b is left untouched. Then the batch is re-rendered (as mp_state_load does). A restored env's timestep
+ * (reward, discount, step type, scalar observations, events), images and variant are those of the stored env at store
+ * time: if that step was LAST, its next step starts a new episode. The key is state, so resets keep it.
+ * flags: MP_RESTORE_REKEY = restored envs take their own key (seed + env_index_base + b) instead of the record's.
+ * slot_of_env: DEVICE i32 [B]. Asynchronous on `stream`; one kernel plus what mp_render launches. Refused
+ * (MP_E_UNSUPPORTED) once mp_exchange_connect or mp_gather_obs_connect has run: the peers' stacked rows would go stale.
+ * Both calls check their arguments before anything is enqueued; a refused call touches nothing. */
+#define MP_RESTORE_REKEY 1u
+int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, void* stream);
 
 /* Diagnostic: how the renderer was laid out for this substrate: teams per CTA, threads per team, log2 of the pixel
  * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes,

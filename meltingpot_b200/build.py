@@ -8,7 +8,7 @@ import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ['engine.cu']
-HEADERS = ['common.cuh', 'family_load.h', 'render.cuh', 'step_common.cuh', 'step_clean_up.cuh', 'step_commons.cuh', 'step_territory.cuh', 'step_coins.cuh', 'step_mining.cuh']
+HEADERS = ['common.cuh', 'family_load.h', 'render.cuh', 'step_common.cuh', 'step_clean_up.cuh', 'step_commons.cuh', 'step_territory.cuh', 'step_coins.cuh', 'step_mining.cuh', 'state_bank.cuh']
 LIB_PATH = os.path.join(_HERE, 'libmpengine.so')
 
 NVCC_FLAGS = [

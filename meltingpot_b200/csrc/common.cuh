@@ -12,6 +12,7 @@
 //   apple/dirt/water/apple_count u8 [B][n_pad]  per-entity state (family specific)
 //   env         i32 [B][8]              step, episode, done, dirt count, cleaned flags, ate flags,
 //                                       beam-dirty, spare
+//   key         u64 [B]                 Philox key of each env (seed + env_index_base + b at creation)
 // cells_pad keeps every layer row 16-byte aligned so rows can be moved with 128-bit accesses.
 #pragma once
 
@@ -89,7 +90,7 @@ struct ScalarTargets {
 
 struct State {
   int B;
-  uint64_t seed;  // key of env b = seed + b (env_index_base already folded in)
+  uint64_t* key;  // [B] Philox key of each env: seed + env_index_base + b at mp_create; state, so a restored env keeps its source's
   uint16_t* grid;
   int32_t* avatar;
   int32_t* av_timer;

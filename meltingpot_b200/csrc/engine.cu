@@ -20,6 +20,7 @@
 #include "step_territory.cuh"
 #include "step_coins.cuh"
 #include "step_mining.cuh"
+#include "state_bank.cuh"
 
 namespace {
 
@@ -246,6 +247,7 @@ struct mp_engine {
   uint64_t state_bytes = 0;
   int lane_map_players = 0, lane_map_world = 0;  // 0 plain, 2 scattered colouring, 1 + 16 * (extra wavefronts left) whole-cell dealing
   int inst_ncp = 0, inst_ncw = 0;                // the k_render<NCP, NCW> instantiation this engine launches
+  uint64_t key_base = 0;   // seed + env_index_base: env b's key at creation is key_base + b (State::key)
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
 
@@ -801,7 +803,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   if (rc != MP_OK) { mp_destroy(E); return rc; }
   const Tables& T = E->T;
   State& S = E->S;
-  S.B = num_envs; S.seed = seed + env_index_base;
+  S.B = num_envs; E->key_base = seed + env_index_base;
   const size_t B = num_envs, P = T.P;
   {  // Worst case of events one step can emit per env: per avatar, every cell of every beam footprint can carry a hit
      // with up to three events (zap + sanctioning + removal), plus the contact / regrowth events (<= 4) and the pair
@@ -811,7 +813,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   S.fam_u8_stride = std::max(16, RU_COUNT * T.nR_pad); S.fam_u16_stride = std::max(16, RS_COUNT * T.nR_pad);
   if ((rc = E->alloc(B * T.L * T.cells_pad, &S.grid)) || (rc = E->alloc(B * P * 4, &S.avatar)) || (rc = E->alloc(B * P * 4, &S.av_timer)) ||
       (rc = E->alloc(B * T.nA_pad, &S.apple)) || (rc = E->alloc(B * T.nD_pad, &S.dirt)) || (rc = E->alloc(B * T.nW_pad, &S.water)) || (rc = E->alloc(B * T.nA_pad, &S.apple_count)) || (rc = E->alloc(B * (size_t)S.fam_u8_stride, &S.fam_u8)) || (rc = E->alloc(B * (size_t)S.fam_u16_stride, &S.fam_u16)) || (rc = E->alloc(B * P * 8, &S.av_extra)) || (rc = E->alloc(B * (P + 2), &S.packed)) ||
-      (rc = E->alloc(B * ENV_COLS, &S.env)) ||
+      (rc = E->alloc(B * ENV_COLS, &S.env)) || (rc = E->alloc(B, &S.key)) ||
       (rc = E->alloc((B * P + B + B + std::max<size_t>(1, T.n_scalar) * B * P) * 8, &E->scalar_block)) ||
       (rc = E->alloc(B * P * E->R.player_bytes, &S.rgb)) || (rc = E->alloc(B * (size_t)E->R.world_bytes, &S.world_rgb)) ||
       (rc = E->alloc(B * (size_t)S.max_events * 3, &S.events)) || (rc = E->alloc(B, &S.n_events)) ||
@@ -839,13 +841,17 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     span(S.reward, B * P * sizeof(*S.reward)); span(S.discount, B * sizeof(*S.discount));
     span(S.step_type, B * sizeof(*S.step_type)); span(S.scalar_obs, ns * B * P * sizeof(*S.scalar_obs));
     span(S.events, B * (size_t)S.max_events * 3 * sizeof(*S.events)); span(S.n_events, B * sizeof(*S.n_events));
+    span(S.key, B * sizeof(*S.key));  // (record_layout below is one env's row of each of these)
   }
   // episode counter starts at -1 so that the first reset plays episode 0; envs start "done".
   {
     std::vector<int32_t> env0(B * ENV_COLS, 0);
     for (size_t b = 0; b < B; ++b) { env0[b * ENV_COLS + ENV_EPISODE] = -1; env0[b * ENV_COLS + ENV_DONE] = 1; }
+    std::vector<uint64_t> key0(B);
+    for (size_t b = 0; b < B; ++b) key0[b] = E->key_base + b;
     cudaError_t ce = cudaMemcpy(S.env, env0.data(), env0.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
-    if (ce != cudaSuccess) { mp_destroy(E); return fail(MP_E_CUDA, "cudaMemcpy(env) failed: %s", cudaGetErrorString(ce)); }
+    if (ce == cudaSuccess) ce = cudaMemcpy(S.key, key0.data(), key0.size() * sizeof(uint64_t), cudaMemcpyHostToDevice);
+    if (ce != cudaSuccess) { mp_destroy(E); return fail(MP_E_CUDA, "cudaMemcpy(env / key) failed: %s", cudaGetErrorString(ce)); }
   }
   E->step_smem = E->family->step_smem(T);
   {  // cells per lane per strip: ceil(view_w / 4) for player rows, ceil(W / 8) for world half-rows
@@ -901,6 +907,47 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
 }
 
 namespace {
+// The record of one env in a state bank (mp_state_store / mp_state_restore): env b's row of each state span of mp_create
+// (images excepted: a restore re-renders them). Every offset and length follows from the blob (or the variant set)
+// alone, so a record restores into any engine built from it, whatever its num_envs, seed, env_index_base or device.
+//   [0, 16)   tag: format word, record bytes, blob_hash (the hash of the ordered variant set for a variant engine)
+//   [16, 24)  key u64; [24] active, [25] pending variant (0 in a single-blob engine)
+//   [32, ..)  grid, avatar, av_timer, apple, dirt, water, apple_count, fam_u8, fam_u16, av_extra, packed, env, reward,
+//             discount, step_type, the n_scalar rows of scalar_obs [n][B][P], events [max_events][3], n_events; each
+//             row at a 16-byte offset
+constexpr uint32_t kRecordFormat = 0x3152504du;  // "MPR1"
+RecordLayout record_layout(const mp_engine* E) {
+  const Tables& T = E->T;
+  const State& S = E->S;
+  const uint64_t B = E->B, P = T.P;
+  RecordLayout R{};
+  R.key_row = 0;
+  uint32_t off = 16;
+  auto row = [&](const void* base, uint64_t env_stride, uint64_t bytes, uint32_t align) {
+    off = (off + align - 1) / align * align;
+    R.row[R.n_rows++] = {static_cast<uint8_t*>(const_cast<void*>(base)), env_stride, (uint32_t)bytes, off};
+    off += (uint32_t)bytes;
+  };
+  row(S.key, 8, 8, 8);
+  row(E->variants.n > 1 ? E->variants.active : nullptr, 1, 1, 1);
+  row(E->variants.n > 1 ? E->variants.pending : nullptr, 1, 1, 1);
+  const uint64_t grid = (uint64_t)T.L * T.cells_pad * sizeof(*S.grid);
+  row(S.grid, grid, grid, 16);
+  row(S.avatar, P * 16, P * 16, 16); row(S.av_timer, P * 16, P * 16, 16);
+  row(S.apple, T.nA_pad, T.nA_pad, 16); row(S.dirt, T.nD_pad, T.nD_pad, 16); row(S.water, T.nW_pad, T.nW_pad, 16);
+  row(S.apple_count, T.nA_pad, T.nA_pad, 16);
+  row(S.fam_u8, S.fam_u8_stride, S.fam_u8_stride, 16); row(S.fam_u16, S.fam_u16_stride * 2, S.fam_u16_stride * 2, 16);
+  row(S.av_extra, P * 32, P * 32, 16); row(S.packed, (P + 2) * 8, (P + 2) * 8, 16); row(S.env, ENV_COLS * 4, ENV_COLS * 4, 16);
+  row(S.reward, P * 8, P * 8, 16); row(S.discount, 8, 8, 16); row(S.step_type, 8, 8, 16);
+  for (int k = 0; k < T.n_scalar; ++k) row(S.scalar_obs + (size_t)k * B * P, P * 8, P * 8, 16);
+  row(S.events, (uint64_t)S.max_events * 12, (uint64_t)S.max_events * 12, 16); row(S.n_events, 4, 4, 16);
+  R.record_bytes = (off + 15) / 16 * 16;
+  const uint64_t h = E->blob_hash;
+  R.tag = make_uint4(kRecordFormat, (uint32_t)R.record_bytes, (uint32_t)h, (uint32_t)(h >> 32));
+  return R;
+}
+static_assert(17 + 4 + 3 <= MP_RECORD_MAX_ROWS, "record rows: 17 state spans, up to 4 scalar_obs rows, key and variants");
+
 // Rule (a) of mp_create_variants: variant `v` has the same sections as variant 0, byte for byte, except the family's
 // parameter blocks, the component tables and the metadata string.
 int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
@@ -1075,50 +1122,14 @@ int mp_step(mp_handle h, const int32_t* actions, void* stream) {
 }  // extern "C"
 
 namespace {
-// Every check of mp_step_into / mp_reset_into (include/mp_engine.h), before anything is enqueued: a pointer that fails
-// one never reaches a kernel. Extents are computed in 128 bits, so no stride can wrap them around.
-int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn) {
-  if (!o) return fail(MP_E_INVALID, "%s: null outputs (use mp_step / mp_reset)", fn);
-  typedef unsigned __int128 u128;
-  const uint64_t B = E->B, P = E->T.P, n = E->T.n_scalar;
-  struct Out { const char* name; uintptr_t p; u128 extent; };
-  std::vector<Out> outs;
-  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_env, uint64_t align, u128 extra) -> int {
-    if (!p) return MP_OK;
-    if ((uintptr_t)p % align || stride % align)
-      return fail(MP_E_INVALID, "%s: %s pointer or env stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
-    if (stride < per_env)
-      return fail(MP_E_INVALID, "%s: %s env stride of %llu bytes is smaller than one env's %llu bytes", fn, name,
-                  (unsigned long long)stride, (unsigned long long)per_env);
-    if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s env stride of 2 GiB or more", fn, name);
-    outs.push_back({name, (uintptr_t)p, (u128)(B - 1) * stride + per_env + extra});
-    return MP_OK;
-  };
-  if (o->rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
-  if (o->world_rgb && !(E->flags & MP_FLAG_RENDER_WORLD)) return fail(MP_E_INVALID, "%s: world_rgb asked for, but the render flags switch WORLD.RGB off", fn);
-  if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
-  if (o->scalar_obs && o->scalar_obs_stride % 8) return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes", fn);
-  int rc;
-  if ((rc = add("rgb", o->rgb, o->rgb_env_stride, P * E->R.player_bytes, 16, 0)) ||
-      (rc = add("world_rgb", o->world_rgb, o->world_rgb_env_stride, (uint64_t)E->R.world_bytes, 16, 0)) ||
-      (rc = add("reward", o->reward, o->reward_env_stride, P * 8, 8, 0)) ||
-      (rc = add("discount", o->discount, o->discount_env_stride, 8, 8, 0)) ||
-      (rc = add("step_type", o->step_type, o->step_type_env_stride, 8, 8, 0)) ||
-      (rc = add("scalar_obs", o->scalar_obs, o->scalar_obs_env_stride, P * 8, 8, (u128)(n - 1) * o->scalar_obs_stride)))
-    return rc;
-  for (const Out& x : outs)
-    if (x.extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, x.name);
-  if (o->scalar_obs) {
-    // The n x B rows of P doubles start at k * s + b * e. Rows of one k are e >= P * 8 apart; rows j = k' - k apart
-    // are |j * s + m * e| apart, m = b' - b in [-(B - 1), B - 1], closest at m = -floor(j * s / e) or one below.
-    const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_env_stride;
-    for (uint64_t j = 1; j < n; ++j) {
-      const u128 d = (u128)j * s, q = d / e, r = d % e;
-      const u128 gap = q > B - 1 ? d - (u128)(B - 1) * e : (q + 1 <= B - 1 ? std::min<u128>(r, e - r) : r);
-      if (gap < P * 8) return fail(MP_E_INVALID, "%s: scalar_obs rows overlap (env stride %llu, stride %llu bytes)", fn,
-                                   (unsigned long long)e, (unsigned long long)s);
-    }
-  }
+typedef unsigned __int128 u128;
+// A caller-owned device range an entry point reads or writes: `extent` bytes from `p`.
+struct DeviceExtent { const char* name; uintptr_t p; u128 extent; };
+
+// Each extent lies inside one device allocation on the engine's device and overlaps neither another extent nor the
+// engine's own buffers (mp_step_into's targets, mp_state_store / mp_state_restore's bank and index arrays).
+int check_extents(mp_engine* E, const std::vector<DeviceExtent>& outs, const char* fn) {
+  const uint64_t B = E->B, P = E->T.P;
   // each extent inside one device allocation on the engine's device (cuMemGetAddressRange through the runtime's driver
   // entry point, as mp_ipc_export does, so the library does not link libcuda)
   typedef int (*GetRange)(unsigned long long*, size_t*, unsigned long long);
@@ -1126,7 +1137,7 @@ int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* f
   cudaDriverEntryPointQueryResult qr;
   CUDA_TRY(cudaGetDriverEntryPoint("cuMemGetAddressRange", &range_fn, cudaEnableDefault, &qr));
   if (!range_fn || qr != cudaDriverEntryPointSuccess) return fail(MP_E_CUDA, "cuMemGetAddressRange is not available");
-  for (const Out& x : outs) {
+  for (const DeviceExtent& x : outs) {
     cudaPointerAttributes a{};
     if (cudaPointerGetAttributes(&a, (const void*)x.p) != cudaSuccess) {
       cudaGetLastError();
@@ -1160,6 +1171,51 @@ int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* f
       if (lo < (u128)sp.first + sp.second && (u128)sp.first < hi) return fail(MP_E_INVALID, "%s: %s overlaps the engine's own buffers", fn, outs[i].name);
   }
   return MP_OK;
+}
+
+// Every check of mp_step_into / mp_reset_into (include/mp_engine.h), before anything is enqueued: a pointer that fails
+// one never reaches a kernel. Extents are computed in 128 bits, so no stride can wrap them around.
+int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn) {
+  if (!o) return fail(MP_E_INVALID, "%s: null outputs (use mp_step / mp_reset)", fn);
+  const uint64_t B = E->B, P = E->T.P, n = E->T.n_scalar;
+  std::vector<DeviceExtent> outs;
+  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_env, uint64_t align, u128 extra) -> int {
+    if (!p) return MP_OK;
+    if ((uintptr_t)p % align || stride % align)
+      return fail(MP_E_INVALID, "%s: %s pointer or env stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
+    if (stride < per_env)
+      return fail(MP_E_INVALID, "%s: %s env stride of %llu bytes is smaller than one env's %llu bytes", fn, name,
+                  (unsigned long long)stride, (unsigned long long)per_env);
+    if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s env stride of 2 GiB or more", fn, name);
+    outs.push_back({name, (uintptr_t)p, (u128)(B - 1) * stride + per_env + extra});
+    return MP_OK;
+  };
+  if (o->rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
+  if (o->world_rgb && !(E->flags & MP_FLAG_RENDER_WORLD)) return fail(MP_E_INVALID, "%s: world_rgb asked for, but the render flags switch WORLD.RGB off", fn);
+  if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
+  if (o->scalar_obs && o->scalar_obs_stride % 8) return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes", fn);
+  int rc;
+  if ((rc = add("rgb", o->rgb, o->rgb_env_stride, P * E->R.player_bytes, 16, 0)) ||
+      (rc = add("world_rgb", o->world_rgb, o->world_rgb_env_stride, (uint64_t)E->R.world_bytes, 16, 0)) ||
+      (rc = add("reward", o->reward, o->reward_env_stride, P * 8, 8, 0)) ||
+      (rc = add("discount", o->discount, o->discount_env_stride, 8, 8, 0)) ||
+      (rc = add("step_type", o->step_type, o->step_type_env_stride, 8, 8, 0)) ||
+      (rc = add("scalar_obs", o->scalar_obs, o->scalar_obs_env_stride, P * 8, 8, (u128)(n - 1) * o->scalar_obs_stride)))
+    return rc;
+  for (const DeviceExtent& x : outs)
+    if (x.extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, x.name);
+  if (o->scalar_obs) {
+    // The n x B rows of P doubles start at k * s + b * e. Rows of one k are e >= P * 8 apart; rows j = k' - k apart
+    // are |j * s + m * e| apart, m = b' - b in [-(B - 1), B - 1], closest at m = -floor(j * s / e) or one below.
+    const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_env_stride;
+    for (uint64_t j = 1; j < n; ++j) {
+      const u128 d = (u128)j * s, q = d / e, r = d % e;
+      const u128 gap = q > B - 1 ? d - (u128)(B - 1) * e : (q + 1 <= B - 1 ? std::min<u128>(r, e - r) : r);
+      if (gap < P * 8) return fail(MP_E_INVALID, "%s: scalar_obs rows overlap (env stride %llu, stride %llu bytes)", fn,
+                                   (unsigned long long)e, (unsigned long long)s);
+    }
+  }
+  return check_extents(E, outs, fn);
 }
 }  // namespace
 
@@ -1450,7 +1506,7 @@ int mp_state_save(mp_handle h, void* host_dst, void* stream) {
   if (!h || !host_dst) return fail(MP_E_INVALID, "mp_state_save: null argument");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
-  SnapshotHeader hd{{'M', 'P', 'S', '3'}, 3u, (uint64_t)h->B, h->state_bytes, (uint64_t)h->state_spans.size(), h->S.seed, h->blob_hash};
+  SnapshotHeader hd{{'M', 'P', 'S', '4'}, 4u, (uint64_t)h->B, h->state_bytes, (uint64_t)h->state_spans.size(), h->key_base, h->blob_hash};
   memcpy(host_dst, &hd, sizeof(hd));
   uint8_t* dst = static_cast<uint8_t*>(host_dst) + sizeof(hd);
   for (const auto& sp : h->state_spans) {
@@ -1466,7 +1522,7 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
   if (nbytes < sizeof(SnapshotHeader)) return fail(MP_E_INVALID, "mp_state_load: %llu bytes is shorter than a snapshot header", (unsigned long long)nbytes);
   SnapshotHeader hd;
   memcpy(&hd, host_src, sizeof(hd));
-  if (memcmp(hd.magic, "MPS3", 4) != 0 || hd.version != 3u) return fail(MP_E_INVALID, "mp_state_load: not a snapshot (or one of an older engine)");
+  if (memcmp(hd.magic, "MPS4", 4) != 0 || hd.version != 4u) return fail(MP_E_INVALID, "mp_state_load: not a snapshot (or one of an older engine)");
   if (hd.num_envs != (uint64_t)h->B || hd.payload_bytes != h->state_bytes || hd.n_spans != h->state_spans.size())
     return fail(MP_E_INVALID, "mp_state_load: snapshot of %llu envs / %llu bytes does not fit this engine (%d envs / %llu bytes)",
                 (unsigned long long)hd.num_envs, (unsigned long long)hd.payload_bytes, h->B, (unsigned long long)h->state_bytes);
@@ -1474,8 +1530,8 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
     return fail(MP_E_INVALID, "mp_state_load: buffer of %llu bytes, snapshot needs %llu (truncated?)", (unsigned long long)nbytes,
                 (unsigned long long)(sizeof(SnapshotHeader) + hd.payload_bytes));
   if (hd.blob_hash != h->blob_hash) return fail(MP_E_INVALID, "mp_state_load: snapshot was taken from a different compiled substrate");
-  if (hd.rng_key0 != h->S.seed) return fail(MP_E_INVALID, "mp_state_load: snapshot was taken with a different seed / env_index_base (key %llu, engine %llu)",
-                                            (unsigned long long)hd.rng_key0, (unsigned long long)h->S.seed);
+  if (hd.rng_key0 != h->key_base) return fail(MP_E_INVALID, "mp_state_load: snapshot was taken with a different seed / env_index_base (key %llu, engine %llu)",
+                                              (unsigned long long)hd.rng_key0, (unsigned long long)h->key_base);
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   const uint8_t* src = static_cast<const uint8_t*>(host_src) + sizeof(hd);
@@ -1487,6 +1543,58 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
   if (rc) return rc;
   CUDA_TRY(cudaStreamSynchronize(st));
   return MP_OK;
+}
+
+// ---- per-env state bank (record layout: record_layout) ------------------------------------------------------------
+int mp_state_record_bytes(mp_handle h, uint64_t* bytes, uint8_t tag[16]) {
+  if (!h) return fail(MP_E_INVALID, "null handle");
+  const RecordLayout R = record_layout(h);
+  if (bytes) *bytes = R.record_bytes;
+  if (tag) memcpy(tag, &R.tag, 16);
+  return MP_OK;
+}
+
+namespace {
+// The host checks of mp_state_store / mp_state_restore: the bank and the index array lie in device allocations on the
+// engine's device, overlap neither each other nor the engine's buffers, and the bank is 16-byte aligned.
+int check_bank(mp_engine* E, const void* bank, int n_slots, const int32_t* index, uint64_t index_count, uint64_t record_bytes, const char* fn) {
+  if ((uintptr_t)bank % 16) return fail(MP_E_INVALID, "%s: bank is not 16-byte aligned", fn);
+  if ((uintptr_t)index % 4) return fail(MP_E_INVALID, "%s: index array is not 4-byte aligned", fn);
+  const std::vector<DeviceExtent> ext{{"bank", (uintptr_t)bank, (u128)n_slots * record_bytes},
+                                      {"index array", (uintptr_t)index, (u128)index_count * 4}};
+  return check_extents(E, ext, fn);
+}
+}  // namespace
+
+int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* bank, void* stream) {
+  if (!h || !env_of_slot || !bank) return fail(MP_E_INVALID, "mp_state_store: null argument");
+  if (n_slots < 1) return fail(MP_E_INVALID, "mp_state_store: n_slots %d < 1", n_slots);
+  DeviceGuard guard(h->device);
+  const RecordLayout R = record_layout(h);
+  int rc = check_bank(h, bank, n_slots, env_of_slot, (uint64_t)n_slots, R.record_bytes, "mp_state_store");
+  if (rc) return rc;
+  k_state_store<<<(n_slots + 7) / 8, 256, 0, (cudaStream_t)stream>>>(R, env_of_slot, n_slots, h->B, static_cast<uint8_t*>(bank));
+  ++h->launches;
+  CUDA_TRY(cudaGetLastError());
+  return MP_OK;
+}
+
+int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, void* stream) {
+  if (!h || !slot_of_env || !bank) return fail(MP_E_INVALID, "mp_state_restore: null argument");
+  if (n_slots < 1) return fail(MP_E_INVALID, "mp_state_restore: n_slots %d < 1", n_slots);
+  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_state_restore: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
+  if (h->S.x_world || h->d_g_flag_ptrs)
+    return fail(MP_E_UNSUPPORTED, "mp_state_restore: not available once mp_exchange_connect / mp_gather_obs_connect has run");
+  DeviceGuard guard(h->device);
+  const RecordLayout R = record_layout(h);
+  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, R.record_bytes, "mp_state_restore");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  k_state_restore<<<(h->B + 7) / 8, 256, 0, st>>>(R, slot_of_env, static_cast<const uint8_t*>(bank), n_slots, h->B,
+                                                  (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base);
+  ++h->launches;
+  CUDA_TRY(cudaGetLastError());
+  return launch_render(h, st);
 }
 
 int mp_launch_count(mp_handle h, uint64_t* out) {

@@ -118,20 +118,28 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
   }
 }
 
-// What an advance of env b starts from: its env row, its sprite grid, its Philox key (seed + b), and the frame number
+// What an advance of env b starts from: its env row, its sprite grid, its Philox key (State::key), and the frame number
 // and episode it runs (frame 0 of the next episode on a reset).
+//
+// The key is per-env state (State::key) that no state-transition kernel writes, so each of its two words is read where
+// it is used instead of once here: a value loaded up front would stay live in two registers across the whole advance,
+// and the step kernels run at their 64-register cap (k_step<CleanUp> spilled 72 bytes more that way). The volatile read
+// keeps the compiler from merging the reads back into one.
+struct KeyWord {
+  const uint32_t* p;
+  __device__ __forceinline__ operator uint32_t() const { uint32_t v; asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(v) : "l"(p)); return v; }
+};
 struct Frame {
   int32_t* env;
   uint16_t* grid;
-  uint32_t k0, k1;
+  KeyWord k0, k1;
   int n, episode;
 };
 __device__ __forceinline__ Frame begin_frame(const Tables& T, const State& S, int b, bool reset) {
   Frame f;
   f.env = S.env + (size_t)b * ENV_COLS;
   f.grid = S.grid + (size_t)b * T.L * T.cells_pad;
-  const uint64_t key = S.seed + (uint64_t)b;
-  f.k0 = (uint32_t)key; f.k1 = (uint32_t)(key >> 32);
+  f.k0.p = reinterpret_cast<const uint32_t*>(S.key + b); f.k1.p = f.k0.p + 1;
   f.n = reset ? 0 : f.env[ENV_STEP] + 1;
   f.episode = f.env[ENV_EPISODE] + (reset ? 1 : 0);
   return f;

@@ -60,8 +60,10 @@ EXPORTED_SYMBOLS = (
     'mp_exchange_connect', 'mp_exchange_wait', 'mp_exchange_slot', 'mp_debug_lane_map', 'mp_debug_observations',
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
     'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
-    'mp_version',
+    'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore',
 )
+
+MP_RESTORE_REKEY = 1
 
 
 class MpBuffers(ctypes.Structure):
@@ -197,6 +199,9 @@ def load_library() -> ctypes.CDLL:
   lib.mp_state_size.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64)]
   lib.mp_state_save.argtypes = [vp, vp, vp]
   lib.mp_state_load.argtypes = [vp, vp, ctypes.c_uint64, vp]
+  lib.mp_state_record_bytes.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), vp]
+  lib.mp_state_store.argtypes = [vp, vp, ctypes.c_int, vp, vp]
+  lib.mp_state_restore.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_uint32, vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
   lib.mp_step_host_async.argtypes = [vp, vp, ctypes.POINTER(MpHostOutputs), ctypes.c_int, vp]
@@ -603,6 +608,53 @@ class Engine:
     snapshot = bytes(snapshot)
     buf = ctypes.create_string_buffer(snapshot, len(snapshot))
     _check(self._lib.mp_state_load(self._h, buf, ctypes.c_uint64(len(snapshot)), self._stream(stream)))
+
+  # -- per-env state bank (mp_state_store / mp_state_restore) ------------------------------
+  @property
+  def state_record_bytes(self) -> int:
+    """Bytes of one env's record in a state bank (a multiple of 16)."""
+    n = ctypes.c_uint64(0)
+    _check(self._lib.mp_state_record_bytes(self._h, ctypes.byref(n), None))
+    return int(n.value)
+
+  @property
+  def state_tag(self) -> bytes:
+    """The 16 bytes every record this engine stores starts with; a restore skips rows that do not start with them."""
+    tag = ctypes.create_string_buffer(16)
+    _check(self._lib.mp_state_record_bytes(self._h, None, tag))
+    return tag.raw
+
+  def _bank(self, bank):
+    torch = self._torch
+    if (not isinstance(bank, torch.Tensor) or bank.dtype != torch.uint8 or not bank.is_cuda or bank.dim() != 2
+        or bank.shape[1] != self.state_record_bytes or bank.shape[0] < 1 or not bank.is_contiguous()):
+      raise ValueError(f'bank must be a contiguous CUDA uint8 tensor [n_slots, {self.state_record_bytes}]')
+    return bank
+
+  def _indices(self, idx, n: int, what: str):
+    torch = self._torch
+    if (not isinstance(idx, torch.Tensor) or idx.dtype != torch.int32 or not idx.is_cuda or idx.shape != (n,)
+        or not idx.is_contiguous()):
+      raise ValueError(f'{what} must be a contiguous CUDA int32 tensor [{n}]')
+    return idx
+
+  def store_states(self, bank, env_of_slot, stream=None) -> None:
+    """Bank row k receives env env_of_slot[k] (mp_state_store); rows whose index is outside 0..B-1 are left as they
+    are. bank: CUDA uint8 [n_slots, state_record_bytes]; env_of_slot: CUDA int32 [n_slots]. Asynchronous."""
+    bank = self._bank(bank)
+    idx = self._indices(env_of_slot, bank.shape[0], 'env_of_slot')
+    _check(self._lib.mp_state_store(self._h, ctypes.c_void_p(idx.data_ptr()), int(bank.shape[0]),
+                                    ctypes.c_void_p(bank.data_ptr()), self._stream(stream)))
+
+  def restore_states(self, bank, slot_of_env, rekey: bool = False, stream=None) -> None:
+    """Env b receives bank row slot_of_env[b] (mp_state_restore) when that index is in range and the row carries this
+    engine's tag; other envs are left as they are. The batch is then re-rendered. rekey: restored envs draw their random
+    numbers under their own key instead of the stored env's. slot_of_env: CUDA int32 [B]. Asynchronous."""
+    bank = self._bank(bank)
+    idx = self._indices(slot_of_env, self.num_envs, 'slot_of_env')
+    _check(self._lib.mp_state_restore(self._h, ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(bank.data_ptr()),
+                                      int(bank.shape[0]), ctypes.c_uint32(MP_RESTORE_REKEY if rekey else 0),
+                                      self._stream(stream)))
 
   def render_plan(self):
     """Layout the renderer chose for this substrate, the lane maps it built and its k_render<ncp, ncw> (diagnostic)."""

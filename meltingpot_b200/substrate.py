@@ -158,12 +158,53 @@ class BatchedTimeStep:
   observation: Dict[str, Any]
 
 
+def bank_index(dest, src, n_dest: int, n_src: int, dest_name: str, src_name: str, device=None):
+  """The index array of a state-bank call: int32 [n_dest] holding src[i] at dest[i] and -1 everywhere else, built on
+  `device`. dest / src are matching sequences or integer tensors; raises ValueError on a length mismatch, an index
+  outside 0..n_dest-1 / 0..n_src-1 or a destination named twice."""
+  import torch  # pylint: disable=g-import-not-at-top
+  d = torch.as_tensor(dest, dtype=torch.int64, device=device).reshape(-1)
+  s = torch.as_tensor(src, dtype=torch.int64, device=device).reshape(-1)
+  if d.shape != s.shape:
+    raise ValueError(f'{dest_name} and {src_name} must have the same length ({d.numel()} vs {s.numel()})')
+  if d.numel():
+    if bool(((d < 0) | (d >= n_dest)).any()):
+      raise ValueError(f'{dest_name} must lie in 0..{n_dest - 1}')
+    if bool(((s < 0) | (s >= n_src)).any()):
+      raise ValueError(f'{src_name} must lie in 0..{n_src - 1}')
+    if torch.unique(d).numel() != d.numel():
+      raise ValueError(f'{dest_name} names a destination twice')
+  idx = torch.full((n_dest,), -1, dtype=torch.int32, device=device)
+  idx[d] = s.to(torch.int32)
+  return idx
+
+
+def check_bank_tags(bank, slots, tag: bytes) -> None:
+  """Raises ValueError unless every bank row in `slots` starts with `tag` (the engine's state_tag): a row that was never
+  stored, or was stored by an engine of another substrate, would be skipped by the restore. One compare on the bank's
+  device."""
+  import torch  # pylint: disable=g-import-not-at-top
+  s = torch.as_tensor(slots, dtype=torch.int64, device=bank.device).reshape(-1)
+  if not s.numel():
+    return
+  want = torch.frombuffer(bytearray(tag), dtype=torch.uint8).to(bank.device)
+  bad = (bank[s, :16] != want).any(dim=1)
+  if bool(bad.any()):
+    raise ValueError(f'bank rows {s[bad].tolist()} hold no record of this engine (never stored, or stored by an engine '
+                     'of another substrate)')
+
+
 class BatchedSubstrate:
   """`num_envs` independent instances of a substrate on one GPU.
 
   Observations are zero-copy views of the engine's output buffers and are overwritten by the
   next `step`/`reset`; clone what must be kept, or step into tensors of your own with
   `step(actions, out=traj.at(t))` (see `trajectory`), which costs no copy.
+
+  Single envs can be stored into and restored from a device state bank (`state_bank`, `store`, `restore`), e.g. to
+  branch rollouts from one state or restart episodes from stored start states. A clone is a store followed by a
+  restore: `store(bank, [i], [0]); restore(bank, [j, k], [0, 0])` makes envs j and k twins of env i, drawing the same
+  random numbers as env i would (with `rekey=True` they draw their own).
   """
 
   def __init__(self, blob, num_envs: int, device: int = 0, seed: Optional[int] = None,
@@ -278,6 +319,34 @@ class BatchedSubstrate:
   def load_state(self, snapshot: bytes) -> BatchedTimeStep:
     """Restores a snapshot taken from an identically built BatchedSubstrate; returns the timestep it held."""
     self._engine.load_state(snapshot)
+    return self._timestep()
+
+  def state_bank(self, capacity: int):
+    """A zeroed CUDA uint8 bank [capacity, record_bytes] for `store` / `restore`. A record restores into any
+    BatchedSubstrate built from the same substrate (or the same variants, in the same order), whatever its num_envs,
+    seed or device (copy the bank there)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    if capacity < 1:
+      raise ValueError(f'a state bank needs capacity >= 1, got {capacity}')
+    e = self._engine
+    return torch.zeros((int(capacity), e.state_record_bytes), dtype=torch.uint8, device=torch.device('cuda', e.device))
+
+  def store(self, bank, envs, slots) -> None:
+    """Stores env envs[i] into bank row slots[i] for every i (asynchronous, on the current stream). The record holds
+    the env's state, its current timestep and its random stream, not its images."""
+    e = self._engine
+    idx = bank_index(slots, envs, int(bank.shape[0]), self.num_envs, 'slots', 'envs', device=bank.device)
+    e.store_states(bank, idx)
+
+  def restore(self, bank, envs, slots, rekey: bool = False) -> BatchedTimeStep:
+    """Restores bank row slots[i] into env envs[i] for every i and re-renders; returns the timestep, in which each
+    restored env shows the stored env's timestep and images at store time. The other envs are untouched. A restored env
+    continues exactly as the stored env would have (given the same actions), from an auto-reset if its stored step was
+    LAST, and under the stored env's variant; rekey=True gives it its own random stream instead."""
+    e = self._engine
+    idx = bank_index(envs, slots, self.num_envs, int(bank.shape[0]), 'envs', 'slots', device=bank.device)
+    check_bank_tags(bank, slots, e.state_tag)
+    e.restore_states(bank, idx, rekey=rekey)
     return self._timestep()
 
   def action_spec(self):

@@ -1,4 +1,4 @@
-"""Small workload for compute-sanitizer (memcheck / racecheck / synccheck) on both kernels.
+"""Small workload for compute-sanitizer (memcheck / racecheck / synccheck) on the engine's kernels.
 
   compute-sanitizer --tool memcheck  python tools/sanitize_run.py
   compute-sanitizer --tool racecheck python tools/sanitize_run.py
@@ -27,6 +27,13 @@ for name, players, n_act, B in CASES:
     if name in ('clean_up', 'territory__rooms'):
       eng.exchange_wait(); eng.gather_obs_wait()
   eng.debug_observations()
+  if name not in ('clean_up', 'territory__rooms'):  # state bank (a restore is refused once peers are connected)
+    bank = torch.zeros((4, eng.state_record_bytes), dtype=torch.uint8, device='cuda')
+    eng.store_states(bank, torch.tensor([0, B - 1, -1, B], dtype=torch.int32, device='cuda'))  # rows 2, 3 skipped
+    slots = torch.full((B,), -1, dtype=torch.int32, device='cuda')
+    slots[1::3] = 0; slots[2::5] = 1; slots[3::7] = 2   # fan-out, and row 2 is untagged
+    eng.restore_states(bank, slots); eng.restore_states(bank, slots, rekey=True)
+    eng.step(torch.randint(0, n_act, (B, len(roles)), generator=gen, device='cuda', dtype=torch.int32))
   torch.cuda.synchronize()
   if name in ('clean_up', 'territory__rooms'):
     assert torch.equal(eng.gathered_timestep(), eng.timestep_packed) and torch.equal(eng.gathered_observations()[0], eng.rgb)
