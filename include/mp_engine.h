@@ -319,6 +319,22 @@ int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* b
 #define MP_RESTORE_REKEY 1u
 int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, void* stream);
 
+/* A step that restores at the same time: env b takes bank row slot_of_env[b] under mp_state_restore's rule (index in
+ * 0..n_slots-1, this engine's tag) instead of advancing, and ignores its action; the restore takes precedence over its
+ * auto-reset after LAST. Every other env steps as in mp_step. The state transition does the restore in the same kernel,
+ * so the render that follows draws the restored envs with all the others: no second render, no extra launch. For an
+ * engine that is not connected, the call gives, byte for byte, what mp_step(actions) followed by mp_state_restore(
+ * slot_of_env, bank, n_slots, flags) gives: outputs, events, state, variants and keys. flags: MP_RESTORE_REKEY as for
+ * mp_state_restore. out: NULL launches as mp_step does, a target as mp_step_into does (same kernels, same count, the
+ * restored envs' timestep and images delivered into it like any env's). It is accepted after mp_exchange_connect /
+ * mp_gather_obs_connect and counts as a step in their sequence, so the restored envs' rows and images are published as
+ * a step's; every rank issues it wherever the others issue a step (an index of all -1 restores nothing). Its render
+ * waits for slot 0's copy-out of mp_step_host_async as mp_step's does. Every check runs before anything is enqueued, and
+ * a refused call steps no env: those of mp_state_restore's bank and index array, those of mp_step_into's `out`, and
+ * the bank and the index array must not overlap `out`'s targets. */
+int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
+                    const mp_device_outputs* out, void* stream);
+
 /* Diagnostic: how the renderer was laid out for this substrate: teams per CTA, threads per team, log2 of the pixel
  * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes,
  * then the lane -> cell dealing built for player strips and for WORLD.RGB strips (0 plain, 2 scattered colouring,

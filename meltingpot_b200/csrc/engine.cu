@@ -139,18 +139,22 @@ struct VariantSet {
   uint8_t* pending = nullptr;    // [B] the variant each env's next episode runs
   int n = 1;
 };
+// The launches take the restore of mp_step_restore, or null for the plain k_step.
 struct FamilyEntry {
   int id;  // MpbFamily
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
-  cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int);
+  cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int,
+                        const StepRestore*);
   size_t (*step_smem)(const Tables&);
   const void* step;           // k_step<Family>
   // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field), the upload of base's Params with
   // each variant's knobs (base holds the engine's device tables), and the k_step<Family, ParamVariants> launch
   int (*same_shape)(const FamilyParams&, const FamilyParams&);
   int (*upload_variants)(std::vector<void*>&, const FamilyParams& base, const std::vector<FamilyParams>&, const void**);
-  cudaError_t (*launch_variants)(const cudaLaunchConfig_t&, const Tables&, const VariantSet&, const State&, const int32_t*, const uint8_t*, int);
+  cudaError_t (*launch_variants)(const cudaLaunchConfig_t&, const Tables&, const VariantSet&, const State&, const int32_t*, const uint8_t*, int,
+                                 const StepRestore*);
   const void* step_variants;  // k_step<Family, ParamVariants<Family::Params>>
+  const void* step_restore[2];  // the kRestore instantiations of both (mp_step_restore)
 };
 
 template <class Family>
@@ -159,8 +163,10 @@ int load_family(FamilyLoad& ld, const Tables& T, FamilyParams& params) {
 }
 template <class Family>
 cudaError_t launch_family(const cudaLaunchConfig_t& cfg, const Tables& T, const FamilyParams& params, const State& S,
-                          const int32_t* actions, const uint8_t* mask, int mode) {
-  return cudaLaunchKernelEx(&cfg, k_step<Family>, T, std::get<typename Family::Params>(params), S, actions, mask, mode);
+                          const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore) {
+  const typename Family::Params& F = std::get<typename Family::Params>(params);
+  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, typename Family::Params, true>, T, F, S, actions, mask, mode, *restore);
+  return cudaLaunchKernelEx(&cfg, k_step<Family>, T, F, S, actions, mask, mode, StepRestore{});
 }
 template <class Family>
 int same_shape_family(const FamilyParams& a, const FamilyParams& b) {
@@ -178,16 +184,19 @@ int upload_variants_family(std::vector<void*>& allocs, const FamilyParams& base,
 }
 template <class Family>
 cudaError_t launch_variants_family(const cudaLaunchConfig_t& cfg, const Tables& T, const VariantSet& V, const State& S,
-                                   const int32_t* actions, const uint8_t* mask, int mode) {
+                                   const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore) {
   using P = typename Family::Params;
   const ParamVariants<P> src{static_cast<const P*>(V.params), V.active, V.pending, V.n};
-  return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode);
+  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true>, T, src, S, actions, mask, mode, *restore);
+  return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode, StepRestore{});
 }
 template <class Family>
 FamilyEntry family_entry(int id) {
   return {id, load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
           same_shape_family<Family>, upload_variants_family<Family>, launch_variants_family<Family>,
-          reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>)};
+          reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>),
+          {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true>),
+           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, true>)}};
 }
 const FamilyEntry kFamilies[] = {
     family_entry<CleanUp>(MPB_FAMILY_CLEAN_UP),
@@ -250,6 +259,7 @@ struct mp_engine {
   uint64_t key_base = 0;   // seed + env_index_base: env b's key at creation is key_base + b (State::key)
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
+  RecordLayout* d_record_layout = nullptr;  // device copy of record_layout(this), read by mp_step_restore's k_step
 
   template <typename T>
   int alloc(size_t count, T** out) {
@@ -650,7 +660,9 @@ int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
 }
 
 // `render_follows`: the caller launches the renderer next on the same stream; it raises the exchange flags.
-int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int mode, cudaStream_t st, bool render_follows = true) {
+// `restore`: a step (mode 0) that restores the envs it names instead of advancing them (k_step<..., true>), or null.
+int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int mode, cudaStream_t st, bool render_follows = true,
+                 const StepRestore* restore = nullptr) {
   const int blocks = (E->B + 3) / 4;
   if (E->S.x_world) E->S.x_step = ++E->x_seq;
   cudaLaunchConfig_t cfg = {};
@@ -659,8 +671,8 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  if (E->variants.n > 1) CUDA_TRY(E->family->launch_variants(cfg, E->T, E->variants, E->S, actions, mask, mode));
-  else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode));
+  if (E->variants.n > 1) CUDA_TRY(E->family->launch_variants(cfg, E->T, E->variants, E->S, actions, mask, mode, restore));
+  else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode, restore));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st, E->S); }
@@ -780,6 +792,10 @@ extern "C" {
 const char* mp_last_error(void) { return g_error.c_str(); }
 const char* mp_version(void) { return "meltingpot_b200 engine 0.1 (sm_90a)"; }
 
+namespace {
+int upload_record_layout(mp_engine* E);  // (after record_layout, below)
+}
+
 int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
   if (!blob || !out || num_envs < 1) return fail(MP_E_INVALID, "mp_create: bad arguments");
   int n_dev = 0;
@@ -886,6 +902,8 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
       for (const FamilyEntry& f : kFamilies) {
         if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
         if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step_variants, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+        for (const void* k : f.step_restore)
+          if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
       }
       if (ce == cudaSuccess) step_smem_max[device] = need;
     }
@@ -902,6 +920,10 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   // SURVEY.md section 8d: observations + scalars + actions + one read and one write of the compact grid.
   E->render_bytes = (uint64_t)P * E->R.player_bytes + (uint64_t)E->R.world_bytes + (uint64_t)T.L * T.cells * 2;
   E->algo_bytes = (uint64_t)P * E->R.player_bytes + (uint64_t)E->R.world_bytes + 8ull * ((1 + T.n_scalar) * P + 2) + 8ull * P + 2ull * T.L * T.cells * 2;
+  if ((rc = E->alloc(1, &E->d_record_layout)) || (rc = upload_record_layout(E))) {
+    mp_destroy(E);
+    return rc;
+  }
   *out = E;
   return MP_OK;
 }
@@ -947,6 +969,13 @@ RecordLayout record_layout(const mp_engine* E) {
   return R;
 }
 static_assert(17 + 4 + 3 <= MP_RECORD_MAX_ROWS, "record rows: 17 state spans, up to 4 scalar_obs rows, key and variants");
+
+// The layout mp_step_restore's k_step reads: set at mp_create and again once mp_create_variants has added the variant rows.
+int upload_record_layout(mp_engine* E) {
+  const RecordLayout R = record_layout(E);
+  CUDA_TRY(cudaMemcpy(E->d_record_layout, &R, sizeof R, cudaMemcpyHostToDevice));
+  return MP_OK;
+}
 
 // Rule (a) of mp_create_variants: variant `v` has the same sections as variant 0, byte for byte, except the family's
 // parameter blocks, the component tables and the metadata string.
@@ -1026,7 +1055,7 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
   uint64_t h = fnv1a(&n, sizeof n);
   for (int v = 0; v < n; ++v) { const uint64_t hv = fnv1a(blobs[v], blob_bytes[v]); h = fnv1a(&hv, sizeof hv, h); }
   E->blob_hash = h;
-  return MP_OK;
+  return upload_record_layout(E);
 }
 }  // namespace
 
@@ -1174,11 +1203,11 @@ int check_extents(mp_engine* E, const std::vector<DeviceExtent>& outs, const cha
 }
 
 // Every check of mp_step_into / mp_reset_into (include/mp_engine.h), before anything is enqueued: a pointer that fails
-// one never reaches a kernel. Extents are computed in 128 bits, so no stride can wrap them around.
-int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn) {
+// one never reaches a kernel. Extents are computed in 128 bits, so no stride can wrap them around. `outs`: other
+// extents of the call (mp_step_restore's bank and index array), which must not overlap the targets either.
+int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn, std::vector<DeviceExtent> outs = {}) {
   if (!o) return fail(MP_E_INVALID, "%s: null outputs (use mp_step / mp_reset)", fn);
   const uint64_t B = E->B, P = E->T.P, n = E->T.n_scalar;
-  std::vector<DeviceExtent> outs;
   auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_env, uint64_t align, u128 extra) -> int {
     if (!p) return MP_OK;
     if ((uintptr_t)p % align || stride % align)
@@ -1555,14 +1584,16 @@ int mp_state_record_bytes(mp_handle h, uint64_t* bytes, uint8_t tag[16]) {
 }
 
 namespace {
-// The host checks of mp_state_store / mp_state_restore: the bank and the index array lie in device allocations on the
-// engine's device, overlap neither each other nor the engine's buffers, and the bank is 16-byte aligned.
-int check_bank(mp_engine* E, const void* bank, int n_slots, const int32_t* index, uint64_t index_count, uint64_t record_bytes, const char* fn) {
+// The host checks of mp_state_store / mp_state_restore / mp_step_restore: the bank is 16-byte aligned, and the bank
+// and the index array lie in device allocations on the engine's device and overlap neither each other nor the
+// engine's buffers (nor the targets of mp_step_restore's `out`).
+int check_bank(mp_engine* E, const void* bank, int n_slots, const int32_t* index, uint64_t index_count, uint64_t record_bytes, const char* fn,
+               const mp_device_outputs* out = nullptr) {
   if ((uintptr_t)bank % 16) return fail(MP_E_INVALID, "%s: bank is not 16-byte aligned", fn);
   if ((uintptr_t)index % 4) return fail(MP_E_INVALID, "%s: index array is not 4-byte aligned", fn);
-  const std::vector<DeviceExtent> ext{{"bank", (uintptr_t)bank, (u128)n_slots * record_bytes},
-                                      {"index array", (uintptr_t)index, (u128)index_count * 4}};
-  return check_extents(E, ext, fn);
+  std::vector<DeviceExtent> ext{{"bank", (uintptr_t)bank, (u128)n_slots * record_bytes},
+                                {"index array", (uintptr_t)index, (u128)index_count * 4}};
+  return out ? check_device_outputs(E, out, fn, std::move(ext)) : check_extents(E, ext, fn);
 }
 }  // namespace
 
@@ -1595,6 +1626,22 @@ int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, 
   ++h->launches;
   CUDA_TRY(cudaGetLastError());
   return launch_render(h, st);
+}
+
+int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
+                    const mp_device_outputs* out, void* stream) {
+  if (!h || !actions || !slot_of_env || !bank) return fail(MP_E_INVALID, "mp_step_restore: null argument");
+  if (n_slots < 1) return fail(MP_E_INVALID, "mp_step_restore: n_slots %d < 1", n_slots);
+  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_restore: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
+  DeviceGuard guard(h->device);
+  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, record_layout(h).record_bytes, "mp_step_restore", out);
+  if (rc) return rc;
+  const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
+                            (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
+  cudaStream_t st = (cudaStream_t)stream;
+  // launched as mp_step (out == NULL) or mp_step_into: the same kernels, the same exchange and gather sequence
+  if ((rc = launch_state(h, actions, nullptr, 0, st, /*render_follows=*/out != nullptr, &restore))) return rc;
+  return launch_render(h, st, out);
 }
 
 int mp_launch_count(mp_handle h, uint64_t* out) {

@@ -6,6 +6,8 @@
 // a store, an env for a restore) is written by one warp that reads exactly one source, so no two threads ever write the
 // same bytes, whatever indices the caller passes (a fan-out of one record to many envs included). Indices out of range
 // and records whose tag is not this engine's are skipped in-kernel; they can neither fault nor write anything.
+// The same per-warp restore (restore_env) also runs inside a step (k_step<..., kRestore>, step_common.cuh): the warp of a named
+// env copies the record instead of advancing it, and the render that follows draws it with every other env.
 #pragma once
 
 #include "common.cuh"
@@ -60,17 +62,16 @@ __global__ void __launch_bounds__(256) k_state_store(const __grid_constant__ Rec
   }
 }
 
-// One warp per env b: env b receives bank row slot_of_env[b] when that is in 0..n_slots-1 and carries this engine's
-// tag. rekey: the key row becomes key_base + b instead of the record's key.
-__global__ void __launch_bounds__(256) k_state_restore(const __grid_constant__ RecordLayout R, const int32_t* __restrict__ slot_of_env,
-                                                       const uint8_t* __restrict__ bank, int n_slots, int B, int rekey, uint64_t key_base) {
-  const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (b >= B) return;
+// Called by every lane of the warp that owns env b: env b receives bank row slot_of_env[b] when that is in
+// 0..n_slots-1 and carries this engine's tag. rekey: the key row becomes key_base + b instead of the record's key.
+// Returns whether the env was restored (the same on every lane).
+__device__ __forceinline__ bool restore_env(const RecordLayout& R, const int32_t* __restrict__ slot_of_env, const uint8_t* __restrict__ bank,
+                                            int n_slots, int b, int lane, int rekey, uint64_t key_base) {
   const int s = slot_of_env[b];
-  if (s < 0 || s >= n_slots) return;
+  if (s < 0 || s >= n_slots) return false;
   const uint8_t* rec = bank + (size_t)s * R.record_bytes;
   const uint4 t = *reinterpret_cast<const uint4*>(rec);
-  if (t.x != R.tag.x || t.y != R.tag.y || t.z != R.tag.z || t.w != R.tag.w) return;
+  if (t.x != R.tag.x || t.y != R.tag.y || t.z != R.tag.z || t.w != R.tag.w) return false;
   for (int r = 0; r < R.n_rows; ++r) {
     const RecordRow& w = R.row[r];
     if (!w.base) continue;
@@ -81,4 +82,25 @@ __global__ void __launch_bounds__(256) k_state_restore(const __grid_constant__ R
     }
     copy_row(dst, rec + w.offset, w.bytes, lane);
   }
+  return true;
 }
+
+// One warp per env b (restore_env).
+__global__ void __launch_bounds__(256) k_state_restore(const __grid_constant__ RecordLayout R, const int32_t* __restrict__ slot_of_env,
+                                                       const uint8_t* __restrict__ bank, int n_slots, int B, int rekey, uint64_t key_base) {
+  const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  restore_env(R, slot_of_env, bank, n_slots, b, lane, rekey, key_base);
+}
+
+// The restore a step carries out in place of advancing the envs it names (mp_step_restore, k_step<..., true>): the
+// engine's record layout (a device copy made at mp_create, so the step's parameter space grows by one pointer, not a
+// whole RecordLayout) and the call's index array, bank and rekey flag.
+struct StepRestore {
+  const RecordLayout* layout;
+  const int32_t* slot_of_env;  // [B]
+  const uint8_t* bank;
+  int n_slots;
+  int rekey;
+  uint64_t key_base;
+};

@@ -11,6 +11,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "state_bank.cuh"
 
 __host__ __device__ inline size_t scratch_round16(size_t n) { return (n + 15) & ~(size_t)15; }
 
@@ -84,9 +85,14 @@ __device__ __forceinline__ const Params& env_params(const ParamVariants<Params>&
 // without it, the compiler copies a small Params that is indexed with a run-time value (coins' coin_reward[who],
 // coop_mining's ore_sprite[state]) to the stack, and passed on as it is, it keeps its constant-bank reads. Variants are
 // read through the L1 from the device array.
-template <class Family, class Source = typename Family::Params>
+//
+// kRestore (mp_step_restore, mode 0 only): the warp of an env that `restore` names (restore_env's predicate, read after
+// the dependency wait) copies that record instead of advancing, which also takes precedence over the auto-reset after
+// LAST; the record carries the timestep and the events, so event_begin / event_end are skipped too. Every other warp
+// runs the plain step. With kRestore = false, `restore` is never read and the kernel is the plain step.
+template <class Family, class Source = typename Family::Params, bool kRestore = false>
 __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant__ Source src, State S, const int32_t* __restrict__ actions,
-                                                 const uint8_t* __restrict__ mask, int mode) {
+                                                 const uint8_t* __restrict__ mask, int mode, const __grid_constant__ StepRestore restore) {
   constexpr bool kVariants = !std::is_same<Source, typename Family::Params>::value;
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -102,6 +108,9 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
   if constexpr (Family::kStagesTables) __syncthreads();
   const int b = blockIdx.x * 4 + warp;
   if (b >= S.B) return;
+  if constexpr (kRestore) {
+    if (restore_env(*restore.layout, restore.slot_of_env, restore.bank, restore.n_slots, b, lane, restore.rekey, restore.key_base)) return;
+  }
   typename Family::Scratch sc = Family::carve(T, smem + warp * Family::scratch_bytes(T), tables);
   if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
     event_begin(lane);

@@ -119,8 +119,11 @@ class ShardedSubstrate:
     """out: a BatchedTimeStep of this rank's envs to fill (BatchedSubstrate.step)."""
     return self.local.reset(out=out)
 
-  def step(self, local_actions, out=None):
-    return self.local.step(local_actions, out=out)
+  def step(self, local_actions, out=None, restore=None, bank=None, rekey: bool = False):
+    """restore / bank / rekey: as BatchedSubstrate.step, with restore indexed by LOCAL env. On a connected shard the
+    restored envs' rows and images are published like any step's; every rank steps when the others do (passing an
+    index of all -1 when it restores nothing)."""
+    return self.local.step(local_actions, out=out, restore=restore, bank=bank, rekey=rekey)
 
   # -- engine-level exchanges (peer-memory stores from the kernels; no collective per step) ---------------------------
   def connect(self, observations: bool = False) -> None:

@@ -60,7 +60,7 @@ EXPORTED_SYMBOLS = (
     'mp_exchange_connect', 'mp_exchange_wait', 'mp_exchange_slot', 'mp_debug_lane_map', 'mp_debug_observations',
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
     'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
-    'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore',
+    'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_step_restore',
 )
 
 MP_RESTORE_REKEY = 1
@@ -202,6 +202,7 @@ def load_library() -> ctypes.CDLL:
   lib.mp_state_record_bytes.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), vp]
   lib.mp_state_store.argtypes = [vp, vp, ctypes.c_int, vp, vp]
   lib.mp_state_restore.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_uint32, vp]
+  lib.mp_step_restore.argtypes = [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(MpDeviceOutputs), vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
   lib.mp_step_host_async.argtypes = [vp, vp, ctypes.POINTER(MpHostOutputs), ctypes.c_int, vp]
@@ -406,14 +407,37 @@ class Engine:
       s = self._device_outputs(out)
       _check(self._lib.mp_reset_into(self._h, ptr, ctypes.byref(s), self._stream(stream)))
 
-  def step(self, actions, stream=None, out=None) -> None:
+  def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False) -> None:
     """actions: int32 CUDA tensor [B, P] of discrete action ids.
 
     out: {name: CUDA tensor} for any of DEVICE_OUTPUTS (mp_step_into): the step's images are rendered straight into
     out['rgb'] / out['world_rgb'] instead of this engine's own image buffers, and its scalars are written into the
     others as well as into this engine's buffers. Shapes and dtypes are those of the engine's views (rgb, reward, ...);
-    the env axis may have any stride (and the observation axis of scalar_obs), every other axis is dense."""
+    the env axis may have any stride (and the observation axis of scalar_obs), every other axis is dense.
+
+    restore, bank: restore envs within the step (mp_step_restore). restore is a contiguous CUDA int32 tensor [B] and
+    bank a state bank (see restore_states). Env b takes bank row restore[b] instead of stepping, ignoring its action,
+    when that index is in 0..n_slots-1 and the row holds one of this engine's records; -1, any other out-of-range index
+    and rows without this engine's tag step env b as usual. The result is that of a step followed by
+    restore_states(bank, restore, rekey), without the second render. Only the tensors' shape, dtype, device and
+    layout are checked, never their values, so the call never synchronises: build the index on the device, e.g.
+    `torch.where(step_type == 2, row, -1)`. rekey: as for restore_states."""
     self._check_actions(actions)
+    if restore is not None or bank is not None:
+      if restore is None or bank is None:
+        raise ValueError('restore and bank go together')
+      bank = self._bank(bank)
+      idx = self._indices(restore, self.num_envs, 'restore')
+      for name, t in (('bank', bank), ('restore', idx)):
+        if t.device.index != self.device:
+          raise ValueError(f'{name} is on {t.device}, the engine runs on cuda:{self.device}')
+      s = None if out is None else ctypes.byref(self._device_outputs(out))
+      _check(self._lib.mp_step_restore(self._h, ctypes.c_void_p(actions.data_ptr()), ctypes.c_void_p(idx.data_ptr()),
+                                       ctypes.c_void_p(bank.data_ptr()), int(bank.shape[0]),
+                                       ctypes.c_uint32(MP_RESTORE_REKEY if rekey else 0), s, self._stream(stream)))
+      return
+    if rekey:
+      raise ValueError('rekey needs restore and bank')
     if out is None:
       _check(self._lib.mp_step(self._h, ctypes.c_void_p(actions.data_ptr()), self._stream(stream)))
     else:

@@ -249,19 +249,27 @@ class BatchedSubstrate:
     self._engine.reset(mask, out=self._engine_outputs(out))
     return self._fill_collective(out)
 
-  def step(self, actions, out: Optional[BatchedTimeStep] = None) -> BatchedTimeStep:
+  def step(self, actions, out: Optional[BatchedTimeStep] = None, restore=None, bank=None,
+           rekey: bool = False) -> BatchedTimeStep:
     """actions: integer tensor [B, P] on the engine's device (int32 preferred).
 
     out: a BatchedTimeStep of caller-owned tensors to fill and return instead of views of the engine's buffers, e.g.
     `trajectory(T).at(t)`: the engine renders the images straight into it and delivers the scalars there too, so a
-    learner keeps T steps without copying them."""
+    learner keeps T steps without copying them.
+
+    restore, bank: restarts or clones envs within this step, at no extra render. restore is a CUDA int32 tensor [B]:
+    env b takes bank row restore[b] (a `state_bank` row written by `store`) instead of stepping, and shows that
+    record's timestep and images. -1, other out-of-range indices and rows that hold no record of this substrate step
+    env b as usual. The values are not checked, so nothing synchronises; e.g. restart finished episodes from stored
+    start states with `restore = torch.where(ts.step_type == 2, rows, -1)`. rekey: as for `restore`."""
     import torch  # pylint: disable=g-import-not-at-top
     if actions.dtype != torch.int32:
       actions = actions.to(torch.int32)
+    kw = dict(restore=restore, bank=bank, rekey=rekey)
     if out is None:
-      self._engine.step(actions.contiguous())
+      self._engine.step(actions.contiguous(), **kw)
       return self._timestep()
-    self._engine.step(actions.contiguous(), out=self._engine_outputs(out))
+    self._engine.step(actions.contiguous(), out=self._engine_outputs(out), **kw)
     return self._fill_collective(out)
 
   def trajectory(self, T: int, time_major: bool = True) -> 'Trajectory':

@@ -7,7 +7,11 @@ For each workload (clean_up x 4096 and commons_harvest__open 16p x 8192, each wi
   render:          mp_render (what a restore re-renders);
   restore:         mp_state_restore with rendering on (kernel + render);
   step:            a plain step with uniform-random actions, for scale;
-  d2d_copy:        a device-to-device copy of the same 2 x record_bytes x B bytes (read + write), the bandwidth yardstick.
+  d2d_copy:        a device-to-device copy of the same 2 x record_bytes x B bytes (read + write), the bandwidth yardstick;
+  step_restore:    a step that restores a fraction of the envs instead of advancing them (mp_step_restore);
+  step+restore:    a step followed by mp_state_restore of the same envs (what step_restore replaces).
+The last two run at restored fractions 0, 1/64, 1/8 and 1 of B (field `restored`: envs restored per call, spread evenly
+over the batch).
 
 Timed with CUDA events over --reps calls after a warm-up of every call. The kernels' rate is reported against the bytes
 they have to move, 2 x record_bytes x B (each record is read once and written once). Prints one JSON line per
@@ -26,6 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = (('clean_up', 7, 4096), ('commons_harvest__open', 16, 8192))
+FRACTIONS = ((0, 1), (1, 64), (1, 8), (1, 1))
 
 
 def _gpu():
@@ -87,6 +92,26 @@ def main():
       copy_dst = torch.empty_like(copy_src)
       calls = {'store': lambda: eng.store_states(bank, every), 'restore_kernel': restore_kernel, 'render': eng.render,
                'restore': lambda: eng.restore_states(bank, every), 'step': step, 'd2d_copy': lambda: copy_dst.copy_(copy_src)}
+      restored = {}
+      for num, den in FRACTIONS:
+        n = B * num // den
+        idx = torch.full((B,), -1, dtype=torch.int32, device='cuda')
+        if n:
+          envs = torch.arange(0, B, B // n, device='cuda')[:n]
+          idx[envs] = envs.to(torch.int32)
+
+        def step_restore(idx=idx):
+          eng.step(actions[k[0] % len(actions)], restore=idx, bank=bank)
+          k[0] += 1
+
+        def step_then_restore(idx=idx):
+          step()
+          eng.restore_states(bank, idx)
+
+        tag = f'{num}/{den}'
+        calls[f'step_restore {tag}'] = step_restore
+        calls[f'step+restore {tag}'] = step_then_restore
+        restored[f'step_restore {tag}'] = restored[f'step+restore {tag}'] = n
       for fn in calls.values():  # warm-up
         for _ in range(3):
           fn()
@@ -96,6 +121,8 @@ def main():
         ms = _time(fn, args.reps)
         row = dict(substrate=name, players=P, envs=B, world_rgb=world, call=call, ms=round(ms, 4), record_bytes=R,
                    reps=args.reps, gpu=gpu)
+        if call in restored:
+          row['restored'] = restored[call]
         if call in ('store', 'restore_kernel', 'd2d_copy'):
           row['bytes'] = moved
           row['GB_per_s'] = round(moved / (ms * 1e-3) / 1e9, 1)
