@@ -252,14 +252,13 @@ struct mp_engine {
   uint64_t algo_bytes = 0, render_bytes = 0;
   std::vector<uint8_t> host_pair, host_sflags;  // kept for mp_debug_render_tables
   int black_sprite = -1;
-  std::vector<std::pair<void*, size_t>> state_spans;  // what mp_state_save / mp_state_load copy
-  uint64_t state_bytes = 0;
   int lane_map_players = 0, lane_map_world = 0;  // 0 plain, 2 scattered colouring, 1 + 16 * (extra wavefronts left) whole-cell dealing
   int inst_ncp = 0, inst_ncw = 0;                // the k_render<NCP, NCW> instantiation this engine launches
   uint64_t key_base = 0;   // seed + env_index_base: env b's key at creation is key_base + b (State::key)
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
-  RecordLayout* d_record_layout = nullptr;  // device copy of record_layout(this), read by mp_step_restore's k_step
+  RecordLayout record{};                     // every per-env state array (layout_state): what records and snapshots copy
+  RecordLayout* d_record_layout = nullptr;  // device copy of `record`, read by mp_step_restore's k_step
 
   template <typename T>
   int alloc(size_t count, T** out) {
@@ -785,16 +784,64 @@ struct DeviceGuard {
   ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
+uint64_t fnv1a(const void* p, size_t n, uint64_t h = 1469598103934665603ull) {
+  const uint8_t* bp = static_cast<const uint8_t*>(p);
+  for (size_t i = 0; i < n; ++i) { h ^= bp[i]; h *= 1099511628211ull; }
+  return h;
+}
+
+// The one list of per-env state arrays, as E->record and its device copy. Env b's row of an array is its `bytes` bytes
+// at base + b * bytes: one env's rows make its state-bank record (mp_state_store / mp_state_restore), the arrays whole
+// make a snapshot (mp_state_save / mp_state_load). Images are not state; a restore or a load re-renders them. Every
+// size follows from the blob (or the variant set) alone, so a record restores into any engine built from it, whatever
+// its num_envs, seed, env_index_base or device. A record:
+//   [0, 16)   tag: format word, record bytes, blob_hash (the hash of the ordered variant set for a variant engine)
+//   [16, 24)  key u64; [24] active, [25] pending variant (0 in a single-blob engine, which has neither array)
+//   [32, ..)  every other array in list order, each row at a 16-byte offset
+// `allocate` (mp_create): first gives every array that has an allocation of its own its B zeroed rows. reward,
+// discount, step_type and scalar_obs are carved from the scalar block; mp_create_variants adds active and pending.
+constexpr uint32_t kRecordFormat = 0x3152504du;  // "MPR1"
+int layout_state(mp_engine* E, bool allocate) {
+  const Tables& T = E->T;
+  State& S = E->S;
+  const uint32_t P = T.P;
+  RecordLayout& R = E->record;
+  R = RecordLayout{};  // key_row 0: the key is the first row
+  uint32_t off = 16;
+  int rc = MP_OK;
+  auto row = [&](void* base, uint32_t bytes, uint32_t align) {
+    if (R.n_rows == MP_RECORD_MAX_ROWS) { rc = fail(MP_E_UNSUPPORTED, "more than %d per-env state arrays", MP_RECORD_MAX_ROWS); return; }
+    off = (off + align - 1) / align * align;
+    R.row[R.n_rows++] = {static_cast<uint8_t*>(base), bytes, bytes, off};
+    off += bytes;
+  };
+  auto own = [&](auto*& p, uint32_t bytes, uint32_t align = 16) {
+    if (allocate && !rc) rc = E->alloc((size_t)E->B * bytes / sizeof *p, &p);
+    row(p, bytes, align);
+  };
+  own(S.key, 8, 8);
+  row(E->variants.active, 1, 1); row(E->variants.pending, 1, 1);
+  own(S.grid, T.L * T.cells_pad * 2); own(S.avatar, P * 16); own(S.av_timer, P * 16);
+  own(S.apple, T.nA_pad); own(S.dirt, T.nD_pad); own(S.water, T.nW_pad); own(S.apple_count, T.nA_pad);
+  own(S.fam_u8, S.fam_u8_stride); own(S.fam_u16, S.fam_u16_stride * 2); own(S.av_extra, P * 32);
+  own(S.packed, (P + 2) * 8); own(S.env, ENV_COLS * 4);
+  row(S.reward, P * 8, 16); row(S.discount, 8, 16); row(S.step_type, 8, 16);
+  for (int k = 0; k < T.n_scalar; ++k) row(S.scalar_obs + (size_t)k * E->B * P, P * 8, 16);
+  own(S.events, S.max_events * 12); own(S.n_events, 4);
+  if (rc) return rc;
+  R.record_bytes = (off + 15) / 16 * 16;
+  const uint64_t h = E->blob_hash;
+  R.tag = make_uint4(kRecordFormat, (uint32_t)R.record_bytes, (uint32_t)h, (uint32_t)(h >> 32));
+  CUDA_TRY(cudaMemcpy(E->d_record_layout, &R, sizeof R, cudaMemcpyHostToDevice));
+  return MP_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
 const char* mp_last_error(void) { return g_error.c_str(); }
 const char* mp_version(void) { return "meltingpot_b200 engine 0.1 (sm_90a)"; }
-
-namespace {
-int upload_record_layout(mp_engine* E);  // (after record_layout, below)
-}
 
 int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
   if (!blob || !out || num_envs < 1) return fail(MP_E_INVALID, "mp_create: bad arguments");
@@ -808,12 +855,7 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   DeviceGuard guard(device);
   mp_engine* E = new mp_engine();
   E->device = device; E->B = num_envs; E->flags = flags; E->sm_count = prop.multiProcessorCount;
-  {
-    uint64_t hsh = 1469598103934665603ull;
-    const uint8_t* bp = static_cast<const uint8_t*>(blob);
-    for (size_t i = 0; i < blob_bytes; ++i) { hsh ^= bp[i]; hsh *= 1099511628211ull; }
-    E->blob_hash = hsh;
-  }
+  E->blob_hash = fnv1a(blob, blob_bytes);
   int rc = build_tables(E, blob, blob_bytes);
   if (rc == MP_OK) rc = build_plan(E);
   if (rc != MP_OK) { mp_destroy(E); return rc; }
@@ -827,38 +869,23 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
     S.max_events = round_up(std::max(MP_MIN_EVENTS, T.P * (3 * E->beam_cells + 4 + T.P)), 16);
   }
   S.fam_u8_stride = std::max(16, RU_COUNT * T.nR_pad); S.fam_u16_stride = std::max(16, RS_COUNT * T.nR_pad);
-  if ((rc = E->alloc(B * T.L * T.cells_pad, &S.grid)) || (rc = E->alloc(B * P * 4, &S.avatar)) || (rc = E->alloc(B * P * 4, &S.av_timer)) ||
-      (rc = E->alloc(B * T.nA_pad, &S.apple)) || (rc = E->alloc(B * T.nD_pad, &S.dirt)) || (rc = E->alloc(B * T.nW_pad, &S.water)) || (rc = E->alloc(B * T.nA_pad, &S.apple_count)) || (rc = E->alloc(B * (size_t)S.fam_u8_stride, &S.fam_u8)) || (rc = E->alloc(B * (size_t)S.fam_u16_stride, &S.fam_u16)) || (rc = E->alloc(B * P * 8, &S.av_extra)) || (rc = E->alloc(B * (P + 2), &S.packed)) ||
-      (rc = E->alloc(B * ENV_COLS, &S.env)) || (rc = E->alloc(B, &S.key)) ||
-      (rc = E->alloc((B * P + B + B + std::max<size_t>(1, T.n_scalar) * B * P) * 8, &E->scalar_block)) ||
-      (rc = E->alloc(B * P * E->R.player_bytes, &S.rgb)) || (rc = E->alloc(B * (size_t)E->R.world_bytes, &S.world_rgb)) ||
-      (rc = E->alloc(B * (size_t)S.max_events * 3, &S.events)) || (rc = E->alloc(B, &S.n_events)) ||
-      (rc = E->alloc(B * P, &E->d_actions))) {
+  // reward [B][P] | discount [B] | step_type [B] | scalar_obs [n][B][P], all 8-byte elements, one block
+  E->scalar_block_bytes = (B * P + B + B + std::max<size_t>(1, T.n_scalar) * B * P) * 8;
+  if ((rc = E->alloc(E->scalar_block_bytes, &E->scalar_block)) || (rc = E->alloc(B * P * E->R.player_bytes, &S.rgb)) ||
+      (rc = E->alloc(B * (size_t)E->R.world_bytes, &S.world_rgb)) || (rc = E->alloc(B * P, &E->d_actions)) ||
+      (rc = E->alloc(1, &E->d_record_layout))) {
     mp_destroy(E);
     return rc;
   }
-  {  // reward [B][P] | discount [B] | step_type [B] | scalar_obs [n][B][P], all 8-byte elements, one block
-    E->scalar_block_bytes = (B * P + B + B + std::max<size_t>(1, T.n_scalar) * B * P) * 8;
-    S.reward = reinterpret_cast<double*>(E->scalar_block);
-    S.discount = S.reward + B * P;
-    S.step_type = reinterpret_cast<int64_t*>(S.discount + B);
-    S.scalar_obs = reinterpret_cast<double*>(S.step_type + B);
+  S.reward = reinterpret_cast<double*>(E->scalar_block);
+  S.discount = S.reward + B * P;
+  S.step_type = reinterpret_cast<int64_t*>(S.discount + B);
+  S.scalar_obs = reinterpret_cast<double*>(S.step_type + B);
+  if ((rc = layout_state(E, /*allocate=*/true))) {
+    mp_destroy(E);
+    return rc;
   }
   S.rgb_env_stride = P * E->R.player_bytes; S.world_env_stride = E->R.world_bytes;  // the own images: dense
-  {  // everything a later step depends on, plus the current timestep scalars; the images are re-rendered on load
-    const size_t ns = std::max<size_t>(1, T.n_scalar);
-    auto span = [&](void* p, size_t bytes) { E->state_spans.push_back({p, bytes}); E->state_bytes += bytes; };
-    span(S.grid, B * T.L * T.cells_pad * sizeof(*S.grid)); span(S.avatar, B * P * 4 * sizeof(*S.avatar));
-    span(S.av_timer, B * P * 4 * sizeof(*S.av_timer)); span(S.apple, B * T.nA_pad * sizeof(*S.apple));
-    span(S.dirt, B * T.nD_pad * sizeof(*S.dirt)); span(S.water, B * T.nW_pad * sizeof(*S.water));
-    span(S.apple_count, B * T.nA_pad * sizeof(*S.apple_count)); span(S.fam_u8, B * (size_t)S.fam_u8_stride * sizeof(*S.fam_u8));
-    span(S.fam_u16, B * (size_t)S.fam_u16_stride * sizeof(*S.fam_u16)); span(S.av_extra, B * P * 8 * sizeof(*S.av_extra));
-    span(S.packed, B * (P + 2) * sizeof(*S.packed)); span(S.env, B * ENV_COLS * sizeof(*S.env));
-    span(S.reward, B * P * sizeof(*S.reward)); span(S.discount, B * sizeof(*S.discount));
-    span(S.step_type, B * sizeof(*S.step_type)); span(S.scalar_obs, ns * B * P * sizeof(*S.scalar_obs));
-    span(S.events, B * (size_t)S.max_events * 3 * sizeof(*S.events)); span(S.n_events, B * sizeof(*S.n_events));
-    span(S.key, B * sizeof(*S.key));  // (record_layout below is one env's row of each of these)
-  }
   // episode counter starts at -1 so that the first reset plays episode 0; envs start "done".
   {
     std::vector<int32_t> env0(B * ENV_COLS, 0);
@@ -920,63 +947,11 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   // SURVEY.md section 8d: observations + scalars + actions + one read and one write of the compact grid.
   E->render_bytes = (uint64_t)P * E->R.player_bytes + (uint64_t)E->R.world_bytes + (uint64_t)T.L * T.cells * 2;
   E->algo_bytes = (uint64_t)P * E->R.player_bytes + (uint64_t)E->R.world_bytes + 8ull * ((1 + T.n_scalar) * P + 2) + 8ull * P + 2ull * T.L * T.cells * 2;
-  if ((rc = E->alloc(1, &E->d_record_layout)) || (rc = upload_record_layout(E))) {
-    mp_destroy(E);
-    return rc;
-  }
   *out = E;
   return MP_OK;
 }
 
 namespace {
-// The record of one env in a state bank (mp_state_store / mp_state_restore): env b's row of each state span of mp_create
-// (images excepted: a restore re-renders them). Every offset and length follows from the blob (or the variant set)
-// alone, so a record restores into any engine built from it, whatever its num_envs, seed, env_index_base or device.
-//   [0, 16)   tag: format word, record bytes, blob_hash (the hash of the ordered variant set for a variant engine)
-//   [16, 24)  key u64; [24] active, [25] pending variant (0 in a single-blob engine)
-//   [32, ..)  grid, avatar, av_timer, apple, dirt, water, apple_count, fam_u8, fam_u16, av_extra, packed, env, reward,
-//             discount, step_type, the n_scalar rows of scalar_obs [n][B][P], events [max_events][3], n_events; each
-//             row at a 16-byte offset
-constexpr uint32_t kRecordFormat = 0x3152504du;  // "MPR1"
-RecordLayout record_layout(const mp_engine* E) {
-  const Tables& T = E->T;
-  const State& S = E->S;
-  const uint64_t B = E->B, P = T.P;
-  RecordLayout R{};
-  R.key_row = 0;
-  uint32_t off = 16;
-  auto row = [&](const void* base, uint64_t env_stride, uint64_t bytes, uint32_t align) {
-    off = (off + align - 1) / align * align;
-    R.row[R.n_rows++] = {static_cast<uint8_t*>(const_cast<void*>(base)), env_stride, (uint32_t)bytes, off};
-    off += (uint32_t)bytes;
-  };
-  row(S.key, 8, 8, 8);
-  row(E->variants.n > 1 ? E->variants.active : nullptr, 1, 1, 1);
-  row(E->variants.n > 1 ? E->variants.pending : nullptr, 1, 1, 1);
-  const uint64_t grid = (uint64_t)T.L * T.cells_pad * sizeof(*S.grid);
-  row(S.grid, grid, grid, 16);
-  row(S.avatar, P * 16, P * 16, 16); row(S.av_timer, P * 16, P * 16, 16);
-  row(S.apple, T.nA_pad, T.nA_pad, 16); row(S.dirt, T.nD_pad, T.nD_pad, 16); row(S.water, T.nW_pad, T.nW_pad, 16);
-  row(S.apple_count, T.nA_pad, T.nA_pad, 16);
-  row(S.fam_u8, S.fam_u8_stride, S.fam_u8_stride, 16); row(S.fam_u16, S.fam_u16_stride * 2, S.fam_u16_stride * 2, 16);
-  row(S.av_extra, P * 32, P * 32, 16); row(S.packed, (P + 2) * 8, (P + 2) * 8, 16); row(S.env, ENV_COLS * 4, ENV_COLS * 4, 16);
-  row(S.reward, P * 8, P * 8, 16); row(S.discount, 8, 8, 16); row(S.step_type, 8, 8, 16);
-  for (int k = 0; k < T.n_scalar; ++k) row(S.scalar_obs + (size_t)k * B * P, P * 8, P * 8, 16);
-  row(S.events, (uint64_t)S.max_events * 12, (uint64_t)S.max_events * 12, 16); row(S.n_events, 4, 4, 16);
-  R.record_bytes = (off + 15) / 16 * 16;
-  const uint64_t h = E->blob_hash;
-  R.tag = make_uint4(kRecordFormat, (uint32_t)R.record_bytes, (uint32_t)h, (uint32_t)(h >> 32));
-  return R;
-}
-static_assert(17 + 4 + 3 <= MP_RECORD_MAX_ROWS, "record rows: 17 state spans, up to 4 scalar_obs rows, key and variants");
-
-// The layout mp_step_restore's k_step reads: set at mp_create and again once mp_create_variants has added the variant rows.
-int upload_record_layout(mp_engine* E) {
-  const RecordLayout R = record_layout(E);
-  CUDA_TRY(cudaMemcpy(E->d_record_layout, &R, sizeof R, cudaMemcpyHostToDevice));
-  return MP_OK;
-}
-
 // Rule (a) of mp_create_variants: variant `v` has the same sections as variant 0, byte for byte, except the family's
 // parameter blocks, the component tables and the metadata string.
 int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
@@ -1006,12 +981,6 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
   };
   int rc = check(s0, h0->n_sections, bv, nv, b0);
   return rc ? rc : check(sv, hv->n_sections, b0, n0, bv);
-}
-
-uint64_t fnv1a(const void* p, size_t n, uint64_t h = 1469598103934665603ull) {
-  const uint8_t* bp = static_cast<const uint8_t*>(p);
-  for (size_t i = 0; i < n; ++i) { h ^= bp[i]; h *= 1099511628211ull; }
-  return h;
 }
 
 // Rules (b)-(d) of mp_create_variants for an engine built from variant 0, then the variant set's device arrays.
@@ -1049,13 +1018,11 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
   if ((rc = upload(E->allocs, assign, &d))) return rc;
   E->variants.pending = const_cast<uint8_t*>(d);
   E->variants.n = n;
-  // snapshots carry the assignments, and only load into an engine with the same variants in the same order
-  E->state_spans.push_back({E->variants.active, B}); E->state_spans.push_back({E->variants.pending, B});
-  E->state_bytes += 2 * B;
+  // records and snapshots carry the assignments, and only load into an engine with the same variants in the same order
   uint64_t h = fnv1a(&n, sizeof n);
   for (int v = 0; v < n; ++v) { const uint64_t hv = fnv1a(blobs[v], blob_bytes[v]); h = fnv1a(&hv, sizeof hv, h); }
   E->blob_hash = h;
-  return upload_record_layout(E);
+  return layout_state(E, /*allocate=*/false);
 }
 }  // namespace
 
@@ -1183,8 +1150,10 @@ int check_extents(mp_engine* E, const std::vector<DeviceExtent>& outs, const cha
                   (unsigned long long)((u128)x.p + x.extent - ((u128)base + size)));
   }
   // no extent overlaps another output or the engine's own buffers
-  std::vector<std::pair<uintptr_t, uint64_t>> own;
-  for (const auto& sp : E->state_spans) own.push_back({(uintptr_t)sp.first, sp.second});
+  // (the whole scalar block: it also holds the unused scalar_obs row of a substrate without scalar observations)
+  std::vector<std::pair<uintptr_t, uint64_t>> own{{(uintptr_t)E->scalar_block, E->scalar_block_bytes}};
+  for (int r = 0; r < E->record.n_rows; ++r)
+    if (E->record.row[r].base) own.push_back({(uintptr_t)E->record.row[r].base, B * E->record.row[r].bytes});
   own.push_back({(uintptr_t)E->S.rgb, B * P * E->R.player_bytes});
   own.push_back({(uintptr_t)E->S.world_rgb, B * E->R.world_bytes});
   if (E->async_ready) {
@@ -1522,12 +1491,20 @@ int mp_exchange_slot(mp_handle h, int* slot, uint64_t* step) {
 }
 
 namespace {
-struct SnapshotHeader { char magic[4]; uint32_t version; uint64_t num_envs, payload_bytes, n_spans, rng_key0, blob_hash; };
+// A snapshot: this header, then every per-env state array of the engine (layout_state) whole, in list order.
+struct SnapshotHeader { char magic[4]; uint32_t version; uint64_t num_envs, payload_bytes, n_arrays, rng_key0, blob_hash; };
+
+SnapshotHeader snapshot_header(const mp_engine* E) {
+  SnapshotHeader hd{{'M', 'P', 'S', '5'}, 5u, (uint64_t)E->B, 0, 0, E->key_base, E->blob_hash};
+  for (int r = 0; r < E->record.n_rows; ++r)
+    if (E->record.row[r].base) { hd.payload_bytes += (uint64_t)E->B * E->record.row[r].bytes; ++hd.n_arrays; }
+  return hd;
 }
+}  // namespace
 
 int mp_state_size(mp_handle h, uint64_t* bytes) {
   if (!h || !bytes) return fail(MP_E_INVALID, "mp_state_size: null argument");
-  *bytes = sizeof(SnapshotHeader) + h->state_bytes;
+  *bytes = sizeof(SnapshotHeader) + snapshot_header(h).payload_bytes;
   return MP_OK;
 }
 
@@ -1535,12 +1512,14 @@ int mp_state_save(mp_handle h, void* host_dst, void* stream) {
   if (!h || !host_dst) return fail(MP_E_INVALID, "mp_state_save: null argument");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
-  SnapshotHeader hd{{'M', 'P', 'S', '4'}, 4u, (uint64_t)h->B, h->state_bytes, (uint64_t)h->state_spans.size(), h->key_base, h->blob_hash};
+  const SnapshotHeader hd = snapshot_header(h);
   memcpy(host_dst, &hd, sizeof(hd));
   uint8_t* dst = static_cast<uint8_t*>(host_dst) + sizeof(hd);
-  for (const auto& sp : h->state_spans) {
-    CUDA_TRY(cudaMemcpyAsync(dst, sp.first, sp.second, cudaMemcpyDeviceToHost, st));
-    dst += sp.second;
+  for (int r = 0; r < h->record.n_rows; ++r) {
+    const RecordRow& w = h->record.row[r];
+    if (!w.base) continue;
+    CUDA_TRY(cudaMemcpyAsync(dst, w.base, (size_t)h->B * w.bytes, cudaMemcpyDeviceToHost, st));
+    dst += (size_t)h->B * w.bytes;
   }
   CUDA_TRY(cudaStreamSynchronize(st));
   return MP_OK;
@@ -1551,10 +1530,11 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
   if (nbytes < sizeof(SnapshotHeader)) return fail(MP_E_INVALID, "mp_state_load: %llu bytes is shorter than a snapshot header", (unsigned long long)nbytes);
   SnapshotHeader hd;
   memcpy(&hd, host_src, sizeof(hd));
-  if (memcmp(hd.magic, "MPS4", 4) != 0 || hd.version != 4u) return fail(MP_E_INVALID, "mp_state_load: not a snapshot (or one of an older engine)");
-  if (hd.num_envs != (uint64_t)h->B || hd.payload_bytes != h->state_bytes || hd.n_spans != h->state_spans.size())
+  const SnapshotHeader own = snapshot_header(h);
+  if (memcmp(hd.magic, own.magic, 4) != 0 || hd.version != own.version) return fail(MP_E_INVALID, "mp_state_load: not a snapshot (or one of an older engine)");
+  if (hd.num_envs != own.num_envs || hd.payload_bytes != own.payload_bytes || hd.n_arrays != own.n_arrays)
     return fail(MP_E_INVALID, "mp_state_load: snapshot of %llu envs / %llu bytes does not fit this engine (%d envs / %llu bytes)",
-                (unsigned long long)hd.num_envs, (unsigned long long)hd.payload_bytes, h->B, (unsigned long long)h->state_bytes);
+                (unsigned long long)hd.num_envs, (unsigned long long)hd.payload_bytes, h->B, (unsigned long long)own.payload_bytes);
   if (nbytes != sizeof(SnapshotHeader) + hd.payload_bytes)
     return fail(MP_E_INVALID, "mp_state_load: buffer of %llu bytes, snapshot needs %llu (truncated?)", (unsigned long long)nbytes,
                 (unsigned long long)(sizeof(SnapshotHeader) + hd.payload_bytes));
@@ -1564,9 +1544,11 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   const uint8_t* src = static_cast<const uint8_t*>(host_src) + sizeof(hd);
-  for (const auto& sp : h->state_spans) {
-    CUDA_TRY(cudaMemcpyAsync(sp.first, src, sp.second, cudaMemcpyHostToDevice, st));
-    src += sp.second;
+  for (int r = 0; r < h->record.n_rows; ++r) {
+    const RecordRow& w = h->record.row[r];
+    if (!w.base) continue;
+    CUDA_TRY(cudaMemcpyAsync(w.base, src, (size_t)h->B * w.bytes, cudaMemcpyHostToDevice, st));
+    src += (size_t)h->B * w.bytes;
   }
   int rc = launch_render(h, st);
   if (rc) return rc;
@@ -1574,12 +1556,11 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
   return MP_OK;
 }
 
-// ---- per-env state bank (record layout: record_layout) ------------------------------------------------------------
+// ---- per-env state bank (record layout: layout_state) -------------------------------------------------------------
 int mp_state_record_bytes(mp_handle h, uint64_t* bytes, uint8_t tag[16]) {
   if (!h) return fail(MP_E_INVALID, "null handle");
-  const RecordLayout R = record_layout(h);
-  if (bytes) *bytes = R.record_bytes;
-  if (tag) memcpy(tag, &R.tag, 16);
+  if (bytes) *bytes = h->record.record_bytes;
+  if (tag) memcpy(tag, &h->record.tag, 16);
   return MP_OK;
 }
 
@@ -1601,10 +1582,9 @@ int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* b
   if (!h || !env_of_slot || !bank) return fail(MP_E_INVALID, "mp_state_store: null argument");
   if (n_slots < 1) return fail(MP_E_INVALID, "mp_state_store: n_slots %d < 1", n_slots);
   DeviceGuard guard(h->device);
-  const RecordLayout R = record_layout(h);
-  int rc = check_bank(h, bank, n_slots, env_of_slot, (uint64_t)n_slots, R.record_bytes, "mp_state_store");
+  int rc = check_bank(h, bank, n_slots, env_of_slot, (uint64_t)n_slots, h->record.record_bytes, "mp_state_store");
   if (rc) return rc;
-  k_state_store<<<(n_slots + 7) / 8, 256, 0, (cudaStream_t)stream>>>(R, env_of_slot, n_slots, h->B, static_cast<uint8_t*>(bank));
+  k_state_store<<<(n_slots + 7) / 8, 256, 0, (cudaStream_t)stream>>>(h->record, env_of_slot, n_slots, h->B, static_cast<uint8_t*>(bank));
   ++h->launches;
   CUDA_TRY(cudaGetLastError());
   return MP_OK;
@@ -1617,11 +1597,10 @@ int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, 
   if (h->S.x_world || h->d_g_flag_ptrs)
     return fail(MP_E_UNSUPPORTED, "mp_state_restore: not available once mp_exchange_connect / mp_gather_obs_connect has run");
   DeviceGuard guard(h->device);
-  const RecordLayout R = record_layout(h);
-  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, R.record_bytes, "mp_state_restore");
+  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_state_restore");
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  k_state_restore<<<(h->B + 7) / 8, 256, 0, st>>>(R, slot_of_env, static_cast<const uint8_t*>(bank), n_slots, h->B,
+  k_state_restore<<<(h->B + 7) / 8, 256, 0, st>>>(h->record, slot_of_env, static_cast<const uint8_t*>(bank), n_slots, h->B,
                                                   (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base);
   ++h->launches;
   CUDA_TRY(cudaGetLastError());
@@ -1634,7 +1613,7 @@ int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_
   if (n_slots < 1) return fail(MP_E_INVALID, "mp_step_restore: n_slots %d < 1", n_slots);
   if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_restore: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
   DeviceGuard guard(h->device);
-  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, record_layout(h).record_bytes, "mp_step_restore", out);
+  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_step_restore", out);
   if (rc) return rc;
   const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
                             (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};

@@ -2,9 +2,9 @@
 // mp_state_restore, include/mp_engine.h).
 //
 // A record is one env's row of every state array plus its RNG key and variant bytes, at offsets engine.cu decides
-// (record_layout, next to the state spans of mp_create). The two kernels only gather: every destination (a bank row for
-// a store, an env for a restore) is written by one warp that reads exactly one source, so no two threads ever write the
-// same bytes, whatever indices the caller passes (a fan-out of one record to many envs included). Indices out of range
+// (layout_state, the one list of per-env state arrays, from which snapshots are derived too). The two kernels only
+// gather: every destination (a bank row for a store, an env for a restore) is written by one warp that reads exactly one
+// source, so no two threads ever write the same bytes, whatever indices the caller passes (a fan-out of one record to many envs included). Indices out of range
 // and records whose tag is not this engine's are skipped in-kernel; they can neither fault nor write anything.
 // The same per-warp restore (restore_env) also runs inside a step (k_step<..., kRestore>, step_common.cuh): the warp of a named
 // env copies the record instead of advancing it, and the render that follows draws it with every other env.
