@@ -290,6 +290,51 @@ class SpriteSet:
     return np.stack([self.images[n] for n in self.names])
 
 
+class SharedSprites:
+  """The one sprite table of a draw set (compile_settings_set): every entry's sprites, deduplicated by name and pixels,
+  in first-appearance order. Two entries may register one name with different pixels (coins' avatars take the palette
+  of their draw's coin colours); each pair is a sprite of its own. `view(sprites)` is the table as one entry sees it."""
+
+  def __init__(self, size: int):
+    self.size = size
+    self.names: List[str] = []
+    self._images: List[np.ndarray] = []
+
+  def _find(self, name: str, image: np.ndarray) -> int:
+    for i, (n, img) in enumerate(zip(self.names, self._images)):
+      if n == name and np.array_equal(img, image):
+        return i
+    return -1
+
+  def add(self, sprites: SpriteSet) -> None:
+    for name in sprites.names:
+      if self._find(name, sprites.images[name]) < 0:
+        self.names.append(name)
+        self._images.append(sprites.images[name])
+
+  def view(self, sprites: SpriteSet) -> 'SpriteView':
+    return SpriteView(self, {name: self._find(name, sprites.images[name]) for name in sprites.names})
+
+  def atlas(self) -> np.ndarray:
+    return np.stack(self._images)
+
+
+class SpriteView:
+  """A SharedSprites table indexed by the sprite names of one entry of the set."""
+
+  def __init__(self, shared: SharedSprites, ids: Mapping[str, int]):
+    self.size = shared.size
+    self.names = shared.names
+    self._shared = shared
+    self._ids = ids
+
+  def index(self, name: str) -> int:
+    return self._ids[name]
+
+  def atlas(self) -> np.ndarray:
+    return self._shared.atlas()
+
+
 # ---------------------------------------------------------------------------
 # World model
 # ---------------------------------------------------------------------------
@@ -382,7 +427,8 @@ def _expand_prefab(spec, prefabs, out, x, y, rng, choices=None):
 class WorldModel:
   """Everything the engines need, as python lists prior to packing."""
 
-  def __init__(self, settings: Mapping[str, Any], build_seed: Optional[int] = None):
+  def __init__(self, settings: Mapping[str, Any], build_seed: Optional[int] = None,
+               shared_sprites: Optional[SharedSprites] = None):
     s = _plain(settings)
     sim = s['simulation']
     self.level = s['levelName']
@@ -465,7 +511,8 @@ class WorldModel:
           sp.add_color(f"claimBeamSprite_{int(kw['playerIndex'])}", kw['color'])
         elif c['component'] == 'Paintbrush':  # four explicit facings, noRotate (components.lua:374-385)
           sp.add_shape(f"brush{int(kw['playerIndex'])}", list(kw['shape']), kw['palette'], True)
-    self.sprites = sp
+    self.own_sprites = sp  # this build's sprites alone
+    self.sprites = shared_sprites.view(sp) if shared_sprites is not None else sp
 
     # ---- groups -------------------------------------------------------------
     self.groups: List[str] = []
@@ -1233,7 +1280,35 @@ def compile_settings(settings: Mapping[str, Any],
   """
   if prefab_overrides:
     settings = apply_prefab_overrides(settings, prefab_overrides)
-  model = WorldModel(settings, build_seed)
+  return _compile_model(WorldModel(settings, build_seed), config)
+
+
+def compile_settings_set(settings_list: Sequence[Mapping[str, Any]],
+                         config: Optional[Any] = None,
+                         build_seeds: Optional[Sequence[Optional[int]]] = None) -> List[bytes]:
+  """A draw set: one blob per entry of `settings_list` (e.g. the builds of one substrate under several build seeds), all
+  on one sprite table. That table is the union of every entry's sprites, deduplicated by name and pixels, in
+  first-appearance order (SharedSprites), so the sprite-side sections (atlas, sprite_opaque, sprite_map, the
+  OutOfBounds / OutOfView ids) are byte-identical across the set, and an engine can run the blobs as per-env variants
+  (mp_create_variants). What differs is which sprite ids the states and avatars refer to, and whatever the map decides.
+  A set of one is compile_settings' blob, byte for byte. `build_seeds[i]` resolves entry i's 'choice' prefabs."""
+  settings_list = list(settings_list)
+  if not settings_list:
+    raise ValueError('compile_settings_set needs at least one settings entry')
+  seeds = list(build_seeds) if build_seeds is not None else [None] * len(settings_list)
+  if len(seeds) != len(settings_list):
+    raise ValueError(f'{len(seeds)} build seeds for {len(settings_list)} settings entries')
+  own = [WorldModel(s, seed) for s, seed in zip(settings_list, seeds)]
+  shared = SharedSprites(own[0].sprite_size)
+  for model in own:
+    if model.sprite_size != shared.size:
+      raise ValueError('the entries of a draw set need one sprite size')
+    shared.add(model.own_sprites)
+  return [_compile_model(WorldModel(s, seed, shared), config) for s, seed in zip(settings_list, seeds)]
+
+
+def _compile_model(model: WorldModel, config: Optional[Any]) -> bytes:
+  """The blob of one world model."""
   rewarded = model.avatar_roles & model.rewarded_roles
   if rewarded:
     raise NotImplementedError(f'RoleBasedRewardTile paying roles {sorted(rewarded)} is not supported by the CUDA engine')
@@ -1339,3 +1414,21 @@ def compile_substrate(name: str, roles: Optional[Sequence[str]] = None,
   finally:
     random.setstate(state)
   return compile_settings(settings, config, build_seed, prefab_overrides)
+
+
+def compile_substrate_set(name: str, roles: Optional[Sequence[str]] = None,
+                          build_seeds: Sequence[int] = (0,),
+                          root: Optional[str] = None) -> List[bytes]:
+  """The draws of a named reference substrate under `build_seeds` (what compile_substrate returns for each seed) as a
+  draw set on one sprite table (compile_settings_set). Needs a reference checkout."""
+  config = load_reference_config(name, root)
+  roles = tuple(roles) if roles is not None else tuple(config.default_player_roles)
+  settings_list = []
+  state = random.getstate()
+  try:
+    for seed in build_seeds:
+      random.seed(seed)
+      settings_list.append(config.lab2d_settings_builder(roles=roles, config=config))
+  finally:
+    random.setstate(state)
+  return compile_settings_set(settings_list, config, list(build_seeds))

@@ -138,10 +138,13 @@ struct VariantSet {
   uint8_t* active = nullptr;     // [B] the variant each env's current episode runs
   uint8_t* pending = nullptr;    // [B] the variant each env's next episode runs
   int n = 1;
+  const Tables* maps = nullptr;  // [n] the Tables of each variant's map (a family with map variants), else null
 };
 // The launches take the restore of mp_step_restore, or null for the plain k_step.
 struct FamilyEntry {
   int id;  // MpbFamily
+  bool map_variants;  // Family::kMapVariants: its variants may be draws of different maps (mp_create_variants)
+  const char* const* map_sections;  // then Family::kMapSections: its own entity tables, which such variants may differ in
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
   cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int,
                         const StepRestore*);
@@ -176,7 +179,10 @@ template <class Family>
 int upload_variants_family(std::vector<void*>& allocs, const FamilyParams& base, const std::vector<FamilyParams>& variants, const void** out) {
   using P = typename Family::Params;
   std::vector<P> host(variants.size(), std::get<P>(base));
-  for (size_t v = 0; v < variants.size(); ++v) Family::copy_knobs(host[v], std::get<P>(variants[v]));
+  for (size_t v = 0; v < variants.size(); ++v) {
+    Family::copy_knobs(host[v], std::get<P>(variants[v]));
+    if constexpr (Family::kMapVariants) Family::copy_map(host[v], std::get<P>(variants[v]));
+  }
   const P* d = nullptr;
   int rc = upload(allocs, host, &d);
   *out = d;
@@ -186,13 +192,18 @@ template <class Family>
 cudaError_t launch_variants_family(const cudaLaunchConfig_t& cfg, const Tables& T, const VariantSet& V, const State& S,
                                    const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore) {
   using P = typename Family::Params;
-  const ParamVariants<P> src{static_cast<const P*>(V.params), V.active, V.pending, V.n};
+  const ParamVariants<P> src{static_cast<const P*>(V.params), V.active, V.pending, V.n, V.maps};
   if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true>, T, src, S, actions, mask, mode, *restore);
   return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode, StepRestore{});
 }
 template <class Family>
+constexpr const char* const* map_sections() {
+  if constexpr (Family::kMapVariants) return Family::kMapSections;
+  else return nullptr;
+}
+template <class Family>
 FamilyEntry family_entry(int id) {
-  return {id, load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
+  return {id, Family::kMapVariants, map_sections<Family>(), load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
           same_shape_family<Family>, upload_variants_family<Family>, launch_variants_family<Family>,
           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>),
           {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true>),
@@ -257,6 +268,7 @@ struct mp_engine {
   uint64_t key_base = 0;   // seed + env_index_base: env b's key at creation is key_base + b (State::key)
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
+  int spawn_groups[3] = {-1, -1, -1};  // the respawn group and the two initial spawn groups (or -1) of every variant
   RecordLayout record{};                     // every per-env state array (layout_state): what records and snapshots copy
   RecordLayout* d_record_layout = nullptr;  // device copy of `record`, read by mp_step_restore's k_step
 
@@ -274,7 +286,77 @@ struct mp_engine {
 
 namespace {
 
-int build_tables(mp_engine* E, const void* blob, size_t n) {
+// What a map decides of the Tables (load_map).
+struct MapVariant {
+  const uint16_t* init_grid;  // [L][cells_pad]
+  const uint8_t* solid;       // [cells_pad]
+  const int32_t* spawn_cell;  // [n_spawn]
+  const int32_t* spawn_init_cell[2];
+  int n_spawn, n_spawn_init[2];
+  int avatar_sprite[MP_MAX_PLAYERS];
+};
+void apply_map(Tables& T, const MapVariant& M) {
+  T.init_grid = M.init_grid; T.solid = M.solid; T.spawn_cell = M.spawn_cell; T.n_spawn = M.n_spawn;
+  for (int k = 0; k < 2; ++k) { T.spawn_init_cell[k] = M.spawn_init_cell[k]; T.n_spawn_init[k] = M.n_spawn_init[k]; }
+  memcpy(T.avatar_sprite, M.avatar_sprite, sizeof M.avatar_sprite);
+}
+
+// The map of one blob, which apply_map puts into a Tables: its initial grid padded to cells_pad, the static occupancy of
+// the avatar layer (non-avatar pieces that start there), the cells of the respawn group and of the initial spawn groups,
+// and the avatars' sprites. `T` holds the geometry and the avatar tables of the engine, `groups` the respawn group and
+// the two initial groups (or -1).
+// build_tables takes variant 0's map into the Tables; a map-variant engine keeps every variant's (setup_variants).
+int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], std::vector<void*>& allocs, MapVariant& M) {
+  Section<int32_t> meta, objects, kinds, states, av_table;
+  Section<uint16_t> init_grid;
+  if (!get_section(blob, n, "meta", MPB_I32, &meta) || !get_section(blob, n, "objects", MPB_I32, &objects) ||
+      !get_section(blob, n, "kinds", MPB_I32, &kinds) || !get_section(blob, n, "states", MPB_I32, &states) ||
+      !get_section(blob, n, "av_table", MPB_I32, &av_table) || !get_section(blob, n, "init_grid", MPB_U16, &init_grid))
+    return fail(MP_E_INVALID, "blob: missing map sections");
+  if (init_grid.count < (size_t)T.L * T.cells) return fail(MP_E_INVALID, "blob: 'init_grid' has %zu cells (expected %d)", init_grid.count, T.L * T.cells);
+  char name[64];
+  std::vector<int32_t> cells[3];
+  for (int k = 0; k < 3; ++k) {
+    if (groups[k] < 0) continue;
+    snprintf(name, sizeof name, "spawn_cells_%d", groups[k]);
+    Section<int32_t> sec;
+    if (!get_section(blob, n, name, MPB_I32, &sec)) return fail(MP_E_INVALID, "blob: missing section '%s'", name);
+    cells[k].assign(sec.data, sec.data + sec.count);
+  }
+  M.n_spawn = (int)cells[0].size();
+  for (int k = 0; k < 2; ++k) {
+    M.n_spawn_init[k] = (int)cells[1 + k].size();
+    if (groups[1 + k] < 0) continue;
+    int users = 0;
+    for (int p = 0; p < T.P; ++p) users += T.avatar_init_group[p] == k;
+    if (M.n_spawn_init[k] < users || M.n_spawn_init[k] > 64) return fail(MP_E_UNSUPPORTED, "%d spawn points for %d avatars (need n..64)", M.n_spawn_init[k], users);
+  }
+  if (M.n_spawn < 1) return fail(MP_E_INVALID, "empty respawn group");
+  for (int p = 0; p < T.P; ++p) M.avatar_sprite[p] = av_table.data[p * 8 + 1];
+  std::vector<uint16_t> grid0((size_t)T.L * T.cells_pad, 0);
+  for (int l = 0; l < T.L; ++l) memcpy(&grid0[(size_t)l * T.cells_pad], init_grid.data + (size_t)l * T.cells, T.cells * sizeof(uint16_t));
+  std::vector<uint8_t> solid(T.cells_pad, 0);
+  for (int o = 0; o < meta.data[MPB_META_N_OBJECTS]; ++o) {  // non-avatar pieces that start on the avatar layer
+    const int32_t* od = objects.data + o * MPB_OBJ_COLS;
+    const int32_t* kd = kinds.data + od[MPB_OBJ_KIND] * MPB_KIND_COLS;
+    if (kd[MPB_KIND_IS_AVATAR]) continue;
+    const int32_t* st = states.data + (kd[MPB_KIND_STATE0] + od[MPB_OBJ_STATE]) * MPB_STATE_COLS;
+    if (st[MPB_STATE_LAYER] == T.avatar_layer) solid[od[MPB_OBJ_Y] * T.W + od[MPB_OBJ_X]] = 255;
+  }
+  int rc;
+  if ((rc = upload(allocs, grid0, &M.init_grid)) || (rc = upload(allocs, cells[0], &M.spawn_cell)) || (rc = upload(allocs, solid, &M.solid))) return rc;
+  for (int k = 0; k < 2; ++k) {
+    if (cells[1 + k].empty()) { M.spawn_init_cell[k] = M.spawn_cell; continue; }
+    if ((rc = upload(allocs, cells[1 + k], &M.spawn_init_cell[k]))) return rc;
+  }
+  return MP_OK;
+}
+
+// The engine's tables from blob 0 of `blobs`. The pre-merged sprites cover the cell stacks of every blob: the variants
+// of a map-variant engine share one sprite table and the renderer's pre-merged pairs.
+int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_sizes, int n_blobs) {
+  const void* blob = blobs[0];
+  const size_t n = blob_sizes[0];
   Section<int32_t> meta, states, kinds, comps, objects, hits, action_table, sprite_map, scalar_obs, av_table;
   Section<double> comps_f;
   Section<uint8_t> atlas, sprite_opaque, cell_flags;
@@ -321,32 +403,14 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     if (g < 0) return fail(MP_E_UNSUPPORTED, "more than two initial spawn groups");
     T.avatar_init_group[p] = g;
   }
-  char name[64];
-  auto load_group = [&](int gid, std::vector<int32_t>* out) -> int {
-    snprintf(name, sizeof name, "spawn_cells_%d", gid);
-    Section<int32_t> sec;
-    if (!get_section(blob, n, name, MPB_I32, &sec)) return fail(MP_E_INVALID, "blob: missing section '%s'", name);
-    out->assign(sec.data, sec.data + sec.count);
-    return MP_OK;
-  };
-  std::vector<int32_t> v_spawn, v_init[2];
-  int rc0;
-  if ((rc0 = load_group(respawn_group, &v_spawn))) return rc0;
-  T.n_spawn = (int)v_spawn.size();
-  for (int k = 0; k < 2; ++k) {
-    T.n_spawn_init[k] = 0;
-    if (init_groups[k] < 0) continue;
-    if ((rc0 = load_group(init_groups[k], &v_init[k]))) return rc0;
-    T.n_spawn_init[k] = (int)v_init[k].size();
-    int users = 0;
-    for (int p = 0; p < T.P; ++p) users += T.avatar_init_group[p] == k;
-    if (T.n_spawn_init[k] < users || T.n_spawn_init[k] > 64) return fail(MP_E_UNSUPPORTED, "%d spawn points for %d avatars (need n..64)", T.n_spawn_init[k], users);
-  }
-  if (T.n_spawn < 1) return fail(MP_E_INVALID, "empty respawn group");
+  E->spawn_groups[0] = respawn_group; E->spawn_groups[1] = init_groups[0]; E->spawn_groups[2] = init_groups[1];
+  MapVariant map0{};
+  int rc;
+  if ((rc = load_map(blob, n, T, E->spawn_groups, E->allocs, map0))) return rc;
+  apply_map(T, map0);
 
   // ---- family tables -----------------------------------------------------------------------------
   FamilyLoad ld{blob, n, hits, E->allocs};
-  int rc;
   if ((rc = E->family->load(ld, T, E->params))) return rc;
 #undef NEED
   T.nA = ld.nA; T.nD = ld.nD; T.nW = ld.nW; T.nR = ld.nR; T.nR_pad = ld.nR_pad;
@@ -354,6 +418,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   E->beam_cells = ld.beam_cells;
   {  // 'choice' prefabs left to the engine (drawn per env and episode)
     Section<int32_t> choice_groups, obj_choice, spawn_cond;
+    char name[64];
     if (get_section(blob, n, "choice_groups", MPB_I32, &choice_groups)) {
       if (E->family->id != MPB_FAMILY_TERRITORY) return fail(MP_E_UNSUPPORTED, "per-env 'choice' prefabs are implemented for the territory family only (compile with a build_seed)");
       T.n_choice = (int)choice_groups.count;
@@ -371,26 +436,11 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
   T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16); T.nW_pad = round_up(std::max(T.nW, 1), 16);
 
   // ---- device copies -----------------------------------------------------------------------------
-  std::vector<uint16_t> grid0((size_t)T.L * T.cells_pad, 0);
-  for (int l = 0; l < T.L; ++l) memcpy(&grid0[(size_t)l * T.cells_pad], init_grid.data + (size_t)l * T.cells, T.cells * sizeof(uint16_t));
-  if ((rc = upload(E->allocs, grid0, &T.init_grid))) return rc;
   std::vector<int32_t> act(action_table.data, action_table.data + action_table.count);
   if ((rc = upload(E->allocs, act, &T.action_table))) return rc;
-  if ((rc = upload(E->allocs, v_spawn, &T.spawn_cell))) return rc;
-  for (int k = 0; k < 2; ++k) {
-    if (v_init[k].empty()) { T.spawn_init_cell[k] = T.spawn_cell; continue; }
-    if ((rc = upload(E->allocs, v_init[k], &T.spawn_init_cell[k]))) return rc;
-  }
-  std::vector<uint8_t> solid(T.cells_pad, 0), flags(T.cells_pad, 0);
-  for (int o = 0; o < m[MPB_META_N_OBJECTS]; ++o) {  // non-avatar pieces that start on the avatar layer
-    const int32_t* od = objects.data + o * MPB_OBJ_COLS;
-    const int32_t* kd = kinds.data + od[MPB_OBJ_KIND] * MPB_KIND_COLS;
-    if (kd[MPB_KIND_IS_AVATAR]) continue;
-    const int32_t* st = states.data + (kd[MPB_KIND_STATE0] + od[MPB_OBJ_STATE]) * MPB_STATE_COLS;
-    if (st[MPB_STATE_LAYER] == T.avatar_layer) solid[od[MPB_OBJ_Y] * T.W + od[MPB_OBJ_X]] = 255;
-  }
+  std::vector<uint8_t> flags(T.cells_pad, 0);
   memcpy(flags.data(), cell_flags.data, std::min<size_t>(cell_flags.count, T.cells));
-  if ((rc = upload(E->allocs, solid, &T.solid)) || (rc = upload(E->allocs, flags, &T.cell_flags))) return rc;
+  if ((rc = upload(E->allocs, flags, &T.cell_flags))) return rc;
 
   // ---- render tables ------------------------------------------------------------------------------
   if (atlas.count != (size_t)T.n_sprites * 1024) return fail(MP_E_INVALID, "atlas has %zu bytes, expected %d", atlas.count, T.n_sprites * 1024);
@@ -431,27 +481,40 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
     return id;
   };
   {
+    // Per blob: the sprites each (cell, layer) can show (opts_of) and the initial grid (init_of).
     struct Opt { std::vector<int> sprites; bool absent = false; int orient = -1; bool bad = false; };
-    std::vector<Opt> opts((size_t)T.cells * T.L);
-    std::vector<uint8_t> has_obj((size_t)T.cells * T.L, 0);
-    for (int o = 0; o < m[MPB_META_N_OBJECTS]; ++o) {
-      const int32_t* od = objects.data + o * MPB_OBJ_COLS;
-      const int32_t* kd = kinds.data + od[MPB_OBJ_KIND] * MPB_KIND_COLS;
-      if (kd[MPB_KIND_IS_AVATAR]) continue;
-      const int cell = od[MPB_OBJ_Y] * T.W + od[MPB_OBJ_X];
-      const int ns = kd[MPB_KIND_NSTATES];
-      for (int si = 0; si < ns; ++si) {
-        const int32_t* st = states.data + (kd[MPB_KIND_STATE0] + si) * MPB_STATE_COLS;
-        const int l = st[MPB_STATE_LAYER], sp = st[MPB_STATE_SPRITE];
-        if (l < 0 || sp < 0) continue;
-        Opt& op = opts[(size_t)cell * T.L + l];
-        if (std::find(op.sprites.begin(), op.sprites.end(), sp) == op.sprites.end()) op.sprites.push_back(sp);
-        if (op.orient >= 0 && op.orient != od[MPB_OBJ_ORIENT]) op.bad = true;
-        op.orient = od[MPB_OBJ_ORIENT];
-        // the piece may also be somewhere else (another layer / off grid / sprite-less state)
-        for (int sj = 0; sj < ns; ++sj) {
-          const int32_t* s2 = states.data + (kd[MPB_KIND_STATE0] + sj) * MPB_STATE_COLS;
-          if (s2[MPB_STATE_LAYER] != l || s2[MPB_STATE_SPRITE] < 0) op.absent = true;
+    // (the variants of other families have one map: rule (a) of mp_create_variants)
+    const int n_maps = E->family->map_variants ? n_blobs : 1;
+    std::vector<std::vector<Opt>> opts_of(n_maps, std::vector<Opt>((size_t)T.cells * T.L));
+    std::vector<const uint16_t*> init_of(n_maps);
+    for (int v = 0; v < n_maps; ++v) {
+      Section<int32_t> v_meta, v_states, v_kinds, v_objects;
+      Section<uint16_t> v_init;
+      if (!get_section(blobs[v], blob_sizes[v], "meta", MPB_I32, &v_meta) || !get_section(blobs[v], blob_sizes[v], "states", MPB_I32, &v_states) ||
+          !get_section(blobs[v], blob_sizes[v], "kinds", MPB_I32, &v_kinds) || !get_section(blobs[v], blob_sizes[v], "objects", MPB_I32, &v_objects) ||
+          !get_section(blobs[v], blob_sizes[v], "init_grid", MPB_U16, &v_init) || v_init.count < (size_t)T.L * T.cells)
+        return fail(MP_E_INVALID, "blob %d: missing map sections", v);
+      init_of[v] = v_init.data;
+      std::vector<Opt>& opts = opts_of[v];
+      for (int o = 0; o < v_meta.data[MPB_META_N_OBJECTS]; ++o) {
+        const int32_t* od = v_objects.data + o * MPB_OBJ_COLS;
+        const int32_t* kd = v_kinds.data + od[MPB_OBJ_KIND] * MPB_KIND_COLS;
+        if (kd[MPB_KIND_IS_AVATAR]) continue;
+        const int cell = od[MPB_OBJ_Y] * T.W + od[MPB_OBJ_X];
+        const int ns = kd[MPB_KIND_NSTATES];
+        for (int si = 0; si < ns; ++si) {
+          const int32_t* st = v_states.data + (kd[MPB_KIND_STATE0] + si) * MPB_STATE_COLS;
+          const int l = st[MPB_STATE_LAYER], sp = st[MPB_STATE_SPRITE];
+          if (l < 0 || sp < 0) continue;
+          Opt& op = opts[(size_t)cell * T.L + l];
+          if (std::find(op.sprites.begin(), op.sprites.end(), sp) == op.sprites.end()) op.sprites.push_back(sp);
+          if (op.orient >= 0 && op.orient != od[MPB_OBJ_ORIENT]) op.bad = true;
+          op.orient = od[MPB_OBJ_ORIENT];
+          // the piece may also be somewhere else (another layer / off grid / sprite-less state)
+          for (int sj = 0; sj < ns; ++sj) {
+            const int32_t* s2 = v_states.data + (kd[MPB_KIND_STATE0] + sj) * MPB_STATE_COLS;
+            if (s2[MPB_STATE_LAYER] != l || s2[MPB_STATE_SPRITE] < 0) op.absent = true;
+          }
         }
       }
     }
@@ -461,8 +524,11 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
       for (size_t q = 1; q < hs.size() && cur; ++q) { if (remapped[hs[q]] || remapped[cur]) break; cur = merged_id(cur, hs[q]); }
     }
     std::vector<int> stack_s, stack_o;
-    for (int pass = 0; pass < 2; ++pass)  // pass 0: the map as it is at reset (most common stacks) gets the budget first
+    for (int pass = 0; pass < 2; ++pass)  // pass 0: the maps as they are at reset (most common stacks) get the budget first
+    for (int v = 0; v < n_maps; ++v)        // (a map-variant engine: the stacks of every variant's map)
     for (int cell = 0; cell < T.cells; ++cell) {
+      const std::vector<Opt>& opts = opts_of[v];
+      const uint16_t* init_grid = init_of[v];
       // enumerate the cartesian product of per-layer options, bottom up (bounded)
       size_t combos = 1;
       bool bad = false;
@@ -480,7 +546,7 @@ int build_tables(mp_engine* E, const void* blob, size_t n) {
         for (int l = 0; l < T.L; ++l) {
           const Opt& op = opts[(size_t)cell * T.L + l];
           const int i = idx[l];
-          const int init_v = init_grid.data[(size_t)l * T.cells + cell];
+          const int init_v = init_grid[(size_t)l * T.cells + cell];
           const int init_sprite = init_v ? (init_v - 1) >> 2 : -1;
           if (i < (int)op.sprites.size()) { stack_s.push_back(op.sprites[i]); stack_o.push_back(op.orient); is_initial &= op.sprites[i] == init_sprite; }
           else is_initial &= init_sprite < 0;
@@ -843,8 +909,14 @@ extern "C" {
 const char* mp_last_error(void) { return g_error.c_str(); }
 const char* mp_version(void) { return "meltingpot_b200 engine 0.1 (sm_90a)"; }
 
-int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
-  if (!blob || !out || num_envs < 1) return fail(MP_E_INVALID, "mp_create: bad arguments");
+}  // extern "C"
+
+namespace {
+int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host);
+
+// mp_create (one blob) and mp_create_variants (a checked variant set of n_blobs > 1, env b starting on env_variant[b]).
+int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, const uint8_t* env_variant, int num_envs, int device,
+           uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);
   if (e != cudaSuccess || n_dev == 0) return fail(MP_E_NO_DEVICE, "no CUDA device available (%s); this engine has no CPU path", cudaGetErrorString(e));
@@ -855,10 +927,17 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   DeviceGuard guard(device);
   mp_engine* E = new mp_engine();
   E->device = device; E->B = num_envs; E->flags = flags; E->sm_count = prop.multiProcessorCount;
-  E->blob_hash = fnv1a(blob, blob_bytes);
-  int rc = build_tables(E, blob, blob_bytes);
+  E->blob_hash = fnv1a(blobs[0], blob_sizes[0]);
+  int rc = build_tables(E, blobs, blob_sizes, n_blobs);
+  // before the state is sized: the variants of a map-variant engine size its entity arrays for the largest of them
+  if (rc == MP_OK && n_blobs > 1) rc = setup_variants(E, blobs, blob_sizes, n_blobs, env_variant);
   if (rc == MP_OK) rc = build_plan(E);
-  if (rc != MP_OK) { mp_destroy(E); return rc; }
+  if (rc != MP_OK) {
+    const std::string msg = g_error;
+    mp_destroy(E);
+    g_error = msg;
+    return rc;
+  }
   const Tables& T = E->T;
   State& S = E->S;
   S.B = num_envs; E->key_base = seed + env_index_base;
@@ -951,20 +1030,41 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
   return MP_OK;
 }
 
-namespace {
 // Rule (a) of mp_create_variants: variant `v` has the same sections as variant 0, byte for byte, except the family's
-// parameter blocks, the component tables and the metadata string.
-int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
+// parameter blocks, the component tables and the metadata string. The variants of a family with map variants (draws of
+// one builder compiled as a draw set; `map_sections` lists the family's entity tables, null for other families) may
+// also differ in their map: the initial grid, the object table, the spawn points and those entity tables, and in three
+// columns: the object count of 'meta', the sprite of each state and the sprite of each avatar. The sprite table itself
+// (atlas, sprite_opaque, sprite_map) stays identical.
+int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const char* const* map_sections) {
+  const bool maps = map_sections != nullptr;
   const MpbHeader* h0 = static_cast<const MpbHeader*>(b0);
   const MpbHeader* hv = static_cast<const MpbHeader*>(bv);
   if (n0 < sizeof(MpbHeader) || nv < sizeof(MpbHeader) || memcmp(hv->magic, MPB_MAGIC, 4) != 0 || hv->version != MPB_VERSION ||
       nv < sizeof(MpbHeader) + (size_t)hv->n_sections * sizeof(MpbSection))
     return fail(MP_E_INVALID, "blob: not an MPB%u blob", MPB_VERSION);
-  auto free_to_differ = [](const char* name) {
+  auto free_to_differ = [maps, map_sections](const char* name) {
     const size_t len = strnlen(name, MPB_NAME_LEN);
-    return (len == 5 && name[2] == '_' && (name[3] == 'i' || name[3] == 'd') && name[4] == 'p') || !strcmp(name, "comps") ||
-           !strcmp(name, "comps_f") || !strcmp(name, "info_json");
+    if ((len == 5 && name[2] == '_' && (name[3] == 'i' || name[3] == 'd') && name[4] == 'p') || !strcmp(name, "comps") ||
+        !strcmp(name, "comps_f") || !strcmp(name, "info_json"))
+      return true;
+    if (!maps) return false;
+    if (!strcmp(name, "init_grid") || !strcmp(name, "objects") || !strncmp(name, "spawn_cells_", 12)) return true;
+    for (const char* const* t = map_sections; *t; ++t) if (!strcmp(name, *t)) return true;
+    return false;
   };
+  // map variants: the one column of an int32 section that may differ (of `cols`), or -1
+  auto free_column = [maps](const char* name, int* cols) {
+    if (!maps) return -1;
+    if (!strcmp(name, "meta")) { *cols = MPB_META_COUNT; return (int)MPB_META_N_OBJECTS; }
+    if (!strcmp(name, "states")) { *cols = MPB_STATE_COLS; return (int)MPB_STATE_SPRITE; }
+    if (!strcmp(name, "av_table")) { *cols = 8; return 1; }
+    return -1;
+  };
+  static const char* const kMetaNames[] = {"family", "W", "H", "layers", "players", "sprite size", "topology", "max frames", "objects",
+                                           "kinds", "states", "comps", "sprites", "hits", "groups", "view left", "view right",
+                                           "view forward", "view backward", "actions", "action fields", "OutOfBounds sprite",
+                                           "OutOfView sprite", "scalar observations"};
   const MpbSection* s0 = reinterpret_cast<const MpbSection*>(h0 + 1);
   const MpbSection* sv = reinterpret_cast<const MpbSection*>(hv + 1);
   auto check = [&](const MpbSection* s, uint32_t count, const void* other, size_t n_other, const void* own) -> int {
@@ -973,9 +1073,24 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
       memcpy(name, s[i].name, MPB_NAME_LEN);
       if (free_to_differ(name)) continue;
       const MpbSection* t = mpb_find(other, n_other, name);
-      if (!t || t->dtype != s[i].dtype || t->ndim != s[i].ndim || memcmp(t->shape, s[i].shape, sizeof t->shape) != 0 ||
-          t->nbytes != s[i].nbytes || memcmp(mpb_data(other, t), mpb_data(own, &s[i]), s[i].nbytes) != 0)
-        return fail(MP_E_UNSUPPORTED, "section '%s' differs (variants may differ only in the family's parameters)", name);
+      const bool same_shape = t && t->dtype == s[i].dtype && t->ndim == s[i].ndim && memcmp(t->shape, s[i].shape, sizeof t->shape) == 0 &&
+                              t->nbytes == s[i].nbytes;
+      int cols = 0;
+      const int col = free_column(name, &cols);
+      if (same_shape && col >= 0 && s[i].dtype == MPB_I32) {
+        const int32_t* x = static_cast<const int32_t*>(mpb_data(own, &s[i]));
+        const int32_t* y = static_cast<const int32_t*>(mpb_data(other, t));
+        for (size_t k = 0; k < s[i].nbytes / 4; ++k) {
+          if ((int)(k % cols) == col || x[k] == y[k]) continue;
+          if (!strcmp(name, "meta") && k < sizeof kMetaNames / sizeof *kMetaNames)
+            return fail(MP_E_UNSUPPORTED, "section 'meta' differs in field '%s' (%d vs %d)", kMetaNames[k], x[k], y[k]);
+          return fail(MP_E_UNSUPPORTED, "section '%s' differs in value %zu (column %zu)", name, k, k % cols);
+        }
+        continue;
+      }
+      if (!same_shape || memcmp(mpb_data(other, t), mpb_data(own, &s[i]), s[i].nbytes) != 0)
+        return fail(MP_E_UNSUPPORTED, maps ? "section '%s' differs (map variants may differ only in the family's parameters and their map)"
+                                           : "section '%s' differs (variants may differ only in the family's parameters)", name);
     }
     return MP_OK;
   };
@@ -983,31 +1098,47 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv) {
   return rc ? rc : check(sv, hv->n_sections, b0, n0, bv);
 }
 
-// Rules (b)-(d) of mp_create_variants for an engine built from variant 0, then the variant set's device arrays.
+// Rules (b)-(d) of mp_create_variants for an engine whose tables are built from variant 0 (build_tables), then the
+// variant set's device arrays. Runs before the engine's state is sized: a family with map variants keeps each variant's
+// map (MapVariant) and entity tables, and the State's entity arrays (T.nA_pad) are sized for the variant with the most.
 int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host) {
   struct Decided { int nA, nD, nW, nR, nR_pad, end_min_frames, end_interval, beam_cells; double end_prob; std::vector<std::vector<int>> hints; };
   std::vector<FamilyParams> params(n);
   std::vector<Decided> decided;
-  std::vector<void*> scratch;  // the loaders' device uploads: every variant uses the engine's own (same sections)
+  const bool maps = E->family->map_variants;
+  // the loaders' device uploads: every variant of a plain set uses the engine's own (same sections); map variants keep theirs
+  std::vector<void*> scratch;
+  std::vector<MapVariant> map(maps ? n : 0);
+  Tables& T = E->T;
   int rc = MP_OK;
   for (int v = 0; v < n && rc == MP_OK; ++v) {
     Section<int32_t> hits;
     if (!get_section(blobs[v], blob_bytes[v], "hits", MPB_I32, &hits)) { rc = fail(MP_E_INVALID, "blob: missing section 'hits'"); break; }
-    FamilyLoad ld{blobs[v], blob_bytes[v], hits, scratch};
-    if ((rc = E->family->load(ld, E->T, params[v]))) break;
+    FamilyLoad ld{blobs[v], blob_bytes[v], hits, maps ? E->allocs : scratch};
+    if ((rc = E->family->load(ld, T, params[v]))) break;
     decided.push_back({ld.nA, ld.nD, ld.nW, ld.nR, ld.nR_pad, ld.end_min_frames, ld.end_interval, ld.beam_cells, ld.end_prob, ld.hint_stacks});
     const Decided& a = decided[0];
     const Decided& b = decided[v];
-    if (a.nA != b.nA || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
+    if ((!maps && a.nA != b.nA) || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
     else if (a.end_min_frames != b.end_min_frames || a.end_interval != b.end_interval || memcmp(&a.end_prob, &b.end_prob, sizeof a.end_prob) != 0)
       rc = fail(MP_E_UNSUPPORTED, "episode ending differs");
     else if (a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
     else if (a.hints != b.hints) rc = fail(MP_E_UNSUPPORTED, "pre-merged sprite hints differ");
     else rc = E->family->same_shape(params[0], params[v]);
+    if (rc == MP_OK && maps) rc = load_map(blobs[v], blob_bytes[v], T, E->spawn_groups, E->allocs, map[v]);
     if (rc) g_error = "variant " + std::to_string(v) + ": " + g_error;
   }
   for (void* p : scratch) cudaFree(p);
   if (rc) return rc;
+  if (maps) {
+    for (const Decided& dv : decided) T.nA = std::max(T.nA, dv.nA);
+    T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16);
+    std::vector<Tables> tv(n, T);  // T is final here: create changes nothing in it after this
+    for (int v = 0; v < n; ++v) { apply_map(tv[v], map[v]); tv[v].nA = decided[v].nA; }
+    const Tables* d = nullptr;
+    if ((rc = upload(E->allocs, tv, &d))) return rc;
+    E->variants.maps = d;
+  }
   if ((rc = E->family->upload_variants(E->allocs, E->params, params, &E->variants.params))) return rc;
   const size_t B = E->B;
   std::vector<uint8_t> assign(B, 0);
@@ -1022,9 +1153,16 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
   uint64_t h = fnv1a(&n, sizeof n);
   for (int v = 0; v < n; ++v) { const uint64_t hv = fnv1a(blobs[v], blob_bytes[v]); h = fnv1a(&hv, sizeof hv, h); }
   E->blob_hash = h;
-  return layout_state(E, /*allocate=*/false);
+  return MP_OK;
 }
 }  // namespace
+
+extern "C" {
+
+int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
+  if (!blob || !out || num_envs < 1) return fail(MP_E_INVALID, "mp_create: bad arguments");
+  return create(&blob, &blob_bytes, 1, nullptr, num_envs, device, seed, env_index_base, flags, out);
+}
 
 int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n_variants, const uint8_t* env_variant_host, int num_envs,
                        int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
@@ -1035,25 +1173,18 @@ int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n
   if (env_variant_host)
     for (int b = 0; b < num_envs; ++b)
       if (env_variant_host[b] >= n_variants) return fail(MP_E_INVALID, "mp_create_variants: env %d assigned variant %d of %d", b, env_variant_host[b], n_variants);
+  // whether the family (of variant 0) takes map variants decides which sections may differ
+  const char* const* map_sections = nullptr;
+  if (const MpbSection* m = mpb_find(blobs[0], blob_bytes[0], "meta"))
+    if (m->dtype == MPB_I32 && m->nbytes >= 4)
+      for (const FamilyEntry& f : kFamilies)
+        if (f.id == static_cast<const int32_t*>(mpb_data(blobs[0], m))[MPB_META_FAMILY]) map_sections = f.map_sections;
   for (int v = 1; v < n_variants; ++v)
-    if (int rc = same_sections(blobs[0], blob_bytes[0], blobs[v], blob_bytes[v])) {
+    if (int rc = same_sections(blobs[0], blob_bytes[0], blobs[v], blob_bytes[v], map_sections)) {
       g_error = "variant " + std::to_string(v) + ": " + g_error;
       return rc;
     }
-  mp_handle E = nullptr;
-  int rc = mp_create(blobs[0], blob_bytes[0], num_envs, device, seed, env_index_base, flags, &E);
-  if (rc) return rc;
-  if (n_variants > 1) {
-    DeviceGuard guard(device);
-    if ((rc = setup_variants(E, blobs, blob_bytes, n_variants, env_variant_host))) {
-      const std::string msg = g_error;
-      mp_destroy(E);
-      g_error = msg;
-      return rc;
-    }
-  }
-  *out = E;
-  return MP_OK;
+  return create(blobs, blob_bytes, n_variants, env_variant_host, num_envs, device, seed, env_index_base, flags, out);
 }
 
 int mp_set_env_variants(mp_handle h, const uint8_t* env_variant, void* stream) {

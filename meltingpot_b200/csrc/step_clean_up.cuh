@@ -85,6 +85,7 @@ struct CleanUp {
   }
 
   using Scratch = WarpScratch;
+  static constexpr bool kMapVariants = false;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables& T) { return scratch_round16((size_t)T.cells_pad * 6) + (size_t)T.n_actions * 16 + 2 * sizeof(BeamGeom); }

@@ -47,17 +47,26 @@ struct Coins {
     return MP_OK;
   }
 
-  // Host: per-env variants may differ in the coin rewards, the regrowth rate and the termination rule.
+  // Host: per-env variants may differ in the coin rewards, the regrowth rate and the termination rule, and, as draws of
+  // the builder (map variants), in the coins, their cells and the coin sprites (the draw's colours).
   static int same_shape(const Params& a, const Params& b) {
-    MP_SAME(coin_layer) MP_SAME(coin_sprite) MP_SAME(coin_type)
+    MP_SAME(coin_layer) MP_SAME(coin_type)
     return MP_OK;
   }
   static void copy_knobs(Params& dst, const Params& src) {
     memcpy(dst.coin_reward, src.coin_reward, sizeof dst.coin_reward);
     dst.coin_rate = src.coin_rate; dst.terminate = src.terminate; dst.terminate_n = src.terminate_n;
   }
+  static void copy_map(Params& dst, const Params& src) {
+    memcpy(dst.coin_sprite, src.coin_sprite, sizeof dst.coin_sprite);
+    dst.coin = src.coin; dst.coin_of_cell = src.coin_of_cell;
+  }
 
   using Scratch = WarpScratch;
+  // Draws of the builder may differ in their map (mp_create_variants): the coin table is their entity table, and the coin
+  // count is the nA of each variant's Tables (setup_variants).
+  static constexpr bool kMapVariants = true;
+  static constexpr const char* kMapSections[] = {"co_coin", nullptr};
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
@@ -69,7 +78,9 @@ struct Coins {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, true);
     __syncwarp();
     copy_init_grid(T, grid, lane);
-    for (int k = lane; k < T.nA; k += 32) S.apple[(size_t)b * T.nA_pad + k] = 0;
+    // the whole padded row, so that an env that moved from a draw with more coins keeps no bytes of it (records and
+    // snapshots of equal envs stay equal byte for byte)
+    for (int k = lane; k < T.nA_pad / 16; k += 32) reinterpret_cast<uint4*>(S.apple + (size_t)b * T.nA_pad)[k] = make_uint4(0, 0, 0, 0);
     __syncwarp();
     const auto all = [](int) { return true; };
     spawn_group(T, S, b, lane, grid, sc.tmp, T.spawn_init_cell[0], T.n_spawn_init[0], all, all, episode, k0, k1, [&](int) {

@@ -59,26 +59,34 @@ __host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * 
 // Per-env parameter variants (mp_create_variants): env b runs under params[active[b]]. An episode start first takes the
 // env's pending assignment (active[b] = pending[b]), so a reassignment never changes an episode that is under way.
 // Every variant stages the same per-CTA tables (the compatibility check of mp_create_variants), so stage() reads params[0].
+// A family with kMapVariants (coins) also advances under maps[active[b]]: the engine's Tables with that variant's initial
+// grid, static occupancy, spawn points, avatar sprites and entity count (the State's entity arrays are sized for the
+// largest variant). The map is only ever read through the env's active variant, which changes at an episode start, so
+// an env's map changes there too and never mid-episode. The Tables are read from the device array through the L1: a
+// local copy of the kernel's Tables with the variant's fields swapped in would sit on the stack (392 bytes for coins,
+// since avatar_sprite is indexed by lane).
 template <class Params>
 struct ParamVariants {
   const Params* __restrict__ params;  // [n]
   uint8_t* active;                    // [B]
   const uint8_t* pending;             // [B]
   int n;
+  const Tables* __restrict__ maps;    // [n] (families with kMapVariants), else null
 };
 
 // The variant env b advances under: on an episode start its pending assignment, which lane 0 makes the active one; an
 // index outside the set reads as variant 0.
 template <class Params>
-__device__ __forceinline__ const Params& env_params(const ParamVariants<Params>& V, int b, int lane, bool reset) {
+__device__ __forceinline__ int env_variant(const ParamVariants<Params>& V, int b, int lane, bool reset) {
   int k = reset ? V.pending[b] : V.active[b];
   if (k >= V.n) k = 0;
   if (reset && lane == 0) V.active[b] = (uint8_t)k;
-  return V.params[k];
+  return k;
 }
 
 // A Family provides: Params (what only its kernel reads), the host-side load(FamilyLoad&, T, Params&) that decodes its
-// blob sections (family_load.h), Scratch, kStagesTables, scratch_bytes(T) per warp, table_bytes(T) per CTA,
+// blob sections (family_load.h), Scratch, kStagesTables, kMapVariants (whether its variants may differ in the map, and
+// then copy_map(dst, src) on the host, which copies a variant's map-dependent Params), scratch_bytes(T) per warp, table_bytes(T) per CTA,
 // stage(T, F, tables) (copies static tables into shared memory), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
 // and step(T, F, S, b, lane, actions, sc), and on the host same_shape(a, b) and copy_knobs(dst, src) for per-env
 // variants. `Source` is the family's Params (one blob) or ParamVariants<Params>. A single Params is a grid constant:
@@ -116,9 +124,16 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
     event_begin(lane);
     if constexpr (kVariants) {
       const bool reset = mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE];
-      const typename Family::Params& F = env_params(src, b, lane, reset);
-      if (reset) Family::reset(T, F, S, b, lane, sc);
-      else Family::step(T, F, S, b, lane, actions, sc);
+      const int k = env_variant(src, b, lane, reset);
+      const typename Family::Params& F = src.params[k];
+      if constexpr (Family::kMapVariants) {
+        const Tables& Tm = src.maps[k];
+        if (reset) Family::reset(Tm, F, S, b, lane, sc);
+        else Family::step(Tm, F, S, b, lane, actions, sc);
+      } else {
+        if (reset) Family::reset(T, F, S, b, lane, sc);
+        else Family::step(T, F, S, b, lane, actions, sc);
+      }
     } else {
       if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, src, S, b, lane, sc);
       else Family::step(T, src, S, b, lane, actions, sc);

@@ -189,6 +189,7 @@ struct Territory {
   }
 
   using Scratch = TerritoryScratch;
+  static constexpr bool kMapVariants = false;
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return territory_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables& T) { return territory_table_bytes(T); }

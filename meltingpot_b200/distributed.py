@@ -94,9 +94,10 @@ class ShardedSubstrate:
   """One rank's shard of a globally indexed batch of env instances."""
 
   def __init__(self, name: str, roles, global_num_envs: int, seed: int, device: Optional[int] = None,
-               world_rgb: bool = True, group=None, prefab_overrides=None, env_variant=None):
-    """prefab_overrides / env_variant: as substrate.build_batched, with env_variant indexed by GLOBAL env; each rank
-    takes the slice of its own envs."""
+               world_rgb: bool = True, group=None, prefab_overrides=None, env_variant=None, build_seeds=None):
+    """prefab_overrides / build_seeds / env_variant: as substrate.build_batched, with env_variant indexed by GLOBAL env;
+    each rank takes the slice of its own envs (with build_seeds and no env_variant, global env g plays draw
+    g % len(build_seeds))."""
     import torch.distributed as dist  # pylint: disable=g-import-not-at-top
     from meltingpot_b200 import substrate  # pylint: disable=g-import-not-at-top
     self._group = group
@@ -113,7 +114,8 @@ class ShardedSubstrate:
       local_variant = list(env_variant[self.env_index_base:self.env_index_base + self.local_num_envs])
     self.local = substrate.build_batched(name, roles=roles, num_envs=self.local_num_envs, device=device, seed=seed,
                                          env_index_base=self.env_index_base, world_rgb=world_rgb,
-                                         prefab_overrides=prefab_overrides, env_variant=local_variant)
+                                         prefab_overrides=prefab_overrides, env_variant=local_variant,
+                                         build_seeds=build_seeds)
 
   def reset(self, out=None):
     """out: a BatchedTimeStep of this rank's envs to fill (BatchedSubstrate.step)."""

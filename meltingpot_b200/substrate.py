@@ -605,9 +605,18 @@ class SubstrateFactory:
 
   def build_batched(self, roles: Sequence[str], num_envs: int, seed: Optional[int] = None,
                     env_index_base: int = 0, world_rgb: bool = True, prefab_overrides=None,
-                    env_variant=None) -> BatchedSubstrate:
+                    env_variant=None, build_seeds=None) -> BatchedSubstrate:
     _validate_roles(self._config, roles)
-    if prefab_overrides is None:
+    if build_seeds is not None:  # one draw of the config builder per seed
+      if prefab_overrides is not None:
+        raise ValueError('pass build_seeds or prefab_overrides, not both')
+      build_seeds = [int(s) for s in build_seeds]
+      if not build_seeds:
+        raise ValueError('build_seeds is empty')
+      blob = substrate_blobs.compile_draws(self._name, tuple(roles), build_seeds)
+      if env_variant is None:
+        env_variant = draw_of_env(env_index_base, num_envs, len(build_seeds))
+    elif prefab_overrides is None:
       if env_variant is not None:
         raise ValueError('env_variant needs a sequence of prefab_overrides')
       blob = substrate_blobs.load_blob(self._name, tuple(roles))
@@ -639,14 +648,24 @@ def build_from_config(config: config_dict.ConfigDict, *, roles: Sequence[str],
   return get_factory_from_config(config, device).build(roles, env_seed=env_seed)
 
 
+def draw_of_env(env_index_base: int, num_envs: int, num_draws: int) -> np.ndarray:
+  """The default draw of each env of a build_seeds batch: global env g plays draw g % num_draws."""
+  return (np.arange(env_index_base, env_index_base + num_envs) % num_draws).astype(np.int64)
+
+
 def build_batched(name: str, *, roles: Sequence[str], num_envs: int, device: int = 0,
                   seed: Optional[int] = None, env_index_base: int = 0,
-                  world_rgb: bool = True, prefab_overrides=None, env_variant=None) -> BatchedSubstrate:
+                  world_rgb: bool = True, prefab_overrides=None, env_variant=None, build_seeds=None) -> BatchedSubstrate:
   """Builds `num_envs` instances on one GPU; see `BatchedSubstrate`.
 
   `prefab_overrides` (the reference builder's, builder.py:70-87) is one mapping for every env, or a sequence of
   mappings: a heterogeneous batch whose env b runs variant env_variant[b] (default 0). Compiling overrides needs a
-  reference checkout."""
+  reference checkout.
+
+  `build_seeds` (coins): one draw of the substrate's config builder per seed, as separate reference builds would
+  make (coins draws its map size and its two coin colours on every build), compiled as one draw set. Env b plays
+  draw env_variant[b], by default (env_index_base + b) % len(build_seeds); a draw is a variant, so set_env_variant
+  moves an env to another draw at its next episode. Needs a reference checkout; not combined with prefab_overrides."""
   return get_factory(name, device).build_batched(roles, num_envs, seed=seed, env_index_base=env_index_base,
                                                  world_rgb=world_rgb, prefab_overrides=prefab_overrides,
-                                                 env_variant=env_variant)
+                                                 env_variant=env_variant, build_seeds=build_seeds)

@@ -63,6 +63,17 @@ def compile_with_overrides(name: str, roles: Sequence[str], prefab_overrides) ->
   return compiler.compile_substrate(name, roles, build_seed=BUILD_SEEDS.get(name), prefab_overrides=prefab_overrides)
 
 
+def compile_draws(name: str, roles: Sequence[str], build_seeds: Sequence[int]) -> list:
+  """The draws of `name` with `roles` under `build_seeds`, one blob per seed on one sprite table
+  (compiler.compile_substrate_set; compiled from a reference checkout)."""
+  from meltingpot_b200 import compiler  # pylint: disable=g-import-not-at-top
+  if compiler.reference_root() is None:
+    raise FileNotFoundError(
+        f'build_seeds for {name!r} need a Melting Pot reference checkout to compile from '
+        '(set MELTINGPOT_REFERENCE_ROOT)')
+  return compiler.compile_substrate_set(name, roles, list(build_seeds))
+
+
 def _is_default_role(name: str, role: str) -> bool:
   del name
   return role == 'default'
