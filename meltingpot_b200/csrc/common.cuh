@@ -88,6 +88,20 @@ struct ScalarTargets {
   int on;  // any of the four is set
 };
 
+// Caller-owned per-player rows of one step (mp_player_outputs, mp_step_players): player p of env b goes to row
+// row_of_player[b][p] when that is in [0, n_rows). Strides in bytes; scalar_obs row (k, r) starts at
+// scalar_obs + k * scalar_obs_stride + r * scalar_obs_row_stride. Read only by k_render<..., RENDER_ROUTED> and
+// k_exchange_push.
+struct PlayerTargets {
+  const int32_t* row_of_player;  // [B][P]
+  int n_rows;
+  int scalars_on;  // reward or scalar_obs is set
+  uint8_t* rgb;
+  double* reward;
+  double* scalar_obs;
+  uint64_t rgb_row_stride, reward_row_stride, scalar_obs_row_stride, scalar_obs_stride;
+};
+
 struct State {
   int B;
   uint64_t* key;  // [B] Philox key of each env: seed + env_index_base + b at mp_create; state, so a restored env keeps its source's
@@ -135,6 +149,7 @@ struct State {
   // a caller's tensors. (Kept behind every field the state-transition kernels read.)
   uint64_t rgb_env_stride, world_env_stride;
   ScalarTargets out;                       // the step's scalar rows into caller-owned memory (mp_step_into), or none
+  PlayerTargets pr;                        // the step's per-player rows (mp_step_players), or all zero
 };
 
 // Events of the current step (the reference's events:add calls on the hot path). Types follow
@@ -266,11 +281,35 @@ __device__ __forceinline__ void deliver_scalars(const Tables& T, const State& S)
   }
 }
 
+// Delivery of the routed players' reward and scalar observations into their rows (State::pr), like deliver_scalars:
+// one warp per env, lane i covering (output k = i / P, player p = i % P); output 0 is the reward, output 1 + j
+// scalar observation j. A player without a row gets nothing; nothing outside [0, n_rows) is written.
+__device__ __forceinline__ void deliver_player_scalars(const Tables& T, const State& S) {
+  const PlayerTargets& o = S.pr;
+  if (!o.scalars_on) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = (int)blockDim.x >> 5;
+  const int P = T.P, n = P * (1 + (o.scalar_obs ? T.n_scalar : 0));
+  for (int b = (int)blockIdx.x + warp * (int)gridDim.x; b < S.B; b += n_warps * (int)gridDim.x) {
+    for (int i = lane; i < n; i += 32) {
+      const int k = i / P, p = i - k * P;
+      const int row = o.row_of_player[(size_t)b * P + p];
+      if ((uint32_t)row >= (uint32_t)o.n_rows) continue;
+      if (k == 0) {
+        if (o.reward) *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.reward) + (size_t)row * o.reward_row_stride) = S.reward[(size_t)b * P + p];
+      } else {
+        *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.scalar_obs) + (size_t)(k - 1) * o.scalar_obs_stride + (size_t)row * o.scalar_obs_row_stride) =
+            S.scalar_obs[((size_t)(k - 1) * S.B + b) * P + p];
+      }
+    }
+  }
+}
+
 // Delivery when no render follows the state transition (mp_step_state on its own, or rendering switched off).
 __global__ void __launch_bounds__(256) k_exchange_push(Tables T, State S) {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   exchange_push(T, S);
   deliver_scalars(T, S);
+  deliver_player_scalars(T, S);
 }
 
 // The consumer side, enqueued by EVERY rank after its step (mp_exchange_wait; stream-ordered after the kernel that

@@ -253,6 +253,7 @@ struct mp_engine {
   size_t step_smem = 0;  // dynamic shared memory of one state-transition launch
   void (*render_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
   void (*render_gather_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
+  void (*render_routed_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;  // mp_step_players / mp_reset_players
   // mp_gather_obs_*: this rank's stacked-observation block [flags 256 B][2 slots][rgb of all ranks | world_rgb of all ranks]
   uint8_t* g_block = nullptr;
   uint64_t g_block_bytes = 0, g_slot_bytes = 0, g_world_off = 0;
@@ -771,18 +772,27 @@ int copy_scalars(mp_engine* E, const ScalarTargets& o, cudaStream_t st) {
   return MP_OK;
 }
 
+// Points a launch's copy of the state at the per-player rows of `p` (checked by check_player_outputs).
+void apply_players(const mp_player_outputs& p, State& S) {
+  S.pr = PlayerTargets{p.row_of_player, p.n_rows, (p.reward || p.scalar_obs) ? 1 : 0, p.rgb, p.reward, p.scalar_obs,
+                       p.rgb_row_stride, p.reward_row_stride, p.scalar_obs_row_stride, p.scalar_obs_stride};
+}
+
 // `out`: where this render's outputs go besides / instead of the engine's own buffers (see apply_outputs), or null.
-int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = nullptr) {
+// `players`: per-player rows (mp_step_players): the render runs k_render<..., RENDER_ROUTED>, or, with rendering off,
+// k_exchange_push delivers the routed scalars (one launch).
+int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = nullptr, const mp_player_outputs* routed = nullptr) {
   const bool players = E->flags & MP_FLAG_RENDER_PLAYERS, world = E->flags & MP_FLAG_RENDER_WORLD;
   if (!players && !world) {
     State S = E->S;
     if (out) apply_outputs(*out, S);
-    if (E->x_pending_raise) return raise_flags(E, st, S);
+    if (routed) apply_players(*routed, S);
+    if (E->x_pending_raise || S.pr.scalars_on) return raise_flags(E, st, S);  // (k_exchange_push also delivers S.out)
     return S.out.on ? copy_scalars(E, S.out, st) : MP_OK;
   }
   // The engine's own images are also slot 0's of mp_step_host_async: a render into them must not start before that
   // slot's device->host copy has read them, whichever call issues it. (A render into a target does not touch them.)
-  const bool own_images = (players && !(out && out->rgb)) || (world && !(out && out->world_rgb));
+  const bool own_images = (players && !(out && out->rgb) && !(routed && routed->rgb)) || (world && !(out && out->world_rgb));
   if (E->async_ready && own_images) CUDA_TRY(cudaStreamWaitEvent(st, E->slot[0].copied, 0));
   E->S.x_raise = E->x_pending_raise ? 1 : 0;
   E->x_pending_raise = false;
@@ -815,7 +825,8 @@ int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = 
   }
   State S = E->S;
   if (out) apply_outputs(*out, S);
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, gather ? E->render_gather_fn : E->render_fn, E->T, S, R, E->flags));
+  if (routed) apply_players(*routed, S);  // (never with gather: mp_step_players refuses it)
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, routed ? E->render_routed_fn : gather ? E->render_gather_fn : E->render_fn, E->T, S, R, E->flags));
   if (gather) {
     k_gather_raise<<<1, 32, 0, st>>>(E->d_g_flag_ptrs, E->g_world, E->g_rank, E->g_seq);
     ++E->launches;
@@ -978,10 +989,16 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
   E->step_smem = E->family->step_smem(T);
   {  // cells per lane per strip: ceil(view_w / 4) for player rows, ceil(W / 8) for world half-rows
     const int ncp = (E->R.view_w + 3) / 4, ncw = (T.W + (32 >> E->R.wstrip_log2) - 1) / (32 >> E->R.wstrip_log2);
-    if (ncp <= 3 && ncw <= 3) { E->render_fn = k_render<3, 3, false>; E->render_gather_fn = k_render<3, 3, true>; E->inst_ncp = 3; E->inst_ncw = 3; }
-    else if (ncp <= 3 && ncw <= 4) { E->render_fn = k_render<3, 4, false>; E->render_gather_fn = k_render<3, 4, true>; E->inst_ncp = 3; E->inst_ncw = 4; }
-    else if (ncp <= 3 && ncw <= 5) { E->render_fn = k_render<3, 5, false>; E->render_gather_fn = k_render<3, 5, true>; E->inst_ncp = 3; E->inst_ncw = 5; }
-    else if (ncp <= 4 && ncw <= 5) { E->render_fn = k_render<4, 5, false>; E->render_gather_fn = k_render<4, 5, true>; E->inst_ncp = 4; E->inst_ncw = 5; }
+#define MP_RENDER_INST(NCP, NCW)                                                                                  \
+  {                                                                                                               \
+    E->render_fn = k_render<NCP, NCW, RENDER_PLAIN>; E->render_gather_fn = k_render<NCP, NCW, RENDER_GATHER>;     \
+    E->render_routed_fn = k_render<NCP, NCW, RENDER_ROUTED>; E->inst_ncp = NCP; E->inst_ncw = NCW;                \
+  }
+    if (ncp <= 3 && ncw <= 3) MP_RENDER_INST(3, 3)
+    else if (ncp <= 3 && ncw <= 4) MP_RENDER_INST(3, 4)
+    else if (ncp <= 3 && ncw <= 5) MP_RENDER_INST(3, 5)
+    else if (ncp <= 4 && ncw <= 5) MP_RENDER_INST(4, 5)
+#undef MP_RENDER_INST
     else { mp_destroy(E); return fail(MP_E_UNSUPPORTED, "view of %d cells / map of %d cells wide (max 16 / 40)", E->R.view_w, T.W); }
     // lane -> cell dealing (see make_lane_map_cells / make_lane_map): whole cells per lane group with the cell order chosen
     // to minimise store bank conflicts by default; the fully conflict-free scattered colouring or the plain order for A/B.
@@ -1001,6 +1018,7 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
   // lower each other's limit, so the renderer always gets the opt-in maximum and the step kernels only ever raise theirs.
   cudaError_t ce = cudaFuncSetAttribute(E->render_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
   if (ce == cudaSuccess) ce = cudaFuncSetAttribute(E->render_gather_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
+  if (ce == cudaSuccess) ce = cudaFuncSetAttribute(E->render_routed_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
   {
     static int step_smem_max[MP_MAX_DEVICES] = {};
     const int need = (int)E->step_smem;
@@ -1699,13 +1717,61 @@ namespace {
 // The host checks of mp_state_store / mp_state_restore / mp_step_restore: the bank is 16-byte aligned, and the bank
 // and the index array lie in device allocations on the engine's device and overlap neither each other nor the
 // engine's buffers (nor the targets of mp_step_restore's `out`).
+// `more`: further extents of the call (mp_step_players' per-player targets), checked with the bank's.
 int check_bank(mp_engine* E, const void* bank, int n_slots, const int32_t* index, uint64_t index_count, uint64_t record_bytes, const char* fn,
-               const mp_device_outputs* out = nullptr) {
+               const mp_device_outputs* out = nullptr, const std::vector<DeviceExtent>& more = {}) {
   if ((uintptr_t)bank % 16) return fail(MP_E_INVALID, "%s: bank is not 16-byte aligned", fn);
   if ((uintptr_t)index % 4) return fail(MP_E_INVALID, "%s: index array is not 4-byte aligned", fn);
   std::vector<DeviceExtent> ext{{"bank", (uintptr_t)bank, (u128)n_slots * record_bytes},
                                 {"index array", (uintptr_t)index, (u128)index_count * 4}};
+  ext.insert(ext.end(), more.begin(), more.end());
   return out ? check_device_outputs(E, out, fn, std::move(ext)) : check_extents(E, ext, fn);
+}
+
+// The checks of mp_step_players / mp_reset_players' `players` that need no other argument (include/mp_engine.h); its
+// extents are appended to `ext` for the overlap and allocation checks that follow (check_bank / check_device_outputs /
+// check_extents). Extents are computed in 128 bits.
+int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_device_outputs* out, const char* fn, std::vector<DeviceExtent>& ext) {
+  if (!o) return fail(MP_E_INVALID, "%s: null players (use mp_step_into / mp_reset_into)", fn);
+  if (o->n_rows < 1) return fail(MP_E_INVALID, "%s: n_rows %d < 1", fn, o->n_rows);
+  if (!o->row_of_player || (uintptr_t)o->row_of_player % 4) return fail(MP_E_INVALID, "%s: row_of_player is null or not 4-byte aligned", fn);
+  if (E->g_world > 0 && E->S.g_world > 0)
+    return fail(MP_E_UNSUPPORTED, "%s: the observation gather is enabled: its stacked slots stay dense and complete", fn);
+  const uint64_t R = (uint64_t)o->n_rows, n = E->T.n_scalar;
+  if (o->rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
+  if (o->rgb && out && out->rgb) return fail(MP_E_INVALID, "%s: rgb is both routed (players) and per env (out)", fn);
+  if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
+  if (o->scalar_obs && (o->scalar_obs_stride % 8 || o->scalar_obs_stride >= (1ull << 31)))
+    return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes or is 2 GiB or more", fn);
+  ext.push_back({"row_of_player", (uintptr_t)o->row_of_player, (u128)E->B * E->T.P * 4});
+  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_row, uint64_t align, u128 extra) -> int {
+    if (!p) return MP_OK;
+    if ((uintptr_t)p % align || stride % align)
+      return fail(MP_E_INVALID, "%s: %s pointer or row stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
+    if (stride < per_row)
+      return fail(MP_E_INVALID, "%s: %s row stride of %llu bytes is smaller than one row's %llu bytes", fn, name,
+                  (unsigned long long)stride, (unsigned long long)per_row);
+    if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s row stride of 2 GiB or more", fn, name);
+    const u128 extent = (u128)(R - 1) * stride + per_row + extra;
+    if (extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, name);
+    ext.push_back({name, (uintptr_t)p, extent});
+    return MP_OK;
+  };
+  int rc;
+  if ((rc = add("players rgb", o->rgb, o->rgb_row_stride, (uint64_t)E->R.player_bytes, 16, 0)) ||
+      (rc = add("players reward", o->reward, o->reward_row_stride, 8, 8, 0)) ||
+      (rc = add("players scalar_obs", o->scalar_obs, o->scalar_obs_row_stride, 8, 8, (u128)(n - 1) * o->scalar_obs_stride)))
+    return rc;
+  if (o->scalar_obs) {  // n x n_rows rows of one double at k * s + r * e (the overlap rule of check_device_outputs)
+    const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_row_stride;
+    for (uint64_t j = 1; j < n; ++j) {
+      const u128 d = (u128)j * s, q = d / e, r = d % e;
+      const u128 gap = q > R - 1 ? d - (u128)(R - 1) * e : (q + 1 <= R - 1 ? std::min<u128>(r, e - r) : r);
+      if (gap < 8) return fail(MP_E_INVALID, "%s: players scalar_obs rows overlap (row stride %llu, stride %llu bytes)", fn,
+                               (unsigned long long)e, (unsigned long long)s);
+    }
+  }
+  return MP_OK;
 }
 }  // namespace
 
@@ -1752,6 +1818,39 @@ int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_
   // launched as mp_step (out == NULL) or mp_step_into: the same kernels, the same exchange and gather sequence
   if ((rc = launch_state(h, actions, nullptr, 0, st, /*render_follows=*/out != nullptr, &restore))) return rc;
   return launch_render(h, st, out);
+}
+
+int mp_step_players(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
+                    const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
+  if (!h || !actions) return fail(MP_E_INVALID, "mp_step_players: null handle or actions");
+  const bool restoring = slot_of_env || bank;
+  if (restoring && (!slot_of_env || !bank)) return fail(MP_E_INVALID, "mp_step_players: slot_of_env and bank go together");
+  if (restoring && n_slots < 1) return fail(MP_E_INVALID, "mp_step_players: n_slots %d < 1", n_slots);
+  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_players: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
+  if (flags && !restoring) return fail(MP_E_INVALID, "mp_step_players: flags without a bank");
+  DeviceGuard guard(h->device);
+  std::vector<DeviceExtent> ext;
+  int rc = check_player_outputs(h, players, out, "mp_step_players", ext);
+  if (!rc) {
+    if (restoring) rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_step_players", out, ext);
+    else rc = out ? check_device_outputs(h, out, "mp_step_players", ext) : check_extents(h, ext, "mp_step_players");
+  }
+  if (rc) return rc;
+  const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
+                            (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = launch_state(h, actions, nullptr, 0, st, /*render_follows=*/true, restoring ? &restore : nullptr))) return rc;
+  return launch_render(h, st, out, players);
+}
+
+int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
+  if (!h) return fail(MP_E_INVALID, "mp_reset_players: null handle");
+  DeviceGuard guard(h->device);
+  std::vector<DeviceExtent> ext;
+  int rc = check_player_outputs(h, players, out, "mp_reset_players", ext);
+  if (!rc) rc = out ? check_device_outputs(h, out, "mp_reset_players", ext) : check_extents(h, ext, "mp_reset_players");
+  if (!rc) rc = launch_state(h, nullptr, env_mask, 1, (cudaStream_t)stream);
+  return rc ? rc : launch_render(h, (cudaStream_t)stream, out, players);
 }
 
 int mp_launch_count(mp_handle h, uint64_t* out) {

@@ -243,9 +243,16 @@ struct ViewerInfo {  // per player, refreshed once per env
 // a half / quarter cell row (4 / 2 pixel rows) of WORLD.RGB -- compose them into a warp-private staging slot and
 // hand the slot to the TMA store engine. Two team barriers per env; everything else is warp-local.
 // Each lane handles NC cells per strip with the loads of all NC cells issued before any is packed.
-// GATHER: also deliver every strip into every rank's stacked observation buffer (State::g_*).
-template <int NCP, int NCW, bool GATHER>
+// MODE (exclusive):
+//   RENDER_GATHER: also deliver every strip into every rank's stacked observation buffer (State::g_*);
+//   RENDER_ROUTED: deliver player p of env b to the row State::pr.row_of_player[b][p] of the caller's per-player
+//     targets (mp_step_players). The team's first warp reads the env's row map with its avatars and compacts the
+//     routed players into s_players; the env's item loop then runs over those players' strips and WORLD.RGB's only,
+//     so an unrouted player is neither composited nor stored.
+enum { RENDER_PLAIN = 0, RENDER_GATHER = 1, RENDER_ROUTED = 2 };
+template <int NCP, int NCW, int MODE>
 __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, State S, RenderPlan R, uint32_t flags) {
+  constexpr bool GATHER = MODE == RENDER_GATHER, ROUTED = MODE == RENDER_ROUTED;
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem);  // [0] atlas, [1 + team] grid
   uint8_t* s_atlas = smem + R.off_atlas;
@@ -254,6 +261,9 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
   __shared__ uint8_t s_opaque[256];
   __shared__ ViewerInfo s_view_all[RENDER_MAX_TEAMS][MP_MAX_PLAYERS];
   __shared__ int s_next_item[RENDER_MAX_TEAMS];
+  // RENDER_ROUTED: the env's routed players in player order and its player strips (routed players x view_h)
+  __shared__ uint8_t s_players_all[RENDER_MAX_TEAMS][MP_MAX_PLAYERS];
+  __shared__ int s_n_pitems[RENDER_MAX_TEAMS];
 
   const int tid = threadIdx.x;
   int team = 0;
@@ -269,6 +279,8 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
   uint16_t* s_rec = reinterpret_cast<uint16_t*>(s_team + R.toff_rec);
   uint8_t* s_stage = s_team + R.toff_stage + twarp * R.stage_bytes;  // warp-private
   ViewerInfo* s_view = s_view_all[team];
+  uint8_t* s_players = s_players_all[team];
+  int* s_npi = &s_n_pitems[team];
   uint64_t* gbar = &bar[1 + team];
 
   // Work split. Balanced part: `rounds` = B / (teams in the grid) envs per team, rendered team by team with no
@@ -329,6 +341,7 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
       s_grid = reinterpret_cast<uint16_t*>(s_team0 + R.toff_grid);
       s_rec = reinterpret_cast<uint16_t*>(s_team0 + R.toff_rec);
       s_view = s_view_all[0];
+      s_players = s_players_all[0]; s_npi = &s_n_pitems[0];
       gbar = &bar[1];
       next_ctr = &s_next_item[0];
       gtid = tid; gthreads = (int)blockDim.x; bar_id = 0;
@@ -345,6 +358,13 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
       vi.fdx = dir_dx(a.z); vi.fdy = dir_dy(a.z); vi.rdx = dir_dx((a.z + 1) & 3); vi.rdy = dir_dy((a.z + 1) & 3);
       s_view[gtid] = vi;
     }
+    if (ROUTED && gtid < 32) {  // the group's first warp, whole: compact the routed players (all of them when the images are not routed)
+      bool on = gtid < T.P;
+      if (on && S.pr.rgb) on = (uint32_t)S.pr.row_of_player[(size_t)b * T.P + gtid] < (uint32_t)S.pr.n_rows;
+      const uint32_t m = __ballot_sync(MP_FULL, on);
+      if (on) s_players[__popc(m & ((1u << gtid) - 1u))] = (uint8_t)gtid;
+      if (gtid == 0) *s_npi = S.pr.rgb ? __popc(m) * R.view_h : R.n_player_items;
+    }  // (published by the group barrier after the cell pass, like s_view)
     mbar_wait(gbar, (uint32_t)(it & 1));  // (team 0's barrier has completed `rounds` phases when the tail starts, so the parity carries over)
     // ---- per-cell pass: flatten the layer stack, folding map sprites into pre-merged ones -------
     if (!(flags & 64u) || it == 0) {  // (bit 6: debug -- reuse the first env's records)
@@ -363,16 +383,18 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
     // ---- strip items, pulled by warps -------------------------------------------------------------
     int next_item = 0;  // claimed one strip ahead so that the atomic's latency hides behind the strip being drawn
     if (lane == 0) next_item = atomicAdd(next_ctr, 1);
+    const int r_pitems = ROUTED ? *s_npi : 0;  // RENDER_ROUTED: this env's player strips (the other modes read R's, as constant operands)
     for (;;) {
       const int item = __shfl_sync(MP_FULL, next_item, 0);
-      if (item >= R.n_items) break;
+      if (ROUTED ? item - r_pitems >= R.n_items - R.n_player_items : item >= R.n_items) break;
       if (lane == 0) next_item = atomicAdd(next_ctr, 1);
       uint8_t* buf = s_stage + (slot % RENDER_SLOTS) * slot_bytes;
       ++slot;
       if (lane == 0) bulk_wait_read<RENDER_SLOTS - 1>();  // the store that last used this slot has drained
       __syncwarp();
-      if (item < R.n_player_items) {
-        const int p = (int)(((uint32_t)item * R.magic_view_h) >> 16), cy = item - p * R.view_h;
+      if (item < (ROUTED ? r_pitems : R.n_player_items)) {
+        const int k = (int)(((uint32_t)item * R.magic_view_h) >> 16), cy = item - k * R.view_h;
+        const int p = ROUTED ? (int)s_players[k] : k;
         const ViewerInfo vi = s_view[p];
         const int16_t* map = s_map + p * R.n_total;
         const int py = lane & 7;
@@ -407,14 +429,18 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
         __syncwarp();
         if (lane == 0 && !(flags & 32u)) {
           const size_t in_env = (size_t)p * R.player_bytes + (size_t)cy * R.pitem_bytes;
-          bulk_store(S.rgb + b * S.rgb_env_stride + in_env, buf, (uint32_t)R.pitem_bytes, store_policy);
+          if (ROUTED && S.pr.rgb) {
+            const int row = S.pr.row_of_player[(size_t)b * T.P + p];
+            bulk_store(S.pr.rgb + (size_t)row * S.pr.rgb_row_stride + (size_t)cy * R.pitem_bytes, buf, (uint32_t)R.pitem_bytes, store_policy);
+          }
+          else bulk_store(S.rgb + b * S.rgb_env_stride + in_env, buf, (uint32_t)R.pitem_bytes, store_policy);
           if (GATHER) {  // the stacked slots stay dense, whatever the local target's stride
             const size_t off = (size_t)b * T.P * R.player_bytes + in_env;
             for (int r = 0; r < S.g_world; ++r) bulk_store(S.g_rgb[r] + off, buf, (uint32_t)R.pitem_bytes, store_policy);
           }
         }
       } else {
-        const int wi = item - R.n_player_items, wy = wi >> (3 - wlog);
+        const int wi = item - (ROUTED ? r_pitems : R.n_player_items), wy = wi >> (3 - wlog);
         const int py = ((wi & ((8 >> wlog) - 1)) << wlog) | (lane & (wrows - 1));
         const int16_t* map = s_map + T.P * R.n_total;
         const uint16_t* rowrec = s_rec + wy * T.W * R.rec_stride;
@@ -451,6 +477,7 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
     // drawing instead of delaying the kernel's start
     if (S.x_raise && it == 0) exchange_push(T, S);
     if (S.out.on && it == 0) deliver_scalars(T, S);  // (tested here, not only inside: measured, k_render<3, 3, true> spills otherwise)
+    if (ROUTED && S.pr.scalars_on && it == 0) deliver_player_scalars(T, S);
     group_sync(bar_id, gthreads);  // every warp is done with s_rec / s_view
     if (gtid == 0) *next_ctr = 0;
     // (the reset is ordered before the next env's item loop by the group barrier after its cell pass)

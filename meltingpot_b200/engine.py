@@ -61,6 +61,7 @@ EXPORTED_SYMBOLS = (
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
     'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
     'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_step_restore',
+    'mp_step_players', 'mp_reset_players',
 )
 
 MP_RESTORE_REKEY = 1
@@ -108,6 +109,83 @@ class MpDeviceOutputs(ctypes.Structure):
 
 # The outputs a step can deliver into caller-owned tensors (mp_step_into), each with the axis that indexes envs.
 DEVICE_OUTPUTS = ('rgb', 'world_rgb', 'reward', 'discount', 'step_type', 'scalar_obs')
+
+
+class MpPlayerOutputs(ctypes.Structure):
+  _fields_ = [
+      ('row_of_player', ctypes.c_void_p), ('n_rows', ctypes.c_int32),
+      ('rgb', ctypes.c_void_p), ('rgb_row_stride', ctypes.c_uint64),
+      ('reward', ctypes.c_void_p), ('reward_row_stride', ctypes.c_uint64),
+      ('scalar_obs', ctypes.c_void_p), ('scalar_obs_row_stride', ctypes.c_uint64), ('scalar_obs_stride', ctypes.c_uint64),
+  ]
+
+
+# The per-player outputs a step can deliver into rows of caller-owned tensors (mp_step_players).
+PLAYER_OUTPUTS = ('rgb', 'reward', 'scalar_obs')
+
+
+def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num_envs: int, num_players: int,
+                     num_scalar_obs: int, device: int) -> MpPlayerOutputs:
+  """The mp_player_outputs of `players`: 'row_of_player' (TensorLayout of a contiguous int32 CUDA [B, P]) and any of
+  'rgb' (uint8 [n_rows, *rgb_shape], dense inside a row), 'reward' (float64 [n_rows]) and 'scalar_obs' (float64
+  [num_scalar_obs, n_rows]); the row axis (and the observation axis of scalar_obs) may have any stride. Every target
+  must have the same n_rows. Only shapes, dtypes, devices and layouts are checked, never the row map's values."""
+  import torch  # pylint: disable=g-import-not-at-top
+  unknown = set(players) - set(PLAYER_OUTPUTS) - {'row_of_player'}
+  if unknown:
+    raise ValueError(f'players: unknown entries {sorted(unknown)} (row_of_player and any of {", ".join(PLAYER_OUTPUTS)})')
+
+  def on_device(name, t):
+    dev = torch.device(t.device)
+    if dev.type != 'cuda' or dev.index != device:
+      raise ValueError(f'players[{name!r}]: on {dev}, the engine runs on cuda:{device}')
+
+  rmap = players.get('row_of_player')
+  if rmap is None:
+    raise ValueError('players: row_of_player is missing')
+  if (tuple(rmap.shape) != (num_envs, num_players) or rmap.dtype != torch.int32
+      or tuple(rmap.stride) != (num_players, 1)):
+    raise ValueError(f'players[\'row_of_player\']: must be a contiguous int32 tensor [{num_envs}, {num_players}]')
+  on_device('row_of_player', rmap)
+  s = MpPlayerOutputs()
+  s.row_of_player = ctypes.c_void_p(int(rmap.data_ptr))
+  n_rows = None
+  targets = {k: v for k, v in players.items() if k in PLAYER_OUTPUTS and v is not None}
+  if not targets:
+    raise ValueError(f'players: give at least one of {", ".join(PLAYER_OUTPUTS)}')
+  for name, t in targets.items():
+    row_axis = 1 if name == 'scalar_obs' else 0
+    if name == 'scalar_obs' and num_scalar_obs == 0:
+      raise ValueError('players[\'scalar_obs\']: this substrate has no scalar observations')
+    dtype = torch.uint8 if name == 'rgb' else torch.float64
+    inner = tuple(rgb_shape) if name == 'rgb' else ()
+    lead = (num_scalar_obs,) if name == 'scalar_obs' else ()
+    if len(t.shape) != len(lead) + 1 + len(inner) or tuple(t.shape[:row_axis]) != lead or tuple(t.shape[row_axis + 1:]) != inner:
+      raise ValueError(f'players[{name!r}]: shape {tuple(t.shape)}, must be {lead + ("n_rows",) + inner}')
+    if t.dtype != dtype:
+      raise ValueError(f'players[{name!r}]: dtype {t.dtype}, must be {dtype}')
+    on_device(name, t)
+    rows = int(t.shape[row_axis])
+    if rows < 1:
+      raise ValueError(f'players[{name!r}]: no rows')
+    if n_rows is None:
+      n_rows = rows
+    elif rows != n_rows:
+      raise ValueError(f'players[{name!r}]: {rows} rows, another target has {n_rows}')
+    dense = 1
+    for axis in range(len(t.shape) - 1, row_axis, -1):
+      if t.shape[axis] != 1 and t.stride[axis] != dense:
+        raise ValueError(f'players[{name!r}]: axis {axis} has stride {t.stride[axis]}, must be {dense} (only the row axis'
+                         f'{" and the observation axis" if row_axis else ""} may be strided)')
+      dense *= t.shape[axis]
+    item = torch.empty((), dtype=dtype).element_size()
+    row_stride = (t.stride[row_axis] if rows > 1 else dense) * item  # with one row the stride is never used
+    setattr(s, name, ctypes.c_void_p(int(t.data_ptr)))
+    setattr(s, f'{name}_row_stride', row_stride)
+    if name == 'scalar_obs':
+      s.scalar_obs_stride = (t.stride[0] if t.shape[0] > 1 else rows * dense) * item
+  s.n_rows = n_rows
+  return s
 
 
 class TensorLayout(NamedTuple):
@@ -203,6 +281,9 @@ def load_library() -> ctypes.CDLL:
   lib.mp_state_store.argtypes = [vp, vp, ctypes.c_int, vp, vp]
   lib.mp_state_restore.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_uint32, vp]
   lib.mp_step_restore.argtypes = [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(MpDeviceOutputs), vp]
+  lib.mp_step_players.argtypes = [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(MpDeviceOutputs),
+                                  ctypes.POINTER(MpPlayerOutputs), vp]
+  lib.mp_reset_players.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
   lib.mp_step_host_async.argtypes = [vp, vp, ctypes.POINTER(MpHostOutputs), ctypes.c_int, vp]
@@ -395,19 +476,22 @@ class Engine:
   def set_flags(self, flags: int) -> None:
     _check(self._lib.mp_set_flags(self._h, ctypes.c_uint32(flags)))
 
-  def reset(self, mask=None, stream=None, out=None) -> None:
-    """out: as for step."""
+  def reset(self, mask=None, stream=None, out=None, players=None) -> None:
+    """out, players: as for step."""
     ptr = None
     if mask is not None:
       assert mask.dtype == self._torch.uint8 and mask.is_cuda and mask.numel() == self.num_envs
       ptr = ctypes.c_void_p(mask.data_ptr())
-    if out is None:
+    if players is not None:
+      s = None if out is None else ctypes.byref(self._device_outputs(out))
+      _check(self._lib.mp_reset_players(self._h, ptr, s, ctypes.byref(self._player_outputs(players)), self._stream(stream)))
+    elif out is None:
       _check(self._lib.mp_reset(self._h, ptr, self._stream(stream)))
     else:
       s = self._device_outputs(out)
       _check(self._lib.mp_reset_into(self._h, ptr, ctypes.byref(s), self._stream(stream)))
 
-  def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False) -> None:
+  def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False, players=None) -> None:
     """actions: int32 CUDA tensor [B, P] of discrete action ids.
 
     out: {name: CUDA tensor} for any of DEVICE_OUTPUTS (mp_step_into): the step's images are rendered straight into
@@ -421,8 +505,32 @@ class Engine:
     and rows without this engine's tag step env b as usual. The result is that of a step followed by
     restore_states(bank, restore, rekey), without the second render. Only the tensors' shape, dtype, device and
     layout are checked, never their values, so the call never synchronises: build the index on the device, e.g.
-    `torch.where(step_type == 2, row, -1)`. rekey: as for restore_states."""
+    `torch.where(step_type == 2, row, -1)`. rekey: as for restore_states.
+
+    players: per-player rows (mp_step_players), {'row_of_player': contiguous CUDA int32 [B, P]} plus any of 'rgb'
+    (uint8 [n_rows, h, w, 3]), 'reward' (float64 [n_rows]) and 'scalar_obs' (float64 [num_scalar_obs, n_rows]). Player p
+    of env b is delivered to row row_of_player[b, p] when that lies in 0..n_rows-1, and nowhere otherwise; with 'rgb'
+    the images are drawn straight into the rows, an unrouted player is not drawn at all and this engine's own rgb is
+    not written. Combines with out (whose rgb it replaces) and with restore / bank. The row map's values are never
+    checked on the host; two players routed to one row leave one of them there."""
     self._check_actions(actions)
+    if players is not None:
+      flags, idx, bank_ptr, n_slots = 0, None, None, 0
+      if restore is not None or bank is not None:
+        if restore is None or bank is None:
+          raise ValueError('restore and bank go together')
+        bank = self._bank(bank)
+        idx = self._indices(restore, self.num_envs, 'restore')
+        for name, t in (('bank', bank), ('restore', idx)):
+          if t.device.index != self.device:
+            raise ValueError(f'{name} is on {t.device}, the engine runs on cuda:{self.device}')
+        flags, bank_ptr, n_slots, idx = (MP_RESTORE_REKEY if rekey else 0), ctypes.c_void_p(bank.data_ptr()), int(bank.shape[0]), ctypes.c_void_p(idx.data_ptr())
+      elif rekey:
+        raise ValueError('rekey needs restore and bank')
+      s = None if out is None else ctypes.byref(self._device_outputs(out))
+      _check(self._lib.mp_step_players(self._h, ctypes.c_void_p(actions.data_ptr()), idx, bank_ptr, n_slots, ctypes.c_uint32(flags),
+                                       s, ctypes.byref(self._player_outputs(players)), self._stream(stream)))
+      return
     if restore is not None or bank is not None:
       if restore is None or bank is None:
         raise ValueError('restore and bank go together')
@@ -450,6 +558,10 @@ class Engine:
 
   def _device_outputs(self, out) -> MpDeviceOutputs:
     return describe_outputs({k: (None if v is None else layout_of(v)) for k, v in out.items()}, self.output_views(), self.device)
+
+  def _player_outputs(self, players) -> MpPlayerOutputs:
+    return describe_players({k: (None if v is None else layout_of(v)) for k, v in players.items()}, tuple(self.rgb.shape[2:]),
+                            self.num_envs, self.num_players, self.num_scalar_obs, self.device)
 
   def step_state(self, actions, stream=None) -> None:
     self._check_actions(actions)

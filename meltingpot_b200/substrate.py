@@ -241,16 +241,27 @@ class BatchedSubstrate:
     obs[_COLLECTIVE_REWARD_OBS] = e.reward.sum(dim=1)
     return BatchedTimeStep(step_type=e.step_type, reward=e.reward, discount=e.discount, observation=obs)
 
-  def reset(self, mask=None, out: Optional[BatchedTimeStep] = None) -> BatchedTimeStep:
-    """out: as for step."""
+  def reset(self, mask=None, out: Optional[BatchedTimeStep] = None, players: Optional['PlayerOutputs'] = None) -> BatchedTimeStep:
+    """out, players: as for step."""
+    if players is not None:
+      self._engine.reset(mask, out=None if out is None else self._engine_outputs(out, routed=players),
+                         players=self._routed_outputs(players))
+      return self._without_rgb(self._timestep() if out is None else self._fill_collective(out))
     if out is None:
       self._engine.reset(mask)
       return self._timestep()
     self._engine.reset(mask, out=self._engine_outputs(out))
     return self._fill_collective(out)
 
+  def player_routes(self, groups) -> 'PlayerRoutes':
+    """Rows for per-player delivery: groups is an integer [B, P] array of group ids (e.g. the policy of each player
+    slot), -1 for a player nobody reads. See PlayerRoutes."""
+    import torch  # pylint: disable=g-import-not-at-top
+    return PlayerRoutes(groups, self.num_envs, self.num_players, tuple(self._engine.rgb.shape[2:]), self._scalar_names,
+                        torch.device('cuda', self._engine.device))
+
   def step(self, actions, out: Optional[BatchedTimeStep] = None, restore=None, bank=None,
-           rekey: bool = False) -> BatchedTimeStep:
+           rekey: bool = False, players: Optional['PlayerOutputs'] = None) -> BatchedTimeStep:
     """actions: integer tensor [B, P] on the engine's device (int32 preferred).
 
     out: a BatchedTimeStep of caller-owned tensors to fill and return instead of views of the engine's buffers, e.g.
@@ -261,11 +272,20 @@ class BatchedSubstrate:
     env b takes bank row restore[b] (a `state_bank` row written by `store`) instead of stepping, and shows that
     record's timestep and images. -1, other out-of-range indices and rows that hold no record of this substrate step
     env b as usual. The values are not checked, so nothing synchronises; e.g. restart finished episodes from stored
-    start states with `restore = torch.where(ts.step_type == 2, rows, -1)`. rekey: as for `restore`."""
+    start states with `restore = torch.where(ts.step_type == 2, rows, -1)`. rekey: as for `restore`.
+
+    players: a PlayerOutputs (`player_routes(groups).outputs()`, or `.at(t)` of one with T slots): each routed
+    player's image, reward and scalar observations go to its row, the images drawn straight there; unrouted players are
+    not drawn. The returned timestep then has no 'RGB'; every other field is as without players. Combines with out and
+    restore / bank."""
     import torch  # pylint: disable=g-import-not-at-top
     if actions.dtype != torch.int32:
       actions = actions.to(torch.int32)
     kw = dict(restore=restore, bank=bank, rekey=rekey)
+    if players is not None:
+      self._engine.step(actions.contiguous(), out=None if out is None else self._engine_outputs(out, routed=players),
+                        players=self._routed_outputs(players), **kw)
+      return self._without_rgb(self._timestep() if out is None else self._fill_collective(out))
     if out is None:
       self._engine.step(actions.contiguous(), **kw)
       return self._timestep()
@@ -280,11 +300,30 @@ class BatchedSubstrate:
     return Trajectory(int(T), self.num_envs, self.num_players, e.rgb.shape[1:], e.world_rgb.shape[1:] if self._world_rgb else None,
                       self._scalar_names, bool(time_major), torch.device('cuda', e.device))
 
-  def _engine_outputs(self, ts: BatchedTimeStep):
-    """The engine's output tensors of a BatchedTimeStep (the scalar observations as one [n, B, P] view)."""
+  def _routed_outputs(self, po: 'PlayerOutputs'):
+    """The engine's per-player targets of a PlayerOutputs (the scalar observations as one [n, n_rows] view)."""
+    if not isinstance(po, PlayerOutputs):
+      raise ValueError('players must be a PlayerOutputs (player_routes(groups).outputs())')
+    import torch  # pylint: disable=g-import-not-at-top
+    r = po.routes
+    if (r.num_envs, r.num_players) != (self.num_envs, self.num_players) or r.device != torch.device('cuda', self._engine.device):
+      raise ValueError(f'players: routes of {r.num_envs} envs x {r.num_players} players on {r.device}, this batch has '
+                       f'{self.num_envs} x {self.num_players} on cuda:{self._engine.device}')
+    if po.T is not None:
+      raise ValueError('players: pick one slot of a PlayerOutputs with T slots (outputs(T).at(t))')
+    return {'row_of_player': r.row_of_player, 'rgb': po['RGB'], 'reward': po['REWARD'], 'scalar_obs': po.scalar_block}
+
+  @staticmethod
+  def _without_rgb(ts: BatchedTimeStep) -> BatchedTimeStep:
+    return BatchedTimeStep(step_type=ts.step_type, reward=ts.reward, discount=ts.discount,
+                           observation={k: v for k, v in ts.observation.items() if k != 'RGB'})
+
+  def _engine_outputs(self, ts: BatchedTimeStep, routed=None):
+    """The engine's output tensors of a BatchedTimeStep (the scalar observations as one [n, B, P] view). routed: the
+    images go to those rows instead, so ts's 'RGB' is left alone."""
     import torch  # pylint: disable=g-import-not-at-top
     obs = ts.observation
-    out = {'rgb': obs.get('RGB'), 'world_rgb': obs.get('WORLD.RGB') if self._world_rgb else None,
+    out = {'rgb': None if routed is not None else obs.get('RGB'), 'world_rgb': obs.get('WORLD.RGB') if self._world_rgb else None,
            'reward': ts.reward, 'discount': ts.discount, 'step_type': ts.step_type}
     scalars = [obs[name] for name in self._scalar_names if name in obs]
     if scalars:
@@ -407,6 +446,115 @@ class Trajectory:
     pick = (lambda x: x[t]) if self.time_major else (lambda x: x[:, t])
     return BatchedTimeStep(step_type=pick(self.step_type), reward=pick(self.reward), discount=pick(self.discount),
                            observation={k: pick(v) for k, v in self.observation.items()})
+
+
+class PlayerRoutes:
+  """Where each player's outputs go (BatchedSubstrate.player_routes): an immutable assignment of player slots to rows.
+
+  groups[b, p] is the group of player p of env b (e.g. the policy that plays that slot), -1 for a player whose
+  observations nobody reads. Rows are laid out group-major, then env, then player, so each group's rows are one
+  contiguous block, `rows(g)`. The assignment is validated once, here, on the host; the device tensors are then used as
+  they are by every step.
+    row_of_player  int32 CUDA [B, P]: the row of each player, -1 if unrouted (what the engine reads);
+    env_of_row, player_of_row  int64 CUDA [n_rows]: the env and player of each row, e.g. to scatter per-row actions
+      into the [B, P] actions of a step: actions[env_of_row, player_of_row] = row_actions.
+  Do not write to these tensors: they are shared by every PlayerOutputs made from this object."""
+
+  __slots__ = ('num_envs', 'num_players', 'num_groups', 'n_rows', 'device', 'row_of_player', 'env_of_row', 'player_of_row',
+               '_starts', '_rgb_shape', '_scalar_names')
+
+  def __init__(self, groups, num_envs: int, num_players: int, rgb_shape, scalar_names: Sequence[str], device):
+    """rgb_shape: one player's [h, w, 3]; device: where the tensors live (a CUDA device for the engine)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    g = groups.detach().cpu().numpy() if isinstance(groups, torch.Tensor) else np.asarray(groups)
+    if g.shape != (num_envs, num_players):
+      raise ValueError(f'groups must have shape [{num_envs}, {num_players}], got {list(g.shape)}')
+    if g.dtype == np.bool_ or not np.issubdtype(g.dtype, np.integer):
+      raise ValueError(f'groups must hold integer group ids, got dtype {g.dtype}')
+    g = g.astype(np.int64)
+    if (g < -1).any():
+      raise ValueError('group ids must be >= 0, or -1 for a player that is not delivered')
+    routed = np.flatnonzero(g.reshape(-1) >= 0)
+    if routed.size == 0:
+      raise ValueError('groups routes no player (every id is -1)')
+    if routed.size >= 2**31:
+      raise ValueError('more than 2^31 - 1 rows')
+    flat = routed[np.argsort(g.reshape(-1)[routed], kind='stable')]  # group-major; env, then player within a group
+    rows = np.full(num_envs * num_players, -1, np.int32)
+    rows[flat] = np.arange(flat.size, dtype=np.int32)
+    n_groups = int(g.max()) + 1
+    counts = np.bincount(g.reshape(-1)[routed], minlength=n_groups)
+    dev = torch.device(device)
+    set_ = lambda k, v: object.__setattr__(self, k, v)
+    set_('num_envs', int(num_envs)); set_('num_players', int(num_players)); set_('num_groups', n_groups)
+    set_('n_rows', int(flat.size)); set_('device', dev)
+    set_('_starts', tuple(int(x) for x in np.concatenate([[0], np.cumsum(counts)])))
+    set_('_rgb_shape', tuple(int(x) for x in rgb_shape)); set_('_scalar_names', tuple(scalar_names))
+    set_('row_of_player', torch.from_numpy(rows.reshape(num_envs, num_players)).to(dev))
+    set_('env_of_row', torch.from_numpy(flat // num_players).to(dev))
+    set_('player_of_row', torch.from_numpy(flat % num_players).to(dev))
+
+  def __setattr__(self, name, value):
+    raise AttributeError('PlayerRoutes is immutable; build a new one with player_routes(groups)')
+
+  def rows(self, g: int) -> slice:
+    """The rows of group g (empty for a group id nobody has)."""
+    if not 0 <= g < self.num_groups:
+      raise IndexError(f'group {g} outside 0..{self.num_groups - 1}')
+    return slice(self._starts[g], self._starts[g + 1])
+
+  def outputs(self, T: Optional[int] = None) -> 'PlayerOutputs':
+    """Zeroed CUDA tensors for the routed outputs: 'RGB' uint8 [n_rows, h, w, 3], 'REWARD' float64 [n_rows] and each
+    scalar observation float64 [n_rows] (views of one tensor); with T, each gets a leading time axis [T, n_rows, ...]
+    and `at(t)` is slot t."""
+    return PlayerOutputs(self, T)
+
+
+class PlayerOutputs:
+  """Caller-owned CUDA tensors for the routed outputs of PlayerRoutes (routes.outputs(T)); `po[name]` is one of them.
+  Pass it (or, with T slots, `at(t)`) to BatchedSubstrate.step / reset as players=."""
+
+  def __init__(self, routes: PlayerRoutes, T: Optional[int] = None, tensors=None, scalar_block=None):
+    import torch  # pylint: disable=g-import-not-at-top
+    self.routes, self.T = routes, T
+    if tensors is not None:  # a view (at / group)
+      self.tensors, self.scalar_block = tensors, scalar_block
+      return
+    if T is not None and T < 1:
+      raise ValueError(f'outputs need T >= 1 slots, got {T}')
+    lead = (routes.n_rows,) if T is None else (int(T), routes.n_rows)
+    dev = routes.device
+    self.tensors = {'RGB': torch.zeros(lead + routes._rgb_shape, dtype=torch.uint8, device=dev),  # pylint: disable=protected-access
+                    'REWARD': torch.zeros(lead, dtype=torch.float64, device=dev)}
+    names = routes._scalar_names  # pylint: disable=protected-access
+    self.scalar_block = torch.zeros((len(names),) + lead, dtype=torch.float64, device=dev) if names else None
+    for k, name in enumerate(names):  # one tensor, so that a slot's scalar observations are one [n, n_rows] view
+      self.tensors[name] = self.scalar_block[k]
+
+  def __getitem__(self, name):
+    return self.tensors[name]
+
+  def keys(self):
+    return self.tensors.keys()
+
+  def at(self, t: int) -> 'PlayerOutputs':
+    """Slot t of outputs made with T slots, as views."""
+    if self.T is None:
+      raise ValueError('at() needs outputs made with T slots')
+    if not -self.T <= t < self.T:
+      raise IndexError(f'slot {t} of {self.T}')
+    sb = None if self.scalar_block is None else self.scalar_block[:, t]
+    tensors = {k: v[t] for k, v in self.tensors.items()}
+    for k, name in enumerate(self.routes._scalar_names):  # pylint: disable=protected-access
+      tensors[name] = sb[k]
+    return PlayerOutputs(self.routes, None, tensors, sb)
+
+  def group(self, g: int) -> Dict[str, Any]:
+    """{name: view of group g's rows} ([rows, ...], or [T, rows, ...] with T slots)."""
+    r = self.routes.rows(g)
+    if self.T is None:
+      return {k: v[r] for k, v in self.tensors.items()}
+    return {k: v[:, r] for k, v in self.tensors.items()}
 
 
 # ---------------------------------------------------------------------------------------------
