@@ -376,6 +376,35 @@ int mp_step_players(mp_handle h, const int32_t* actions, const int32_t* slot_of_
 int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out,
                      const mp_player_outputs* players, void* stream);
 
+/* Caller-owned DEVICE rows a step's actions are read from: player p of env b takes the action id in row
+ * row_of_player[b][p] when 0 <= row < n_rows, and action 0 (NOOP in every shipped substrate) otherwise. A learner that
+ * gets its observations in rows (mp_player_outputs) writes its actions into rows laid out the same way, and nothing is
+ * scattered back into [B][P]. The row map may be the same tensor as mp_player_outputs.row_of_player. Stride in bytes. */
+typedef struct mp_player_actions {
+  const int32_t* row_of_player;  /* DEVICE i32 [B][P]; may be the same tensor as mp_player_outputs.row_of_player */
+  int32_t n_rows;
+  const int32_t* action; uint64_t action_row_stride;  /* [n_rows] x i32, stride in bytes */
+} mp_player_actions;
+
+/* A step whose actions come from rows. With dense[b][p] the action the rule above gives player p of env b, the call is,
+ * byte for byte (outputs, events, state, keys, variant bytes) and launch for launch:
+ *   - mp_step_players(dense, slot_of_env, bank, n_slots, flags, out, players) when players is set;
+ *   - mp_step_restore(dense, slot_of_env, bank, n_slots, flags, out) when only slot_of_env / bank are given;
+ *   - mp_step_into(dense, out), or mp_step(dense) when out is NULL, when neither is given.
+ * An id out of range in a row is action 0, as in a dense step; a restored env and an env stepping after LAST ignore
+ * their actions. The row map and the rows are read on the device and never checked on the host. With players NULL the
+ * call is accepted while the observation gather is enabled (no image is routed); with players set it is refused as
+ * mp_step_players refuses it.
+ * Every check runs before anything is enqueued, and a refused call (MP_E_INVALID) steps no env. Refused besides every
+ * refusal of the composed call: a NULL actions or n_rows < 1; a row map not 4-byte aligned or not B * P i32 inside one
+ * device allocation on the engine's device; an action pointer or stride not a multiple of 4, or of 2 GiB or more; a
+ * stride smaller than 4; action rows not inside one device allocation on the engine's device; a row map or action
+ * rows that overlap any target, the bank, the index array or the engine's buffers (the two row maps may be one tensor,
+ * both are only read). */
+int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t* slot_of_env, const void* bank,
+                   int n_slots, uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players,
+                   void* stream);
+
 /* Diagnostic: how the renderer was laid out for this substrate: teams per CTA, threads per team, log2 of the pixel
  * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes,
  * then the lane -> cell dealing built for player strips and for WORLD.RGB strips (0 plain, 2 scattered colouring,

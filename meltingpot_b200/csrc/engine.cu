@@ -140,14 +140,15 @@ struct VariantSet {
   int n = 1;
   const Tables* maps = nullptr;  // [n] the Tables of each variant's map (a family with map variants), else null
 };
-// The launches take the restore of mp_step_restore, or null for the plain k_step.
+// The launches take the restore of mp_step_restore, or null for the plain k_step, and the row actions of
+// mp_step_routed (then `actions` is unused), or null for dense actions.
 struct FamilyEntry {
   int id;  // MpbFamily
   bool map_variants;  // Family::kMapVariants: its variants may be draws of different maps (mp_create_variants)
   const char* const* map_sections;  // then Family::kMapSections: its own entity tables, which such variants may differ in
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
   cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int,
-                        const StepRestore*);
+                        const StepRestore*, const RowActions*);
   size_t (*step_smem)(const Tables&);
   const void* step;           // k_step<Family>
   // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field), the upload of base's Params with
@@ -155,9 +156,10 @@ struct FamilyEntry {
   int (*same_shape)(const FamilyParams&, const FamilyParams&);
   int (*upload_variants)(std::vector<void*>&, const FamilyParams& base, const std::vector<FamilyParams>&, const void**);
   cudaError_t (*launch_variants)(const cudaLaunchConfig_t&, const Tables&, const VariantSet&, const State&, const int32_t*, const uint8_t*, int,
-                                 const StepRestore*);
+                                 const StepRestore*, const RowActions*);
   const void* step_variants;  // k_step<Family, ParamVariants<Family::Params>>
   const void* step_restore[2];  // the kRestore instantiations of both (mp_step_restore)
+  const void* step_routed[4];   // the RowActions instantiations of all four (mp_step_routed)
 };
 
 template <class Family>
@@ -166,10 +168,13 @@ int load_family(FamilyLoad& ld, const Tables& T, FamilyParams& params) {
 }
 template <class Family>
 cudaError_t launch_family(const cudaLaunchConfig_t& cfg, const Tables& T, const FamilyParams& params, const State& S,
-                          const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore) {
-  const typename Family::Params& F = std::get<typename Family::Params>(params);
-  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, typename Family::Params, true>, T, F, S, actions, mask, mode, *restore);
-  return cudaLaunchKernelEx(&cfg, k_step<Family>, T, F, S, actions, mask, mode, StepRestore{});
+                          const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore, const RowActions* rows) {
+  using P = typename Family::Params;
+  const P& F = std::get<P>(params);
+  if (rows && restore) return cudaLaunchKernelEx(&cfg, k_step<Family, P, true, RowActions>, T, F, S, nullptr, mask, mode, *restore, *rows);
+  if (rows) return cudaLaunchKernelEx(&cfg, k_step<Family, P, false, RowActions>, T, F, S, nullptr, mask, mode, StepRestore{}, *rows);
+  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, typename Family::Params, true>, T, F, S, actions, mask, mode, *restore, RowActions{});
+  return cudaLaunchKernelEx(&cfg, k_step<Family>, T, F, S, actions, mask, mode, StepRestore{}, RowActions{});
 }
 template <class Family>
 int same_shape_family(const FamilyParams& a, const FamilyParams& b) {
@@ -190,11 +195,13 @@ int upload_variants_family(std::vector<void*>& allocs, const FamilyParams& base,
 }
 template <class Family>
 cudaError_t launch_variants_family(const cudaLaunchConfig_t& cfg, const Tables& T, const VariantSet& V, const State& S,
-                                   const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore) {
+                                   const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore, const RowActions* rows) {
   using P = typename Family::Params;
   const ParamVariants<P> src{static_cast<const P*>(V.params), V.active, V.pending, V.n, V.maps};
-  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true>, T, src, S, actions, mask, mode, *restore);
-  return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode, StepRestore{});
+  if (rows && restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true, RowActions>, T, src, S, nullptr, mask, mode, *restore, *rows);
+  if (rows) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, false, RowActions>, T, src, S, nullptr, mask, mode, StepRestore{}, *rows);
+  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true>, T, src, S, actions, mask, mode, *restore, RowActions{});
+  return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode, StepRestore{}, RowActions{});
 }
 template <class Family>
 constexpr const char* const* map_sections() {
@@ -207,7 +214,11 @@ FamilyEntry family_entry(int id) {
           same_shape_family<Family>, upload_variants_family<Family>, launch_variants_family<Family>,
           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>),
           {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true>),
-           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, true>)}};
+           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, true>)},
+          {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, false, RowActions>),
+           reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true, RowActions>),
+           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, false, RowActions>),
+           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, true, RowActions>)}};
 }
 const FamilyEntry kFamilies[] = {
     family_entry<CleanUp>(MPB_FAMILY_CLEAN_UP),
@@ -727,8 +738,9 @@ int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
 
 // `render_follows`: the caller launches the renderer next on the same stream; it raises the exchange flags.
 // `restore`: a step (mode 0) that restores the envs it names instead of advancing them (k_step<..., true>), or null.
+// `rows`: the step's actions come from rows (mp_step_routed, k_step<..., RowActions>; `actions` unused), or null.
 int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int mode, cudaStream_t st, bool render_follows = true,
-                 const StepRestore* restore = nullptr) {
+                 const StepRestore* restore = nullptr, const RowActions* rows = nullptr) {
   const int blocks = (E->B + 3) / 4;
   if (E->S.x_world) E->S.x_step = ++E->x_seq;
   cudaLaunchConfig_t cfg = {};
@@ -737,8 +749,8 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  if (E->variants.n > 1) CUDA_TRY(E->family->launch_variants(cfg, E->T, E->variants, E->S, actions, mask, mode, restore));
-  else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode, restore));
+  if (E->variants.n > 1) CUDA_TRY(E->family->launch_variants(cfg, E->T, E->variants, E->S, actions, mask, mode, restore, rows));
+  else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode, restore, rows));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st, E->S); }
@@ -1027,6 +1039,8 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
         if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
         if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step_variants, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
         for (const void* k : f.step_restore)
+          if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
+        for (const void* k : f.step_routed)
           if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
       }
       if (ce == cudaSuccess) step_smem_max[device] = need;
@@ -1773,6 +1787,23 @@ int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_devi
   }
   return MP_OK;
 }
+
+// The checks of mp_step_routed's `actions` that need no other argument (include/mp_engine.h); its extents are appended
+// to `ext` like check_player_outputs'. The row map is left out when it is `players`' own row map (both are only read).
+int check_player_actions(mp_engine* E, const mp_player_actions* a, const mp_player_outputs* players, const char* fn,
+                         std::vector<DeviceExtent>& ext) {
+  if (!a) return fail(MP_E_INVALID, "%s: null actions", fn);
+  if (a->n_rows < 1) return fail(MP_E_INVALID, "%s: actions n_rows %d < 1", fn, a->n_rows);
+  if (!a->row_of_player || (uintptr_t)a->row_of_player % 4) return fail(MP_E_INVALID, "%s: actions row_of_player is null or not 4-byte aligned", fn);
+  if (!a->action || (uintptr_t)a->action % 4 || a->action_row_stride % 4 || a->action_row_stride >= (1ull << 31))
+    return fail(MP_E_INVALID, "%s: action is null, or its pointer or row stride is not a multiple of 4 bytes or is 2 GiB or more", fn);
+  if (a->action_row_stride < 4) return fail(MP_E_INVALID, "%s: action row stride of %llu bytes is smaller than one row's 4 bytes", fn,
+                                            (unsigned long long)a->action_row_stride);
+  if (!players || players->row_of_player != a->row_of_player)
+    ext.push_back({"actions row_of_player", (uintptr_t)a->row_of_player, (u128)E->B * E->T.P * 4});
+  ext.push_back({"action", (uintptr_t)a->action, (u128)(a->n_rows - 1) * a->action_row_stride + 4});
+  return MP_OK;
+}
 }  // namespace
 
 int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* bank, void* stream) {
@@ -1851,6 +1882,32 @@ int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outpu
   if (!rc) rc = out ? check_device_outputs(h, out, "mp_reset_players", ext) : check_extents(h, ext, "mp_reset_players");
   if (!rc) rc = launch_state(h, nullptr, env_mask, 1, (cudaStream_t)stream);
   return rc ? rc : launch_render(h, (cudaStream_t)stream, out, players);
+}
+
+int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t* slot_of_env, const void* bank, int n_slots,
+                   uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
+  if (!h) return fail(MP_E_INVALID, "mp_step_routed: null handle");
+  const bool restoring = slot_of_env || bank;
+  if (restoring && (!slot_of_env || !bank)) return fail(MP_E_INVALID, "mp_step_routed: slot_of_env and bank go together");
+  if (restoring && n_slots < 1) return fail(MP_E_INVALID, "mp_step_routed: n_slots %d < 1", n_slots);
+  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_routed: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
+  if (flags && !restoring) return fail(MP_E_INVALID, "mp_step_routed: flags without a bank");
+  DeviceGuard guard(h->device);
+  std::vector<DeviceExtent> ext;
+  int rc = check_player_actions(h, actions, players, "mp_step_routed", ext);
+  if (!rc && players) rc = check_player_outputs(h, players, out, "mp_step_routed", ext);
+  if (!rc) {
+    if (restoring) rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_step_routed", out, ext);
+    else rc = out ? check_device_outputs(h, out, "mp_step_routed", ext) : check_extents(h, ext, "mp_step_routed");
+  }
+  if (rc) return rc;
+  const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
+                            (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
+  const RowActions rows{actions->row_of_player, reinterpret_cast<const uint8_t*>(actions->action), actions->action_row_stride, actions->n_rows};
+  cudaStream_t st = (cudaStream_t)stream;
+  // launched as the composed call: mp_step (render_follows false), mp_step_into, mp_step_restore or mp_step_players
+  if ((rc = launch_state(h, nullptr, nullptr, 0, st, /*render_follows=*/out || players, restoring ? &restore : nullptr, &rows))) return rc;
+  return launch_render(h, st, out, players);
 }
 
 int mp_launch_count(mp_handle h, uint64_t* out) {

@@ -142,7 +142,8 @@ struct CleanUp {
     reset_env_row(T, S, b, lane, episode, F.dirt_count0);
   }
 
-  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+  template <class Actions>
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const Actions& actions, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
     int dirt_count = env[ENV_DIRT];
     const unsigned cleaned_prev = (unsigned)env[ENV_CLEANED];

@@ -100,7 +100,8 @@ struct Coins {
     reset_env_row(T, S, b, lane, episode, 0);
   }
 
-  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+  template <class Actions>
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const Actions& actions, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
     const bool is_av = lane < T.P;
     uint8_t* s_state = sc.apple;  // [nA_pad] bits 0-1 state code, bits 4-5 state queued by ChoiceCoinRegrow, bit 6 collected

@@ -84,11 +84,29 @@ __device__ __forceinline__ int env_variant(const ParamVariants<Params>& V, int b
   return k;
 }
 
+// Where a step's actions come from. DenseActions: an id per player, [B][P] (null on territory's frame 0: every avatar
+// does nothing). RowActions (mp_step_routed): player p of env b takes the id in row row_of_player[b][p] of `action`,
+// rows `stride` bytes apart, or action 0 when that row lies outside [0, n_rows). The row is read on the avatar's lane
+// where the action is decoded (load_avatar), so nothing of it stays live across the frame.
+using DenseActions = const int32_t* __restrict__;
+struct RowActions {
+  const int32_t* row_of_player;  // [B][P]
+  const uint8_t* action;         // [n_rows] x i32
+  uint64_t stride;
+  int n_rows;
+};
+
+template <class Actions>
+__device__ __forceinline__ const Actions& select_actions(const DenseActions& dense, const RowActions& rows) {
+  if constexpr (std::is_same<Actions, RowActions>::value) return rows;
+  else return dense;
+}
+
 // A Family provides: Params (what only its kernel reads), the host-side load(FamilyLoad&, T, Params&) that decodes its
 // blob sections (family_load.h), Scratch, kStagesTables, kMapVariants (whether its variants may differ in the map, and
 // then copy_map(dst, src) on the host, which copies a variant's map-dependent Params), scratch_bytes(T) per warp, table_bytes(T) per CTA,
 // stage(T, F, tables) (copies static tables into shared memory), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
-// and step(T, F, S, b, lane, actions, sc), and on the host same_shape(a, b) and copy_knobs(dst, src) for per-env
+// and step(T, F, S, b, lane, actions, sc) for either action source, and on the host same_shape(a, b) and copy_knobs(dst, src) for per-env
 // variants. `Source` is the family's Params (one blob) or ParamVariants<Params>. A single Params is a grid constant:
 // without it, the compiler copies a small Params that is indexed with a run-time value (coins' coin_reward[who],
 // coop_mining's ore_sprite[state]) to the stack, and passed on as it is, it keeps its constant-bank reads. Variants are
@@ -98,10 +116,14 @@ __device__ __forceinline__ int env_variant(const ParamVariants<Params>& V, int b
 // the dependency wait) copies that record instead of advancing, which also takes precedence over the auto-reset after
 // LAST; the record carries the timestep and the events, so event_begin / event_end are skipped too. Every other warp
 // runs the plain step. With kRestore = false, `restore` is never read and the kernel is the plain step.
-template <class Family, class Source = typename Family::Params, bool kRestore = false>
+// Actions: DenseActions (`actions`; `rows` is never read), or RowActions (`rows`; launched by mp_step_routed only, mode 0,
+// and `actions` is never read).
+template <class Family, class Source = typename Family::Params, bool kRestore = false, class Actions = DenseActions>
 __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant__ Source src, State S, const int32_t* __restrict__ actions,
-                                                 const uint8_t* __restrict__ mask, int mode, const __grid_constant__ StepRestore restore) {
+                                                 const uint8_t* __restrict__ mask, int mode, const __grid_constant__ StepRestore restore,
+                                                 const __grid_constant__ RowActions rows) {
   constexpr bool kVariants = !std::is_same<Source, typename Family::Params>::value;
+  const Actions& acts = select_actions<Actions>(actions, rows);
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // Programmatic dependent launch, both ways: let the renderer that follows in the stream stage its tables while this
@@ -129,14 +151,14 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
       if constexpr (Family::kMapVariants) {
         const Tables& Tm = src.maps[k];
         if (reset) Family::reset(Tm, F, S, b, lane, sc);
-        else Family::step(Tm, F, S, b, lane, actions, sc);
+        else Family::template step<Actions>(Tm, F, S, b, lane, acts, sc);
       } else {
         if (reset) Family::reset(T, F, S, b, lane, sc);
-        else Family::step(T, F, S, b, lane, actions, sc);
+        else Family::template step<Actions>(T, F, S, b, lane, acts, sc);
       }
     } else {
       if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, src, S, b, lane, sc);
-      else Family::step(T, src, S, b, lane, actions, sc);
+      else Family::template step<Actions>(T, src, S, b, lane, acts, sc);
     }
     event_end(S, b, lane);
   }
@@ -253,17 +275,28 @@ __device__ __forceinline__ void reset_env_row(const Tables& T, const State& S, i
 // ---------------------------------------------------------------------------------------------
 // One frame
 // ---------------------------------------------------------------------------------------------
+// The action id of player i = b * P + p (see DenseActions / RowActions); null dense actions are no actions. Actions
+// are read-only for the whole step, so they are read through the non-coherent path.
+__device__ __forceinline__ bool has_actions(DenseActions actions) { return actions != nullptr; }
+__device__ __forceinline__ bool has_actions(const RowActions&) { return true; }
+__device__ __forceinline__ int action_id(DenseActions actions, size_t i) { return __ldg(actions + i); }
+__device__ __forceinline__ int action_id(const RowActions& a, size_t i) {
+  const int row = __ldg(a.row_of_player + i);
+  return (uint32_t)row < (uint32_t)a.n_rows ? __ldg(reinterpret_cast<const int32_t*>(a.action + (size_t)row * a.stride)) : 0;
+}
+
 // This lane's avatar (x, y, orientation, alive), its timers, and its action decoded by the action table
 // (discrete_action_wrapper.py:97-100; an id out of range is action 0). Zeros on lanes >= P, and for the action when
 // `actions` is null (territory's frame 0: every avatar does nothing).
-__device__ __forceinline__ void load_avatar(const Tables& T, const State& S, int b, int lane, const int32_t* __restrict__ actions,
+template <class Actions>
+__device__ __forceinline__ void load_avatar(const Tables& T, const State& S, int b, int lane, const Actions& actions,
                                             const int32_t* act_table, int4& av, int4& timer, int4& act) {
   av = timer = act = make_int4(0, 0, 0, 0);
   if (lane < T.P) {
     av = *reinterpret_cast<const int4*>(S.avatar + ((size_t)b * T.P + lane) * 4);
     timer = *reinterpret_cast<const int4*>(S.av_timer + ((size_t)b * T.P + lane) * 4);
-    if (actions) {
-      int id = actions[(size_t)b * T.P + lane];
+    if (has_actions(actions)) {
+      int id = action_id(actions, (size_t)b * T.P + lane);
       if (id < 0 || id >= T.n_actions) id = 0;
       act = *reinterpret_cast<const int4*>(act_table + id * 4);
     }

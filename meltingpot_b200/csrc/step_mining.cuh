@@ -108,7 +108,8 @@ struct Mining {
     reset_env_row(T, S, b, lane, episode, 0);
   }
 
-  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, WarpScratch& sc) {
+  template <class Actions>
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const Actions& actions, WarpScratch& sc) {
     const auto [env, grid, k0, k1, n, episode] = begin_frame(T, S, b, false);
     const bool is_av = lane < T.P;
     // bits 0-1 state code; bits 2-3 state set in round 1 (1 single-miner ore, 2 two-miner ore; by a reset or by

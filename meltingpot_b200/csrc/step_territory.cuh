@@ -246,7 +246,8 @@ struct Territory {
   }
 
   // One frame. `actions` is null on frame 0 of an episode: every avatar does nothing.
-  __device__ static void frame(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, TerritoryScratch& sc,
+  template <class Actions>
+  __device__ static void frame(const Tables& T, const Params& F, const State& S, int b, int lane, const Actions& actions, TerritoryScratch& sc,
                                const Frame& f) {
     const auto [env, grid, k0, k1, n, episode] = f;
     uint8_t* u8 = S.fam_u8 + (size_t)b * S.fam_u8_stride;
@@ -557,10 +558,11 @@ struct Territory {
     __syncwarp();
     init(T, F, S, b, lane, sc, f.grid, f.episode, f.k0, f.k1);
     reset_env_row(T, S, b, lane, f.episode, 0);
-    frame(T, F, S, b, lane, nullptr, sc, f);
+    frame<DenseActions>(T, F, S, b, lane, nullptr, sc, f);
   }
 
-  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const int32_t* __restrict__ actions, TerritoryScratch& sc) {
-    frame(T, F, S, b, lane, actions, sc, begin_frame(T, S, b, false));
+  template <class Actions>
+  __device__ static void step(const Tables& T, const Params& F, const State& S, int b, int lane, const Actions& actions, TerritoryScratch& sc) {
+    frame<Actions>(T, F, S, b, lane, actions, sc, begin_frame(T, S, b, false));
   }
 };

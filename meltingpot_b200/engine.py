@@ -61,7 +61,7 @@ EXPORTED_SYMBOLS = (
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
     'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
     'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_step_restore',
-    'mp_step_players', 'mp_reset_players',
+    'mp_step_players', 'mp_reset_players', 'mp_step_routed',
 )
 
 MP_RESTORE_REKEY = 1
@@ -188,6 +188,42 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
   return s
 
 
+class MpPlayerActions(ctypes.Structure):
+  _fields_ = [
+      ('row_of_player', ctypes.c_void_p), ('n_rows', ctypes.c_int32),
+      ('action', ctypes.c_void_p), ('action_row_stride', ctypes.c_uint64),
+  ]
+
+
+def describe_player_actions(player_actions: Mapping[str, Any], num_envs: int, num_players: int, device: int) -> MpPlayerActions:
+  """The mp_player_actions of `player_actions`: 'row_of_player' (TensorLayout of a contiguous int32 CUDA [B, P]) and
+  'action' (int32 [n_rows], any row stride). Only shapes, dtypes, devices and layouts are checked, never the values."""
+  import torch  # pylint: disable=g-import-not-at-top
+  unknown = set(player_actions) - {'row_of_player', 'action'}
+  if unknown:
+    raise ValueError(f'player_actions: unknown entries {sorted(unknown)} (row_of_player and action)')
+  rmap, action = player_actions.get('row_of_player'), player_actions.get('action')
+  if rmap is None or action is None:
+    raise ValueError('player_actions: needs both row_of_player and action')
+  if (tuple(rmap.shape) != (num_envs, num_players) or rmap.dtype != torch.int32
+      or tuple(rmap.stride) != (num_players, 1)):
+    raise ValueError(f'player_actions[\'row_of_player\']: must be a contiguous int32 tensor [{num_envs}, {num_players}]')
+  if len(action.shape) != 1 or action.dtype != torch.int32:
+    raise ValueError(f'player_actions[\'action\']: must be an int32 tensor [n_rows], got {action.dtype} {tuple(action.shape)}')
+  if action.shape[0] < 1:
+    raise ValueError('player_actions[\'action\']: no rows')
+  for name, t in (('row_of_player', rmap), ('action', action)):
+    dev = torch.device(t.device)
+    if dev.type != 'cuda' or dev.index != device:
+      raise ValueError(f'player_actions[{name!r}]: on {dev}, the engine runs on cuda:{device}')
+  s = MpPlayerActions()
+  s.row_of_player = ctypes.c_void_p(int(rmap.data_ptr))
+  s.n_rows = int(action.shape[0])
+  s.action = ctypes.c_void_p(int(action.data_ptr))
+  s.action_row_stride = (action.stride[0] if action.shape[0] > 1 else 1) * 4  # with one row the stride is never used
+  return s
+
+
 class TensorLayout(NamedTuple):
   """What describe_outputs needs of a tensor: shape and strides in elements, dtype, device and address."""
   shape: Tuple[int, ...]
@@ -284,6 +320,8 @@ def load_library() -> ctypes.CDLL:
   lib.mp_step_players.argtypes = [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(MpDeviceOutputs),
                                   ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_reset_players.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
+  lib.mp_step_routed.argtypes = [vp, ctypes.POINTER(MpPlayerActions), vp, vp, ctypes.c_int, ctypes.c_uint32,
+                                 ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
   lib.mp_step_host_async.argtypes = [vp, vp, ctypes.POINTER(MpHostOutputs), ctypes.c_int, vp]
@@ -491,8 +529,9 @@ class Engine:
       s = self._device_outputs(out)
       _check(self._lib.mp_reset_into(self._h, ptr, ctypes.byref(s), self._stream(stream)))
 
-  def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False, players=None) -> None:
-    """actions: int32 CUDA tensor [B, P] of discrete action ids.
+  def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False, players=None,
+           player_actions=None) -> None:
+    """actions: int32 CUDA tensor [B, P] of discrete action ids, or None with player_actions.
 
     out: {name: CUDA tensor} for any of DEVICE_OUTPUTS (mp_step_into): the step's images are rendered straight into
     out['rgb'] / out['world_rgb'] instead of this engine's own image buffers, and its scalars are written into the
@@ -512,21 +551,28 @@ class Engine:
     of env b is delivered to row row_of_player[b, p] when that lies in 0..n_rows-1, and nowhere otherwise; with 'rgb'
     the images are drawn straight into the rows, an unrouted player is not drawn at all and this engine's own rgb is
     not written. Combines with out (whose rgb it replaces) and with restore / bank. The row map's values are never
-    checked on the host; two players routed to one row leave one of them there."""
+    checked on the host; two players routed to one row leave one of them there.
+
+    player_actions: actions read from rows (mp_step_routed), {'row_of_player': contiguous CUDA int32 [B, P],
+    'action': CUDA int32 [n_rows], any stride}, with actions None. Player p of env b takes action[row_of_player[b, p]]
+    when that row lies in 0..n_rows-1, and action 0 (NOOP) otherwise. The row map may be players' own. Combines with
+    out, players and restore / bank; the result is that of the same call with the dense actions those rows give."""
+    if player_actions is not None:
+      if actions is not None:
+        raise ValueError('give actions or player_actions, not both')
+      pa = describe_player_actions({k: (None if v is None else layout_of(v)) for k, v in player_actions.items()},
+                                   self.num_envs, self.num_players, self.device)
+      flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
+      s = None if out is None else ctypes.byref(self._device_outputs(out))
+      p = None if players is None else ctypes.byref(self._player_outputs(players))
+      _check(self._lib.mp_step_routed(self._h, ctypes.byref(pa), idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, p,
+                                      self._stream(stream)))
+      return
+    if actions is None:
+      raise ValueError('actions is None: give actions, or player_actions')
     self._check_actions(actions)
     if players is not None:
-      flags, idx, bank_ptr, n_slots = 0, None, None, 0
-      if restore is not None or bank is not None:
-        if restore is None or bank is None:
-          raise ValueError('restore and bank go together')
-        bank = self._bank(bank)
-        idx = self._indices(restore, self.num_envs, 'restore')
-        for name, t in (('bank', bank), ('restore', idx)):
-          if t.device.index != self.device:
-            raise ValueError(f'{name} is on {t.device}, the engine runs on cuda:{self.device}')
-        flags, bank_ptr, n_slots, idx = (MP_RESTORE_REKEY if rekey else 0), ctypes.c_void_p(bank.data_ptr()), int(bank.shape[0]), ctypes.c_void_p(idx.data_ptr())
-      elif rekey:
-        raise ValueError('rekey needs restore and bank')
+      flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
       s = None if out is None else ctypes.byref(self._device_outputs(out))
       _check(self._lib.mp_step_players(self._h, ctypes.c_void_p(actions.data_ptr()), idx, bank_ptr, n_slots, ctypes.c_uint32(flags),
                                        s, ctypes.byref(self._player_outputs(players)), self._stream(stream)))
@@ -551,6 +597,21 @@ class Engine:
     else:
       s = self._device_outputs(out)
       _check(self._lib.mp_step_into(self._h, ctypes.c_void_p(actions.data_ptr()), ctypes.byref(s), self._stream(stream)))
+
+  def _restore_args(self, restore, bank, rekey):
+    """flags, index pointer, bank pointer and slot count of restore / bank (None, None, 0 without them)."""
+    if restore is None and bank is None:
+      if rekey:
+        raise ValueError('rekey needs restore and bank')
+      return 0, None, None, 0
+    if restore is None or bank is None:
+      raise ValueError('restore and bank go together')
+    bank = self._bank(bank)
+    idx = self._indices(restore, self.num_envs, 'restore')
+    for name, t in (('bank', bank), ('restore', idx)):
+      if t.device.index != self.device:
+        raise ValueError(f'{name} is on {t.device}, the engine runs on cuda:{self.device}')
+    return (MP_RESTORE_REKEY if rekey else 0), ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(bank.data_ptr()), int(bank.shape[0])
 
   def output_views(self):
     """name -> (shape, dtype) of the engine's own view of each output a step can deliver into caller tensors."""

@@ -7,10 +7,10 @@ SURVEY.md section 8f, row N2. Mirrors `meltingpot/utils/scenarios/scenario.py`:
     error texts. The background population is any object with the reference `Population`
     surface used here: `await_action()`, `send_timestep(timestep)`, `reset()`, `close()`
     (`utils/policies/...` SavedModel bots are out of scope and stay external).
-  * `BatchedScenario` — the same split as tensor ops over B env instances: focal / background
-    slots are index tensors, per-player observations are `index_select`ed on the player axis,
-    actions are scattered back into the full [B, P] action tensor. The background policy is a
-    callable on the background `BatchedTimeStep`.
+  * `BatchedScenario` — the same split over B env instances on player routes: focal players are
+    group 0 and background players group 1 of `BatchedSubstrate.player_routes`, so each step draws
+    their observations straight into focal and background rows and reads their actions from rows
+    laid out the same way. The background policy is a callable on the background `BatchedTimeStep`.
 
 Scenario configs (`meltingpot/configs/scenarios`) name SavedModel bots and are not compiled here.
 """
@@ -150,11 +150,16 @@ class BatchedScenario:
 
   `background_policy(background_timestep) -> int tensor [B, n_background]` is called once per
   step with the timestep the background players see (all their observations, unrestricted).
+
+  Focal and background players are routed (`BatchedSubstrate.player_routes`): every step renders their images, rewards
+  and scalar observations straight into rows of new tensors, focal rows first, each group laid out [B, n, ...] in slot
+  order, and reads their actions from rows laid out the same way. A returned timestep's per-player tensors therefore
+  stay valid after the next step.
   """
 
   def __init__(self, substrate: substrate_lib.BatchedSubstrate, background_policy: Callable[[Any], Any],
                is_focal: Sequence[bool], permitted_observations: Collection[str]) -> None:
-    import torch  # pylint: disable=g-import-not-at-top
+    import numpy as np  # pylint: disable=g-import-not-at-top
     if len(is_focal) != substrate.num_players:
       raise ValueError(f'is_focal is length {len(is_focal)} but substrate is '
                        f'{substrate.num_players}-player.')
@@ -162,40 +167,59 @@ class BatchedScenario:
     self._policy = background_policy
     self._is_focal = tuple(bool(f) for f in is_focal)
     self._permitted = frozenset(permitted_observations)
-    device = substrate.engine.rgb.device
-    self._focal_idx = torch.tensor([i for i, f in enumerate(self._is_focal) if f], dtype=torch.long, device=device)
-    self._background_idx = torch.tensor([i for i, f in enumerate(self._is_focal) if not f], dtype=torch.long, device=device)
-    self._actions = torch.zeros((substrate.num_envs, substrate.num_players), dtype=torch.int32, device=device)
     self._background_timestep = None
     self.num_envs = substrate.num_envs
-    self.num_focal = int(self._focal_idx.numel())
-    self.num_background = int(self._background_idx.numel())
+    self.num_focal = sum(self._is_focal)
+    self.num_background = substrate.num_players - self.num_focal
+    groups = np.tile(np.array([0 if f else 1 for f in self._is_focal], np.int64), (self.num_envs, 1))
+    self._routes = substrate.player_routes(groups)
+    self._actions = self._routes.actions()
+    n = self._routes.n_rows  # every player is routed: B * P rows, focal rows first
+    self._focal_rows, self._background_rows = slice(0, self.num_envs * self.num_focal), slice(self.num_envs * self.num_focal, n)
 
-  def _select(self, timestep, idx, permitted):
+  def _outputs(self):
+    """Fresh row tensors for one step (every row is written, so they are not zeroed)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    r = self._routes
+    dev = r.device
+    tensors = {'RGB': torch.empty((r.n_rows,) + tuple(self._substrate.engine.rgb.shape[2:]), dtype=torch.uint8, device=dev),
+               'REWARD': torch.empty((r.n_rows,), dtype=torch.float64, device=dev)}
+    names = self._substrate._scalar_names  # pylint: disable=protected-access
+    block = torch.empty((len(names), r.n_rows), dtype=torch.float64, device=dev) if names else None
+    for k, name in enumerate(names):
+      tensors[name] = block[k]
+    return substrate_lib.PlayerOutputs(r, None, tensors, block)
+
+  def _select(self, timestep, po, rows, n, permitted):
+    def view(v):
+      return v[rows].view((self.num_envs, n) + tuple(v.shape[1:]))
     obs = {}
-    for key, value in timestep.observation.items():
+    for key in ('RGB',) + tuple(timestep.observation):  # a routed timestep has no 'RGB': the rows hold the images
       if permitted is not None and key not in permitted:
         continue
-      obs[key] = value if key in _GLOBAL_KEYS else value.index_select(1, idx)
-    return substrate_lib.BatchedTimeStep(step_type=timestep.step_type, reward=timestep.reward.index_select(1, idx),
+      obs[key] = timestep.observation[key] if key in _GLOBAL_KEYS else view(po[key])
+    return substrate_lib.BatchedTimeStep(step_type=timestep.step_type, reward=view(po['REWARD']),
                                          discount=timestep.discount, observation=obs)
 
-  def _split(self, timestep):
-    self._background_timestep = self._select(timestep, self._background_idx, None)
-    return self._select(timestep, self._focal_idx, self._permitted)
+  def _split(self, timestep, po):
+    self._background_timestep = self._select(timestep, po, self._background_rows, self.num_background, None)
+    return self._select(timestep, po, self._focal_rows, self.num_focal, self._permitted)
 
   def reset(self):
-    return self._split(self._substrate.reset())
+    po = self._outputs()
+    return self._split(self._substrate.reset(players=po), po)
 
   def step(self, focal_actions):
     """focal_actions: int tensor [B, num_focal]; returns the focal players' BatchedTimeStep."""
     if tuple(focal_actions.shape) != (self.num_envs, self.num_focal):
       raise ValueError(f'Expected {self.num_focal} focal actions per env, got shape {tuple(focal_actions.shape)}.')
-    self._actions.index_copy_(1, self._focal_idx, focal_actions.to(self._actions.dtype))
+    rows = self._actions.tensor
+    rows[self._focal_rows].view(self.num_envs, self.num_focal).copy_(focal_actions)
     if self.num_background:
       background_actions = self._policy(self._background_timestep)
-      self._actions.index_copy_(1, self._background_idx, background_actions.to(self._actions.dtype))
-    return self._split(self._substrate.step(self._actions))
+      rows[self._background_rows].view(self.num_envs, self.num_background).copy_(background_actions)
+    po = self._outputs()
+    return self._split(self._substrate.step(players=po, player_actions=self._actions), po)
 
   @property
   def background_timestep(self):

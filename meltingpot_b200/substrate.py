@@ -260,9 +260,10 @@ class BatchedSubstrate:
     return PlayerRoutes(groups, self.num_envs, self.num_players, tuple(self._engine.rgb.shape[2:]), self._scalar_names,
                         torch.device('cuda', self._engine.device))
 
-  def step(self, actions, out: Optional[BatchedTimeStep] = None, restore=None, bank=None,
-           rekey: bool = False, players: Optional['PlayerOutputs'] = None) -> BatchedTimeStep:
-    """actions: integer tensor [B, P] on the engine's device (int32 preferred).
+  def step(self, actions=None, out: Optional[BatchedTimeStep] = None, restore=None, bank=None,
+           rekey: bool = False, players: Optional['PlayerOutputs'] = None,
+           player_actions: Optional['PlayerActions'] = None) -> BatchedTimeStep:
+    """actions: integer tensor [B, P] on the engine's device (int32 preferred), or None with player_actions.
 
     out: a BatchedTimeStep of caller-owned tensors to fill and return instead of views of the engine's buffers, e.g.
     `trajectory(T).at(t)`: the engine renders the images straight into it and delivers the scalars there too, so a
@@ -277,19 +278,32 @@ class BatchedSubstrate:
     players: a PlayerOutputs (`player_routes(groups).outputs()`, or `.at(t)` of one with T slots): each routed
     player's image, reward and scalar observations go to its row, the images drawn straight there; unrouted players are
     not drawn. The returned timestep then has no 'RGB'; every other field is as without players. Combines with out and
-    restore / bank."""
+    restore / bank.
+
+    player_actions: a PlayerActions (`player_routes(groups).actions()`, or `.at(t)` of one with T slots), with actions
+    None: each routed player takes the action in its row, an unrouted player action 0 (NOOP). The routes may be the
+    players' own, so a learner reads observations from rows and writes actions into the same rows. Combines with out,
+    players and restore / bank."""
     import torch  # pylint: disable=g-import-not-at-top
-    if actions.dtype != torch.int32:
-      actions = actions.to(torch.int32)
     kw = dict(restore=restore, bank=bank, rekey=rekey)
+    if player_actions is not None:
+      if actions is not None:
+        raise ValueError('give actions or player_actions, not both')
+      kw['player_actions'] = self._routed_actions(player_actions)
+    else:
+      if actions is None:
+        raise ValueError('actions is None: give actions, or player_actions')
+      if actions.dtype != torch.int32:
+        actions = actions.to(torch.int32)
+      actions = actions.contiguous()
     if players is not None:
-      self._engine.step(actions.contiguous(), out=None if out is None else self._engine_outputs(out, routed=players),
+      self._engine.step(actions, out=None if out is None else self._engine_outputs(out, routed=players),
                         players=self._routed_outputs(players), **kw)
       return self._without_rgb(self._timestep() if out is None else self._fill_collective(out))
     if out is None:
-      self._engine.step(actions.contiguous(), **kw)
+      self._engine.step(actions, **kw)
       return self._timestep()
-    self._engine.step(actions.contiguous(), out=self._engine_outputs(out), **kw)
+    self._engine.step(actions, out=self._engine_outputs(out), **kw)
     return self._fill_collective(out)
 
   def trajectory(self, T: int, time_major: bool = True) -> 'Trajectory':
@@ -304,14 +318,26 @@ class BatchedSubstrate:
     """The engine's per-player targets of a PlayerOutputs (the scalar observations as one [n, n_rows] view)."""
     if not isinstance(po, PlayerOutputs):
       raise ValueError('players must be a PlayerOutputs (player_routes(groups).outputs())')
-    import torch  # pylint: disable=g-import-not-at-top
     r = po.routes
-    if (r.num_envs, r.num_players) != (self.num_envs, self.num_players) or r.device != torch.device('cuda', self._engine.device):
-      raise ValueError(f'players: routes of {r.num_envs} envs x {r.num_players} players on {r.device}, this batch has '
-                       f'{self.num_envs} x {self.num_players} on cuda:{self._engine.device}')
+    self._check_routes(r, 'players')
     if po.T is not None:
       raise ValueError('players: pick one slot of a PlayerOutputs with T slots (outputs(T).at(t))')
     return {'row_of_player': r.row_of_player, 'rgb': po['RGB'], 'reward': po['REWARD'], 'scalar_obs': po.scalar_block}
+
+  def _check_routes(self, r: 'PlayerRoutes', what: str) -> None:
+    import torch  # pylint: disable=g-import-not-at-top
+    if (r.num_envs, r.num_players) != (self.num_envs, self.num_players) or r.device != torch.device('cuda', self._engine.device):
+      raise ValueError(f'{what}: routes of {r.num_envs} envs x {r.num_players} players on {r.device}, this batch has '
+                       f'{self.num_envs} x {self.num_players} on cuda:{self._engine.device}')
+
+  def _routed_actions(self, pa: 'PlayerActions'):
+    """The engine's player_actions of a PlayerActions."""
+    if not isinstance(pa, PlayerActions):
+      raise ValueError('player_actions must be a PlayerActions (player_routes(groups).actions())')
+    self._check_routes(pa.routes, 'player_actions')
+    if pa.T is not None:
+      raise ValueError('player_actions: pick one slot of a PlayerActions with T slots (actions(T).at(t))')
+    return {'row_of_player': pa.routes.row_of_player, 'action': pa.tensor}
 
   @staticmethod
   def _without_rgb(ts: BatchedTimeStep) -> BatchedTimeStep:
@@ -456,9 +482,10 @@ class PlayerRoutes:
   contiguous block, `rows(g)`. The assignment is validated once, here, on the host; the device tensors are then used as
   they are by every step.
     row_of_player  int32 CUDA [B, P]: the row of each player, -1 if unrouted (what the engine reads);
-    env_of_row, player_of_row  int64 CUDA [n_rows]: the env and player of each row, e.g. to scatter per-row actions
-      into the [B, P] actions of a step: actions[env_of_row, player_of_row] = row_actions.
-  Do not write to these tensors: they are shared by every PlayerOutputs made from this object."""
+    env_of_row, player_of_row  int64 CUDA [n_rows]: the env and player of each row.
+  Actions go the same way: `actions(T)` gives rows a step reads its actions from (step(player_actions=)), laid out
+  like the outputs' rows, so nothing is scattered back into [B, P].
+  Do not write to these tensors: they are shared by every PlayerOutputs and PlayerActions made from this object."""
 
   __slots__ = ('num_envs', 'num_players', 'num_groups', 'n_rows', 'device', 'row_of_player', 'env_of_row', 'player_of_row',
                '_starts', '_rgb_shape', '_scalar_names')
@@ -509,6 +536,10 @@ class PlayerRoutes:
     and `at(t)` is slot t."""
     return PlayerOutputs(self, T)
 
+  def actions(self, T: Optional[int] = None) -> 'PlayerActions':
+    """A zeroed int32 CUDA tensor of actions, one per row: [n_rows], or [T, n_rows] with T, whose `at(t)` is slot t."""
+    return PlayerActions(self, T)
+
 
 class PlayerOutputs:
   """Caller-owned CUDA tensors for the routed outputs of PlayerRoutes (routes.outputs(T)); `po[name]` is one of them.
@@ -555,6 +586,36 @@ class PlayerOutputs:
     if self.T is None:
       return {k: v[r] for k, v in self.tensors.items()}
     return {k: v[:, r] for k, v in self.tensors.items()}
+
+
+class PlayerActions:
+  """Caller-owned CUDA rows of actions for PlayerRoutes (routes.actions(T)): `tensor` is int32 [n_rows], or
+  [T, n_rows] with T slots. Write row r's action id into tensor[r] and pass this (or, with T slots, `at(t)`) to
+  BatchedSubstrate.step as player_actions=; `group(g)` is the view of group g's rows."""
+
+  def __init__(self, routes: PlayerRoutes, T: Optional[int] = None, tensor=None):
+    import torch  # pylint: disable=g-import-not-at-top
+    self.routes, self.T = routes, T
+    if tensor is not None:  # a view (at)
+      self.tensor = tensor
+      return
+    if T is not None and T < 1:
+      raise ValueError(f'actions need T >= 1 slots, got {T}')
+    lead = (routes.n_rows,) if T is None else (int(T), routes.n_rows)
+    self.tensor = torch.zeros(lead, dtype=torch.int32, device=routes.device)
+
+  def at(self, t: int) -> 'PlayerActions':
+    """Slot t of actions made with T slots, as a view."""
+    if self.T is None:
+      raise ValueError('at() needs actions made with T slots')
+    if not -self.T <= t < self.T:
+      raise IndexError(f'slot {t} of {self.T}')
+    return PlayerActions(self.routes, None, self.tensor[t])
+
+  def group(self, g: int):
+    """View of group g's rows ([rows], or [T, rows] with T slots)."""
+    r = self.routes.rows(g)
+    return self.tensor[r] if self.T is None else self.tensor[:, r]
 
 
 # ---------------------------------------------------------------------------------------------
