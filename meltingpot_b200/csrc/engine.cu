@@ -306,24 +306,27 @@ struct MapVariant {
   const int32_t* spawn_init_cell[2];
   int n_spawn, n_spawn_init[2];
   int avatar_sprite[MP_MAX_PLAYERS];
+  const uint8_t* cell_flags;  // [cells_pad] BeamBlocker bits
 };
 void apply_map(Tables& T, const MapVariant& M) {
-  T.init_grid = M.init_grid; T.solid = M.solid; T.spawn_cell = M.spawn_cell; T.n_spawn = M.n_spawn;
+  T.init_grid = M.init_grid; T.solid = M.solid; T.spawn_cell = M.spawn_cell; T.n_spawn = M.n_spawn; T.cell_flags = M.cell_flags;
   for (int k = 0; k < 2; ++k) { T.spawn_init_cell[k] = M.spawn_init_cell[k]; T.n_spawn_init[k] = M.n_spawn_init[k]; }
   memcpy(T.avatar_sprite, M.avatar_sprite, sizeof M.avatar_sprite);
 }
 
 // The map of one blob, which apply_map puts into a Tables: its initial grid padded to cells_pad, the static occupancy of
 // the avatar layer (non-avatar pieces that start there), the cells of the respawn group and of the initial spawn groups,
-// and the avatars' sprites. `T` holds the geometry and the avatar tables of the engine, `groups` the respawn group and
-// the two initial groups (or -1).
+// the avatars' sprites and the BeamBlocker bits of each cell (its walls). `T` holds the geometry and the avatar tables of
+// the engine, `groups` the respawn group and the two initial groups (or -1).
 // build_tables takes variant 0's map into the Tables; a map-variant engine keeps every variant's (setup_variants).
 int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], std::vector<void*>& allocs, MapVariant& M) {
   Section<int32_t> meta, objects, kinds, states, av_table;
   Section<uint16_t> init_grid;
+  Section<uint8_t> cell_flags;
   if (!get_section(blob, n, "meta", MPB_I32, &meta) || !get_section(blob, n, "objects", MPB_I32, &objects) ||
       !get_section(blob, n, "kinds", MPB_I32, &kinds) || !get_section(blob, n, "states", MPB_I32, &states) ||
-      !get_section(blob, n, "av_table", MPB_I32, &av_table) || !get_section(blob, n, "init_grid", MPB_U16, &init_grid))
+      !get_section(blob, n, "av_table", MPB_I32, &av_table) || !get_section(blob, n, "init_grid", MPB_U16, &init_grid) ||
+      !get_section(blob, n, "cell_flags", MPB_U8, &cell_flags))
     return fail(MP_E_INVALID, "blob: missing map sections");
   if (init_grid.count < (size_t)T.L * T.cells) return fail(MP_E_INVALID, "blob: 'init_grid' has %zu cells (expected %d)", init_grid.count, T.L * T.cells);
   char name[64];
@@ -355,8 +358,12 @@ int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], s
     const int32_t* st = states.data + (kd[MPB_KIND_STATE0] + od[MPB_OBJ_STATE]) * MPB_STATE_COLS;
     if (st[MPB_STATE_LAYER] == T.avatar_layer) solid[od[MPB_OBJ_Y] * T.W + od[MPB_OBJ_X]] = 255;
   }
+  std::vector<uint8_t> flags(T.cells_pad, 0);
+  memcpy(flags.data(), cell_flags.data, std::min<size_t>(cell_flags.count, T.cells));
   int rc;
-  if ((rc = upload(allocs, grid0, &M.init_grid)) || (rc = upload(allocs, cells[0], &M.spawn_cell)) || (rc = upload(allocs, solid, &M.solid))) return rc;
+  if ((rc = upload(allocs, grid0, &M.init_grid)) || (rc = upload(allocs, cells[0], &M.spawn_cell)) || (rc = upload(allocs, solid, &M.solid)) ||
+      (rc = upload(allocs, flags, &M.cell_flags)))
+    return rc;
   for (int k = 0; k < 2; ++k) {
     if (cells[1 + k].empty()) { M.spawn_init_cell[k] = M.spawn_cell; continue; }
     if ((rc = upload(allocs, cells[1 + k], &M.spawn_init_cell[k]))) return rc;
@@ -371,13 +378,13 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   const size_t n = blob_sizes[0];
   Section<int32_t> meta, states, kinds, comps, objects, hits, action_table, sprite_map, scalar_obs, av_table;
   Section<double> comps_f;
-  Section<uint8_t> atlas, sprite_opaque, cell_flags;
+  Section<uint8_t> atlas, sprite_opaque;
   Section<uint16_t> init_grid;
   if (!get_section(blob, n, "meta", MPB_I32, &meta) || meta.count < MPB_META_COUNT) return fail(MP_E_INVALID, "blob: missing/invalid 'meta' (not an MPB%u blob?)", MPB_VERSION);
 #define NEED(sec, dt) if (!get_section(blob, n, #sec, dt, &sec)) return fail(MP_E_INVALID, "blob: missing section '%s'", #sec);
   NEED(states, MPB_I32) NEED(kinds, MPB_I32) NEED(comps, MPB_I32) NEED(comps_f, MPB_F64) NEED(objects, MPB_I32) NEED(hits, MPB_I32)
   NEED(action_table, MPB_I32) NEED(sprite_map, MPB_I32) NEED(scalar_obs, MPB_I32) NEED(av_table, MPB_I32)
-  NEED(atlas, MPB_U8) NEED(sprite_opaque, MPB_U8) NEED(cell_flags, MPB_U8) NEED(init_grid, MPB_U16)
+  NEED(atlas, MPB_U8) NEED(sprite_opaque, MPB_U8) NEED(init_grid, MPB_U16)
   const int32_t* m = meta.data;
   Tables& T = E->T;
   T.W = m[MPB_META_W]; T.H = m[MPB_META_H]; T.cells = T.W * T.H; T.cells_pad = round_up(T.cells, 8);
@@ -450,9 +457,6 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   // ---- device copies -----------------------------------------------------------------------------
   std::vector<int32_t> act(action_table.data, action_table.data + action_table.count);
   if ((rc = upload(E->allocs, act, &T.action_table))) return rc;
-  std::vector<uint8_t> flags(T.cells_pad, 0);
-  memcpy(flags.data(), cell_flags.data, std::min<size_t>(cell_flags.count, T.cells));
-  if ((rc = upload(E->allocs, flags, &T.cell_flags))) return rc;
 
   // ---- render tables ------------------------------------------------------------------------------
   if (atlas.count != (size_t)T.n_sprites * 1024) return fail(MP_E_INVALID, "atlas has %zu bytes, expected %d", atlas.count, T.n_sprites * 1024);
@@ -1063,11 +1067,13 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
 }
 
 // Rule (a) of mp_create_variants: variant `v` has the same sections as variant 0, byte for byte, except the family's
-// parameter blocks, the component tables and the metadata string. The variants of a family with map variants (draws of
-// one builder compiled as a draw set; `map_sections` lists the family's entity tables, null for other families) may
-// also differ in their map: the initial grid, the object table, the spawn points and those entity tables, and in three
-// columns: the object count of 'meta', the sprite of each state and the sprite of each avatar. The sprite table itself
-// (atlas, sprite_opaque, sprite_map) stays identical.
+// parameter blocks, the component tables and the metadata string. The variants of a family with map variants (maps
+// compiled as one set on one sprite table; `map_sections` lists the family's entity tables, null for other families) may
+// also differ in their map: the initial grid, the object table, the kind and state tables, the BeamBlocker bits, the
+// spawn points and those entity tables, in the object, kind, state and component counts of 'meta', and in the sprite of
+// each avatar. The kind and state tables are only read per blob, by load_map and the pre-merge enumeration of
+// build_tables, never from variant 0 for every env. The sprite table itself (atlas, sprite_opaque, sprite_map) stays
+// identical.
 int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const char* const* map_sections) {
   const bool maps = map_sections != nullptr;
   const MpbHeader* h0 = static_cast<const MpbHeader*>(b0);
@@ -1081,17 +1087,21 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
         !strcmp(name, "comps_f") || !strcmp(name, "info_json"))
       return true;
     if (!maps) return false;
-    if (!strcmp(name, "init_grid") || !strcmp(name, "objects") || !strncmp(name, "spawn_cells_", 12)) return true;
+    if (!strcmp(name, "init_grid") || !strcmp(name, "objects") || !strcmp(name, "kinds") || !strcmp(name, "states") ||
+        !strcmp(name, "cell_flags") || !strncmp(name, "spawn_cells_", 12))
+      return true;
     for (const char* const* t = map_sections; *t; ++t) if (!strcmp(name, *t)) return true;
     return false;
   };
-  // map variants: the one column of an int32 section that may differ (of `cols`), or -1
-  auto free_column = [maps](const char* name, int* cols) {
-    if (!maps) return -1;
-    if (!strcmp(name, "meta")) { *cols = MPB_META_COUNT; return (int)MPB_META_N_OBJECTS; }
-    if (!strcmp(name, "states")) { *cols = MPB_STATE_COLS; return (int)MPB_STATE_SPRITE; }
-    if (!strcmp(name, "av_table")) { *cols = 8; return 1; }
-    return -1;
+  // map variants: the columns of an int32 section that may differ (a bit per column, of `cols`), or 0
+  auto free_columns = [maps](const char* name, int* cols) -> uint64_t {
+    if (!maps) return 0;
+    if (!strcmp(name, "meta")) {
+      *cols = MPB_META_COUNT;
+      return 1ull << MPB_META_N_OBJECTS | 1ull << MPB_META_N_KINDS | 1ull << MPB_META_N_STATES | 1ull << MPB_META_N_COMPS;
+    }
+    if (!strcmp(name, "av_table")) { *cols = 8; return 1ull << 1; }
+    return 0;
   };
   static const char* const kMetaNames[] = {"family", "W", "H", "layers", "players", "sprite size", "topology", "max frames", "objects",
                                            "kinds", "states", "comps", "sprites", "hits", "groups", "view left", "view right",
@@ -1108,12 +1118,12 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
       const bool same_shape = t && t->dtype == s[i].dtype && t->ndim == s[i].ndim && memcmp(t->shape, s[i].shape, sizeof t->shape) == 0 &&
                               t->nbytes == s[i].nbytes;
       int cols = 0;
-      const int col = free_column(name, &cols);
-      if (same_shape && col >= 0 && s[i].dtype == MPB_I32) {
+      const uint64_t free_cols = free_columns(name, &cols);
+      if (same_shape && free_cols && s[i].dtype == MPB_I32) {
         const int32_t* x = static_cast<const int32_t*>(mpb_data(own, &s[i]));
         const int32_t* y = static_cast<const int32_t*>(mpb_data(other, t));
         for (size_t k = 0; k < s[i].nbytes / 4; ++k) {
-          if ((int)(k % cols) == col || x[k] == y[k]) continue;
+          if ((free_cols >> (k % cols) & 1u) || x[k] == y[k]) continue;
           if (!strcmp(name, "meta") && k < sizeof kMetaNames / sizeof *kMetaNames)
             return fail(MP_E_UNSUPPORTED, "section 'meta' differs in field '%s' (%d vs %d)", kMetaNames[k], x[k], y[k]);
           return fail(MP_E_UNSUPPORTED, "section '%s' differs in value %zu (column %zu)", name, k, k % cols);
@@ -1133,6 +1143,8 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
 // Rules (b)-(d) of mp_create_variants for an engine whose tables are built from variant 0 (build_tables), then the
 // variant set's device arrays. Runs before the engine's state is sized: a family with map variants keeps each variant's
 // map (MapVariant) and entity tables, and the State's entity arrays (T.nA_pad) are sized for the variant with the most.
+// Its variants may also differ in their beam footprints, as far as the family's same_shape allows (commons_harvest:
+// the Zapper's length and radius; coins has no beams), and State::max_events is sized for the largest footprint.
 int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host) {
   struct Decided { int nA, nD, nW, nR, nR_pad, end_min_frames, end_interval, beam_cells; double end_prob; std::vector<std::vector<int>> hints; };
   std::vector<FamilyParams> params(n);
@@ -1154,7 +1166,7 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
     if ((!maps && a.nA != b.nA) || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
     else if (a.end_min_frames != b.end_min_frames || a.end_interval != b.end_interval || memcmp(&a.end_prob, &b.end_prob, sizeof a.end_prob) != 0)
       rc = fail(MP_E_UNSUPPORTED, "episode ending differs");
-    else if (a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
+    else if (!maps && a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
     else if (a.hints != b.hints) rc = fail(MP_E_UNSUPPORTED, "pre-merged sprite hints differ");
     else rc = E->family->same_shape(params[0], params[v]);
     if (rc == MP_OK && maps) rc = load_map(blobs[v], blob_bytes[v], T, E->spawn_groups, E->allocs, map[v]);
@@ -1163,7 +1175,7 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
   for (void* p : scratch) cudaFree(p);
   if (rc) return rc;
   if (maps) {
-    for (const Decided& dv : decided) T.nA = std::max(T.nA, dv.nA);
+    for (const Decided& dv : decided) { T.nA = std::max(T.nA, dv.nA); E->beam_cells = std::max(E->beam_cells, dv.beam_cells); }
     T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16);
     std::vector<Tables> tv(n, T);  // T is final here: create changes nothing in it after this
     for (int v = 0; v < n; ++v) { apply_map(tv[v], map[v]); tv[v].nA = decided[v].nA; }

@@ -59,9 +59,10 @@ __host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * 
 // Per-env parameter variants (mp_create_variants): env b runs under params[active[b]]. An episode start first takes the
 // env's pending assignment (active[b] = pending[b]), so a reassignment never changes an episode that is under way.
 // Every variant stages the same per-CTA tables (the compatibility check of mp_create_variants), so stage() reads params[0].
-// A family with kMapVariants (coins) also advances under maps[active[b]]: the engine's Tables with that variant's initial
-// grid, static occupancy, spawn points, avatar sprites and entity count (the State's entity arrays are sized for the
-// largest variant). The map is only ever read through the env's active variant, which changes at an episode start, so
+// A family with kMapVariants (coins, commons_harvest) also advances under maps[active[b]]: the engine's Tables with that
+// variant's initial grid, static occupancy, BeamBlocker bits, spawn points, avatar sprites and entity count (the State's
+// entity arrays are sized for the largest variant). Such a family may provide reset_map, which then starts the episodes
+// of map-variant engines instead of reset (commons_harvest: its reset writes only the map's own apples). The map is only ever read through the env's active variant, which changes at an episode start, so
 // an env's map changes there too and never mid-episode. The Tables are read from the device array through the L1: a
 // local copy of the kernel's Tables with the variant's fields swapped in would sit on the stack (392 bytes for coins,
 // since avatar_sprite is indexed by lane).
@@ -101,6 +102,11 @@ __device__ __forceinline__ const Actions& select_actions(const DenseActions& den
   if constexpr (std::is_same<Actions, RowActions>::value) return rows;
   else return dense;
 }
+
+template <class F, class = void>
+struct HasResetMap : std::false_type {};
+template <class F>
+struct HasResetMap<F, std::void_t<decltype(&F::reset_map)>> : std::true_type {};
 
 // A Family provides: Params (what only its kernel reads), the host-side load(FamilyLoad&, T, Params&) that decodes its
 // blob sections (family_load.h), Scratch, kStagesTables, kMapVariants (whether its variants may differ in the map, and
@@ -150,8 +156,10 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
       const typename Family::Params& F = src.params[k];
       if constexpr (Family::kMapVariants) {
         const Tables& Tm = src.maps[k];
-        if (reset) Family::reset(Tm, F, S, b, lane, sc);
-        else Family::template step<Actions>(Tm, F, S, b, lane, acts, sc);
+        if (reset) {
+          if constexpr (HasResetMap<Family>::value) Family::reset_map(Tm, F, S, b, lane, sc);
+          else Family::reset(Tm, F, S, b, lane, sc);
+        } else Family::template step<Actions>(Tm, F, S, b, lane, acts, sc);
       } else {
         if (reset) Family::reset(T, F, S, b, lane, sc);
         else Family::template step<Actions>(T, F, S, b, lane, acts, sc);

@@ -54,20 +54,29 @@ struct Commons {
     return MP_OK;
   }
 
-  // Host: per-env variants may differ in the Zapper knobs, the DensityRegrow probabilities and the Edible reward.
+  // Host: per-env variants may differ in the Zapper knobs and its beam footprint (length and radius), the DensityRegrow
+  // probabilities and the Edible reward, and, as maps of one set (map variants: commons_harvest__open, __closed and
+  // __partnership), in the apples, their regrowth discs and the walls.
   static int same_shape(const Params& a, const Params& b) {
-    MP_SAME_ZAPPER MP_SAME(apple_layer) MP_SAME(apple_sprite) MP_SAME(wait_layer) MP_SAME(wait_sprite) MP_SAME(grass_layer) MP_SAME(grass_sprite)
+    MP_SAME(zap.layer) MP_SAME(zap.sprite) MP_SAME(zap.hit) MP_SAME(apple_layer) MP_SAME(apple_sprite) MP_SAME(wait_layer) MP_SAME(wait_sprite) MP_SAME(grass_layer) MP_SAME(grass_sprite)
     MP_SAME(dess_sprite) MP_SAME(ch_n_wait) MP_SAME(ch_n_probs)
     return MP_OK;
   }
   static void copy_knobs(Params& dst, const Params& src) {
     copy_zapper_knobs(dst.zap, src.zap);
+    dst.zap.geom = src.zap.geom;
     for (int i = 0; i < 4; ++i) dst.ch_probs[i] = src.ch_probs[i];
     dst.eat_reward = src.eat_reward;
   }
+  static void copy_map(Params& dst, const Params& src) {
+    dst.ch_apple = src.ch_apple; dst.ch_nbr = src.ch_nbr; dst.apple_of_cell = src.apple_of_cell;
+  }
 
   using Scratch = WarpScratch;
-  static constexpr bool kMapVariants = false;
+  // Maps of one set may differ in their walls and apples (mp_create_variants): the apple table and the regrowth discs are
+  // their entity tables, and the apple count is the nA of each variant's Tables (setup_variants).
+  static constexpr bool kMapVariants = true;
+  static constexpr const char* kMapSections[] = {"ch_apple", "ch_nbr", nullptr};
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }
@@ -92,6 +101,14 @@ struct Commons {
       });
     }
     reset_env_row(T, S, b, lane, episode, 0);
+  }
+
+  // Episode start of an env of a map-variant engine: also zeroes the env's apple rows past this map's apples, up to the
+  // padding of the largest map, so that an env that moved from a map with more apples keeps none of their bytes (records
+  // and snapshots of equal envs stay equal byte for byte). A single-map engine never writes there.
+  __device__ static void reset_map(const Tables& T, const Params& F, const State& S, int b, int lane, WarpScratch& sc) {
+    for (int k = T.nA + lane; k < T.nA_pad; k += 32) { S.apple[(size_t)b * T.nA_pad + k] = 0; S.apple_count[(size_t)b * T.nA_pad + k] = 0; }
+    reset(T, F, S, b, lane, sc);
   }
 
   template <class Actions>

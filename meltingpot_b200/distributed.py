@@ -95,9 +95,9 @@ class ShardedSubstrate:
 
   def __init__(self, name: str, roles, global_num_envs: int, seed: int, device: Optional[int] = None,
                world_rgb: bool = True, group=None, prefab_overrides=None, env_variant=None, build_seeds=None):
-    """prefab_overrides / build_seeds / env_variant: as substrate.build_batched, with env_variant indexed by GLOBAL env;
-    each rank takes the slice of its own envs (with build_seeds and no env_variant, global env g plays draw
-    g % len(build_seeds))."""
+    """name / prefab_overrides / build_seeds / env_variant: as substrate.build_batched, with env_variant indexed by
+    GLOBAL env; each rank takes the slice of its own envs (with build_seeds, or a sequence of names, and no env_variant,
+    global env g plays variant g % len(build_seeds) or g % len(name))."""
     import torch.distributed as dist  # pylint: disable=g-import-not-at-top
     from meltingpot_b200 import substrate  # pylint: disable=g-import-not-at-top
     self._group = group

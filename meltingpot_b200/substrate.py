@@ -862,10 +862,18 @@ def draw_of_env(env_index_base: int, num_envs: int, num_draws: int) -> np.ndarra
   return (np.arange(env_index_base, env_index_base + num_envs) % num_draws).astype(np.int64)
 
 
-def build_batched(name: str, *, roles: Sequence[str], num_envs: int, device: int = 0,
+def build_batched(name, *, roles: Sequence[str], num_envs: int, device: int = 0,
                   seed: Optional[int] = None, env_index_base: int = 0,
                   world_rgb: bool = True, prefab_overrides=None, env_variant=None, build_seeds=None) -> BatchedSubstrate:
   """Builds `num_envs` instances on one GPU; see `BatchedSubstrate`.
+
+  `name` is a substrate name, or a sequence of substrate names whose maps the engine runs side by side, e.g.
+  ('commons_harvest__open', 'commons_harvest__closed', 'commons_harvest__partnership'): each name's blob is
+  load_blob(name, roles), and env b plays names[env_variant[b]], by default (env_index_base + b) % len(name). The names
+  are variants, so active_variant / pending_variant / set_env_variant index into the sequence and set_env_variant moves
+  an env to another map at its next episode. A name may repeat, which weights the default assignment. The names must
+  share the action set, observation names and timestep spec, and their blobs must form one map set (mp_create_variants
+  refuses another family, player count or map size); not combined with prefab_overrides or build_seeds.
 
   `prefab_overrides` (the reference builder's, builder.py:70-87) is one mapping for every env, or a sequence of
   mappings: a heterogeneous batch whose env b runs variant env_variant[b] (default 0). Compiling overrides needs a
@@ -875,6 +883,40 @@ def build_batched(name: str, *, roles: Sequence[str], num_envs: int, device: int
   make (coins draws its map size and its two coin colours on every build), compiled as one draw set. Env b plays
   draw env_variant[b], by default (env_index_base + b) % len(build_seeds); a draw is a variant, so set_env_variant
   moves an env to another draw at its next episode. Needs a reference checkout; not combined with prefab_overrides."""
+  if not isinstance(name, str):
+    return _build_map_set(tuple(name), roles=roles, num_envs=num_envs, device=device, seed=seed,
+                          env_index_base=env_index_base, world_rgb=world_rgb, prefab_overrides=prefab_overrides,
+                          env_variant=env_variant, build_seeds=build_seeds)
   return get_factory(name, device).build_batched(roles, num_envs, seed=seed, env_index_base=env_index_base,
                                                  world_rgb=world_rgb, prefab_overrides=prefab_overrides,
                                                  env_variant=env_variant, build_seeds=build_seeds)
+
+
+_SHARED_CONFIG_FIELDS = ('action_set', 'individual_observation_names', 'global_observation_names', 'timestep_spec')
+
+
+def _build_map_set(names: Sequence[str], *, roles, num_envs, device, seed, env_index_base, world_rgb, prefab_overrides,
+                   env_variant, build_seeds) -> BatchedSubstrate:
+  """build_batched over a sequence of substrate names: every argument is checked here, before an engine exists."""
+  if not names:
+    raise ValueError('the sequence of substrate names is empty')
+  if prefab_overrides is not None or build_seeds is not None:
+    raise ValueError('a sequence of substrate names takes neither prefab_overrides nor build_seeds')
+  configs = [get_config(n) for n in names]
+  for config in configs:
+    _validate_roles(config, roles)
+  for n, config in zip(names[1:], configs[1:]):
+    for field in _SHARED_CONFIG_FIELDS:
+      if config[field] != configs[0][field]:
+        raise ValueError(f'{n!r} differs from {names[0]!r} in its {field}')
+  if env_variant is None:
+    env_variant = draw_of_env(env_index_base, num_envs, len(names))
+  else:
+    env_variant = np.asarray(env_variant, np.int64).reshape(-1)
+    if env_variant.shape != (num_envs,):
+      raise ValueError(f'env_variant has {env_variant.size} entries for {num_envs} envs')
+    if env_variant.size and (env_variant.min() < 0 or env_variant.max() >= len(names)):
+      raise ValueError(f'env_variant must index the {len(names)} names (0..{len(names) - 1})')
+  blobs = [substrate_blobs.load_blob(n, tuple(roles)) for n in names]
+  return BatchedSubstrate(blobs, num_envs, device=device, seed=seed, env_index_base=env_index_base,
+                          world_rgb=world_rgb, env_variant=env_variant)
