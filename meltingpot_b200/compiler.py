@@ -1285,19 +1285,28 @@ def compile_settings(settings: Mapping[str, Any],
 
 def compile_settings_set(settings_list: Sequence[Mapping[str, Any]],
                          config: Optional[Any] = None,
-                         build_seeds: Optional[Sequence[Optional[int]]] = None) -> List[bytes]:
-  """A draw set: one blob per entry of `settings_list` (e.g. the builds of one substrate under several build seeds), all
-  on one sprite table. That table is the union of every entry's sprites, deduplicated by name and pixels, in
-  first-appearance order (SharedSprites), so the sprite-side sections (atlas, sprite_opaque, sprite_map, the
-  OutOfBounds / OutOfView ids) are byte-identical across the set, and an engine can run the blobs as per-env variants
-  (mp_create_variants). What differs is which sprite ids the states and avatars refer to, and whatever the map decides.
-  A set of one is compile_settings' blob, byte for byte. `build_seeds[i]` resolves entry i's 'choice' prefabs."""
+                         build_seeds: Optional[Sequence[Optional[int]]] = None,
+                         prefab_overrides: Optional[Sequence[Optional[Mapping[str, Any]]]] = None) -> List[bytes]:
+  """A draw set: one blob per entry of `settings_list` (e.g. the builds of one substrate under several build seeds, or
+  one build under several `prefab_overrides`), all on one sprite table. That table is the union of every entry's
+  sprites, deduplicated by name and pixels, in first-appearance order (SharedSprites), so the sprite-side sections
+  (atlas, sprite_opaque, sprite_map, the OutOfBounds / OutOfView ids) are byte-identical across the set, and an engine
+  can run the blobs as per-env variants (mp_create_variants). What differs is which sprite ids the states, avatars and
+  family tables refer to, and whatever the map decides. When no entry adds a sprite of its own (no appearance
+  override), each blob equals the entry compiled alone. A set of one is compile_settings' blob, byte for byte.
+  `build_seeds[i]` resolves entry i's 'choice' prefabs; `prefab_overrides[i]` is applied to entry i as
+  compile_settings applies it."""
   settings_list = list(settings_list)
   if not settings_list:
     raise ValueError('compile_settings_set needs at least one settings entry')
   seeds = list(build_seeds) if build_seeds is not None else [None] * len(settings_list)
   if len(seeds) != len(settings_list):
     raise ValueError(f'{len(seeds)} build seeds for {len(settings_list)} settings entries')
+  if prefab_overrides is not None:
+    prefab_overrides = list(prefab_overrides)
+    if len(prefab_overrides) != len(settings_list):
+      raise ValueError(f'{len(prefab_overrides)} prefab_overrides for {len(settings_list)} settings entries')
+    settings_list = [apply_prefab_overrides(s, o) if o else s for s, o in zip(settings_list, prefab_overrides)]
   own = [WorldModel(s, seed) for s, seed in zip(settings_list, seeds)]
   shared = SharedSprites(own[0].sprite_size)
   for model in own:
@@ -1417,18 +1426,20 @@ def compile_substrate(name: str, roles: Optional[Sequence[str]] = None,
 
 
 def compile_substrate_set(name: str, roles: Optional[Sequence[str]] = None,
-                          build_seeds: Sequence[int] = (0,),
-                          root: Optional[str] = None) -> List[bytes]:
-  """The draws of a named reference substrate under `build_seeds` (what compile_substrate returns for each seed) as a
-  draw set on one sprite table (compile_settings_set). Needs a reference checkout."""
+                          build_seeds: Sequence[Optional[int]] = (0,),
+                          root: Optional[str] = None,
+                          prefab_overrides: Optional[Sequence[Optional[Mapping[str, Any]]]] = None) -> List[bytes]:
+  """The builds of a named reference substrate under `build_seeds` and `prefab_overrides` (what compile_substrate
+  returns for each pair) as a draw set on one sprite table (compile_settings_set). Needs a reference checkout."""
   config = load_reference_config(name, root)
   roles = tuple(roles) if roles is not None else tuple(config.default_player_roles)
   settings_list = []
   state = random.getstate()
   try:
     for seed in build_seeds:
-      random.seed(seed)
+      if seed is not None:
+        random.seed(seed)
       settings_list.append(config.lab2d_settings_builder(roles=roles, config=config))
   finally:
     random.setstate(state)
-  return compile_settings_set(settings_list, config, list(build_seeds))
+  return compile_settings_set(settings_list, config, list(build_seeds), prefab_overrides)

@@ -138,7 +138,7 @@ struct VariantSet {
   uint8_t* active = nullptr;     // [B] the variant each env's current episode runs
   uint8_t* pending = nullptr;    // [B] the variant each env's next episode runs
   int n = 1;
-  const Tables* maps = nullptr;  // [n] the Tables of each variant's map (a family with map variants), else null
+  const Tables* maps = nullptr;  // [n] the Tables of each variant (its map, or for other families its initial grid)
 };
 // The launches take the restore of mp_step_restore, or null for the plain k_step, and the row actions of
 // mp_step_routed (then `actions` is unused), or null for dense actions.
@@ -146,6 +146,7 @@ struct FamilyEntry {
   int id;  // MpbFamily
   bool map_variants;  // Family::kMapVariants: its variants may be draws of different maps (mp_create_variants)
   const char* const* map_sections;  // then Family::kMapSections: its own entity tables, which such variants may differ in
+  const char* const* sprite_sections;  // Family::kSpriteSections: its int32 tables that hold nothing but sprite ids, or null
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
   cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int,
                         const StepRestore*, const RowActions*);
@@ -208,9 +209,18 @@ constexpr const char* const* map_sections() {
   if constexpr (Family::kMapVariants) return Family::kMapSections;
   else return nullptr;
 }
+template <class F, class = void>
+struct HasSpriteSections : std::false_type {};
+template <class F>
+struct HasSpriteSections<F, std::void_t<decltype(F::kSpriteSections)>> : std::true_type {};
+template <class Family>
+constexpr const char* const* sprite_sections() {
+  if constexpr (HasSpriteSections<Family>::value) return Family::kSpriteSections;
+  else return nullptr;
+}
 template <class Family>
 FamilyEntry family_entry(int id) {
-  return {id, Family::kMapVariants, map_sections<Family>(), load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
+  return {id, Family::kMapVariants, map_sections<Family>(), sprite_sections<Family>(), load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
           same_shape_family<Family>, upload_variants_family<Family>, launch_variants_family<Family>,
           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>),
           {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true>),
@@ -371,8 +381,10 @@ int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], s
   return MP_OK;
 }
 
-// The engine's tables from blob 0 of `blobs`. The pre-merged sprites cover the cell stacks of every blob: the variants
-// of a map-variant engine share one sprite table and the renderer's pre-merged pairs.
+// The engine's tables from blob 0 of `blobs`. The pre-merged sprites cover the cell stacks and the family's hint stacks
+// of every blob: the variants of an engine share one sprite table and the renderer's pre-merged pairs, and may differ in
+// their maps (map variants) or in the sprites their pieces show (appearance overrides). Variants that differ in neither
+// add no stack of their own, so their engine has the pre-merged sprites of blob 0 alone.
 int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_sizes, int n_blobs) {
   const void* blob = blobs[0];
   const size_t n = blob_sizes[0];
@@ -431,6 +443,18 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   // ---- family tables -----------------------------------------------------------------------------
   FamilyLoad ld{blob, n, hits, E->allocs};
   if ((rc = E->family->load(ld, T, E->params))) return rc;
+  std::vector<std::vector<int>> hint_stacks = ld.hint_stacks;
+  {  // every other variant's hint stacks (its loader's uploads are freed; setup_variants checks and loads it again)
+    std::vector<void*> scratch;
+    for (int v = 1; v < n_blobs; ++v) {
+      Section<int32_t> v_hits;
+      FamilyParams scratch_params;
+      if (!get_section(blobs[v], blob_sizes[v], "hits", MPB_I32, &v_hits)) continue;
+      FamilyLoad lv{blobs[v], blob_sizes[v], v_hits, scratch};
+      if (E->family->load(lv, T, scratch_params) == MP_OK) hint_stacks.insert(hint_stacks.end(), lv.hint_stacks.begin(), lv.hint_stacks.end());
+    }
+    for (void* p : scratch) cudaFree(p);
+  }
 #undef NEED
   T.nA = ld.nA; T.nD = ld.nD; T.nW = ld.nW; T.nR = ld.nR; T.nR_pad = ld.nR_pad;
   T.end_min_frames = ld.end_min_frames; T.end_interval = ld.end_interval; T.end_prob = ld.end_prob;
@@ -499,11 +523,9 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   {
     // Per blob: the sprites each (cell, layer) can show (opts_of) and the initial grid (init_of).
     struct Opt { std::vector<int> sprites; bool absent = false; int orient = -1; bool bad = false; };
-    // (the variants of other families have one map: rule (a) of mp_create_variants)
-    const int n_maps = E->family->map_variants ? n_blobs : 1;
-    std::vector<std::vector<Opt>> opts_of(n_maps, std::vector<Opt>((size_t)T.cells * T.L));
-    std::vector<const uint16_t*> init_of(n_maps);
-    for (int v = 0; v < n_maps; ++v) {
+    std::vector<std::vector<Opt>> opts_of(n_blobs, std::vector<Opt>((size_t)T.cells * T.L));
+    std::vector<const uint16_t*> init_of(n_blobs);
+    for (int v = 0; v < n_blobs; ++v) {
       Section<int32_t> v_meta, v_states, v_kinds, v_objects;
       Section<uint16_t> v_init;
       if (!get_section(blobs[v], blob_sizes[v], "meta", MPB_I32, &v_meta) || !get_section(blobs[v], blob_sizes[v], "states", MPB_I32, &v_states) ||
@@ -534,14 +556,14 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
         }
       }
     }
-    for (const auto& hs : ld.hint_stacks) {
+    for (const auto& hs : hint_stacks) {
       if (hs.empty() || !opq[hs[0]]) continue;
       int cur = hs[0];
       for (size_t q = 1; q < hs.size() && cur; ++q) { if (remapped[hs[q]] || remapped[cur]) break; cur = merged_id(cur, hs[q]); }
     }
     std::vector<int> stack_s, stack_o;
     for (int pass = 0; pass < 2; ++pass)  // pass 0: the maps as they are at reset (most common stacks) get the budget first
-    for (int v = 0; v < n_maps; ++v)        // (a map-variant engine: the stacks of every variant's map)
+    for (int v = 0; v < n_blobs; ++v)        // (the stacks of every variant's map)
     for (int cell = 0; cell < T.cells; ++cell) {
       const std::vector<Opt>& opts = opts_of[v];
       const uint16_t* init_grid = init_of[v];
@@ -1074,7 +1096,12 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
 // each avatar. The kind and state tables are only read per blob, by load_map and the pre-merge enumeration of
 // build_tables, never from variant 0 for every env. The sprite table itself (atlas, sprite_opaque, sprite_map) stays
 // identical.
-int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const char* const* map_sections) {
+// Variants of any family (one set on one sprite table: appearance overrides) may also differ in which sprite ids their
+// pieces use: the sprite column of 'states', the sprite of each non-empty cell of 'init_grid' (not which cells are
+// empty, nor their orientations) and the family's tables of sprite ids (`sprite_sections`), where a sprite may change
+// but not whether there is one. A section that differs in anything else is refused as before.
+int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const char* const* map_sections,
+                  const char* const* sprite_sections) {
   const bool maps = map_sections != nullptr;
   const MpbHeader* h0 = static_cast<const MpbHeader*>(b0);
   const MpbHeader* hv = static_cast<const MpbHeader*>(bv);
@@ -1109,6 +1136,31 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
                                            "OutOfView sprite", "scalar observations"};
   const MpbSection* s0 = reinterpret_cast<const MpbSection*>(h0 + 1);
   const MpbSection* sv = reinterpret_cast<const MpbSection*>(hv + 1);
+  // whether two sections of the same shape differ in sprite ids only
+  auto sprite_ids_only = [sprite_sections](const char* name, const MpbSection* s, const void* x, const void* y) {
+    const size_t n = s->nbytes / 4;
+    const int32_t* a = static_cast<const int32_t*>(x);
+    const int32_t* b = static_cast<const int32_t*>(y);
+    if (!strcmp(name, "init_grid") && s->dtype == MPB_U16) {
+      const uint16_t* p = static_cast<const uint16_t*>(x);
+      const uint16_t* q = static_cast<const uint16_t*>(y);
+      for (size_t k = 0; k < s->nbytes / 2; ++k)
+        if ((p[k] == 0) != (q[k] == 0) || (p[k] && ((p[k] - 1) & 3) != ((q[k] - 1) & 3))) return false;
+      return true;
+    }
+    if (s->dtype != MPB_I32) return false;
+    if (!strcmp(name, "states")) {
+      for (size_t k = 0; k < n; ++k)
+        if (k % MPB_STATE_COLS == MPB_STATE_SPRITE ? (a[k] < 0) != (b[k] < 0) : a[k] != b[k]) return false;
+      return true;
+    }
+    for (const char* const* t = sprite_sections; t && *t; ++t)
+      if (!strcmp(name, *t)) {
+        for (size_t k = 0; k < n; ++k) if ((a[k] < 0) != (b[k] < 0)) return false;
+        return true;
+      }
+    return false;
+  };
   auto check = [&](const MpbSection* s, uint32_t count, const void* other, size_t n_other, const void* own) -> int {
     for (uint32_t i = 0; i < count; ++i) {
       char name[MPB_NAME_LEN + 1] = {};
@@ -1117,6 +1169,7 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
       const MpbSection* t = mpb_find(other, n_other, name);
       const bool same_shape = t && t->dtype == s[i].dtype && t->ndim == s[i].ndim && memcmp(t->shape, s[i].shape, sizeof t->shape) == 0 &&
                               t->nbytes == s[i].nbytes;
+      if (same_shape && sprite_ids_only(name, &s[i], mpb_data(own, &s[i]), mpb_data(other, t))) continue;
       int cols = 0;
       const uint64_t free_cols = free_columns(name, &cols);
       if (same_shape && free_cols && s[i].dtype == MPB_I32) {
@@ -1145,14 +1198,16 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
 // map (MapVariant) and entity tables, and the State's entity arrays (T.nA_pad) are sized for the variant with the most.
 // Its variants may also differ in their beam footprints, as far as the family's same_shape allows (commons_harvest:
 // the Zapper's length and radius; coins has no beams), and State::max_events is sized for the largest footprint.
+// Every variant engine keeps the Tables of each variant (VariantSet::maps), from which an episode start reads: the
+// variants of the other families differ there in their initial grid only (the sprites of an appearance override).
 int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host) {
-  struct Decided { int nA, nD, nW, nR, nR_pad, end_min_frames, end_interval, beam_cells; double end_prob; std::vector<std::vector<int>> hints; };
+  struct Decided { int nA, nD, nW, nR, nR_pad, end_min_frames, end_interval, beam_cells; double end_prob; };
   std::vector<FamilyParams> params(n);
   std::vector<Decided> decided;
   const bool maps = E->family->map_variants;
   // the loaders' device uploads: every variant of a plain set uses the engine's own (same sections); map variants keep theirs
   std::vector<void*> scratch;
-  std::vector<MapVariant> map(maps ? n : 0);
+  std::vector<MapVariant> map(n);
   Tables& T = E->T;
   int rc = MP_OK;
   for (int v = 0; v < n && rc == MP_OK; ++v) {
@@ -1160,16 +1215,15 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
     if (!get_section(blobs[v], blob_bytes[v], "hits", MPB_I32, &hits)) { rc = fail(MP_E_INVALID, "blob: missing section 'hits'"); break; }
     FamilyLoad ld{blobs[v], blob_bytes[v], hits, maps ? E->allocs : scratch};
     if ((rc = E->family->load(ld, T, params[v]))) break;
-    decided.push_back({ld.nA, ld.nD, ld.nW, ld.nR, ld.nR_pad, ld.end_min_frames, ld.end_interval, ld.beam_cells, ld.end_prob, ld.hint_stacks});
+    decided.push_back({ld.nA, ld.nD, ld.nW, ld.nR, ld.nR_pad, ld.end_min_frames, ld.end_interval, ld.beam_cells, ld.end_prob});
     const Decided& a = decided[0];
     const Decided& b = decided[v];
     if ((!maps && a.nA != b.nA) || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
     else if (a.end_min_frames != b.end_min_frames || a.end_interval != b.end_interval || memcmp(&a.end_prob, &b.end_prob, sizeof a.end_prob) != 0)
       rc = fail(MP_E_UNSUPPORTED, "episode ending differs");
     else if (!maps && a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
-    else if (a.hints != b.hints) rc = fail(MP_E_UNSUPPORTED, "pre-merged sprite hints differ");
     else rc = E->family->same_shape(params[0], params[v]);
-    if (rc == MP_OK && maps) rc = load_map(blobs[v], blob_bytes[v], T, E->spawn_groups, E->allocs, map[v]);
+    if (rc == MP_OK) rc = load_map(blobs[v], blob_bytes[v], T, E->spawn_groups, E->allocs, map[v]);
     if (rc) g_error = "variant " + std::to_string(v) + ": " + g_error;
   }
   for (void* p : scratch) cudaFree(p);
@@ -1177,6 +1231,8 @@ int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_by
   if (maps) {
     for (const Decided& dv : decided) { T.nA = std::max(T.nA, dv.nA); E->beam_cells = std::max(E->beam_cells, dv.beam_cells); }
     T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16);
+  }
+  {
     std::vector<Tables> tv(n, T);  // T is final here: create changes nothing in it after this
     for (int v = 0; v < n; ++v) { apply_map(tv[v], map[v]); tv[v].nA = decided[v].nA; }
     const Tables* d = nullptr;
@@ -1219,12 +1275,13 @@ int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n
       if (env_variant_host[b] >= n_variants) return fail(MP_E_INVALID, "mp_create_variants: env %d assigned variant %d of %d", b, env_variant_host[b], n_variants);
   // whether the family (of variant 0) takes map variants decides which sections may differ
   const char* const* map_sections = nullptr;
+  const char* const* sprite_sections = nullptr;
   if (const MpbSection* m = mpb_find(blobs[0], blob_bytes[0], "meta"))
     if (m->dtype == MPB_I32 && m->nbytes >= 4)
       for (const FamilyEntry& f : kFamilies)
-        if (f.id == static_cast<const int32_t*>(mpb_data(blobs[0], m))[MPB_META_FAMILY]) map_sections = f.map_sections;
+        if (f.id == static_cast<const int32_t*>(mpb_data(blobs[0], m))[MPB_META_FAMILY]) { map_sections = f.map_sections; sprite_sections = f.sprite_sections; }
   for (int v = 1; v < n_variants; ++v)
-    if (int rc = same_sections(blobs[0], blob_bytes[0], blobs[v], blob_bytes[v], map_sections)) {
+    if (int rc = same_sections(blobs[0], blob_bytes[0], blobs[v], blob_bytes[v], map_sections, sprite_sections)) {
       g_error = "variant " + std::to_string(v) + ": " + g_error;
       return rc;
     }

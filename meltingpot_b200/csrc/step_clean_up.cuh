@@ -71,10 +71,11 @@ struct CleanUp {
   }
 
   // Host: per-env variants may differ in the Zapper and Cleaner cooldowns and rewards, DirtSpawner, AppleGrow, Edible
-  // and the water Animation's timing; layers, sprites, hits, beam footprints and the number of animation states agree.
+  // and the water Animation's timing, and in the apple, dirt and water sprites (appearance overrides); layers, beam hit
+  // sprites, hits, beam footprints and the number of animation states agree.
   static int same_shape(const Params& a, const Params& b) {
-    MP_SAME_ZAPPER MP_SAME(apple_layer) MP_SAME(apple_sprite) MP_SAME(dirt_layer) MP_SAME(dirt_sprite) MP_SAME(water_layer) MP_SAME(n_anim)
-    MP_SAME(water_sprite) MP_SAME(clean_layer) MP_SAME(clean_sprite) MP_SAME(clean_hit) MP_SAME(clean_geom) MP_SAME(dirt_count0)
+    MP_SAME_ZAPPER MP_SAME(apple_layer) MP_SAME(dirt_layer) MP_SAME(water_layer) MP_SAME(n_anim)
+    MP_SAME(clean_layer) MP_SAME(clean_sprite) MP_SAME(clean_hit) MP_SAME(clean_geom) MP_SAME(dirt_count0)
     return MP_OK;
   }
   static void copy_knobs(Params& dst, const Params& src) {
@@ -82,10 +83,14 @@ struct CleanUp {
     dst.clean_cooldown = src.clean_cooldown; dst.dirt_delay = src.dirt_delay; dst.dirt_prob = src.dirt_prob;
     dst.grow_rate = src.grow_rate; dst.grow_depletion = src.grow_depletion; dst.grow_restoration = src.grow_restoration;
     dst.eat_reward = src.eat_reward; dst.anim_frames = src.anim_frames; dst.anim_random = src.anim_random;
+    dst.apple_sprite = src.apple_sprite; dst.dirt_sprite = src.dirt_sprite;
+    memcpy(dst.water_sprite, src.water_sprite, sizeof dst.water_sprite);
   }
 
   using Scratch = WarpScratch;
   static constexpr bool kMapVariants = false;
+  // Its tables that hold only sprite ids: variants of one set (appearance overrides) may differ there (mp_create_variants).
+  static constexpr const char* kSpriteSections[] = {"cu_water_sprites", nullptr};
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables& T) { return scratch_round16((size_t)T.cells_pad * 6) + (size_t)T.n_actions * 16 + 2 * sizeof(BeamGeom); }

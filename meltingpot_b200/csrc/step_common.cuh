@@ -66,13 +66,17 @@ __host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * 
 // an env's map changes there too and never mid-episode. The Tables are read from the device array through the L1: a
 // local copy of the kernel's Tables with the variant's fields swapped in would sit on the stack (392 bytes for coins,
 // since avatar_sprite is indexed by lane).
+// The variants of any other family may differ in their initial grid (appearance overrides: which sprite each piece
+// shows), so their episode starts also read maps[k], whose Tables equal the kernel's except for init_grid; their steps
+// read the kernel's Tables. Sprite ids are read from the env's Params, never from the per-CTA tables stage() builds from
+// params[0] (which hold cell indices, walls and beam footprints only).
 template <class Params>
 struct ParamVariants {
   const Params* __restrict__ params;  // [n]
   uint8_t* active;                    // [B]
   const uint8_t* pending;             // [B]
   int n;
-  const Tables* __restrict__ maps;    // [n] (families with kMapVariants), else null
+  const Tables* __restrict__ maps;    // [n] each variant's Tables (its map; for other families, its initial grid)
 };
 
 // The variant env b advances under: on an episode start its pending assignment, which lane 0 makes the active one; an
@@ -160,8 +164,8 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
           if constexpr (HasResetMap<Family>::value) Family::reset_map(Tm, F, S, b, lane, sc);
           else Family::reset(Tm, F, S, b, lane, sc);
         } else Family::template step<Actions>(Tm, F, S, b, lane, acts, sc);
-      } else {
-        if (reset) Family::reset(T, F, S, b, lane, sc);
+      } else {  // the variants differ in their initial grid only (appearance overrides): an episode start reads maps[k]
+        if (reset) Family::reset(src.maps[k], F, S, b, lane, sc);
         else Family::template step<Actions>(T, F, S, b, lane, acts, sc);
       }
     } else {

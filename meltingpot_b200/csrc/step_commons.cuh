@@ -56,10 +56,11 @@ struct Commons {
 
   // Host: per-env variants may differ in the Zapper knobs and its beam footprint (length and radius), the DensityRegrow
   // probabilities and the Edible reward, and, as maps of one set (map variants: commons_harvest__open, __closed and
-  // __partnership), in the apples, their regrowth discs and the walls.
+  // __partnership), in the apples, their regrowth discs and the walls. The apple, wait, grass and desert sprites are
+  // knobs too (appearance overrides).
   static int same_shape(const Params& a, const Params& b) {
-    MP_SAME(zap.layer) MP_SAME(zap.sprite) MP_SAME(zap.hit) MP_SAME(apple_layer) MP_SAME(apple_sprite) MP_SAME(wait_layer) MP_SAME(wait_sprite) MP_SAME(grass_layer) MP_SAME(grass_sprite)
-    MP_SAME(dess_sprite) MP_SAME(ch_n_wait) MP_SAME(ch_n_probs)
+    MP_SAME(zap.layer) MP_SAME(zap.sprite) MP_SAME(zap.hit) MP_SAME(apple_layer) MP_SAME(wait_layer) MP_SAME(grass_layer)
+    MP_SAME(ch_n_wait) MP_SAME(ch_n_probs)
     return MP_OK;
   }
   static void copy_knobs(Params& dst, const Params& src) {
@@ -67,6 +68,7 @@ struct Commons {
     dst.zap.geom = src.zap.geom;
     for (int i = 0; i < 4; ++i) dst.ch_probs[i] = src.ch_probs[i];
     dst.eat_reward = src.eat_reward;
+    dst.apple_sprite = src.apple_sprite; dst.wait_sprite = src.wait_sprite; dst.grass_sprite = src.grass_sprite; dst.dess_sprite = src.dess_sprite;
   }
   static void copy_map(Params& dst, const Params& src) {
     dst.ch_apple = src.ch_apple; dst.ch_nbr = src.ch_nbr; dst.apple_of_cell = src.apple_of_cell;

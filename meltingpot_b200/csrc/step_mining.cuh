@@ -60,14 +60,16 @@ struct Mining {
     return MP_OK;
   }
 
-  // Host: per-env variants may differ in the mining window, the mine cooldown, the regrowth rates and the rewards.
+  // Host: per-env variants may differ in the mining window, the mine cooldown, the regrowth rates, the rewards and the
+  // ore sprites (appearance overrides).
   static int same_shape(const Params& a, const Params& b) {
-    MP_SAME(ore_layer) MP_SAME(ore_sprite) MP_SAME(mine_length) MP_SAME(mine_layer) MP_SAME(mine_sprite) MP_SAME(mine_hit)
+    MP_SAME(ore_layer) MP_SAME(mine_length) MP_SAME(mine_layer) MP_SAME(mine_sprite) MP_SAME(mine_hit)
     return MP_OK;
   }
   static void copy_knobs(Params& dst, const Params& src) {
     dst.mine_window = src.mine_window; dst.mine_cooldown = src.mine_cooldown;
     for (int i = 0; i < 2; ++i) { dst.mine_rate[i] = src.mine_rate[i]; dst.mine_reward[i] = src.mine_reward[i]; dst.extract_reward[i] = src.extract_reward[i]; }
+    memcpy(dst.ore_sprite, src.ore_sprite, sizeof dst.ore_sprite);
   }
 
   using Scratch = WarpScratch;

@@ -167,12 +167,13 @@ struct Territory {
   }
 
   // Host: per-env variants may differ in the Zapper knobs, the marking's initial level, recovery, per-level increments,
-  // removals, freezes and rewards, the claim wait and the Resource knobs; layers, sprites, beams, the number of marking
+  // removals, freezes and rewards, the claim wait, the Resource knobs and the resource, texture, damage, marking and
+  // per-player claimed / dry sprites (appearance overrides); layers, beam hit sprites, beams, the number of marking
   // levels and the Taste role agree.
   static int same_shape(const Params& a, const Params& b) {
-    MP_SAME_ZAPPER MP_SAME(res_layer) MP_SAME(unclaimed_sprite) MP_SAME(tex_layer) MP_SAME(tex_sprite) MP_SAME(ind_layer) MP_SAME(dmg_layer)
-    MP_SAME(dmg_sprite) MP_SAME(mark_layer) MP_SAME(mark_n_levels) MP_SAME(mark_sprite) MP_SAME(brush_layer) MP_SAME(claim_layer)
-    MP_SAME(tr_taste_role) MP_SAME(claimed_sprite) MP_SAME(dry_sprite) MP_SAME(brush_sprite) MP_SAME(claimbeam_sprite)
+    MP_SAME_ZAPPER MP_SAME(res_layer) MP_SAME(tex_layer) MP_SAME(ind_layer) MP_SAME(dmg_layer)
+    MP_SAME(mark_layer) MP_SAME(mark_n_levels) MP_SAME(brush_layer) MP_SAME(claim_layer)
+    MP_SAME(tr_taste_role) MP_SAME(brush_sprite) MP_SAME(claimbeam_sprite)
     MP_SAME(claim_geom) MP_SAME(brush_geom)
     return MP_OK;
   }
@@ -186,10 +187,17 @@ struct Territory {
     dst.claim_wait = src.claim_wait; dst.res_health0 = src.res_health0; dst.res_reward_delay = src.res_reward_delay;
     dst.res_repair_delay = src.res_repair_delay; dst.res_reward = src.res_reward; dst.res_rate = src.res_rate;
     dst.res_repair_prob = src.res_repair_prob;
+    dst.unclaimed_sprite = src.unclaimed_sprite; dst.tex_sprite = src.tex_sprite; dst.dmg_sprite = src.dmg_sprite;
+    memcpy(dst.mark_sprite, src.mark_sprite, sizeof dst.mark_sprite);
+    memcpy(dst.claimed_sprite, src.claimed_sprite, sizeof dst.claimed_sprite);
+    memcpy(dst.dry_sprite, src.dry_sprite, sizeof dst.dry_sprite);
   }
 
   using Scratch = TerritoryScratch;
   static constexpr bool kMapVariants = false;
+  // Its tables that hold only sprite ids (per player: claimed, dry, brush and claim-beam sprites): variants of one set may
+  // differ there (mp_create_variants), as far as same_shape allows.
+  static constexpr const char* kSpriteSections[] = {"tr_player_sprites", nullptr};
   static constexpr bool kStagesTables = true;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return territory_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables& T) { return territory_table_bytes(T); }

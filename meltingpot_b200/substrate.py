@@ -833,8 +833,16 @@ class SubstrateFactory:
       if env_variant is not None:
         raise ValueError('env_variant needs a sequence of prefab_overrides')
       blob = substrate_blobs.compile_with_overrides(self._name, tuple(roles), prefab_overrides)
-    else:  # one variant per entry
-      blob = [substrate_blobs.compile_with_overrides(self._name, tuple(roles), o) for o in prefab_overrides]
+    else:  # one variant per entry, compiled as one set on one sprite table
+      prefab_overrides = list(prefab_overrides)
+      if not prefab_overrides:
+        raise ValueError('the sequence of prefab_overrides is empty')
+      for i, o in enumerate(prefab_overrides):
+        if o is not None and not isinstance(o, Mapping):
+          raise ValueError(f'prefab_overrides[{i}] is a {type(o).__name__}, not a mapping')
+      if env_variant is not None:
+        env_variant = _checked_env_variant(env_variant, num_envs, len(prefab_overrides), 'prefab_overrides')
+      blob = substrate_blobs.compile_with_overrides(self._name, tuple(roles), prefab_overrides)
     return BatchedSubstrate(blob, num_envs, device=self._device, seed=seed,
                             env_index_base=env_index_base, world_rgb=world_rgb, env_variant=env_variant)
 
@@ -876,8 +884,10 @@ def build_batched(name, *, roles: Sequence[str], num_envs: int, device: int = 0,
   refuses another family, player count or map size); not combined with prefab_overrides or build_seeds.
 
   `prefab_overrides` (the reference builder's, builder.py:70-87) is one mapping for every env, or a sequence of
-  mappings: a heterogeneous batch whose env b runs variant env_variant[b] (default 0). Compiling overrides needs a
-  reference checkout.
+  mappings: a heterogeneous batch whose env b runs variant env_variant[b] (default 0). The sequence is compiled as one
+  set on one sprite table, so its entries may also change how pieces look (an `Appearance` palette or sprite shape),
+  e.g. [{}, {'potential_apple': {'Appearance': {'palettes': [recoloured]}}}]. Compiling overrides needs a reference
+  checkout.
 
   `build_seeds` (coins): one draw of the substrate's config builder per seed, as separate reference builds would
   make (coins draws its map size and its two coin colours on every build), compiled as one draw set. Env b plays
@@ -890,6 +900,16 @@ def build_batched(name, *, roles: Sequence[str], num_envs: int, device: int = 0,
   return get_factory(name, device).build_batched(roles, num_envs, seed=seed, env_index_base=env_index_base,
                                                  world_rgb=world_rgb, prefab_overrides=prefab_overrides,
                                                  env_variant=env_variant, build_seeds=build_seeds)
+
+
+def _checked_env_variant(env_variant, num_envs: int, num_variants: int, what: str) -> np.ndarray:
+  """env_variant as an int64 array of num_envs entries, each indexing the num_variants `what`."""
+  env_variant = np.asarray(env_variant, np.int64).reshape(-1)
+  if env_variant.shape != (num_envs,):
+    raise ValueError(f'env_variant has {env_variant.size} entries for {num_envs} envs')
+  if env_variant.size and (env_variant.min() < 0 or env_variant.max() >= num_variants):
+    raise ValueError(f'env_variant must index the {num_variants} {what} (0..{num_variants - 1})')
+  return env_variant
 
 
 _SHARED_CONFIG_FIELDS = ('action_set', 'individual_observation_names', 'global_observation_names', 'timestep_spec')
@@ -912,11 +932,7 @@ def _build_map_set(names: Sequence[str], *, roles, num_envs, device, seed, env_i
   if env_variant is None:
     env_variant = draw_of_env(env_index_base, num_envs, len(names))
   else:
-    env_variant = np.asarray(env_variant, np.int64).reshape(-1)
-    if env_variant.shape != (num_envs,):
-      raise ValueError(f'env_variant has {env_variant.size} entries for {num_envs} envs')
-    if env_variant.size and (env_variant.min() < 0 or env_variant.max() >= len(names)):
-      raise ValueError(f'env_variant must index the {len(names)} names (0..{len(names) - 1})')
+    env_variant = _checked_env_variant(env_variant, num_envs, len(names), 'names')
   blobs = [substrate_blobs.load_blob(n, tuple(roles)) for n in names]
   return BatchedSubstrate(blobs, num_envs, device=device, seed=seed, env_index_base=env_index_base,
                           world_rgb=world_rgb, env_variant=env_variant)

@@ -3,7 +3,7 @@
 from __future__ import annotations
 
 import os
-from typing import Optional, Sequence
+from typing import Mapping, Optional, Sequence
 
 _DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'data')
 
@@ -53,14 +53,21 @@ def load_blob(name: str, roles: Optional[Sequence[str]] = None) -> bytes:
   return compiler.compile_substrate(name, roles, build_seed=BUILD_SEEDS.get(name))
 
 
-def compile_with_overrides(name: str, roles: Sequence[str], prefab_overrides) -> bytes:
-  """The blob of `name` with `roles` and the reference's `prefab_overrides` (compiled from a reference checkout)."""
+def compile_with_overrides(name: str, roles: Sequence[str], prefab_overrides):
+  """The blob of `name` with `roles` and the reference's `prefab_overrides` (compiled from a reference checkout).
+
+  One mapping gives one blob. A sequence of mappings gives one blob per entry, compiled as one set on one sprite table
+  (compiler.compile_substrate_set), so that entries whose overrides change how pieces look can run side by side in one
+  engine; without such overrides each blob equals the entry compiled alone."""
   from meltingpot_b200 import compiler  # pylint: disable=g-import-not-at-top
   if compiler.reference_root() is None:
     raise FileNotFoundError(
         f'prefab_overrides for {name!r} need a Melting Pot reference checkout to compile from '
         '(set MELTINGPOT_REFERENCE_ROOT)')
-  return compiler.compile_substrate(name, roles, build_seed=BUILD_SEEDS.get(name), prefab_overrides=prefab_overrides)
+  if isinstance(prefab_overrides, Mapping):
+    return compiler.compile_substrate(name, roles, build_seed=BUILD_SEEDS.get(name), prefab_overrides=prefab_overrides)
+  overrides = list(prefab_overrides)
+  return compiler.compile_substrate_set(name, roles, [BUILD_SEEDS.get(name)] * len(overrides), prefab_overrides=overrides)
 
 
 def compile_draws(name: str, roles: Sequence[str], build_seeds: Sequence[int]) -> list:
