@@ -140,42 +140,29 @@ struct VariantSet {
   int n = 1;
   const Tables* maps = nullptr;  // [n] the Tables of each variant (its map, or for other families its initial grid)
 };
-// The launches take the restore of mp_step_restore, or null for the plain k_step, and the row actions of
-// mp_step_routed (then `actions` is unused), or null for dense actions.
 struct FamilyEntry {
   int id;  // MpbFamily
   bool map_variants;  // Family::kMapVariants: its variants may be draws of different maps (mp_create_variants)
-  const char* const* map_sections;  // then Family::kMapSections: its own entity tables, which such variants may differ in
+  const char* const* map_sections;  // Family::kMapSections: its own entity tables, which such variants may differ in, or null
   const char* const* sprite_sections;  // Family::kSpriteSections: its int32 tables that hold nothing but sprite ids, or null
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
-  cudaError_t (*launch)(const cudaLaunchConfig_t&, const Tables&, const FamilyParams&, const State&, const int32_t*, const uint8_t*, int,
-                        const StepRestore*, const RowActions*);
   size_t (*step_smem)(const Tables&);
-  const void* step;           // k_step<Family>
-  // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field), the upload of base's Params with
-  // each variant's knobs (base holds the engine's device tables), and the k_step<Family, ParamVariants> launch
+  // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field) and the upload of base's Params
+  // with each variant's knobs (base holds the engine's device tables)
   int (*same_shape)(const FamilyParams&, const FamilyParams&);
   int (*upload_variants)(std::vector<void*>&, const FamilyParams& base, const std::vector<FamilyParams>&, const void**);
-  cudaError_t (*launch_variants)(const cudaLaunchConfig_t&, const Tables&, const VariantSet&, const State&, const int32_t*, const uint8_t*, int,
-                                 const StepRestore*, const RowActions*);
-  const void* step_variants;  // k_step<Family, ParamVariants<Family::Params>>
-  const void* step_restore[2];  // the kRestore instantiations of both (mp_step_restore)
-  const void* step_routed[4];   // the RowActions instantiations of all four (mp_step_routed)
+  // Every k_step<Family, ...> an engine may launch, [variants][restore][routed]: Source Params or ParamVariants<Params>
+  // (mp_create_variants), kRestore (a step that restores envs from a bank), Actions DenseActions or RowActions
+  // (mp_step_routed).
+  const void* step[2][2][2];
+  // Launches `kernel`, one of `step`, with the kernel arguments `args` after filling in its Source argument (args[1]):
+  // `params` for one blob, or the ParamVariants<Params> of `variants`.
+  cudaError_t (*launch)(const cudaLaunchConfig_t&, const void* kernel, void** args, const FamilyParams& params, const VariantSet& variants);
 };
 
 template <class Family>
 int load_family(FamilyLoad& ld, const Tables& T, FamilyParams& params) {
   return Family::load(ld, T, params.emplace<typename Family::Params>());
-}
-template <class Family>
-cudaError_t launch_family(const cudaLaunchConfig_t& cfg, const Tables& T, const FamilyParams& params, const State& S,
-                          const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore, const RowActions* rows) {
-  using P = typename Family::Params;
-  const P& F = std::get<P>(params);
-  if (rows && restore) return cudaLaunchKernelEx(&cfg, k_step<Family, P, true, RowActions>, T, F, S, nullptr, mask, mode, *restore, *rows);
-  if (rows) return cudaLaunchKernelEx(&cfg, k_step<Family, P, false, RowActions>, T, F, S, nullptr, mask, mode, StepRestore{}, *rows);
-  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, typename Family::Params, true>, T, F, S, actions, mask, mode, *restore, RowActions{});
-  return cudaLaunchKernelEx(&cfg, k_step<Family>, T, F, S, actions, mask, mode, StepRestore{}, RowActions{});
 }
 template <class Family>
 int same_shape_family(const FamilyParams& a, const FamilyParams& b) {
@@ -195,40 +182,27 @@ int upload_variants_family(std::vector<void*>& allocs, const FamilyParams& base,
   return rc;
 }
 template <class Family>
-cudaError_t launch_variants_family(const cudaLaunchConfig_t& cfg, const Tables& T, const VariantSet& V, const State& S,
-                                   const int32_t* actions, const uint8_t* mask, int mode, const StepRestore* restore, const RowActions* rows) {
+cudaError_t launch_family(const cudaLaunchConfig_t& cfg, const void* kernel, void** args, const FamilyParams& params, const VariantSet& V) {
   using P = typename Family::Params;
-  const ParamVariants<P> src{static_cast<const P*>(V.params), V.active, V.pending, V.n, V.maps};
-  if (rows && restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true, RowActions>, T, src, S, nullptr, mask, mode, *restore, *rows);
-  if (rows) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, false, RowActions>, T, src, S, nullptr, mask, mode, StepRestore{}, *rows);
-  if (restore) return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>, true>, T, src, S, actions, mask, mode, *restore, RowActions{});
-  return cudaLaunchKernelEx(&cfg, k_step<Family, ParamVariants<P>>, T, src, S, actions, mask, mode, StepRestore{}, RowActions{});
+  ParamVariants<P> variants{static_cast<const P*>(V.params), V.active, V.pending, V.n, V.maps};
+  args[1] = V.n > 1 ? static_cast<void*>(&variants) : const_cast<P*>(&std::get<P>(params));
+  return cudaLaunchKernelExC(&cfg, kernel, args);
 }
-template <class Family>
-constexpr const char* const* map_sections() {
-  if constexpr (Family::kMapVariants) return Family::kMapSections;
-  else return nullptr;
-}
-template <class F, class = void>
-struct HasSpriteSections : std::false_type {};
-template <class F>
-struct HasSpriteSections<F, std::void_t<decltype(F::kSpriteSections)>> : std::true_type {};
-template <class Family>
-constexpr const char* const* sprite_sections() {
-  if constexpr (HasSpriteSections<Family>::value) return Family::kSpriteSections;
-  else return nullptr;
+template <class Family, class Source, bool kRestore, class Actions>
+const void* step_kernel() {
+  return reinterpret_cast<const void*>(k_step<Family, Source, kRestore, Actions>);
 }
 template <class Family>
 FamilyEntry family_entry(int id) {
-  return {id, Family::kMapVariants, map_sections<Family>(), sprite_sections<Family>(), load_family<Family>, launch_family<Family>, step_smem_bytes<Family>, reinterpret_cast<const void*>(k_step<Family>),
-          same_shape_family<Family>, upload_variants_family<Family>, launch_variants_family<Family>,
-          reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>>),
-          {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true>),
-           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, true>)},
-          {reinterpret_cast<const void*>(k_step<Family, typename Family::Params, false, RowActions>),
-           reinterpret_cast<const void*>(k_step<Family, typename Family::Params, true, RowActions>),
-           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, false, RowActions>),
-           reinterpret_cast<const void*>(k_step<Family, ParamVariants<typename Family::Params>, true, RowActions>)}};
+  using P = typename Family::Params;
+  using V = ParamVariants<P>;
+  return {id, Family::kMapVariants, Family::kMapSections, Family::kSpriteSections, load_family<Family>, step_smem_bytes<Family>,
+          same_shape_family<Family>, upload_variants_family<Family>,
+          {{{step_kernel<Family, P, false, DenseActions>(), step_kernel<Family, P, false, RowActions>()},
+            {step_kernel<Family, P, true, DenseActions>(), step_kernel<Family, P, true, RowActions>()}},
+           {{step_kernel<Family, V, false, DenseActions>(), step_kernel<Family, V, false, RowActions>()},
+            {step_kernel<Family, V, true, DenseActions>(), step_kernel<Family, V, true, RowActions>()}}},
+          launch_family<Family>};
 }
 const FamilyEntry kFamilies[] = {
     family_entry<CleanUp>(MPB_FAMILY_CLEAN_UP),
@@ -237,6 +211,10 @@ const FamilyEntry kFamilies[] = {
     family_entry<Coins>(MPB_FAMILY_COINS),
     family_entry<Mining>(MPB_FAMILY_COOP_MINING),
 };
+const FamilyEntry* find_family(int id) {
+  for (const FamilyEntry& f : kFamilies) if (f.id == id) return &f;
+  return nullptr;
+}
 
 }  // namespace
 
@@ -414,7 +392,7 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   if (T.topology == 1 && (T.view_l + T.view_r + 1 > T.W || T.view_f + T.view_b + 1 > T.H || T.view_l + T.view_r + 1 > T.H || T.view_f + T.view_b + 1 > T.W))
     return fail(MP_E_UNSUPPORTED, "TORUS map smaller than the view window");
   for (int k = 0; k < T.n_scalar; ++k) T.scalar_obs[k] = scalar_obs.data[k];
-  for (const FamilyEntry& f : kFamilies) if (f.id == m[MPB_META_FAMILY]) E->family = &f;
+  E->family = find_family(m[MPB_META_FAMILY]);
   if (!E->family) return fail(MP_E_UNSUPPORTED, "substrate family %d has no CUDA state-transition kernel yet", m[MPB_META_FAMILY]);
 
   // ---- avatars ---------------------------------------------------------------------------------
@@ -775,8 +753,11 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  if (E->variants.n > 1) CUDA_TRY(E->family->launch_variants(cfg, E->T, E->variants, E->S, actions, mask, mode, restore, rows));
-  else CUDA_TRY(E->family->launch(cfg, E->T, E->params, E->S, actions, mask, mode, restore, rows));
+  StepRestore restore_arg = restore ? *restore : StepRestore{};
+  RowActions rows_arg = rows ? *rows : RowActions{};
+  void* args[] = {&E->T, nullptr, &E->S, &actions, &mask, &mode, &restore_arg, &rows_arg};  // k_step's parameters; Source by `launch`
+  const void* kernel = E->family->step[E->variants.n > 1][restore != nullptr][rows != nullptr];
+  CUDA_TRY(E->family->launch(cfg, kernel, args, E->params, E->variants));
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st, E->S); }
@@ -1061,14 +1042,11 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
     static int step_smem_max[MP_MAX_DEVICES] = {};
     const int need = (int)E->step_smem;
     if (ce == cudaSuccess && need > 48 * 1024 && need > step_smem_max[device]) {
-      for (const FamilyEntry& f : kFamilies) {
-        if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-        if (ce == cudaSuccess) ce = cudaFuncSetAttribute(f.step_variants, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-        for (const void* k : f.step_restore)
-          if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-        for (const void* k : f.step_routed)
-          if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
-      }
+      for (const FamilyEntry& f : kFamilies)
+        for (const auto& by_restore : f.step)
+          for (const auto& by_actions : by_restore)
+            for (const void* k : by_actions)
+              if (ce == cudaSuccess) ce = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, need);
       if (ce == cudaSuccess) step_smem_max[device] = need;
     }
   }
@@ -1274,12 +1252,11 @@ int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n
     for (int b = 0; b < num_envs; ++b)
       if (env_variant_host[b] >= n_variants) return fail(MP_E_INVALID, "mp_create_variants: env %d assigned variant %d of %d", b, env_variant_host[b], n_variants);
   // whether the family (of variant 0) takes map variants decides which sections may differ
-  const char* const* map_sections = nullptr;
-  const char* const* sprite_sections = nullptr;
+  const FamilyEntry* family = nullptr;
   if (const MpbSection* m = mpb_find(blobs[0], blob_bytes[0], "meta"))
-    if (m->dtype == MPB_I32 && m->nbytes >= 4)
-      for (const FamilyEntry& f : kFamilies)
-        if (f.id == static_cast<const int32_t*>(mpb_data(blobs[0], m))[MPB_META_FAMILY]) { map_sections = f.map_sections; sprite_sections = f.sprite_sections; }
+    if (m->dtype == MPB_I32 && m->nbytes >= 4) family = find_family(static_cast<const int32_t*>(mpb_data(blobs[0], m))[MPB_META_FAMILY]);
+  const char* const* map_sections = family ? family->map_sections : nullptr;
+  const char* const* sprite_sections = family ? family->sprite_sections : nullptr;
   for (int v = 1; v < n_variants; ++v)
     if (int rc = same_sections(blobs[0], blob_bytes[0], blobs[v], blob_bytes[v], map_sections, sprite_sections)) {
       g_error = "variant " + std::to_string(v) + ": " + g_error;
@@ -1321,13 +1298,6 @@ int mp_set_flags(mp_handle h, uint32_t flags) {
   if (!h) return fail(MP_E_INVALID, "null handle");
   h->flags = (flags & ~(uint32_t)MP_FLAGS_CREATE_ONLY) | (h->flags & (uint32_t)MP_FLAGS_CREATE_ONLY);
   return MP_OK;
-}
-
-int mp_reset(mp_handle h, const uint8_t* env_mask, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "null handle");
-  DeviceGuard guard(h->device);
-  int rc = launch_state(h, nullptr, env_mask, 1, (cudaStream_t)stream);
-  return rc ? rc : launch_render(h, (cudaStream_t)stream);
 }
 
 int mp_step_state(mp_handle h, const int32_t* actions, void* stream) {
@@ -1450,22 +1420,6 @@ int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* f
 }  // namespace
 
 extern "C" {
-
-int mp_step_into(mp_handle h, const int32_t* actions, const mp_device_outputs* out, void* stream) {
-  if (!h || !actions) return fail(MP_E_INVALID, "mp_step_into: null handle or actions");
-  DeviceGuard guard(h->device);
-  int rc = check_device_outputs(h, out, "mp_step_into");
-  if (!rc) rc = launch_state(h, actions, nullptr, 0, (cudaStream_t)stream);
-  return rc ? rc : launch_render(h, (cudaStream_t)stream, out);
-}
-
-int mp_reset_into(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "null handle");
-  DeviceGuard guard(h->device);
-  int rc = check_device_outputs(h, out, "mp_reset_into");
-  if (!rc) rc = launch_state(h, nullptr, env_mask, 1, (cudaStream_t)stream);
-  return rc ? rc : launch_render(h, (cudaStream_t)stream, out);
-}
 
 int mp_get_buffers(mp_handle h, mp_buffers* out) {
   if (!h || !out) return fail(MP_E_INVALID, "null argument");
@@ -1873,6 +1827,66 @@ int check_player_actions(mp_engine* E, const mp_player_actions* a, const mp_play
   ext.push_back({"action", (uintptr_t)a->action, (u128)(a->n_rows - 1) * a->action_row_stride + 4});
   return MP_OK;
 }
+
+// The restore of a call that may restore envs from a state bank (mp_state_restore, mp_step_restore, mp_step_players,
+// mp_step_routed): slot_of_env and bank, or neither; MP_RESTORE_REKEY or no flags.
+struct RestoreArgs { const int32_t* slot_of_env = nullptr; const void* bank = nullptr; int n_slots = 0; uint32_t flags = 0; };
+
+int check_restore(const RestoreArgs& r, const char* fn) {
+  const bool restoring = r.slot_of_env || r.bank;
+  if (restoring && (!r.slot_of_env || !r.bank)) return fail(MP_E_INVALID, "%s: slot_of_env and bank go together", fn);
+  if (restoring && r.n_slots < 1) return fail(MP_E_INVALID, "%s: n_slots %d < 1", fn, r.n_slots);
+  if (r.flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "%s: unknown flags 0x%x", fn, r.flags & ~MP_RESTORE_REKEY);
+  if (r.flags && !restoring) return fail(MP_E_INVALID, "%s: flags without a bank", fn);
+  return MP_OK;
+}
+
+// One state-transition call of the step and reset entry points that compose targets, restores and row actions.
+struct StateCall {
+  const char* fn;  // the entry point, for messages
+  int mode;        // k_step's: 0 step, 1 reset
+  const uint8_t* mask = nullptr;            // reset: the envs to reset, or null for all
+  const int32_t* actions = nullptr;         // step: dense actions [B][P]
+  bool routed = false;                      // step: actions from `rows` instead (mp_step_routed)
+  const mp_player_actions* rows = nullptr;
+  RestoreArgs restore;
+  const mp_device_outputs* out = nullptr;   // targets (check_device_outputs)
+  bool needs_out = false;                   // refuse a null `out`
+  const mp_player_outputs* players = nullptr;  // per-player rows (check_player_outputs)
+  bool needs_players = false;               // refuse null `players`
+  bool render_follows = true;               // launch_state's; false launches k_exchange_push as mp_step does
+};
+
+// Every check of `c`, in the order the entry points document: restore, row actions, player rows, then the bank, targets
+// and extents together. A call with nothing to check does no check work.
+int check_call(mp_engine* E, const StateCall& c) {
+  int rc = check_restore(c.restore, c.fn);
+  std::vector<DeviceExtent> ext;
+  if (!rc && c.routed) rc = check_player_actions(E, c.rows, c.players, c.fn, ext);
+  if (!rc && (c.players || c.needs_players)) rc = check_player_outputs(E, c.players, c.out, c.fn, ext);
+  if (rc) return rc;
+  const RestoreArgs& r = c.restore;
+  if (r.bank) return check_bank(E, r.bank, r.n_slots, r.slot_of_env, (uint64_t)E->B, E->record.record_bytes, c.fn, c.out, ext);
+  if (c.out || c.needs_out) return check_device_outputs(E, c.out, c.fn, std::move(ext));
+  return ext.empty() ? MP_OK : check_extents(E, ext, c.fn);
+}
+
+// Checks `c` and, when every check passes, launches it: the state transition, then the render. A refused call enqueues
+// nothing.
+int run_call(mp_engine* E, const StateCall& c, void* stream) {
+  DeviceGuard guard(E->device);
+  int rc = check_call(E, c);
+  if (rc) return rc;
+  const RestoreArgs& r = c.restore;
+  const StepRestore restore{E->d_record_layout, r.slot_of_env, static_cast<const uint8_t*>(r.bank), r.n_slots,
+                            (r.flags & MP_RESTORE_REKEY) ? 1 : 0, E->key_base};
+  RowActions rows{};
+  if (c.routed) rows = {c.rows->row_of_player, reinterpret_cast<const uint8_t*>(c.rows->action), c.rows->action_row_stride, c.rows->n_rows};
+  const cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = launch_state(E, c.actions, c.mask, c.mode, st, c.render_follows, r.bank ? &restore : nullptr, c.routed ? &rows : nullptr)))
+    return rc;
+  return launch_render(E, st, c.out, c.players);
+}
 }  // namespace
 
 int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* bank, void* stream) {
@@ -1889,8 +1903,7 @@ int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* b
 
 int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, void* stream) {
   if (!h || !slot_of_env || !bank) return fail(MP_E_INVALID, "mp_state_restore: null argument");
-  if (n_slots < 1) return fail(MP_E_INVALID, "mp_state_restore: n_slots %d < 1", n_slots);
-  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_state_restore: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
+  if (int rc = check_restore({slot_of_env, bank, n_slots, flags}, "mp_state_restore")) return rc;
   if (h->S.x_world || h->d_g_flag_ptrs)
     return fail(MP_E_UNSUPPORTED, "mp_state_restore: not available once mp_exchange_connect / mp_gather_obs_connect has run");
   DeviceGuard guard(h->device);
@@ -1904,79 +1917,58 @@ int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, 
   return launch_render(h, st);
 }
 
+int mp_reset(mp_handle h, const uint8_t* env_mask, void* stream) {
+  if (!h) return fail(MP_E_INVALID, "null handle");
+  StateCall c{"mp_reset", 1};
+  c.mask = env_mask;
+  return run_call(h, c, stream);
+}
+
+int mp_reset_into(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, void* stream) {
+  if (!h) return fail(MP_E_INVALID, "null handle");
+  StateCall c{"mp_reset_into", 1};
+  c.mask = env_mask; c.out = out; c.needs_out = true;
+  return run_call(h, c, stream);
+}
+
+int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
+  if (!h) return fail(MP_E_INVALID, "mp_reset_players: null handle");
+  StateCall c{"mp_reset_players", 1};
+  c.mask = env_mask; c.out = out; c.players = players; c.needs_players = true;
+  return run_call(h, c, stream);
+}
+
+int mp_step_into(mp_handle h, const int32_t* actions, const mp_device_outputs* out, void* stream) {
+  if (!h || !actions) return fail(MP_E_INVALID, "mp_step_into: null handle or actions");
+  StateCall c{"mp_step_into", 0};
+  c.actions = actions; c.out = out; c.needs_out = true;
+  return run_call(h, c, stream);
+}
+
 int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
                     const mp_device_outputs* out, void* stream) {
   if (!h || !actions || !slot_of_env || !bank) return fail(MP_E_INVALID, "mp_step_restore: null argument");
-  if (n_slots < 1) return fail(MP_E_INVALID, "mp_step_restore: n_slots %d < 1", n_slots);
-  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_restore: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
-  DeviceGuard guard(h->device);
-  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_step_restore", out);
-  if (rc) return rc;
-  const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
-                            (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
-  cudaStream_t st = (cudaStream_t)stream;
-  // launched as mp_step (out == NULL) or mp_step_into: the same kernels, the same exchange and gather sequence
-  if ((rc = launch_state(h, actions, nullptr, 0, st, /*render_follows=*/out != nullptr, &restore))) return rc;
-  return launch_render(h, st, out);
+  StateCall c{"mp_step_restore", 0};
+  c.actions = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out;
+  c.render_follows = out != nullptr;  // launched as mp_step (out == NULL) or mp_step_into
+  return run_call(h, c, stream);
 }
 
 int mp_step_players(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
                     const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
   if (!h || !actions) return fail(MP_E_INVALID, "mp_step_players: null handle or actions");
-  const bool restoring = slot_of_env || bank;
-  if (restoring && (!slot_of_env || !bank)) return fail(MP_E_INVALID, "mp_step_players: slot_of_env and bank go together");
-  if (restoring && n_slots < 1) return fail(MP_E_INVALID, "mp_step_players: n_slots %d < 1", n_slots);
-  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_players: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
-  if (flags && !restoring) return fail(MP_E_INVALID, "mp_step_players: flags without a bank");
-  DeviceGuard guard(h->device);
-  std::vector<DeviceExtent> ext;
-  int rc = check_player_outputs(h, players, out, "mp_step_players", ext);
-  if (!rc) {
-    if (restoring) rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_step_players", out, ext);
-    else rc = out ? check_device_outputs(h, out, "mp_step_players", ext) : check_extents(h, ext, "mp_step_players");
-  }
-  if (rc) return rc;
-  const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
-                            (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
-  cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = launch_state(h, actions, nullptr, 0, st, /*render_follows=*/true, restoring ? &restore : nullptr))) return rc;
-  return launch_render(h, st, out, players);
-}
-
-int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "mp_reset_players: null handle");
-  DeviceGuard guard(h->device);
-  std::vector<DeviceExtent> ext;
-  int rc = check_player_outputs(h, players, out, "mp_reset_players", ext);
-  if (!rc) rc = out ? check_device_outputs(h, out, "mp_reset_players", ext) : check_extents(h, ext, "mp_reset_players");
-  if (!rc) rc = launch_state(h, nullptr, env_mask, 1, (cudaStream_t)stream);
-  return rc ? rc : launch_render(h, (cudaStream_t)stream, out, players);
+  StateCall c{"mp_step_players", 0};
+  c.actions = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out; c.players = players; c.needs_players = true;
+  return run_call(h, c, stream);
 }
 
 int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t* slot_of_env, const void* bank, int n_slots,
                    uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
   if (!h) return fail(MP_E_INVALID, "mp_step_routed: null handle");
-  const bool restoring = slot_of_env || bank;
-  if (restoring && (!slot_of_env || !bank)) return fail(MP_E_INVALID, "mp_step_routed: slot_of_env and bank go together");
-  if (restoring && n_slots < 1) return fail(MP_E_INVALID, "mp_step_routed: n_slots %d < 1", n_slots);
-  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "mp_step_routed: unknown flags 0x%x", flags & ~MP_RESTORE_REKEY);
-  if (flags && !restoring) return fail(MP_E_INVALID, "mp_step_routed: flags without a bank");
-  DeviceGuard guard(h->device);
-  std::vector<DeviceExtent> ext;
-  int rc = check_player_actions(h, actions, players, "mp_step_routed", ext);
-  if (!rc && players) rc = check_player_outputs(h, players, out, "mp_step_routed", ext);
-  if (!rc) {
-    if (restoring) rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_step_routed", out, ext);
-    else rc = out ? check_device_outputs(h, out, "mp_step_routed", ext) : check_extents(h, ext, "mp_step_routed");
-  }
-  if (rc) return rc;
-  const StepRestore restore{h->d_record_layout, slot_of_env, static_cast<const uint8_t*>(bank), n_slots,
-                            (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
-  const RowActions rows{actions->row_of_player, reinterpret_cast<const uint8_t*>(actions->action), actions->action_row_stride, actions->n_rows};
-  cudaStream_t st = (cudaStream_t)stream;
-  // launched as the composed call: mp_step (render_follows false), mp_step_into, mp_step_restore or mp_step_players
-  if ((rc = launch_state(h, nullptr, nullptr, 0, st, /*render_follows=*/out || players, restoring ? &restore : nullptr, &rows))) return rc;
-  return launch_render(h, st, out, players);
+  StateCall c{"mp_step_routed", 0};
+  c.routed = true; c.rows = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out; c.players = players;
+  c.render_follows = out || players;  // launched as the composed call: mp_step, mp_step_into, mp_step_restore or mp_step_players
+  return run_call(h, c, stream);
 }
 
 int mp_launch_count(mp_handle h, uint64_t* out) {

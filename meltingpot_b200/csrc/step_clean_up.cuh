@@ -89,6 +89,7 @@ struct CleanUp {
 
   using Scratch = WarpScratch;
   static constexpr bool kMapVariants = false;
+  static constexpr const char* const* kMapSections = nullptr;
   // Its tables that hold only sprite ids: variants of one set (appearance overrides) may differ there (mp_create_variants).
   static constexpr const char* kSpriteSections[] = {"cu_water_sprites", nullptr};
   static constexpr bool kStagesTables = true;

@@ -79,6 +79,7 @@ struct Commons {
   // their entity tables, and the apple count is the nA of each variant's Tables (setup_variants).
   static constexpr bool kMapVariants = true;
   static constexpr const char* kMapSections[] = {"ch_apple", "ch_nbr", nullptr};
+  static constexpr const char* const* kSpriteSections = nullptr;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }

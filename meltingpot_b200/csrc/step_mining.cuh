@@ -74,6 +74,8 @@ struct Mining {
 
   using Scratch = WarpScratch;
   static constexpr bool kMapVariants = false;
+  static constexpr const char* const* kMapSections = nullptr;
+  static constexpr const char* const* kSpriteSections = nullptr;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
   __host__ __device__ static size_t table_bytes(const Tables&) { return 0; }

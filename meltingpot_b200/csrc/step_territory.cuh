@@ -195,6 +195,7 @@ struct Territory {
 
   using Scratch = TerritoryScratch;
   static constexpr bool kMapVariants = false;
+  static constexpr const char* const* kMapSections = nullptr;
   // Its tables that hold only sprite ids (per player: claimed, dry, brush and claim-beam sprites): variants of one set may
   // differ there (mp_create_variants), as far as same_shape allows.
   static constexpr const char* kSpriteSections[] = {"tr_player_sprites", nullptr};

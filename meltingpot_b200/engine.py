@@ -562,41 +562,25 @@ class Engine:
         raise ValueError('give actions or player_actions, not both')
       pa = describe_player_actions({k: (None if v is None else layout_of(v)) for k, v in player_actions.items()},
                                    self.num_envs, self.num_players, self.device)
-      flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
-      s = None if out is None else ctypes.byref(self._device_outputs(out))
-      p = None if players is None else ctypes.byref(self._player_outputs(players))
+    elif actions is None:
+      raise ValueError('actions is None: give actions, or player_actions')
+    else:
+      self._check_actions(actions)
+      a = ctypes.c_void_p(actions.data_ptr())
+    flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
+    s = None if out is None else ctypes.byref(self._device_outputs(out))
+    p = None if players is None else ctypes.byref(self._player_outputs(players))
+    if player_actions is not None:
       _check(self._lib.mp_step_routed(self._h, ctypes.byref(pa), idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, p,
                                       self._stream(stream)))
-      return
-    if actions is None:
-      raise ValueError('actions is None: give actions, or player_actions')
-    self._check_actions(actions)
-    if players is not None:
-      flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
-      s = None if out is None else ctypes.byref(self._device_outputs(out))
-      _check(self._lib.mp_step_players(self._h, ctypes.c_void_p(actions.data_ptr()), idx, bank_ptr, n_slots, ctypes.c_uint32(flags),
-                                       s, ctypes.byref(self._player_outputs(players)), self._stream(stream)))
-      return
-    if restore is not None or bank is not None:
-      if restore is None or bank is None:
-        raise ValueError('restore and bank go together')
-      bank = self._bank(bank)
-      idx = self._indices(restore, self.num_envs, 'restore')
-      for name, t in (('bank', bank), ('restore', idx)):
-        if t.device.index != self.device:
-          raise ValueError(f'{name} is on {t.device}, the engine runs on cuda:{self.device}')
-      s = None if out is None else ctypes.byref(self._device_outputs(out))
-      _check(self._lib.mp_step_restore(self._h, ctypes.c_void_p(actions.data_ptr()), ctypes.c_void_p(idx.data_ptr()),
-                                       ctypes.c_void_p(bank.data_ptr()), int(bank.shape[0]),
-                                       ctypes.c_uint32(MP_RESTORE_REKEY if rekey else 0), s, self._stream(stream)))
-      return
-    if rekey:
-      raise ValueError('rekey needs restore and bank')
-    if out is None:
-      _check(self._lib.mp_step(self._h, ctypes.c_void_p(actions.data_ptr()), self._stream(stream)))
+    elif players is not None:
+      _check(self._lib.mp_step_players(self._h, a, idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, p, self._stream(stream)))
+    elif bank_ptr is not None:
+      _check(self._lib.mp_step_restore(self._h, a, idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, self._stream(stream)))
+    elif out is None:
+      _check(self._lib.mp_step(self._h, a, self._stream(stream)))
     else:
-      s = self._device_outputs(out)
-      _check(self._lib.mp_step_into(self._h, ctypes.c_void_p(actions.data_ptr()), ctypes.byref(s), self._stream(stream)))
+      _check(self._lib.mp_step_into(self._h, a, s, self._stream(stream)))
 
   def _restore_args(self, restore, bank, rekey):
     """flags, index pointer, bank pointer and slot count of restore / bank (None, None, 0 without them)."""
