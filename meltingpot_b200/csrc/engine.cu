@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <string>
 #include <variant>
 #include <vector>
@@ -147,10 +148,10 @@ struct FamilyEntry {
   const char* const* sprite_sections;  // Family::kSpriteSections: its int32 tables that hold nothing but sprite ids, or null
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
   size_t (*step_smem)(const Tables&);
-  // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field) and the upload of base's Params
-  // with each variant's knobs (base holds the engine's device tables)
+  // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field) and the upload of every variant's
+  // own Params
   int (*same_shape)(const FamilyParams&, const FamilyParams&);
-  int (*upload_variants)(std::vector<void*>&, const FamilyParams& base, const std::vector<FamilyParams>&, const void**);
+  int (*upload_variants)(std::vector<void*>&, const std::vector<FamilyParams>&, const void**);
   // Every k_step<Family, ...> an engine may launch, [variants][restore][routed]: Source Params or ParamVariants<Params>
   // (mp_create_variants), kRestore (a step that restores envs from a bank), Actions DenseActions or RowActions
   // (mp_step_routed).
@@ -169,13 +170,10 @@ int same_shape_family(const FamilyParams& a, const FamilyParams& b) {
   return Family::same_shape(std::get<typename Family::Params>(a), std::get<typename Family::Params>(b));
 }
 template <class Family>
-int upload_variants_family(std::vector<void*>& allocs, const FamilyParams& base, const std::vector<FamilyParams>& variants, const void** out) {
+int upload_variants_family(std::vector<void*>& allocs, const std::vector<FamilyParams>& variants, const void** out) {
   using P = typename Family::Params;
-  std::vector<P> host(variants.size(), std::get<P>(base));
-  for (size_t v = 0; v < variants.size(); ++v) {
-    Family::copy_knobs(host[v], std::get<P>(variants[v]));
-    if constexpr (Family::kMapVariants) Family::copy_map(host[v], std::get<P>(variants[v]));
-  }
+  std::vector<P> host;
+  for (const FamilyParams& v : variants) host.push_back(std::get<P>(v));
   const P* d = nullptr;
   int rc = upload(allocs, host, &d);
   *out = d;
@@ -226,7 +224,6 @@ struct mp_engine {
   int n_total = 0;  // atlas sprites incl. pre-merged
   Tables T{};
   FamilyParams params;
-  int beam_cells = 0;  // FamilyLoad::beam_cells: sizes State::max_events
   State S{};
   RenderPlan R{};
   mp_buffers buffers{};
@@ -268,7 +265,6 @@ struct mp_engine {
   uint64_t key_base = 0;   // seed + env_index_base: env b's key at creation is key_base + b (State::key)
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
-  int spawn_groups[3] = {-1, -1, -1};  // the respawn group and the two initial spawn groups (or -1) of every variant
   RecordLayout record{};                     // every per-env state array (layout_state): what records and snapshots copy
   RecordLayout* d_record_layout = nullptr;  // device copy of `record`, read by mp_step_restore's k_step
 
@@ -304,10 +300,10 @@ void apply_map(Tables& T, const MapVariant& M) {
 
 // The map of one blob, which apply_map puts into a Tables: its initial grid padded to cells_pad, the static occupancy of
 // the avatar layer (non-avatar pieces that start there), the cells of the respawn group and of the initial spawn groups,
-// the avatars' sprites and the BeamBlocker bits of each cell (its walls). `T` holds the geometry and the avatar tables of
-// the engine, `groups` the respawn group and the two initial groups (or -1).
-// build_tables takes variant 0's map into the Tables; a map-variant engine keeps every variant's (setup_variants).
-int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], std::vector<void*>& allocs, MapVariant& M) {
+// the avatars' sprites and the BeamBlocker bits of each cell (its walls), as host tables aimed at M's fields. `T` holds the
+// geometry and the avatar tables of the engine, `groups` the respawn group and the two initial groups (or -1).
+// build_tables decodes variant 0's map, which create puts into the Tables; setup_variants decodes every other variant's.
+int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], std::vector<HostTable>& tables, MapVariant& M) {
   Section<int32_t> meta, objects, kinds, states, av_table;
   Section<uint16_t> init_grid;
   Section<uint8_t> cell_flags;
@@ -348,22 +344,38 @@ int load_map(const void* blob, size_t n, const Tables& T, const int groups[3], s
   }
   std::vector<uint8_t> flags(T.cells_pad, 0);
   memcpy(flags.data(), cell_flags.data, std::min<size_t>(cell_flags.count, T.cells));
-  int rc;
-  if ((rc = upload(allocs, grid0, &M.init_grid)) || (rc = upload(allocs, cells[0], &M.spawn_cell)) || (rc = upload(allocs, solid, &M.solid)) ||
-      (rc = upload(allocs, flags, &M.cell_flags)))
-    return rc;
-  for (int k = 0; k < 2; ++k) {
-    if (cells[1 + k].empty()) { M.spawn_init_cell[k] = M.spawn_cell; continue; }
-    if ((rc = upload(allocs, cells[1 + k], &M.spawn_init_cell[k]))) return rc;
-  }
+  add_table(tables, &M.init_grid, grid0); add_table(tables, &M.spawn_cell, cells[0]); add_table(tables, &M.solid, solid);
+  add_table(tables, &M.cell_flags, flags);
+  // an initial group without cells of its own spawns on the respawn group's (the same bytes, so the same device table)
+  for (int k = 0; k < 2; ++k) add_table(tables, &M.spawn_init_cell[k], cells[1 + k].empty() ? cells[0] : cells[1 + k]);
   return MP_OK;
 }
+
+// What create decodes from the blobs before it opens a device (build_tables, setup_variants). The device tables are
+// host tables so far, each aimed at a field of `T`, of a variant's Params or of a variant's map; upload_tables uploads
+// them once the device is checked. Everything per variant is sized to the set before decoding starts, so no field a
+// table is aimed at moves.
+struct Decoded {
+  const FamilyEntry* family = nullptr;
+  Tables T{};
+  int spawn_groups[3] = {-1, -1, -1};  // the respawn group and the two initial spawn groups (or -1) of every variant
+  int beam_cells = 0;                  // FamilyLoad::beam_cells: sizes State::max_events
+  int n_total = 0, black_sprite = -1;
+  std::vector<uint8_t> host_pair, host_sflags;
+  std::vector<HostTable> tables;     // the Tables' own and those of every map
+  std::vector<FamilyParams> params;  // [n] each variant's own Params
+  std::vector<FamilyLoad> loads;     // [n] what each variant's loader handed back, with its Params' tables
+  std::vector<int> load_rc;          // [n] each loader's refusal: variant 0's is reported at once, the others' by setup_variants
+  std::vector<std::string> load_error;
+  std::vector<MapVariant> maps;      // [n]
+  explicit Decoded(int n) : params(n), loads(n), load_rc(n), load_error(n), maps(n) {}
+};
 
 // The engine's tables from blob 0 of `blobs`. The pre-merged sprites cover the cell stacks and the family's hint stacks
 // of every blob: the variants of an engine share one sprite table and the renderer's pre-merged pairs, and may differ in
 // their maps (map variants) or in the sprites their pieces show (appearance overrides). Variants that differ in neither
 // add no stack of their own, so their engine has the pre-merged sprites of blob 0 alone.
-int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_sizes, int n_blobs) {
+int build_tables(Decoded& D, const void* const* blobs, const size_t* blob_sizes, int n_blobs, uint32_t flags) {
   const void* blob = blobs[0];
   const size_t n = blob_sizes[0];
   Section<int32_t> meta, states, kinds, comps, objects, hits, action_table, sprite_map, scalar_obs, av_table;
@@ -376,7 +388,7 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   NEED(action_table, MPB_I32) NEED(sprite_map, MPB_I32) NEED(scalar_obs, MPB_I32) NEED(av_table, MPB_I32)
   NEED(atlas, MPB_U8) NEED(sprite_opaque, MPB_U8) NEED(init_grid, MPB_U16)
   const int32_t* m = meta.data;
-  Tables& T = E->T;
+  Tables& T = D.T;
   T.W = m[MPB_META_W]; T.H = m[MPB_META_H]; T.cells = T.W * T.H; T.cells_pad = round_up(T.cells, 8);
   T.L = m[MPB_META_L]; T.P = m[MPB_META_P]; T.topology = m[MPB_META_TOPOLOGY]; T.max_frames = m[MPB_META_MAX_FRAMES];
   T.view_l = m[MPB_META_VIEW_LEFT]; T.view_r = m[MPB_META_VIEW_RIGHT]; T.view_f = m[MPB_META_VIEW_FORWARD]; T.view_b = m[MPB_META_VIEW_BACKWARD];
@@ -392,8 +404,8 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
   if (T.topology == 1 && (T.view_l + T.view_r + 1 > T.W || T.view_f + T.view_b + 1 > T.H || T.view_l + T.view_r + 1 > T.H || T.view_f + T.view_b + 1 > T.W))
     return fail(MP_E_UNSUPPORTED, "TORUS map smaller than the view window");
   for (int k = 0; k < T.n_scalar; ++k) T.scalar_obs[k] = scalar_obs.data[k];
-  E->family = find_family(m[MPB_META_FAMILY]);
-  if (!E->family) return fail(MP_E_UNSUPPORTED, "substrate family %d has no CUDA state-transition kernel yet", m[MPB_META_FAMILY]);
+  D.family = find_family(m[MPB_META_FAMILY]);
+  if (!D.family) return fail(MP_E_UNSUPPORTED, "substrate family %d has no CUDA state-transition kernel yet", m[MPB_META_FAMILY]);
 
   // ---- avatars ---------------------------------------------------------------------------------
   T.avatar_layer = av_table.data[2];
@@ -412,53 +424,50 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
     if (g < 0) return fail(MP_E_UNSUPPORTED, "more than two initial spawn groups");
     T.avatar_init_group[p] = g;
   }
-  E->spawn_groups[0] = respawn_group; E->spawn_groups[1] = init_groups[0]; E->spawn_groups[2] = init_groups[1];
-  MapVariant map0{};
+  D.spawn_groups[0] = respawn_group; D.spawn_groups[1] = init_groups[0]; D.spawn_groups[2] = init_groups[1];
+  const MapVariant& map0 = D.maps[0];
   int rc;
-  if ((rc = load_map(blob, n, T, E->spawn_groups, E->allocs, map0))) return rc;
-  apply_map(T, map0);
+  if ((rc = load_map(blob, n, T, D.spawn_groups, D.tables, D.maps[0]))) return rc;
 
-  // ---- family tables -----------------------------------------------------------------------------
-  FamilyLoad ld{blob, n, hits, E->allocs};
-  if ((rc = E->family->load(ld, T, E->params))) return rc;
-  std::vector<std::vector<int>> hint_stacks = ld.hint_stacks;
-  {  // every other variant's hint stacks (its loader's uploads are freed; setup_variants checks and loads it again)
-    std::vector<void*> scratch;
-    for (int v = 1; v < n_blobs; ++v) {
-      Section<int32_t> v_hits;
-      FamilyParams scratch_params;
-      if (!get_section(blobs[v], blob_sizes[v], "hits", MPB_I32, &v_hits)) continue;
-      FamilyLoad lv{blobs[v], blob_sizes[v], v_hits, scratch};
-      if (E->family->load(lv, T, scratch_params) == MP_OK) hint_stacks.insert(hint_stacks.end(), lv.hint_stacks.begin(), lv.hint_stacks.end());
+  // ---- family tables: every blob's loader, once. Variant 0's refusal is reported here, every other variant's by
+  // setup_variants; the hint stacks of every loader that succeeded go to the pre-merge.
+  for (int v = 0; v < n_blobs; ++v) {
+    Section<int32_t> v_hits;
+    if (!get_section(blobs[v], blob_sizes[v], "hits", MPB_I32, &v_hits)) {
+      D.load_rc[v] = fail(MP_E_INVALID, "blob: missing section 'hits'");
+    } else {
+      D.loads[v] = FamilyLoad{blobs[v], blob_sizes[v], v_hits};
+      D.load_rc[v] = D.family->load(D.loads[v], T, D.params[v]);
     }
-    for (void* p : scratch) cudaFree(p);
+    if (D.load_rc[v] && v == 0) return D.load_rc[v];
+    if (D.load_rc[v]) D.load_error[v] = g_error;
   }
+  std::vector<std::vector<int>> hint_stacks;
+  for (int v = 0; v < n_blobs; ++v)
+    if (!D.load_rc[v]) hint_stacks.insert(hint_stacks.end(), D.loads[v].hint_stacks.begin(), D.loads[v].hint_stacks.end());
 #undef NEED
+  const FamilyLoad& ld = D.loads[0];
   T.nA = ld.nA; T.nD = ld.nD; T.nW = ld.nW; T.nR = ld.nR; T.nR_pad = ld.nR_pad;
   T.end_min_frames = ld.end_min_frames; T.end_interval = ld.end_interval; T.end_prob = ld.end_prob;
-  E->beam_cells = ld.beam_cells;
+  D.beam_cells = ld.beam_cells;
   {  // 'choice' prefabs left to the engine (drawn per env and episode)
     Section<int32_t> choice_groups, obj_choice, spawn_cond;
     char name[64];
     if (get_section(blob, n, "choice_groups", MPB_I32, &choice_groups)) {
-      if (E->family->id != MPB_FAMILY_TERRITORY) return fail(MP_E_UNSUPPORTED, "per-env 'choice' prefabs are implemented for the territory family only (compile with a build_seed)");
+      if (D.family->id != MPB_FAMILY_TERRITORY) return fail(MP_E_UNSUPPORTED, "per-env 'choice' prefabs are implemented for the territory family only (compile with a build_seed)");
       T.n_choice = (int)choice_groups.count;
       for (size_t g = 0; g < choice_groups.count; ++g) if (choice_groups.data[g] < 1 || choice_groups.data[g] > 31) return fail(MP_E_INVALID, "blob: choice group with %d options", choice_groups.data[g]);
-      std::vector<int32_t> v(choice_groups.data, choice_groups.data + choice_groups.count);
-      if ((rc = upload(E->allocs, v, &T.choice_n))) return rc;
+      add_table(D.tables, &T.choice_n, std::vector<int32_t>(choice_groups.data, choice_groups.data + choice_groups.count));
       snprintf(name, sizeof name, "spawn_cond_%d", respawn_group);
       if (get_section(blob, n, name, MPB_I32, &spawn_cond)) {
-        if ((int)spawn_cond.count != T.n_spawn * 2 || T.n_spawn > 64) return fail(MP_E_UNSUPPORTED, "%d conditional spawn candidates (max 64)", T.n_spawn);
-        std::vector<int32_t> c(spawn_cond.data, spawn_cond.data + spawn_cond.count);
-        if ((rc = upload(E->allocs, c, &T.spawn_cond))) return rc;
+        if ((int)spawn_cond.count != map0.n_spawn * 2 || map0.n_spawn > 64) return fail(MP_E_UNSUPPORTED, "%d conditional spawn candidates (max 64)", map0.n_spawn);
+        add_table(D.tables, &T.spawn_cond, std::vector<int32_t>(spawn_cond.data, spawn_cond.data + spawn_cond.count));
       }
     }
   }
   T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16); T.nW_pad = round_up(std::max(T.nW, 1), 16);
 
-  // ---- device copies -----------------------------------------------------------------------------
-  std::vector<int32_t> act(action_table.data, action_table.data + action_table.count);
-  if ((rc = upload(E->allocs, act, &T.action_table))) return rc;
+  add_table(D.tables, &T.action_table, std::vector<int32_t>(action_table.data, action_table.data + action_table.count));
 
   // ---- render tables ------------------------------------------------------------------------------
   if (atlas.count != (size_t)T.n_sprites * 1024) return fail(MP_E_INVALID, "atlas has %zu bytes, expected %d", atlas.count, T.n_sprites * 1024);
@@ -483,7 +492,7 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
     if ((int)pair_of[base].size() <= top) pair_of[base].resize(top + 1, 0);
     if (pair_of[base][top]) return pair_of[base][top];
     if (n_now() >= kMaxAtlasSprites) return 0;  // budget: the atlas has to fit in shared memory next to the staging buffers
-    if (E->flags & MP_FLAG_DEBUG_NO_PREMERGE) return 0;  // budget zero: every stack takes the general compositing path
+    if (flags & MP_FLAG_DEBUG_NO_PREMERGE) return 0;  // budget zero: every stack takes the general compositing path
     int id = n_now();
     img.resize((size_t)(id + 1) * 1024);
     for (int f = 0; f < 4; ++f)
@@ -590,7 +599,7 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
     }
   }
   const int n_total = n_now();
-  E->n_total = n_total;
+  D.n_total = n_total;
   // atlas re-laid out as [sprite][facing][half][row][16 B] so that the 8 rows of one half are 128
   // contiguous bytes (conflict-free 128-bit shared loads).
   std::vector<uint8_t> at((size_t)n_total * 1024);
@@ -598,7 +607,7 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
     for (int row = 0; row < 8; ++row)
       for (int half = 0; half < 2; ++half)
         memcpy(&at[(size_t)s * 256 + half * 128 + row * 16], &img[(size_t)s * 256 + row * 32 + half * 16], 16);
-  if ((rc = upload(E->allocs, at, &T.atlas))) return rc;
+  add_table(D.tables, &T.atlas, at);
   std::vector<int16_t> smap((size_t)(T.P + 1) * n_total);
   for (int v = 0; v <= T.P; ++v)
     for (int s = 0; s < n_total; ++s)
@@ -620,15 +629,15 @@ int build_tables(mp_engine* E, const void* const* blobs, const size_t* blob_size
     }
     sflags[i] = (uint8_t)((opq[i] ? 1 : 0) | (remapped[i] ? 2 : 0) | (bin ? 4 : 0) | (invisible ? 8 : 0));
   }
-  E->host_pair = pair; E->host_sflags = sflags;
-  E->black_sprite = -1;  // an opaque, never remapped, all-black sprite stands in for cells with nothing to draw
-  for (int i = 0; i < n_total && E->black_sprite < 0; ++i) {
+  D.host_pair = pair; D.host_sflags = sflags;
+  // an opaque, never remapped, all-black sprite (D.black_sprite) stands in for cells with nothing to draw
+  for (int i = 0; i < n_total && D.black_sprite < 0; ++i) {
     if (!opq[i] || remapped[i]) continue;
     bool black = true;
     for (int px = 0; px < 256 && black; ++px) { const uint8_t* q = &img[(size_t)i * 1024 + px * 4]; black = q[0] == 0 && q[1] == 0 && q[2] == 0; }
-    if (black) E->black_sprite = i;
+    if (black) D.black_sprite = i;
   }
-  if ((rc = upload(E->allocs, smap, &T.sprite_map)) || (rc = upload(E->allocs, sflags, &T.sprite_opaque)) || (rc = upload(E->allocs, pair, &T.sprite_pair))) return rc;
+  add_table(D.tables, &T.sprite_map, smap); add_table(D.tables, &T.sprite_opaque, sflags); add_table(D.tables, &T.sprite_pair, pair);
   return MP_OK;
 }
 
@@ -942,11 +951,19 @@ const char* mp_version(void) { return "meltingpot_b200 engine 0.1 (sm_90a)"; }
 }  // extern "C"
 
 namespace {
-int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host);
+int setup_variants(Decoded& D, const void* const* blobs, const size_t* blob_bytes, int n);
+int upload_tables(mp_engine* E, Decoded& D);
+int upload_variants(mp_engine* E, const Decoded& D, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host);
 
 // mp_create (one blob) and mp_create_variants (a checked variant set of n_blobs > 1, env b starting on env_variant[b]).
+// Every check of the blobs runs before the device is opened.
 int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, const uint8_t* env_variant, int num_envs, int device,
            uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out) {
+  Decoded D(n_blobs);
+  int rc = build_tables(D, blobs, blob_sizes, n_blobs, flags);
+  // before the state is sized: the variants of a map-variant engine size its entity arrays for the largest of them
+  if (rc == MP_OK && n_blobs > 1) rc = setup_variants(D, blobs, blob_sizes, n_blobs);
+  if (rc != MP_OK) return rc;
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);
   if (e != cudaSuccess || n_dev == 0) return fail(MP_E_NO_DEVICE, "no CUDA device available (%s); this engine has no CPU path", cudaGetErrorString(e));
@@ -958,9 +975,8 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
   mp_engine* E = new mp_engine();
   E->device = device; E->B = num_envs; E->flags = flags; E->sm_count = prop.multiProcessorCount;
   E->blob_hash = fnv1a(blobs[0], blob_sizes[0]);
-  int rc = build_tables(E, blobs, blob_sizes, n_blobs);
-  // before the state is sized: the variants of a map-variant engine size its entity arrays for the largest of them
-  if (rc == MP_OK && n_blobs > 1) rc = setup_variants(E, blobs, blob_sizes, n_blobs, env_variant);
+  rc = upload_tables(E, D);
+  if (rc == MP_OK && n_blobs > 1) rc = upload_variants(E, D, blobs, blob_sizes, n_blobs, env_variant);
   if (rc == MP_OK) rc = build_plan(E);
   if (rc != MP_OK) {
     const std::string msg = g_error;
@@ -975,7 +991,7 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
   {  // Worst case of events one step can emit per env: per avatar, every cell of every beam footprint can carry a hit
      // with up to three events (zap + sanctioning + removal), plus the contact / regrowth events (<= 4) and the pair
      // events of coop_mining (<= P). Sized so that emit_event never drops a row.
-    S.max_events = round_up(std::max(MP_MIN_EVENTS, T.P * (3 * E->beam_cells + 4 + T.P)), 16);
+    S.max_events = round_up(std::max(MP_MIN_EVENTS, T.P * (3 * D.beam_cells + 4 + T.P)), 16);
   }
   S.fam_u8_stride = std::max(16, RU_COUNT * T.nR_pad); S.fam_u16_stride = std::max(16, RS_COUNT * T.nR_pad);
   // reward [B][P] | discount [B] | step_type [B] | scalar_obs [n][B][P], all 8-byte elements, one block
@@ -1171,53 +1187,76 @@ int same_sections(const void* b0, size_t n0, const void* bv, size_t nv, const ch
   return rc ? rc : check(sv, hv->n_sections, b0, n0, bv);
 }
 
-// Rules (b)-(d) of mp_create_variants for an engine whose tables are built from variant 0 (build_tables), then the
-// variant set's device arrays. Runs before the engine's state is sized: a family with map variants keeps each variant's
-// map (MapVariant) and entity tables, and the State's entity arrays (T.nA_pad) are sized for the variant with the most.
-// Its variants may also differ in their beam footprints, as far as the family's same_shape allows (commons_harvest:
-// the Zapper's length and radius; coins has no beams), and State::max_events is sized for the largest footprint.
-// Every variant engine keeps the Tables of each variant (VariantSet::maps), from which an episode start reads: the
-// variants of the other families differ there in their initial grid only (the sprites of an appearance override).
-int setup_variants(mp_engine* E, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host) {
-  struct Decided { int nA, nD, nW, nR, nR_pad, end_min_frames, end_interval, beam_cells; double end_prob; };
-  std::vector<FamilyParams> params(n);
-  std::vector<Decided> decided;
-  const bool maps = E->family->map_variants;
-  // the loaders' device uploads: every variant of a plain set uses the engine's own (same sections); map variants keep theirs
-  std::vector<void*> scratch;
-  std::vector<MapVariant> map(n);
-  Tables& T = E->T;
-  int rc = MP_OK;
-  for (int v = 0; v < n && rc == MP_OK; ++v) {
-    Section<int32_t> hits;
-    if (!get_section(blobs[v], blob_bytes[v], "hits", MPB_I32, &hits)) { rc = fail(MP_E_INVALID, "blob: missing section 'hits'"); break; }
-    FamilyLoad ld{blobs[v], blob_bytes[v], hits, maps ? E->allocs : scratch};
-    if ((rc = E->family->load(ld, T, params[v]))) break;
-    decided.push_back({ld.nA, ld.nD, ld.nW, ld.nR, ld.nR_pad, ld.end_min_frames, ld.end_interval, ld.beam_cells, ld.end_prob});
-    const Decided& a = decided[0];
-    const Decided& b = decided[v];
-    if ((!maps && a.nA != b.nA) || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
+// Rules (b)-(d) of mp_create_variants for a set whose blob 0 build_tables has decoded: each variant's loader (its
+// refusal, kept by build_tables), its entity counts, episode ending, beam footprints and Params (same_shape), then its
+// map. A family with map variants keeps each variant's map (MapVariant) and entity tables, and the State's entity
+// arrays (T.nA_pad) are sized for the variant with the most. Its variants may also differ in their beam footprints, as
+// far as the family's same_shape allows (commons_harvest: the Zapper's length and radius; coins has no beams), and
+// State::max_events is sized for the largest footprint. Every variant engine keeps the Tables of each variant
+// (VariantSet::maps), from which an episode start reads: the variants of the other families differ there in their
+// initial grid only (the sprites of an appearance override).
+int setup_variants(Decoded& D, const void* const* blobs, const size_t* blob_bytes, int n) {
+  const bool maps = D.family->map_variants;
+  Tables& T = D.T;
+  const FamilyLoad& a = D.loads[0];
+  for (int v = 1; v < n; ++v) {
+    const FamilyLoad& b = D.loads[v];
+    int rc = D.load_rc[v];
+    if (rc) g_error = D.load_error[v];
+    else if ((!maps && a.nA != b.nA) || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
     else if (a.end_min_frames != b.end_min_frames || a.end_interval != b.end_interval || memcmp(&a.end_prob, &b.end_prob, sizeof a.end_prob) != 0)
       rc = fail(MP_E_UNSUPPORTED, "episode ending differs");
     else if (!maps && a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
-    else rc = E->family->same_shape(params[0], params[v]);
-    if (rc == MP_OK) rc = load_map(blobs[v], blob_bytes[v], T, E->spawn_groups, E->allocs, map[v]);
-    if (rc) g_error = "variant " + std::to_string(v) + ": " + g_error;
+    else rc = D.family->same_shape(D.params[0], D.params[v]);
+    if (rc == MP_OK) rc = load_map(blobs[v], blob_bytes[v], T, D.spawn_groups, D.tables, D.maps[v]);
+    if (rc) {
+      g_error = "variant " + std::to_string(v) + ": " + g_error;
+      return rc;
+    }
   }
-  for (void* p : scratch) cudaFree(p);
-  if (rc) return rc;
   if (maps) {
-    for (const Decided& dv : decided) { T.nA = std::max(T.nA, dv.nA); E->beam_cells = std::max(E->beam_cells, dv.beam_cells); }
+    for (const FamilyLoad& l : D.loads) { T.nA = std::max(T.nA, l.nA); D.beam_cells = std::max(D.beam_cells, l.beam_cells); }
     T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16);
   }
+  return MP_OK;
+}
+
+// Uploads every table the decode recorded and writes its device address into the field it is aimed at, then puts the
+// decoded Tables and variant 0's Params into the engine. No kernel writes these tables, so tables with the same bytes
+// share one allocation: the variants of a set point at one copy of every table they may not differ in (rule (a) of
+// mp_create_variants), as map variants do at the tables their maps share.
+int upload_tables(mp_engine* E, Decoded& D) {
+  std::map<std::vector<uint8_t>, const uint8_t*> shared;
+  auto put = [&](const std::vector<HostTable>& tables) {
+    for (const HostTable& t : tables) {
+      const uint8_t*& d = shared[t.bytes];
+      int rc;
+      if (!d && (rc = upload(E->allocs, t.bytes, &d))) return rc;
+      memcpy(t.field, &d, sizeof d);
+    }
+    return (int)MP_OK;
+  };
+  int rc = put(D.tables);
+  for (const FamilyLoad& l : D.loads) if (rc == MP_OK) rc = put(l.tables);
+  if (rc) return rc;
+  apply_map(D.T, D.maps[0]);
+  E->family = D.family; E->T = D.T; E->params = D.params[0];
+  E->n_total = D.n_total; E->black_sprite = D.black_sprite; E->host_pair = D.host_pair; E->host_sflags = D.host_sflags;
+  return MP_OK;
+}
+
+// The device arrays of a variant set: each variant's Tables (the engine's, with its map and entity count) and own Params,
+// and the env assignments.
+int upload_variants(mp_engine* E, const Decoded& D, const void* const* blobs, const size_t* blob_bytes, int n, const uint8_t* env_variant_host) {
+  int rc;
   {
-    std::vector<Tables> tv(n, T);  // T is final here: create changes nothing in it after this
-    for (int v = 0; v < n; ++v) { apply_map(tv[v], map[v]); tv[v].nA = decided[v].nA; }
+    std::vector<Tables> tv(n, E->T);  // T is final here: create changes nothing in it after this
+    for (int v = 0; v < n; ++v) { apply_map(tv[v], D.maps[v]); tv[v].nA = D.loads[v].nA; }
     const Tables* d = nullptr;
     if ((rc = upload(E->allocs, tv, &d))) return rc;
     E->variants.maps = d;
   }
-  if ((rc = E->family->upload_variants(E->allocs, E->params, params, &E->variants.params))) return rc;
+  if ((rc = E->family->upload_variants(E->allocs, D.params, &E->variants.params))) return rc;
   const size_t B = E->B;
   std::vector<uint8_t> assign(B, 0);
   if (env_variant_host) assign.assign(env_variant_host, env_variant_host + B);

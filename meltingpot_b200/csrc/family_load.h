@@ -1,5 +1,6 @@
-// family_load.h -- host side: the blob access, error reporting and device uploads that build_tables (engine.cu) and the
-// family loaders (`load` in each step_<family>.cuh) share. engine.cu is the only translation unit; it includes this
+// family_load.h -- host side: the blob access, error reporting and host tables that the decode of engine.cu
+// (build_tables, load_map) and the family loaders (`load` in each step_<family>.cuh) share, and the device upload that
+// create runs on those tables once the device is checked. engine.cu is the only translation unit; it includes this
 // header through the family headers.
 #pragma once
 
@@ -62,6 +63,19 @@ bool get_section(const void* blob, size_t n, const char* name, int dtype, Sectio
 
 int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
+// A device table decoded on the host: its bytes, and the `const T*` field of a Params, Tables or MapVariant that its
+// device address goes into (upload_tables in engine.cu).
+struct HostTable {
+  std::vector<uint8_t> bytes;
+  void* field;
+};
+
+template <typename T>
+void add_table(std::vector<HostTable>& tables, const T** field, const std::vector<T>& host) {
+  const uint8_t* p = reinterpret_cast<const uint8_t*>(host.data());
+  tables.push_back({std::vector<uint8_t>(p, p + host.size() * sizeof(T)), field});
+}
+
 // Copies `host` into a new zero-padded device allocation (at least 16 bytes), recorded in `allocs`.
 template <typename T>
 int upload(std::vector<void*>& allocs, const std::vector<T>& host, const T** out) {
@@ -112,13 +126,16 @@ struct FamilyLoad {
   const void* blob;
   size_t n;
   Section<int32_t> hits;               // [n_hits][2] layer, sprite
-  std::vector<void*>& allocs;          // the engine's device allocations
   // handed back: the Tables fields the family decides
   int nA = 0, nD = 0, nW = 0, nR = 0, nR_pad = 16;  // per-env entity counts (State's array sizes, Tables::nA...)
   int end_min_frames = 0, end_interval = 0;          // StochasticIntervalEpisodeEnding
   double end_prob = 0.0;
   int beam_cells = 0;                  // footprint cells of the beams State::max_events provides for
   std::vector<std::vector<int>> hint_stacks;  // sprite stacks (bottom up) worth a pre-merged sprite before the generic enumeration
+  std::vector<HostTable> tables;       // the device tables of its Params
+
+  template <typename T>
+  void table(const T** field, const std::vector<T>& host) { add_table(tables, field, host); }
 
   template <typename T>
   int need(const char* name, int dtype, Section<T>* out) const {
@@ -144,8 +161,8 @@ struct FamilyLoad {
 // The cell -> entity index of the n entities of section `name`, entity k standing on cell rows.data[k * row_len + 1]:
 // [cells_pad] index or -1. Refuses a section shorter than n rows or an entity off the map, so that neither this index nor
 // the kernels, which read the section's first n rows, reach past what the blob holds.
-int upload_cell_index(FamilyLoad& ld, const Tables& T, const char* name, const Section<int32_t>& rows, int n, int row_len,
-                      const int16_t** out) {
+int cell_index(FamilyLoad& ld, const Tables& T, const char* name, const Section<int32_t>& rows, int n, int row_len,
+               const int16_t** out) {
   if (n < 0 || rows.count < (size_t)n * row_len)
     return fail(MP_E_INVALID, "blob: section '%s' has %zu values for %d entities of %d", name, rows.count, n, row_len);
   std::vector<int16_t> of(T.cells_pad, -1);
@@ -154,21 +171,20 @@ int upload_cell_index(FamilyLoad& ld, const Tables& T, const char* name, const S
     if (cell < 0 || cell >= T.cells) return fail(MP_E_INVALID, "blob: section '%s' puts entity %d on cell %d of a %d-cell map", name, k, cell, T.cells);
     of[cell] = (int16_t)k;
   }
-  return upload(ld.allocs, of, out);
+  ld.table(out, of);
+  return MP_OK;
 }
 
-// Per-env variants (mp_create_variants): a family's same_shape(a, b) checks, field by field, that two Params agree on
-// everything outside the family's scalar knobs (what is staged per CTA or shapes per-env state); copy_knobs(dst, src)
-// copies those knobs. The Zapper's knobs are its cooldown, respawn, removal, penalty and reward. MP_SAME compares one field's bytes (Params are value-initialised, so padding and unused array
-// entries are zero) and names it when they differ.
+// Per-env variants (mp_create_variants): each variant runs under its own Params, and a family's same_shape(a, b) checks,
+// field by field, that two Params agree on what the kernels read from params[0] (what stage() puts in shared memory) or
+// what shapes per-env state. Every other field is the variant's own: its scalar knobs, and its table pointers, which
+// point at the same bytes wherever the variants' tables agree. MP_SAME compares one field's bytes (Params are
+// value-initialised, so padding and unused array entries are zero) and names it when they differ.
 #define MP_SAME(field)                                                                                                  \
   if (memcmp(&a.field, &b.field, sizeof(a.field)) != 0)                                                               \
     return fail(MP_E_UNSUPPORTED, "Params field '%s' differs (variants may differ only in the family's scalar knobs)", #field);
 
 #define MP_SAME_ZAPPER MP_SAME(zap.layer) MP_SAME(zap.sprite) MP_SAME(zap.hit) MP_SAME(zap.geom)
-void copy_zapper_knobs(Zapper& dst, const Zapper& src) {
-  dst.cooldown = src.cooldown; dst.respawn = src.respawn; dst.remove = src.remove; dst.penalty = src.penalty; dst.reward = src.reward;
-}
 
 // The Zapper and episode-ending slots (MPB_FP_*) of clean_up, commons_harvest and territory. The penalty and reward sit
 // in each family's own f64 slots.

@@ -62,8 +62,8 @@ struct CleanUp {
     F.dirt_prob = dp[MPB_CU_D_DIRT_PROB]; ld.end_prob = dp[MPB_CU_D_END_PROB];
     std::vector<int32_t> v_apple(apple.data, apple.data + apple.count), v_dirt(dirt.data, dirt.data + dirt.count);
     std::vector<int32_t> v_water(water.data, water.data + water.count);
-    if ((rc = upload(ld.allocs, v_apple, &F.apple)) || (rc = upload(ld.allocs, v_dirt, &F.dirt)) || (rc = upload(ld.allocs, v_water, &F.water)) ||
-        (rc = upload_cell_index(ld, T, "cu_apple", apple, ld.nA, 3, &F.apple_of_cell)) || (rc = upload_cell_index(ld, T, "cu_dirt", dirt, ld.nD, 3, &F.dirt_of_cell)))
+    ld.table(&F.apple, v_apple); ld.table(&F.dirt, v_dirt); ld.table(&F.water, v_water);
+    if ((rc = cell_index(ld, T, "cu_apple", apple, ld.nA, 3, &F.apple_of_cell)) || (rc = cell_index(ld, T, "cu_dirt", dirt, ld.nD, 3, &F.dirt_of_cell)))
       return rc;
     F.dirt_count0 = 0;
     for (int j = 0; j < ld.nD; ++j) F.dirt_count0 += v_dirt[j * 3 + 2];
@@ -77,14 +77,6 @@ struct CleanUp {
     MP_SAME_ZAPPER MP_SAME(apple_layer) MP_SAME(dirt_layer) MP_SAME(water_layer) MP_SAME(n_anim)
     MP_SAME(clean_layer) MP_SAME(clean_sprite) MP_SAME(clean_hit) MP_SAME(clean_geom) MP_SAME(dirt_count0)
     return MP_OK;
-  }
-  static void copy_knobs(Params& dst, const Params& src) {
-    copy_zapper_knobs(dst.zap, src.zap);
-    dst.clean_cooldown = src.clean_cooldown; dst.dirt_delay = src.dirt_delay; dst.dirt_prob = src.dirt_prob;
-    dst.grow_rate = src.grow_rate; dst.grow_depletion = src.grow_depletion; dst.grow_restoration = src.grow_restoration;
-    dst.eat_reward = src.eat_reward; dst.anim_frames = src.anim_frames; dst.anim_random = src.anim_random;
-    dst.apple_sprite = src.apple_sprite; dst.dirt_sprite = src.dirt_sprite;
-    memcpy(dst.water_sprite, src.water_sprite, sizeof dst.water_sprite);
   }
 
   using Scratch = WarpScratch;

@@ -43,8 +43,8 @@ struct Coins {
     F.coin_rate = dp[MPB_CO_D_REGROW_RATE]; ld.end_prob = dp[MPB_CO_D_END_PROB];
     for (int p = 0; p < 2; ++p) for (int k = 0; k < 4; ++k) F.coin_reward[p][k] = dp[MPB_CO_D_REWARD_0_SELF_MATCH + 4 * p + k];
     std::vector<int32_t> v_coin(coin.data, coin.data + coin.count);
-    if ((rc = upload(ld.allocs, v_coin, &F.coin)) || (rc = upload_cell_index(ld, T, "co_coin", coin, ld.nA, 2, &F.coin_of_cell))) return rc;
-    return MP_OK;
+    ld.table(&F.coin, v_coin);
+    return cell_index(ld, T, "co_coin", coin, ld.nA, 2, &F.coin_of_cell);
   }
 
   // Host: per-env variants may differ in the coin rewards, the regrowth rate and the termination rule, and, as draws of
@@ -52,14 +52,6 @@ struct Coins {
   static int same_shape(const Params& a, const Params& b) {
     MP_SAME(coin_layer) MP_SAME(coin_type)
     return MP_OK;
-  }
-  static void copy_knobs(Params& dst, const Params& src) {
-    memcpy(dst.coin_reward, src.coin_reward, sizeof dst.coin_reward);
-    dst.coin_rate = src.coin_rate; dst.terminate = src.terminate; dst.terminate_n = src.terminate_n;
-  }
-  static void copy_map(Params& dst, const Params& src) {
-    memcpy(dst.coin_sprite, src.coin_sprite, sizeof dst.coin_sprite);
-    dst.coin = src.coin; dst.coin_of_cell = src.coin_of_cell;
   }
 
   using Scratch = WarpScratch;

@@ -113,12 +113,12 @@ template <class F>
 struct HasResetMap<F, std::void_t<decltype(&F::reset_map)>> : std::true_type {};
 
 // A Family provides: Params (what only its kernel reads), the host-side load(FamilyLoad&, T, Params&) that decodes its
-// blob sections (family_load.h), Scratch, kStagesTables, kMapVariants (whether its variants may differ in the map, and
-// then copy_map(dst, src) on the host, which copies a variant's map-dependent Params), kMapSections and kSpriteSections
+// blob sections into Params and host tables (family_load.h), Scratch, kStagesTables, kMapVariants (whether its variants
+// may differ in the map), kMapSections and kSpriteSections
 // (the sections its variants may differ in, see same_sections in engine.cu; null if none), scratch_bytes(T) per warp, table_bytes(T) per CTA,
 // stage(T, F, tables) (copies static tables into shared memory), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
-// and step(T, F, S, b, lane, actions, sc) for either action source, and on the host same_shape(a, b) and copy_knobs(dst, src) for per-env
-// variants. `Source` is the family's Params (one blob) or ParamVariants<Params>. A single Params is a grid constant:
+// and step(T, F, S, b, lane, actions, sc) for either action source, and on the host same_shape(a, b) for per-env
+// variants, which run under their own Params. `Source` is the family's Params (one blob) or ParamVariants<Params>. A single Params is a grid constant:
 // without it, the compiler copies a small Params that is indexed with a run-time value (coins' coin_reward[who],
 // coop_mining's ore_sprite[state]) to the stack, and passed on as it is, it keeps its constant-bank reads. Variants are
 // read through the L1 from the device array.

@@ -48,10 +48,8 @@ struct Commons {
     for (int i = 0; i < 4; ++i) F.ch_probs[i] = dp[MPB_CH_D_PROB_0 + i];
     F.eat_reward = dp[MPB_CH_D_EAT_REWARD]; ld.end_prob = dp[MPB_CH_D_END_PROB];
     std::vector<int32_t> v_apple(apple.data, apple.data + apple.count), v_nbr(nbr.data, nbr.data + nbr.count);
-    if ((rc = upload(ld.allocs, v_apple, &F.ch_apple)) || (rc = upload(ld.allocs, v_nbr, &F.ch_nbr)) ||
-        (rc = upload_cell_index(ld, T, "ch_apple", apple, ld.nA, 4, &F.apple_of_cell)))
-      return rc;
-    return MP_OK;
+    ld.table(&F.ch_apple, v_apple); ld.table(&F.ch_nbr, v_nbr);
+    return cell_index(ld, T, "ch_apple", apple, ld.nA, 4, &F.apple_of_cell);
   }
 
   // Host: per-env variants may differ in the Zapper knobs and its beam footprint (length and radius), the DensityRegrow
@@ -62,16 +60,6 @@ struct Commons {
     MP_SAME(zap.layer) MP_SAME(zap.sprite) MP_SAME(zap.hit) MP_SAME(apple_layer) MP_SAME(wait_layer) MP_SAME(grass_layer)
     MP_SAME(ch_n_wait) MP_SAME(ch_n_probs)
     return MP_OK;
-  }
-  static void copy_knobs(Params& dst, const Params& src) {
-    copy_zapper_knobs(dst.zap, src.zap);
-    dst.zap.geom = src.zap.geom;
-    for (int i = 0; i < 4; ++i) dst.ch_probs[i] = src.ch_probs[i];
-    dst.eat_reward = src.eat_reward;
-    dst.apple_sprite = src.apple_sprite; dst.wait_sprite = src.wait_sprite; dst.grass_sprite = src.grass_sprite; dst.dess_sprite = src.dess_sprite;
-  }
-  static void copy_map(Params& dst, const Params& src) {
-    dst.ch_apple = src.ch_apple; dst.ch_nbr = src.ch_nbr; dst.apple_of_cell = src.apple_of_cell;
   }
 
   using Scratch = WarpScratch;

@@ -56,8 +56,8 @@ struct Mining {
     F.mine_reward[0] = dp[MPB_CM_D_MINE_REWARD_0]; F.mine_reward[1] = dp[MPB_CM_D_MINE_REWARD_1];
     F.extract_reward[0] = dp[MPB_CM_D_EXTRACT_REWARD_0]; F.extract_reward[1] = dp[MPB_CM_D_EXTRACT_REWARD_1];
     std::vector<int32_t> v_ore(ore.data, ore.data + ore.count);
-    if ((rc = upload(ld.allocs, v_ore, &F.ore)) || (rc = upload_cell_index(ld, T, "cm_ore", ore, ld.nA, 2, &F.ore_of_cell))) return rc;
-    return MP_OK;
+    ld.table(&F.ore, v_ore);
+    return cell_index(ld, T, "cm_ore", ore, ld.nA, 2, &F.ore_of_cell);
   }
 
   // Host: per-env variants may differ in the mining window, the mine cooldown, the regrowth rates, the rewards and the
@@ -65,11 +65,6 @@ struct Mining {
   static int same_shape(const Params& a, const Params& b) {
     MP_SAME(ore_layer) MP_SAME(mine_length) MP_SAME(mine_layer) MP_SAME(mine_sprite) MP_SAME(mine_hit)
     return MP_OK;
-  }
-  static void copy_knobs(Params& dst, const Params& src) {
-    dst.mine_window = src.mine_window; dst.mine_cooldown = src.mine_cooldown;
-    for (int i = 0; i < 2; ++i) { dst.mine_rate[i] = src.mine_rate[i]; dst.mine_reward[i] = src.mine_reward[i]; dst.extract_reward[i] = src.extract_reward[i]; }
-    memcpy(dst.ore_sprite, src.ore_sprite, sizeof dst.ore_sprite);
   }
 
   using Scratch = WarpScratch;

@@ -154,14 +154,14 @@ struct Territory {
     std::vector<int32_t> v_res(res.data, res.data + res.count);
     std::vector<uint8_t> wall(T.cells_pad, 0);
     memcpy(wall.data(), wall_sec.data, std::min<size_t>(wall_sec.count, T.cells));
-    if ((rc = upload(ld.allocs, v_res, &F.tr_res)) || (rc = upload_cell_index(ld, T, "tr_res", res, ld.nR, 3, &F.res_of_cell)) ||
-        (rc = upload(ld.allocs, wall, &F.wall)))
-      return rc;
+    ld.table(&F.tr_res, v_res);
+    if ((rc = cell_index(ld, T, "tr_res", res, ld.nR, 3, &F.res_of_cell))) return rc;
+    ld.table(&F.wall, wall);
     Section<int32_t> res_cond;
     if (get_section(ld.blob, ld.n, "tr_res_cond", MPB_I32, &res_cond)) {
       if ((int)res_cond.count != ld.nR * 2) return fail(MP_E_INVALID, "blob: tr_res_cond has %zu values for %d resources", res_cond.count, ld.nR);
       std::vector<int32_t> v(res_cond.data, res_cond.data + res_cond.count);
-      if ((rc = upload(ld.allocs, v, &F.tr_res_cond))) return rc;
+      ld.table(&F.tr_res_cond, v);
     }
     return MP_OK;
   }
@@ -176,21 +176,6 @@ struct Territory {
     MP_SAME(tr_taste_role) MP_SAME(brush_sprite) MP_SAME(claimbeam_sprite)
     MP_SAME(claim_geom) MP_SAME(brush_geom)
     return MP_OK;
-  }
-  static void copy_knobs(Params& dst, const Params& src) {
-    copy_zapper_knobs(dst.zap, src.zap);
-    dst.mark_initial_level = src.mark_initial_level; dst.mark_recovery = src.mark_recovery;
-    for (int l = 0; l < 3; ++l) {
-      dst.mark_inc[l] = src.mark_inc[l]; dst.mark_remove[l] = src.mark_remove[l]; dst.mark_freeze[l] = src.mark_freeze[l];
-      dst.mark_src_reward[l] = src.mark_src_reward[l]; dst.mark_tgt_reward[l] = src.mark_tgt_reward[l];
-    }
-    dst.claim_wait = src.claim_wait; dst.res_health0 = src.res_health0; dst.res_reward_delay = src.res_reward_delay;
-    dst.res_repair_delay = src.res_repair_delay; dst.res_reward = src.res_reward; dst.res_rate = src.res_rate;
-    dst.res_repair_prob = src.res_repair_prob;
-    dst.unclaimed_sprite = src.unclaimed_sprite; dst.tex_sprite = src.tex_sprite; dst.dmg_sprite = src.dmg_sprite;
-    memcpy(dst.mark_sprite, src.mark_sprite, sizeof dst.mark_sprite);
-    memcpy(dst.claimed_sprite, src.claimed_sprite, sizeof dst.claimed_sprite);
-    memcpy(dst.dry_sprite, src.dry_sprite, sizeof dst.dry_sprite);
   }
 
   using Scratch = TerritoryScratch;

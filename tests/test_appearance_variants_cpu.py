@@ -83,8 +83,8 @@ def test_compile_settings_set_checks_the_length_of_prefab_overrides():
     compiler.compile_settings_set([AV.settings('coins')], AV.config('coins'), [0], [{}, {}])
 
 
-# --- the section check of mp_create_variants (no device needed: it runs before the device is opened; the Params checks
-# that follow it run on the GPU, tests/test_gpu_appearance_variants.py) ---
+# --- the section check of mp_create_variants (no device needed: it runs before the device is opened, as do the Params
+# checks that follow it, tests/test_create_checks_cpu.py) ---
 MP_E_UNSUPPORTED, MP_E_NO_DEVICE = -2, -4
 
 

@@ -111,7 +111,7 @@ def test_refused_variant_is_refused_cleanly(name):
     if name == 'commons/dense_disc':
       assert 'more than 16 other apples' in str(e.value)
   else:
-    V.compile(name)  # the compiler accepts it; mp_create refuses it (test_gpu_param_envelope.py)
+    V.compile(name)  # the compiler accepts it; mp_create refuses it (test_create_checks_cpu.py, test_gpu_param_envelope.py)
     assert variant.refused_by == 'engine'
 
 
