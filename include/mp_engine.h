@@ -414,6 +414,46 @@ int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t*
                    int n_slots, uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players,
                    void* stream);
 
+/* Drawn routes: the row of each player is drawn again at every episode start, on the device, as a scenario's
+ * background population is resampled at every reset. Player slot p lists n_choices[p] (0..MP_MAX_ROUTE_CHOICES)
+ * choices, e.g. the bots that may fill it. In episode e of env b (Philox key k), slot p plays choice
+ *   o = pick(philox4x32_10(counter {0, e, p, 6}, key k).x, n_choices[p])     (stream 6: RS_ROUTE; pick(w, n) = w * n >> 32)
+ * that is, uniformly with replacement, independently per slot and episode. Like every other draw of the engine it is
+ * addressed by (key, episode), so it does not depend on num_envs, env_index_base or sharding, a clone plays its source's
+ * draw and MP_RESTORE_REKEY gives it its own. It is not Python's `random` stream. The row of (b, p) is then
+ *   row_base[p][o] + b * rows_per_env[p][o],
+ * and a slot without choices has no row. A group-major layout gives choice group g a block [start_g, start_g + B * n_g)
+ * with n_g the number of slots that list g, and slot p the rows start_g + rank_g(p) + b * n_g, rank_g(p) being p's
+ * position among those slots: row_base = start_g + rank_g(p), rows_per_env = n_g. The row map is WRITTEN by the call. */
+#define MP_MAX_ROUTE_CHOICES 8
+#define MP_MAX_ROUTE_PLAYERS 16
+typedef struct mp_route_draw {
+  int32_t* row_of_player; /* DEVICE i32 [B][P]: written by every call, row of player p of env b, -1 for none */
+  int32_t n_rows;
+  int32_t n_choices[MP_MAX_ROUTE_PLAYERS];  /* per player slot; entries >= P are ignored */
+  int32_t row_base[MP_MAX_ROUTE_PLAYERS][MP_MAX_ROUTE_CHOICES];
+  int32_t rows_per_env[MP_MAX_ROUTE_PLAYERS][MP_MAX_ROUTE_CHOICES];
+} mp_route_draw;
+
+/* mp_step_players / mp_reset_players on drawn routes. After every call, row_of_player[b][p] is the row the rule above
+ * gives for the episode env b is in then, for every env: one that stepped, started an episode (auto-reset, or reset),
+ * was masked out of a reset, was restored (a record's key and episode, or its own key with MP_RESTORE_REKEY) or switched
+ * variant. In mp_step_drawn, player p takes the action id in row row_of_player[b][p] of `action` (rows
+ * action_row_stride bytes apart) for the episode it is in before the step, action 0 without a row; envs that start an
+ * episode or are restored ignore their actions. For every routed (b, p) the call gives, byte for byte, what
+ * mp_step_routed (with players) and mp_reset_players give when handed the map as a fixed input, and it launches the same
+ * kernels, as many of them. players->row_of_player and players->n_rows must be the draw's map and n_rows.
+ * Every check runs before anything is enqueued, and a refused call (MP_E_INVALID) steps no env. Refused besides every
+ * refusal of mp_step_routed (with players) / mp_reset_players: a NULL draw, draw n_rows < 1, players whose map or n_rows
+ * are not the draw's, a slot with more than MP_MAX_ROUTE_CHOICES choices (or fewer than 0), and a choice whose rows of
+ * some env fall outside [0, n_rows). The map must not overlap any target, the action rows, the bank, the index array or
+ * the engine's buffers; MP_E_UNSUPPORTED while the observation gather is enabled, as for mp_step_players. */
+int mp_step_drawn(mp_handle h, const mp_route_draw* draw, const int32_t* action, uint64_t action_row_stride,
+                  const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, const mp_device_outputs* out,
+                  const mp_player_outputs* players, void* stream);
+int mp_reset_drawn(mp_handle h, const uint8_t* env_mask, const mp_route_draw* draw, const mp_device_outputs* out,
+                   const mp_player_outputs* players, void* stream);
+
 /* Diagnostic: how the renderer was laid out for this substrate: teams per CTA, threads per team, log2 of the pixel
  * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes,
  * then the lane -> cell dealing built for player strips and for WORLD.RGB strips (0 plain, 2 scattered colouring,

@@ -28,8 +28,8 @@
 enum { ENV_STEP = 0, ENV_EPISODE = 1, ENV_DONE = 2, ENV_DIRT = 3, ENV_CLEANED = 4, ENV_ATE = 5, ENV_BEAM = 6, ENV_COLS = 8 };
 enum { AV_X = 0, AV_Y = 1, AV_ORIENT = 2, AV_ALIVE = 3 };
 enum { TM_ZAP = 0, TM_BEAM2 = 1, TM_FRAME = 2 };
-// RNG streams: must match oracle/mp_oracle.c (the RNG addressing is part of the engine policy).
-enum { RS_SCENE = 0, RS_AVATAR = 1, RS_OBJECT = 2, RS_AVATAR_RESET = 3, RS_OBJECT_RESET = 4, RS_CHOICE = 5 };
+// RNG streams: must match oracle/mp_oracle.c (the RNG addressing is part of the engine policy); RS_ROUTE (drawn routes only) by tests/drawn_routes.py.
+enum { RS_SCENE = 0, RS_AVATAR = 1, RS_OBJECT = 2, RS_AVATAR_RESET = 3, RS_OBJECT_RESET = 4, RS_CHOICE = 5, RS_ROUTE = 6 };
 enum { SCENE_DRAW_DIRT = 0, SCENE_DRAW_EPISODE_END = 1 };
 
 struct BeamGeom {  // one beam footprint, cells in visiting order (policy A.8)

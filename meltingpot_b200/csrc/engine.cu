@@ -23,6 +23,8 @@
 #include "step_mining.cuh"
 #include "state_bank.cuh"
 
+static_assert(MP_MAX_ROUTE_CHOICES == MP_ROUTE_CHOICES && MP_MAX_ROUTE_PLAYERS == MP_MAX_PLAYERS,
+              "mp_route_draw's table is DrawnActions'");
 namespace {
 
 constexpr int kRenderSmemLimit = 227 * 1024 - 2560;  // dynamic shared memory: the 227 KB opt-in maximum less k_render's static arrays
@@ -152,10 +154,10 @@ struct FamilyEntry {
   // own Params
   int (*same_shape)(const FamilyParams&, const FamilyParams&);
   int (*upload_variants)(std::vector<void*>&, const std::vector<FamilyParams>&, const void**);
-  // Every k_step<Family, ...> an engine may launch, [variants][restore][routed]: Source Params or ParamVariants<Params>
-  // (mp_create_variants), kRestore (a step that restores envs from a bank), Actions DenseActions or RowActions
-  // (mp_step_routed).
-  const void* step[2][2][2];
+  // Every k_step<Family, ...> an engine may launch, [variants][restore][actions]: Source Params or ParamVariants<Params>
+  // (mp_create_variants), kRestore (a step that restores envs from a bank), and the action source: DenseActions,
+  // RowActions (mp_step_routed) or drawn routes (k_step_drawn: mp_step_drawn, and mp_reset_drawn without restore).
+  const void* step[2][2][3];
   // Launches `kernel`, one of `step`, with the kernel arguments `args` after filling in its Source argument (args[1]):
   // `params` for one blob, or the ParamVariants<Params> of `variants`.
   cudaError_t (*launch)(const cudaLaunchConfig_t&, const void* kernel, void** args, const FamilyParams& params, const VariantSet& variants);
@@ -190,16 +192,20 @@ template <class Family, class Source, bool kRestore, class Actions>
 const void* step_kernel() {
   return reinterpret_cast<const void*>(k_step<Family, Source, kRestore, Actions>);
 }
+template <class Family, class Source, bool kRestore>
+const void* drawn_kernel() {
+  return reinterpret_cast<const void*>(k_step_drawn<Family, Source, kRestore>);
+}
 template <class Family>
 FamilyEntry family_entry(int id) {
   using P = typename Family::Params;
   using V = ParamVariants<P>;
   return {id, Family::kMapVariants, Family::kMapSections, Family::kSpriteSections, load_family<Family>, step_smem_bytes<Family>,
           same_shape_family<Family>, upload_variants_family<Family>,
-          {{{step_kernel<Family, P, false, DenseActions>(), step_kernel<Family, P, false, RowActions>()},
-            {step_kernel<Family, P, true, DenseActions>(), step_kernel<Family, P, true, RowActions>()}},
-           {{step_kernel<Family, V, false, DenseActions>(), step_kernel<Family, V, false, RowActions>()},
-            {step_kernel<Family, V, true, DenseActions>(), step_kernel<Family, V, true, RowActions>()}}},
+          {{{step_kernel<Family, P, false, DenseActions>(), step_kernel<Family, P, false, RowActions>(), drawn_kernel<Family, P, false>()},
+            {step_kernel<Family, P, true, DenseActions>(), step_kernel<Family, P, true, RowActions>(), drawn_kernel<Family, P, true>()}},
+           {{step_kernel<Family, V, false, DenseActions>(), step_kernel<Family, V, false, RowActions>(), drawn_kernel<Family, V, false>()},
+            {step_kernel<Family, V, true, DenseActions>(), step_kernel<Family, V, true, RowActions>(), drawn_kernel<Family, V, true>()}}},
           launch_family<Family>};
 }
 const FamilyEntry kFamilies[] = {
@@ -752,8 +758,9 @@ int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
 // `render_follows`: the caller launches the renderer next on the same stream; it raises the exchange flags.
 // `restore`: a step (mode 0) that restores the envs it names instead of advancing them (k_step<..., true>), or null.
 // `rows`: the step's actions come from rows (mp_step_routed, k_step<..., RowActions>; `actions` unused), or null.
+// `drawn`: drawn routes (k_step_drawn, which writes the row map; `actions` and `rows` unused), or null.
 int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int mode, cudaStream_t st, bool render_follows = true,
-                 const StepRestore* restore = nullptr, const RowActions* rows = nullptr) {
+                 const StepRestore* restore = nullptr, const RowActions* rows = nullptr, const DrawnActions* drawn = nullptr) {
   const int blocks = (E->B + 3) / 4;
   if (E->S.x_world) E->S.x_step = ++E->x_seq;
   cudaLaunchConfig_t cfg = {};
@@ -764,8 +771,9 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   cfg.attrs = attr; cfg.numAttrs = 1;
   StepRestore restore_arg = restore ? *restore : StepRestore{};
   RowActions rows_arg = rows ? *rows : RowActions{};
-  void* args[] = {&E->T, nullptr, &E->S, &actions, &mask, &mode, &restore_arg, &rows_arg};  // k_step's parameters; Source by `launch`
-  const void* kernel = E->family->step[E->variants.n > 1][restore != nullptr][rows != nullptr];
+  void* args[] = {&E->T, nullptr, &E->S, &actions, &mask, &mode, &restore_arg,
+                  drawn ? const_cast<DrawnActions*>(drawn) : static_cast<void*>(&rows_arg)};  // k_step's parameters; Source by `launch`
+  const void* kernel = E->family->step[E->variants.n > 1][restore != nullptr][drawn ? 2 : rows != nullptr];
   CUDA_TRY(E->family->launch(cfg, kernel, args, E->params, E->variants));
   if (E->S.x_world) {
     E->x_pending_raise = true;
@@ -1867,8 +1875,29 @@ int check_player_actions(mp_engine* E, const mp_player_actions* a, const mp_play
   return MP_OK;
 }
 
+// The checks of mp_step_drawn / mp_reset_drawn's `draw` (include/mp_engine.h). Its row map is `players`' own, whose
+// extent check_player_outputs appends (check_call requires `players` for these calls).
+int check_route_draw(mp_engine* E, const mp_route_draw* d, const mp_player_outputs* players, const char* fn) {
+  if (!d) return fail(MP_E_INVALID, "%s: null draw", fn);
+  if (d->n_rows < 1) return fail(MP_E_INVALID, "%s: draw n_rows %d < 1", fn, d->n_rows);
+  if (players && (players->row_of_player != d->row_of_player || players->n_rows != d->n_rows))
+    return fail(MP_E_INVALID, "%s: players must deliver through the draw's row map and n_rows", fn);
+  for (int p = 0; p < E->T.P; ++p) {
+    const int n = d->n_choices[p];
+    if (n < 0 || n > MP_MAX_ROUTE_CHOICES)
+      return fail(MP_E_INVALID, "%s: player %d has %d choices, not 0..%d", fn, p, n, MP_MAX_ROUTE_CHOICES);
+    for (int j = 0; j < n; ++j) {
+      const int64_t base = d->row_base[p][j], per_env = d->rows_per_env[p][j];
+      if (base < 0 || per_env < 0 || base + (int64_t)(E->B - 1) * per_env >= d->n_rows)
+        return fail(MP_E_INVALID, "%s: choice %d of player %d (row base %lld, %lld rows per env) leaves rows [0, %d) for %d envs",
+                    fn, j, p, (long long)base, (long long)per_env, d->n_rows, E->B);
+    }
+  }
+  return MP_OK;
+}
+
 // The restore of a call that may restore envs from a state bank (mp_state_restore, mp_step_restore, mp_step_players,
-// mp_step_routed): slot_of_env and bank, or neither; MP_RESTORE_REKEY or no flags.
+// mp_step_routed, mp_step_drawn): slot_of_env and bank, or neither; MP_RESTORE_REKEY or no flags.
 struct RestoreArgs { const int32_t* slot_of_env = nullptr; const void* bank = nullptr; int n_slots = 0; uint32_t flags = 0; };
 
 int check_restore(const RestoreArgs& r, const char* fn) {
@@ -1886,8 +1915,9 @@ struct StateCall {
   int mode;        // k_step's: 0 step, 1 reset
   const uint8_t* mask = nullptr;            // reset: the envs to reset, or null for all
   const int32_t* actions = nullptr;         // step: dense actions [B][P]
-  bool routed = false;                      // step: actions from `rows` instead (mp_step_routed)
+  bool routed = false;                      // step: actions from `rows` instead (mp_step_routed, mp_step_drawn)
   const mp_player_actions* rows = nullptr;
+  const mp_route_draw* draw = nullptr;      // drawn routes (mp_step_drawn, mp_reset_drawn): the rows' map is written
   RestoreArgs restore;
   const mp_device_outputs* out = nullptr;   // targets (check_device_outputs)
   bool needs_out = false;                   // refuse a null `out`
@@ -1896,11 +1926,12 @@ struct StateCall {
   bool render_follows = true;               // launch_state's; false launches k_exchange_push as mp_step does
 };
 
-// Every check of `c`, in the order the entry points document: restore, row actions, player rows, then the bank, targets
-// and extents together. A call with nothing to check does no check work.
+// Every check of `c`, in the order the entry points document: restore, drawn routes, row actions, player rows, then the
+// bank, targets and extents together. A call with nothing to check does no check work.
 int check_call(mp_engine* E, const StateCall& c) {
   int rc = check_restore(c.restore, c.fn);
   std::vector<DeviceExtent> ext;
+  if (!rc && c.draw) rc = check_route_draw(E, c.draw, c.players, c.fn);
   if (!rc && c.routed) rc = check_player_actions(E, c.rows, c.players, c.fn, ext);
   if (!rc && (c.players || c.needs_players)) rc = check_player_outputs(E, c.players, c.out, c.fn, ext);
   if (rc) return rc;
@@ -1921,8 +1952,18 @@ int run_call(mp_engine* E, const StateCall& c, void* stream) {
                             (r.flags & MP_RESTORE_REKEY) ? 1 : 0, E->key_base};
   RowActions rows{};
   if (c.routed) rows = {c.rows->row_of_player, reinterpret_cast<const uint8_t*>(c.rows->action), c.rows->action_row_stride, c.rows->n_rows};
+  DrawnActions drawn{};
+  if (c.draw) {
+    const mp_route_draw& d = *c.draw;
+    drawn.row_of_player = d.row_of_player; drawn.action = reinterpret_cast<const uint8_t*>(rows.action); drawn.stride = rows.stride;
+    drawn.n_rows = d.n_rows;
+    memcpy(drawn.n_choices, d.n_choices, sizeof drawn.n_choices);
+    memcpy(drawn.base, d.row_base, sizeof drawn.base);
+    memcpy(drawn.per_env, d.rows_per_env, sizeof drawn.per_env);
+  }
   const cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = launch_state(E, c.actions, c.mask, c.mode, st, c.render_follows, r.bank ? &restore : nullptr, c.routed ? &rows : nullptr)))
+  if ((rc = launch_state(E, c.actions, c.mask, c.mode, st, c.render_follows, r.bank ? &restore : nullptr, c.routed ? &rows : nullptr,
+                         c.draw ? &drawn : nullptr)))
     return rc;
   return launch_render(E, st, c.out, c.players);
 }
@@ -2007,6 +2048,25 @@ int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t*
   StateCall c{"mp_step_routed", 0};
   c.routed = true; c.rows = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out; c.players = players;
   c.render_follows = out || players;  // launched as the composed call: mp_step, mp_step_into, mp_step_restore or mp_step_players
+  return run_call(h, c, stream);
+}
+
+int mp_step_drawn(mp_handle h, const mp_route_draw* draw, const int32_t* action, uint64_t action_row_stride, const int32_t* slot_of_env,
+                  const void* bank, int n_slots, uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players,
+                  void* stream) {
+  if (!h || !draw) return fail(MP_E_INVALID, "mp_step_drawn: null handle or draw");
+  const mp_player_actions rows{draw->row_of_player, draw->n_rows, action, action_row_stride};
+  StateCall c{"mp_step_drawn", 0};
+  c.routed = true; c.rows = &rows; c.draw = draw; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out;
+  c.players = players; c.needs_players = true;
+  return run_call(h, c, stream);
+}
+
+int mp_reset_drawn(mp_handle h, const uint8_t* env_mask, const mp_route_draw* draw, const mp_device_outputs* out,
+                   const mp_player_outputs* players, void* stream) {
+  if (!h || !draw) return fail(MP_E_INVALID, "mp_reset_drawn: null handle or draw");
+  StateCall c{"mp_reset_drawn", 1};
+  c.mask = env_mask; c.draw = draw; c.out = out; c.players = players; c.needs_players = true;
   return run_call(h, c, stream);
 }
 

@@ -107,6 +107,30 @@ __device__ __forceinline__ const Actions& select_actions(const DenseActions& den
   else return dense;
 }
 
+// Drawn routes (mp_step_drawn / mp_reset_drawn, k_step_drawn): each episode, player slot p of env b plays choice
+// o = pick(philox(0, episode, p, RS_ROUTE).x, n_choices[p]) under env b's key (uniform with replacement per slot and
+// episode, like choice_present), and its row is base[p][o] + b * per_env[p][o]; a slot without choices has no row. The
+// step reads player p's action from the row of the episode it is in, and writes every env's row map after the advance
+// (row_of_player[b][p]: the row of the episode env b is in now, -1 for no row), which the render that follows reads.
+// mp_step_drawn checks every row of the table against [0, n_rows) for every env, so a drawn row is always in range.
+#define MP_ROUTE_CHOICES 8  // = MP_MAX_ROUTE_CHOICES (include/mp_engine.h)
+struct DrawnActions {
+  int32_t* row_of_player;  // [B][P], written
+  const uint8_t* action;   // [n_rows] x i32
+  uint64_t stride;
+  int n_rows;
+  int32_t n_choices[MP_MAX_PLAYERS];
+  int32_t base[MP_MAX_PLAYERS][MP_ROUTE_CHOICES];
+  int32_t per_env[MP_MAX_PLAYERS][MP_ROUTE_CHOICES];
+};
+
+__device__ __forceinline__ int drawn_row(const DrawnActions& d, int b, int p, int episode, uint32_t k0, uint32_t k1) {
+  const int n = d.n_choices[p];
+  if (n <= 0) return -1;
+  const int o = (int)pick(philox4x32_10(0u, (uint32_t)episode, (uint32_t)p, RS_ROUTE, k0, k1).x, (uint32_t)n);
+  return d.base[p][o] + b * d.per_env[p][o];
+}
+
 template <class F, class = void>
 struct HasResetMap : std::false_type {};
 template <class F>
@@ -128,7 +152,59 @@ struct HasResetMap<F, std::void_t<decltype(&F::reset_map)>> : std::true_type {};
 // LAST; the record carries the timestep and the events, so event_begin / event_end are skipped too. Every other warp
 // runs the plain step. With kRestore = false, `restore` is never read and the kernel is the plain step.
 // Actions: DenseActions (`actions`; `rows` is never read), or RowActions (`rows`; launched by mp_step_routed only, mode 0,
-// and `actions` is never read).
+// and `actions` is never read); k_step_drawn reads DrawnActions.
+//
+// k_step's body as a function, for k_step_drawn: stages the family's tables, waits for the kernel before, then restores
+// or advances (or, masked out of a reset, leaves) this warp's env. Returns the env, or -1 for a warp past the batch.
+// k_step keeps its own copy of these lines: calling this function from it schedules the 40 k_step instantiations
+// differently (32 of them got other SASS, 17 other register or spill counts), which the copy avoids.
+template <class Family, class Source, bool kRestore, class Actions>
+__device__ __forceinline__ int advance_env(const Tables& T, const Source& src, const State& S, const uint8_t* __restrict__ mask,
+                                           int mode, const StepRestore& restore, const Actions& acts) {
+  constexpr bool kVariants = !std::is_same<Source, typename Family::Params>::value;
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // Programmatic dependent launch, both ways: let the renderer that follows in the stream stage its tables while this
+  // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  uint8_t* tables = smem + 4 * Family::scratch_bytes(T);
+  if constexpr (Family::kStagesTables) {  // before the dependency wait: the tables never change
+    if constexpr (kVariants) Family::stage(T, src.params[0], tables);
+    else Family::stage(T, src, tables);
+  }
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if constexpr (Family::kStagesTables) __syncthreads();
+  const int b = blockIdx.x * 4 + warp;
+  if (b >= S.B) return -1;
+  if constexpr (kRestore) {
+    if (restore_env(*restore.layout, restore.slot_of_env, restore.bank, restore.n_slots, b, lane, restore.rekey, restore.key_base)) return b;
+  }
+  typename Family::Scratch sc = Family::carve(T, smem + warp * Family::scratch_bytes(T), tables);
+  if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
+    event_begin(lane);
+    if constexpr (kVariants) {
+      const bool reset = mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE];
+      const int k = env_variant(src, b, lane, reset);
+      const typename Family::Params& F = src.params[k];
+      if constexpr (Family::kMapVariants) {
+        const Tables& Tm = src.maps[k];
+        if (reset) {
+          if constexpr (HasResetMap<Family>::value) Family::reset_map(Tm, F, S, b, lane, sc);
+          else Family::reset(Tm, F, S, b, lane, sc);
+        } else Family::template step<Actions>(Tm, F, S, b, lane, acts, sc);
+      } else {  // the variants differ in their initial grid only (appearance overrides): an episode start reads maps[k]
+        if (reset) Family::reset(src.maps[k], F, S, b, lane, sc);
+        else Family::template step<Actions>(T, F, S, b, lane, acts, sc);
+      }
+    } else {
+      if (mode == 1 || S.env[(size_t)b * ENV_COLS + ENV_DONE]) Family::reset(T, src, S, b, lane, sc);
+      else Family::template step<Actions>(T, src, S, b, lane, acts, sc);
+    }
+    event_end(S, b, lane);
+  }
+  return b;
+}
+
 template <class Family, class Source = typename Family::Params, bool kRestore = false, class Actions = DenseActions>
 __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant__ Source src, State S, const int32_t* __restrict__ actions,
                                                  const uint8_t* __restrict__ mask, int mode, const __grid_constant__ StepRestore restore,
@@ -174,6 +250,25 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
       else Family::template step<Actions>(T, src, S, b, lane, acts, sc);
     }
     event_end(S, b, lane);
+  }
+}
+
+// k_step with drawn routes (mp_step_drawn, mode 0, and mp_reset_drawn, mode 1): the same advance, with actions from
+// the rows of DrawnActions; then every env's row map is written from the episode and key the env now has, whether it
+// advanced, started an episode, was restored (a record's key, or its own with rekey) or was masked out of a reset.
+// `actions` and `rows` are those of k_step, so one argument list launches either kernel; neither is read here.
+template <class Family, class Source = typename Family::Params, bool kRestore = false>
+__global__ void __launch_bounds__(128, 8) k_step_drawn(Tables T, const __grid_constant__ Source src, State S, const int32_t* __restrict__ actions,
+                                                       const uint8_t* __restrict__ mask, int mode, const __grid_constant__ StepRestore restore,
+                                                       const __grid_constant__ DrawnActions drawn) {
+  const int b = advance_env<Family, Source, kRestore, DrawnActions>(T, src, S, mask, mode, restore, drawn);
+  if (b < 0) return;
+  __syncwarp();  // the env row and key were written by lanes of this warp
+  const int lane = threadIdx.x & 31;
+  if (lane < T.P) {
+    const uint64_t key = *reinterpret_cast<volatile const uint64_t*>(S.key + b);
+    const int episode = *reinterpret_cast<volatile const int32_t*>(S.env + (size_t)b * ENV_COLS + ENV_EPISODE);
+    drawn.row_of_player[(size_t)b * T.P + lane] = drawn_row(drawn, b, lane, episode, (uint32_t)key, (uint32_t)(key >> 32));
   }
 }
 
@@ -292,10 +387,21 @@ __device__ __forceinline__ void reset_env_row(const Tables& T, const State& S, i
 // are read-only for the whole step, so they are read through the non-coherent path.
 __device__ __forceinline__ bool has_actions(DenseActions actions) { return actions != nullptr; }
 __device__ __forceinline__ bool has_actions(const RowActions&) { return true; }
-__device__ __forceinline__ int action_id(DenseActions actions, size_t i) { return __ldg(actions + i); }
-__device__ __forceinline__ int action_id(const RowActions& a, size_t i) {
+__device__ __forceinline__ bool has_actions(const DrawnActions&) { return true; }
+__device__ __forceinline__ int action_id(DenseActions actions, const State&, int b, int P, int lane) {
+  const size_t i = (size_t)b * P + lane;
+  return __ldg(actions + i);
+}
+__device__ __forceinline__ int action_id(const RowActions& a, const State&, int b, int P, int lane) {
+  const size_t i = (size_t)b * P + lane;
   const int row = __ldg(a.row_of_player + i);
   return (uint32_t)row < (uint32_t)a.n_rows ? __ldg(reinterpret_cast<const int32_t*>(a.action + (size_t)row * a.stride)) : 0;
+}
+// The row of the episode a stepping env is in (its key is never written by a stepping env's warp, see KeyWord).
+__device__ __forceinline__ int action_id(const DrawnActions& a, const State& S, int b, int, int lane) {
+  const uint64_t key = __ldg(reinterpret_cast<const unsigned long long*>(S.key + b));
+  const int row = drawn_row(a, b, lane, S.env[(size_t)b * ENV_COLS + ENV_EPISODE], (uint32_t)key, (uint32_t)(key >> 32));
+  return row >= 0 ? __ldg(reinterpret_cast<const int32_t*>(a.action + (size_t)row * a.stride)) : 0;
 }
 
 // This lane's avatar (x, y, orientation, alive), its timers, and its action decoded by the action table
@@ -309,7 +415,7 @@ __device__ __forceinline__ void load_avatar(const Tables& T, const State& S, int
     av = *reinterpret_cast<const int4*>(S.avatar + ((size_t)b * T.P + lane) * 4);
     timer = *reinterpret_cast<const int4*>(S.av_timer + ((size_t)b * T.P + lane) * 4);
     if (has_actions(actions)) {
-      int id = action_id(actions, (size_t)b * T.P + lane);
+      int id = action_id(actions, S, b, T.P, lane);
       if (id < 0 || id >= T.n_actions) id = 0;
       act = *reinterpret_cast<const int4*>(act_table + id * 4);
     }

@@ -61,7 +61,7 @@ EXPORTED_SYMBOLS = (
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
     'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
     'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_step_restore',
-    'mp_step_players', 'mp_reset_players', 'mp_step_routed',
+    'mp_step_players', 'mp_reset_players', 'mp_step_routed', 'mp_step_drawn', 'mp_reset_drawn',
 )
 
 MP_RESTORE_REKEY = 1
@@ -195,6 +195,32 @@ class MpPlayerActions(ctypes.Structure):
   ]
 
 
+MP_MAX_ROUTE_CHOICES = 8
+MP_MAX_ROUTE_PLAYERS = 16
+
+
+class MpRouteDraw(ctypes.Structure):
+  _fields_ = [
+      ('row_of_player', ctypes.c_void_p), ('n_rows', ctypes.c_int32),
+      ('n_choices', ctypes.c_int32 * MP_MAX_ROUTE_PLAYERS),
+      ('row_base', (ctypes.c_int32 * MP_MAX_ROUTE_CHOICES) * MP_MAX_ROUTE_PLAYERS),
+      ('rows_per_env', (ctypes.c_int32 * MP_MAX_ROUTE_CHOICES) * MP_MAX_ROUTE_PLAYERS),
+  ]
+
+
+def describe_draw(row_of_player, n_rows: int, row_base, rows_per_env) -> MpRouteDraw:
+  """The mp_route_draw of drawn routes: row_of_player is the CUDA int32 [B, P] map the engine writes, row_base[p] and
+  rows_per_env[p] list the row base and rows per env of each of slot p's choices (as many as it has)."""
+  d = MpRouteDraw()
+  d.row_of_player = ctypes.c_void_p(int(row_of_player.data_ptr()))
+  d.n_rows = int(n_rows)
+  for p, (bases, per_env) in enumerate(zip(row_base, rows_per_env)):
+    d.n_choices[p] = len(bases)
+    for j, (r, n) in enumerate(zip(bases, per_env)):
+      d.row_base[p][j], d.rows_per_env[p][j] = int(r), int(n)
+  return d
+
+
 def describe_player_actions(player_actions: Mapping[str, Any], num_envs: int, num_players: int, device: int) -> MpPlayerActions:
   """The mp_player_actions of `player_actions`: 'row_of_player' (TensorLayout of a contiguous int32 CUDA [B, P]) and
   'action' (int32 [n_rows], any row stride). Only shapes, dtypes, devices and layouts are checked, never the values."""
@@ -322,6 +348,10 @@ def load_library() -> ctypes.CDLL:
   lib.mp_reset_players.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_step_routed.argtypes = [vp, ctypes.POINTER(MpPlayerActions), vp, vp, ctypes.c_int, ctypes.c_uint32,
                                  ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
+  lib.mp_step_drawn.argtypes = [vp, ctypes.POINTER(MpRouteDraw), vp, ctypes.c_uint64, vp, vp, ctypes.c_int, ctypes.c_uint32,
+                                ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
+  lib.mp_reset_drawn.argtypes = [vp, vp, ctypes.POINTER(MpRouteDraw), ctypes.POINTER(MpDeviceOutputs),
+                                 ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
   lib.mp_step_host_async.argtypes = [vp, vp, ctypes.POINTER(MpHostOutputs), ctypes.c_int, vp]
@@ -514,13 +544,19 @@ class Engine:
   def set_flags(self, flags: int) -> None:
     _check(self._lib.mp_set_flags(self._h, ctypes.c_uint32(flags)))
 
-  def reset(self, mask=None, stream=None, out=None, players=None) -> None:
-    """out, players: as for step."""
+  def reset(self, mask=None, stream=None, out=None, players=None, draw=None) -> None:
+    """out, players, draw: as for step."""
     ptr = None
     if mask is not None:
       assert mask.dtype == self._torch.uint8 and mask.is_cuda and mask.numel() == self.num_envs
       ptr = ctypes.c_void_p(mask.data_ptr())
-    if players is not None:
+    if draw is not None:
+      if players is None:
+        raise ValueError('draw needs players')
+      s = None if out is None else ctypes.byref(self._device_outputs(out))
+      _check(self._lib.mp_reset_drawn(self._h, ptr, ctypes.byref(draw), s, ctypes.byref(self._player_outputs(players)),
+                                      self._stream(stream)))
+    elif players is not None:
       s = None if out is None else ctypes.byref(self._device_outputs(out))
       _check(self._lib.mp_reset_players(self._h, ptr, s, ctypes.byref(self._player_outputs(players)), self._stream(stream)))
     elif out is None:
@@ -530,7 +566,7 @@ class Engine:
       _check(self._lib.mp_reset_into(self._h, ptr, ctypes.byref(s), self._stream(stream)))
 
   def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False, players=None,
-           player_actions=None) -> None:
+           player_actions=None, draw=None) -> None:
     """actions: int32 CUDA tensor [B, P] of discrete action ids, or None with player_actions.
 
     out: {name: CUDA tensor} for any of DEVICE_OUTPUTS (mp_step_into): the step's images are rendered straight into
@@ -556,7 +592,13 @@ class Engine:
     player_actions: actions read from rows (mp_step_routed), {'row_of_player': contiguous CUDA int32 [B, P],
     'action': CUDA int32 [n_rows], any stride}, with actions None. Player p of env b takes action[row_of_player[b, p]]
     when that row lies in 0..n_rows-1, and action 0 (NOOP) otherwise. The row map may be players' own. Combines with
-    out, players and restore / bank; the result is that of the same call with the dense actions those rows give."""
+    out, players and restore / bank; the result is that of the same call with the dense actions those rows give.
+
+    draw: drawn routes (mp_step_drawn; an MpRouteDraw from describe_draw), with players and player_actions whose
+    row_of_player is the draw's map: the step writes the map (each player's row for the episode its env is in
+    afterwards) and reads each player's action from the row of the episode it is in before the step."""
+    if draw is not None and (players is None or player_actions is None):
+      raise ValueError('draw needs players and player_actions')
     if player_actions is not None:
       if actions is not None:
         raise ValueError('give actions or player_actions, not both')
@@ -570,7 +612,10 @@ class Engine:
     flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
     s = None if out is None else ctypes.byref(self._device_outputs(out))
     p = None if players is None else ctypes.byref(self._player_outputs(players))
-    if player_actions is not None:
+    if draw is not None:
+      _check(self._lib.mp_step_drawn(self._h, ctypes.byref(draw), pa.action, pa.action_row_stride, idx, bank_ptr, n_slots,
+                                     ctypes.c_uint32(flags), s, p, self._stream(stream)))
+    elif player_actions is not None:
       _check(self._lib.mp_step_routed(self._h, ctypes.byref(pa), idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, p,
                                       self._stream(stream)))
     elif players is not None:

@@ -11,6 +11,9 @@ SURVEY.md section 8f, row N2. Mirrors `meltingpot/utils/scenarios/scenario.py`:
     group 0 and background players group 1 of `BatchedSubstrate.player_routes`, so each step draws
     their observations straight into focal and background rows and reads their actions from rows
     laid out the same way. The background policy is a callable on the background `BatchedTimeStep`.
+    With `roles` and `bots_by_role` it plays a background population instead, as the reference's `Population`
+    (`utils/scenarios/population.py`) does: each background slot draws one of its role's bots at every episode start,
+    on the device (`BatchedSubstrate.drawn_routes`), and each bot's policy acts on its own rows.
 
 Scenario configs (`meltingpot/configs/scenarios`) name SavedModel bots and are not compiled here.
 """
@@ -18,7 +21,7 @@ Scenario configs (`meltingpot/configs/scenarios`) name SavedModel bots and are n
 from __future__ import annotations
 
 import dataclasses
-from typing import Any, Callable, Collection, Dict, Mapping, Sequence, Tuple
+from typing import Any, Collection, Dict, Mapping, Sequence, Tuple
 
 from meltingpot_b200 import substrate as substrate_lib
 
@@ -155,10 +158,20 @@ class BatchedScenario:
   and scalar observations straight into rows of new tensors, focal rows first, each group laid out [B, n, ...] in slot
   order, and reads their actions from rows laid out the same way. A returned timestep's per-player tensors therefore
   stay valid after the next step.
+
+  Population mode (`roles` and `bots_by_role` given): `roles[p]` is the role of player slot p and `bots_by_role` maps
+  each background slot's role to the names of the bots that may fill it; `background_policy` maps each bot name to a
+  callable `policy(timestep, active) -> int tensor [B, n_k]`. At every episode start of every env, each background slot
+  plays a bot drawn uniformly with replacement from its role's bots, as the reference's `Population.reset` does
+  (`population.py:114-128`), though not from Python's `random` stream. Bot k's rows hold every slot that may play it,
+  [B, n_k] in slot order; its callable gets their timestep and `active` (bool [B, n_k]: the rows played this episode)
+  and returns an action for each row. Inactive rows are neither rendered nor read. `background_bots()` tells which bot
+  each background slot plays. Focal players are routed as without a population.
   """
 
-  def __init__(self, substrate: substrate_lib.BatchedSubstrate, background_policy: Callable[[Any], Any],
-               is_focal: Sequence[bool], permitted_observations: Collection[str]) -> None:
+  def __init__(self, substrate: substrate_lib.BatchedSubstrate, background_policy, is_focal: Sequence[bool],
+               permitted_observations: Collection[str], *, roles: Sequence[str] = None,
+               bots_by_role: Mapping[str, Collection[str]] = None) -> None:
     import numpy as np  # pylint: disable=g-import-not-at-top
     if len(is_focal) != substrate.num_players:
       raise ValueError(f'is_focal is length {len(is_focal)} but substrate is '
@@ -171,11 +184,43 @@ class BatchedScenario:
     self.num_envs = substrate.num_envs
     self.num_focal = sum(self._is_focal)
     self.num_background = substrate.num_players - self.num_focal
-    groups = np.tile(np.array([0 if f else 1 for f in self._is_focal], np.int64), (self.num_envs, 1))
-    self._routes = substrate.player_routes(groups)
+    self.bot_names: Tuple[str, ...] = ()
+    if bots_by_role is None:
+      if roles is not None:
+        raise ValueError('roles needs bots_by_role')
+      groups = np.tile(np.array([0 if f else 1 for f in self._is_focal], np.int64), (self.num_envs, 1))
+      self._routes = substrate.player_routes(groups)
+      n = self._routes.n_rows  # every player is routed: B * P rows, focal rows first
+      self._background_rows = slice(self.num_envs * self.num_focal, n)
+    else:
+      self._routes = substrate.drawn_routes(self._population_choices(background_policy, roles, bots_by_role))
     self._actions = self._routes.actions()
-    n = self._routes.n_rows  # every player is routed: B * P rows, focal rows first
-    self._focal_rows, self._background_rows = slice(0, self.num_envs * self.num_focal), slice(self.num_envs * self.num_focal, n)
+    self._focal_rows = slice(0, self.num_envs * self.num_focal)
+
+  def _population_choices(self, policies, roles, bots_by_role):
+    """Validates population mode and returns each slot's groups for drawn_routes: group 0 for focal slots, group
+    1 + k for bot k of bot_names (the bots that some background slot may play, sorted)."""
+    if roles is None:
+      raise ValueError('bots_by_role needs roles, the role of each player slot')
+    if isinstance(roles, str) or len(roles) != len(self._is_focal):
+      raise ValueError('roles and is_focal must be the same length.')
+    names_by_role = {role: tuple(sorted(set(names))) for role, names in bots_by_role.items()}
+    background_roles = [role for role, f in zip(roles, self._is_focal) if not f]
+    for role in background_roles:
+      if role not in names_by_role:
+        raise ValueError(f'no bots for role {role!r}: bots_by_role has roles {sorted(names_by_role)}')
+      if not names_by_role[role]:
+        raise ValueError(f'bots_by_role[{role!r}] is empty')
+      if len(names_by_role[role]) > 8:
+        raise ValueError(f'bots_by_role[{role!r}] lists {len(names_by_role[role])} bots, at most 8')
+    self.bot_names = tuple(sorted({n for role in background_roles for n in names_by_role[role]}))
+    if not isinstance(policies, Mapping):
+      raise ValueError('with bots_by_role, background_policy must map each bot name to a callable')
+    for name in self.bot_names:
+      if not callable(policies.get(name)):
+        raise ValueError(f'background_policy has no callable for bot {name!r}')
+    index = {n: k for k, n in enumerate(self.bot_names)}
+    return [(0,) if f else tuple(1 + index[n] for n in names_by_role[role]) for role, f in zip(roles, self._is_focal)]
 
   def _outputs(self):
     """Fresh row tensors for one step (every row is written, so they are not zeroed)."""
@@ -202,7 +247,12 @@ class BatchedScenario:
                                          discount=timestep.discount, observation=obs)
 
   def _split(self, timestep, po):
-    self._background_timestep = self._select(timestep, po, self._background_rows, self.num_background, None)
+    if self.bot_names:
+      r = self._routes
+      self._background_timestep = {n: self._select(timestep, po, r.rows(k + 1), len(r.group(k + 1)), None)
+                                   for k, n in enumerate(self.bot_names)}
+    else:
+      self._background_timestep = self._select(timestep, po, self._background_rows, self.num_background, None)
     return self._select(timestep, po, self._focal_rows, self.num_focal, self._permitted)
 
   def reset(self):
@@ -215,7 +265,13 @@ class BatchedScenario:
       raise ValueError(f'Expected {self.num_focal} focal actions per env, got shape {tuple(focal_actions.shape)}.')
     rows = self._actions.tensor
     rows[self._focal_rows].view(self.num_envs, self.num_focal).copy_(focal_actions)
-    if self.num_background:
+    if self.bot_names:
+      r = self._routes
+      for k, name in enumerate(self.bot_names):
+        g = k + 1
+        actions = self._policy[name](self._background_timestep[name], r.active(g))
+        rows[r.rows(g)].view(self.num_envs, len(r.group(g))).copy_(actions)
+    elif self.num_background:
       background_actions = self._policy(self._background_timestep)
       rows[self._background_rows].view(self.num_envs, self.num_background).copy_(background_actions)
     po = self._outputs()
@@ -223,8 +279,20 @@ class BatchedScenario:
 
   @property
   def background_timestep(self):
-    """What the background players saw last (unrestricted observations)."""
+    """What the background players saw last (unrestricted observations); in population mode, a dict of each bot's."""
     return self._background_timestep
+
+  def background_bots(self):
+    """Population mode: int64 CUDA [B, num_background], the index in bot_names of the bot each background slot plays
+    in the episode its env is in (from the routes' row map, with torch ops on the current stream)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    if not self.bot_names:
+      raise ValueError('background_bots needs population mode (roles and bots_by_role)')
+    r = self._routes
+    slots = [p for p, f in enumerate(self._is_focal) if not f]
+    starts = torch.tensor([r.rows(g).start for g in range(1, r.num_groups)], dtype=torch.int64, device=r.device)
+    rows = r.row_of_player[:, slots].to(torch.int64)
+    return torch.bucketize(rows, starts, right=True) - 1
 
   def close(self):
     self._substrate.close()

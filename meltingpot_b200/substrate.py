@@ -20,7 +20,7 @@ from __future__ import annotations
 
 import dataclasses
 import json
-from typing import Any, Callable, Collection, Dict, List, Mapping, Optional, Sequence
+from typing import Any, Callable, Collection, Dict, List, Mapping, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -244,8 +244,10 @@ class BatchedSubstrate:
   def reset(self, mask=None, out: Optional[BatchedTimeStep] = None, players: Optional['PlayerOutputs'] = None) -> BatchedTimeStep:
     """out, players: as for step."""
     if players is not None:
+      routes = getattr(players, 'routes', None)
       self._engine.reset(mask, out=None if out is None else self._engine_outputs(out, routed=players),
-                         players=self._routed_outputs(players))
+                         players=self._routed_outputs(players),
+                         draw=routes.draw if isinstance(routes, DrawnRoutes) else None)
       return self._without_rgb(self._timestep() if out is None else self._fill_collective(out))
     if out is None:
       self._engine.reset(mask)
@@ -259,6 +261,13 @@ class BatchedSubstrate:
     import torch  # pylint: disable=g-import-not-at-top
     return PlayerRoutes(groups, self.num_envs, self.num_players, tuple(self._engine.rgb.shape[2:]), self._scalar_names,
                         torch.device('cuda', self._engine.device))
+
+  def drawn_routes(self, choices) -> 'DrawnRoutes':
+    """Rows for per-player delivery that are drawn again at every episode start: choices[p] is a sequence of group ids
+    (e.g. the bots that may fill slot p), empty for a player nobody reads. See DrawnRoutes."""
+    import torch  # pylint: disable=g-import-not-at-top
+    return DrawnRoutes(choices, self.num_envs, self.num_players, tuple(self._engine.rgb.shape[2:]), self._scalar_names,
+                       torch.device('cuda', self._engine.device))
 
   def step(self, actions=None, out: Optional[BatchedTimeStep] = None, restore=None, bank=None,
            rekey: bool = False, players: Optional['PlayerOutputs'] = None,
@@ -283,9 +292,17 @@ class BatchedSubstrate:
     player_actions: a PlayerActions (`player_routes(groups).actions()`, or `.at(t)` of one with T slots), with actions
     None: each routed player takes the action in its row, an unrouted player action 0 (NOOP). The routes may be the
     players' own, so a learner reads observations from rows and writes actions into the same rows. Combines with out,
-    players and restore / bank."""
+    players and restore / bank.
+
+    players and player_actions of one DrawnRoutes (`drawn_routes(choices)`) go together: the step draws each player's
+    row again at every episode start (see DrawnRoutes)."""
     import torch  # pylint: disable=g-import-not-at-top
     kw = dict(restore=restore, bank=bank, rekey=rekey)
+    routes, action_routes = getattr(players, 'routes', None), getattr(player_actions, 'routes', None)
+    if isinstance(routes, DrawnRoutes) or isinstance(action_routes, DrawnRoutes):
+      if routes is not action_routes:
+        raise ValueError('drawn routes: give players and player_actions of the same DrawnRoutes')
+      kw['draw'] = routes.draw
     if player_actions is not None:
       if actions is not None:
         raise ValueError('give actions or player_actions, not both')
@@ -317,7 +334,7 @@ class BatchedSubstrate:
   def _routed_outputs(self, po: 'PlayerOutputs'):
     """The engine's per-player targets of a PlayerOutputs (the scalar observations as one [n, n_rows] view)."""
     if not isinstance(po, PlayerOutputs):
-      raise ValueError('players must be a PlayerOutputs (player_routes(groups).outputs())')
+      raise ValueError('players must be a PlayerOutputs (player_routes(groups).outputs() or drawn_routes(choices).outputs())')
     r = po.routes
     self._check_routes(r, 'players')
     if po.T is not None:
@@ -538,6 +555,102 @@ class PlayerRoutes:
 
   def actions(self, T: Optional[int] = None) -> 'PlayerActions':
     """A zeroed int32 CUDA tensor of actions, one per row: [n_rows], or [T, n_rows] with T, whose `at(t)` is slot t."""
+    return PlayerActions(self, T)
+
+
+class DrawnRoutes:
+  """Where each player's outputs go when the rows are drawn per env and episode (BatchedSubstrate.drawn_routes).
+
+  choices[p] lists the groups player slot p may play in (up to 8, e.g. the bots that may fill a background slot; empty
+  for a player nobody reads). At every episode start of every env, each slot draws one of its choices, uniformly with
+  replacement and independently per slot and episode, on the device (the draw is addressed by the env's key and episode,
+  like every other draw of the engine, so it does not depend on num_envs or env_index_base, and a restored clone plays
+  its source's draw). It is not Python's `random` stream. Listing a group twice for one slot doubles its weight.
+
+  Rows are laid out group-major: group g has capacity n_g, the number of slots that list g, and its block `rows(g)` is
+  [B, n_g] in env, then slot order; `group(g)` names those n_g slots. Player p of env b sits in row
+  start_g + b * n_g + rank_g(p) of the group it drew, rank_g(p) being p's position in group(g); the other rows of the
+  block are inactive this episode: not rendered, their actions not read. Every step and reset writes
+    row_of_player  int32 CUDA [B, P]: each player's row for the episode its env is in, -1 if it has no choices;
+  `active(g)` derives which rows of group g are played from it. outputs(T) and actions(T) are as for PlayerRoutes; pass
+  both to BatchedSubstrate.step (players=, player_actions=) and the outputs to reset (players=)."""
+
+  __slots__ = ('num_envs', 'num_players', 'num_groups', 'n_rows', 'device', 'row_of_player', 'choices', 'draw',
+               '_starts', '_members', '_rgb_shape', '_scalar_names')
+
+  def __init__(self, choices, num_envs: int, num_players: int, rgb_shape, scalar_names: Sequence[str], device):
+    """rgb_shape: one player's [h, w, 3]; device: where the tensors live (a CUDA device for the engine)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    from meltingpot_b200 import engine as engine_lib  # pylint: disable=g-import-not-at-top
+    if isinstance(choices, (str, bytes)) or len(choices) != num_players:
+      raise ValueError(f'choices must list the groups of each of the {num_players} player slots')
+    norm = []
+    for p, c in enumerate(choices):
+      if isinstance(c, (str, bytes)) or not isinstance(c, Sequence) and not isinstance(c, np.ndarray):
+        raise ValueError(f'choices[{p}] must be a sequence of group ids')
+      c = tuple(c)
+      if len(c) > engine_lib.MP_MAX_ROUTE_CHOICES:
+        raise ValueError(f'choices[{p}] lists {len(c)} groups, at most {engine_lib.MP_MAX_ROUTE_CHOICES}')
+      for g in c:
+        if isinstance(g, (bool, np.bool_)) or not isinstance(g, (int, np.integer)) or g < 0:
+          raise ValueError(f'choices[{p}]: group ids must be integers >= 0, got {g!r}')
+      norm.append(tuple(int(g) for g in c))
+    if not any(norm):
+      raise ValueError('choices routes no player (every slot lists no group)')
+    n_groups = max(max(c) for c in norm if c) + 1
+    members = tuple(tuple(p for p, c in enumerate(norm) if g in c) for g in range(n_groups))
+    starts = [0]
+    for g in range(n_groups):
+      starts.append(starts[-1] + num_envs * len(members[g]))
+    if starts[-1] >= 2**31:
+      raise ValueError('more than 2^31 - 1 rows')
+    row_base = [[starts[g] + members[g].index(p) for g in c] for p, c in enumerate(norm)]
+    rows_per_env = [[len(members[g]) for g in c] for c in norm]
+    dev = torch.device(device)
+    set_ = lambda k, v: object.__setattr__(self, k, v)
+    set_('num_envs', int(num_envs)); set_('num_players', int(num_players)); set_('num_groups', n_groups)
+    set_('n_rows', starts[-1]); set_('device', dev); set_('choices', tuple(norm))
+    set_('_starts', tuple(starts)); set_('_members', members)
+    set_('_rgb_shape', tuple(int(x) for x in rgb_shape)); set_('_scalar_names', tuple(scalar_names))
+    set_('row_of_player', torch.full((num_envs, num_players), -1, dtype=torch.int32, device=dev))
+    set_('draw', engine_lib.describe_draw(self.row_of_player, self.n_rows, row_base, rows_per_env))
+
+  def __setattr__(self, name, value):
+    raise AttributeError('DrawnRoutes is immutable; build a new one with drawn_routes(choices)')
+
+  def _check_group(self, g: int) -> None:
+    if not 0 <= g < self.num_groups:
+      raise IndexError(f'group {g} outside 0..{self.num_groups - 1}')
+
+  def rows(self, g: int) -> slice:
+    """The rows of group g, [B, n_g] in env-major order (empty for a group id no slot lists)."""
+    self._check_group(g)
+    return slice(self._starts[g], self._starts[g + 1])
+
+  def group(self, g: int) -> Tuple[int, ...]:
+    """The player slots that list group g, in rank order: column k of rows(g) viewed as [B, n_g] belongs to slot
+    group(g)[k] whenever that slot drew g."""
+    self._check_group(g)
+    return self._members[g]
+
+  def active(self, g: int):
+    """bool CUDA [B, n_g]: which rows of group g are played in the episode each env is in (from row_of_player, with
+    torch ops on the current stream)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    r = self.rows(g)
+    n = r.stop - r.start
+    flat = self.row_of_player.reshape(-1).to(torch.int64)
+    inside = (flat >= r.start) & (flat < r.stop)
+    act = torch.zeros(n + 1, dtype=torch.bool, device=self.device)  # the last entry takes every other player
+    act.scatter_(0, torch.where(inside, flat - r.start, n), True)
+    return act[:n].view(self.num_envs, len(self._members[g]))
+
+  def outputs(self, T: Optional[int] = None) -> 'PlayerOutputs':
+    """As PlayerRoutes.outputs."""
+    return PlayerOutputs(self, T)
+
+  def actions(self, T: Optional[int] = None) -> 'PlayerActions':
+    """As PlayerRoutes.actions."""
     return PlayerActions(self, T)
 
 
