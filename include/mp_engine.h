@@ -127,11 +127,13 @@ int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uin
  *   - the entity counts, the episode ending and the beam footprints agree;
  *   - the family's parameters differ only in its scalar knobs (cooldowns, rewards, probabilities, rates, delays, ...):
  *     layers, sprites, hit ids, beam shapes and whatever sizes per-env state agree.
- * Two families take map variants: blobs compiled as one set on one sprite table (compiler.compile_settings_set), such as
- * the draws of coins' config builder or commons_harvest__open, __closed and __partnership. Their variants may also
- * differ in the map: the initial grid, the object, kind and state tables, the walls (BeamBlocker bits), the spawn
- * points, the family's entity tables (coins: the coins; commons_harvest: the apples and their regrowth discs), the
- * entity count, the object, kind, state and component counts of "meta", and the sprite of each state and avatar. An env
+ * Four families take map variants: blobs compiled as one set on one sprite table (compiler.compile_settings_set), such
+ * as the draws of coins' config builder, commons_harvest__open, __closed and __partnership, or layouts of one territory
+ * or coop_mining map. Their variants may also differ in the map: the initial grid, the object, kind and state tables,
+ * the walls (BeamBlocker bits), the spawn points, the family's entity tables (coins: the coins; commons_harvest: the
+ * apples and their regrowth discs; territory: the resources, walls and the resources' 'choice' conditions; coop_mining:
+ * the ores), the entity count, the object, kind, state and component counts of "meta", and the sprite of each state and
+ * avatar. An env
  * plays its variant's map, which changes only at an episode start. Every other "meta" field (size, layers, players,
  * view, ...), the sprite table, the other avatar columns, the hits and the episode ending still agree. commons_harvest
  * variants may also differ in the Zapper's beam footprint (its beamLength / beamRadius, such as the longer beam of

@@ -1443,3 +1443,23 @@ def compile_substrate_set(name: str, roles: Optional[Sequence[str]] = None,
   finally:
     random.setstate(state)
   return compile_settings_set(settings_list, config, list(build_seeds), prefab_overrides)
+
+
+def compile_substrate_maps(name: str, roles: Optional[Sequence[str]], maps: Sequence[str],
+                           root: Optional[str] = None) -> List[bytes]:
+  """The builds of a named reference substrate with each of `maps` as its ASCII map, as one map set on one sprite table
+  (compile_settings_set). A territory map replaces `config.layout.ascii_map`, which territory.py's builder turns into
+  the level's map; any other substrate's (coop_mining) replaces the map of its lab2d settings. Needs a reference
+  checkout."""
+  config = load_reference_config(name, root)
+  roles = tuple(roles) if roles is not None else tuple(config.default_player_roles)
+  settings_list = []
+  for ascii_map in maps:
+    if 'layout' in config and 'ascii_map' in config.layout:
+      config.layout.ascii_map = ascii_map
+      settings_list.append(config.lab2d_settings_builder(roles=roles, config=config))
+    else:
+      settings = config.lab2d_settings_builder(roles=roles, config=config)
+      settings['simulation']['map'] = ascii_map
+      settings_list.append(settings)
+  return compile_settings_set(settings_list, config)

@@ -149,7 +149,7 @@ struct FamilyEntry {
   const char* const* map_sections;  // Family::kMapSections: its own entity tables, which such variants may differ in, or null
   const char* const* sprite_sections;  // Family::kSpriteSections: its int32 tables that hold nothing but sprite ids, or null
   int (*load)(FamilyLoad&, const Tables&, FamilyParams&);
-  size_t (*step_smem)(const Tables&);
+  size_t (*step_smem)(const Tables&, bool variants);
   // per-env variants: same_shape(a, b) (MP_OK or MP_E_UNSUPPORTED naming the field) and the upload of every variant's
   // own Params
   int (*same_shape)(const FamilyParams&, const FamilyParams&);
@@ -1029,7 +1029,7 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
     if (ce == cudaSuccess) ce = cudaMemcpy(S.key, key0.data(), key0.size() * sizeof(uint64_t), cudaMemcpyHostToDevice);
     if (ce != cudaSuccess) { mp_destroy(E); return fail(MP_E_CUDA, "cudaMemcpy(env / key) failed: %s", cudaGetErrorString(ce)); }
   }
-  E->step_smem = E->family->step_smem(T);
+  E->step_smem = E->family->step_smem(T, n_blobs > 1);
   {  // cells per lane per strip: ceil(view_w / 4) for player rows, ceil(W / 8) for world half-rows
     const int ncp = (E->R.view_w + 3) / 4, ncw = (T.W + (32 >> E->R.wstrip_log2) - 1) / (32 >> E->R.wstrip_log2);
 #define MP_RENDER_INST(NCP, NCW)                                                                                  \
@@ -1211,7 +1211,7 @@ int setup_variants(Decoded& D, const void* const* blobs, const size_t* blob_byte
     const FamilyLoad& b = D.loads[v];
     int rc = D.load_rc[v];
     if (rc) g_error = D.load_error[v];
-    else if ((!maps && a.nA != b.nA) || a.nD != b.nD || a.nW != b.nW || a.nR != b.nR || a.nR_pad != b.nR_pad) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
+    else if ((!maps && (a.nA != b.nA || a.nR != b.nR || a.nR_pad != b.nR_pad)) || a.nD != b.nD || a.nW != b.nW) rc = fail(MP_E_UNSUPPORTED, "entity counts differ");
     else if (a.end_min_frames != b.end_min_frames || a.end_interval != b.end_interval || memcmp(&a.end_prob, &b.end_prob, sizeof a.end_prob) != 0)
       rc = fail(MP_E_UNSUPPORTED, "episode ending differs");
     else if (!maps && a.beam_cells != b.beam_cells) rc = fail(MP_E_UNSUPPORTED, "beam footprints differ");
@@ -1223,7 +1223,10 @@ int setup_variants(Decoded& D, const void* const* blobs, const size_t* blob_byte
     }
   }
   if (maps) {
-    for (const FamilyLoad& l : D.loads) { T.nA = std::max(T.nA, l.nA); D.beam_cells = std::max(D.beam_cells, l.beam_cells); }
+    for (const FamilyLoad& l : D.loads) {
+      T.nA = std::max(T.nA, l.nA); T.nR = std::max(T.nR, l.nR); T.nR_pad = std::max(T.nR_pad, l.nR_pad);
+      D.beam_cells = std::max(D.beam_cells, l.beam_cells);
+    }
     T.nA_pad = round_up(std::max(T.nA, 1), 16); T.nD_pad = round_up(std::max(std::max(T.nD, T.nA), 1), 16);
   }
   return MP_OK;
@@ -1259,7 +1262,7 @@ int upload_variants(mp_engine* E, const Decoded& D, const void* const* blobs, co
   int rc;
   {
     std::vector<Tables> tv(n, E->T);  // T is final here: create changes nothing in it after this
-    for (int v = 0; v < n; ++v) { apply_map(tv[v], D.maps[v]); tv[v].nA = D.loads[v].nA; }
+    for (int v = 0; v < n; ++v) { apply_map(tv[v], D.maps[v]); tv[v].nA = D.loads[v].nA; tv[v].nR = D.loads[v].nR; }
     const Tables* d = nullptr;
     if ((rc = upload(E->allocs, tv, &d))) return rc;
     E->variants.maps = d;

@@ -49,21 +49,33 @@ __device__ __forceinline__ WarpScratch carve_scratch(const Tables& T, uint8_t* b
   return s;
 }
 
-// Dynamic shared memory of one step launch: four env warps' scratch, then the family's per-CTA tables.
+// A map-variant engine of a family that stages tables (territory) stages them per warp, from the env's own map, after the
+// dependency wait and the env's variant promotion: the four envs of a CTA may play four maps (see k_step).
+template <class Family, class Source>
+constexpr bool kWarpTables = Family::kStagesTables && Family::kMapVariants && !std::is_same<Source, typename Family::Params>::value;
+
+// Dynamic shared memory of one step launch: four env warps' scratch, then the family's per-CTA tables (one copy per warp
+// with kWarpTables).
 template <class Family>
-__host__ __device__ inline size_t step_smem_bytes(const Tables& T) { return 4 * Family::scratch_bytes(T) + Family::table_bytes(T); }
+__host__ __device__ inline size_t step_smem_bytes(const Tables& T, bool variants) {
+  const bool per_warp = variants && Family::kStagesTables && Family::kMapVariants;
+  return 4 * Family::scratch_bytes(T) + (per_warp ? 4 : 1) * Family::table_bytes(T);
+}
 
 // mode 0: step (envs whose last step was LAST start a new episode instead, policy A.17)
 // mode 1: reset envs selected by `mask` (all if null)
 //
 // Per-env parameter variants (mp_create_variants): env b runs under params[active[b]]. An episode start first takes the
 // env's pending assignment (active[b] = pending[b]), so a reassignment never changes an episode that is under way.
-// Every variant stages the same per-CTA tables (the compatibility check of mp_create_variants), so stage() reads params[0].
-// A family with kMapVariants (coins, commons_harvest) also advances under maps[active[b]]: the engine's Tables with that
-// variant's initial grid, static occupancy, BeamBlocker bits, spawn points, avatar sprites and entity count (the State's
-// entity arrays are sized for the largest variant). Such a family may provide reset_map, which then starts the episodes
-// of map-variant engines instead of reset (commons_harvest: its reset writes only the map's own apples). The map is only ever read through the env's active variant, which changes at an episode start, so
-// an env's map changes there too and never mid-episode. The Tables are read from the device array through the L1: a
+// The variants of a family without map variants stage the same per-CTA tables (the compatibility check of
+// mp_create_variants), so stage() reads params[0].
+// A family with kMapVariants (coins, commons_harvest, territory, coop_mining) also advances under maps[active[b]]: the
+// engine's Tables with that variant's initial grid, static occupancy, BeamBlocker bits, spawn points, avatar sprites and
+// entity count (the State's entity arrays are sized for the largest variant). Such a family may provide reset_map, which
+// then starts the episodes of map-variant engines instead of reset (it also zeroes the env's entity bytes past its map's
+// count). A map-variant family that stages tables (territory) stages them per warp (kWarpTables), from the env's own
+// variant, once the dependency wait and the promotion have fixed it. The map is only ever read through the env's active
+// variant, which changes at an episode start, so an env's map changes there too and never mid-episode. The Tables are read from the device array through the L1: a
 // local copy of the kernel's Tables with the variant's fields swapped in would sit on the stack (392 bytes for coins,
 // since avatar_sprite is indexed by lane).
 // The variants of any other family may differ in their initial grid (appearance overrides: which sprite each piece
@@ -140,7 +152,8 @@ struct HasResetMap<F, std::void_t<decltype(&F::reset_map)>> : std::true_type {};
 // blob sections into Params and host tables (family_load.h), Scratch, kStagesTables, kMapVariants (whether its variants
 // may differ in the map), kMapSections and kSpriteSections
 // (the sections its variants may differ in, see same_sections in engine.cu; null if none), scratch_bytes(T) per warp, table_bytes(T) per CTA,
-// stage(T, F, tables) (copies static tables into shared memory), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
+// stage(T, F, tables) (copies static tables into shared memory; with kMapVariants also stage_warp(T, F, tables, lane),
+// one warp's copy), carve(T, warp_base, tables), reset(T, F, S, b, lane, sc)
 // and step(T, F, S, b, lane, actions, sc) for either action source, and on the host same_shape(a, b) for per-env
 // variants, which run under their own Params. `Source` is the family's Params (one blob) or ParamVariants<Params>. A single Params is a grid constant:
 // without it, the compiler copies a small Params that is indexed with a run-time value (coins' coin_reward[who],
@@ -168,17 +181,19 @@ __device__ __forceinline__ int advance_env(const Tables& T, const Source& src, c
   // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   uint8_t* tables = smem + 4 * Family::scratch_bytes(T);
-  if constexpr (Family::kStagesTables) {  // before the dependency wait: the tables never change
+  constexpr bool kCtaTables = Family::kStagesTables && !kWarpTables<Family, Source>;
+  if constexpr (kCtaTables) {  // before the dependency wait: the tables never change
     if constexpr (kVariants) Family::stage(T, src.params[0], tables);
     else Family::stage(T, src, tables);
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  if constexpr (Family::kStagesTables) __syncthreads();
+  if constexpr (kCtaTables) __syncthreads();
   const int b = blockIdx.x * 4 + warp;
   if (b >= S.B) return -1;
   if constexpr (kRestore) {
     if (restore_env(*restore.layout, restore.slot_of_env, restore.bank, restore.n_slots, b, lane, restore.rekey, restore.key_base)) return b;
   }
+  if constexpr (kWarpTables<Family, Source>) tables += warp * Family::table_bytes(T);
   typename Family::Scratch sc = Family::carve(T, smem + warp * Family::scratch_bytes(T), tables);
   if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
     event_begin(lane);
@@ -188,6 +203,10 @@ __device__ __forceinline__ int advance_env(const Tables& T, const Source& src, c
       const typename Family::Params& F = src.params[k];
       if constexpr (Family::kMapVariants) {
         const Tables& Tm = src.maps[k];
+        if constexpr (kWarpTables<Family, Source>) {  // this env's map, known only now
+          Family::stage_warp(Tm, F, tables, lane);
+          __syncwarp();
+        }
         if (reset) {
           if constexpr (HasResetMap<Family>::value) Family::reset_map(Tm, F, S, b, lane, sc);
           else Family::reset(Tm, F, S, b, lane, sc);
@@ -217,17 +236,19 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
   // grid drains, and do not touch env state before the kernel that precedes this one (the previous render) is complete.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   uint8_t* tables = smem + 4 * Family::scratch_bytes(T);
-  if constexpr (Family::kStagesTables) {  // before the dependency wait: the tables never change
+  constexpr bool kCtaTables = Family::kStagesTables && !kWarpTables<Family, Source>;
+  if constexpr (kCtaTables) {  // before the dependency wait: the tables never change
     if constexpr (kVariants) Family::stage(T, src.params[0], tables);
     else Family::stage(T, src, tables);
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  if constexpr (Family::kStagesTables) __syncthreads();
+  if constexpr (kCtaTables) __syncthreads();
   const int b = blockIdx.x * 4 + warp;
   if (b >= S.B) return;
   if constexpr (kRestore) {
     if (restore_env(*restore.layout, restore.slot_of_env, restore.bank, restore.n_slots, b, lane, restore.rekey, restore.key_base)) return;
   }
+  if constexpr (kWarpTables<Family, Source>) tables += warp * Family::table_bytes(T);
   typename Family::Scratch sc = Family::carve(T, smem + warp * Family::scratch_bytes(T), tables);
   if (!(mode == 1 && !(mask == nullptr || mask[b]))) {
     event_begin(lane);
@@ -237,6 +258,10 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
       const typename Family::Params& F = src.params[k];
       if constexpr (Family::kMapVariants) {
         const Tables& Tm = src.maps[k];
+        if constexpr (kWarpTables<Family, Source>) {  // this env's map, known only now
+          Family::stage_warp(Tm, F, tables, lane);
+          __syncwarp();
+        }
         if (reset) {
           if constexpr (HasResetMap<Family>::value) Family::reset_map(Tm, F, S, b, lane, sc);
           else Family::reset(Tm, F, S, b, lane, sc);

@@ -68,8 +68,10 @@ struct Mining {
   }
 
   using Scratch = WarpScratch;
-  static constexpr bool kMapVariants = false;
-  static constexpr const char* const* kMapSections = nullptr;
+  // Maps of one set may differ in their walls, ores and spawn points: the ore table is their entity table, and the ore
+  // count is the nA of each variant's Tables (setup_variants).
+  static constexpr bool kMapVariants = true;
+  static constexpr const char* kMapSections[] = {"cm_ore", nullptr};
   static constexpr const char* const* kSpriteSections = nullptr;
   static constexpr bool kStagesTables = false;
   __host__ __device__ static size_t scratch_bytes(const Tables& T) { return warp_scratch_bytes(T); }
@@ -105,6 +107,14 @@ struct Mining {
       }
     }
     reset_env_row(T, S, b, lane, episode, 0);
+  }
+
+  // Episode start of an env of a map-variant engine: also zeroes the env's ore bytes past this map's ores, up to the
+  // padding of the largest map (as Commons::reset_map does for apples).
+  __device__ static void reset_map(const Tables& T, const Params& F, const State& S, int b, int lane, WarpScratch& sc) {
+    for (int k = T.nA + lane; k < T.nA_pad; k += 32) { S.apple[(size_t)b * T.nA_pad + k] = 0; S.apple_count[(size_t)b * T.nA_pad + k] = 0; }
+    for (int k = T.nA + lane; k < T.nD_pad; k += 32) S.dirt[(size_t)b * T.nD_pad + k] = 0;
+    reset(T, F, S, b, lane, sc);
   }
 
   template <class Actions>

@@ -179,8 +179,11 @@ struct Territory {
   }
 
   using Scratch = TerritoryScratch;
-  static constexpr bool kMapVariants = false;
-  static constexpr const char* const* kMapSections = nullptr;
+  // Maps of one set (same size, topology, players and 'choice' groups) may differ in their walls, resources and spawn
+  // points: the resource table, the walls and the resources' 'choice' conditions are their entity tables, and the resource
+  // count is the nR of each variant's Tables (nR_pad is the largest map's, setup_variants).
+  static constexpr bool kMapVariants = true;
+  static constexpr const char* kMapSections[] = {"tr_res", "tr_wall", "tr_res_cond", nullptr};
   // Its tables that hold only sprite ids (per player: claimed, dry, brush and claim-beam sprites): variants of one set may
   // differ there (mp_create_variants), as far as same_shape allows.
   static constexpr const char* kSpriteSections[] = {"tr_player_sprites", nullptr};
@@ -196,6 +199,18 @@ struct Territory {
     int32_t* s_res_obj = reinterpret_cast<int32_t*>(tb);
     for (int i = threadIdx.x; i < T.cells_pad; i += (int)blockDim.x) { s_wall[i] = F.wall[i] ? 255 : 0; s_res_of[i] = F.res_of_cell[i]; }
     for (int i = threadIdx.x; i < T.nR_pad; i += (int)blockDim.x) { s_res_cell[i] = i < T.nR ? (int16_t)F.tr_res[i * 3 + 1] : (int16_t)0; s_res_obj[i] = i < T.nR ? F.tr_res[i * 3] : 0; }
+  }
+
+  // The same tables for one env of a map-variant engine, by its warp, from its own map (T: that map's Tables, whose
+  // nR_pad is the largest map's). stage() keeps its own copy of these lines: sharing them changed the SASS of the
+  // single-blob kernels.
+  __device__ static void stage_warp(const Tables& T, const Params& F, uint8_t* tb, int lane) {
+    uint8_t* s_wall = tb; tb += scratch_round16(T.cells_pad);
+    int16_t* s_res_of = reinterpret_cast<int16_t*>(tb); tb += scratch_round16((size_t)T.cells_pad * 2);
+    int16_t* s_res_cell = reinterpret_cast<int16_t*>(tb); tb += (size_t)T.nR_pad * 2;
+    int32_t* s_res_obj = reinterpret_cast<int32_t*>(tb);
+    for (int i = lane; i < T.cells_pad; i += 32) { s_wall[i] = F.wall[i] ? 255 : 0; s_res_of[i] = F.res_of_cell[i]; }
+    for (int i = lane; i < T.nR_pad; i += 32) { s_res_cell[i] = i < T.nR ? (int16_t)F.tr_res[i * 3 + 1] : (int16_t)0; s_res_obj[i] = i < T.nR ? F.tr_res[i * 3] : 0; }
   }
 
   __device__ static TerritoryScratch carve(const Tables& T, uint8_t* base, const uint8_t* tb) {
@@ -553,6 +568,19 @@ struct Territory {
     init(T, F, S, b, lane, sc, f.grid, f.episode, f.k0, f.k1);
     reset_env_row(T, S, b, lane, f.episode, 0);
     frame<DenseActions>(T, F, S, b, lane, nullptr, sc, f);
+  }
+
+  // Episode start of an env of a map-variant engine: also zeroes the env's resource bytes past this map's resources, up
+  // to the padding of the largest map, so that an env that moved from a map with more resources keeps none of their
+  // bytes (records and snapshots of equal envs stay equal byte for byte). A single-map engine never writes there.
+  __device__ static void reset_map(const Tables& T, const Params& F, const State& S, int b, int lane, TerritoryScratch& sc) {
+    uint8_t* u8 = S.fam_u8 + (size_t)b * S.fam_u8_stride;
+    uint16_t* u16 = S.fam_u16 + (size_t)b * S.fam_u16_stride;
+    for (int k = T.nR + lane; k < T.nR_pad; k += 32) {
+      for (int r = 0; r < RU_COUNT; ++r) u8[r * T.nR_pad + k] = 0;
+      for (int r = 0; r < RS_COUNT; ++r) u16[r * T.nR_pad + k] = 0;
+    }
+    reset(T, F, S, b, lane, sc);
   }
 
   template <class Actions>

@@ -94,10 +94,10 @@ class ShardedSubstrate:
   """One rank's shard of a globally indexed batch of env instances."""
 
   def __init__(self, name: str, roles, global_num_envs: int, seed: int, device: Optional[int] = None,
-               world_rgb: bool = True, group=None, prefab_overrides=None, env_variant=None, build_seeds=None):
-    """name / prefab_overrides / build_seeds / env_variant: as substrate.build_batched, with env_variant indexed by
-    GLOBAL env; each rank takes the slice of its own envs (with build_seeds, or a sequence of names, and no env_variant,
-    global env g plays variant g % len(build_seeds) or g % len(name))."""
+               world_rgb: bool = True, group=None, prefab_overrides=None, env_variant=None, build_seeds=None, maps=None):
+    """name / prefab_overrides / build_seeds / maps / env_variant: as substrate.build_batched, with env_variant indexed
+    by GLOBAL env; each rank takes the slice of its own envs (with build_seeds, maps or a sequence of names, and no
+    env_variant, global env g plays variant g % len(build_seeds), g % len(maps) or g % len(name))."""
     import torch.distributed as dist  # pylint: disable=g-import-not-at-top
     from meltingpot_b200 import substrate  # pylint: disable=g-import-not-at-top
     self._group = group
@@ -115,7 +115,7 @@ class ShardedSubstrate:
     self.local = substrate.build_batched(name, roles=roles, num_envs=self.local_num_envs, device=device, seed=seed,
                                          env_index_base=self.env_index_base, world_rgb=world_rgb,
                                          prefab_overrides=prefab_overrides, env_variant=local_variant,
-                                         build_seeds=build_seeds)
+                                         build_seeds=build_seeds, maps=maps)
 
   def reset(self, out=None):
     """out: a BatchedTimeStep of this rank's envs to fill (BatchedSubstrate.step)."""

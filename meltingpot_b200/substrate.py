@@ -927,9 +927,18 @@ class SubstrateFactory:
 
   def build_batched(self, roles: Sequence[str], num_envs: int, seed: Optional[int] = None,
                     env_index_base: int = 0, world_rgb: bool = True, prefab_overrides=None,
-                    env_variant=None, build_seeds=None) -> BatchedSubstrate:
+                    env_variant=None, build_seeds=None, maps=None) -> BatchedSubstrate:
     _validate_roles(self._config, roles)
-    if build_seeds is not None:  # one draw of the config builder per seed
+    if maps is not None:  # one map set: the substrate under each ASCII map
+      if prefab_overrides is not None or build_seeds is not None:
+        raise ValueError('maps take neither prefab_overrides nor build_seeds')
+      maps = substrate_blobs.checked_maps(self._name, maps)
+      if env_variant is None:
+        env_variant = draw_of_env(env_index_base, num_envs, len(maps))
+      else:
+        env_variant = _checked_env_variant(env_variant, num_envs, len(maps), 'maps')
+      blob = substrate_blobs.compile_maps(self._name, tuple(roles), maps)
+    elif build_seeds is not None:  # one draw of the config builder per seed
       if prefab_overrides is not None:
         raise ValueError('pass build_seeds or prefab_overrides, not both')
       build_seeds = [int(s) for s in build_seeds]
@@ -985,7 +994,8 @@ def draw_of_env(env_index_base: int, num_envs: int, num_draws: int) -> np.ndarra
 
 def build_batched(name, *, roles: Sequence[str], num_envs: int, device: int = 0,
                   seed: Optional[int] = None, env_index_base: int = 0,
-                  world_rgb: bool = True, prefab_overrides=None, env_variant=None, build_seeds=None) -> BatchedSubstrate:
+                  world_rgb: bool = True, prefab_overrides=None, env_variant=None, build_seeds=None,
+                  maps=None) -> BatchedSubstrate:
   """Builds `num_envs` instances on one GPU; see `BatchedSubstrate`.
 
   `name` is a substrate name, or a sequence of substrate names whose maps the engine runs side by side, e.g.
@@ -1005,14 +1015,23 @@ def build_batched(name, *, roles: Sequence[str], num_envs: int, device: int = 0,
   `build_seeds` (coins): one draw of the substrate's config builder per seed, as separate reference builds would
   make (coins draws its map size and its two coin colours on every build), compiled as one draw set. Env b plays
   draw env_variant[b], by default (env_index_base + b) % len(build_seeds); a draw is a variant, so set_env_variant
-  moves an env to another draw at its next episode. Needs a reference checkout; not combined with prefab_overrides."""
+  moves an env to another draw at its next episode. Needs a reference checkout; not combined with prefab_overrides.
+
+  `maps` (territory__rooms, __open, __inside_out and coop_mining): a sequence of ASCII maps, each replacing the
+  substrate's own (territory's `config.layout.ascii_map`, coop_mining's level map), compiled as one map set on one
+  sprite table. Every map keeps the substrate's rows and row width; its walls, resources or ores and spawn points may
+  move, and their counts may differ. Env b plays maps[env_variant[b]], by default (env_index_base + b) % len(maps),
+  and set_env_variant moves an env to another map at its next episode. Needs a reference checkout; not combined with
+  prefab_overrides or build_seeds, nor with a sequence of names."""
   if not isinstance(name, str):
+    if maps is not None:
+      raise ValueError('maps take one substrate name, not a sequence of names')
     return _build_map_set(tuple(name), roles=roles, num_envs=num_envs, device=device, seed=seed,
                           env_index_base=env_index_base, world_rgb=world_rgb, prefab_overrides=prefab_overrides,
                           env_variant=env_variant, build_seeds=build_seeds)
   return get_factory(name, device).build_batched(roles, num_envs, seed=seed, env_index_base=env_index_base,
                                                  world_rgb=world_rgb, prefab_overrides=prefab_overrides,
-                                                 env_variant=env_variant, build_seeds=build_seeds)
+                                                 env_variant=env_variant, build_seeds=build_seeds, maps=maps)
 
 
 def _checked_env_variant(env_variant, num_envs: int, num_variants: int, what: str) -> np.ndarray:

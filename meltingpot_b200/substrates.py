@@ -81,6 +81,48 @@ def compile_draws(name: str, roles: Sequence[str], build_seeds: Sequence[int]) -
   return compiler.compile_substrate_set(name, roles, list(build_seeds))
 
 
+# Substrates whose ASCII map build_batched(maps=...) replaces: every map of a set keeps the substrate's size, topology,
+# players and view, so the engine runs the set side by side (map variants).
+MAP_SUBSTRATES = ('territory__rooms', 'territory__open', 'territory__inside_out', 'coop_mining')
+
+
+def checked_maps(name: str, maps: Sequence[str]) -> list:
+  """`maps` as a list of ASCII maps of `name`, each with the rows and row width of the substrate's own map."""
+  from meltingpot_b200 import blob as blob_lib  # pylint: disable=g-import-not-at-top
+  from meltingpot_b200 import compiler  # pylint: disable=g-import-not-at-top
+  if name not in MAP_SUBSTRATES:
+    raise ValueError(f'maps replace the map of {", ".join(MAP_SUBSTRATES)}, not of {name!r}')
+  if isinstance(maps, str):
+    raise ValueError('maps is a sequence of ASCII maps, not one map')
+  maps = list(maps)
+  if not maps:
+    raise ValueError('the sequence of maps is empty')
+  with open(blob_path(name, PRECOMPILED[name][0]), 'rb') as f:
+    meta = blob_lib.unpack(f.read())['meta']
+  W, H = int(meta[1]), int(meta[2])
+  for i, ascii_map in enumerate(maps):
+    if not isinstance(ascii_map, str):
+      raise ValueError(f'maps[{i}] is a {type(ascii_map).__name__}, not a str')
+    rows = compiler._map_rows(ascii_map)  # pylint: disable=protected-access
+    if len(rows) != H:
+      raise ValueError(f'maps[{i}] has {len(rows)} rows; {name} has {H}')
+    for y, row in enumerate(rows):
+      if len(row) != W:
+        raise ValueError(f'row {y} of maps[{i}] is {len(row)} wide; {name} is {W} wide')
+  return maps
+
+
+def compile_maps(name: str, roles: Sequence[str], maps: Sequence[str]) -> list:
+  """The blobs of `name` with `roles` and each of `maps` as its ASCII map, compiled as one map set on one sprite table
+  (compiler.compile_substrate_maps; compiled from a reference checkout)."""
+  from meltingpot_b200 import compiler  # pylint: disable=g-import-not-at-top
+  if compiler.reference_root() is None:
+    raise FileNotFoundError(
+        f'maps for {name!r} need a Melting Pot reference checkout to compile from '
+        '(set MELTINGPOT_REFERENCE_ROOT)')
+  return compiler.compile_substrate_maps(name, roles, list(maps))
+
+
 def _is_default_role(name: str, role: str) -> bool:
   del name
   return role == 'default'
