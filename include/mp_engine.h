@@ -349,13 +349,19 @@ int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_
 /* Caller-owned DEVICE rows of a step's per-player outputs: player p of env b is delivered to row row_of_player[b][p]
  * when 0 <= row < n_rows, and to no row otherwise. A learner lays rows out as it consumes them, e.g. one contiguous block
  * per policy of a population, focal players apart from background players, or unread players left out. Every target
- * pointer is optional (NULL: not delivered per player). Strides in bytes. */
+ * pointer is optional (NULL: not delivered per player). Strides in bytes.
+ * WORLD.RGB is routed per env the same way: env b's image goes to row world_row_of_env[b] of world_rgb when
+ * 0 <= row < world_n_rows, and is not rendered otherwise, e.g. for the few envs of a video. A zeroed tail (world_rgb and
+ * world_row_of_env NULL) leaves WORLD.RGB per env. */
 typedef struct mp_player_outputs {
   const int32_t* row_of_player;  /* DEVICE i32 [B][P]: row of player p of env b; < 0 or >= n_rows = not delivered */
   int32_t n_rows;
   uint8_t* rgb;        uint64_t rgb_row_stride;        /* [n_rows] x u8 [rgb_h][rgb_w][3], dense inside a row */
   double*  reward;     uint64_t reward_row_stride;     /* [n_rows] x f64 */
   double*  scalar_obs; uint64_t scalar_obs_row_stride, scalar_obs_stride; /* [n_scalar] x [n_rows] x f64 */
+  const int32_t* world_row_of_env;  /* DEVICE i32 [B]: row of env b's WORLD.RGB; < 0 or >= world_n_rows = not rendered */
+  int32_t world_n_rows;
+  uint8_t* world_rgb; uint64_t world_rgb_row_stride;  /* [world_n_rows] x u8 [world_h][world_w][3], dense inside a row */
 } mp_player_outputs;
 
 /* mp_step_restore (slot_of_env and bank set) or mp_step_into (both NULL) whose per-player outputs also go to rows:
@@ -365,23 +371,31 @@ typedef struct mp_player_outputs {
  *     mp_step_into puts them;
  *   - reward and scalar observations of a routed player are written to its row as well; the engine's scalar block is
  *     still written in full, so mp_buffers, the exchange and the host paths see every player;
- *   - WORLD.RGB, discount and step type stay per env: they go to `out` (any subset, or NULL) or the engine's buffers;
+ *   - WORLD.RGB: when players->world_rgb is set, env b's image is drawn straight into players->world_rgb + row *
+ *     world_rgb_row_stride, row = world_row_of_env[b]; an env without a row is neither composited nor stored, and the
+ *     engine's own world_rgb is written for no env. Without players->world_rgb, WORLD.RGB stays per env;
+ *   - discount and step type stay per env: they and any WORLD.RGB not routed go to `out` (any subset, or NULL) or the
+ *     engine's buffers;
  *   - restored envs are routed like any other; flags: MP_RESTORE_REKEY, only with a bank.
- * For every routed player the call gives, byte for byte, what mp_step_into / mp_step_restore / mp_reset_into with the
- * same `out` give at (b, p), and it launches as many kernels when a render follows. With rendering off, the routed
- * scalars are delivered by one small kernel (k_exchange_push), which that case adds.
- * Two players routed to one row are the caller's error: the row then holds one of them, unspecified which. The row map
- * is read on the device and never checked on the host (that would synchronise); nothing outside [0, n_rows) is
- * written. The exchange (mp_exchange_*) works unchanged and the call counts as a step in its sequence. Refused with
- * MP_E_UNSUPPORTED while the observation gather (mp_gather_obs_*) is connected and enabled: its stacked slots stay
- * dense and complete.
+ * For every routed player and every env with a world row the call gives, byte for byte, what mp_step_into /
+ * mp_step_restore / mp_reset_into with the same `out` give at (b, p) and for env b's WORLD.RGB, and it launches as many
+ * kernels when a render follows. With rendering off, the routed scalars are delivered by one small kernel
+ * (k_exchange_push), which that case adds.
+ * Two players routed to one row, or two envs to one world row, are the caller's error: the row then holds one of them,
+ * unspecified which. The row maps are read on the device and never checked on the host (that would synchronise); nothing
+ * outside [0, n_rows) or [0, world_n_rows) is written. The exchange (mp_exchange_*) works unchanged and the call
+ * counts as a step in its sequence. Refused with MP_E_UNSUPPORTED while the observation gather (mp_gather_obs_*) is
+ * connected and enabled: its stacked slots stay dense and complete.
  * Every check runs before anything is enqueued, and a refused call (MP_E_INVALID) steps no env. Refused: a NULL handle,
  * actions or players, n_rows < 1; row_of_player not 4-byte aligned or not B * P i32 inside one device allocation on the
  * engine's device; rgb while the render flags switch player images off, or together with out->rgb; scalar_obs on a
  * substrate without scalar observations; rgb or its row stride not a multiple of 16 bytes; reward / scalar_obs pointers
  * or strides not multiples of 8, or of 2 GiB or more; a row stride smaller than one row; scalar_obs rows (n_scalar x
- * n_rows) that overlap; any target that overlaps another, `out`'s targets, the row map, the bank, the index array or
- * the engine's buffers; and every refusal of mp_step_into's `out` and mp_step_restore's bank. */
+ * n_rows) that overlap; world_rgb without world_row_of_env or the reverse, world_n_rows < 1, world_row_of_env not 4-byte
+ * aligned or not B i32 inside one device allocation on the engine's device, world_rgb or its row stride not a multiple
+ * of 16 bytes, a world row stride smaller than one WORLD.RGB image, world_rgb while the render flags switch WORLD.RGB
+ * off, or together with out->world_rgb; any target or row map that overlaps another, `out`'s targets, the bank, the
+ * index array or the engine's buffers; and every refusal of mp_step_into's `out` and mp_step_restore's bank. */
 int mp_step_players(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots,
                     uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players, void* stream);
 int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out,

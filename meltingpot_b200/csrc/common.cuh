@@ -90,7 +90,8 @@ struct ScalarTargets {
 
 // Caller-owned per-player rows of one step (mp_player_outputs, mp_step_players): player p of env b goes to row
 // row_of_player[b][p] when that is in [0, n_rows). Strides in bytes; scalar_obs row (k, r) starts at
-// scalar_obs + k * scalar_obs_stride + r * scalar_obs_row_stride. Read only by k_render<..., RENDER_ROUTED> and
+// scalar_obs + k * scalar_obs_stride + r * scalar_obs_row_stride. Env b's WORLD.RGB goes to row world_row_of_env[b]
+// of world_rgb when that is in [0, world_n_rows) and world_rgb is set. Read only by k_render<..., RENDER_ROUTED> and
 // k_exchange_push.
 struct PlayerTargets {
   const int32_t* row_of_player;  // [B][P]
@@ -100,6 +101,10 @@ struct PlayerTargets {
   double* reward;
   double* scalar_obs;
   uint64_t rgb_row_stride, reward_row_stride, scalar_obs_row_stride, scalar_obs_stride;
+  const int32_t* world_row_of_env;  // [B]
+  uint8_t* world_rgb;
+  uint64_t world_rgb_row_stride;
+  int world_n_rows;
 };
 
 struct State {

@@ -811,7 +811,8 @@ int copy_scalars(mp_engine* E, const ScalarTargets& o, cudaStream_t st) {
 // Points a launch's copy of the state at the per-player rows of `p` (checked by check_player_outputs).
 void apply_players(const mp_player_outputs& p, State& S) {
   S.pr = PlayerTargets{p.row_of_player, p.n_rows, (p.reward || p.scalar_obs) ? 1 : 0, p.rgb, p.reward, p.scalar_obs,
-                       p.rgb_row_stride, p.reward_row_stride, p.scalar_obs_row_stride, p.scalar_obs_stride};
+                       p.rgb_row_stride, p.reward_row_stride, p.scalar_obs_row_stride, p.scalar_obs_stride,
+                       p.world_row_of_env, p.world_rgb, p.world_rgb_row_stride, p.world_n_rows};
 }
 
 // `out`: where this render's outputs go besides / instead of the engine's own buffers (see apply_outputs), or null.
@@ -828,7 +829,8 @@ int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = 
   }
   // The engine's own images are also slot 0's of mp_step_host_async: a render into them must not start before that
   // slot's device->host copy has read them, whichever call issues it. (A render into a target does not touch them.)
-  const bool own_images = (players && !(out && out->rgb) && !(routed && routed->rgb)) || (world && !(out && out->world_rgb));
+  const bool own_images = (players && !(out && out->rgb) && !(routed && routed->rgb)) ||
+                          (world && !(out && out->world_rgb) && !(routed && routed->world_rgb));
   if (E->async_ready && own_images) CUDA_TRY(cudaStreamWaitEvent(st, E->slot[0].copied, 0));
   E->S.x_raise = E->x_pending_raise ? 1 : 0;
   E->x_pending_raise = false;
@@ -1830,8 +1832,16 @@ int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_devi
   if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
   if (o->scalar_obs && (o->scalar_obs_stride % 8 || o->scalar_obs_stride >= (1ull << 31)))
     return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes or is 2 GiB or more", fn);
+  if (!o->world_rgb != !o->world_row_of_env) return fail(MP_E_INVALID, "%s: world_rgb and world_row_of_env go together", fn);
+  if (o->world_rgb) {
+    if (o->world_n_rows < 1) return fail(MP_E_INVALID, "%s: world_n_rows %d < 1", fn, o->world_n_rows);
+    if ((uintptr_t)o->world_row_of_env % 4) return fail(MP_E_INVALID, "%s: world_row_of_env is not 4-byte aligned", fn);
+    if (!(E->flags & MP_FLAG_RENDER_WORLD)) return fail(MP_E_INVALID, "%s: world_rgb asked for, but the render flags switch WORLD.RGB off", fn);
+    if (out && out->world_rgb) return fail(MP_E_INVALID, "%s: world_rgb is both routed (players) and per env (out)", fn);
+    ext.push_back({"world_row_of_env", (uintptr_t)o->world_row_of_env, (u128)E->B * 4});
+  }
   ext.push_back({"row_of_player", (uintptr_t)o->row_of_player, (u128)E->B * E->T.P * 4});
-  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_row, uint64_t align, u128 extra) -> int {
+  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_row, uint64_t align, u128 extra, uint64_t rows) -> int {
     if (!p) return MP_OK;
     if ((uintptr_t)p % align || stride % align)
       return fail(MP_E_INVALID, "%s: %s pointer or row stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
@@ -1839,15 +1849,16 @@ int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_devi
       return fail(MP_E_INVALID, "%s: %s row stride of %llu bytes is smaller than one row's %llu bytes", fn, name,
                   (unsigned long long)stride, (unsigned long long)per_row);
     if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s row stride of 2 GiB or more", fn, name);
-    const u128 extent = (u128)(R - 1) * stride + per_row + extra;
+    const u128 extent = (u128)(rows - 1) * stride + per_row + extra;
     if (extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, name);
     ext.push_back({name, (uintptr_t)p, extent});
     return MP_OK;
   };
   int rc;
-  if ((rc = add("players rgb", o->rgb, o->rgb_row_stride, (uint64_t)E->R.player_bytes, 16, 0)) ||
-      (rc = add("players reward", o->reward, o->reward_row_stride, 8, 8, 0)) ||
-      (rc = add("players scalar_obs", o->scalar_obs, o->scalar_obs_row_stride, 8, 8, (u128)(n - 1) * o->scalar_obs_stride)))
+  if ((rc = add("players rgb", o->rgb, o->rgb_row_stride, (uint64_t)E->R.player_bytes, 16, 0, R)) ||
+      (rc = add("players reward", o->reward, o->reward_row_stride, 8, 8, 0, R)) ||
+      (rc = add("players scalar_obs", o->scalar_obs, o->scalar_obs_row_stride, 8, 8, (u128)(n - 1) * o->scalar_obs_stride, R)) ||
+      (rc = add("players world_rgb", o->world_rgb, o->world_rgb_row_stride, (uint64_t)E->R.world_bytes, 16, 0, (uint64_t)o->world_n_rows)))
     return rc;
   if (o->scalar_obs) {  // n x n_rows rows of one double at k * s + r * e (the overlap rule of check_device_outputs)
     const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_row_stride;

@@ -248,7 +248,9 @@ struct ViewerInfo {  // per player, refreshed once per env
 //   RENDER_ROUTED: deliver player p of env b to the row State::pr.row_of_player[b][p] of the caller's per-player
 //     targets (mp_step_players). The team's first warp reads the env's row map with its avatars and compacts the
 //     routed players into s_players; the env's item loop then runs over those players' strips and WORLD.RGB's only,
-//     so an unrouted player is neither composited nor stored.
+//     so an unrouted player is neither composited nor stored. With State::pr.world_rgb set, the same warp also reads
+//     the env's WORLD.RGB row (State::pr.world_row_of_env[b]): an env with a row stores its WORLD.RGB strips there,
+//     an env without one has no WORLD.RGB strips.
 enum { RENDER_PLAIN = 0, RENDER_GATHER = 1, RENDER_ROUTED = 2 };
 template <int NCP, int NCW, int MODE>
 __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, State S, RenderPlan R, uint32_t flags) {
@@ -261,9 +263,10 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
   __shared__ uint8_t s_opaque[256];
   __shared__ ViewerInfo s_view_all[RENDER_MAX_TEAMS][MP_MAX_PLAYERS];
   __shared__ int s_next_item[RENDER_MAX_TEAMS];
-  // RENDER_ROUTED: the env's routed players in player order and its player strips (routed players x view_h)
+  // RENDER_ROUTED: the env's routed players in player order, its player strips (routed players x view_h), its
+  // WORLD.RGB strips and its WORLD.RGB row
   __shared__ uint8_t s_players_all[RENDER_MAX_TEAMS][MP_MAX_PLAYERS];
-  __shared__ int s_n_pitems[RENDER_MAX_TEAMS];
+  __shared__ int s_route_all[RENDER_MAX_TEAMS][3];
 
   const int tid = threadIdx.x;
   int team = 0;
@@ -280,7 +283,7 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
   uint8_t* s_stage = s_team + R.toff_stage + twarp * R.stage_bytes;  // warp-private
   ViewerInfo* s_view = s_view_all[team];
   uint8_t* s_players = s_players_all[team];
-  int* s_npi = &s_n_pitems[team];
+  int* s_route = s_route_all[team];  // [0] player strips, [1] WORLD.RGB strips, [2] WORLD.RGB row
   uint64_t* gbar = &bar[1 + team];
 
   // Work split. Balanced part: `rounds` = B / (teams in the grid) envs per team, rendered team by team with no
@@ -341,7 +344,7 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
       s_grid = reinterpret_cast<uint16_t*>(s_team0 + R.toff_grid);
       s_rec = reinterpret_cast<uint16_t*>(s_team0 + R.toff_rec);
       s_view = s_view_all[0];
-      s_players = s_players_all[0]; s_npi = &s_n_pitems[0];
+      s_players = s_players_all[0]; s_route = s_route_all[0];
       gbar = &bar[1];
       next_ctr = &s_next_item[0];
       gtid = tid; gthreads = (int)blockDim.x; bar_id = 0;
@@ -363,7 +366,15 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
       if (on && S.pr.rgb) on = (uint32_t)S.pr.row_of_player[(size_t)b * T.P + gtid] < (uint32_t)S.pr.n_rows;
       const uint32_t m = __ballot_sync(MP_FULL, on);
       if (on) s_players[__popc(m & ((1u << gtid) - 1u))] = (uint8_t)gtid;
-      if (gtid == 0) *s_npi = S.pr.rgb ? __popc(m) * R.view_h : R.n_player_items;
+      if (gtid == 0) {
+        s_route[0] = S.pr.rgb ? __popc(m) * R.view_h : R.n_player_items;
+        int wrow = 0, wn = R.n_items - R.n_player_items;
+        if (S.pr.world_rgb) {
+          wrow = S.pr.world_row_of_env[b];
+          if ((uint32_t)wrow >= (uint32_t)S.pr.world_n_rows) wn = 0;
+        }
+        s_route[1] = wn; s_route[2] = wrow;
+      }
     }  // (published by the group barrier after the cell pass, like s_view)
     mbar_wait(gbar, (uint32_t)(it & 1));  // (team 0's barrier has completed `rounds` phases when the tail starts, so the parity carries over)
     // ---- per-cell pass: flatten the layer stack, folding map sprites into pre-merged ones -------
@@ -383,10 +394,11 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
     // ---- strip items, pulled by warps -------------------------------------------------------------
     int next_item = 0;  // claimed one strip ahead so that the atomic's latency hides behind the strip being drawn
     if (lane == 0) next_item = atomicAdd(next_ctr, 1);
-    const int r_pitems = ROUTED ? *s_npi : 0;  // RENDER_ROUTED: this env's player strips (the other modes read R's, as constant operands)
+    // RENDER_ROUTED: this env's player and WORLD.RGB strips (the other modes read R's, as constant operands); the WORLD.RGB count is re-read at each item (held in a register, it spilled in <4, 5>)
+    const int r_pitems = ROUTED ? s_route[0] : 0;
     for (;;) {
       const int item = __shfl_sync(MP_FULL, next_item, 0);
-      if (ROUTED ? item - r_pitems >= R.n_items - R.n_player_items : item >= R.n_items) break;
+      if (ROUTED ? item - r_pitems >= s_route[1] : item >= R.n_items) break;
       if (lane == 0) next_item = atomicAdd(next_ctr, 1);
       uint8_t* buf = s_stage + (slot % RENDER_SLOTS) * slot_bytes;
       ++slot;
@@ -464,7 +476,9 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
         __syncwarp();
         if (lane == 0 && !(flags & 32u)) {
           const size_t in_env = (size_t)wi * R.witem_bytes;
-          bulk_store(S.world_rgb + b * S.world_env_stride + in_env, buf, (uint32_t)R.witem_bytes, store_policy);
+          if (ROUTED && S.pr.world_rgb)
+            bulk_store(S.pr.world_rgb + (size_t)s_route[2] * S.pr.world_rgb_row_stride + in_env, buf, (uint32_t)R.witem_bytes, store_policy);
+          else bulk_store(S.world_rgb + b * S.world_env_stride + in_env, buf, (uint32_t)R.witem_bytes, store_policy);
           if (GATHER) {
             const size_t off = (size_t)b * R.world_bytes + in_env;
             for (int r = 0; r < S.g_world; ++r) bulk_store(S.g_wrgb[r] + off, buf, (uint32_t)R.witem_bytes, store_policy);

@@ -117,23 +117,30 @@ class MpPlayerOutputs(ctypes.Structure):
       ('rgb', ctypes.c_void_p), ('rgb_row_stride', ctypes.c_uint64),
       ('reward', ctypes.c_void_p), ('reward_row_stride', ctypes.c_uint64),
       ('scalar_obs', ctypes.c_void_p), ('scalar_obs_row_stride', ctypes.c_uint64), ('scalar_obs_stride', ctypes.c_uint64),
+      ('world_row_of_env', ctypes.c_void_p), ('world_n_rows', ctypes.c_int32),
+      ('world_rgb', ctypes.c_void_p), ('world_rgb_row_stride', ctypes.c_uint64),
   ]
 
 
 # The per-player outputs a step can deliver into rows of caller-owned tensors (mp_step_players).
 PLAYER_OUTPUTS = ('rgb', 'reward', 'scalar_obs')
+# WORLD.RGB routed per env in the same call: the row map and the rows, given together.
+WORLD_OUTPUTS = ('world_row_of_env', 'world_rgb')
 
 
 def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num_envs: int, num_players: int,
-                     num_scalar_obs: int, device: int) -> MpPlayerOutputs:
+                     num_scalar_obs: int, device: int, world_shape: Optional[Tuple[int, ...]] = None) -> MpPlayerOutputs:
   """The mp_player_outputs of `players`: 'row_of_player' (TensorLayout of a contiguous int32 CUDA [B, P]) and any of
   'rgb' (uint8 [n_rows, *rgb_shape], dense inside a row), 'reward' (float64 [n_rows]) and 'scalar_obs' (float64
   [num_scalar_obs, n_rows]); the row axis (and the observation axis of scalar_obs) may have any stride. Every target
-  must have the same n_rows. Only shapes, dtypes, devices and layouts are checked, never the row map's values."""
+  must have the same n_rows. WORLD.RGB rows, optional: 'world_row_of_env' (contiguous int32 CUDA [B]) with 'world_rgb'
+  (uint8 [n, *world_shape], dense inside a row, 16-byte aligned rows; world_shape None: the engine renders no
+  WORLD.RGB). Only shapes, dtypes, devices and layouts are checked, never the row maps' values."""
   import torch  # pylint: disable=g-import-not-at-top
-  unknown = set(players) - set(PLAYER_OUTPUTS) - {'row_of_player'}
+  unknown = set(players) - set(PLAYER_OUTPUTS) - set(WORLD_OUTPUTS) - {'row_of_player'}
   if unknown:
-    raise ValueError(f'players: unknown entries {sorted(unknown)} (row_of_player and any of {", ".join(PLAYER_OUTPUTS)})')
+    raise ValueError(f'players: unknown entries {sorted(unknown)} (row_of_player and any of {", ".join(PLAYER_OUTPUTS)}, '
+                     f'or {" with ".join(WORLD_OUTPUTS)})')
 
   def on_device(name, t):
     dev = torch.device(t.device)
@@ -185,6 +192,37 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
     if name == 'scalar_obs':
       s.scalar_obs_stride = (t.stride[0] if t.shape[0] > 1 else rows * dense) * item
   s.n_rows = n_rows
+  wmap, world = players.get('world_row_of_env'), players.get('world_rgb')
+  if (wmap is None) != (world is None):
+    raise ValueError('players: world_row_of_env and world_rgb go together')
+  if world is not None:
+    if world_shape is None:
+      raise ValueError('players[\'world_rgb\']: this engine renders no WORLD.RGB')
+    if tuple(wmap.shape) != (num_envs,) or wmap.dtype != torch.int32 or (num_envs > 1 and tuple(wmap.stride) != (1,)):
+      raise ValueError(f'players[\'world_row_of_env\']: must be a contiguous int32 tensor [{num_envs}]')
+    on_device('world_row_of_env', wmap)
+    inner = tuple(world_shape)
+    if len(world.shape) != 1 + len(inner) or tuple(world.shape[1:]) != inner:
+      raise ValueError(f'players[\'world_rgb\']: shape {tuple(world.shape)}, must be {("n",) + inner}')
+    if world.dtype != torch.uint8:
+      raise ValueError(f'players[\'world_rgb\']: dtype {world.dtype}, must be torch.uint8')
+    on_device('world_rgb', world)
+    rows = int(world.shape[0])
+    if rows < 1:
+      raise ValueError('players[\'world_rgb\']: no rows')
+    dense = 1
+    for axis in range(len(world.shape) - 1, 0, -1):
+      if world.shape[axis] != 1 and world.stride[axis] != dense:
+        raise ValueError(f'players[\'world_rgb\']: axis {axis} has stride {world.stride[axis]}, must be {dense} (only the row '
+                         'axis may be strided)')
+      dense *= world.shape[axis]
+    row_stride = world.stride[0] if rows > 1 else dense  # with one row the stride is never used
+    if world.data_ptr % 16 or row_stride % 16:
+      raise ValueError('players[\'world_rgb\']: the pointer and the row stride must be multiples of 16 bytes')
+    s.world_row_of_env = ctypes.c_void_p(int(wmap.data_ptr))
+    s.world_n_rows = rows
+    s.world_rgb = ctypes.c_void_p(int(world.data_ptr))
+    s.world_rgb_row_stride = row_stride
   return s
 
 
@@ -587,7 +625,10 @@ class Engine:
     of env b is delivered to row row_of_player[b, p] when that lies in 0..n_rows-1, and nowhere otherwise; with 'rgb'
     the images are drawn straight into the rows, an unrouted player is not drawn at all and this engine's own rgb is
     not written. Combines with out (whose rgb it replaces) and with restore / bank. The row map's values are never
-    checked on the host; two players routed to one row leave one of them there.
+    checked on the host; two players routed to one row leave one of them there. WORLD.RGB may be routed per env in
+    the same call: 'world_row_of_env' (contiguous CUDA int32 [B]) with 'world_rgb' (uint8 [n, H, W, 3]); env b's image
+    is drawn into row world_row_of_env[b] when that lies in 0..n-1, and not at all otherwise, and this engine's own
+    world_rgb is not written (out's world_rgb must then be absent).
 
     player_actions: actions read from rows (mp_step_routed), {'row_of_player': contiguous CUDA int32 [B, P],
     'action': CUDA int32 [n_rows], any stride}, with actions None. Player p of env b takes action[row_of_player[b, p]]
@@ -651,7 +692,8 @@ class Engine:
 
   def _player_outputs(self, players) -> MpPlayerOutputs:
     return describe_players({k: (None if v is None else layout_of(v)) for k, v in players.items()}, tuple(self.rgb.shape[2:]),
-                            self.num_envs, self.num_players, self.num_scalar_obs, self.device)
+                            self.num_envs, self.num_players, self.num_scalar_obs, self.device,
+                            tuple(self.world_rgb.shape[1:]))
 
   def step_state(self, actions, stream=None) -> None:
     self._check_actions(actions)

@@ -167,11 +167,14 @@ class BatchedScenario:
   [B, n_k] in slot order; its callable gets their timestep and `active` (bool [B, n_k]: the rows played this episode)
   and returns an action for each row. Inactive rows are neither rendered nor read. `background_bots()` tells which bot
   each background slot plays. Focal players are routed as without a population.
+
+  world_envs: distinct env indices whose WORLD.RGB is rendered (e.g. the few envs of a video); every other env's is
+  not. The timesteps' 'WORLD.RGB', where permitted, is then uint8 [n, H, W, 3], row k holding env world_envs[k].
   """
 
   def __init__(self, substrate: substrate_lib.BatchedSubstrate, background_policy, is_focal: Sequence[bool],
                permitted_observations: Collection[str], *, roles: Sequence[str] = None,
-               bots_by_role: Mapping[str, Collection[str]] = None) -> None:
+               bots_by_role: Mapping[str, Collection[str]] = None, world_envs=None) -> None:
     import numpy as np  # pylint: disable=g-import-not-at-top
     if len(is_focal) != substrate.num_players:
       raise ValueError(f'is_focal is length {len(is_focal)} but substrate is '
@@ -196,6 +199,11 @@ class BatchedScenario:
       self._routes = substrate.drawn_routes(self._population_choices(background_policy, roles, bots_by_role))
     self._actions = self._routes.actions()
     self._focal_rows = slice(0, self.num_envs * self.num_focal)
+    self._world = None  # (world_envs, world_row_of_env) when WORLD.RGB is routed
+    if world_envs is not None:
+      if substrate._world_shape() is None:  # pylint: disable=protected-access
+        raise ValueError('world_envs: this batch renders no WORLD.RGB (it was built with world_rgb=False)')
+      self._world = substrate_lib.world_row_map(world_envs, self.num_envs, self._routes.device)
 
   def _population_choices(self, policies, roles, bots_by_role):
     """Validates population mode and returns each slot's groups for drawn_routes: group 0 for focal slots, group
@@ -233,7 +241,10 @@ class BatchedScenario:
     block = torch.empty((len(names), r.n_rows), dtype=torch.float64, device=dev) if names else None
     for k, name in enumerate(names):
       tensors[name] = block[k]
-    return substrate_lib.PlayerOutputs(r, None, tensors, block)
+    if self._world is not None:
+      shape = (int(self._world[0].shape[0]),) + self._substrate._world_shape()  # pylint: disable=protected-access
+      tensors['WORLD.RGB'] = torch.empty(shape, dtype=torch.uint8, device=dev)
+    return substrate_lib.PlayerOutputs(r, None, tensors, block, world=self._world)
 
   def _select(self, timestep, po, rows, n, permitted):
     def view(v):

@@ -248,7 +248,7 @@ class BatchedSubstrate:
       self._engine.reset(mask, out=None if out is None else self._engine_outputs(out, routed=players),
                          players=self._routed_outputs(players),
                          draw=routes.draw if isinstance(routes, DrawnRoutes) else None)
-      return self._without_rgb(self._timestep() if out is None else self._fill_collective(out))
+      return self._routed_timestep(self._timestep() if out is None else self._fill_collective(out), players)
     if out is None:
       self._engine.reset(mask)
       return self._timestep()
@@ -260,14 +260,18 @@ class BatchedSubstrate:
     slot), -1 for a player nobody reads. See PlayerRoutes."""
     import torch  # pylint: disable=g-import-not-at-top
     return PlayerRoutes(groups, self.num_envs, self.num_players, tuple(self._engine.rgb.shape[2:]), self._scalar_names,
-                        torch.device('cuda', self._engine.device))
+                        torch.device('cuda', self._engine.device), self._world_shape())
 
   def drawn_routes(self, choices) -> 'DrawnRoutes':
     """Rows for per-player delivery that are drawn again at every episode start: choices[p] is a sequence of group ids
     (e.g. the bots that may fill slot p), empty for a player nobody reads. See DrawnRoutes."""
     import torch  # pylint: disable=g-import-not-at-top
     return DrawnRoutes(choices, self.num_envs, self.num_players, tuple(self._engine.rgb.shape[2:]), self._scalar_names,
-                       torch.device('cuda', self._engine.device))
+                       torch.device('cuda', self._engine.device), self._world_shape())
+
+  def _world_shape(self):
+    """One env's WORLD.RGB shape [H, W, 3], or None when this batch renders no WORLD.RGB."""
+    return tuple(self._engine.world_rgb.shape[1:]) if self._world_rgb else None
 
   def step(self, actions=None, out: Optional[BatchedTimeStep] = None, restore=None, bank=None,
            rekey: bool = False, players: Optional['PlayerOutputs'] = None,
@@ -287,7 +291,9 @@ class BatchedSubstrate:
     players: a PlayerOutputs (`player_routes(groups).outputs()`, or `.at(t)` of one with T slots): each routed
     player's image, reward and scalar observations go to its row, the images drawn straight there; unrouted players are
     not drawn. The returned timestep then has no 'RGB'; every other field is as without players. Combines with out and
-    restore / bank.
+    restore / bank. With outputs made with world_envs (`outputs(world_envs=envs)`), WORLD.RGB is drawn only for those
+    envs, straight into players['WORLD.RGB'] (row k: env envs[k]), and the timestep's 'WORLD.RGB' is that tensor; out's
+    'WORLD.RGB' is then left alone.
 
     player_actions: a PlayerActions (`player_routes(groups).actions()`, or `.at(t)` of one with T slots), with actions
     None: each routed player takes the action in its row, an unrouted player action 0 (NOOP). The routes may be the
@@ -316,7 +322,7 @@ class BatchedSubstrate:
     if players is not None:
       self._engine.step(actions, out=None if out is None else self._engine_outputs(out, routed=players),
                         players=self._routed_outputs(players), **kw)
-      return self._without_rgb(self._timestep() if out is None else self._fill_collective(out))
+      return self._routed_timestep(self._timestep() if out is None else self._fill_collective(out), players)
     if out is None:
       self._engine.step(actions, **kw)
       return self._timestep()
@@ -339,7 +345,12 @@ class BatchedSubstrate:
     self._check_routes(r, 'players')
     if po.T is not None:
       raise ValueError('players: pick one slot of a PlayerOutputs with T slots (outputs(T).at(t))')
-    return {'row_of_player': r.row_of_player, 'rgb': po['RGB'], 'reward': po['REWARD'], 'scalar_obs': po.scalar_block}
+    targets = {'row_of_player': r.row_of_player, 'rgb': po['RGB'], 'reward': po['REWARD'], 'scalar_obs': po.scalar_block}
+    if _routes_world(po):
+      if not self._world_rgb:
+        raise ValueError('players: WORLD.RGB is routed, but this batch was built with world_rgb=False')
+      targets.update(world_row_of_env=po.world_row_of_env, world_rgb=po['WORLD.RGB'])
+    return targets
 
   def _check_routes(self, r: 'PlayerRoutes', what: str) -> None:
     import torch  # pylint: disable=g-import-not-at-top
@@ -357,16 +368,20 @@ class BatchedSubstrate:
     return {'row_of_player': pa.routes.row_of_player, 'action': pa.tensor}
 
   @staticmethod
-  def _without_rgb(ts: BatchedTimeStep) -> BatchedTimeStep:
-    return BatchedTimeStep(step_type=ts.step_type, reward=ts.reward, discount=ts.discount,
-                           observation={k: v for k, v in ts.observation.items() if k != 'RGB'})
+  def _routed_timestep(ts: BatchedTimeStep, po: 'PlayerOutputs') -> BatchedTimeStep:
+    """ts without 'RGB' (the rows hold the images), its 'WORLD.RGB' the routed rows when po routes it."""
+    obs = {k: v for k, v in ts.observation.items() if k != 'RGB'}
+    if _routes_world(po):
+      obs['WORLD.RGB'] = po['WORLD.RGB']
+    return BatchedTimeStep(step_type=ts.step_type, reward=ts.reward, discount=ts.discount, observation=obs)
 
   def _engine_outputs(self, ts: BatchedTimeStep, routed=None):
     """The engine's output tensors of a BatchedTimeStep (the scalar observations as one [n, B, P] view). routed: the
-    images go to those rows instead, so ts's 'RGB' is left alone."""
+    images go to those rows instead, so ts's 'RGB' is left alone (and its 'WORLD.RGB' when routed routes it)."""
     import torch  # pylint: disable=g-import-not-at-top
     obs = ts.observation
-    out = {'rgb': None if routed is not None else obs.get('RGB'), 'world_rgb': obs.get('WORLD.RGB') if self._world_rgb else None,
+    world = self._world_rgb and not (routed is not None and _routes_world(routed))
+    out = {'rgb': None if routed is not None else obs.get('RGB'), 'world_rgb': obs.get('WORLD.RGB') if world else None,
            'reward': ts.reward, 'discount': ts.discount, 'step_type': ts.step_type}
     scalars = [obs[name] for name in self._scalar_names if name in obs]
     if scalars:
@@ -500,15 +515,19 @@ class PlayerRoutes:
   they are by every step.
     row_of_player  int32 CUDA [B, P]: the row of each player, -1 if unrouted (what the engine reads);
     env_of_row, player_of_row  int64 CUDA [n_rows]: the env and player of each row.
+  WORLD.RGB can be routed per env along with them: `outputs(world_envs=envs)` draws it only for envs, into rows of its
+  own (see PlayerOutputs).
   Actions go the same way: `actions(T)` gives rows a step reads its actions from (step(player_actions=)), laid out
   like the outputs' rows, so nothing is scattered back into [B, P].
   Do not write to these tensors: they are shared by every PlayerOutputs and PlayerActions made from this object."""
 
   __slots__ = ('num_envs', 'num_players', 'num_groups', 'n_rows', 'device', 'row_of_player', 'env_of_row', 'player_of_row',
-               '_starts', '_rgb_shape', '_scalar_names')
+               '_starts', '_rgb_shape', '_scalar_names', '_world_shape')
 
-  def __init__(self, groups, num_envs: int, num_players: int, rgb_shape, scalar_names: Sequence[str], device):
-    """rgb_shape: one player's [h, w, 3]; device: where the tensors live (a CUDA device for the engine)."""
+  def __init__(self, groups, num_envs: int, num_players: int, rgb_shape, scalar_names: Sequence[str], device,
+               world_rgb_shape=None):
+    """rgb_shape: one player's [h, w, 3]; device: where the tensors live (a CUDA device for the engine);
+    world_rgb_shape: one env's WORLD.RGB [H, W, 3], or None when the batch renders none."""
     import torch  # pylint: disable=g-import-not-at-top
     g = groups.detach().cpu().numpy() if isinstance(groups, torch.Tensor) else np.asarray(groups)
     if g.shape != (num_envs, num_players):
@@ -534,6 +553,7 @@ class PlayerRoutes:
     set_('n_rows', int(flat.size)); set_('device', dev)
     set_('_starts', tuple(int(x) for x in np.concatenate([[0], np.cumsum(counts)])))
     set_('_rgb_shape', tuple(int(x) for x in rgb_shape)); set_('_scalar_names', tuple(scalar_names))
+    set_('_world_shape', None if world_rgb_shape is None else tuple(int(x) for x in world_rgb_shape))
     set_('row_of_player', torch.from_numpy(rows.reshape(num_envs, num_players)).to(dev))
     set_('env_of_row', torch.from_numpy(flat // num_players).to(dev))
     set_('player_of_row', torch.from_numpy(flat % num_players).to(dev))
@@ -547,11 +567,13 @@ class PlayerRoutes:
       raise IndexError(f'group {g} outside 0..{self.num_groups - 1}')
     return slice(self._starts[g], self._starts[g + 1])
 
-  def outputs(self, T: Optional[int] = None) -> 'PlayerOutputs':
+  def outputs(self, T: Optional[int] = None, world_envs=None) -> 'PlayerOutputs':
     """Zeroed CUDA tensors for the routed outputs: 'RGB' uint8 [n_rows, h, w, 3], 'REWARD' float64 [n_rows] and each
     scalar observation float64 [n_rows] (views of one tensor); with T, each gets a leading time axis [T, n_rows, ...]
-    and `at(t)` is slot t."""
-    return PlayerOutputs(self, T)
+    and `at(t)` is slot t. world_envs: distinct env indices (a sequence or 1-D integer tensor) whose WORLD.RGB is
+    rendered, into 'WORLD.RGB' uint8 [n, H, W, 3] ([T, n, H, W, 3] with T), row k holding env world_envs[k]; no other
+    env's WORLD.RGB is rendered."""
+    return PlayerOutputs(self, T, world_envs=world_envs)
 
   def actions(self, T: Optional[int] = None) -> 'PlayerActions':
     """A zeroed int32 CUDA tensor of actions, one per row: [n_rows], or [T, n_rows] with T, whose `at(t)` is slot t."""
@@ -576,10 +598,12 @@ class DrawnRoutes:
   both to BatchedSubstrate.step (players=, player_actions=) and the outputs to reset (players=)."""
 
   __slots__ = ('num_envs', 'num_players', 'num_groups', 'n_rows', 'device', 'row_of_player', 'choices', 'draw',
-               '_starts', '_members', '_rgb_shape', '_scalar_names')
+               '_starts', '_members', '_rgb_shape', '_scalar_names', '_world_shape')
 
-  def __init__(self, choices, num_envs: int, num_players: int, rgb_shape, scalar_names: Sequence[str], device):
-    """rgb_shape: one player's [h, w, 3]; device: where the tensors live (a CUDA device for the engine)."""
+  def __init__(self, choices, num_envs: int, num_players: int, rgb_shape, scalar_names: Sequence[str], device,
+               world_rgb_shape=None):
+    """rgb_shape: one player's [h, w, 3]; device: where the tensors live (a CUDA device for the engine);
+    world_rgb_shape: one env's WORLD.RGB [H, W, 3], or None when the batch renders none."""
     import torch  # pylint: disable=g-import-not-at-top
     from meltingpot_b200 import engine as engine_lib  # pylint: disable=g-import-not-at-top
     if isinstance(choices, (str, bytes)) or len(choices) != num_players:
@@ -612,6 +636,7 @@ class DrawnRoutes:
     set_('n_rows', starts[-1]); set_('device', dev); set_('choices', tuple(norm))
     set_('_starts', tuple(starts)); set_('_members', members)
     set_('_rgb_shape', tuple(int(x) for x in rgb_shape)); set_('_scalar_names', tuple(scalar_names))
+    set_('_world_shape', None if world_rgb_shape is None else tuple(int(x) for x in world_rgb_shape))
     set_('row_of_player', torch.full((num_envs, num_players), -1, dtype=torch.int32, device=dev))
     set_('draw', engine_lib.describe_draw(self.row_of_player, self.n_rows, row_base, rows_per_env))
 
@@ -645,24 +670,67 @@ class DrawnRoutes:
     act.scatter_(0, torch.where(inside, flat - r.start, n), True)
     return act[:n].view(self.num_envs, len(self._members[g]))
 
-  def outputs(self, T: Optional[int] = None) -> 'PlayerOutputs':
+  def outputs(self, T: Optional[int] = None, world_envs=None) -> 'PlayerOutputs':
     """As PlayerRoutes.outputs."""
-    return PlayerOutputs(self, T)
+    return PlayerOutputs(self, T, world_envs=world_envs)
 
   def actions(self, T: Optional[int] = None) -> 'PlayerActions':
     """As PlayerRoutes.actions."""
     return PlayerActions(self, T)
 
 
+def world_row_map(world_envs, num_envs: int, device):
+  """(world_envs int64 [n], world_row_of_env int32 [B]) on `device` for routed WORLD.RGB: row k holds env
+  world_envs[k], an env not listed has row -1 and is not rendered. world_envs is a sequence or 1-D integer tensor of
+  distinct env indices in [0, num_envs), validated here, on the host."""
+  import torch  # pylint: disable=g-import-not-at-top
+  dev = torch.device(device)
+  if isinstance(world_envs, torch.Tensor):
+    if world_envs.device.type != 'cpu' and world_envs.device != dev:
+      raise ValueError(f'world_envs is on {world_envs.device}, the routes are on {dev}')
+    if world_envs.dtype == torch.bool or world_envs.is_floating_point() or world_envs.is_complex():
+      raise ValueError(f'world_envs must hold integer env indices, got dtype {world_envs.dtype}')
+    e = world_envs.detach().cpu().numpy()
+  else:
+    e = np.asarray(world_envs)
+  if e.ndim != 1:
+    raise ValueError(f'world_envs must be one-dimensional, got shape {list(e.shape)}')
+  if e.size == 0:
+    raise ValueError('world_envs lists no env')
+  if e.dtype == np.bool_ or not np.issubdtype(e.dtype, np.integer):
+    raise ValueError(f'world_envs must hold integer env indices, got dtype {e.dtype}')
+  e = e.astype(np.int64)
+  if (e < 0).any() or (e >= num_envs).any():
+    raise ValueError(f'world_envs must lie in [0, {num_envs}), got {e.min()}..{e.max()}')
+  if np.unique(e).size != e.size:
+    raise ValueError('world_envs lists an env twice')
+  rows = np.full(num_envs, -1, np.int32)
+  rows[e] = np.arange(e.size, dtype=np.int32)
+  return torch.from_numpy(e).to(dev), torch.from_numpy(rows).to(dev)
+
+
+def _routes_world(po) -> bool:
+  """Whether a PlayerOutputs routes WORLD.RGB."""
+  return getattr(po, 'world_row_of_env', None) is not None
+
+
 class PlayerOutputs:
   """Caller-owned CUDA tensors for the routed outputs of PlayerRoutes (routes.outputs(T)); `po[name]` is one of them.
-  Pass it (or, with T slots, `at(t)`) to BatchedSubstrate.step / reset as players=."""
+  Pass it (or, with T slots, `at(t)`) to BatchedSubstrate.step / reset as players=.
+  Made with world_envs, it also holds 'WORLD.RGB' (row k: env world_envs[k]) and
+    world_envs  int64 CUDA [n]: the env of each WORLD.RGB row;
+    world_row_of_env  int32 CUDA [B]: the WORLD.RGB row of each env, -1 if it is not rendered (what the engine reads);
+  both None otherwise."""
 
-  def __init__(self, routes: PlayerRoutes, T: Optional[int] = None, tensors=None, scalar_block=None):
+  def __init__(self, routes: PlayerRoutes, T: Optional[int] = None, tensors=None, scalar_block=None, world_envs=None,
+               world=None):
+    """tensors, scalar_block, world: a view (at / group) or rows made by the caller, world being the (world_envs,
+    world_row_of_env) pair of world_row_map when tensors holds 'WORLD.RGB'."""
     import torch  # pylint: disable=g-import-not-at-top
     self.routes, self.T = routes, T
-    if tensors is not None:  # a view (at / group)
+    if tensors is not None:  # a view (at / group), or rows made by the caller
       self.tensors, self.scalar_block = tensors, scalar_block
+      self.world_envs, self.world_row_of_env = world if world is not None else (None, None)
       return
     if T is not None and T < 1:
       raise ValueError(f'outputs need T >= 1 slots, got {T}')
@@ -674,6 +742,14 @@ class PlayerOutputs:
     self.scalar_block = torch.zeros((len(names),) + lead, dtype=torch.float64, device=dev) if names else None
     for k, name in enumerate(names):  # one tensor, so that a slot's scalar observations are one [n, n_rows] view
       self.tensors[name] = self.scalar_block[k]
+    self.world_envs = self.world_row_of_env = None
+    if world_envs is not None:
+      if routes._world_shape is None:  # pylint: disable=protected-access
+        raise ValueError('world_envs: this batch renders no WORLD.RGB (it was built with world_rgb=False)')
+      self.world_envs, self.world_row_of_env = world_row_map(world_envs, routes.num_envs, dev)
+      n = int(self.world_envs.shape[0])
+      self.tensors['WORLD.RGB'] = torch.zeros(((n,) if T is None else (int(T), n)) + routes._world_shape,  # pylint: disable=protected-access
+                                              dtype=torch.uint8, device=dev)
 
   def __getitem__(self, name):
     return self.tensors[name]
@@ -691,14 +767,16 @@ class PlayerOutputs:
     tensors = {k: v[t] for k, v in self.tensors.items()}
     for k, name in enumerate(self.routes._scalar_names):  # pylint: disable=protected-access
       tensors[name] = sb[k]
-    return PlayerOutputs(self.routes, None, tensors, sb)
+    return PlayerOutputs(self.routes, None, tensors, sb, world=(self.world_envs, self.world_row_of_env))
 
   def group(self, g: int) -> Dict[str, Any]:
-    """{name: view of group g's rows} ([rows, ...], or [T, rows, ...] with T slots)."""
+    """{name: view of group g's rows} ([rows, ...], or [T, rows, ...] with T slots); WORLD.RGB, which is per env, is
+    not among them."""
     r = self.routes.rows(g)
+    per_player = {k: v for k, v in self.tensors.items() if k != 'WORLD.RGB'}
     if self.T is None:
-      return {k: v[r] for k, v in self.tensors.items()}
-    return {k: v[:, r] for k, v in self.tensors.items()}
+      return {k: v[r] for k, v in per_player.items()}
+    return {k: v[:, r] for k, v in per_player.items()}
 
 
 class PlayerActions:
