@@ -478,6 +478,15 @@ int mp_reset_drawn(mp_handle h, const uint8_t* env_mask, const mp_route_draw* dr
 #define MP_RENDER_PLAN_FIELDS 12
 int mp_debug_render_plan(mp_handle h, int32_t out[MP_RENDER_PLAN_FIELDS]);
 
+/* Diagnostic: which kernels the handle's last call that launched a state transition or a render launched, -1 for a
+ * part it did not launch: the family (MpbFamily) and the state-transition kernel's cell (1 if the engine has more than
+ * one variant, 1 if the step restores from a bank, then 0 dense actions, 1 action rows, 2 drawn routes), then the
+ * render mode (0 plain, 1 observation gather, 2 player / WORLD.RGB rows), the k_render instantiation's NCP and NCW and
+ * its layout (teams per CTA, warps per team, log2 of the WORLD.RGB strip rows). A call with rendering off shows -1 from
+ * the render mode on; a render alone (mp_render, mp_state_restore, mp_state_load) shows -1 up to it. */
+#define MP_LAST_LAUNCH_FIELDS 10
+int mp_debug_last_launch(mp_handle h, int32_t out[MP_LAST_LAUNCH_FIELDS]);
+
 /* Diagnostic: the renderer's sprite tables. *n_total = atlas sprites including the pre-merged ones;
  * pair[n_total * n_total] = pre-merged sprite for (bottom, top) or 0; flags[n_total] bit 0 opaque,
  * bit 1 remapped per viewer. Either array may be NULL (call once for n_total, then again). */

@@ -253,9 +253,8 @@ struct mp_engine {
   uint64_t launches = 0;
   int sm_count = 0;
   size_t step_smem = 0;  // dynamic shared memory of one state-transition launch
-  void (*render_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
-  void (*render_gather_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;
-  void (*render_routed_fn)(Tables, State, RenderPlan, uint32_t) = nullptr;  // mp_step_players / mp_reset_players
+  // k_render<inst_ncp, inst_ncw, mode> by mode: RENDER_PLAIN, RENDER_GATHER (mp_gather_obs_*), RENDER_ROUTED (player rows)
+  void (*render_fns[3])(Tables, State, RenderPlan, uint32_t) = {};
   // mp_gather_obs_*: this rank's stacked-observation block [flags 256 B][2 slots][rgb of all ranks | world_rgb of all ranks]
   uint8_t* g_block = nullptr;
   uint64_t g_block_bytes = 0, g_slot_bytes = 0, g_world_off = 0;
@@ -268,6 +267,9 @@ struct mp_engine {
   int black_sprite = -1;
   int lane_map_players = 0, lane_map_world = 0;  // 0 plain, 2 scattered colouring, 1 + 16 * (extra wavefronts left) whole-cell dealing
   int inst_ncp = 0, inst_ncw = 0;                // the k_render<NCP, NCW> instantiation this engine launches
+  // mp_debug_last_launch: the k_step cell and the k_render mode and layout of the last call that launched either, -1 for
+  // a part it did not launch. Written by launch_state and launch_render from the values that pick the kernel.
+  int32_t last_launch[MP_LAST_LAUNCH_FIELDS];
   uint64_t key_base = 0;   // seed + env_index_base: env b's key at creation is key_base + b (State::key)
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
@@ -746,6 +748,9 @@ __global__ void k_debug_obs(Tables T, State S, int32_t* position, int32_t* orien
   }
 }
 
+// For a call that launches no state transition: every field -1 until launch_render records its render.
+void clear_last_launch(mp_engine* E) { std::fill_n(E->last_launch, MP_LAST_LAUNCH_FIELDS, -1); }
+
 // `S`: the engine's state with the step's targets applied (apply_outputs), for the scalar rows k_exchange_push delivers.
 int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
   E->x_pending_raise = false;
@@ -773,8 +778,11 @@ int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int 
   RowActions rows_arg = rows ? *rows : RowActions{};
   void* args[] = {&E->T, nullptr, &E->S, &actions, &mask, &mode, &restore_arg,
                   drawn ? const_cast<DrawnActions*>(drawn) : static_cast<void*>(&rows_arg)};  // k_step's parameters; Source by `launch`
-  const void* kernel = E->family->step[E->variants.n > 1][restore != nullptr][drawn ? 2 : rows != nullptr];
+  const int variants = E->variants.n > 1, restoring = restore != nullptr, source = drawn ? 2 : rows != nullptr;
+  const void* kernel = E->family->step[variants][restoring][source];
   CUDA_TRY(E->family->launch(cfg, kernel, args, E->params, E->variants));
+  const int32_t cell[MP_LAST_LAUNCH_FIELDS] = {E->family->id, variants, restoring, source, -1, -1, -1, -1, -1, -1};
+  memcpy(E->last_launch, cell, sizeof cell);
   if (E->S.x_world) {
     E->x_pending_raise = true;
     if (!render_follows) { ++E->launches; return raise_flags(E, st, E->S); }
@@ -864,7 +872,10 @@ int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = 
   State S = E->S;
   if (out) apply_outputs(*out, S);
   if (routed) apply_players(*routed, S);  // (never with gather: mp_step_players refuses it)
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, routed ? E->render_routed_fn : gather ? E->render_gather_fn : E->render_fn, E->T, S, R, E->flags));
+  const int mode = routed ? RENDER_ROUTED : gather ? RENDER_GATHER : RENDER_PLAIN;
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->render_fns[mode], E->T, S, R, E->flags));
+  const int32_t layout[6] = {mode, E->inst_ncp, E->inst_ncw, R.n_teams, R.team_threads / 32, R.wstrip_log2};
+  memcpy(E->last_launch + 4, layout, sizeof layout);
   if (gather) {
     k_gather_raise<<<1, 32, 0, st>>>(E->d_g_flag_ptrs, E->g_world, E->g_rank, E->g_seq);
     ++E->launches;
@@ -983,6 +994,7 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
   if (prop.major != 9 || prop.minor != 0) return fail(MP_E_NO_DEVICE, "device %d is sm_%d%d; kernels are built for sm_90a only", device, prop.major, prop.minor);
   DeviceGuard guard(device);
   mp_engine* E = new mp_engine();
+  clear_last_launch(E);
   E->device = device; E->B = num_envs; E->flags = flags; E->sm_count = prop.multiProcessorCount;
   E->blob_hash = fnv1a(blobs[0], blob_sizes[0]);
   rc = upload_tables(E, D);
@@ -1036,8 +1048,9 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
     const int ncp = (E->R.view_w + 3) / 4, ncw = (T.W + (32 >> E->R.wstrip_log2) - 1) / (32 >> E->R.wstrip_log2);
 #define MP_RENDER_INST(NCP, NCW)                                                                                  \
   {                                                                                                               \
-    E->render_fn = k_render<NCP, NCW, RENDER_PLAIN>; E->render_gather_fn = k_render<NCP, NCW, RENDER_GATHER>;     \
-    E->render_routed_fn = k_render<NCP, NCW, RENDER_ROUTED>; E->inst_ncp = NCP; E->inst_ncw = NCW;                \
+    E->render_fns[RENDER_PLAIN] = k_render<NCP, NCW, RENDER_PLAIN>;                                               \
+    E->render_fns[RENDER_GATHER] = k_render<NCP, NCW, RENDER_GATHER>;                                             \
+    E->render_fns[RENDER_ROUTED] = k_render<NCP, NCW, RENDER_ROUTED>; E->inst_ncp = NCP; E->inst_ncw = NCW;       \
   }
     if (ncp <= 3 && ncw <= 3) MP_RENDER_INST(3, 3)
     else if (ncp <= 3 && ncw <= 4) MP_RENDER_INST(3, 4)
@@ -1061,9 +1074,9 @@ int create(const void* const* blobs, const size_t* blob_sizes, int n_blobs, cons
   }
   // The attribute belongs to the kernel function, not to this handle: engines that share an instantiation must not
   // lower each other's limit, so the renderer always gets the opt-in maximum and the step kernels only ever raise theirs.
-  cudaError_t ce = cudaFuncSetAttribute(E->render_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
-  if (ce == cudaSuccess) ce = cudaFuncSetAttribute(E->render_gather_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
-  if (ce == cudaSuccess) ce = cudaFuncSetAttribute(E->render_routed_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
+  cudaError_t ce = cudaSuccess;
+  for (auto fn : E->render_fns)
+    if (ce == cudaSuccess) ce = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmemLimit);
   {
     static int step_smem_max[MP_MAX_DEVICES] = {};
     const int need = (int)E->step_smem;
@@ -1361,12 +1374,15 @@ int mp_step_state(mp_handle h, const int32_t* actions, void* stream) {
 int mp_render(mp_handle h, void* stream) {
   if (!h) return fail(MP_E_INVALID, "null handle");
   DeviceGuard guard(h->device);
+  clear_last_launch(h);
   return launch_render(h, (cudaStream_t)stream);
 }
 
 int mp_step(mp_handle h, const int32_t* actions, void* stream) {
   int rc = mp_step_state(h, actions, stream);
-  return rc ? rc : mp_render(h, stream);
+  if (rc) return rc;
+  DeviceGuard guard(h->device);
+  return launch_render(h, (cudaStream_t)stream);
 }
 
 }  // extern "C"
@@ -1788,6 +1804,7 @@ int mp_state_load(mp_handle h, const void* host_src, uint64_t nbytes, void* stre
     CUDA_TRY(cudaMemcpyAsync(w.base, src, (size_t)h->B * w.bytes, cudaMemcpyHostToDevice, st));
     src += (size_t)h->B * w.bytes;
   }
+  clear_last_launch(h);
   int rc = launch_render(h, st);
   if (rc) return rc;
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -2008,6 +2025,7 @@ int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, 
                                                   (flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base);
   ++h->launches;
   CUDA_TRY(cudaGetLastError());
+  clear_last_launch(h);
   return launch_render(h, st);
 }
 
@@ -2096,6 +2114,12 @@ int mp_debug_render_plan(mp_handle h, int32_t out[MP_RENDER_PLAN_FIELDS]) {
   const int32_t v[MP_RENDER_PLAN_FIELDS] = {R.n_teams, R.team_threads, R.wstrip_log2, R.smem_bytes, R.n_total, R.rec_stride, R.stage_bytes,
                                             R.grid_bytes, h->lane_map_players, h->lane_map_world, h->inst_ncp, h->inst_ncw};
   memcpy(out, v, sizeof v);
+  return MP_OK;
+}
+
+int mp_debug_last_launch(mp_handle h, int32_t out[MP_LAST_LAUNCH_FIELDS]) {
+  if (!h || !out) return fail(MP_E_INVALID, "mp_debug_last_launch: null argument");
+  memcpy(out, h->last_launch, sizeof h->last_launch);
   return MP_OK;
 }
 

@@ -61,7 +61,7 @@ EXPORTED_SYMBOLS = (
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
     'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
     'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_step_restore',
-    'mp_step_players', 'mp_reset_players', 'mp_step_routed', 'mp_step_drawn', 'mp_reset_drawn',
+    'mp_step_players', 'mp_reset_players', 'mp_step_routed', 'mp_step_drawn', 'mp_reset_drawn', 'mp_debug_last_launch',
 )
 
 MP_RESTORE_REKEY = 1
@@ -391,6 +391,7 @@ def load_library() -> ctypes.CDLL:
   lib.mp_reset_drawn.argtypes = [vp, vp, ctypes.POINTER(MpRouteDraw), ctypes.POINTER(MpDeviceOutputs),
                                  ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
+  lib.mp_debug_last_launch.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
   lib.mp_step_host_async.argtypes = [vp, vp, ctypes.POINTER(MpHostOutputs), ctypes.c_int, vp]
   lib.mp_wait.argtypes = [vp, ctypes.c_int]
@@ -931,6 +932,19 @@ class Engine:
     out = (ctypes.c_int32 * len(keys))()
     _check(self._lib.mp_debug_render_plan(self._h, out))
     return dict(zip(keys, (int(v) for v in out)))
+
+  # mp_debug_last_launch's fields, in order
+  LAST_LAUNCH_FIELDS = ('family', 'variants', 'restore', 'actions', 'render_mode', 'ncp', 'ncw', 'teams', 'warps',
+                        'wstrip_log2')
+
+  def last_launch(self):
+    """The k_step cell and the k_render mode and layout of the last call that launched either, -1 for a part it did
+    not launch (diagnostic): family (MpbFamily), variants (0/1), restore (0/1), actions (0 dense, 1 rows, 2 drawn),
+    render_mode (0 plain, 1 gather, 2 routed), the k_render<ncp, ncw> instantiation, teams, warps per team and
+    wstrip_log2."""
+    out = (ctypes.c_int32 * len(self.LAST_LAUNCH_FIELDS))()
+    _check(self._lib.mp_debug_last_launch(self._h, out))
+    return dict(zip(self.LAST_LAUNCH_FIELDS, (int(v) for v in out)))
 
   def render_tables(self):
     """(pair[n, n], flags[n]) uint8 numpy arrays of the renderer's sprite tables (diagnostic)."""
