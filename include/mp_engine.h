@@ -61,7 +61,7 @@ enum {
 #define MP_FLAGS_CREATE_ONLY (MP_FLAG_DEBUG_PLAIN_LANE_MAP | MP_FLAG_DEBUG_SCATTER_LANE_MAP | MP_FLAG_DEBUG_NO_PREMERGE | MP_FLAG_LAYOUT_MASK)
 
 /* Device buffers owned by the engine; valid until mp_destroy. Contents are overwritten by the
- * next mp_step/mp_reset on the same handle (mp_step_into / mp_reset_into: see there for the images). B = num_envs, P = players. */
+ * next step or reset on the same handle (mp_run with `out` or `players`: see mp_request for the images). B = num_envs, P = players. */
 typedef struct mp_buffers {
   int32_t num_envs, num_players;
   int32_t rgb_h, rgb_w;     /* per-player view in pixels (88 x 88 for clean_up) */
@@ -111,7 +111,7 @@ typedef struct mp_buffers {
 /* Replaces dmlab2d.Lab2d(...) + dmlab2d.Environment(...) (builder.py:182-187) for `num_envs`
  * independent instances on CUDA device `device`. `blob` is a compiled substrate
  * (include/mpb_format.h). Env b uses RNG key `seed + env_index_base + b`, so results do not
- * depend on how envs are sharded over GPUs. Does NOT start an episode; call mp_reset. */
+ * depend on how envs are sharded over GPUs. Does NOT start an episode; run a reset (mp_run). */
 int mp_create(const void* blob, size_t blob_bytes, int num_envs, int device, uint64_t seed,
               uint64_t env_index_base, uint32_t flags, mp_handle* out);
 
@@ -145,7 +145,7 @@ int mp_create_variants(const void* const* blobs, const size_t* blob_bytes, int n
                        int num_envs, int device, uint64_t seed, uint64_t env_index_base, uint32_t flags, mp_handle* out);
 
 /* Reassigns envs to variants: copies `env_variant` (DEVICE pointer to num_envs bytes) into the pending assignments on
- * `stream`. An env takes its pending variant when its next episode starts (the auto-reset after LAST, or mp_reset), never
+ * `stream`. An env takes its pending variant when its next episode starts (the auto-reset after LAST, or a reset), never
  * mid-episode, as the reference's ResetWrapper rebuilds its env on every reset; reset envs with a mask to switch them
  * at once. A value >= n_variants runs as variant 0. Only for engines with more than one variant. */
 int mp_set_env_variants(mp_handle h, const uint8_t* env_variant, void* stream);
@@ -162,18 +162,6 @@ int mp_destroy(mp_handle h);
 /* Changes the per-launch flags (render outputs, diagnostics); the MP_FLAGS_CREATE_ONLY bits keep their creation values. */
 int mp_set_flags(mp_handle h, uint32_t flags);
 
-/* Replaces dmlab2d.Environment.reset (wrappers/base.py:30-32; api_factory.lua:85-102): every
- * env (or only those with env_mask[b] != 0; `env_mask` is a DEVICE pointer or NULL) starts its
- * next episode and its FIRST observation is rendered. Asynchronous on `stream` (a cudaStream_t). */
-int mp_reset(mp_handle h, const uint8_t* env_mask, void* stream);
-
-/* Replaces dmlab2d.Environment.step (wrappers/base.py:34-36; api_factory.lua:104-111) including
- * the DiscreteActionWrapper table lookup (discrete_action_wrapper.py:97-100).
- * `actions` is a DEVICE pointer to int32 [B][P] discrete action ids. Envs whose previous step was
- * LAST ignore the action and start a new episode (FIRST). Runs the state transition and renders
- * all observations. Asynchronous on `stream`. */
-int mp_step(mp_handle h, const int32_t* actions, void* stream);
-
 /* Caller-owned DEVICE outputs of one step, e.g. slot t of a learner's [T, B, ...] or [B, T, ...] trajectory buffer.
  * Every pointer is optional (NULL: that output is not delivered by this call). Each output is B per-env records at a
  * byte stride between env b and b + 1; inside a record the layout is that of mp_buffers. */
@@ -186,25 +174,7 @@ typedef struct mp_device_outputs {
   double*  scalar_obs; uint64_t scalar_obs_env_stride, scalar_obs_stride; /* [n_scalar] x [B] x f64 [P] */
 } mp_device_outputs;
 
-/* mp_step / mp_reset whose outputs go into `out` (any subset):
- *   - the images named in `out` are stored by the renderer straight into `out` (no second pass over HBM) and the
- *     engine's own images are not written; an image `out` leaves NULL is rendered into the engine's own set as usual;
- *   - reward, discount, step type and scalar observations are written to the engine's scalar block as always (the
- *     exchange, the host paths and mp_buffers read them there) and also delivered into `out` by the kernel that follows
- *     the state transition, so the call launches exactly as many kernels as mp_step / mp_reset (with rendering off and
- *     no exchange connected, the rows travel by device-to-device copies on `stream`);
- *   - afterwards mp_buffers holds that step's state and scalars, plus the images of the last render into the engine's
- *     own set (as after a slot-1 mp_step_host_async call).
- * Every check runs before anything is enqueued; a refused call (MP_E_INVALID) steps no env. Refused: image pointers or
- * image env strides that are not multiples of 16 (the TMA bulk store's alignment); scalar pointers or strides that are
- * not multiples of 8, or of 2 GiB or more; an env stride smaller than one env's bytes; scalar_obs rows (n_scalar x B
- * rows of P doubles) that overlap, or scalar_obs on a substrate without scalar observations; an image the current render
- * flags switch off; an output whose extent does not lie in one device allocation on the engine's device; outputs whose
- * extents overlap each other or the engine's own buffers. */
-int mp_step_into(mp_handle h, const int32_t* actions, const mp_device_outputs* out, void* stream);
-int mp_reset_into(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, void* stream);
-
-/* State transition only / rendering only (mp_step == mp_step_state + mp_render). */
+/* State transition only / rendering only (a step request of mp_run with only `actions` == mp_step_state + mp_render). */
 int mp_step_state(mp_handle h, const int32_t* actions, void* stream);
 int mp_render(mp_handle h, void* stream);
 
@@ -238,9 +208,9 @@ int mp_reset_host(mp_handle h, const mp_host_outputs* out, void* stream);
  * until mp_wait on the same slot returns. Steps are still applied in call order (one state per env). A call refused
  * with an error (e.g. `out` names events, which are not staged per slot) enqueues nothing and steps no env.
  * Slot 0 renders into the engine's own images (mp_buffers.rgb / world_rgb); every other call that renders there
- * (mp_step, mp_render, mp_step_host, mp_reset, mp_reset_host, mp_state_load, and mp_step_into / mp_reset_into when
- * `out` leaves a rendered image NULL) first waits, on its stream, for slot 0's copy-out, so it may be issued before
- * mp_wait(h, 0). Slot 1 renders into a set of its own, as mp_step_into does into a dense target: after a slot-1 call,
+ * (mp_run when neither `out` nor `players` takes a rendered image, mp_render, mp_step_host, mp_reset_host,
+ * mp_state_load) first waits, on its stream, for slot 0's copy-out, so it may be issued before
+ * mp_wait(h, 0). Slot 1 renders into a set of its own, as mp_run does into a dense `out`: after a slot-1 call,
  * mp_buffers holds that step's scalars and state, and the images of the last render into the engine's own set. */
 int mp_step_host_async(mp_handle h, const int32_t* actions_host, const mp_host_outputs* out, int slot, void* stream);
 int mp_wait(mp_handle h, int slot);
@@ -259,8 +229,8 @@ int mp_wait(mp_handle h, int slot);
  *                        and back (one process per GPU: exchange handle and offset through torch.distributed);
  *   mp_enable_peer_access for ranks that live in ONE process (tests): plain cudaDeviceEnablePeerAccess;
  *   mp_exchange_connect  takes, in rank order, every rank's block as mapped into this process (its own entry = the
- *                        pointer mp_exchange_create returned); from then on every mp_step / mp_step_state /
- *                        mp_reset publishes. All ranks must issue the same sequence of steps and resets (the slot
+ *                        pointer mp_exchange_create returned); from then on every mp_run / mp_step_state
+ *                        publishes. All ranks must issue the same sequence of steps and resets (the slot
  *                        is the parity of the launch sequence number);
  *   mp_exchange_wait     enqueues on `stream` (ordered after the step's kernels) the publish-and-wait of the most recent step;
  *                        every rank must call it once per step;
@@ -330,22 +300,6 @@ int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* b
 #define MP_RESTORE_REKEY 1u
 int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, void* stream);
 
-/* A step that restores at the same time: env b takes bank row slot_of_env[b] under mp_state_restore's rule (index in
- * 0..n_slots-1, this engine's tag) instead of advancing, and ignores its action; the restore takes precedence over its
- * auto-reset after LAST. Every other env steps as in mp_step. The state transition does the restore in the same kernel,
- * so the render that follows draws the restored envs with all the others: no second render, no extra launch. For an
- * engine that is not connected, the call gives, byte for byte, what mp_step(actions) followed by mp_state_restore(
- * slot_of_env, bank, n_slots, flags) gives: outputs, events, state, variants and keys. flags: MP_RESTORE_REKEY as for
- * mp_state_restore. out: NULL launches as mp_step does, a target as mp_step_into does (same kernels, same count, the
- * restored envs' timestep and images delivered into it like any env's). It is accepted after mp_exchange_connect /
- * mp_gather_obs_connect and counts as a step in their sequence, so the restored envs' rows and images are published as
- * a step's; every rank issues it wherever the others issue a step (an index of all -1 restores nothing). Its render
- * waits for slot 0's copy-out of mp_step_host_async as mp_step's does. Every check runs before anything is enqueued, and
- * a refused call steps no env: those of mp_state_restore's bank and index array, those of mp_step_into's `out`, and
- * the bank and the index array must not overlap `out`'s targets. */
-int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
-                    const mp_device_outputs* out, void* stream);
-
 /* Caller-owned DEVICE rows of a step's per-player outputs: player p of env b is delivered to row row_of_player[b][p]
  * when 0 <= row < n_rows, and to no row otherwise. A learner lays rows out as it consumes them, e.g. one contiguous block
  * per policy of a population, focal players apart from background players, or unread players left out. Every target
@@ -364,43 +318,6 @@ typedef struct mp_player_outputs {
   uint8_t* world_rgb; uint64_t world_rgb_row_stride;  /* [world_n_rows] x u8 [world_h][world_w][3], dense inside a row */
 } mp_player_outputs;
 
-/* mp_step_restore (slot_of_env and bank set) or mp_step_into (both NULL) whose per-player outputs also go to rows:
- *   - images: when players->rgb is set, player p of env b is drawn straight into players->rgb + row * rgb_row_stride,
- *     and the engine's own rgb is written for no player. A player without a row is neither composited nor stored, so
- *     leaving unread players out saves their share of the render. Without players->rgb the images go where
- *     mp_step_into puts them;
- *   - reward and scalar observations of a routed player are written to its row as well; the engine's scalar block is
- *     still written in full, so mp_buffers, the exchange and the host paths see every player;
- *   - WORLD.RGB: when players->world_rgb is set, env b's image is drawn straight into players->world_rgb + row *
- *     world_rgb_row_stride, row = world_row_of_env[b]; an env without a row is neither composited nor stored, and the
- *     engine's own world_rgb is written for no env. Without players->world_rgb, WORLD.RGB stays per env;
- *   - discount and step type stay per env: they and any WORLD.RGB not routed go to `out` (any subset, or NULL) or the
- *     engine's buffers;
- *   - restored envs are routed like any other; flags: MP_RESTORE_REKEY, only with a bank.
- * For every routed player and every env with a world row the call gives, byte for byte, what mp_step_into /
- * mp_step_restore / mp_reset_into with the same `out` give at (b, p) and for env b's WORLD.RGB, and it launches as many
- * kernels when a render follows. With rendering off, the routed scalars are delivered by one small kernel
- * (k_exchange_push), which that case adds.
- * Two players routed to one row, or two envs to one world row, are the caller's error: the row then holds one of them,
- * unspecified which. The row maps are read on the device and never checked on the host (that would synchronise); nothing
- * outside [0, n_rows) or [0, world_n_rows) is written. The exchange (mp_exchange_*) works unchanged and the call
- * counts as a step in its sequence. Refused with MP_E_UNSUPPORTED while the observation gather (mp_gather_obs_*) is
- * connected and enabled: its stacked slots stay dense and complete.
- * Every check runs before anything is enqueued, and a refused call (MP_E_INVALID) steps no env. Refused: a NULL handle,
- * actions or players, n_rows < 1; row_of_player not 4-byte aligned or not B * P i32 inside one device allocation on the
- * engine's device; rgb while the render flags switch player images off, or together with out->rgb; scalar_obs on a
- * substrate without scalar observations; rgb or its row stride not a multiple of 16 bytes; reward / scalar_obs pointers
- * or strides not multiples of 8, or of 2 GiB or more; a row stride smaller than one row; scalar_obs rows (n_scalar x
- * n_rows) that overlap; world_rgb without world_row_of_env or the reverse, world_n_rows < 1, world_row_of_env not 4-byte
- * aligned or not B i32 inside one device allocation on the engine's device, world_rgb or its row stride not a multiple
- * of 16 bytes, a world row stride smaller than one WORLD.RGB image, world_rgb while the render flags switch WORLD.RGB
- * off, or together with out->world_rgb; any target or row map that overlaps another, `out`'s targets, the bank, the
- * index array or the engine's buffers; and every refusal of mp_step_into's `out` and mp_step_restore's bank. */
-int mp_step_players(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots,
-                    uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players, void* stream);
-int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out,
-                     const mp_player_outputs* players, void* stream);
-
 /* Caller-owned DEVICE rows a step's actions are read from: player p of env b takes the action id in row
  * row_of_player[b][p] when 0 <= row < n_rows, and action 0 (NOOP in every shipped substrate) otherwise. A learner that
  * gets its observations in rows (mp_player_outputs) writes its actions into rows laid out the same way, and nothing is
@@ -410,25 +327,6 @@ typedef struct mp_player_actions {
   int32_t n_rows;
   const int32_t* action; uint64_t action_row_stride;  /* [n_rows] x i32, stride in bytes */
 } mp_player_actions;
-
-/* A step whose actions come from rows. With dense[b][p] the action the rule above gives player p of env b, the call is,
- * byte for byte (outputs, events, state, keys, variant bytes) and launch for launch:
- *   - mp_step_players(dense, slot_of_env, bank, n_slots, flags, out, players) when players is set;
- *   - mp_step_restore(dense, slot_of_env, bank, n_slots, flags, out) when only slot_of_env / bank are given;
- *   - mp_step_into(dense, out), or mp_step(dense) when out is NULL, when neither is given.
- * An id out of range in a row is action 0, as in a dense step; a restored env and an env stepping after LAST ignore
- * their actions. The row map and the rows are read on the device and never checked on the host. With players NULL the
- * call is accepted while the observation gather is enabled (no image is routed); with players set it is refused as
- * mp_step_players refuses it.
- * Every check runs before anything is enqueued, and a refused call (MP_E_INVALID) steps no env. Refused besides every
- * refusal of the composed call: a NULL actions or n_rows < 1; a row map not 4-byte aligned or not B * P i32 inside one
- * device allocation on the engine's device; an action pointer or stride not a multiple of 4, or of 2 GiB or more; a
- * stride smaller than 4; action rows not inside one device allocation on the engine's device; a row map or action
- * rows that overlap any target, the bank, the index array or the engine's buffers (the two row maps may be one tensor,
- * both are only read). */
-int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t* slot_of_env, const void* bank,
-                   int n_slots, uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players,
-                   void* stream);
 
 /* Drawn routes: the row of each player is drawn again at every episode start, on the device, as a scenario's
  * background population is resampled at every reset. Player slot p lists n_choices[p] (0..MP_MAX_ROUTE_CHOICES)
@@ -451,24 +349,116 @@ typedef struct mp_route_draw {
   int32_t rows_per_env[MP_MAX_ROUTE_PLAYERS][MP_MAX_ROUTE_CHOICES];
 } mp_route_draw;
 
-/* mp_step_players / mp_reset_players on drawn routes. After every call, row_of_player[b][p] is the row the rule above
- * gives for the episode env b is in then, for every env: one that stepped, started an episode (auto-reset, or reset),
- * was masked out of a reset, was restored (a record's key and episode, or its own key with MP_RESTORE_REKEY) or switched
- * variant. In mp_step_drawn, player p takes the action id in row row_of_player[b][p] of `action` (rows
- * action_row_stride bytes apart) for the episode it is in before the step, action 0 without a row; envs that start an
- * episode or are restored ignore their actions. For every routed (b, p) the call gives, byte for byte, what
- * mp_step_routed (with players) and mp_reset_players give when handed the map as a fixed input, and it launches the same
- * kernels, as many of them. players->row_of_player and players->n_rows must be the draw's map and n_rows.
- * Every check runs before anything is enqueued, and a refused call (MP_E_INVALID) steps no env. Refused besides every
- * refusal of mp_step_routed (with players) / mp_reset_players: a NULL draw, draw n_rows < 1, players whose map or n_rows
- * are not the draw's, a slot with more than MP_MAX_ROUTE_CHOICES choices (or fewer than 0), and a choice whose rows of
- * some env fall outside [0, n_rows). The map must not overlap any target, the action rows, the bank, the index array or
- * the engine's buffers; MP_E_UNSUPPORTED while the observation gather is enabled, as for mp_step_players. */
-int mp_step_drawn(mp_handle h, const mp_route_draw* draw, const int32_t* action, uint64_t action_row_stride,
-                  const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, const mp_device_outputs* out,
-                  const mp_player_outputs* players, void* stream);
-int mp_reset_drawn(mp_handle h, const uint8_t* env_mask, const mp_route_draw* draw, const mp_device_outputs* out,
-                   const mp_player_outputs* players, void* stream);
+/* One step or reset of the batch for mp_run. Every pointer is optional (NULL: not asked for) unless stated, and the
+ * fields compose; what each one adds:
+ *
+ * reset, env_mask: reset = 1 replaces dmlab2d.Environment.reset (wrappers/base.py:30-32; api_factory.lua:85-102): every
+ *   env, or only those with env_mask[b] != 0 (DEVICE u8 [B]), starts its next episode and its FIRST observation is
+ *   rendered. reset = 0 is a step.
+ * actions: a step replaces dmlab2d.Environment.step (wrappers/base.py:34-36; api_factory.lua:104-111) including the
+ *   DiscreteActionWrapper table lookup (discrete_action_wrapper.py:97-100): DEVICE i32 [B][P] discrete action ids. Envs
+ *   whose previous step was LAST ignore the action and start a new episode (FIRST). The step runs the state transition
+ *   and renders all observations.
+ * player_actions: a step's actions read from rows (mp_player_actions) instead of `actions`. With dense[b][p] the action
+ *   the rule of mp_player_actions gives player p of env b, the request gives, byte for byte (outputs, events, state, keys,
+ *   variant bytes) and launch for launch, what the same request with the dense actions those rows give does. An id out of
+ *   range in a row is action 0, as in a dense step; a restored env and an env stepping after LAST ignore their actions.
+ *   The row map and the rows are read on the device and never checked on the host. Without `players` the request is
+ *   accepted while the observation gather is enabled (no image is routed).
+ * slot_of_env, bank, n_slots, restore_flags: a step that restores at the same time: env b takes bank row slot_of_env[b]
+ *   (slot_of_env: DEVICE i32 [B]) under mp_state_restore's rule (index in 0..n_slots-1, this engine's tag) instead of
+ *   advancing, and ignores its action; the restore takes precedence over its auto-reset after LAST. Every other env
+ *   steps as it would without them. The state transition does the restore in the same kernel, so the render that
+ *   follows draws the restored envs with all the others: no second render, no extra launch. For an engine that is not
+ *   connected, a request without `out` and `players` gives, byte for byte, what the same step without a restore followed
+ *   by mp_state_restore(slot_of_env, bank, n_slots, restore_flags) gives: outputs, events, state, variants and keys; with
+ *   `out` or `players`, the restored envs' timestep and images are delivered into them like any env's. restore_flags:
+ *   MP_RESTORE_REKEY as for mp_state_restore. A restoring step is accepted after mp_exchange_connect /
+ *   mp_gather_obs_connect and counts as a step in their sequence, so the restored envs' rows and images are published as
+ *   a step's; every rank issues it wherever the others issue a step (an index of all -1 restores nothing).
+ * out: the outputs go into caller-owned targets (mp_device_outputs, any subset):
+ *   - the images named in `out` are stored by the renderer straight into `out` (no second pass over HBM) and the
+ *     engine's own images are not written; an image `out` leaves NULL is rendered into the engine's own set as usual;
+ *   - reward, discount, step type and scalar observations are written to the engine's scalar block as always (the
+ *     exchange, the host paths and mp_buffers read them there) and also delivered into `out` by the kernel that follows
+ *     the state transition, so `out` adds no launch (with rendering off and no exchange connected, the rows travel by
+ *     device-to-device copies on `stream`);
+ *   - afterwards mp_buffers holds that step's state and scalars, plus the images of the last render into the engine's
+ *     own set (as after a slot-1 mp_step_host_async call).
+ * players: the per-player outputs also go to rows (mp_player_outputs):
+ *   - images: when players->rgb is set, player p of env b is drawn straight into players->rgb + row * rgb_row_stride,
+ *     and the engine's own rgb is written for no player. A player without a row is neither composited nor stored, so
+ *     leaving unread players out saves their share of the render. Without players->rgb the images go to `out` or the
+ *     engine's own set, as without `players`;
+ *   - reward and scalar observations of a routed player are written to its row as well; the engine's scalar block is
+ *     still written in full, so mp_buffers, the exchange and the host paths see every player;
+ *   - WORLD.RGB: when players->world_rgb is set, env b's image is drawn straight into players->world_rgb + row *
+ *     world_rgb_row_stride, row = world_row_of_env[b]; an env without a row is neither composited nor stored, and the
+ *     engine's own world_rgb is written for no env. Without players->world_rgb, WORLD.RGB stays per env;
+ *   - discount and step type stay per env: they and any WORLD.RGB not routed go to `out` or the engine's buffers;
+ *   - restored envs are routed like any other.
+ *   For every routed player and every env with a world row the request gives, byte for byte, what the same request
+ *   without `players` gives at (b, p) and for env b's WORLD.RGB. Two players routed to one row, or two envs to one world
+ *   row, are the caller's error: the row then holds one of them, unspecified which. The row maps are read on the device
+ *   and never checked on the host (that would synchronise); nothing outside [0, n_rows) or [0, world_n_rows) is written.
+ *   The exchange (mp_exchange_*) works unchanged. Refused with MP_E_UNSUPPORTED while the observation gather
+ *   (mp_gather_obs_*) is connected and enabled: its stacked slots stay dense and complete.
+ * draw: drawn routes (mp_route_draw), with `players` and, on a step, `player_actions`. After every request,
+ *   row_of_player[b][p] is the row the draw's rule gives for the episode env b is in then, for every env: one that
+ *   stepped, started an episode (auto-reset, or reset), was masked out of a reset, was restored (a record's key and
+ *   episode, or its own key with MP_RESTORE_REKEY) or switched variant. On a step, player p takes the action id in row
+ *   row_of_player[b][p] of player_actions->action for the episode it is in before the step, action 0 without a row; envs
+ *   that start an episode or are restored ignore their actions. players and player_actions must deliver and read through
+ *   the draw's row map and n_rows. For every routed (b, p) the request gives, byte for byte, what the same request
+ *   without `draw` gives when handed the map as a fixed input (the map before a step for its actions, the map after it
+ *   for its outputs), and it launches the same kernels, as many of them.
+ *
+ * Launches: a reset, and a request with `out` or `players`, launch the state transition and one render, which also
+ * publishes the step to a connected exchange. A step with neither launches as mp_step_state followed by mp_render: with
+ * the exchange connected, k_exchange_push follows the state transition. With rendering off, `players` with reward or
+ * scalar_obs rows adds one small kernel (k_exchange_push) that delivers them.
+ *
+ * Every check runs before anything is enqueued, and a refused request (MP_E_INVALID) steps no env. Refused:
+ *   - the request: a NULL handle or request; a reset with actions, player_actions, slot_of_env, bank or restore_flags; a
+ *     step with env_mask; a step with both actions and player_actions, or with neither; draw without players;
+ *   - player_actions: n_rows < 1; a row map not 4-byte aligned or not B * P i32 inside one device allocation on the
+ *     engine's device; an action pointer or stride not a multiple of 4, or of 2 GiB or more; a stride smaller than 4;
+ *     action rows not inside one device allocation on the engine's device; a row map or action rows that overlap any
+ *     target, the bank, the index array or the engine's buffers (the two row maps may be one tensor, both are only read);
+ *   - the restore: slot_of_env without bank or the reverse; n_slots < 1; restore_flags other than MP_RESTORE_REKEY, or
+ *     any without a bank; the refusals of mp_state_restore's bank and index array; a bank or index array that overlaps a
+ *     target;
+ *   - out: image pointers or image env strides that are not multiples of 16 (the TMA bulk store's alignment); scalar
+ *     pointers or strides that are not multiples of 8, or of 2 GiB or more; an env stride smaller than one env's bytes;
+ *     scalar_obs rows (n_scalar x B rows of P doubles) that overlap, or scalar_obs on a substrate without scalar
+ *     observations; an image the current render flags switch off; an output whose extent does not lie in one device
+ *     allocation on the engine's device; outputs whose extents overlap each other or the engine's own buffers;
+ *   - players: n_rows < 1; row_of_player not 4-byte aligned or not B * P i32 inside one device allocation on the engine's
+ *     device; rgb while the render flags switch player images off, or together with out->rgb; scalar_obs on a substrate
+ *     without scalar observations; rgb or its row stride not a multiple of 16 bytes; reward / scalar_obs pointers or
+ *     strides not multiples of 8, or of 2 GiB or more; a row stride smaller than one row; scalar_obs rows (n_scalar x
+ *     n_rows) that overlap; world_rgb without world_row_of_env or the reverse, world_n_rows < 1, world_row_of_env not
+ *     4-byte aligned or not B i32 inside one device allocation on the engine's device, world_rgb or its row stride not a
+ *     multiple of 16 bytes, a world row stride smaller than one WORLD.RGB image, world_rgb while the render flags switch
+ *     WORLD.RGB off, or together with out->world_rgb; any target or row map that overlaps another, `out`'s targets, the
+ *     bank, the index array or the engine's buffers;
+ *   - draw: draw n_rows < 1; players whose map or n_rows are not the draw's; a step whose player_actions are missing or
+ *     have a map or n_rows that are not the draw's; a slot with more than MP_MAX_ROUTE_CHOICES choices (or fewer than
+ *     0); a choice whose rows of some env fall outside [0, n_rows). The map must not overlap any target, the action
+ *     rows, the bank, the index array or the engine's buffers. */
+typedef struct mp_request {
+  int32_t reset;                            /* 0: a step, 1: a reset */
+  const uint8_t* env_mask;                  /* reset only: DEVICE u8 [B], NULL = every env */
+  const int32_t* actions;                   /* step: DEVICE i32 [B][P]; NULL when player_actions is given */
+  const mp_player_actions* player_actions;  /* step only: actions read from rows */
+  const mp_route_draw* draw;                /* drawn routes; needs players */
+  const int32_t* slot_of_env; const void* bank; int32_t n_slots; uint32_t restore_flags;  /* step only */
+  const mp_device_outputs* out;             /* optional */
+  const mp_player_outputs* players;         /* optional */
+} mp_request;
+
+/* Runs request `r` on `stream` (a cudaStream_t): see mp_request. */
+int mp_run(mp_handle h, const mp_request* r, void* stream);
 
 /* Diagnostic: how the renderer was laid out for this substrate: teams per CTA, threads per team, log2 of the pixel
  * rows per WORLD.RGB strip, shared memory bytes, atlas sprites, record stride (u16), staging bytes per warp, grid bytes,

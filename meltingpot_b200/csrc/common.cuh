@@ -88,7 +88,7 @@ struct ScalarTargets {
   int on;  // any of the four is set
 };
 
-// Caller-owned per-player rows of one step (mp_player_outputs, mp_step_players): player p of env b goes to row
+// Caller-owned per-player rows of one step (mp_player_outputs, mp_run's players): player p of env b goes to row
 // row_of_player[b][p] when that is in [0, n_rows). Strides in bytes; scalar_obs row (k, r) starts at
 // scalar_obs + k * scalar_obs_stride + r * scalar_obs_row_stride. Env b's WORLD.RGB goes to row world_row_of_env[b]
 // of world_rgb when that is in [0, world_n_rows) and world_rgb is set. Read only by k_render<..., RENDER_ROUTED> and
@@ -150,11 +150,11 @@ struct State {
   uint8_t* g_wrgb[MP_MAX_PEERS];
   const unsigned long long* g_flags;       // local flags[r] = last render rank r has fully delivered here
   // Where k_render stores env b's images: rgb + b * rgb_env_stride (player p at + p * player_bytes) and
-  // world_rgb + b * world_env_stride, in bytes. The engine's own images are the dense case; mp_step_into points them at
+  // world_rgb + b * world_env_stride, in bytes. The engine's own images are the dense case; mp_run's out points them at
   // a caller's tensors. (Kept behind every field the state-transition kernels read.)
   uint64_t rgb_env_stride, world_env_stride;
-  ScalarTargets out;                       // the step's scalar rows into caller-owned memory (mp_step_into), or none
-  PlayerTargets pr;                        // the step's per-player rows (mp_step_players), or all zero
+  ScalarTargets out;                       // the step's scalar rows into caller-owned memory (mp_run's out), or none
+  PlayerTargets pr;                        // the step's per-player rows (mp_run's players), or all zero
 };
 
 // Events of the current step (the reference's events:add calls on the hot path). Types follow

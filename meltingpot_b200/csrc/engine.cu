@@ -156,7 +156,7 @@ struct FamilyEntry {
   int (*upload_variants)(std::vector<void*>&, const std::vector<FamilyParams>&, const void**);
   // Every k_step<Family, ...> an engine may launch, [variants][restore][actions]: Source Params or ParamVariants<Params>
   // (mp_create_variants), kRestore (a step that restores envs from a bank), and the action source: DenseActions,
-  // RowActions (mp_step_routed) or drawn routes (k_step_drawn: mp_step_drawn, and mp_reset_drawn without restore).
+  // RowActions (mp_run's player_actions) or drawn routes (k_step_drawn: mp_run's draw; a drawn reset without restore).
   const void* step[2][2][3];
   // Launches `kernel`, one of `step`, with the kernel arguments `args` after filling in its Source argument (args[1]):
   // `params` for one blob, or the ParamVariants<Params> of `variants`.
@@ -274,7 +274,7 @@ struct mp_engine {
   uint64_t blob_hash = 0;  // FNV-1a of the compiled blob (of the ordered variant set): a snapshot only loads into an engine built from the same
   VariantSet variants;     // n > 1: per-env parameter variants (mp_create_variants)
   RecordLayout record{};                     // every per-env state array (layout_state): what records and snapshots copy
-  RecordLayout* d_record_layout = nullptr;  // device copy of `record`, read by mp_step_restore's k_step
+  RecordLayout* d_record_layout = nullptr;  // device copy of `record`, read by a restoring mp_run's k_step
 
   template <typename T>
   int alloc(size_t count, T** out) {
@@ -762,7 +762,7 @@ int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
 
 // `render_follows`: the caller launches the renderer next on the same stream; it raises the exchange flags.
 // `restore`: a step (mode 0) that restores the envs it names instead of advancing them (k_step<..., true>), or null.
-// `rows`: the step's actions come from rows (mp_step_routed, k_step<..., RowActions>; `actions` unused), or null.
+// `rows`: the step's actions come from rows (player_actions, k_step<..., RowActions>; `actions` unused), or null.
 // `drawn`: drawn routes (k_step_drawn, which writes the row map; `actions` and `rows` unused), or null.
 int launch_state(mp_engine* E, const int32_t* actions, const uint8_t* mask, int mode, cudaStream_t st, bool render_follows = true,
                  const StepRestore* restore = nullptr, const RowActions* rows = nullptr, const DrawnActions* drawn = nullptr) {
@@ -824,7 +824,7 @@ void apply_players(const mp_player_outputs& p, State& S) {
 }
 
 // `out`: where this render's outputs go besides / instead of the engine's own buffers (see apply_outputs), or null.
-// `players`: per-player rows (mp_step_players): the render runs k_render<..., RENDER_ROUTED>, or, with rendering off,
+// `players`: per-player rows (mp_run's players): the render runs k_render<..., RENDER_ROUTED>, or, with rendering off,
 // k_exchange_push delivers the routed scalars (one launch).
 int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = nullptr, const mp_player_outputs* routed = nullptr) {
   const bool players = E->flags & MP_FLAG_RENDER_PLAYERS, world = E->flags & MP_FLAG_RENDER_WORLD;
@@ -871,7 +871,7 @@ int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = 
   }
   State S = E->S;
   if (out) apply_outputs(*out, S);
-  if (routed) apply_players(*routed, S);  // (never with gather: mp_step_players refuses it)
+  if (routed) apply_players(*routed, S);  // (never with gather: mp_run refuses it)
   const int mode = routed ? RENDER_ROUTED : gather ? RENDER_GATHER : RENDER_PLAIN;
   CUDA_TRY(cudaLaunchKernelEx(&cfg, E->render_fns[mode], E->T, S, R, E->flags));
   const int32_t layout[6] = {mode, E->inst_ncp, E->inst_ncw, R.n_teams, R.team_threads / 32, R.wstrip_log2};
@@ -1378,13 +1378,6 @@ int mp_render(mp_handle h, void* stream) {
   return launch_render(h, (cudaStream_t)stream);
 }
 
-int mp_step(mp_handle h, const int32_t* actions, void* stream) {
-  int rc = mp_step_state(h, actions, stream);
-  if (rc) return rc;
-  DeviceGuard guard(h->device);
-  return launch_render(h, (cudaStream_t)stream);
-}
-
 }  // extern "C"
 
 namespace {
@@ -1392,10 +1385,13 @@ typedef unsigned __int128 u128;
 // A caller-owned device range an entry point reads or writes: `extent` bytes from `p`.
 struct DeviceExtent { const char* name; uintptr_t p; u128 extent; };
 
-// Each extent lies inside one device allocation on the engine's device and overlaps neither another extent nor the
-// engine's own buffers (mp_step_into's targets, mp_state_store / mp_state_restore's bank and index arrays).
+// Each extent spans less than 2^48 bytes, lies inside one device allocation on the engine's device and overlaps neither
+// another extent nor the engine's own buffers (mp_run's targets, row maps and action rows, the bank and index arrays of
+// mp_state_store / mp_state_restore / mp_run).
 int check_extents(mp_engine* E, const std::vector<DeviceExtent>& outs, const char* fn) {
   const uint64_t B = E->B, P = E->T.P;
+  for (const DeviceExtent& x : outs)
+    if (x.extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, x.name);
   // each extent inside one device allocation on the engine's device (cuMemGetAddressRange through the runtime's driver
   // entry point, as mp_ipc_export does, so the library does not link libcuda)
   typedef int (*GetRange)(unsigned long long*, size_t*, unsigned long long);
@@ -1441,49 +1437,55 @@ int check_extents(mp_engine* E, const std::vector<DeviceExtent>& outs, const cha
   return MP_OK;
 }
 
-// Every check of mp_step_into / mp_reset_into (include/mp_engine.h), before anything is enqueued: a pointer that fails
-// one never reaches a kernel. Extents are computed in 128 bits, so no stride can wrap them around. `outs`: other
-// extents of the call (mp_step_restore's bank and index array), which must not overlap the targets either.
-int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn, std::vector<DeviceExtent> outs = {}) {
-  if (!o) return fail(MP_E_INVALID, "%s: null outputs (use mp_step / mp_reset)", fn);
+// A caller-owned target of `count` records (`unit`: "env" or "row") of `per_record` bytes, `stride` bytes apart, plus
+// `extra` bytes past the last one (scalar_obs' other observations): checks the pointer and stride against `align` and
+// one record, and 8-byte targets' stride against 2 GiB, then appends its extent to `ext` for check_extents. Extents are
+// computed in 128 bits, so no stride can wrap them around. A null `p` is not asked for.
+int add_strided(std::vector<DeviceExtent>& ext, const char* fn, const char* unit, const char* name, const void* p, uint64_t stride,
+                uint64_t count, uint64_t per_record, uint64_t align, u128 extra) {
+  if (!p) return MP_OK;
+  if ((uintptr_t)p % align || stride % align)
+    return fail(MP_E_INVALID, "%s: %s pointer or %s stride is not a multiple of %llu bytes", fn, name, unit, (unsigned long long)align);
+  if (stride < per_record)
+    return fail(MP_E_INVALID, "%s: %s %s stride of %llu bytes is smaller than one %s's %llu bytes", fn, name, unit,
+                (unsigned long long)stride, unit, (unsigned long long)per_record);
+  if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s %s stride of 2 GiB or more", fn, name, unit);
+  ext.push_back({name, (uintptr_t)p, (u128)(count - 1) * stride + per_record + extra});
+  return MP_OK;
+}
+
+// scalar_obs targets hold n x count rows of `bytes` bytes at k * s + r * e (observation k, env or row r, e >= bytes).
+// Rows of one k are e apart; rows j = k' - k apart are |j * s + m * e| apart, m = r' - r in [-(count - 1), count - 1],
+// closest at m = -floor(j * s / e) or one below.
+int check_scalar_rows(const char* fn, const char* unit, const char* name, uint64_t s, uint64_t e, uint64_t n, uint64_t count,
+                      uint64_t bytes) {
+  for (uint64_t j = 1; j < n; ++j) {
+    const u128 d = (u128)j * s, q = d / e, r = d % e;
+    const u128 gap = q > count - 1 ? d - (u128)(count - 1) * e : (q + 1 <= count - 1 ? std::min<u128>(r, e - r) : r);
+    if (gap < bytes) return fail(MP_E_INVALID, "%s: %s rows overlap (%s stride %llu, stride %llu bytes)", fn, name, unit,
+                                 (unsigned long long)e, (unsigned long long)s);
+  }
+  return MP_OK;
+}
+
+// The checks of mp_run's `out` that need no other argument (include/mp_engine.h), before anything is enqueued: a pointer
+// that fails one never reaches a kernel. Its extents are appended to `ext` for check_extents.
+int check_device_outputs(mp_engine* E, const mp_device_outputs* o, const char* fn, std::vector<DeviceExtent>& ext) {
   const uint64_t B = E->B, P = E->T.P, n = E->T.n_scalar;
-  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_env, uint64_t align, u128 extra) -> int {
-    if (!p) return MP_OK;
-    if ((uintptr_t)p % align || stride % align)
-      return fail(MP_E_INVALID, "%s: %s pointer or env stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
-    if (stride < per_env)
-      return fail(MP_E_INVALID, "%s: %s env stride of %llu bytes is smaller than one env's %llu bytes", fn, name,
-                  (unsigned long long)stride, (unsigned long long)per_env);
-    if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s env stride of 2 GiB or more", fn, name);
-    outs.push_back({name, (uintptr_t)p, (u128)(B - 1) * stride + per_env + extra});
-    return MP_OK;
-  };
   if (o->rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
   if (o->world_rgb && !(E->flags & MP_FLAG_RENDER_WORLD)) return fail(MP_E_INVALID, "%s: world_rgb asked for, but the render flags switch WORLD.RGB off", fn);
   if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
   if (o->scalar_obs && o->scalar_obs_stride % 8) return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes", fn);
   int rc;
-  if ((rc = add("rgb", o->rgb, o->rgb_env_stride, P * E->R.player_bytes, 16, 0)) ||
-      (rc = add("world_rgb", o->world_rgb, o->world_rgb_env_stride, (uint64_t)E->R.world_bytes, 16, 0)) ||
-      (rc = add("reward", o->reward, o->reward_env_stride, P * 8, 8, 0)) ||
-      (rc = add("discount", o->discount, o->discount_env_stride, 8, 8, 0)) ||
-      (rc = add("step_type", o->step_type, o->step_type_env_stride, 8, 8, 0)) ||
-      (rc = add("scalar_obs", o->scalar_obs, o->scalar_obs_env_stride, P * 8, 8, (u128)(n - 1) * o->scalar_obs_stride)))
+  if ((rc = add_strided(ext, fn, "env", "rgb", o->rgb, o->rgb_env_stride, B, P * E->R.player_bytes, 16, 0)) ||
+      (rc = add_strided(ext, fn, "env", "world_rgb", o->world_rgb, o->world_rgb_env_stride, B, (uint64_t)E->R.world_bytes, 16, 0)) ||
+      (rc = add_strided(ext, fn, "env", "reward", o->reward, o->reward_env_stride, B, P * 8, 8, 0)) ||
+      (rc = add_strided(ext, fn, "env", "discount", o->discount, o->discount_env_stride, B, 8, 8, 0)) ||
+      (rc = add_strided(ext, fn, "env", "step_type", o->step_type, o->step_type_env_stride, B, 8, 8, 0)) ||
+      (rc = add_strided(ext, fn, "env", "scalar_obs", o->scalar_obs, o->scalar_obs_env_stride, B, P * 8, 8,
+                        (u128)(n - 1) * o->scalar_obs_stride)))
     return rc;
-  for (const DeviceExtent& x : outs)
-    if (x.extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, x.name);
-  if (o->scalar_obs) {
-    // The n x B rows of P doubles start at k * s + b * e. Rows of one k are e >= P * 8 apart; rows j = k' - k apart
-    // are |j * s + m * e| apart, m = b' - b in [-(B - 1), B - 1], closest at m = -floor(j * s / e) or one below.
-    const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_env_stride;
-    for (uint64_t j = 1; j < n; ++j) {
-      const u128 d = (u128)j * s, q = d / e, r = d % e;
-      const u128 gap = q > B - 1 ? d - (u128)(B - 1) * e : (q + 1 <= B - 1 ? std::min<u128>(r, e - r) : r);
-      if (gap < P * 8) return fail(MP_E_INVALID, "%s: scalar_obs rows overlap (env stride %llu, stride %llu bytes)", fn,
-                                   (unsigned long long)e, (unsigned long long)s);
-    }
-  }
-  return check_extents(E, outs, fn);
+  return o->scalar_obs ? check_scalar_rows(fn, "env", "scalar_obs", o->scalar_obs_stride, o->scalar_obs_env_stride, n, B, P * 8) : MP_OK;
 }
 }  // namespace
 
@@ -1820,25 +1822,20 @@ int mp_state_record_bytes(mp_handle h, uint64_t* bytes, uint8_t tag[16]) {
 }
 
 namespace {
-// The host checks of mp_state_store / mp_state_restore / mp_step_restore: the bank is 16-byte aligned, and the bank
-// and the index array lie in device allocations on the engine's device and overlap neither each other nor the
-// engine's buffers (nor the targets of mp_step_restore's `out`).
-// `more`: further extents of the call (mp_step_players' per-player targets), checked with the bank's.
-int check_bank(mp_engine* E, const void* bank, int n_slots, const int32_t* index, uint64_t index_count, uint64_t record_bytes, const char* fn,
-               const mp_device_outputs* out = nullptr, const std::vector<DeviceExtent>& more = {}) {
+// The host checks of mp_state_store / mp_state_restore / a restoring mp_run: the bank is 16-byte aligned and the index
+// array 4-byte aligned. Their extents go to the front of `ext`, for check_extents: in device allocations on the engine's
+// device, overlapping neither each other nor the engine's buffers nor the request's targets.
+int check_bank(const void* bank, int n_slots, const int32_t* index, uint64_t index_count, uint64_t record_bytes, const char* fn,
+               std::vector<DeviceExtent>& ext) {
   if ((uintptr_t)bank % 16) return fail(MP_E_INVALID, "%s: bank is not 16-byte aligned", fn);
   if ((uintptr_t)index % 4) return fail(MP_E_INVALID, "%s: index array is not 4-byte aligned", fn);
-  std::vector<DeviceExtent> ext{{"bank", (uintptr_t)bank, (u128)n_slots * record_bytes},
-                                {"index array", (uintptr_t)index, (u128)index_count * 4}};
-  ext.insert(ext.end(), more.begin(), more.end());
-  return out ? check_device_outputs(E, out, fn, std::move(ext)) : check_extents(E, ext, fn);
+  ext.insert(ext.begin(), {{"bank", (uintptr_t)bank, (u128)n_slots * record_bytes}, {"index array", (uintptr_t)index, (u128)index_count * 4}});
+  return MP_OK;
 }
 
-// The checks of mp_step_players / mp_reset_players' `players` that need no other argument (include/mp_engine.h); its
-// extents are appended to `ext` for the overlap and allocation checks that follow (check_bank / check_device_outputs /
-// check_extents). Extents are computed in 128 bits.
+// The checks of mp_run's `players` that need no other argument (include/mp_engine.h); its extents are appended to `ext`
+// for check_extents.
 int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_device_outputs* out, const char* fn, std::vector<DeviceExtent>& ext) {
-  if (!o) return fail(MP_E_INVALID, "%s: null players (use mp_step_into / mp_reset_into)", fn);
   if (o->n_rows < 1) return fail(MP_E_INVALID, "%s: n_rows %d < 1", fn, o->n_rows);
   if (!o->row_of_player || (uintptr_t)o->row_of_player % 4) return fail(MP_E_INVALID, "%s: row_of_player is null or not 4-byte aligned", fn);
   if (E->g_world > 0 && E->S.g_world > 0)
@@ -1858,42 +1855,21 @@ int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_devi
     ext.push_back({"world_row_of_env", (uintptr_t)o->world_row_of_env, (u128)E->B * 4});
   }
   ext.push_back({"row_of_player", (uintptr_t)o->row_of_player, (u128)E->B * E->T.P * 4});
-  auto add = [&](const char* name, const void* p, uint64_t stride, uint64_t per_row, uint64_t align, u128 extra, uint64_t rows) -> int {
-    if (!p) return MP_OK;
-    if ((uintptr_t)p % align || stride % align)
-      return fail(MP_E_INVALID, "%s: %s pointer or row stride is not a multiple of %llu bytes", fn, name, (unsigned long long)align);
-    if (stride < per_row)
-      return fail(MP_E_INVALID, "%s: %s row stride of %llu bytes is smaller than one row's %llu bytes", fn, name,
-                  (unsigned long long)stride, (unsigned long long)per_row);
-    if (align == 8 && stride >= (1ull << 31)) return fail(MP_E_INVALID, "%s: %s row stride of 2 GiB or more", fn, name);
-    const u128 extent = (u128)(rows - 1) * stride + per_row + extra;
-    if (extent >= ((u128)1 << 48)) return fail(MP_E_INVALID, "%s: %s spans more than 2^48 bytes", fn, name);
-    ext.push_back({name, (uintptr_t)p, extent});
-    return MP_OK;
-  };
   int rc;
-  if ((rc = add("players rgb", o->rgb, o->rgb_row_stride, (uint64_t)E->R.player_bytes, 16, 0, R)) ||
-      (rc = add("players reward", o->reward, o->reward_row_stride, 8, 8, 0, R)) ||
-      (rc = add("players scalar_obs", o->scalar_obs, o->scalar_obs_row_stride, 8, 8, (u128)(n - 1) * o->scalar_obs_stride, R)) ||
-      (rc = add("players world_rgb", o->world_rgb, o->world_rgb_row_stride, (uint64_t)E->R.world_bytes, 16, 0, (uint64_t)o->world_n_rows)))
+  if ((rc = add_strided(ext, fn, "row", "players rgb", o->rgb, o->rgb_row_stride, R, (uint64_t)E->R.player_bytes, 16, 0)) ||
+      (rc = add_strided(ext, fn, "row", "players reward", o->reward, o->reward_row_stride, R, 8, 8, 0)) ||
+      (rc = add_strided(ext, fn, "row", "players scalar_obs", o->scalar_obs, o->scalar_obs_row_stride, R, 8, 8,
+                        (u128)(n - 1) * o->scalar_obs_stride)) ||
+      (rc = add_strided(ext, fn, "row", "players world_rgb", o->world_rgb, o->world_rgb_row_stride, (uint64_t)o->world_n_rows,
+                        (uint64_t)E->R.world_bytes, 16, 0)))
     return rc;
-  if (o->scalar_obs) {  // n x n_rows rows of one double at k * s + r * e (the overlap rule of check_device_outputs)
-    const uint64_t s = o->scalar_obs_stride, e = o->scalar_obs_row_stride;
-    for (uint64_t j = 1; j < n; ++j) {
-      const u128 d = (u128)j * s, q = d / e, r = d % e;
-      const u128 gap = q > R - 1 ? d - (u128)(R - 1) * e : (q + 1 <= R - 1 ? std::min<u128>(r, e - r) : r);
-      if (gap < 8) return fail(MP_E_INVALID, "%s: players scalar_obs rows overlap (row stride %llu, stride %llu bytes)", fn,
-                               (unsigned long long)e, (unsigned long long)s);
-    }
-  }
-  return MP_OK;
+  return o->scalar_obs ? check_scalar_rows(fn, "row", "players scalar_obs", o->scalar_obs_stride, o->scalar_obs_row_stride, n, R, 8) : MP_OK;
 }
 
-// The checks of mp_step_routed's `actions` that need no other argument (include/mp_engine.h); its extents are appended
+// The checks of mp_run's `player_actions` that need no other argument (include/mp_engine.h); its extents are appended
 // to `ext` like check_player_outputs'. The row map is left out when it is `players`' own row map (both are only read).
 int check_player_actions(mp_engine* E, const mp_player_actions* a, const mp_player_outputs* players, const char* fn,
                          std::vector<DeviceExtent>& ext) {
-  if (!a) return fail(MP_E_INVALID, "%s: null actions", fn);
   if (a->n_rows < 1) return fail(MP_E_INVALID, "%s: actions n_rows %d < 1", fn, a->n_rows);
   if (!a->row_of_player || (uintptr_t)a->row_of_player % 4) return fail(MP_E_INVALID, "%s: actions row_of_player is null or not 4-byte aligned", fn);
   if (!a->action || (uintptr_t)a->action % 4 || a->action_row_stride % 4 || a->action_row_stride >= (1ull << 31))
@@ -1906,13 +1882,16 @@ int check_player_actions(mp_engine* E, const mp_player_actions* a, const mp_play
   return MP_OK;
 }
 
-// The checks of mp_step_drawn / mp_reset_drawn's `draw` (include/mp_engine.h). Its row map is `players`' own, whose
-// extent check_player_outputs appends (check_call requires `players` for these calls).
-int check_route_draw(mp_engine* E, const mp_route_draw* d, const mp_player_outputs* players, const char* fn) {
-  if (!d) return fail(MP_E_INVALID, "%s: null draw", fn);
+// The checks of mp_run's `draw` (include/mp_engine.h). Its row map is `players`' own, whose extent check_player_outputs
+// appends (check_call requires `players` with a draw).
+int check_route_draw(mp_engine* E, const mp_request& r, const char* fn) {
+  const mp_route_draw* d = r.draw;
   if (d->n_rows < 1) return fail(MP_E_INVALID, "%s: draw n_rows %d < 1", fn, d->n_rows);
-  if (players && (players->row_of_player != d->row_of_player || players->n_rows != d->n_rows))
+  if (r.players->row_of_player != d->row_of_player || r.players->n_rows != d->n_rows)
     return fail(MP_E_INVALID, "%s: players must deliver through the draw's row map and n_rows", fn);
+  const mp_player_actions* a = r.player_actions;
+  if (!r.reset && (!a || a->row_of_player != d->row_of_player || a->n_rows != d->n_rows))
+    return fail(MP_E_INVALID, "%s: a drawn step must read player_actions through the draw's row map and n_rows", fn);
   for (int p = 0; p < E->T.P; ++p) {
     const int n = d->n_choices[p];
     if (n < 0 || n > MP_MAX_ROUTE_CHOICES)
@@ -1927,76 +1906,35 @@ int check_route_draw(mp_engine* E, const mp_route_draw* d, const mp_player_outpu
   return MP_OK;
 }
 
-// The restore of a call that may restore envs from a state bank (mp_state_restore, mp_step_restore, mp_step_players,
-// mp_step_routed, mp_step_drawn): slot_of_env and bank, or neither; MP_RESTORE_REKEY or no flags.
-struct RestoreArgs { const int32_t* slot_of_env = nullptr; const void* bank = nullptr; int n_slots = 0; uint32_t flags = 0; };
-
-int check_restore(const RestoreArgs& r, const char* fn) {
-  const bool restoring = r.slot_of_env || r.bank;
-  if (restoring && (!r.slot_of_env || !r.bank)) return fail(MP_E_INVALID, "%s: slot_of_env and bank go together", fn);
-  if (restoring && r.n_slots < 1) return fail(MP_E_INVALID, "%s: n_slots %d < 1", fn, r.n_slots);
-  if (r.flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "%s: unknown flags 0x%x", fn, r.flags & ~MP_RESTORE_REKEY);
-  if (r.flags && !restoring) return fail(MP_E_INVALID, "%s: flags without a bank", fn);
+// The restore of mp_state_restore or a restoring mp_run: slot_of_env and bank, or neither; MP_RESTORE_REKEY or no flags.
+int check_restore(const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, const char* fn) {
+  const bool restoring = slot_of_env || bank;
+  if (restoring && (!slot_of_env || !bank)) return fail(MP_E_INVALID, "%s: slot_of_env and bank go together", fn);
+  if (restoring && n_slots < 1) return fail(MP_E_INVALID, "%s: n_slots %d < 1", fn, n_slots);
+  if (flags & ~MP_RESTORE_REKEY) return fail(MP_E_INVALID, "%s: unknown flags 0x%x", fn, flags & ~MP_RESTORE_REKEY);
+  if (flags && !restoring) return fail(MP_E_INVALID, "%s: flags without a bank", fn);
   return MP_OK;
 }
 
-// One state-transition call of the step and reset entry points that compose targets, restores and row actions.
-struct StateCall {
-  const char* fn;  // the entry point, for messages
-  int mode;        // k_step's: 0 step, 1 reset
-  const uint8_t* mask = nullptr;            // reset: the envs to reset, or null for all
-  const int32_t* actions = nullptr;         // step: dense actions [B][P]
-  bool routed = false;                      // step: actions from `rows` instead (mp_step_routed, mp_step_drawn)
-  const mp_player_actions* rows = nullptr;
-  const mp_route_draw* draw = nullptr;      // drawn routes (mp_step_drawn, mp_reset_drawn): the rows' map is written
-  RestoreArgs restore;
-  const mp_device_outputs* out = nullptr;   // targets (check_device_outputs)
-  bool needs_out = false;                   // refuse a null `out`
-  const mp_player_outputs* players = nullptr;  // per-player rows (check_player_outputs)
-  bool needs_players = false;               // refuse null `players`
-  bool render_follows = true;               // launch_state's; false launches k_exchange_push as mp_step does
-};
-
-// Every check of `c`, in the order the entry points document: restore, drawn routes, row actions, player rows, then the
-// bank, targets and extents together. A call with nothing to check does no check work.
-int check_call(mp_engine* E, const StateCall& c) {
-  int rc = check_restore(c.restore, c.fn);
+// Every check of `r`, in the order include/mp_engine.h lists them: the request's shape, the restore, drawn routes, row
+// actions, player rows, the bank and the targets, then every extent together. A plain request does no check work.
+int check_call(mp_engine* E, const mp_request& r) {
+  const char* fn = "mp_run";
+  if (r.reset && (r.actions || r.player_actions || r.slot_of_env || r.bank || r.restore_flags))
+    return fail(MP_E_INVALID, "%s: a reset takes no actions, player_actions, slot_of_env, bank or restore_flags", fn);
+  if (!r.reset && r.env_mask) return fail(MP_E_INVALID, "%s: env_mask is for a reset, not a step", fn);
+  if (!r.reset && r.actions && r.player_actions) return fail(MP_E_INVALID, "%s: a step takes actions or player_actions, not both", fn);
+  if (!r.reset && !r.actions && !r.player_actions) return fail(MP_E_INVALID, "%s: a step needs actions or player_actions, and has neither", fn);
+  if (r.draw && !r.players) return fail(MP_E_INVALID, "%s: draw needs players", fn);
+  int rc = check_restore(r.slot_of_env, r.bank, r.n_slots, r.restore_flags, fn);
   std::vector<DeviceExtent> ext;
-  if (!rc && c.draw) rc = check_route_draw(E, c.draw, c.players, c.fn);
-  if (!rc && c.routed) rc = check_player_actions(E, c.rows, c.players, c.fn, ext);
-  if (!rc && (c.players || c.needs_players)) rc = check_player_outputs(E, c.players, c.out, c.fn, ext);
+  if (!rc && r.draw) rc = check_route_draw(E, r, fn);
+  if (!rc && r.player_actions) rc = check_player_actions(E, r.player_actions, r.players, fn, ext);
+  if (!rc && r.players) rc = check_player_outputs(E, r.players, r.out, fn, ext);
+  if (!rc && r.bank) rc = check_bank(r.bank, r.n_slots, r.slot_of_env, (uint64_t)E->B, E->record.record_bytes, fn, ext);
+  if (!rc && r.out) rc = check_device_outputs(E, r.out, fn, ext);
   if (rc) return rc;
-  const RestoreArgs& r = c.restore;
-  if (r.bank) return check_bank(E, r.bank, r.n_slots, r.slot_of_env, (uint64_t)E->B, E->record.record_bytes, c.fn, c.out, ext);
-  if (c.out || c.needs_out) return check_device_outputs(E, c.out, c.fn, std::move(ext));
-  return ext.empty() ? MP_OK : check_extents(E, ext, c.fn);
-}
-
-// Checks `c` and, when every check passes, launches it: the state transition, then the render. A refused call enqueues
-// nothing.
-int run_call(mp_engine* E, const StateCall& c, void* stream) {
-  DeviceGuard guard(E->device);
-  int rc = check_call(E, c);
-  if (rc) return rc;
-  const RestoreArgs& r = c.restore;
-  const StepRestore restore{E->d_record_layout, r.slot_of_env, static_cast<const uint8_t*>(r.bank), r.n_slots,
-                            (r.flags & MP_RESTORE_REKEY) ? 1 : 0, E->key_base};
-  RowActions rows{};
-  if (c.routed) rows = {c.rows->row_of_player, reinterpret_cast<const uint8_t*>(c.rows->action), c.rows->action_row_stride, c.rows->n_rows};
-  DrawnActions drawn{};
-  if (c.draw) {
-    const mp_route_draw& d = *c.draw;
-    drawn.row_of_player = d.row_of_player; drawn.action = reinterpret_cast<const uint8_t*>(rows.action); drawn.stride = rows.stride;
-    drawn.n_rows = d.n_rows;
-    memcpy(drawn.n_choices, d.n_choices, sizeof drawn.n_choices);
-    memcpy(drawn.base, d.row_base, sizeof drawn.base);
-    memcpy(drawn.per_env, d.rows_per_env, sizeof drawn.per_env);
-  }
-  const cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = launch_state(E, c.actions, c.mask, c.mode, st, c.render_follows, r.bank ? &restore : nullptr, c.routed ? &rows : nullptr,
-                         c.draw ? &drawn : nullptr)))
-    return rc;
-  return launch_render(E, st, c.out, c.players);
+  return ext.empty() ? MP_OK : check_extents(E, ext, fn);
 }
 }  // namespace
 
@@ -2004,7 +1942,9 @@ int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* b
   if (!h || !env_of_slot || !bank) return fail(MP_E_INVALID, "mp_state_store: null argument");
   if (n_slots < 1) return fail(MP_E_INVALID, "mp_state_store: n_slots %d < 1", n_slots);
   DeviceGuard guard(h->device);
-  int rc = check_bank(h, bank, n_slots, env_of_slot, (uint64_t)n_slots, h->record.record_bytes, "mp_state_store");
+  std::vector<DeviceExtent> ext;
+  int rc = check_bank(bank, n_slots, env_of_slot, (uint64_t)n_slots, h->record.record_bytes, "mp_state_store", ext);
+  if (!rc) rc = check_extents(h, ext, "mp_state_store");
   if (rc) return rc;
   k_state_store<<<(n_slots + 7) / 8, 256, 0, (cudaStream_t)stream>>>(h->record, env_of_slot, n_slots, h->B, static_cast<uint8_t*>(bank));
   ++h->launches;
@@ -2014,11 +1954,13 @@ int mp_state_store(mp_handle h, const int32_t* env_of_slot, int n_slots, void* b
 
 int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags, void* stream) {
   if (!h || !slot_of_env || !bank) return fail(MP_E_INVALID, "mp_state_restore: null argument");
-  if (int rc = check_restore({slot_of_env, bank, n_slots, flags}, "mp_state_restore")) return rc;
+  if (int rc = check_restore(slot_of_env, bank, n_slots, flags, "mp_state_restore")) return rc;
   if (h->S.x_world || h->d_g_flag_ptrs)
     return fail(MP_E_UNSUPPORTED, "mp_state_restore: not available once mp_exchange_connect / mp_gather_obs_connect has run");
   DeviceGuard guard(h->device);
-  int rc = check_bank(h, bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_state_restore");
+  std::vector<DeviceExtent> ext;
+  int rc = check_bank(bank, n_slots, slot_of_env, (uint64_t)h->B, h->record.record_bytes, "mp_state_restore", ext);
+  if (!rc) rc = check_extents(h, ext, "mp_state_restore");
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   k_state_restore<<<(h->B + 7) / 8, 256, 0, st>>>(h->record, slot_of_env, static_cast<const uint8_t*>(bank), n_slots, h->B,
@@ -2029,77 +1971,34 @@ int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, 
   return launch_render(h, st);
 }
 
-int mp_reset(mp_handle h, const uint8_t* env_mask, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "null handle");
-  StateCall c{"mp_reset", 1};
-  c.mask = env_mask;
-  return run_call(h, c, stream);
-}
-
-int mp_reset_into(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "null handle");
-  StateCall c{"mp_reset_into", 1};
-  c.mask = env_mask; c.out = out; c.needs_out = true;
-  return run_call(h, c, stream);
-}
-
-int mp_reset_players(mp_handle h, const uint8_t* env_mask, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "mp_reset_players: null handle");
-  StateCall c{"mp_reset_players", 1};
-  c.mask = env_mask; c.out = out; c.players = players; c.needs_players = true;
-  return run_call(h, c, stream);
-}
-
-int mp_step_into(mp_handle h, const int32_t* actions, const mp_device_outputs* out, void* stream) {
-  if (!h || !actions) return fail(MP_E_INVALID, "mp_step_into: null handle or actions");
-  StateCall c{"mp_step_into", 0};
-  c.actions = actions; c.out = out; c.needs_out = true;
-  return run_call(h, c, stream);
-}
-
-int mp_step_restore(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
-                    const mp_device_outputs* out, void* stream) {
-  if (!h || !actions || !slot_of_env || !bank) return fail(MP_E_INVALID, "mp_step_restore: null argument");
-  StateCall c{"mp_step_restore", 0};
-  c.actions = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out;
-  c.render_follows = out != nullptr;  // launched as mp_step (out == NULL) or mp_step_into
-  return run_call(h, c, stream);
-}
-
-int mp_step_players(mp_handle h, const int32_t* actions, const int32_t* slot_of_env, const void* bank, int n_slots, uint32_t flags,
-                    const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
-  if (!h || !actions) return fail(MP_E_INVALID, "mp_step_players: null handle or actions");
-  StateCall c{"mp_step_players", 0};
-  c.actions = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out; c.players = players; c.needs_players = true;
-  return run_call(h, c, stream);
-}
-
-int mp_step_routed(mp_handle h, const mp_player_actions* actions, const int32_t* slot_of_env, const void* bank, int n_slots,
-                   uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players, void* stream) {
-  if (!h) return fail(MP_E_INVALID, "mp_step_routed: null handle");
-  StateCall c{"mp_step_routed", 0};
-  c.routed = true; c.rows = actions; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out; c.players = players;
-  c.render_follows = out || players;  // launched as the composed call: mp_step, mp_step_into, mp_step_restore or mp_step_players
-  return run_call(h, c, stream);
-}
-
-int mp_step_drawn(mp_handle h, const mp_route_draw* draw, const int32_t* action, uint64_t action_row_stride, const int32_t* slot_of_env,
-                  const void* bank, int n_slots, uint32_t flags, const mp_device_outputs* out, const mp_player_outputs* players,
-                  void* stream) {
-  if (!h || !draw) return fail(MP_E_INVALID, "mp_step_drawn: null handle or draw");
-  const mp_player_actions rows{draw->row_of_player, draw->n_rows, action, action_row_stride};
-  StateCall c{"mp_step_drawn", 0};
-  c.routed = true; c.rows = &rows; c.draw = draw; c.restore = {slot_of_env, bank, n_slots, flags}; c.out = out;
-  c.players = players; c.needs_players = true;
-  return run_call(h, c, stream);
-}
-
-int mp_reset_drawn(mp_handle h, const uint8_t* env_mask, const mp_route_draw* draw, const mp_device_outputs* out,
-                   const mp_player_outputs* players, void* stream) {
-  if (!h || !draw) return fail(MP_E_INVALID, "mp_reset_drawn: null handle or draw");
-  StateCall c{"mp_reset_drawn", 1};
-  c.mask = env_mask; c.draw = draw; c.out = out; c.players = players; c.needs_players = true;
-  return run_call(h, c, stream);
+// Checks `r` and, when every check passes, launches it: the state transition, then the render. A refused request
+// enqueues nothing. A step with neither targets nor player rows publishes its step to the exchange from a
+// k_exchange_push of its own, as mp_step_state does.
+int mp_run(mp_handle h, const mp_request* r, void* stream) {
+  if (!h || !r) return fail(MP_E_INVALID, "mp_run: null handle or request");
+  DeviceGuard guard(h->device);
+  int rc = check_call(h, *r);
+  if (rc) return rc;
+  const StepRestore restore{h->d_record_layout, r->slot_of_env, static_cast<const uint8_t*>(r->bank), r->n_slots,
+                            (r->restore_flags & MP_RESTORE_REKEY) ? 1 : 0, h->key_base};
+  const mp_player_actions* a = r->player_actions;
+  RowActions rows{};
+  if (a) rows = {a->row_of_player, reinterpret_cast<const uint8_t*>(a->action), a->action_row_stride, a->n_rows};
+  DrawnActions drawn{};
+  if (r->draw) {
+    const mp_route_draw& d = *r->draw;
+    drawn.row_of_player = d.row_of_player; drawn.action = rows.action; drawn.stride = rows.stride;
+    drawn.n_rows = d.n_rows;
+    memcpy(drawn.n_choices, d.n_choices, sizeof drawn.n_choices);
+    memcpy(drawn.base, d.row_base, sizeof drawn.base);
+    memcpy(drawn.per_env, d.rows_per_env, sizeof drawn.per_env);
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  const bool render_follows = r->reset || r->out || r->players;
+  if ((rc = launch_state(h, r->actions, r->env_mask, r->reset ? 1 : 0, st, render_follows, r->bank ? &restore : nullptr,
+                         a ? &rows : nullptr, r->draw ? &drawn : nullptr)))
+    return rc;
+  return launch_render(h, st, r->out, r->players);
 }
 
 int mp_launch_count(mp_handle h, uint64_t* out) {

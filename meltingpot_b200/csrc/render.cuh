@@ -246,7 +246,7 @@ struct ViewerInfo {  // per player, refreshed once per env
 // MODE (exclusive):
 //   RENDER_GATHER: also deliver every strip into every rank's stacked observation buffer (State::g_*);
 //   RENDER_ROUTED: deliver player p of env b to the row State::pr.row_of_player[b][p] of the caller's per-player
-//     targets (mp_step_players). The team's first warp reads the env's row map with its avatars and compacts the
+//     targets (mp_run's players). The team's first warp reads the env's row map with its avatars and compacts the
 //     routed players into s_players; the env's item loop then runs over those players' strips and WORLD.RGB's only,
 //     so an unrouted player is neither composited nor stored. With State::pr.world_rgb set, the same warp also reads
 //     the env's WORLD.RGB row (State::pr.world_row_of_env[b]): an env with a row stores its WORLD.RGB strips there,

@@ -93,7 +93,7 @@ __global__ void __launch_bounds__(256) k_state_restore(const __grid_constant__ R
   restore_env(R, slot_of_env, bank, n_slots, b, lane, rekey, key_base);
 }
 
-// The restore a step carries out in place of advancing the envs it names (mp_step_restore, k_step<..., true>): the
+// The restore a step carries out in place of advancing the envs it names (a restoring mp_run, k_step<..., true>): the
 // engine's record layout (a device copy made at mp_create, so the step's parameter space grows by one pointer, not a
 // whole RecordLayout) and the call's index array, bank and rekey flag.
 struct StepRestore {

@@ -102,7 +102,7 @@ __device__ __forceinline__ int env_variant(const ParamVariants<Params>& V, int b
 }
 
 // Where a step's actions come from. DenseActions: an id per player, [B][P] (null on territory's frame 0: every avatar
-// does nothing). RowActions (mp_step_routed): player p of env b takes the id in row row_of_player[b][p] of `action`,
+// does nothing). RowActions (player_actions): player p of env b takes the id in row row_of_player[b][p] of `action`,
 // rows `stride` bytes apart, or action 0 when that row lies outside [0, n_rows). The row is read on the avatar's lane
 // where the action is decoded (load_avatar), so nothing of it stays live across the frame.
 using DenseActions = const int32_t* __restrict__;
@@ -119,12 +119,12 @@ __device__ __forceinline__ const Actions& select_actions(const DenseActions& den
   else return dense;
 }
 
-// Drawn routes (mp_step_drawn / mp_reset_drawn, k_step_drawn): each episode, player slot p of env b plays choice
+// Drawn routes (mp_run's draw, k_step_drawn): each episode, player slot p of env b plays choice
 // o = pick(philox(0, episode, p, RS_ROUTE).x, n_choices[p]) under env b's key (uniform with replacement per slot and
 // episode, like choice_present), and its row is base[p][o] + b * per_env[p][o]; a slot without choices has no row. The
 // step reads player p's action from the row of the episode it is in, and writes every env's row map after the advance
 // (row_of_player[b][p]: the row of the episode env b is in now, -1 for no row), which the render that follows reads.
-// mp_step_drawn checks every row of the table against [0, n_rows) for every env, so a drawn row is always in range.
+// mp_run checks every row of the table against [0, n_rows) for every env, so a drawn row is always in range.
 #define MP_ROUTE_CHOICES 8  // = MP_MAX_ROUTE_CHOICES (include/mp_engine.h)
 struct DrawnActions {
   int32_t* row_of_player;  // [B][P], written
@@ -160,11 +160,11 @@ struct HasResetMap<F, std::void_t<decltype(&F::reset_map)>> : std::true_type {};
 // coop_mining's ore_sprite[state]) to the stack, and passed on as it is, it keeps its constant-bank reads. Variants are
 // read through the L1 from the device array.
 //
-// kRestore (mp_step_restore, mode 0 only): the warp of an env that `restore` names (restore_env's predicate, read after
+// kRestore (a restoring mp_run, mode 0 only): the warp of an env that `restore` names (restore_env's predicate, read after
 // the dependency wait) copies that record instead of advancing, which also takes precedence over the auto-reset after
 // LAST; the record carries the timestep and the events, so event_begin / event_end are skipped too. Every other warp
 // runs the plain step. With kRestore = false, `restore` is never read and the kernel is the plain step.
-// Actions: DenseActions (`actions`; `rows` is never read), or RowActions (`rows`; launched by mp_step_routed only, mode 0,
+// Actions: DenseActions (`actions`; `rows` is never read), or RowActions (`rows`; launched by mp_run's player_actions only, mode 0,
 // and `actions` is never read); k_step_drawn reads DrawnActions.
 //
 // k_step's body as a function, for k_step_drawn: stages the family's tables, waits for the kernel before, then restores
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(128, 8) k_step(Tables T, const __grid_constant
   }
 }
 
-// k_step with drawn routes (mp_step_drawn, mode 0, and mp_reset_drawn, mode 1): the same advance, with actions from
+// k_step with drawn routes (mp_run's draw: a step, mode 0, or a reset, mode 1): the same advance, with actions from
 // the rows of DrawnActions; then every env's row map is written from the episode and key the env now has, whether it
 // advanced, started an episode, was restored (a record's key, or its own with rekey) or was masked out of a reset.
 // `actions` and `rows` are those of k_step, so one argument list launches either kernel; neither is read here.

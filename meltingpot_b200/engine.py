@@ -53,15 +53,13 @@ def render_layout_candidates():
   return [(t, w, l) for t in range(t0, t1 + 1) for w in range(w0, w1 + 1) for l in range(l0, l1 + 1) if t * w <= 32]
 
 EXPORTED_SYMBOLS = (
-    'mp_create', 'mp_destroy', 'mp_set_flags', 'mp_reset', 'mp_step',
-    'mp_step_state', 'mp_render', 'mp_get_buffers', 'mp_step_host',
+    'mp_create', 'mp_destroy', 'mp_set_flags', 'mp_run', 'mp_step_state', 'mp_render', 'mp_get_buffers', 'mp_step_host',
     'mp_reset_host', 'mp_launch_count', 'mp_algorithmic_bytes', 'mp_debug_render_tables', 'mp_debug_render_plan', 'mp_state_size', 'mp_state_save', 'mp_state_load',
     'mp_step_host_async', 'mp_wait', 'mp_exchange_create', 'mp_ipc_export', 'mp_ipc_open', 'mp_enable_peer_access',
     'mp_exchange_connect', 'mp_exchange_wait', 'mp_exchange_slot', 'mp_debug_lane_map', 'mp_debug_observations',
     'mp_gather_obs_create', 'mp_gather_obs_connect', 'mp_gather_obs_enable', 'mp_gather_obs_wait', 'mp_gather_obs_slot',
-    'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_step_into', 'mp_reset_into', 'mp_last_error',
-    'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_step_restore',
-    'mp_step_players', 'mp_reset_players', 'mp_step_routed', 'mp_step_drawn', 'mp_reset_drawn', 'mp_debug_last_launch',
+    'mp_create_variants', 'mp_set_env_variants', 'mp_env_variants', 'mp_last_error',
+    'mp_version', 'mp_state_record_bytes', 'mp_state_store', 'mp_state_restore', 'mp_debug_last_launch',
 )
 
 MP_RESTORE_REKEY = 1
@@ -107,8 +105,24 @@ class MpDeviceOutputs(ctypes.Structure):
   ]
 
 
-# The outputs a step can deliver into caller-owned tensors (mp_step_into), each with the axis that indexes envs.
+# The outputs a step can deliver into caller-owned tensors (mp_request.out).
 DEVICE_OUTPUTS = ('rgb', 'world_rgb', 'reward', 'discount', 'step_type', 'scalar_obs')
+
+
+def _strides(label: str, t, lead: int, unit: str, item: int) -> Tuple[int, ...]:
+  """The byte strides of the first `lead` axes of `t` (a TensorLayout), which must be dense in every other axis. An
+  axis of length 1 gets the stride it would have if dense (its stride is never used)."""
+  dense = 1
+  for axis in range(len(t.shape) - 1, lead - 1, -1):
+    if t.shape[axis] != 1 and t.stride[axis] != dense:
+      raise ValueError(f'{label}: axis {axis} has stride {t.stride[axis]}, must be {dense} (only the {unit} axis'
+                       f'{" and the observation axis" if lead > 1 else ""} may be strided)')
+    dense *= t.shape[axis]
+  strides = []
+  for axis in range(lead - 1, -1, -1):
+    strides.insert(0, (t.stride[axis] if t.shape[axis] > 1 else dense) * item)
+    dense *= t.shape[axis]
+  return tuple(strides)
 
 
 class MpPlayerOutputs(ctypes.Structure):
@@ -122,7 +136,7 @@ class MpPlayerOutputs(ctypes.Structure):
   ]
 
 
-# The per-player outputs a step can deliver into rows of caller-owned tensors (mp_step_players).
+# The per-player outputs a step can deliver into rows of caller-owned tensors (mp_request.players).
 PLAYER_OUTPUTS = ('rgb', 'reward', 'scalar_obs')
 # WORLD.RGB routed per env in the same call: the row map and the rows, given together.
 WORLD_OUTPUTS = ('world_row_of_env', 'world_rgb')
@@ -179,18 +193,11 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
       n_rows = rows
     elif rows != n_rows:
       raise ValueError(f'players[{name!r}]: {rows} rows, another target has {n_rows}')
-    dense = 1
-    for axis in range(len(t.shape) - 1, row_axis, -1):
-      if t.shape[axis] != 1 and t.stride[axis] != dense:
-        raise ValueError(f'players[{name!r}]: axis {axis} has stride {t.stride[axis]}, must be {dense} (only the row axis'
-                         f'{" and the observation axis" if row_axis else ""} may be strided)')
-      dense *= t.shape[axis]
-    item = torch.empty((), dtype=dtype).element_size()
-    row_stride = (t.stride[row_axis] if rows > 1 else dense) * item  # with one row the stride is never used
+    strides = _strides(f'players[{name!r}]', t, row_axis + 1, 'row', torch.empty((), dtype=dtype).element_size())
     setattr(s, name, ctypes.c_void_p(int(t.data_ptr)))
-    setattr(s, f'{name}_row_stride', row_stride)
+    setattr(s, f'{name}_row_stride', strides[-1])
     if name == 'scalar_obs':
-      s.scalar_obs_stride = (t.stride[0] if t.shape[0] > 1 else rows * dense) * item
+      s.scalar_obs_stride = strides[0]
   s.n_rows = n_rows
   wmap, world = players.get('world_row_of_env'), players.get('world_rgb')
   if (wmap is None) != (world is None):
@@ -210,13 +217,7 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
     rows = int(world.shape[0])
     if rows < 1:
       raise ValueError('players[\'world_rgb\']: no rows')
-    dense = 1
-    for axis in range(len(world.shape) - 1, 0, -1):
-      if world.shape[axis] != 1 and world.stride[axis] != dense:
-        raise ValueError(f'players[\'world_rgb\']: axis {axis} has stride {world.stride[axis]}, must be {dense} (only the row '
-                         'axis may be strided)')
-      dense *= world.shape[axis]
-    row_stride = world.stride[0] if rows > 1 else dense  # with one row the stride is never used
+    (row_stride,) = _strides('players[\'world_rgb\']', world, 1, 'row', 1)
     if world.data_ptr % 16 or row_stride % 16:
       raise ValueError('players[\'world_rgb\']: the pointer and the row stride must be multiples of 16 bytes')
     s.world_row_of_env = ctypes.c_void_p(int(wmap.data_ptr))
@@ -257,6 +258,15 @@ def describe_draw(row_of_player, n_rows: int, row_base, rows_per_env) -> MpRoute
     for j, (r, n) in enumerate(zip(bases, per_env)):
       d.row_base[p][j], d.rows_per_env[p][j] = int(r), int(n)
   return d
+
+
+class MpRequest(ctypes.Structure):
+  _fields_ = [
+      ('reset', ctypes.c_int32), ('env_mask', ctypes.c_void_p), ('actions', ctypes.c_void_p),
+      ('player_actions', ctypes.POINTER(MpPlayerActions)), ('draw', ctypes.POINTER(MpRouteDraw)),
+      ('slot_of_env', ctypes.c_void_p), ('bank', ctypes.c_void_p), ('n_slots', ctypes.c_int32), ('restore_flags', ctypes.c_uint32),
+      ('out', ctypes.POINTER(MpDeviceOutputs)), ('players', ctypes.POINTER(MpPlayerOutputs)),
+  ]
 
 
 def describe_player_actions(player_actions: Mapping[str, Any], num_envs: int, num_players: int, device: int) -> MpPlayerActions:
@@ -321,20 +331,11 @@ def describe_outputs(out: Mapping[str, TensorLayout], views: Mapping[str, Tuple[
     dev = torch.device(t.device)
     if dev.type != 'cuda' or dev.index != device:
       raise ValueError(f'out[{name!r}]: on {dev}, the engine runs on cuda:{device}')
-    env_axis = 1 if name == 'scalar_obs' else 0
-    dense = 1
-    for axis in range(len(shape) - 1, env_axis, -1):
-      if shape[axis] != 1 and t.stride[axis] != dense:
-        raise ValueError(f'out[{name!r}]: axis {axis} has stride {t.stride[axis]}, must be {dense} '
-                         f'(only the env axis{" and the observation axis" if env_axis else ""} may be strided)')
-      dense *= shape[axis]
-    item = torch.empty((), dtype=dtype).element_size()
-    # with one env (one observation) the stride is never used: pass the dense one
-    env_stride = (t.stride[env_axis] if shape[env_axis] > 1 else dense) * item
+    strides = _strides(f'out[{name!r}]', t, 2 if name == 'scalar_obs' else 1, 'env', torch.empty((), dtype=dtype).element_size())
     setattr(s, name, ctypes.c_void_p(int(t.data_ptr)))
-    setattr(s, f'{name}_env_stride', env_stride)
+    setattr(s, f'{name}_env_stride', strides[-1])
     if name == 'scalar_obs':
-      s.scalar_obs_stride = (t.stride[0] if shape[0] > 1 else shape[1] * dense) * item
+      s.scalar_obs_stride = strides[0]
   return s
 
 
@@ -362,10 +363,7 @@ def load_library() -> ctypes.CDLL:
   lib.mp_env_variants.argtypes = [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(vp), ctypes.POINTER(vp)]
   lib.mp_destroy.argtypes = [vp]
   lib.mp_set_flags.argtypes = [vp, ctypes.c_uint32]
-  lib.mp_reset.argtypes = [vp, vp, vp]
-  lib.mp_step.argtypes = [vp, vp, vp]
-  lib.mp_step_into.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), vp]
-  lib.mp_reset_into.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), vp]
+  lib.mp_run.argtypes = [vp, ctypes.POINTER(MpRequest), vp]
   lib.mp_step_state.argtypes = [vp, vp, vp]
   lib.mp_render.argtypes = [vp, vp]
   lib.mp_get_buffers.argtypes = [vp, ctypes.POINTER(MpBuffers)]
@@ -380,16 +378,6 @@ def load_library() -> ctypes.CDLL:
   lib.mp_state_record_bytes.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), vp]
   lib.mp_state_store.argtypes = [vp, vp, ctypes.c_int, vp, vp]
   lib.mp_state_restore.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_uint32, vp]
-  lib.mp_step_restore.argtypes = [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(MpDeviceOutputs), vp]
-  lib.mp_step_players.argtypes = [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(MpDeviceOutputs),
-                                  ctypes.POINTER(MpPlayerOutputs), vp]
-  lib.mp_reset_players.argtypes = [vp, vp, ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
-  lib.mp_step_routed.argtypes = [vp, ctypes.POINTER(MpPlayerActions), vp, vp, ctypes.c_int, ctypes.c_uint32,
-                                 ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
-  lib.mp_step_drawn.argtypes = [vp, ctypes.POINTER(MpRouteDraw), vp, ctypes.c_uint64, vp, vp, ctypes.c_int, ctypes.c_uint32,
-                                ctypes.POINTER(MpDeviceOutputs), ctypes.POINTER(MpPlayerOutputs), vp]
-  lib.mp_reset_drawn.argtypes = [vp, vp, ctypes.POINTER(MpRouteDraw), ctypes.POINTER(MpDeviceOutputs),
-                                 ctypes.POINTER(MpPlayerOutputs), vp]
   lib.mp_debug_render_plan.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_last_launch.argtypes = [vp, ctypes.POINTER(ctypes.c_int32)]
   lib.mp_debug_render_tables.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), vp, vp]
@@ -585,35 +573,26 @@ class Engine:
 
   def reset(self, mask=None, stream=None, out=None, players=None, draw=None) -> None:
     """out, players, draw: as for step."""
-    ptr = None
+    r = MpRequest(reset=1)
     if mask is not None:
       assert mask.dtype == self._torch.uint8 and mask.is_cuda and mask.numel() == self.num_envs
-      ptr = ctypes.c_void_p(mask.data_ptr())
-    if draw is not None:
-      if players is None:
-        raise ValueError('draw needs players')
-      s = None if out is None else ctypes.byref(self._device_outputs(out))
-      _check(self._lib.mp_reset_drawn(self._h, ptr, ctypes.byref(draw), s, ctypes.byref(self._player_outputs(players)),
-                                      self._stream(stream)))
-    elif players is not None:
-      s = None if out is None else ctypes.byref(self._device_outputs(out))
-      _check(self._lib.mp_reset_players(self._h, ptr, s, ctypes.byref(self._player_outputs(players)), self._stream(stream)))
-    elif out is None:
-      _check(self._lib.mp_reset(self._h, ptr, self._stream(stream)))
-    else:
-      s = self._device_outputs(out)
-      _check(self._lib.mp_reset_into(self._h, ptr, ctypes.byref(s), self._stream(stream)))
+      r.env_mask = mask.data_ptr()
+    if draw is not None and players is None:
+      raise ValueError('draw needs players')
+    self._run(r, stream, out, players, draw)
 
   def step(self, actions, stream=None, out=None, restore=None, bank=None, rekey: bool = False, players=None,
            player_actions=None, draw=None) -> None:
     """actions: int32 CUDA tensor [B, P] of discrete action ids, or None with player_actions.
 
-    out: {name: CUDA tensor} for any of DEVICE_OUTPUTS (mp_step_into): the step's images are rendered straight into
+    One mp_run request (include/mp_engine.h, mp_request) carries the step and everything below.
+
+    out: {name: CUDA tensor} for any of DEVICE_OUTPUTS: the step's images are rendered straight into
     out['rgb'] / out['world_rgb'] instead of this engine's own image buffers, and its scalars are written into the
     others as well as into this engine's buffers. Shapes and dtypes are those of the engine's views (rgb, reward, ...);
     the env axis may have any stride (and the observation axis of scalar_obs), every other axis is dense.
 
-    restore, bank: restore envs within the step (mp_step_restore). restore is a contiguous CUDA int32 tensor [B] and
+    restore, bank: restore envs within the step. restore is a contiguous CUDA int32 tensor [B] and
     bank a state bank (see restore_states). Env b takes bank row restore[b] instead of stepping, ignoring its action,
     when that index is in 0..n_slots-1 and the row holds one of this engine's records; -1, any other out-of-range index
     and rows without this engine's tag step env b as usual. The result is that of a step followed by
@@ -621,7 +600,7 @@ class Engine:
     layout are checked, never their values, so the call never synchronises: build the index on the device, e.g.
     `torch.where(step_type == 2, row, -1)`. rekey: as for restore_states.
 
-    players: per-player rows (mp_step_players), {'row_of_player': contiguous CUDA int32 [B, P]} plus any of 'rgb'
+    players: per-player rows, {'row_of_player': contiguous CUDA int32 [B, P]} plus any of 'rgb'
     (uint8 [n_rows, h, w, 3]), 'reward' (float64 [n_rows]) and 'scalar_obs' (float64 [num_scalar_obs, n_rows]). Player p
     of env b is delivered to row row_of_player[b, p] when that lies in 0..n_rows-1, and nowhere otherwise; with 'rgb'
     the images are drawn straight into the rows, an unrouted player is not drawn at all and this engine's own rgb is
@@ -631,46 +610,43 @@ class Engine:
     is drawn into row world_row_of_env[b] when that lies in 0..n-1, and not at all otherwise, and this engine's own
     world_rgb is not written (out's world_rgb must then be absent).
 
-    player_actions: actions read from rows (mp_step_routed), {'row_of_player': contiguous CUDA int32 [B, P],
+    player_actions: actions read from rows, {'row_of_player': contiguous CUDA int32 [B, P],
     'action': CUDA int32 [n_rows], any stride}, with actions None. Player p of env b takes action[row_of_player[b, p]]
     when that row lies in 0..n_rows-1, and action 0 (NOOP) otherwise. The row map may be players' own. Combines with
     out, players and restore / bank; the result is that of the same call with the dense actions those rows give.
 
-    draw: drawn routes (mp_step_drawn; an MpRouteDraw from describe_draw), with players and player_actions whose
+    draw: drawn routes (an MpRouteDraw from describe_draw), with players and player_actions whose
     row_of_player is the draw's map: the step writes the map (each player's row for the episode its env is in
     afterwards) and reads each player's action from the row of the episode it is in before the step."""
     if draw is not None and (players is None or player_actions is None):
       raise ValueError('draw needs players and player_actions')
+    r = MpRequest()
     if player_actions is not None:
       if actions is not None:
         raise ValueError('give actions or player_actions, not both')
-      pa = describe_player_actions({k: (None if v is None else layout_of(v)) for k, v in player_actions.items()},
-                                   self.num_envs, self.num_players, self.device)
+      r.player_actions = ctypes.pointer(describe_player_actions(
+          {k: (None if v is None else layout_of(v)) for k, v in player_actions.items()}, self.num_envs, self.num_players,
+          self.device))
     elif actions is None:
       raise ValueError('actions is None: give actions, or player_actions')
     else:
       self._check_actions(actions)
-      a = ctypes.c_void_p(actions.data_ptr())
-    flags, idx, bank_ptr, n_slots = self._restore_args(restore, bank, rekey)
-    s = None if out is None else ctypes.byref(self._device_outputs(out))
-    p = None if players is None else ctypes.byref(self._player_outputs(players))
+      r.actions = actions.data_ptr()
+    r.restore_flags, r.slot_of_env, r.bank, r.n_slots = self._restore_args(restore, bank, rekey)
+    self._run(r, stream, out, players, draw)
+
+  def _run(self, r: MpRequest, stream, out, players, draw) -> None:
+    """Adds the targets and drawn routes to request `r` and runs it: one mp_run call."""
+    if out is not None:
+      r.out = ctypes.pointer(self._device_outputs(out))
+    if players is not None:
+      r.players = ctypes.pointer(self._player_outputs(players))
     if draw is not None:
-      _check(self._lib.mp_step_drawn(self._h, ctypes.byref(draw), pa.action, pa.action_row_stride, idx, bank_ptr, n_slots,
-                                     ctypes.c_uint32(flags), s, p, self._stream(stream)))
-    elif player_actions is not None:
-      _check(self._lib.mp_step_routed(self._h, ctypes.byref(pa), idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, p,
-                                      self._stream(stream)))
-    elif players is not None:
-      _check(self._lib.mp_step_players(self._h, a, idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, p, self._stream(stream)))
-    elif bank_ptr is not None:
-      _check(self._lib.mp_step_restore(self._h, a, idx, bank_ptr, n_slots, ctypes.c_uint32(flags), s, self._stream(stream)))
-    elif out is None:
-      _check(self._lib.mp_step(self._h, a, self._stream(stream)))
-    else:
-      _check(self._lib.mp_step_into(self._h, a, s, self._stream(stream)))
+      r.draw = ctypes.pointer(draw)
+    _check(self._lib.mp_run(self._h, ctypes.byref(r), self._stream(stream)))
 
   def _restore_args(self, restore, bank, rekey):
-    """flags, index pointer, bank pointer and slot count of restore / bank (None, None, 0 without them)."""
+    """flags, index pointer, bank pointer and slot count of restore / bank (0, None, None, 0 without them)."""
     if restore is None and bank is None:
       if rekey:
         raise ValueError('rekey needs restore and bank')
@@ -682,7 +658,7 @@ class Engine:
     for name, t in (('bank', bank), ('restore', idx)):
       if t.device.index != self.device:
         raise ValueError(f'{name} is on {t.device}, the engine runs on cuda:{self.device}')
-    return (MP_RESTORE_REKEY if rekey else 0), ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(bank.data_ptr()), int(bank.shape[0])
+    return (MP_RESTORE_REKEY if rekey else 0), idx.data_ptr(), bank.data_ptr(), int(bank.shape[0])
 
   def output_views(self):
     """name -> (shape, dtype) of the engine's own view of each output a step can deliver into caller tensors."""

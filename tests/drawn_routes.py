@@ -1,4 +1,4 @@
-"""The draw rule of drawn routes (mp_step_drawn / mp_reset_drawn), on the host, for the tests.
+"""The draw rule of drawn routes (mp_run's draw), on the host, for the tests.
 
 Player slot p of an env with Philox key `key` plays, in episode `episode`, choice
 pick(philox4x32_10(counter {0, episode, p, RS_ROUTE}, key {key low, key high}).x, n) of its n choices, where

@@ -3,6 +3,8 @@
 import ctypes
 import os
 import re
+import shutil
+import subprocess
 
 import numpy as np
 import pytest
@@ -84,6 +86,40 @@ def test_c_abi_exports_every_declared_symbol():
   for sym in declared:
     assert hasattr(lib, sym), sym
   assert b'sm_90a' in lib.mp_version()
+
+
+def test_c_abi_declares_mp_run():
+  with open(os.path.join(ROOT, 'include', 'mp_engine.h')) as f:
+    header = f.read()
+  decl = [p.strip() for p in re.search(r'\bint mp_run\(([^;]*)\);', header).group(1).split(',')]
+  assert decl == ['mp_handle h', 'const mp_request* r', 'void* stream']
+  lib = engine.load_library()
+  assert lib.mp_run.argtypes == [ctypes.c_void_p, ctypes.POINTER(engine.MpRequest), ctypes.c_void_p]
+  for name, value in re.findall(r'#define (MP_MAX_ROUTE_\w+) (\d+)', header):
+    assert getattr(engine, name) == int(value)
+
+
+# every struct the C ABI shares with the ctypes binding, by its C name
+ABI_STRUCTS = {'mp_buffers': engine.MpBuffers, 'mp_host_outputs': engine.MpHostOutputs,
+               'mp_device_outputs': engine.MpDeviceOutputs, 'mp_player_outputs': engine.MpPlayerOutputs,
+               'mp_player_actions': engine.MpPlayerActions, 'mp_route_draw': engine.MpRouteDraw,
+               'mp_request': engine.MpRequest}
+
+
+@pytest.mark.skipif(not (shutil.which('cc') or shutil.which('gcc')), reason='needs a C compiler')
+@pytest.mark.parametrize('c_name', sorted(ABI_STRUCTS))
+def test_abi_struct_matches_the_header(c_name, tmp_path):
+  cls = ABI_STRUCTS[c_name]
+  fields = [name for name, _ in cls._fields_]
+  src = tmp_path / 'layout.c'
+  src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "mp_engine.h"\nint main(void) {\n'
+                 f'  printf("%zu", sizeof({c_name}));\n'
+                 + ''.join(f'  printf(" %zu", offsetof({c_name}, {f}));\n' for f in fields) + '  return 0;\n}\n')
+  exe = tmp_path / 'layout'
+  subprocess.check_call([shutil.which('cc') or shutil.which('gcc'), '-I', os.path.join(ROOT, 'include'), str(src), '-o', str(exe)])
+  got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
+  assert got[0] == ctypes.sizeof(cls)
+  assert got[1:] == [getattr(cls, f).offset for f in fields]
 
 
 def _cuda_available():

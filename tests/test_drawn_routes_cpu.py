@@ -3,10 +3,6 @@ mp_route_draw struct and entry points against the header, and the draw rule (tes
 Philox: uniform, and a function of (key, episode, slot) only)."""
 
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,7 +15,6 @@ from meltingpot_b200 import substrate
 from oracle import binding as oracle
 from tests.drawn_routes import route_draw
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 B, P, H, W = 3, 5, 16, 24
 NAMES = ['READY_TO_SHOOT']
 
@@ -205,39 +200,11 @@ def test_draw_is_uniform(n):
 
 
 # -- C ABI ----------------------------------------------------------------------------------------------------------------
-def test_c_abi_declares_the_entry_points():
-  with open(os.path.join(ROOT, 'include', 'mp_engine.h')) as f:
-    header = f.read()
-  decl = lambda name: [p.strip() for p in re.search(rf'\bint {name}\(([^;]*)\);', header).group(1).split(',')]
-  assert decl('mp_step_drawn') == ['mp_handle h', 'const mp_route_draw* draw', 'const int32_t* action', 'uint64_t action_row_stride',
-                                   'const int32_t* slot_of_env', 'const void* bank', 'int n_slots', 'uint32_t flags',
-                                   'const mp_device_outputs* out', 'const mp_player_outputs* players', 'void* stream']
-  assert decl('mp_reset_drawn') == ['mp_handle h', 'const uint8_t* env_mask', 'const mp_route_draw* draw',
-                                    'const mp_device_outputs* out', 'const mp_player_outputs* players', 'void* stream']
-  assert 'mp_step_drawn' in engine.EXPORTED_SYMBOLS and 'mp_reset_drawn' in engine.EXPORTED_SYMBOLS
-  for name, value in re.findall(r'#define (MP_MAX_ROUTE_\w+) (\d+)', header):
-    assert getattr(engine, name) == int(value)
-
-
-@pytest.mark.skipif(not (shutil.which('cc') or shutil.which('gcc')), reason='needs a C compiler')
-def test_route_draw_struct_matches_the_header(tmp_path):
-  fields = [name for name, _ in engine.MpRouteDraw._fields_]
-  src = tmp_path / 'layout.c'
-  src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "mp_engine.h"\nint main(void) {\n'
-                 '  printf("%zu", sizeof(mp_route_draw));\n'
-                 + ''.join(f'  printf(" %zu", offsetof(mp_route_draw, {f}));\n' for f in fields) + '  return 0;\n}\n')
-  exe = tmp_path / 'layout'
-  subprocess.check_call([shutil.which('cc') or shutil.which('gcc'), '-I', os.path.join(ROOT, 'include'), str(src), '-o', str(exe)])
-  got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-  assert got[0] == ctypes.sizeof(engine.MpRouteDraw)
-  assert got[1:] == [getattr(engine.MpRouteDraw, f).offset for f in fields]
-
-
 @pytest.mark.skipif(torch.cuda.is_available(), reason='checks the no-GPU failure mode')
 def test_entry_points_refuse_a_null_handle_without_gpu():
   lib = engine.load_library()
-  d, players = engine.MpRouteDraw(), engine.MpPlayerOutputs()
-  assert lib.mp_step_drawn(None, ctypes.byref(d), None, 4, None, None, 0, 0, None, ctypes.byref(players), None) == -1
-  assert b'mp_step_drawn: null handle or draw' in lib.mp_last_error()
-  assert lib.mp_reset_drawn(None, None, ctypes.byref(d), None, ctypes.byref(players), None) == -1
-  assert b'mp_reset_drawn: null handle or draw' in lib.mp_last_error()
+  d, players = ctypes.pointer(engine.MpRouteDraw()), ctypes.pointer(engine.MpPlayerOutputs())
+  pa = ctypes.pointer(engine.MpPlayerActions())
+  for req in (engine.MpRequest(player_actions=pa, draw=d, players=players), engine.MpRequest(reset=1, draw=d, players=players)):
+    assert lib.mp_run(None, ctypes.byref(req), None) == -1
+    assert b'mp_run: null handle or request' in lib.mp_last_error()

@@ -19,7 +19,7 @@ def _cmp(eng, envs, where):
 
 
 def test_masked_reset_restarts_only_the_selected_envs(clean_up_blob, oracle):
-  # mp_reset(env_mask): the reference has one env per object, so a "masked reset" is env[i].reset() for some i.
+  # a reset with env_mask (mp_run): the reference has one env per object, so a "masked reset" is env[i].reset() for some i.
   _masked_reset(clean_up_blob, 'clean_up', oracle)
 
 

@@ -1,10 +1,10 @@
-"""The kernels one call of each step and reset entry point launches (mp_launch_count): rendering on or off, with or
-without the timestep exchange connected (world 1).
+"""The kernels one call of each step and reset request (mp_run) and of the other step and reset entry points launches
+(mp_launch_count): rendering on or off, with or without the timestep exchange connected (world 1).
 
 A state transition that the renderer follows on the stream lets k_render raise the exchange flags. A call that
-publishes its step without that (mp_step, mp_step_state, mp_step_restore without `out`, mp_step_routed without targets)
-launches k_exchange_push of its own, before k_render when rendering is on. With rendering off, k_exchange_push also
-delivers per-player scalars; scalars into `out` are copies, not kernels.
+publishes its step without that (a step request without `out` and `players`, mp_step_state) launches k_exchange_push of
+its own, before k_render when rendering is on. With rendering off, k_exchange_push also delivers per-player scalars;
+scalars into `out` are copies, not kernels.
 """
 
 import pytest
@@ -13,24 +13,24 @@ pytestmark = pytest.mark.gpu
 
 B = 16
 
-# entry point (and arguments) -> launches in the settings
+# mp_run request (by its fields) or entry point -> launches in the settings
 # (render on, render on + exchange, render off, render off + exchange)
 EXPECTED = {
-    'mp_reset': (2, 2, 1, 2),
-    'mp_reset_into': (2, 2, 1, 2),
-    'mp_reset_players': (2, 2, 2, 2),
+    'reset': (2, 2, 1, 2),
+    'reset out': (2, 2, 1, 2),
+    'reset players': (2, 2, 2, 2),
     'mp_step_state': (1, 2, 1, 2),
-    'mp_step': (2, 3, 1, 2),
-    'mp_step_into': (2, 2, 1, 2),
-    'mp_step_restore': (2, 3, 1, 2),
-    'mp_step_restore out': (2, 2, 1, 2),
-    'mp_step_players': (2, 2, 2, 2),
-    'mp_step_players restore': (2, 2, 2, 2),
-    'mp_step_routed': (2, 3, 1, 2),
-    'mp_step_routed out': (2, 2, 1, 2),
-    'mp_step_routed players': (2, 2, 2, 2),
-    'mp_step_routed restore': (2, 3, 1, 2),
-    'mp_step_routed restore out players': (2, 2, 2, 2),
+    'step': (2, 3, 1, 2),
+    'step out': (2, 2, 1, 2),
+    'step restore': (2, 3, 1, 2),
+    'step restore out': (2, 2, 1, 2),
+    'step players': (2, 2, 2, 2),
+    'step players restore': (2, 2, 2, 2),
+    'step player_actions': (2, 3, 1, 2),
+    'step player_actions out': (2, 2, 1, 2),
+    'step player_actions players': (2, 2, 2, 2),
+    'step player_actions restore': (2, 3, 1, 2),
+    'step player_actions restore out players': (2, 2, 2, 2),
     'mp_step_host': (2, 2, 1, 2),
     'mp_reset_host': (2, 2, 1, 2),
     'mp_step_host_async': (2, 2, 1, 2),
@@ -54,21 +54,21 @@ def _calls(eng):
     eng.wait(0)
 
   return {
-      'mp_reset': lambda: eng.reset(),
-      'mp_reset_into': lambda: eng.reset(out=out),
-      'mp_reset_players': lambda: eng.reset(players=players),
+      'reset': lambda: eng.reset(),
+      'reset out': lambda: eng.reset(out=out),
+      'reset players': lambda: eng.reset(players=players),
       'mp_step_state': lambda: eng.step_state(a),
-      'mp_step': lambda: eng.step(a),
-      'mp_step_into': lambda: eng.step(a, out=out),
-      'mp_step_restore': lambda: eng.step(a, **rs),
-      'mp_step_restore out': lambda: eng.step(a, out=out, **rs),
-      'mp_step_players': lambda: eng.step(a, players=players),
-      'mp_step_players restore': lambda: eng.step(a, players=players, **rs),
-      'mp_step_routed': lambda: eng.step(None, player_actions=pa),
-      'mp_step_routed out': lambda: eng.step(None, player_actions=pa, out=out),
-      'mp_step_routed players': lambda: eng.step(None, player_actions=pa, players=players),
-      'mp_step_routed restore': lambda: eng.step(None, player_actions=pa, **rs),
-      'mp_step_routed restore out players': lambda: eng.step(None, player_actions=pa, out=out, players=players, **rs),
+      'step': lambda: eng.step(a),
+      'step out': lambda: eng.step(a, out=out),
+      'step restore': lambda: eng.step(a, **rs),
+      'step restore out': lambda: eng.step(a, out=out, **rs),
+      'step players': lambda: eng.step(a, players=players),
+      'step players restore': lambda: eng.step(a, players=players, **rs),
+      'step player_actions': lambda: eng.step(None, player_actions=pa),
+      'step player_actions out': lambda: eng.step(None, player_actions=pa, out=out),
+      'step player_actions players': lambda: eng.step(None, player_actions=pa, players=players),
+      'step player_actions restore': lambda: eng.step(None, player_actions=pa, **rs),
+      'step player_actions restore out players': lambda: eng.step(None, player_actions=pa, out=out, players=players, **rs),
       'mp_step_host': lambda: eng.step_host(host_a, None),
       'mp_reset_host': lambda: eng.reset_host(None),
       'mp_step_host_async': host_async,

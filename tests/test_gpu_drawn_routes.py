@@ -1,8 +1,8 @@
-"""Drawn routes (mp_step_drawn / mp_reset_drawn, BatchedSubstrate.drawn_routes, BatchedScenario population mode).
+"""Drawn routes (mp_run's draw, BatchedSubstrate.drawn_routes, BatchedScenario population mode).
 
 A drawn engine steps beside a lockstep twin built with the same seed, which is handed the drawn engine's row maps as
-fixed inputs: its actions come from the map the drawn engine held before the call (mp_step_routed) and its outputs go
-to the map the drawn engine wrote (mp_step_players / mp_reset_players). Both deliver into sentinel-filled targets, which
+fixed inputs: its actions come from the map the drawn engine held before the call (player_actions) and its outputs go
+to the map the drawn engine wrote (players). Both deliver into sentinel-filled targets, which
 must then be equal byte for byte, as must every per-env output and, at the end, every env's state record. Each written
 map must equal the draw rule (tests/drawn_routes.py, on the oracle's Philox) for every env, with each env's episode and key tracked
 on the host across auto-resets, masked resets and in-step restores (clones keep the record's key, rekeyed restores take
@@ -244,6 +244,72 @@ def test_refused_calls_change_nothing():
   refused(bad, players, 'overlap', actions={'row_of_player': over[:B * eng.num_players].view(B, -1), 'action': over[B:B + r.n_rows]})
   torch.cuda.synchronize()
   assert eng.launch_count() == n and torch.equal(r.row_of_player, before)
+
+
+def test_refused_request_shapes_change_nothing():
+  """mp_run refuses a request that mixes a step's and a reset's fields, gives both action sources or neither, or draws
+  without the rows the draw delivers to and reads from, before anything is enqueued."""
+  import ctypes
+  import torch
+  from meltingpot_b200 import engine
+  blob, B = _blob('clean_up'), 8
+  eng = engine.Engine(blob, B, seed=1)
+  P = eng.num_players
+  lib = engine.load_library()
+  r = _routes(eng, _choices(P, np.random.default_rng(2)))
+  tg = _Rows(eng, r.n_rows)
+  eng.reset(players=tg.players(r.row_of_player), draw=r.draw)
+  a = torch.zeros((B, P), dtype=torch.int32, device='cuda')
+  mask = torch.ones(B, dtype=torch.uint8, device='cuda')
+  idx = torch.full((B,), -1, dtype=torch.int32, device='cuda')
+  bank = torch.zeros((4, eng.state_record_bytes), dtype=torch.uint8, device='cuda')
+  action = torch.zeros(r.n_rows, dtype=torch.int32, device='cuda')
+  other = r.row_of_player.clone()
+  stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+  def rows(rmap, n_rows):
+    s = engine.MpPlayerActions()
+    s.row_of_player, s.n_rows, s.action, s.action_row_stride = rmap.data_ptr(), n_rows, action.data_ptr(), 4
+    return ctypes.pointer(s)
+
+  pa = rows(r.row_of_player, r.n_rows)
+  players = ctypes.pointer(eng._player_outputs(tg.players(r.row_of_player)))  # pylint: disable=protected-access
+  draw = ctypes.pointer(r.draw)
+
+  def refused(match, **request):
+    torch.cuda.synchronize()
+    state, n, rmap = eng.save_state(), eng.launch_count(), r.row_of_player.clone()
+    rc = lib.mp_run(eng._h, ctypes.byref(engine.MpRequest(**request)), stream)  # pylint: disable=protected-access
+    assert rc == -1, (match, rc)
+    assert match in lib.mp_last_error().decode(), (match, lib.mp_last_error())
+    torch.cuda.synchronize()
+    assert eng.launch_count() == n, match
+    assert eng.save_state() == state and torch.equal(r.row_of_player, rmap), match
+
+  # a reset with any field of a step
+  no_step_fields = 'a reset takes no actions, player_actions, slot_of_env, bank or restore_flags'
+  refused(no_step_fields, reset=1, actions=a.data_ptr())
+  refused(no_step_fields, reset=1, player_actions=pa, players=players)
+  refused(no_step_fields, reset=1, slot_of_env=idx.data_ptr(), bank=bank.data_ptr(), n_slots=4)
+  refused(no_step_fields, reset=1, slot_of_env=idx.data_ptr())
+  refused(no_step_fields, reset=1, bank=bank.data_ptr())
+  refused(no_step_fields, reset=1, restore_flags=engine.MP_RESTORE_REKEY)
+  # a step with a reset's mask, with both action sources, or with neither
+  refused('env_mask is for a reset', actions=a.data_ptr(), env_mask=mask.data_ptr())
+  refused('not both', actions=a.data_ptr(), player_actions=pa)
+  refused('has neither', out=None)
+  refused('has neither', slot_of_env=idx.data_ptr(), bank=bank.data_ptr(), n_slots=4, players=players)
+  # draw without players, on a step or a reset
+  refused('draw needs players', reset=1, draw=draw)
+  refused('draw needs players', player_actions=pa, draw=draw)
+  # a drawn step whose actions do not come from the draw's rows
+  through = "a drawn step must read player_actions through the draw's row map and n_rows"
+  refused(through, actions=a.data_ptr(), draw=draw, players=players)
+  refused(through, player_actions=rows(other, r.n_rows), draw=draw, players=players)
+  refused(through, player_actions=rows(r.row_of_player, r.n_rows - 1), draw=draw, players=players)
+  # accepted as a control: the same drawn step, reading through the draw's rows
+  engine._check(lib.mp_run(eng._h, ctypes.byref(engine.MpRequest(player_actions=pa, draw=draw, players=players)), stream))  # pylint: disable=protected-access
+  torch.cuda.synchronize()
 
 
 def test_batched_scenario_population_equals_manual_stepping():

@@ -1,6 +1,6 @@
 """The C ABI's other entry points against the oracle, bit for bit, on every kernel family.
 
-The parity suites reach the kernels through mp_step / mp_reset on the current stream and read the engine's own
+The parity suites reach the kernels through mp_run's plain steps and resets on the current stream and read the engine's own
 buffers. These tests run the same kernels through the calls that use other buffers, streams or launch sequences: the
 pipelined host path (mp_step_host_async / mp_wait), split launches (mp_step_state / mp_render), host-buffer events at
 B > 1, snapshots across episode boundaries and render layouts, caller-created streams, and Philox keys whose high word

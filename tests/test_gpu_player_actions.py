@@ -1,4 +1,4 @@
-"""Actions read from rows (mp_step_routed, Engine.step(player_actions=), PlayerRoutes.actions).
+"""Actions read from rows (mp_run's player_actions, Engine.step(player_actions=), PlayerRoutes.actions).
 
 A routed engine steps beside a lockstep twin built with the same seed. The twin is stepped with the dense [B, P] actions
 the rule gives, composed on the host: player p of env b takes action[row_of_player[b, p]] when that row lies in
@@ -232,10 +232,16 @@ def test_refused_calls_change_nothing():
     before = [t.clone() for t in (eng.avatar_state, eng.grid, eng.step_type, eng.reward, act, rew)]
     snap = eng.save_state()
     n = eng.launch_count()
-    rc = lib.mp_step_routed(eng._h, None if s is None else ctypes.byref(s),  # pylint: disable=protected-access
-                            ctypes.c_void_p(idx.data_ptr()) if restore else None, ctypes.c_void_p(bank.data_ptr()) if restore else None,
-                            n_slots, flags, None if out is None else ctypes.byref(out),
-                            None if players is None else ctypes.byref(players), stream)
+    r = engine.MpRequest(n_slots=n_slots, restore_flags=flags)
+    if s is not None:
+      r.player_actions = ctypes.pointer(s)
+    if restore:
+      r.slot_of_env, r.bank = idx.data_ptr(), bank.data_ptr()
+    if out is not None:
+      r.out = ctypes.pointer(out)
+    if players is not None:
+      r.players = ctypes.pointer(players)
+    rc = lib.mp_run(eng._h, ctypes.byref(r), stream)  # pylint: disable=protected-access
     assert rc == -1, (match, rc)
     assert match in lib.mp_last_error().decode(), (match, lib.mp_last_error())
     torch.cuda.synchronize()
@@ -244,7 +250,7 @@ def test_refused_calls_change_nothing():
     for x, y in zip(before, (eng.avatar_state, eng.grid, eng.step_type, eng.reward, act, rew)):
       assert torch.equal(x, y), match
 
-  refused(None, 'null actions')
+  refused(None, 'has neither')  # a step with neither actions nor player_actions
   refused(struct(n_rows=0), 'n_rows')
   refused(struct(row_of_player=None), 'row_of_player')
   refused(struct(row_of_player=rmap.data_ptr() + 2), 'row_of_player')
@@ -275,7 +281,8 @@ def test_refused_calls_change_nothing():
   p = engine.MpPlayerOutputs(); p.row_of_player, p.n_rows, p.reward, p.reward_row_stride = rmap.data_ptr() + 4, B * P, rew.data_ptr(), 8
   refused(struct(), 'overlap', players=p)  # two row maps that overlap without being one tensor
   # the refusals of the composed calls
-  assert lib.mp_step_routed(eng._h, ctypes.byref(struct()), ctypes.c_void_p(idx.data_ptr()), None, 4, 0, None, None, stream) == -1  # pylint: disable=protected-access
+  r = engine.MpRequest(player_actions=ctypes.pointer(struct()), slot_of_env=idx.data_ptr(), n_slots=4)
+  assert lib.mp_run(eng._h, ctypes.byref(r), stream) == -1  # pylint: disable=protected-access
   assert 'go together' in lib.mp_last_error().decode()
   refused(struct(), 'n_slots', restore=True, n_slots=0)
   refused(struct(), 'unknown flags', restore=True, flags=2)
@@ -283,7 +290,8 @@ def test_refused_calls_change_nothing():
   refused(struct(), 'n_rows', players=engine.MpPlayerOutputs())
   # accepted: the two row maps are one tensor, and the player outputs take the rows
   p = engine.MpPlayerOutputs(); p.row_of_player, p.n_rows, p.reward, p.reward_row_stride = rmap.data_ptr(), B * P, rew.data_ptr(), 8
-  assert lib.mp_step_routed(eng._h, ctypes.byref(struct()), None, None, 0, 0, None, ctypes.byref(p), stream) == 0  # pylint: disable=protected-access
+  r = engine.MpRequest(player_actions=ctypes.pointer(struct()), players=ctypes.pointer(p))
+  assert lib.mp_run(eng._h, ctypes.byref(r), stream) == 0  # pylint: disable=protected-access
   torch.cuda.synchronize()
   assert torch.equal(rew, eng.reward.reshape(-1))
 

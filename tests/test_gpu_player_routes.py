@@ -1,4 +1,4 @@
-"""Per-player delivery to caller-chosen rows (mp_step_players / mp_reset_players, Engine.step(players=),
+"""Per-player delivery to caller-chosen rows (mp_run's players, Engine.step(players=),
 BatchedSubstrate.player_routes).
 
 Each run steps a routed engine beside a lockstep twin built with the same seed and fed the same actions. Every routed
@@ -306,8 +306,10 @@ def test_refused_calls_change_nothing():
     n = eng.launch_count()
     if flags is not None:
       eng.set_flags(flags)
-    o = None if out is None else ctypes.byref(out)
-    rc = lib.mp_step_players(eng._h, ctypes.c_void_p(a.data_ptr()), None, None, 0, 0, o, None if s is None else ctypes.byref(s), stream)  # pylint: disable=protected-access
+    r = engine.MpRequest(actions=a.data_ptr(), players=ctypes.pointer(s))
+    if out is not None:
+      r.out = ctypes.pointer(out)
+    rc = lib.mp_run(eng._h, ctypes.byref(r), stream)  # pylint: disable=protected-access
     eng.set_flags(engine.MP_FLAG_DEFAULT)
     assert rc == code, (match, rc)
     assert match in lib.mp_last_error().decode(), (match, lib.mp_last_error())
@@ -316,7 +318,6 @@ def test_refused_calls_change_nothing():
     for x, y in zip(before, (eng.avatar_state, eng.grid, eng.step_type, eng.reward, big, rew)):
       assert torch.equal(x, y), match
 
-  refused(None, 'null players')
   refused(struct(n_rows=0), 'n_rows')
   refused(struct(row_of_player=rmap.data_ptr() + 2), 'row_of_player')
   cudart = _cudart()
@@ -346,8 +347,8 @@ def test_refused_calls_change_nothing():
   bank = torch.zeros((4, eng.state_record_bytes), dtype=torch.uint8, device='cuda')
   idx = torch.full((B,), -1, dtype=torch.int32, device='cuda')
   s = struct(reward=bank.data_ptr(), reward_row_stride=8, rgb=None)
-  assert lib.mp_step_players(eng._h, ctypes.c_void_p(a.data_ptr()), ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(bank.data_ptr()), 4, 0,  # pylint: disable=protected-access
-                             None, ctypes.byref(s), stream) == -1
+  r = engine.MpRequest(actions=a.data_ptr(), slot_of_env=idx.data_ptr(), bank=bank.data_ptr(), n_slots=4, players=ctypes.pointer(s))
+  assert lib.mp_run(eng._h, ctypes.byref(r), stream) == -1  # pylint: disable=protected-access
   assert 'overlap' in lib.mp_last_error().decode()
 
 

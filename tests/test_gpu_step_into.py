@@ -1,4 +1,4 @@
-"""Steps and resets into caller-owned device tensors (mp_step_into / mp_reset_into, Engine.step(out=),
+"""Steps and resets into caller-owned device tensors (mp_run's out, Engine.step(out=),
 BatchedSubstrate.trajectory).
 
 An engine that steps into a trajectory buffer must give, slot for slot and byte for byte, what an engine stepped plainly
@@ -401,7 +401,8 @@ def test_refused_outputs_step_no_env():
   host = torch.zeros(B * P, dtype=torch.float64).pin_memory()
   s = engine.MpDeviceOutputs()
   s.reward, s.reward_env_stride = host.data_ptr(), P * 8
-  refused(None, 'not device memory', lambda: lib.mp_step_into(eng._h, ctypes.c_void_p(a.data_ptr()), ctypes.byref(s), None))  # pylint: disable=protected-access
+  step_into = lambda s: lib.mp_run(eng._h, ctypes.byref(engine.MpRequest(actions=a.data_ptr(), out=ctypes.pointer(s))), None)  # pylint: disable=protected-access
+  refused(None, 'not device memory', lambda: step_into(s))
   cudart = _cudart()
   ptr = ctypes.c_void_p()
   mib = 1 << 20
@@ -409,10 +410,10 @@ def test_refused_outputs_step_no_env():
   try:
     s = engine.MpDeviceOutputs()
     s.reward, s.reward_env_stride = ptr.value, mib  # env B - 1's row starts at the end of the allocation
-    refused(None, 'past the end', lambda: lib.mp_step_into(eng._h, ctypes.c_void_p(a.data_ptr()), ctypes.byref(s), None))  # pylint: disable=protected-access
+    refused(None, 'past the end', lambda: step_into(s))
     s.reward_env_stride = mib - P * 8  # ... and ends exactly at it: accepted
     torch.cuda.synchronize()
-    engine._check(lib.mp_step_into(eng._h, ctypes.c_void_p(a.data_ptr()), ctypes.byref(s), None))  # pylint: disable=protected-access
+    engine._check(step_into(s))  # pylint: disable=protected-access
     torch.cuda.synchronize()
   finally:
     cudart.cudaFree(ptr)

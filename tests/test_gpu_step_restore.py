@@ -1,4 +1,4 @@
-"""Restores inside a step (mp_step_restore, Engine.step(restore=, bank=), BatchedSubstrate / ShardedSubstrate.step).
+"""Restores inside a step (mp_run's slot_of_env and bank, Engine.step(restore=, bank=), BatchedSubstrate / ShardedSubstrate.step).
 
 The fused call must give, byte for byte, what a step followed by mp_state_restore with the same arguments gives: every
 output, the events, the state, the variant bytes and the mp_state_save snapshot, after the call and on every step that
@@ -125,7 +125,7 @@ def _run(fam, B, oracle):
   trail = []
   for t in range(43, 88):
     x = torch.from_numpy(np.ascontiguousarray(rng.integers(0, A, size=(B, P)), np.int32)).cuda()
-    if t % 3 == 0:  # no restore: an index of all -1 steps every env as mp_step does
+    if t % 3 == 0:  # no restore: an index of all -1 steps every env as a plain step does
       a.step(x, restore=_idx(B, {}), bank=bank)
       b.step(x)
     else:
@@ -376,11 +376,12 @@ def test_refused_fused_calls_step_no_env(clean_up_blob):
   idx = torch.arange(B, dtype=torch.int32, device='cuda')
   big = torch.zeros((2 * R + 64,), dtype=torch.uint8, device='cuda')
   eng.store_states(big[:2 * R].view(2, R), torch.arange(2, dtype=torch.int32, device='cuda'))
-  vp = ctypes.c_void_p
 
   def call(bank, index, n, flags=0, out=None):
-    return lib.mp_step_restore(eng._h, vp(acts.data_ptr()), vp(index), vp(bank), n, flags,  # pylint: disable=protected-access
-                               ctypes.byref(out) if out is not None else None, None)
+    r = engine.MpRequest(actions=acts.data_ptr(), slot_of_env=index, bank=bank, n_slots=n, restore_flags=flags)
+    if out is not None:
+      r.out = ctypes.pointer(out)
+    return lib.mp_run(eng._h, ctypes.byref(r), None)  # pylint: disable=protected-access
 
   def refused(match, fn):
     torch.cuda.synchronize()
@@ -390,8 +391,8 @@ def test_refused_fused_calls_step_no_env(clean_up_blob):
     assert eng.launch_count() == launches, f'a refused call ({match}) launched a kernel'
     assert eng.save_state() == snap, f'a refused call ({match}) moved an env'
 
-  refused('null', lambda: call(None, idx.data_ptr(), 2))
-  refused('null', lambda: call(big.data_ptr(), None, 2))
+  refused('go together', lambda: call(None, idx.data_ptr(), 2))
+  refused('go together', lambda: call(big.data_ptr(), None, 2))
   refused('n_slots', lambda: call(big.data_ptr(), idx.data_ptr(), 0))
   refused('flags', lambda: call(big.data_ptr(), idx.data_ptr(), 2, flags=6))
   refused('aligned', lambda: call(big.data_ptr() + 1, idx.data_ptr(), 2))

@@ -313,9 +313,12 @@ def test_refused_calls_change_nothing():
     n = eng.launch_count()
     if flags is not None:
       eng.set_flags(flags)
-    o = None if out is None else ctypes.byref(out)
-    idx, bk, n_slots = (None, None, 0) if bank is None else (ctypes.c_void_p(bank[0].data_ptr()), ctypes.c_void_p(bank[1].data_ptr()), 4)
-    rc = lib.mp_step_players(eng._h, ctypes.c_void_p(a.data_ptr()), idx, bk, n_slots, 0, o, ctypes.byref(s), stream)  # pylint: disable=protected-access
+    r = engine.MpRequest(actions=a.data_ptr(), players=ctypes.pointer(s))
+    if out is not None:
+      r.out = ctypes.pointer(out)
+    if bank is not None:
+      r.slot_of_env, r.bank, r.n_slots = bank[0].data_ptr(), bank[1].data_ptr(), 4
+    rc = lib.mp_run(eng._h, ctypes.byref(r), stream)  # pylint: disable=protected-access
     eng.set_flags(engine.MP_FLAG_DEFAULT)
     assert rc == -1, (match, rc)
     assert match in lib.mp_last_error().decode(), (match, lib.mp_last_error())
@@ -363,7 +366,8 @@ def test_refused_calls_change_nothing():
   # a routed call's action rows
   rows = engine.MpPlayerActions(); rows.row_of_player, rows.n_rows, rows.action, rows.action_row_stride = rmap.data_ptr(), B * P, wrgb.data_ptr(), 4
   state, n = eng.save_state(), eng.launch_count()
-  assert lib.mp_step_routed(eng._h, ctypes.byref(rows), None, None, 0, 0, None, ctypes.byref(struct()), stream) == -1  # pylint: disable=protected-access
+  r = engine.MpRequest(player_actions=ctypes.pointer(rows), players=ctypes.pointer(struct()))
+  assert lib.mp_run(eng._h, ctypes.byref(r), stream) == -1  # pylint: disable=protected-access
   assert 'overlap' in lib.mp_last_error().decode() and eng.launch_count() == n and eng.save_state() == state
   # the Python layer refuses before any call on a batch without WORLD.RGB
   from meltingpot_b200 import substrate

@@ -1,12 +1,7 @@
 """CPU test: PlayerActions (routes.actions(T)) shapes, slots and groups, the tensor -> mp_player_actions conversion and
-its refusals, the argument errors of step(player_actions=), the ctypes struct against the header, and the no-GPU failure
-of mp_step_routed."""
+its refusals, the argument errors of step(player_actions=), and the no-GPU failure of a step with player_actions."""
 
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 import types
 
 import numpy as np
@@ -16,7 +11,6 @@ import torch
 from meltingpot_b200 import engine
 from meltingpot_b200 import substrate
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 B, P, H, W = 3, 4, 16, 24
 NAMES = ['READY_TO_SHOOT']
 
@@ -153,37 +147,9 @@ def test_substrate_step_argument_errors():
 
 
 # -- C ABI ----------------------------------------------------------------------------------------------------------------
-def test_c_abi_declares_the_entry_point():
-  with open(os.path.join(ROOT, 'include', 'mp_engine.h')) as f:
-    header = f.read()
-  decl = [p.strip() for p in re.search(r'\bint mp_step_routed\(([^;]*)\);', header).group(1).split(',')]
-  assert decl == ['mp_handle h', 'const mp_player_actions* actions', 'const int32_t* slot_of_env', 'const void* bank',
-                  'int n_slots', 'uint32_t flags', 'const mp_device_outputs* out', 'const mp_player_outputs* players',
-                  'void* stream']
-  lib = engine.load_library()
-  vp = ctypes.c_void_p
-  assert lib.mp_step_routed.argtypes == [vp, ctypes.POINTER(engine.MpPlayerActions), vp, vp, ctypes.c_int, ctypes.c_uint32,
-                                         ctypes.POINTER(engine.MpDeviceOutputs), ctypes.POINTER(engine.MpPlayerOutputs), vp]
-  assert 'mp_step_routed' in engine.EXPORTED_SYMBOLS
-
-
-@pytest.mark.skipif(not (shutil.which('cc') or shutil.which('gcc')), reason='needs a C compiler')
-def test_player_actions_struct_matches_the_header(tmp_path):
-  fields = [name for name, _ in engine.MpPlayerActions._fields_]
-  src = tmp_path / 'layout.c'
-  src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "mp_engine.h"\nint main(void) {\n'
-                 '  printf("%zu", sizeof(mp_player_actions));\n'
-                 + ''.join(f'  printf(" %zu", offsetof(mp_player_actions, {f}));\n' for f in fields) + '  return 0;\n}\n')
-  exe = tmp_path / 'layout'
-  subprocess.check_call([shutil.which('cc') or shutil.which('gcc'), '-I', os.path.join(ROOT, 'include'), str(src), '-o', str(exe)])
-  got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-  assert got[0] == ctypes.sizeof(engine.MpPlayerActions)
-  assert got[1:] == [getattr(engine.MpPlayerActions, f).offset for f in fields]
-
-
 @pytest.mark.skipif(torch.cuda.is_available(), reason='checks the no-GPU failure mode')
 def test_entry_point_raises_without_gpu():
   lib = engine.load_library()
-  actions = engine.MpPlayerActions()
-  assert lib.mp_step_routed(None, ctypes.byref(actions), None, None, 0, 0, None, None, None) == -1
+  req = engine.MpRequest(player_actions=ctypes.pointer(engine.MpPlayerActions()))
+  assert lib.mp_run(None, ctypes.byref(req), None) == -1
   assert b'null handle' in lib.mp_last_error()

@@ -1,11 +1,7 @@
-"""CPU test: the row layout and outputs of PlayerRoutes, the tensor -> mp_player_outputs conversion, the ctypes struct
-against the header, and the no-GPU failure of mp_step_players / mp_reset_players (no device)."""
+"""CPU test: the row layout and outputs of PlayerRoutes, the tensor -> mp_player_outputs conversion, and the no-GPU
+failure of a step and a reset with player rows (no device)."""
 
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,7 +10,6 @@ import torch
 from meltingpot_b200 import engine
 from meltingpot_b200 import substrate
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 B, P, H, W, N = 3, 4, 16, 24, 2
 NAMES = ['READY_TO_SHOOT', 'NUM_OTHERS_WHO_CLEANED_THIS_STEP']
 
@@ -170,37 +165,6 @@ def test_describe_refuses_other_devices_and_missing_scalars():
 
 
 # -- C ABI ----------------------------------------------------------------------------------------------------------------
-def test_c_abi_declares_the_entry_points():
-  with open(os.path.join(ROOT, 'include', 'mp_engine.h')) as f:
-    header = f.read()
-  decl = lambda name: [p.strip() for p in re.search(rf'\bint {name}\(([^;]*)\);', header).group(1).split(',')]
-  assert decl('mp_step_players') == ['mp_handle h', 'const int32_t* actions', 'const int32_t* slot_of_env', 'const void* bank',
-                                     'int n_slots', 'uint32_t flags', 'const mp_device_outputs* out',
-                                     'const mp_player_outputs* players', 'void* stream']
-  assert decl('mp_reset_players') == ['mp_handle h', 'const uint8_t* env_mask', 'const mp_device_outputs* out',
-                                      'const mp_player_outputs* players', 'void* stream']
-  lib = engine.load_library()
-  vp = ctypes.c_void_p
-  assert lib.mp_step_players.argtypes == [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32,
-                                          ctypes.POINTER(engine.MpDeviceOutputs), ctypes.POINTER(engine.MpPlayerOutputs), vp]
-  assert lib.mp_reset_players.argtypes == [vp, vp, ctypes.POINTER(engine.MpDeviceOutputs),
-                                           ctypes.POINTER(engine.MpPlayerOutputs), vp]
-
-
-@pytest.mark.skipif(not (shutil.which('cc') or shutil.which('gcc')), reason='needs a C compiler')
-def test_player_outputs_struct_matches_the_header(tmp_path):
-  fields = [name for name, _ in engine.MpPlayerOutputs._fields_]
-  src = tmp_path / 'layout.c'
-  src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "mp_engine.h"\nint main(void) {\n'
-                 '  printf("%zu", sizeof(mp_player_outputs));\n'
-                 + ''.join(f'  printf(" %zu", offsetof(mp_player_outputs, {f}));\n' for f in fields) + '  return 0;\n}\n')
-  exe = tmp_path / 'layout'
-  subprocess.check_call([shutil.which('cc') or shutil.which('gcc'), '-I', os.path.join(ROOT, 'include'), str(src), '-o', str(exe)])
-  got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-  assert got[0] == ctypes.sizeof(engine.MpPlayerOutputs)
-  assert got[1:] == [getattr(engine.MpPlayerOutputs, f).offset for f in fields]
-
-
 def _cuda_available():
   return torch.cuda.is_available()
 
@@ -208,10 +172,10 @@ def _cuda_available():
 @pytest.mark.skipif(_cuda_available(), reason='checks the no-GPU failure mode')
 def test_entry_points_raise_without_gpu(clean_up_blob):
   lib = engine.load_library()
-  players = engine.MpPlayerOutputs()
-  assert lib.mp_step_players(None, None, None, None, 0, 0, None, ctypes.byref(players), None) == -1
-  assert lib.mp_reset_players(None, None, None, ctypes.byref(players), None) == -1
-  assert b'null handle' in lib.mp_last_error()
+  players = ctypes.pointer(engine.MpPlayerOutputs())
+  for req in (engine.MpRequest(players=players), engine.MpRequest(reset=1, players=players)):
+    assert lib.mp_run(None, ctypes.byref(req), None) == -1
+    assert b'null handle' in lib.mp_last_error()
   with pytest.raises(engine.EngineError):
     substrate.BatchedSubstrate(clean_up_blob, 2, seed=1)
   with pytest.raises(engine.EngineError):

@@ -1,9 +1,6 @@
-"""CPU test: the declarations of mp_step_restore and the argument checks of Engine.step(restore=, bank=), on tensor
-layouts alone (no device). Tensors pose as CUDA tensors through a subclass; the C library is replaced by a recorder."""
+"""CPU test: the argument checks of Engine.step(restore=, bank=) and the mp_run request it makes, on tensor layouts
+alone (no device). Tensors pose as CUDA tensors through a subclass; the C library is replaced by a recorder."""
 
-import ctypes
-import os
-import re
 import types
 
 import pytest
@@ -13,24 +10,8 @@ from meltingpot_b200 import distributed
 from meltingpot_b200 import engine
 from meltingpot_b200 import substrate
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 B, P, R = 6, 3, 64
 STREAM = types.SimpleNamespace(cuda_stream=0)
-
-
-def test_c_abi_declares_step_restore():
-  with open(os.path.join(ROOT, 'include', 'mp_engine.h')) as f:
-    header = f.read()
-  m = re.search(r'\bint mp_step_restore\(([^;]*)\);', header)
-  assert m, 'mp_step_restore is not declared'
-  params = [p.strip() for p in m.group(1).split(',')]
-  assert params == ['mp_handle h', 'const int32_t* actions', 'const int32_t* slot_of_env', 'const void* bank', 'int n_slots',
-                    'uint32_t flags', 'const mp_device_outputs* out', 'void* stream'], params
-  assert 'mp_step_restore' in engine.EXPORTED_SYMBOLS
-  lib = engine.load_library()
-  vp = ctypes.c_void_p
-  assert lib.mp_step_restore.argtypes == [vp, vp, vp, vp, ctypes.c_int, ctypes.c_uint32,
-                                          ctypes.POINTER(engine.MpDeviceOutputs), vp]
 
 
 class _OnDevice(torch.Tensor):
@@ -119,10 +100,13 @@ def test_engine_step_passes_restore_to_the_library():
   eng.step(ACTIONS, stream=STREAM, **_args(rekey=True))
   eng.step(ACTIONS, stream=STREAM, **_args())
   eng.step(ACTIONS, stream=STREAM)
-  (n0, a0), (n1, a1), (n2, _) = eng._lib.calls  # pylint: disable=protected-access
-  assert n0 == n1 == 'mp_step_restore' and n2 == 'mp_step'
-  assert a0[4] == 4 and a0[5].value == engine.MP_RESTORE_REKEY and a1[5].value == 0
-  assert a0[6] is None  # no `out`: the engine's own buffers
+  calls = eng._lib.calls  # pylint: disable=protected-access
+  assert [name for name, _ in calls] == ['mp_run'] * 3
+  r0, r1, r2 = (args[1]._obj for _, args in calls)  # the MpRequest behind each byref
+  assert r0.n_slots == 4 and r0.restore_flags == engine.MP_RESTORE_REKEY and r1.restore_flags == 0
+  assert r0.slot_of_env and r0.bank and r1.slot_of_env and r1.bank
+  assert not r0.out and not r0.players  # no `out`: the engine's own buffers
+  assert r2.actions and not (r2.slot_of_env or r2.bank or r2.n_slots or r2.restore_flags or r2.reset)
 
 
 class _StepRecorder:

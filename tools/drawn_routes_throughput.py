@@ -1,10 +1,10 @@
-"""What drawing player routes on the device (mp_step_drawn) costs against fixed routes and against rerouting in torch.
+"""What drawing player routes on the device (mp_run's draw) costs against fixed routes and against rerouting in torch.
 
 For each workload, alternating in rounds:
 
-  a_fixed:  mp_step_routed with players: fixed routes (the row map of the drawn reset that starts the run, as input);
-  b_drawn:  mp_step_drawn on the same DrawnRoutes: the step draws each slot's bot at every episode start;
-  c_torch:  mp_step_routed with players, after rerouting in torch between steps: envs whose step was FIRST draw their
+  a_fixed:  a step with player_actions and players: fixed routes (the row map of the drawn reset that starts the run, as input);
+  b_drawn:  a drawn step on the same DrawnRoutes: the step draws each slot's bot at every episode start;
+  c_torch:  a step with player_actions and players, after rerouting in torch between steps: envs whose step was FIRST draw their
             slots' bots anew (torch.randint) and the row map is rebuilt from the drawn choices with torch ops.
 
 Workloads: clean_up x 4096 with clean_up_0's split (3 focal slots, 4 background slots drawing from 2 bots), and

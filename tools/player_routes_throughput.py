@@ -1,11 +1,11 @@
-"""What per-player routing (mp_step_players) costs against a dense step and against gathering players after the step.
+"""What per-player routing (mp_run's players) costs against a dense step and against gathering players after the step.
 
 For each workload (clean_up x 4096 and commons_harvest__open 16p x 8192), alternating in rounds:
 
-  a_step_into:    mp_step_into with a dense [B, P, h, w, 3] image target and reward;
-  b_identity:     mp_step_players, row of player p of env b = b * P + p (the same bytes as a);
-  c_permuted:     mp_step_players, a random permutation of those rows;
-  d_half:         mp_step_players with a random half of the players unrouted (neither drawn nor stored);
+  a_step_into:    a step with `out`: a dense [B, P, h, w, 3] image target and reward;
+  b_identity:     a step with players, row of player p of env b = b * P + p (the same bytes as a);
+  c_permuted:     a step with players, a random permutation of those rows;
+  d_half:         a step with players, a random half of the players unrouted (neither drawn nor stored);
   e_index_select: a plain step followed by BatchedScenario's split: index_select of the images and rewards on the player
                   axis, once for the focal and once for the background players (first / second half of the slots).
 

@@ -1,12 +1,12 @@
-"""What actions read from rows (mp_step_routed) cost against dense actions, and what BatchedScenario's step costs on
+"""What actions read from rows (mp_run's player_actions) cost against dense actions, and what BatchedScenario's step costs on
 player routes against the index_select / index_copy_ split it replaced.
 
 For each workload (clean_up 7p x 4096 with 5 focal / 2 background players, commons_harvest__open 16p x 8192 with
 12 / 4), alternating in rounds:
 
-  a_dense:            mp_step with dense [B, P] actions;
-  b_rows_identity:    mp_step_routed, row of player p of env b = b * P + p (the same actions as a);
-  c_rows_permuted:    mp_step_routed, a random permutation of those rows;
+  a_dense:            a step with dense [B, P] actions;
+  b_rows_identity:    a step with player_actions, row of player p of env b = b * P + p (the same actions as a);
+  c_rows_permuted:    a step with player_actions, a random permutation of those rows;
   d_scenario_split:   the scenario step of the previous BatchedScenario, reproduced here: index_copy_ of the focal and
                       background actions into [B, P], a plain step, then index_select of every per-player output, once
                       for the focal and once for the background players;

@@ -8,7 +8,7 @@ For each workload (clean_up x 4096 and commons_harvest__open 16p x 8192, each wi
   restore:         mp_state_restore with rendering on (kernel + render);
   step:            a plain step with uniform-random actions, for scale;
   d2d_copy:        a device-to-device copy of the same 2 x record_bytes x B bytes (read + write), the bandwidth yardstick;
-  step_restore:    a step that restores a fraction of the envs instead of advancing them (mp_step_restore);
+  step_restore:    a step that restores a fraction of the envs instead of advancing them (mp_run's slot_of_env and bank);
   step+restore:    a step followed by mp_state_restore of the same envs (what step_restore replaces).
 The last two run at restored fractions 0, 1/64, 1/8 and 1 of B (field `restored`: envs restored per call, spread evenly
 over the batch).

@@ -2,7 +2,7 @@
 rendering it for every env.
 
 For each workload (clean_up x 4096 and commons_harvest__open 16p x 8192), every player routed to its own row
-(mp_step_players, identity rows), alternating in rounds:
+(a step with players, identity rows), alternating in rounds:
 
   a_world_off:   the engine built without WORLD.RGB (render flags: player images only);
   b_world_dense: WORLD.RGB rendered for every env into the engine's own buffer;
