@@ -306,7 +306,20 @@ int mp_state_restore(mp_handle h, const int32_t* slot_of_env, const void* bank, 
  * pointer is optional (NULL: not delivered per player). Strides in bytes.
  * WORLD.RGB is routed per env the same way: env b's image goes to row world_row_of_env[b] of world_rgb when
  * 0 <= row < world_n_rows, and is not rendered otherwise, e.g. for the few envs of a video. A zeroed tail (world_rgb and
- * world_row_of_env NULL) leaves WORLD.RGB per env. */
+ * world_row_of_env NULL) leaves WORLD.RGB per env.
+ * Row segments send ranges of rows to targets of their own, e.g. one [T_g, n_g, ...] trajectory buffer per group of a
+ * population: with n_segments > 0 (up to MP_MAX_ROW_SEGMENTS) the top-level rgb, reward and scalar_obs stay NULL and row
+ * r with segments[s].row_begin <= r < segments[s].row_end goes to segment s, at target + (r - row_begin) * row_stride
+ * of each of its outputs. Segments are sorted, disjoint, non-empty and inside [0, n_rows), and each carries the same set
+ * of outputs. A row in no segment is treated as a player without a row: it is neither composited nor stored and gets
+ * no scalars. A zeroed tail (n_segments 0) delivers every row to the top-level targets. */
+#define MP_MAX_ROW_SEGMENTS 16
+typedef struct mp_row_segment {
+  int32_t row_begin, row_end;                          /* rows [row_begin, row_end) of the row map */
+  uint8_t* rgb;        uint64_t rgb_row_stride;        /* [row_end - row_begin] x u8 [rgb_h][rgb_w][3], dense inside a row */
+  double*  reward;     uint64_t reward_row_stride;     /* [row_end - row_begin] x f64 */
+  double*  scalar_obs; uint64_t scalar_obs_row_stride, scalar_obs_stride; /* [n_scalar] x [row_end - row_begin] x f64 */
+} mp_row_segment;
 typedef struct mp_player_outputs {
   const int32_t* row_of_player;  /* DEVICE i32 [B][P]: row of player p of env b; < 0 or >= n_rows = not delivered */
   int32_t n_rows;
@@ -316,6 +329,8 @@ typedef struct mp_player_outputs {
   const int32_t* world_row_of_env;  /* DEVICE i32 [B]: row of env b's WORLD.RGB; < 0 or >= world_n_rows = not rendered */
   int32_t world_n_rows;
   uint8_t* world_rgb; uint64_t world_rgb_row_stride;  /* [world_n_rows] x u8 [world_h][world_w][3], dense inside a row */
+  int32_t n_segments;                                  /* 0: rows go to rgb / reward / scalar_obs above */
+  mp_row_segment segments[MP_MAX_ROW_SEGMENTS];
 } mp_player_outputs;
 
 /* Caller-owned DEVICE rows a step's actions are read from: player p of env b takes the action id in row
@@ -416,7 +431,8 @@ typedef struct mp_route_draw {
  * Launches: a reset, and a request with `out` or `players`, launch the state transition and one render, which also
  * publishes the step to a connected exchange. A step with neither launches as mp_step_state followed by mp_render: with
  * the exchange connected, k_exchange_push follows the state transition. With rendering off, `players` with reward or
- * scalar_obs rows adds one small kernel (k_exchange_push) that delivers them.
+ * scalar_obs rows adds one small kernel (k_exchange_push) that delivers them. A request with row segments launches
+ * exactly the kernels of the same request with one target.
  *
  * Every check runs before anything is enqueued, and a refused request (MP_E_INVALID) steps no env. Refused:
  *   - the request: a NULL handle or request; a reset with actions, player_actions, slot_of_env, bank or restore_flags; a
@@ -441,7 +457,10 @@ typedef struct mp_route_draw {
  *     4-byte aligned or not B i32 inside one device allocation on the engine's device, world_rgb or its row stride not a
  *     multiple of 16 bytes, a world row stride smaller than one WORLD.RGB image, world_rgb while the render flags switch
  *     WORLD.RGB off, or together with out->world_rgb; any target or row map that overlaps another, `out`'s targets, the
- *     bank, the index array or the engine's buffers;
+ *     bank, the index array or the engine's buffers; n_segments outside 0..MP_MAX_ROW_SEGMENTS; segments together with a
+ *     top-level rgb, reward or scalar_obs; segments that are empty, unsorted, overlap or leave [0, n_rows); segments
+ *     that carry different sets of outputs; and every refusal above of rgb, reward and scalar_obs, applied to each
+ *     segment's targets over its own rows;
  *   - draw: draw n_rows < 1; players whose map or n_rows are not the draw's; a step whose player_actions are missing or
  *     have a map or n_rows that are not the draw's; a slot with more than MP_MAX_ROUTE_CHOICES choices (or fewer than
  *     0); a choice whose rows of some env fall outside [0, n_rows). The map must not overlap any target, the action

@@ -89,23 +89,43 @@ struct ScalarTargets {
 };
 
 // Caller-owned per-player rows of one step (mp_player_outputs, mp_run's players): player p of env b goes to row
-// row_of_player[b][p] when that is in [0, n_rows). Strides in bytes; scalar_obs row (k, r) starts at
-// scalar_obs + k * scalar_obs_stride + r * scalar_obs_row_stride. Env b's WORLD.RGB goes to row world_row_of_env[b]
-// of world_rgb when that is in [0, world_n_rows) and world_rgb is set. Read only by k_render<..., RENDER_ROUTED> and
-// k_exchange_push.
+// row_of_player[b][p], delivered through the segment that holds the row (RowSegments) and nowhere when no segment does.
+// Env b's WORLD.RGB goes to row world_row_of_env[b] of world_rgb when that is in [0, world_n_rows) and world_rgb is
+// set. Read only by k_render<..., RENDER_ROUTED> and k_exchange_push.
 struct PlayerTargets {
   const int32_t* row_of_player;  // [B][P]
-  int n_rows;
-  int scalars_on;  // reward or scalar_obs is set
-  uint8_t* rgb;
-  double* reward;
-  double* scalar_obs;
-  uint64_t rgb_row_stride, reward_row_stride, scalar_obs_row_stride, scalar_obs_stride;
+  int scalars_on;  // the segments carry reward or scalar_obs
   const int32_t* world_row_of_env;  // [B]
   uint8_t* world_rgb;
   uint64_t world_rgb_row_stride;
   int world_n_rows;
 };
+
+// The per-player targets of a routed step by row range (mp_row_segment, same layout): row r of segment s
+// (row_begin <= r < row_end) goes to target + (r - row_begin) * row_stride; scalar_obs row (k, r) starts at
+// scalar_obs + k * scalar_obs_stride + (r - row_begin) * scalar_obs_row_stride. A request without segments is one segment
+// [0, n_rows). Segments are sorted and disjoint and all carry the same outputs (checked on the host), so s[0] tells which
+// outputs are routed. A __grid_constant__ parameter of k_render and k_exchange_push: the table reaches the kernels with
+// their launch, so no copy, synchronise or extra launch is needed, and only the routed code reads it.
+#define MP_ROW_SEGMENTS 16
+struct RowSegment {
+  int32_t row_begin, row_end;
+  uint8_t* rgb; uint64_t rgb_row_stride;
+  double* reward; uint64_t reward_row_stride;
+  double* scalar_obs; uint64_t scalar_obs_row_stride, scalar_obs_stride;
+};
+struct RowSegments {
+  int n;
+  RowSegment s[MP_ROW_SEGMENTS];
+};
+
+// The segment that holds row `row`, or -1 when none does. A scan with a uniform index: a warp's lanes read the same
+// constant-bank entries.
+__device__ __forceinline__ int row_segment(const RowSegments& G, int row) {
+  int s = -1;
+  for (int k = 0; k < G.n; ++k) s = (row >= G.s[k].row_begin && row < G.s[k].row_end) ? k : s;
+  return s;
+}
 
 struct State {
   int B;
@@ -288,21 +308,23 @@ __device__ __forceinline__ void deliver_scalars(const Tables& T, const State& S)
 
 // Delivery of the routed players' reward and scalar observations into their rows (State::pr), like deliver_scalars:
 // one warp per env, lane i covering (output k = i / P, player p = i % P); output 0 is the reward, output 1 + j
-// scalar observation j. A player without a row gets nothing; nothing outside [0, n_rows) is written.
-__device__ __forceinline__ void deliver_player_scalars(const Tables& T, const State& S) {
-  const PlayerTargets& o = S.pr;
-  if (!o.scalars_on) return;
+// scalar observation j. A player whose row lies in no segment gets nothing; nothing outside the segments is written.
+__device__ __forceinline__ void deliver_player_scalars(const Tables& T, const State& S, const RowSegments& G) {
+  if (!S.pr.scalars_on) return;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = (int)blockDim.x >> 5;
-  const int P = T.P, n = P * (1 + (o.scalar_obs ? T.n_scalar : 0));
+  const int P = T.P, n = P * (1 + (G.s[0].scalar_obs ? T.n_scalar : 0));
   for (int b = (int)blockIdx.x + warp * (int)gridDim.x; b < S.B; b += n_warps * (int)gridDim.x) {
     for (int i = lane; i < n; i += 32) {
       const int k = i / P, p = i - k * P;
-      const int row = o.row_of_player[(size_t)b * P + p];
-      if ((uint32_t)row >= (uint32_t)o.n_rows) continue;
+      const int row = S.pr.row_of_player[(size_t)b * P + p];
+      const int s = row_segment(G, row);
+      if (s < 0) continue;
+      const RowSegment& o = G.s[s];
+      const size_t r = (size_t)(row - o.row_begin);
       if (k == 0) {
-        if (o.reward) *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.reward) + (size_t)row * o.reward_row_stride) = S.reward[(size_t)b * P + p];
+        if (o.reward) *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.reward) + r * o.reward_row_stride) = S.reward[(size_t)b * P + p];
       } else {
-        *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.scalar_obs) + (size_t)(k - 1) * o.scalar_obs_stride + (size_t)row * o.scalar_obs_row_stride) =
+        *reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(o.scalar_obs) + (size_t)(k - 1) * o.scalar_obs_stride + r * o.scalar_obs_row_stride) =
             S.scalar_obs[((size_t)(k - 1) * S.B + b) * P + p];
       }
     }
@@ -310,11 +332,12 @@ __device__ __forceinline__ void deliver_player_scalars(const Tables& T, const St
 }
 
 // Delivery when no render follows the state transition (mp_step_state on its own, or rendering switched off).
-__global__ void __launch_bounds__(256) k_exchange_push(Tables T, State S) {
+// G: the per-player rows' segments (n = 0 when the call routes none).
+__global__ void __launch_bounds__(256) k_exchange_push(Tables T, State S, const __grid_constant__ RowSegments G) {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   exchange_push(T, S);
   deliver_scalars(T, S);
-  deliver_player_scalars(T, S);
+  deliver_player_scalars(T, S, G);
 }
 
 // The consumer side, enqueued by EVERY rank after its step (mp_exchange_wait; stream-ordered after the kernel that

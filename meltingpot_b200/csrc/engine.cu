@@ -254,7 +254,7 @@ struct mp_engine {
   int sm_count = 0;
   size_t step_smem = 0;  // dynamic shared memory of one state-transition launch
   // k_render<inst_ncp, inst_ncw, mode> by mode: RENDER_PLAIN, RENDER_GATHER (mp_gather_obs_*), RENDER_ROUTED (player rows)
-  void (*render_fns[3])(Tables, State, RenderPlan, uint32_t) = {};
+  void (*render_fns[3])(Tables, State, RenderPlan, uint32_t, RowSegments) = {};
   // mp_gather_obs_*: this rank's stacked-observation block [flags 256 B][2 slots][rgb of all ranks | world_rgb of all ranks]
   uint8_t* g_block = nullptr;
   uint64_t g_block_bytes = 0, g_slot_bytes = 0, g_world_off = 0;
@@ -751,10 +751,11 @@ __global__ void k_debug_obs(Tables T, State S, int32_t* position, int32_t* orien
 // For a call that launches no state transition: every field -1 until launch_render records its render.
 void clear_last_launch(mp_engine* E) { std::fill_n(E->last_launch, MP_LAST_LAUNCH_FIELDS, -1); }
 
-// `S`: the engine's state with the step's targets applied (apply_outputs), for the scalar rows k_exchange_push delivers.
-int raise_flags(mp_engine* E, cudaStream_t st, const State& S) {
+// `S`: the engine's state with the step's targets applied (apply_outputs), for the scalar rows k_exchange_push delivers;
+// `G`: the segments of its per-player rows (apply_players).
+int raise_flags(mp_engine* E, cudaStream_t st, const State& S, const RowSegments& G = RowSegments{}) {
   E->x_pending_raise = false;
-  k_exchange_push<<<std::min(E->sm_count, (E->B + 7) / 8), 256, 0, st>>>(E->T, S);
+  k_exchange_push<<<std::min(E->sm_count, (E->B + 7) / 8), 256, 0, st>>>(E->T, S, G);
   ++E->launches;
   CUDA_TRY(cudaGetLastError());
   return MP_OK;
@@ -816,11 +817,31 @@ int copy_scalars(mp_engine* E, const ScalarTargets& o, cudaStream_t st) {
   return MP_OK;
 }
 
-// Points a launch's copy of the state at the per-player rows of `p` (checked by check_player_outputs).
-void apply_players(const mp_player_outputs& p, State& S) {
-  S.pr = PlayerTargets{p.row_of_player, p.n_rows, (p.reward || p.scalar_obs) ? 1 : 0, p.rgb, p.reward, p.scalar_obs,
-                       p.rgb_row_stride, p.reward_row_stride, p.scalar_obs_row_stride, p.scalar_obs_stride,
-                       p.world_row_of_env, p.world_rgb, p.world_rgb_row_stride, p.world_n_rows};
+static_assert(sizeof(RowSegment) == sizeof(mp_row_segment) && offsetof(RowSegment, rgb) == offsetof(mp_row_segment, rgb) &&
+                  offsetof(RowSegment, reward) == offsetof(mp_row_segment, reward) &&
+                  offsetof(RowSegment, scalar_obs_stride) == offsetof(mp_row_segment, scalar_obs_stride) &&
+                  MP_ROW_SEGMENTS == MP_MAX_ROW_SEGMENTS,
+              "RowSegment must match mp_row_segment");
+
+// The per-player targets of `p` as segments: its own, or one segment [0, n_rows) of its top-level targets.
+RowSegments row_segments(const mp_player_outputs& p) {
+  RowSegments G{};
+  if (p.n_segments > 0) {
+    G.n = p.n_segments;
+    memcpy(G.s, p.segments, sizeof(RowSegment) * G.n);
+  } else {
+    G.n = 1;
+    G.s[0] = RowSegment{0, p.n_rows, p.rgb, p.rgb_row_stride, p.reward, p.reward_row_stride, p.scalar_obs,
+                        p.scalar_obs_row_stride, p.scalar_obs_stride};
+  }
+  return G;
+}
+
+// Points a launch's copy of the state at the per-player rows of `p` (checked by check_player_outputs); `G` is
+// row_segments(p).
+void apply_players(const mp_player_outputs& p, const RowSegments& G, State& S) {
+  S.pr = PlayerTargets{p.row_of_player, (G.s[0].reward || G.s[0].scalar_obs) ? 1 : 0, p.world_row_of_env, p.world_rgb,
+                       p.world_rgb_row_stride, p.world_n_rows};
 }
 
 // `out`: where this render's outputs go besides / instead of the engine's own buffers (see apply_outputs), or null.
@@ -828,16 +849,17 @@ void apply_players(const mp_player_outputs& p, State& S) {
 // k_exchange_push delivers the routed scalars (one launch).
 int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = nullptr, const mp_player_outputs* routed = nullptr) {
   const bool players = E->flags & MP_FLAG_RENDER_PLAYERS, world = E->flags & MP_FLAG_RENDER_WORLD;
+  const RowSegments G = routed ? row_segments(*routed) : RowSegments{};
   if (!players && !world) {
     State S = E->S;
     if (out) apply_outputs(*out, S);
-    if (routed) apply_players(*routed, S);
-    if (E->x_pending_raise || S.pr.scalars_on) return raise_flags(E, st, S);  // (k_exchange_push also delivers S.out)
+    if (routed) apply_players(*routed, G, S);
+    if (E->x_pending_raise || S.pr.scalars_on) return raise_flags(E, st, S, G);  // (k_exchange_push also delivers S.out)
     return S.out.on ? copy_scalars(E, S.out, st) : MP_OK;
   }
   // The engine's own images are also slot 0's of mp_step_host_async: a render into them must not start before that
   // slot's device->host copy has read them, whichever call issues it. (A render into a target does not touch them.)
-  const bool own_images = (players && !(out && out->rgb) && !(routed && routed->rgb)) ||
+  const bool own_images = (players && !(out && out->rgb) && !G.s[0].rgb) ||
                           (world && !(out && out->world_rgb) && !(routed && routed->world_rgb));
   if (E->async_ready && own_images) CUDA_TRY(cudaStreamWaitEvent(st, E->slot[0].copied, 0));
   E->S.x_raise = E->x_pending_raise ? 1 : 0;
@@ -871,9 +893,9 @@ int launch_render(mp_engine* E, cudaStream_t st, const mp_device_outputs* out = 
   }
   State S = E->S;
   if (out) apply_outputs(*out, S);
-  if (routed) apply_players(*routed, S);  // (never with gather: mp_run refuses it)
+  if (routed) apply_players(*routed, G, S);  // (never with gather: mp_run refuses it)
   const int mode = routed ? RENDER_ROUTED : gather ? RENDER_GATHER : RENDER_PLAIN;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->render_fns[mode], E->T, S, R, E->flags));
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, E->render_fns[mode], E->T, S, R, E->flags, G));
   const int32_t layout[6] = {mode, E->inst_ncp, E->inst_ncw, R.n_teams, R.team_threads / 32, R.wstrip_log2};
   memcpy(E->last_launch + 4, layout, sizeof layout);
   if (gather) {
@@ -1833,19 +1855,49 @@ int check_bank(const void* bank, int n_slots, const int32_t* index, uint64_t ind
   return MP_OK;
 }
 
+// The names of segment k's targets in refusals ("players segment k rgb", ...); without segments, the top-level names.
+const char* segment_target_name(const mp_player_outputs* o, int k, int output) {
+  static const char* const top[3] = {"players rgb", "players reward", "players scalar_obs"};
+  static const std::vector<std::string> names = [] {
+    std::vector<std::string> v;
+    for (int s = 0; s < MP_MAX_ROW_SEGMENTS; ++s)
+      for (const char* t : {"rgb", "reward", "scalar_obs"}) v.push_back("players segment " + std::to_string(s) + " " + t);
+    return v;
+  }();
+  return o->n_segments > 0 ? names[k * 3 + output].c_str() : top[output];
+}
+
 // The checks of mp_run's `players` that need no other argument (include/mp_engine.h); its extents are appended to `ext`
-// for check_extents.
+// for check_extents. Row segments are checked as a table (range, order, one set of outputs), then each segment's targets
+// over its own rows by the same checks as the top-level targets, which are one segment [0, n_rows) here.
 int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_device_outputs* out, const char* fn, std::vector<DeviceExtent>& ext) {
   if (o->n_rows < 1) return fail(MP_E_INVALID, "%s: n_rows %d < 1", fn, o->n_rows);
   if (!o->row_of_player || (uintptr_t)o->row_of_player % 4) return fail(MP_E_INVALID, "%s: row_of_player is null or not 4-byte aligned", fn);
   if (E->g_world > 0 && E->S.g_world > 0)
     return fail(MP_E_UNSUPPORTED, "%s: the observation gather is enabled: its stacked slots stay dense and complete", fn);
-  const uint64_t R = (uint64_t)o->n_rows, n = E->T.n_scalar;
-  if (o->rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
-  if (o->rgb && out && out->rgb) return fail(MP_E_INVALID, "%s: rgb is both routed (players) and per env (out)", fn);
-  if (o->scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
-  if (o->scalar_obs && (o->scalar_obs_stride % 8 || o->scalar_obs_stride >= (1ull << 31)))
-    return fail(MP_E_INVALID, "%s: scalar_obs stride is not a multiple of 8 bytes or is 2 GiB or more", fn);
+  if (o->n_segments < 0 || o->n_segments > MP_MAX_ROW_SEGMENTS)
+    return fail(MP_E_INVALID, "%s: n_segments %d outside 0..%d", fn, o->n_segments, MP_MAX_ROW_SEGMENTS);
+  if (o->n_segments > 0 && (o->rgb || o->reward || o->scalar_obs))
+    return fail(MP_E_INVALID, "%s: with row segments, the top-level rgb, reward and scalar_obs must be null", fn);
+  for (int k = 0, end = 0; k < o->n_segments; ++k) {
+    const mp_row_segment& g = o->segments[k];
+    if (g.row_begin < end || g.row_end <= g.row_begin || g.row_end > o->n_rows)
+      return fail(MP_E_INVALID, "%s: segment %d rows [%d, %d) are empty, unsorted, overlap segment %d or leave [0, %d)", fn, k,
+                  g.row_begin, g.row_end, k - 1, o->n_rows);
+    end = g.row_end;
+    const mp_row_segment& g0 = o->segments[0];
+    if (!g.rgb != !g0.rgb || !g.reward != !g0.reward || !g.scalar_obs != !g0.scalar_obs)
+      return fail(MP_E_INVALID, "%s: segments 0 and %d carry different sets of outputs", fn, k);
+  }
+  const RowSegments G = row_segments(*o);
+  const uint64_t n = E->T.n_scalar;
+  if (G.s[0].rgb && !(E->flags & MP_FLAG_RENDER_PLAYERS)) return fail(MP_E_INVALID, "%s: rgb asked for, but the render flags switch the player images off", fn);
+  if (G.s[0].rgb && out && out->rgb) return fail(MP_E_INVALID, "%s: rgb is both routed (players) and per env (out)", fn);
+  if (G.s[0].scalar_obs && n == 0) return fail(MP_E_INVALID, "%s: scalar_obs asked for, but this substrate has no scalar observations", fn);
+  for (int k = 0; k < G.n; ++k)
+    if (G.s[k].scalar_obs && (G.s[k].scalar_obs_stride % 8 || G.s[k].scalar_obs_stride >= (1ull << 31)))
+      return fail(MP_E_INVALID, "%s: %s stride is not a multiple of 8 bytes or is 2 GiB or more", fn,
+                  o->n_segments ? segment_target_name(o, k, 2) : "scalar_obs");
   if (!o->world_rgb != !o->world_row_of_env) return fail(MP_E_INVALID, "%s: world_rgb and world_row_of_env go together", fn);
   if (o->world_rgb) {
     if (o->world_n_rows < 1) return fail(MP_E_INVALID, "%s: world_n_rows %d < 1", fn, o->world_n_rows);
@@ -1856,14 +1908,18 @@ int check_player_outputs(mp_engine* E, const mp_player_outputs* o, const mp_devi
   }
   ext.push_back({"row_of_player", (uintptr_t)o->row_of_player, (u128)E->B * E->T.P * 4});
   int rc;
-  if ((rc = add_strided(ext, fn, "row", "players rgb", o->rgb, o->rgb_row_stride, R, (uint64_t)E->R.player_bytes, 16, 0)) ||
-      (rc = add_strided(ext, fn, "row", "players reward", o->reward, o->reward_row_stride, R, 8, 8, 0)) ||
-      (rc = add_strided(ext, fn, "row", "players scalar_obs", o->scalar_obs, o->scalar_obs_row_stride, R, 8, 8,
-                        (u128)(n - 1) * o->scalar_obs_stride)) ||
-      (rc = add_strided(ext, fn, "row", "players world_rgb", o->world_rgb, o->world_rgb_row_stride, (uint64_t)o->world_n_rows,
-                        (uint64_t)E->R.world_bytes, 16, 0)))
-    return rc;
-  return o->scalar_obs ? check_scalar_rows(fn, "row", "players scalar_obs", o->scalar_obs_stride, o->scalar_obs_row_stride, n, R, 8) : MP_OK;
+  for (int k = 0; k < G.n; ++k) {
+    const RowSegment& g = G.s[k];
+    const uint64_t R = (uint64_t)(g.row_end - g.row_begin);
+    if ((rc = add_strided(ext, fn, "row", segment_target_name(o, k, 0), g.rgb, g.rgb_row_stride, R, (uint64_t)E->R.player_bytes, 16, 0)) ||
+        (rc = add_strided(ext, fn, "row", segment_target_name(o, k, 1), g.reward, g.reward_row_stride, R, 8, 8, 0)) ||
+        (rc = add_strided(ext, fn, "row", segment_target_name(o, k, 2), g.scalar_obs, g.scalar_obs_row_stride, R, 8, 8,
+                          (u128)(n - 1) * g.scalar_obs_stride)) ||
+        (g.scalar_obs && (rc = check_scalar_rows(fn, "row", segment_target_name(o, k, 2), g.scalar_obs_stride, g.scalar_obs_row_stride, n, R, 8))))
+      return rc;
+  }
+  return add_strided(ext, fn, "row", "players world_rgb", o->world_rgb, o->world_rgb_row_stride, (uint64_t)o->world_n_rows,
+                     (uint64_t)E->R.world_bytes, 16, 0);
 }
 
 // The checks of mp_run's `player_actions` that need no other argument (include/mp_engine.h); its extents are appended

@@ -246,14 +246,16 @@ struct ViewerInfo {  // per player, refreshed once per env
 // MODE (exclusive):
 //   RENDER_GATHER: also deliver every strip into every rank's stacked observation buffer (State::g_*);
 //   RENDER_ROUTED: deliver player p of env b to the row State::pr.row_of_player[b][p] of the caller's per-player
-//     targets (mp_run's players). The team's first warp reads the env's row map with its avatars and compacts the
-//     routed players into s_players; the env's item loop then runs over those players' strips and WORLD.RGB's only,
-//     so an unrouted player is neither composited nor stored. With State::pr.world_rgb set, the same warp also reads
+//     targets (mp_run's players), through the segment of G that holds the row. The team's first warp reads the env's
+//     row map with its avatars and compacts the players whose rows lie in a segment into s_players; the env's item loop
+//     then runs over those players' strips and WORLD.RGB's only, so an unrouted player is neither composited nor
+//     stored. At each player strip's store, lane 0 reads the row again and resolves its segment and address. With State::pr.world_rgb set, the same warp also reads
 //     the env's WORLD.RGB row (State::pr.world_row_of_env[b]): an env with a row stores its WORLD.RGB strips there,
 //     an env without one has no WORLD.RGB strips.
 enum { RENDER_PLAIN = 0, RENDER_GATHER = 1, RENDER_ROUTED = 2 };
 template <int NCP, int NCW, int MODE>
-__global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, State S, RenderPlan R, uint32_t flags) {
+__global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, State S, RenderPlan R, uint32_t flags,
+                                                            const __grid_constant__ RowSegments G) {
   constexpr bool GATHER = MODE == RENDER_GATHER, ROUTED = MODE == RENDER_ROUTED;
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem);  // [0] atlas, [1 + team] grid
@@ -363,11 +365,11 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
     }
     if (ROUTED && gtid < 32) {  // the group's first warp, whole: compact the routed players (all of them when the images are not routed)
       bool on = gtid < T.P;
-      if (on && S.pr.rgb) on = (uint32_t)S.pr.row_of_player[(size_t)b * T.P + gtid] < (uint32_t)S.pr.n_rows;
+      if (on && G.s[0].rgb) on = row_segment(G, S.pr.row_of_player[(size_t)b * T.P + gtid]) >= 0;
       const uint32_t m = __ballot_sync(MP_FULL, on);
       if (on) s_players[__popc(m & ((1u << gtid) - 1u))] = (uint8_t)gtid;
       if (gtid == 0) {
-        s_route[0] = S.pr.rgb ? __popc(m) * R.view_h : R.n_player_items;
+        s_route[0] = G.s[0].rgb ? __popc(m) * R.view_h : R.n_player_items;
         int wrow = 0, wn = R.n_items - R.n_player_items;
         if (S.pr.world_rgb) {
           wrow = S.pr.world_row_of_env[b];
@@ -441,9 +443,10 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
         __syncwarp();
         if (lane == 0 && !(flags & 32u)) {
           const size_t in_env = (size_t)p * R.player_bytes + (size_t)cy * R.pitem_bytes;
-          if (ROUTED && S.pr.rgb) {
+          if (ROUTED && G.s[0].rgb) {
             const int row = S.pr.row_of_player[(size_t)b * T.P + p];
-            bulk_store(S.pr.rgb + (size_t)row * S.pr.rgb_row_stride + (size_t)cy * R.pitem_bytes, buf, (uint32_t)R.pitem_bytes, store_policy);
+            const RowSegment& g = G.s[row_segment(G, row)];  // (compaction kept only players whose row lies in a segment)
+            bulk_store(g.rgb + (size_t)(row - g.row_begin) * g.rgb_row_stride + (size_t)cy * R.pitem_bytes, buf, (uint32_t)R.pitem_bytes, store_policy);
           }
           else bulk_store(S.rgb + b * S.rgb_env_stride + in_env, buf, (uint32_t)R.pitem_bytes, store_policy);
           if (GATHER) {  // the stacked slots stay dense, whatever the local target's stride
@@ -491,7 +494,7 @@ __global__ void __launch_bounds__(RENDER_MAX_THREADS, 1) k_render(Tables T, Stat
     // drawing instead of delaying the kernel's start
     if (S.x_raise && it == 0) exchange_push(T, S);
     if (S.out.on && it == 0) deliver_scalars(T, S);  // (tested here, not only inside: measured, k_render<3, 3, true> spills otherwise)
-    if (ROUTED && S.pr.scalars_on && it == 0) deliver_player_scalars(T, S);
+    if (ROUTED && S.pr.scalars_on && it == 0) deliver_player_scalars(T, S, G);
     group_sync(bar_id, gthreads);  // every warp is done with s_rec / s_view
     if (gtid == 0) *next_ctr = 0;
     // (the reset is ordered before the next env's item loop by the group barrier after its cell pass)

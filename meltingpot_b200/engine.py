@@ -125,6 +125,18 @@ def _strides(label: str, t, lead: int, unit: str, item: int) -> Tuple[int, ...]:
   return tuple(strides)
 
 
+MP_MAX_ROW_SEGMENTS = 16
+
+
+class MpRowSegment(ctypes.Structure):
+  _fields_ = [
+      ('row_begin', ctypes.c_int32), ('row_end', ctypes.c_int32),
+      ('rgb', ctypes.c_void_p), ('rgb_row_stride', ctypes.c_uint64),
+      ('reward', ctypes.c_void_p), ('reward_row_stride', ctypes.c_uint64),
+      ('scalar_obs', ctypes.c_void_p), ('scalar_obs_row_stride', ctypes.c_uint64), ('scalar_obs_stride', ctypes.c_uint64),
+  ]
+
+
 class MpPlayerOutputs(ctypes.Structure):
   _fields_ = [
       ('row_of_player', ctypes.c_void_p), ('n_rows', ctypes.c_int32),
@@ -133,6 +145,7 @@ class MpPlayerOutputs(ctypes.Structure):
       ('scalar_obs', ctypes.c_void_p), ('scalar_obs_row_stride', ctypes.c_uint64), ('scalar_obs_stride', ctypes.c_uint64),
       ('world_row_of_env', ctypes.c_void_p), ('world_n_rows', ctypes.c_int32),
       ('world_rgb', ctypes.c_void_p), ('world_rgb_row_stride', ctypes.c_uint64),
+      ('n_segments', ctypes.c_int32), ('segments', MpRowSegment * MP_MAX_ROW_SEGMENTS),
   ]
 
 
@@ -143,14 +156,21 @@ WORLD_OUTPUTS = ('world_row_of_env', 'world_rgb')
 
 
 def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num_envs: int, num_players: int,
-                     num_scalar_obs: int, device: int, world_shape: Optional[Tuple[int, ...]] = None) -> MpPlayerOutputs:
+                     num_scalar_obs: int, device: int, world_shape: Optional[Tuple[int, ...]] = None,
+                     _rows_only: bool = False) -> MpPlayerOutputs:
   """The mp_player_outputs of `players`: 'row_of_player' (TensorLayout of a contiguous int32 CUDA [B, P]) and any of
   'rgb' (uint8 [n_rows, *rgb_shape], dense inside a row), 'reward' (float64 [n_rows]) and 'scalar_obs' (float64
   [num_scalar_obs, n_rows]); the row axis (and the observation axis of scalar_obs) may have any stride. Every target
   must have the same n_rows. WORLD.RGB rows, optional: 'world_row_of_env' (contiguous int32 CUDA [B]) with 'world_rgb'
   (uint8 [n, *world_shape], dense inside a row, 16-byte aligned rows; world_shape None: the engine renders no
-  WORLD.RGB). Only shapes, dtypes, devices and layouts are checked, never the row maps' values."""
+  WORLD.RGB). Only shapes, dtypes, devices and layouts are checked, never the row maps' values.
+
+  Row segments instead of the per-player targets: 'n_rows' (the row map's row count) and 'segments', a sequence of up to
+  MP_MAX_ROW_SEGMENTS (row_begin, row_end, {name: TensorLayout}) whose targets are those above for rows
+  [row_begin, row_end) only (row r in the segment's row r - row_begin). A row in no segment is not delivered."""
   import torch  # pylint: disable=g-import-not-at-top
+  if 'segments' in players:
+    return _describe_segments(players, rgb_shape, num_envs, num_players, num_scalar_obs, device, world_shape)
   unknown = set(players) - set(PLAYER_OUTPUTS) - set(WORLD_OUTPUTS) - {'row_of_player'}
   if unknown:
     raise ValueError(f'players: unknown entries {sorted(unknown)} (row_of_player and any of {", ".join(PLAYER_OUTPUTS)}, '
@@ -172,7 +192,7 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
   s.row_of_player = ctypes.c_void_p(int(rmap.data_ptr))
   n_rows = None
   targets = {k: v for k, v in players.items() if k in PLAYER_OUTPUTS and v is not None}
-  if not targets:
+  if not targets and not _rows_only:  # (_rows_only: the row map and WORLD.RGB of a request whose segments hold the rest)
     raise ValueError(f'players: give at least one of {", ".join(PLAYER_OUTPUTS)}')
   for name, t in targets.items():
     row_axis = 1 if name == 'scalar_obs' else 0
@@ -198,7 +218,7 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
     setattr(s, f'{name}_row_stride', strides[-1])
     if name == 'scalar_obs':
       s.scalar_obs_stride = strides[0]
-  s.n_rows = n_rows
+  s.n_rows = n_rows or 0
   wmap, world = players.get('world_row_of_env'), players.get('world_rgb')
   if (wmap is None) != (world is None):
     raise ValueError('players: world_row_of_env and world_rgb go together')
@@ -224,6 +244,39 @@ def describe_players(players: Mapping[str, Any], rgb_shape: Tuple[int, ...], num
     s.world_n_rows = rows
     s.world_rgb = ctypes.c_void_p(int(world.data_ptr))
     s.world_rgb_row_stride = row_stride
+  return s
+
+
+def _describe_segments(players, rgb_shape, num_envs, num_players, num_scalar_obs, device, world_shape) -> MpPlayerOutputs:
+  """describe_players with row segments: each segment's targets are described as a players dict of its own rows, so
+  they take exactly the checks of top-level targets; the C call checks the table (order, range, one set of outputs)."""
+  unknown = set(players) - set(WORLD_OUTPUTS) - {'row_of_player', 'n_rows', 'segments'}
+  if unknown:
+    raise ValueError(f'players: unknown entries {sorted(unknown)} with segments (row_of_player, n_rows, segments, '
+                     f'optionally {" with ".join(WORLD_OUTPUTS)})')
+  segments = list(players['segments'])
+  if not 1 <= len(segments) <= MP_MAX_ROW_SEGMENTS:
+    raise ValueError(f'players: {len(segments)} segments, must be 1..{MP_MAX_ROW_SEGMENTS}')
+  n_rows = players.get('n_rows')
+  if n_rows is None or int(n_rows) < 1:
+    raise ValueError('players: segments need n_rows >= 1, the row count of the row map')
+  base = {k: players.get(k) for k in ('row_of_player',) + WORLD_OUTPUTS if players.get(k) is not None}
+  s = describe_players(base, rgb_shape, num_envs, num_players, num_scalar_obs, device, world_shape, _rows_only=True)
+  s.n_rows = int(n_rows)
+  s.n_segments = len(segments)
+  for k, (begin, end, targets) in enumerate(segments):
+    begin, end = int(begin), int(end)
+    if end - begin < 1:
+      raise ValueError(f'players: segment {k} rows [{begin}, {end}) are empty')
+    one = describe_players(dict(targets, row_of_player=players['row_of_player']), rgb_shape, num_envs, num_players,
+                           num_scalar_obs, device, world_shape)
+    if one.n_rows != end - begin:
+      raise ValueError(f'players: segment {k} targets have {one.n_rows} rows, rows [{begin}, {end}) are {end - begin}')
+    g = s.segments[k]
+    g.row_begin, g.row_end = begin, end
+    for name in ('rgb', 'rgb_row_stride', 'reward', 'reward_row_stride', 'scalar_obs', 'scalar_obs_row_stride',
+                 'scalar_obs_stride'):
+      setattr(g, name, getattr(one, name))
   return s
 
 
@@ -608,7 +661,9 @@ class Engine:
     checked on the host; two players routed to one row leave one of them there. WORLD.RGB may be routed per env in
     the same call: 'world_row_of_env' (contiguous CUDA int32 [B]) with 'world_rgb' (uint8 [n, H, W, 3]); env b's image
     is drawn into row world_row_of_env[b] when that lies in 0..n-1, and not at all otherwise, and this engine's own
-    world_rgb is not written (out's world_rgb must then be absent).
+    world_rgb is not written (out's world_rgb must then be absent). Instead of 'rgb' / 'reward' / 'scalar_obs', players
+    may give 'n_rows' and 'segments': up to 16 sorted, disjoint (row_begin, row_end, {name: tensor}) whose tensors hold
+    rows [row_begin, row_end) only, e.g. one trajectory buffer per group; a row in no segment is not delivered.
 
     player_actions: actions read from rows, {'row_of_player': contiguous CUDA int32 [B, P],
     'action': CUDA int32 [n_rows], any stride}, with actions None. Player p of env b takes action[row_of_player[b, p]]
@@ -668,7 +723,12 @@ class Engine:
     return describe_outputs({k: (None if v is None else layout_of(v)) for k, v in out.items()}, self.output_views(), self.device)
 
   def _player_outputs(self, players) -> MpPlayerOutputs:
-    return describe_players({k: (None if v is None else layout_of(v)) for k, v in players.items()}, tuple(self.rgb.shape[2:]),
+    layouts = lambda d: {k: (None if v is None else layout_of(v)) for k, v in d.items()}
+    described = layouts({k: v for k, v in players.items() if k not in ('n_rows', 'segments')})
+    if 'segments' in players:
+      described.update(n_rows=players.get('n_rows'),
+                       segments=[(begin, end, layouts(targets)) for begin, end, targets in players['segments']])
+    return describe_players(described, tuple(self.rgb.shape[2:]),
                             self.num_envs, self.num_players, self.num_scalar_obs, self.device,
                             tuple(self.world_rgb.shape[1:]))
 

@@ -246,32 +246,87 @@ class BatchedScenario:
       tensors['WORLD.RGB'] = torch.empty(shape, dtype=torch.uint8, device=dev)
     return substrate_lib.PlayerOutputs(r, None, tensors, block, world=self._world)
 
-  def _select(self, timestep, po, rows, n, permitted):
+  def _select(self, timestep, tensors, n, permitted):
+    """The timestep of one group: `tensors` holds its rows ({name: [B * n, ...]})."""
     def view(v):
-      return v[rows].view((self.num_envs, n) + tuple(v.shape[1:]))
+      return v.view((self.num_envs, n) + tuple(v.shape[1:]))
     obs = {}
     for key in ('RGB',) + tuple(timestep.observation):  # a routed timestep has no 'RGB': the rows hold the images
       if permitted is not None and key not in permitted:
         continue
-      obs[key] = timestep.observation[key] if key in _GLOBAL_KEYS else view(po[key])
-    return substrate_lib.BatchedTimeStep(step_type=timestep.step_type, reward=view(po['REWARD']),
+      obs[key] = timestep.observation[key] if key in _GLOBAL_KEYS else view(tensors[key])
+    return substrate_lib.BatchedTimeStep(step_type=timestep.step_type, reward=view(tensors['REWARD']),
                                          discount=timestep.discount, observation=obs)
 
-  def _split(self, timestep, po):
+  def _split(self, timestep, tensors):
+    """tensors(g): {name: tensor} of group g's rows (0 focal, then the background groups)."""
     if self.bot_names:
       r = self._routes
-      self._background_timestep = {n: self._select(timestep, po, r.rows(k + 1), len(r.group(k + 1)), None)
+      self._background_timestep = {n: self._select(timestep, tensors(k + 1), len(r.group(k + 1)), None)
                                    for k, n in enumerate(self.bot_names)}
     else:
-      self._background_timestep = self._select(timestep, po, self._background_rows, self.num_background, None)
-    return self._select(timestep, po, self._focal_rows, self.num_focal, self._permitted)
+      self._background_timestep = self._select(timestep, tensors(1), self.num_background, None)
+    return self._select(timestep, tensors(0), self.num_focal, self._permitted)
 
-  def reset(self):
+  def _rows_of(self, po):
+    """tensors(g) for _split of a PlayerOutputs holding every row."""
+    rows = {0: self._focal_rows}
+    if self.bot_names:
+      rows.update({k + 1: self._routes.rows(k + 1) for k in range(len(self.bot_names))})
+    else:
+      rows[1] = self._background_rows
+    return lambda g: {k: v[rows[g]] for k, v in po.tensors.items() if k != 'WORLD.RGB'}
+
+  def trajectory(self, T: int, time_major: bool = True) -> 'ScenarioTrajectory':
+    """Tensors for T focal timesteps; `reset(out=traj.at(t))` and `step(focal_actions, out=traj.at(t))` deliver the
+    focal players straight into slot t. See ScenarioTrajectory."""
+    return ScenarioTrajectory(self, int(T), bool(time_major))
+
+  def _slot(self, out):
+    """(GroupOutputs of one step into slot `out`, engine targets of its per-env outputs)."""
+    import torch  # pylint: disable=g-import-not-at-top
+    if not isinstance(out, ScenarioSlot) or out.rows.routes is not self._routes:
+      raise ValueError('out must be a slot of this scenario\'s trajectory (trajectory(T).at(t))')
+    r = self._routes
+    groups = {0: out.rows.groups[0]}
+    for g in range(1, r.num_groups):  # the background rows go to fresh tensors, as without out
+      rows = r.rows(g)
+      groups[g] = substrate_lib._group_tensors(r, g, (rows.stop - rows.start,), torch.empty)  # pylint: disable=protected-access
+    world = None
+    if self._world is not None:
+      world = (out.rows.world_envs, out.rows.world_row_of_env, out.rows.world_rgb)
+    po = substrate_lib.GroupOutputs(r, {g: None for g in groups}, groups=groups, world=world)
+    targets = substrate_lib.BatchedTimeStep(step_type=out.step_type, reward=None, discount=out.discount, observation={})
+    return po, targets
+
+  def _slot_timestep(self, timestep, po, out):
+    """_split of a step into slot `out`, its COLLECTIVE_REWARD summed into the slot from the engine's rewards."""
+    import torch  # pylint: disable=g-import-not-at-top
+    sub = self._substrate
+    collective = out.observation[substrate_lib._COLLECTIVE_REWARD_OBS]  # pylint: disable=protected-access
+    sub._fill_collective(substrate_lib.BatchedTimeStep(  # pylint: disable=protected-access
+        step_type=out.step_type, reward=sub.engine.reward, discount=out.discount,
+        observation={substrate_lib._COLLECTIVE_REWARD_OBS: collective}))  # pylint: disable=protected-access
+    # the keys of a routed timestep, in its order; _select reads per-player values from the rows, not from here
+    obs = {name: None for name in sub._scalar_names}  # pylint: disable=protected-access
+    if sub._world_shape() is not None:  # pylint: disable=protected-access
+      obs['WORLD.RGB'] = timestep.observation.get('WORLD.RGB', sub.engine.world_rgb)  # unrouted: per env, as without out
+    obs[substrate_lib._COLLECTIVE_REWARD_OBS] = collective  # pylint: disable=protected-access
+    ts = substrate_lib.BatchedTimeStep(step_type=timestep.step_type, reward=None, discount=timestep.discount, observation=obs)
+    background = lambda g: (po.groups[g][0] if g < self._routes.num_groups else  # (no background players)
+                            substrate_lib._group_tensors(self._routes, g, (0,), torch.empty)[0])  # pylint: disable=protected-access
+    return self._split(ts, background)
+
+  def reset(self, out=None):
+    """out: a slot of trajectory(T) (`traj.at(t)`) to reset into; the returned focal timestep is then views of it."""
+    if out is not None:
+      po, targets = self._slot(out)
+      return self._slot_timestep(self._substrate.reset(out=targets, players=po), po, out)
     po = self._outputs()
-    return self._split(self._substrate.reset(players=po), po)
+    return self._split(self._substrate.reset(players=po), self._rows_of(po))
 
-  def step(self, focal_actions):
-    """focal_actions: int tensor [B, num_focal]; returns the focal players' BatchedTimeStep."""
+  def step(self, focal_actions, out=None):
+    """focal_actions: int tensor [B, num_focal]; returns the focal players' BatchedTimeStep. out: as for reset."""
     if tuple(focal_actions.shape) != (self.num_envs, self.num_focal):
       raise ValueError(f'Expected {self.num_focal} focal actions per env, got shape {tuple(focal_actions.shape)}.')
     rows = self._actions.tensor
@@ -285,8 +340,11 @@ class BatchedScenario:
     elif self.num_background:
       background_actions = self._policy(self._background_timestep)
       rows[self._background_rows].view(self.num_envs, self.num_background).copy_(background_actions)
+    if out is not None:
+      po, targets = self._slot(out)
+      return self._slot_timestep(self._substrate.step(out=targets, players=po, player_actions=self._actions), po, out)
     po = self._outputs()
-    return self._split(self._substrate.step(players=po, player_actions=self._actions), po)
+    return self._split(self._substrate.step(players=po, player_actions=self._actions), self._rows_of(po))
 
   @property
   def background_timestep(self):
@@ -307,3 +365,63 @@ class BatchedScenario:
 
   def close(self):
     self._substrate.close()
+
+
+@dataclasses.dataclass
+class ScenarioSlot(substrate_lib.BatchedTimeStep):
+  """Slot t of a ScenarioTrajectory: the focal timestep's fields as views of the slot, and `rows`, the focal group's
+  rows of the slot (a GroupOutputs) that the engine writes."""
+  rows: Any = None
+
+
+class ScenarioTrajectory:
+  """T focal timesteps of a BatchedScenario in caller-owned CUDA tensors (BatchedScenario.trajectory).
+
+  Per focal player: `reward` float64 and observation 'RGB' uint8 and each scalar observation float64, each
+  [T, B, num_focal, ...] (time_major) or [B, num_focal, T, ...]; the step renders them straight into slot t through
+  the focal group's row segment, so keeping a trajectory costs no copy. Per env: `step_type` int64, `discount` float64
+  and observation 'COLLECTIVE_REWARD' float64, [T, B] or [B, T]. With the scenario's world_envs, observation
+  'WORLD.RGB' uint8 is [T, n, H, W, 3] ([n, T, H, W, 3] when not time_major), row k holding env world_envs[k]. Without
+  world_envs, WORLD.RGB stays per env in the engine's buffer, where the background players see it too. The background
+  players' rows go to fresh tensors every step, as without a trajectory."""
+
+  def __init__(self, scenario: BatchedScenario, T: int, time_major: bool):
+    import torch  # pylint: disable=g-import-not-at-top
+    if T < 1:
+      raise ValueError(f'a trajectory needs T >= 1 slots, got {T}')
+    r = scenario._routes  # pylint: disable=protected-access
+    world = scenario._world  # pylint: disable=protected-access
+    self.T, self.time_major = T, time_major
+    self.num_envs, self.num_focal = scenario.num_envs, scenario.num_focal
+    self.rows = r.group_outputs({0: T}, time_major, world_envs=None if world is None else world[0])
+    B, n = self.num_envs, self.num_focal
+    tensors, block = self.rows.groups[0]
+
+    def per_player(v, lead):  # [T, B * n, ...] -> [T, B, n, ...]; [B * n, T, ...] -> [B, n, T, ...]
+      shape = tuple(v.shape)
+      if time_major:
+        return v.view(shape[:lead + 1] + (B, n) + shape[lead + 2:])
+      return v.view(shape[:lead] + (B, n) + shape[lead + 1:])
+
+    def new(dtype):
+      return torch.zeros((T, B) if time_major else (B, T), dtype=dtype, device=r.device)
+
+    self.step_type = new(torch.int64)
+    self.discount = new(torch.float64)
+    self.reward = per_player(tensors['REWARD'], 0)
+    self.observation = {k: per_player(v, 0) for k, v in tensors.items() if k != 'REWARD'}
+    if self.rows.world_rgb is not None:
+      self.observation['WORLD.RGB'] = self.rows.world_rgb
+    self.observation[substrate_lib._COLLECTIVE_REWARD_OBS] = new(torch.float64)  # pylint: disable=protected-access
+
+  def at(self, t: int) -> ScenarioSlot:
+    """Slot t, for BatchedScenario.reset(out=) / step(out=)."""
+    if not -self.T <= t < self.T:
+      raise IndexError(f'slot {t} of a trajectory of {self.T}')
+    pick = (lambda x: x[t]) if self.time_major else (lambda x: x[:, t])
+    pick_player = (lambda x: x[t]) if self.time_major else (lambda x: x[:, :, t])
+    obs = {}
+    for k, v in self.observation.items():
+      obs[k] = pick(v) if k in _GLOBAL_KEYS else pick_player(v)
+    return ScenarioSlot(step_type=pick(self.step_type), reward=pick_player(self.reward), discount=pick(self.discount),
+                        observation=obs, rows=self.rows.at(t))

@@ -293,7 +293,8 @@ class BatchedSubstrate:
     not drawn. The returned timestep then has no 'RGB'; every other field is as without players. Combines with out and
     restore / bank. With outputs made with world_envs (`outputs(world_envs=envs)`), WORLD.RGB is drawn only for those
     envs, straight into players['WORLD.RGB'] (row k: env envs[k]), and the timestep's 'WORLD.RGB' is that tensor; out's
-    'WORLD.RGB' is then left alone.
+    'WORLD.RGB' is then left alone. players may also be a GroupOutputs (`group_outputs(slots)`, or `.at(t)` of one with
+    slots): each listed group's players go to that group's own tensors, the other groups' players nowhere.
 
     player_actions: a PlayerActions (`player_routes(groups).actions()`, or `.at(t)` of one with T slots), with actions
     None: each routed player takes the action in its row, an unrouted player action 0 (NOOP). The routes may be the
@@ -338,7 +339,18 @@ class BatchedSubstrate:
                       self._scalar_names, bool(time_major), torch.device('cuda', e.device))
 
   def _routed_outputs(self, po: 'PlayerOutputs'):
-    """The engine's per-player targets of a PlayerOutputs (the scalar observations as one [n, n_rows] view)."""
+    """The engine's per-player targets of a PlayerOutputs (the scalar observations as one [n, n_rows] view), or the
+    row segments of a GroupOutputs."""
+    if isinstance(po, GroupOutputs):
+      self._check_routes(po.routes, 'players')
+      if any(T is not None for T in po.slots.values()):
+        raise ValueError('players: pick one slot of a GroupOutputs with slots (group_outputs(slots).at(t))')
+      targets = {'row_of_player': po.routes.row_of_player, 'n_rows': po.routes.n_rows, 'segments': po.segments()}
+      if _routes_world(po):
+        if not self._world_rgb:
+          raise ValueError('players: WORLD.RGB is routed, but this batch was built with world_rgb=False')
+        targets.update(world_row_of_env=po.world_row_of_env, world_rgb=po.world_rgb)
+      return targets
     if not isinstance(po, PlayerOutputs):
       raise ValueError('players must be a PlayerOutputs (player_routes(groups).outputs() or drawn_routes(choices).outputs())')
     r = po.routes
@@ -372,7 +384,7 @@ class BatchedSubstrate:
     """ts without 'RGB' (the rows hold the images), its 'WORLD.RGB' the routed rows when po routes it."""
     obs = {k: v for k, v in ts.observation.items() if k != 'RGB'}
     if _routes_world(po):
-      obs['WORLD.RGB'] = po['WORLD.RGB']
+      obs['WORLD.RGB'] = po.world_rgb if isinstance(po, GroupOutputs) else po['WORLD.RGB']
     return BatchedTimeStep(step_type=ts.step_type, reward=ts.reward, discount=ts.discount, observation=obs)
 
   def _engine_outputs(self, ts: BatchedTimeStep, routed=None):
@@ -575,6 +587,11 @@ class PlayerRoutes:
     env's WORLD.RGB is rendered."""
     return PlayerOutputs(self, T, world_envs=world_envs)
 
+  def group_outputs(self, slots: Mapping[int, Optional[int]], time_major: bool = True, world_envs=None) -> 'GroupOutputs':
+    """Zeroed CUDA tensors of their own for each group listed in slots (group -> T_g, or None for no time axis); see
+    GroupOutputs. A group not listed is not delivered."""
+    return GroupOutputs(self, slots, time_major, world_envs=world_envs)
+
   def actions(self, T: Optional[int] = None) -> 'PlayerActions':
     """A zeroed int32 CUDA tensor of actions, one per row: [n_rows], or [T, n_rows] with T, whose `at(t)` is slot t."""
     return PlayerActions(self, T)
@@ -673,6 +690,10 @@ class DrawnRoutes:
   def outputs(self, T: Optional[int] = None, world_envs=None) -> 'PlayerOutputs':
     """As PlayerRoutes.outputs."""
     return PlayerOutputs(self, T, world_envs=world_envs)
+
+  def group_outputs(self, slots: Mapping[int, Optional[int]], time_major: bool = True, world_envs=None) -> 'GroupOutputs':
+    """As PlayerRoutes.group_outputs: group g's tensors hold its whole block rows(g), [B, n_g] in env-major order."""
+    return GroupOutputs(self, slots, time_major, world_envs=world_envs)
 
   def actions(self, T: Optional[int] = None) -> 'PlayerActions':
     """As PlayerRoutes.actions."""
@@ -777,6 +798,110 @@ class PlayerOutputs:
     if self.T is None:
       return {k: v[r] for k, v in per_player.items()}
     return {k: v[:, r] for k, v in per_player.items()}
+
+
+def _group_tensors(routes, g: int, lead: Tuple[int, ...], alloc):
+  """({name: tensor}, scalar block) of group g's routed outputs: 'RGB', 'REWARD' and each scalar observation, with
+  `lead` in front of each ((n_g,), (T, n_g) or (n_g, T)) and the scalar observations views of one block
+  [n_scalar, *lead]. alloc: torch.zeros or torch.empty."""
+  import torch  # pylint: disable=g-import-not-at-top
+  dev = routes.device
+  tensors = {'RGB': alloc(lead + routes._rgb_shape, dtype=torch.uint8, device=dev),  # pylint: disable=protected-access
+             'REWARD': alloc(lead, dtype=torch.float64, device=dev)}
+  names = routes._scalar_names  # pylint: disable=protected-access
+  block = alloc((len(names),) + lead, dtype=torch.float64, device=dev) if names else None
+  for k, name in enumerate(names):
+    tensors[name] = block[k]
+  return tensors, block
+
+
+class GroupOutputs:
+  """Caller-owned CUDA tensors of routed outputs, one set per group (routes.group_outputs(slots)), so that each group's
+  rows land in a buffer of its own, e.g. one trajectory buffer per learning group of a population, with its own T.
+
+  Group g of `slots` gets 'RGB' uint8, 'REWARD' float64 and each scalar observation float64 (views of one block),
+  each [T_g, n_g, ...] (time_major) or [n_g, T_g, ...], or [n_g, ...] with T_g None; n_g is the size of rows(g), row k
+  of the group being row rows(g).start + k of the routes. Groups not listed are not delivered: their players are
+  neither rendered nor given scalars. Pass it (or `at(t)`) to BatchedSubstrate.step / reset as players=: the step
+  delivers each listed group into its tensors through one row segment per group, in the same kernels as outputs().
+  Made with world_envs, it also holds WORLD.RGB as outputs() does, with a slot axis when some group has slots (T the
+  largest T_g, laid out like the groups'): `world_rgb`, `world_envs`, `world_row_of_env`; all None otherwise."""
+
+  def __init__(self, routes, slots: Mapping[int, Optional[int]], time_major: bool = True, world_envs=None, groups=None,
+               world=None):
+    """groups, world: a view (at), or tensors made by the caller: groups maps g to ({name: tensor}, scalar block) and
+    world is (world_envs, world_row_of_env, world_rgb) or None."""
+    import torch  # pylint: disable=g-import-not-at-top
+    self.routes, self.time_major = routes, bool(time_major)
+    if not isinstance(slots, Mapping) or not slots:
+      raise ValueError('slots must map at least one group id to its number of slots (or None)')
+    norm = {}
+    for g, T in slots.items():
+      if isinstance(g, (bool, np.bool_)) or not isinstance(g, (int, np.integer)) or not 0 <= g < routes.num_groups:
+        raise ValueError(f'slots: group {g!r} outside 0..{routes.num_groups - 1}')
+      if T is not None and (isinstance(T, (bool, np.bool_)) or not isinstance(T, (int, np.integer)) or T < 1):
+        raise ValueError(f'slots: group {g} needs T >= 1 slots or None, got {T!r}')
+      norm[int(g)] = None if T is None else int(T)
+    self.slots = dict(sorted(norm.items()))
+    if all(routes.rows(g).stop == routes.rows(g).start for g in self.slots):
+      raise ValueError('slots: every group listed has no rows')
+    if groups is not None:
+      self.groups = groups
+      self.world_envs, self.world_row_of_env, self.world_rgb = world if world is not None else (None, None, None)
+      return
+    self.groups = {}
+    for g, T in self.slots.items():
+      n = routes.rows(g).stop - routes.rows(g).start
+      lead = (n,) if T is None else ((T, n) if self.time_major else (n, T))
+      self.groups[g] = _group_tensors(routes, g, lead, torch.zeros)
+    self.world_envs = self.world_row_of_env = self.world_rgb = None
+    if world_envs is not None:
+      if routes._world_shape is None:  # pylint: disable=protected-access
+        raise ValueError('world_envs: this batch renders no WORLD.RGB (it was built with world_rgb=False)')
+      self.world_envs, self.world_row_of_env = world_row_map(world_envs, routes.num_envs, routes.device)
+      n = int(self.world_envs.shape[0])
+      T = max((t for t in self.slots.values() if t is not None), default=None)
+      lead = (n,) if T is None else ((T, n) if self.time_major else (n, T))
+      self.world_rgb = torch.zeros(lead + routes._world_shape, dtype=torch.uint8, device=routes.device)  # pylint: disable=protected-access
+
+  def group(self, g: int) -> Dict[str, Any]:
+    """{name: tensor} of group g."""
+    if g not in self.groups:
+      raise KeyError(f'group {g} is not delivered (slots lists {sorted(self.groups)})')
+    return dict(self.groups[g][0])
+
+  def at(self, t: int) -> 'GroupOutputs':
+    """Slot t of every group that has slots (and of WORLD.RGB), as views; groups without slots keep their tensors."""
+    timed = [T for T in self.slots.values() if T is not None]
+    if not timed:
+      raise ValueError('at() needs a group with slots')
+    if not all(-T <= t < T for T in timed):
+      raise IndexError(f'slot {t} of groups with {min(timed)} slots or more')
+    pick = (lambda x: x[t]) if self.time_major else (lambda x: x[:, t])
+    groups = {}
+    for g, (tensors, block) in self.groups.items():
+      if self.slots[g] is None:
+        groups[g] = (tensors, block)
+        continue
+      sb = None if block is None else (block[:, t] if self.time_major else block[:, :, t])
+      view = {k: pick(v) for k, v in tensors.items()}
+      for k, name in enumerate(self.routes._scalar_names):  # pylint: disable=protected-access
+        view[name] = sb[k]
+      groups[g] = (view, sb)
+    world = None
+    if self.world_rgb is not None:
+      world = (self.world_envs, self.world_row_of_env, pick(self.world_rgb))
+    return GroupOutputs(self.routes, {g: None for g in self.slots}, self.time_major, groups=groups, world=world)
+
+  def segments(self):
+    """The engine's row segments of a view without slots: [(row_begin, row_end, {target: tensor})], one per group
+    that has rows."""
+    out = []
+    for g, (tensors, block) in self.groups.items():
+      r = self.routes.rows(g)
+      if r.stop > r.start:
+        out.append((r.start, r.stop, {'rgb': tensors['RGB'], 'reward': tensors['REWARD'], 'scalar_obs': block}))
+    return out
 
 
 class PlayerActions:
